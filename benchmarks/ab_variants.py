@@ -2,7 +2,7 @@
 """A/B timing of differently-compiled builds of the library on BASELINE config 2.
 
 Build variants anywhere nvcc runs (no GPU needed), e.g.
-    GSB_VARIANT=E GSB_EXTRA_NVCC_FLAGS="-DBWD2_MINBLOCKS=10" python -m easygaussiansplatting_b200.build
+    GSB_VARIANT=E GSB_EXTRA_NVCC_FLAGS="-DDRAW_BWD_MINBLOCKS=5" python -m easygaussiansplatting_b200.build
 then on the GPU
     python benchmarks/ab_variants.py            # default build + every libgsplat_b200_*.so found
 Each build runs in its own process (GSB_LIB selects the library): 30 timed fused fwd+bwd steps
@@ -16,7 +16,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CHILD = r"""
-import ctypes as C, json, os, sys
+import ctypes as C, json, sys
 import numpy as np, torch
 sys.path.insert(0, %r)
 from easygaussiansplatting_b200 import _lib
@@ -59,36 +59,19 @@ for i in range(lib.gsb_profile_kernels()):
     lib.gsb_profile_read(i, C.byref(ms), C.byref(cnt))
     if cnt.value:
         kern[lib.gsb_profile_kernel_name(i).decode()] = round(ms.value / 5, 4)
-stats = None
-try:
-    raw = C.CDLL(os.environ.get("GSB_LIB") or _lib.LIB_PATH)
-    buf = (C.c_ulonglong * 8)()
-    raw.gsb_debug_bwd3_stats(buf, 1)
-    step(); torch.cuda.synchronize()
-    raw.gsb_debug_bwd3_stats(buf, 1)
-    stats = list(buf)
-except Exception:
-    pass
-print("RESULT " + json.dumps({"ms_per_step": round(best, 4), "kernels": kern, "stats": stats, "checksum": float(P["pws"].grad.abs().sum())}))
+print("RESULT " + json.dumps({"ms_per_step": round(best, 4), "kernels": kern, "checksum": float(P["pws"].grad.abs().sum())}))
 """
 
 
 def main():
     libs = [("default", "")] + sorted((os.path.basename(p)[len("libgsplat_b200_"):-3], p) for p in
                                       glob.glob(os.path.join(ROOT, "easygaussiansplatting_b200", "libgsplat_b200_*.so")))
-    # GSB_AB_ENVS="name:K=V,K2=V2;name2:K=V": the default build under different environment settings
-    envs = {}
-    for spec in filter(None, os.environ.get("GSB_AB_ENVS", "").split(";")):
-        name, kv = spec.split(":", 1)
-        envs[name] = dict(x.split("=", 1) for x in kv.split(","))
-        libs.append((name, ""))
     only = set(sys.argv[1:])
     out = {}
     for name, path in libs:
         if only and name not in only:
             continue
         env = dict(os.environ)
-        env.update(envs.get(name, {}))
         if path:
             env["GSB_LIB"] = path
         r = subprocess.run([sys.executable, "-c", CHILD % ROOT], env=env, capture_output=True, text=True, timeout=600)

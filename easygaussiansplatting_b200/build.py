@@ -17,8 +17,8 @@ CSRC = os.path.join(HERE, "csrc")
 VARIANT = os.environ.get("GSB_VARIANT", "")
 OBJ = os.path.join(HERE, "_obj" + ("_" + VARIANT if VARIANT else ""))
 LIB = os.path.join(HERE, "libgsplat_b200%s.so" % ("_" + VARIANT if VARIANT else ""))
-SOURCES = ["api.cu", "pergaussian.cu", "fused.cu", "binning.cu", "raster_bwd.cu",
-           "raster_fwd2.cu", "raster_fwd3.cu", "raster_bwd2.cu", "raster_bwd4.cu", "loss.cu", "smallbmm.cu", "density.cu", "comm.cu"]
+SOURCES = ["api.cu", "pergaussian.cu", "fused.cu", "binning.cu", "raster_fwd.cu", "raster_bwd.cu", "loss.cu",
+           "smallbmm.cu", "density.cu", "comm.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo",

@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_90a kernels: constants fixed by the reference,
-// mbarrier / bulk-async-copy (TMA 1-D, SASS UBLKCP) PTX wrappers, fast math.
+// Shared device helpers for the sm_90a kernels: constants fixed by the reference, fast math,
+// the rasterizers' record format and their shared-memory / cp.async PTX wrappers.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,8 +14,8 @@ constexpr float ALPHA_SKIP = 0.002f;  // kernel.cu:246
 constexpr float TAU_STOP = 0.0001f;   // kernel.cu:256
 constexpr float LOG2E = 1.4426950408889634f;
 
-// Packed per-patch record, 48 B, written by pack_records (binning.cu) in sorted order so a
-// tile's records are one contiguous 16-B aligned span -> one cp.async.bulk per batch.
+// Packed record, 48 B, one per Gaussian and indexed by Gaussian id (build_record below): the
+// rasterizers gather a tile's records through its sorted id list, three 16-byte cp.async each.
 //   q0 = (ux, uy, gsid bits, alpha)   mean in pixels, Gaussian id, opacity -- exactly the four
 //                              words the backward's moment phase needs per record (one 16-byte copy)
 //   q1 = (a, b, c, thr)        log2(g) = a dx^2 + b dx dy + c dy^2  (conic pre-scaled by
@@ -66,18 +66,6 @@ __device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) {
 }
 __device__ __forceinline__ float2 add2_rn(float2 a, float2 b) {
   return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
-}
-
-// alpha' of one record at one pixel -- THE single definition used by forward and backward
-// so both take identical skip decisions (kernel.cu:243-246 / :909-913).
-// Returns g = exp(-maha/2) through *g.
-__device__ __forceinline__ float alpha_prime(const float4 &q1, float alpha, float dx, float dy, float *g) {
-  float t = fmaf(q1.y, dy, q1.x * dx);
-  float p = fmaf(t, dx, (q1.z * dy) * dy);
-  p = fminf(p, 0.0f);  // max(0, maha)
-  float gg = ex2_approx(p);
-  *g = gg;
-  return fminf(ALPHA_CLAMP, alpha * gg);
 }
 
 // Can this record reach alpha' >= 0.002 anywhere in the pixel rectangle [bx0,bx1] x [by0,by1]?
@@ -148,59 +136,40 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   return t;
 }
 
-// ---- mbarrier + bulk async copy (global -> shared), single-CTA forms
+// ---- the rasterizers' shared-memory accesses and record gather (raster_fwd.cu, raster_bwd.cu).
+// Shared memory is addressed by 32-bit shared-window addresses; a record is gathered with three
+// 16-byte cp.async (SASS LDGSTS), tracked per lane by cp.async groups.
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+__device__ __forceinline__ uint32_t opaque_u32(uint32_t x) {  // keep an address in a register
+  uint32_t y;
+  asm volatile("mov.u32 %0, %1;" : "=r"(y) : "r"(x));
+  return y;
 }
-__device__ __forceinline__ void fence_mbar_init() {
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+  return v;
 }
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+__device__ __forceinline__ uint4 lds128u(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
+  return v;
 }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
-               "r"(bytes)
-               : "memory");
+__device__ __forceinline__ void sts64u(uint32_t a, uint32_t x, uint32_t y) {
+  asm volatile("st.shared.v2.u32 [%0], {%1, %2};" ::"r"(a), "r"(x), "r"(y) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
+__device__ __forceinline__ void cp_async16_sa(uint32_t dst, const void *src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  while (!mbar_try_wait(bar, parity)) {
-  }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
-// ---- per-thread 16-byte async copies (gather) tracked by an mbarrier: every thread of the
-// CTA issues its copies and then arrives once; the barrier (initialised with the CTA size)
-// completes the phase when all those copies have landed.
-__device__ __forceinline__ void cp_async16(void *dst_smem, const void *src_gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst_smem)), "l"(src_gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t *bar) {
-  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 1-D TMA: bytes must be a multiple of 16, both addresses 16-B aligned.
-__device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, uint32_t bytes,
-                                         uint64_t *bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::
-          "r"(smem_u32(dst_smem)),
-      "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
-      : "memory");
-}
+__device__ __forceinline__ float2 p2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ float2 p2s(float a) { return make_float2(a, a); }
 
 }  // namespace gsb
 
@@ -213,36 +182,4 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
 namespace gsb {
 int set_cuda_error(cudaError_t e, const char *what, const char *file, int line);
 int set_arg_error(const char *msg);
-
-// Stage fill of the rasterizers = a gather: lane `tid` of the 128-thread CTA fetches the 48-byte
-// record of Gaussian g into dst[tid]; `bar` flips when all n_valid records have landed.
-//   GSB_GATHER_BULK = 1: one 48-byte cp.async.bulk (TMA, SASS UBLKCP) per record, completion by
-//                        byte count (mbarrier initialised with 1: thread 0 posts the expected bytes)
-//   GSB_GATHER_BULK = 0: three 16-byte cp.async (LDGSTS) per record, every thread arrives once
-//                        (mbarrier initialised with 128)
-#ifndef GSB_GATHER_BULK
-#define GSB_GATHER_BULK 0
-#endif
-constexpr uint32_t GATHER_ARRIVALS = GSB_GATHER_BULK ? 1 : 128;
-__device__ __forceinline__ void gather_record(Rec *dst, const Rec *__restrict__ recs, int g, bool valid,
-                                              int n_valid, uint64_t *bar, int tid) {
-#if GSB_GATHER_BULK
-  if (tid == 0) mbar_expect_tx(bar, (uint32_t)n_valid * (uint32_t)sizeof(Rec));
-  if (valid) {
-    fence_proxy_async();
-    bulk_g2s(dst + tid, recs + g, (uint32_t)sizeof(Rec), bar);
-  }
-#else
-  (void)n_valid;
-  if (valid) {
-    const char *s = reinterpret_cast<const char *>(recs + g);
-    char *d = reinterpret_cast<char *>(dst + tid);
-    cp_async16(d, s);
-    cp_async16(d + 16, s + 16);
-    cp_async16(d + 32, s + 32);
-  }
-  cp_async_mbar_arrive(bar);
-#endif
-}
-
 }  // namespace gsb

@@ -9,14 +9,13 @@
 //                and the final loss scalar.
 // Algorithmic bytes: 24 (read img, gt) + 36 (write maps) + 36 + 24 (read) + 12 (write grad)
 // = 132 B per pixel (x3 channels already counted) -> HBM roofline.
-#include <stdlib.h>
-
+// Two implementations of that pair, chosen by image size alone: the row-streaming kernels
+// (k_ssim_{fwd,bwd}_rows, below) for every image with H * W < 2^31 / 9 (about 239 Mpixels), and
+// the tiled kernels k_ssim_fwd / k_ssim_bwd above that.  The row kernels index with 32-bit ints,
+// and the bound keeps the whole nine-plane map buffer (9 H W floats) within their range.
 #include "common.cuh"
 #include "kernels.h"
 
-#ifndef GSB_LOSS_DEFAULT_VARIANT
-#define GSB_LOSS_DEFAULT_VARIANT 1
-#endif
 #ifndef GSB_LOSS_FWD_MINB  // resident CTAs (of 4 warps) the row kernels are compiled for
 #define GSB_LOSS_FWD_MINB 4
 #endif
@@ -209,7 +208,7 @@ __global__ void __launch_bounds__(256) k_ssim_bwd(int W, int H, const float *__r
 }
 
 // ---------------------------------------------------------------------------------------
-// Row-streaming variant (default).  The tiled kernels above spend most of their instructions on
+// Row-streaming kernels.  The tiled kernels above spend most of their instructions on
 // staging (index arithmetic, shared-memory traffic for both passes); here one lane owns one
 // image COLUMN and walks down a strip of rows:
 //   * a row of img and gt goes through a 48-column per-warp shared-memory line (the warp's 32
@@ -311,7 +310,7 @@ __global__ void __launch_bounds__(32 * SWARPS, GSB_LOSS_FWD_MINB) k_ssim_fwd_row
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int x0 = (blockIdx.x * SWARPS + wid) * 32, x = x0 + lane;
   const int yb = blockIdx.y * SH, ye = min(yb + SH, H), c = blockIdx.z;
-  const int HW = H * W;  // (the host keeps H * W < 2^31 / 9 for this variant)
+  const int HW = H * W;  // (the host keeps H * W < 2^31 / 9 for these kernels)
   float *__restrict__ mp0 = maps + (size_t)c * HW, *__restrict__ mp1 = mp0 + (size_t)3 * HW,
                       *__restrict__ mp2 = mp0 + (size_t)6 * HW;
   const bool xin = x < W;
@@ -469,13 +468,8 @@ __global__ void __launch_bounds__(32 * SWARPS, GSB_LOSS_BWD_MINB) k_ssim_bwd_row
 }
 
 // rows per strip: about one resident wave of warps (a strip pays 10 halo rows, so the longer the
-// better, but every SM needs its share); GSB_LOSS_STRIP overrides (A/B)
+// better, but every SM needs its share)
 static int strip_rows(int H, int W) {
-  static const int forced = [] {
-    const char *e = getenv("GSB_LOSS_STRIP");
-    return e != nullptr ? atoi(e) : 0;
-  }();
-  if (forced > 0) return forced;
   int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int xblocks = (W + 32 * SWARPS - 1) / (32 * SWARPS);
@@ -505,11 +499,7 @@ int launch_gau_loss(int H, int W, const float *img, const float *gt, float lambd
   double *acc = static_cast<double *>(ws);
   float *maps = reinterpret_cast<float *>(static_cast<char *>(ws) + 256);
   GSB_CUDA_TRY(cudaMemsetAsync(acc, 0, 2 * sizeof(double), st));
-  static const int variant = [] {  // 1 = row streaming (default), 0 = the tiled kernels (A/B)
-    const char *e = getenv("GSB_LOSS_VARIANT");
-    return e != nullptr ? atoi(e) : GSB_LOSS_DEFAULT_VARIANT;
-  }();
-  if (variant == 1 && (long long)H * W < (1ll << 31) / 9) {  // (int element offsets inside the kernels)
+  if ((long long)H * W < (1ll << 31) / 9) {  // (int element offsets inside the row kernels)
     const int SH = strip_rows(H, W);
     const dim3 grid((W + 32 * SWARPS - 1) / (32 * SWARPS), (H + SH - 1) / SH, 3);
     // 16-byte row loads need every row (and plane) of all five arrays 16-byte aligned

@@ -35,9 +35,9 @@ def test_library_exports_every_declared_symbol():
     assert "draw" in names and "draw_backward" in names
 
 
-def test_no_library_kernels_and_host_only_entry_points():
-    """the binary holds no CUB / thrust kernel (round 1 sorted and scanned with them), and the
-    host-only workspace queries answer without a GPU"""
+def test_no_library_or_retired_kernels_and_host_only_entry_points():
+    """the binary holds no CUB / thrust kernel (round 1 sorted and scanned with them) and none of the
+    retired CTA-per-tile rasterizers, and the host-only workspace queries answer without a GPU"""
     from easygaussiansplatting_b200 import _lib, build
     build.build()
     lib = _lib.load()
@@ -46,8 +46,9 @@ def test_no_library_kernels_and_host_only_entry_points():
     assert len(kernels) > 30
     assert not [ln for ln in kernels if "cub" in ln or "thrust" in ln], "a library kernel is linked in"
     for name in ("k_rects_scan", "k_radix_pass", "k_colscan", "k_density_slots", "k_density_apply_rows",
-                 "k_ssim_fwd_rows", "k_ssim_bwd_rows", "k_draw3", "k_draw_bwd4"):
-        assert any(name in ln for ln in kernels), name
+                 "k_ssim_fwd_rows", "k_ssim_bwd_rows", "k_draw", "k_draw_bwd"):
+        assert any(name + "E" in ln or name + "I" in ln for ln in kernels), name  # mangled: name, then E or I
+    assert not [ln for ln in kernels if re.search(r"k_draw(_bwd)?2", ln)], "a retired rasterizer is linked in"
     prev = 0
     for n in (0, 1, 1000, 1 << 20, 5 << 20):
         b = lib.gsb_density_workspace_bytes(n)
@@ -58,17 +59,21 @@ def test_no_library_kernels_and_host_only_entry_points():
     assert lib.gsb_splat_workspace_bytes(1000, 64, 64, 10) <= lib.gsb_splat_workspace_bytes(1000, 64, 64, 100000)
 
 
-def test_library_is_sm90a_with_async_record_gather():
-    """built for sm_90a only; the rasterizers stage records with 16-byte async copies tracked by an
-    mbarrier (SASS LDGSTS + LDGSTSBAR arrive-on + SYNCS try-wait) and use the MUFU exp2"""
+def test_rasterizers_are_sm90a_with_cp_async_record_gather():
+    """built for sm_90a only; each rasterizer (k_draw, k_draw_bwd) gathers records with 16-byte
+    async copies tracked by cp.async groups (SASS LDGSTS + LDGDEPBAR commit + DEPBAR wait) and
+    uses the MUFU exp2"""
     from easygaussiansplatting_b200 import _lib, build
     build.build()
     r = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True)
     archs = set(re.findall(r"code for (sm_\w+)", r.stdout))
     assert archs == {"sm_90a"}, archs
-    assert "LDGSTS.E.BYPASS.128" in r.stdout and "LDGSTSBAR" in r.stdout, "async record gather missing"
-    assert "SYNCS.PHASECHK" in r.stdout, "mbarrier wait missing"
-    assert "MUFU.EX2" in r.stdout
+    funcs = re.split(r"\n\s*Function : ", r.stdout)
+    for name in ("k_draw", "k_draw_bwd"):
+        body = [f for f in funcs if f.startswith("_ZN3gsb%d%sE" % (len(name), name))]
+        assert len(body) == 1, name
+        for op in ("LDGSTS.E.BYPASS.128", "LDGDEPBAR", "DEPBAR.LE", "MUFU.EX2"):
+            assert op in body[0], "%s: %s missing" % (name, op)
 
 
 def test_ops_refuse_cpu_tensors():
