@@ -170,6 +170,10 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
       int item = 0;
       if (lane == 0) item = atomicAdd(work, 1);
       item = __shfl_sync(0xffffffffu, item, 0);
+      // a whole-tile gather whose four blocks all skipped (outside the image / nothing composited)
+      // was never waited for: drain it before the next gather reuses the ring, or the warp exits
+      cp_async_wait<0>();
+      __syncwarp();
       if (item >= items) break;
       const int ent = __ldg(entries + item);
       const int code = ent & 7;

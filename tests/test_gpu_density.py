@@ -157,6 +157,64 @@ def test_plan_and_apply_vs_oracle(N, seed):
         assert torch.equal(dst2[k], dst[k])
 
 
+def random_state_device(N, seed, sense=5.0):
+    """random_state's distribution, drawn on the GPU from a seeded torch.Generator"""
+    gen = torch.Generator(device=DEV).manual_seed(seed)
+    U = lambda shape, a, b: torch.empty(shape, device=DEV).uniform_(a, b, generator=gen)
+    Nn = lambda shape, s=1.0: torch.empty(shape, device=DEV).normal_(0.0, s, generator=gen)
+    scale = U((N, 1), np.log(0.002 * sense), np.log(0.12 * sense)).exp_() * U((N, 3), 0.6, 1.5)
+    P = dict(pws=U((N, 3), -2, 2), low_shs=Nn((N, 3)), high_shs=Nn((N, 45), 0.1), alphas_raw=U((N, 1), -7.5, 4),
+             scales_raw=scale.log_(), rots_raw=Nn((N, 4)).mul_(U((N, 1), 0.3, 2)))
+    M = {k: Nn(v.shape, 1e-3) for k, v in P.items()}
+    V = {k: U(v.shape, 0.0, 1e-6) for k, v in P.items()}
+    cnt = torch.randint(0, 6, (N,), device=DEV, generator=gen, dtype=torch.int32)
+    acc = Nn((N, 1), 1.5e-6).abs_().mul_((cnt > 0).unsqueeze(1))
+    return P, M, V, acc, cnt
+
+
+def test_apply_64bit_kernel_equals_row_group_slices():
+    """N = 23 000 037 takes the per-element kernel with 64-bit indices (all 18 parameter /
+    Adam-moment jobs, element offsets past 1e9 in high_shs); two row slices below 23 M take the
+    row-group kernel.  Classification is per row and slots are prefix sums, so each output row
+    of the full run has a known place in one slice's output: kept row k of slice 2 is full row
+    K1 + k, its clones K + C1 + c, its splits K + C + S1 + s.  All rows must be bit-identical."""
+    from easygaussiansplatting_b200 import density
+    N, N1 = 23_000_037, 11_500_011
+    need = 44 << 30
+    free, total = torch.cuda.mem_get_info()
+    if free < need:
+        pytest.skip("needs %.1f GB of free device memory, %.1f GB of %.1f GB free" % (need / 2**30, free / 2**30,
+                                                                                    total / 2**30))
+    torch.cuda.reset_peak_memory_stats()
+    P, M, V, acc, cnt = random_state_device(N, 23)
+    th = density.raw_thresholds(5.0)
+    cls, slots, (K, Cn, S) = density.plan(P["alphas_raw"], P["scales_raw"], acc, cnt, th)
+    assert K > 0 and Cn > 0 and S > 0 and 0.9 * N < K + Cn + S < 1.1 * N, (K, Cn, S)
+    z = torch.randn((S, 3), device=DEV, generator=torch.Generator(device=DEV).manual_seed(1))
+    full = density.apply(cls, slots, (K, Cn, S), P, M, V, z)
+    sl = lambda d, a, b: {k: v[a:b] for k, v in d.items()}
+    c_done = s_done = 0
+    for a, b in ((0, N1), (N1, N)):
+        cls_i, slots_i, (Ki, Ci, Si) = density.plan(P["alphas_raw"][a:b], P["scales_raw"][a:b], acc[a:b], cnt[a:b],
+                                                   th)
+        assert torch.equal(cls_i, cls[a:b])
+        k_done = 0 if a == 0 else K - Ki
+        part = density.apply(cls_i, slots_i, (Ki, Ci, Si), sl(P, a, b), sl(M, a, b), sl(V, a, b),
+                             z[s_done:s_done + Si])
+        for d_full, d_part, what in zip(full, part, ("param", "exp_avg", "exp_avg_sq")):
+            for k in NAMES:
+                f, p = d_full[k], d_part[k]
+                assert torch.equal(f[k_done:k_done + Ki], p[:Ki]), (a, what, k, "kept")
+                assert torch.equal(f[K + c_done:K + c_done + Ci], p[Ki:Ki + Ci]), (a, what, k, "cloned")
+                assert torch.equal(f[K + Cn + s_done:K + Cn + s_done + Si], p[Ki + Ci:]), (a, what, k, "split")
+        c_done, s_done = c_done + Ci, s_done + Si
+        del part, cls_i, slots_i
+        torch.cuda.empty_cache()
+    assert c_done == Cn and s_done == S
+    print("N %d: K %d C %d S %d, peak device memory %.2f GB" % (N, K, Cn, S,
+                                                                  torch.cuda.max_memory_allocated() / 2**30))
+
+
 def test_degenerate_populations():
     """everything pruned / nothing selected / N = 0"""
     from easygaussiansplatting_b200 import density

@@ -80,7 +80,8 @@ def run_both(sc, W, H, seed=0):
     return out
 
 
-@pytest.mark.parametrize("N,W,H,sh_dim", [(20000, 320, 240, 48), (3000, 250, 130, 12), (500, 64, 64, 3)])
+@pytest.mark.parametrize("N,W,H,sh_dim", [(20000, 320, 240, 48), (3000, 250, 130, 12), (500, 64, 64, 3),
+                                          (4000, 979, 546, 27)])
 def test_fused_function_matches_op_surface(N, W, H, sh_dim):
     a, b = run_both(scene(N, W, H, sh_dim, N + (N // 1000) % 2), W, H, N)  # 3000 -> rotated camera
     assert torch.equal(a["mask"], b["mask"])
@@ -237,7 +238,7 @@ def _lib_call_preprocess_with_records_only(ops, P, cam, N):
                                           *[x.data_ptr() for x in o], None, rec.data_ptr(), None), lib)
 
 
-@pytest.mark.parametrize("N,W,H", [(20000, 320, 240), (400, 1000, 700)])
+@pytest.mark.parametrize("N,W,H", [(20000, 320, 240), (400, 1000, 700), (3000, 979, 546)])
 def test_capacity_path_equals_exact_path(N, W, H):
     """gsb_splat_forward (sort sized from the previous frame, status read after everything is
     enqueued) gives bit-identical outputs to gsb_splat_bin + gsb_splat_render; a frame that outgrows

@@ -171,19 +171,26 @@ def test_inverse_cov2d_nan_cull():
 def run_splat_case(N, W, H, sh_dim=3, seed=0, check_bwd=True, sc=None, tol_scale=1.0):
     # tol_scale > 1 only for adversarial scenes whose fp32 Mahalanobis terms cancel (see the
     # huge/needle test); every BASELINE-shaped case runs at 1.
-    g = gsc()
     sc = sc or scene_with_culls(N, W, H, sh_dim, seed)
     o = stage_pipeline(sc, calc_J=False)
-    alphas = t(sc["alphas"])
-    us, cinv, col = n(o["us"]), n(o["cinv2ds"]), n(o["colors"])
-    d_in, a_in = n(o["depths"]).copy(), n(o["areas"]).copy()
-    image, contrib, ftau, ranges, gsid = g.splat(H, W, o["us"], o["cinv2ds"], alphas, o["depths"], o["colors"],
-                                                 o["areas"])
+    out, ref = check_splat_vs_oracle(H, W, o["us"], o["cinv2ds"], t(sc["alphas"]), o["depths"], o["colors"],
+                                     o["areas"], seed=seed, check_bwd=check_bwd, tol_scale=tol_scale)
+    return sc, o, out, ref
+
+
+def check_splat_vs_oracle(H, W, us_d, cinv_d, alphas_d, depths_d, colors_d, areas_d, seed=0, check_bwd=True,
+                          tol_scale=1.0):
+    """splat (+ splatB) on op-level device inputs against the oracle on the same fp32 values.
+    depths_d / areas_d are culled in place, like the op does.  -> (splat outputs, oracle forward)"""
+    g = gsc()
+    us, cinv, col, al = n(us_d), n(cinv_d), n(colors_d), n(alphas_d)
+    d_in, a_in = n(depths_d).copy(), n(areas_d).copy()
+    image, contrib, ftau, ranges, gsid = g.splat(H, W, us_d, cinv_d, alphas_d, depths_d, colors_d, areas_d)
     d_or, a_or = d_in.copy(), a_in.copy()
-    ref = orc.splat(H, W, us, cinv, sc["alphas"], d_or, col, a_or, margin=2e-5 * tol_scale)
+    ref = orc.splat(H, W, us, cinv, al, d_or, col, a_or, margin=2e-5 * tol_scale)
     # integer side: bit exact, including the in-place culls
-    assert np.array_equal(n(o["depths"]), d_or), "in-place depth cull differs"
-    assert np.array_equal(n(o["areas"]), a_or), "in-place areas cull differs"
+    assert np.array_equal(n(depths_d), d_or), "in-place depth cull differs"
+    assert np.array_equal(n(areas_d), a_or), "in-place areas cull differs"
     assert gsid.numel() == ref["P"]
     assert np.array_equal(n(ranges), ref["ranges"]), "patch_range_per_tile differs"
     assert np.array_equal(n(gsid), ref["gsid"]), "gsid_per_patch (sort order) differs"
@@ -198,11 +205,10 @@ def run_splat_case(N, W, H, sh_dim=3, seed=0, check_bwd=True, sc=None, tol_scale
     terr = np.abs(n(ftau).astype(np.float64) - ref["final_tau"])
     assert terr[~amb].max(initial=0) <= 1e-5 * tol_scale, "final_tau err %.3e" % terr[~amb].max()
     if not check_bwd:
-        return sc, o, (image, contrib, ftau, ranges, gsid), ref
+        return (image, contrib, ftau, ranges, gsid), ref
     dl = upstream_gradient(W, H, seed) * (3.0 * W * H)  # O(1) upstream gradient
-    grads = g.splatB(H, W, o["us"], o["cinv2ds"], alphas, o["depths"], o["colors"], contrib, ftau, ranges, gsid,
-                     t(dl))
-    *refg, amb_gs = orc.splat_backward(H, W, us, cinv, sc["alphas"], col, ref, dl, return_ambiguous=True,
+    grads = g.splatB(H, W, us_d, cinv_d, alphas_d, depths_d, colors_d, contrib, ftau, ranges, gsid, t(dl))
+    *refg, amb_gs = orc.splat_backward(H, W, us, cinv, al, col, ref, dl, return_ambiguous=True,
                                          margin=2e-5 * tol_scale)
     # Gaussians with a replayed alpha' within 2e-5 of the 0.002 skip threshold may take the
     # other branch in fp32, which moves their own gradient by one whole pixel term (the conic
@@ -215,16 +221,126 @@ def run_splat_case(N, W, H, sh_dim=3, seed=0, check_bwd=True, sc=None, tol_scale
         assert err[~amb_gs].max(initial=0) / s <= 1e-4 * tol_scale, "%s: normalised max err %.3e" % (
             name, err[~amb_gs].max() / s)
         assert err.max(initial=0) / s <= 5e-3 * tol_scale, "%s: ambiguous-Gaussian err %.3e" % (name, err.max() / s)
-    return sc, o, (image, contrib, ftau, ranges, gsid), ref
+    return (image, contrib, ftau, ranges, gsid), ref
 
 
 @pytest.mark.parametrize("N,W,H", [(10000, 256, 256),      # BASELINE config 1 shape
                                    (3000, 250, 130),       # ragged right / bottom tiles
                                    (50000, 512, 512),      # config 4 corner
                                    (4001, 320, 200),       # rotated camera, un-normalised quaternions
-                                   (200, 64, 48)])
+                                   (200, 64, 48),
+                                   (3000, 979, 546),       # odd W and H: scalar stores at the right edge
+                                   (2000, 255, 131),
+                                   (40, 17, 9),            # smaller than one tile in y, two tiles in x
+                                   (8, 7, 5)])             # smaller than one 8x8 block
 def test_splat_and_splatB_vs_oracle(N, W, H):
+    # (seed N: the tiny frames' scenes have no threshold-ambiguous pixel or Gaussian at all -- with
+    # 35 pixels a single one would exceed the cap)
     run_splat_case(N, W, H, seed=N)
+
+
+def gaussians_in_tile(tx, ty, k, rng, sigma=(1.5, 4.0), alpha=(0.05, 0.9), lo=4.0, hi=12.0, z0=1.0, area=4):
+    """k Gaussians whose binning box stays inside tile (tx, ty): means within [16 t + lo, 16 t + hi)
+    with area <= lo and hi + area <= 17, so each adds exactly one patch to that tile.
+    Depths z0 + 0.01 j give list position j.  -> (us, cinv2ds, alphas, depths, colors, areas)"""
+    us = np.stack([16 * tx + rng.uniform(lo, hi, k), 16 * ty + rng.uniform(lo, hi, k)], axis=1)
+    sx, sy, th = rng.uniform(*sigma, k), rng.uniform(*sigma, k), rng.uniform(0, np.pi, k)
+    c, s = np.cos(th), np.sin(th)
+    cinv = np.stack([c * c / sx ** 2 + s * s / sy ** 2, c * s * (1 / sx ** 2 - 1 / sy ** 2),
+                     s * s / sx ** 2 + c * c / sy ** 2], axis=1)
+    return (us, cinv, rng.uniform(*alpha, k), z0 + 0.01 * np.arange(k), rng.uniform(0, 1, (k, 3)),
+            np.full((k, 2), area, np.int32))
+
+
+def op_inputs(parts):
+    """concatenates gaussians_in_tile groups into device tensors of the splat op surface"""
+    cols = [np.concatenate([p[i] for p in parts]) for i in range(6)]
+    f32 = lambda a: t(a.astype(np.float32))
+    return f32(cols[0]), f32(cols[1]), f32(cols[2]), f32(cols[3]), f32(cols[4]), t(cols[5], torch.int32)
+
+
+def test_splat_patch_count_and_survivor_boundaries():
+    """Scenes built at the op surface so that every tile's patch count is exactly what was put
+    there: whole-tile entries (<= 32 patches) against four-entry tiles (>= 33) and the 32-record
+    chunk edges at 32/33, 64/65; 6-9 and 16-17 survivors in one 8x8 block (the backward's phase-B
+    flushes); opacities 0.99, nextafter(0.99, 1) and 1.0 at list positions 30-33 (above the clamp:
+    the backward's shuffle path); and near-opaque stacks whose last composited record is list
+    index 31, 32 or 33."""
+    rng = np.random.default_rng(7)
+    gx, parts, expect = 8, [], {}
+    tile = iter(range(1000))
+
+    def add(k, **kw):
+        i = next(tile)
+        parts.append(gaussians_in_tile(i % gx, i // gx, k, rng, **kw))
+        expect[i] = k
+        return i, parts[-1]
+
+    for k in (1, 2, 31, 32, 33, 63, 64, 65, 97):
+        add(k, alpha=(0.02, 0.3) if k > 32 else (0.05, 0.9))
+    survivor_tiles = {}
+    for s in (6, 7, 8, 9, 16, 17):
+        # sigma <= 0.9 px, mean within [2.5, 4.5]: alpha' >= 0.002 needs a distance < 3.2 px, so
+        # only block 0 of the tile keeps these records
+        i, _ = add(s, sigma=(0.6, 0.9), alpha=(0.3, 0.9), lo=2.5, hi=4.5, area=2)
+        survivor_tiles[i] = s
+    for k, pos in ((34, (0.99, np.nextafter(np.float32(0.99), np.float32(1)), 1.0, 1.0)), (32, (1.0, 0.99))):
+        _, p = add(k, sigma=(3.0, 6.0), alpha=(0.02, 0.1))
+        p[2][30:30 + len(pos)] = pos
+    stack_tiles = {}
+    for m in (30, 31, 32):
+        # sigma 200 px: g ~ 1 over the whole tile, so every pixel composites the same list: m records
+        # of alpha 0.05 (tau 0.95^m), then alpha 1.0 (alpha' clamped to 0.99): the second opaque
+        # record drives tau below 1e-4, so the last composited record is list index m + 1
+        i, p = add(40, sigma=(200.0, 200.0), alpha=(0.05, 0.05))
+        p[2][m:] = 1.0
+        stack_tiles[i] = m + 2
+    W, H = 16 * gx, 16 * ((len(expect) + gx - 1) // gx)
+    (image, contrib, ftau, ranges, gsid), ref = check_splat_vs_oracle(H, W, *op_inputs(parts), seed=7)
+    lens = ref["ranges"][:, 1] - ref["ranges"][:, 0]
+    for i, k in expect.items():
+        assert lens[i] == k, (i, lens[i], k)
+    assert (lens[len(expect):] == 0).all()
+    con = ref["contrib"]
+    for i, s in survivor_tiles.items():
+        blk = con[16 * (i // gx):16 * (i // gx) + 16, 16 * (i % gx):16 * (i % gx) + 16].copy()
+        assert blk[:8, :8].max() > 0
+        blk[:8, :8] = 0
+        assert not blk.any(), "survivors of tile %d reach beyond block 0" % i
+    for i, c in stack_tiles.items():
+        assert (con[16 * (i // gx):16 * (i // gx) + 16, 16 * (i % gx):16 * (i % gx) + 16] == c).all(), i
+
+
+def test_splat_dead_sparse_tiles_and_64bit_keys():
+    """3840x2160 with 1-3 patches in every tile: the backward's whole-tile entries alternate between
+    live tiles and dead ones whose patches all have alpha 0.0015 (no pixel composites anything,
+    so all four blocks skip after the tile's record gather was issued), about ten entries per
+    resident warp in a row.  A tenth of the Gaussians sit near 1 km: depth keys of ~20 bits plus
+    15 tile bits need the 64-bit sort key layout."""
+    rng = np.random.default_rng(11)
+    W, H = 3840, 2160
+    gx, gy = W // 16, H // 16
+    parts = []
+    for ty in range(gy):
+        for tx in range(gx):
+            dead = (tx + ty) % 2 == 1
+            p = gaussians_in_tile(tx, ty, int(rng.integers(1, 4)), rng, sigma=(1.0, 4.0),
+                                  alpha=(0.0015, 0.0015) if dead else (0.1, 0.9), z0=rng.uniform(1.0, 20.0))
+            parts.append(p)
+    far = rng.random(len(parts)) < 0.1
+    for p, f in zip(parts, far):
+        if f:
+            p[3][:] = rng.uniform(900.0, 1100.0) + 0.01 * np.arange(len(p[3]))
+    (image, contrib, ftau, ranges, gsid), ref = check_splat_vs_oracle(H, W, *op_inputs(parts), seed=11)
+    lens = ref["ranges"][:, 1] - ref["ranges"][:, 0]
+    assert lens.min() >= 1 and lens.max() <= 3
+    # whole-tile entries that render nothing: exactly the alpha-0.0015 tiles
+    dead_tiles = ref["contrib"].reshape(gy, 16, gx, 16).max(axis=(1, 3)) == 0
+    assert np.array_equal(dead_tiles, (np.add.outer(np.arange(gy), np.arange(gx)) % 2) == 1)
+    assert dead_tiles.sum() == gx * gy // 2
+    depth_bits = int((ref["keys"] & 0xFFFFFFFF).max()).bit_length()
+    tile_bits = (gx * gy - 1).bit_length()
+    assert depth_bits >= 20 and tile_bits == 15 and depth_bits + tile_bits > 32
 
 
 def test_splat_dense_early_termination():

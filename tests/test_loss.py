@@ -62,7 +62,8 @@ def _torch_gau_loss(image, gt, lam=0.2):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("H,W", [(37, 53), (16, 16), (128, 96), (1080, 1920)])
+@pytest.mark.parametrize("H,W", [(37, 53), (16, 16), (128, 96), (1080, 1920),
+                                 (1, 1), (2, 300), (300, 2), (15, 31)])   # strips narrower than a warp
 def test_gpu_gau_loss_vs_oracle(H, W):
     from easygaussiansplatting_b200.loss import gau_loss, gau_loss_with_grad
     rng = np.random.default_rng(H * 1000 + W)
@@ -90,6 +91,103 @@ def test_gpu_gau_loss_vs_oracle(H, W):
     t3 = torch.from_numpy(img).cuda().requires_grad_()
     (3.0 * gau_loss(t3, tg)).backward()
     assert torch.allclose(t3.grad, 3.0 * ti.grad, rtol=1e-6, atol=0)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("which", ["img", "gt"])
+def test_gpu_gau_loss_unaligned_view_is_bit_identical(which):
+    """W % 4 == 0, but the image starts one float into its storage: the row kernels take their
+    scalar loads instead of the 16-byte ones, with the same arithmetic -- loss and gradient are
+    bit-identical to the aligned call"""
+    from easygaussiansplatting_b200.loss import gau_loss_with_grad
+    H, W = 45, 136
+    rng = np.random.default_rng(5)
+    img = torch.from_numpy(rng.uniform(0, 1, (3, H, W)).astype(np.float32)).cuda()
+    gt = torch.from_numpy(rng.uniform(0, 1, (3, H, W)).astype(np.float32)).cuda()
+    la, ga = gau_loss_with_grad(img, gt, 0.2)
+    buf = torch.empty(3 * H * W + 1, device="cuda")
+    view = buf[1:].view(3, H, W)
+    view.copy_(img if which == "img" else gt)
+    assert view.is_contiguous() and view.data_ptr() % 16 == 4
+    lb, gb = gau_loss_with_grad(view, gt, 0.2) if which == "img" else gau_loss_with_grad(img, view, 0.2)
+    assert torch.equal(la, lb) and torch.equal(ga, gb)
+
+
+def _patched_pair(H, W, corners, rng, P=64):
+    """img, gt [3, H, W] on the GPU: zero except P x P patches of random content at `corners`"""
+    img = torch.zeros((3, H, W), device="cuda")
+    gt = torch.zeros((3, H, W), device="cuda")
+    for (y, x) in corners:
+        a = rng.uniform(0, 1, (3, P, P)).astype(np.float32)
+        b = np.clip(a + rng.normal(scale=0.1, size=a.shape), 0, 1).astype(np.float32)
+        img[:, y:y + P, x:x + P] = torch.from_numpy(a).cuda()
+        gt[:, y:y + P, x:x + P] = torch.from_numpy(b).cuda()
+    return img, gt
+
+
+@pytest.mark.gpu
+def test_gpu_gau_loss_at_and_above_the_tiled_bound():
+    """The loss at two sizes next to the switch between the row kernels and the tiled kernels
+    (H W < 2^31 / 9, about 238.6 Mpixels): 14563 x 16384 is the largest row-path image of that
+    width (vector loads), 14567 x 16381 is just above it and takes the tiled kernels with ragged
+    tiles on both axes (W % 32 = 29, H % 16 = 7) and map offsets past 2^31 in channel 2.
+
+    img = gt = 0 except a few 64 x 64 patches (image corners -- the largest offsets of every
+    channel -- and across tile / CTA / strip boundaries).  With zero padding no pixel sees content
+    more than 10 px away, so inside a crop with >= 20 zero pixels (or the image edge) around its
+    patch the gradient is the oracle's gradient of the crop times n_crop / n_full, and it is
+    exactly 0 everywhere else."""
+    from easygaussiansplatting_b200.loss import gau_loss_with_grad
+    need = 18 << 30
+    free, total = torch.cuda.mem_get_info()
+    if free < need:
+        pytest.skip("needs %.1f GB of free device memory, %.1f GB of %.1f GB free" % (need / 2**30, free / 2**30,
+                                                                                    total / 2**30))
+    # the kernels' fp32 SSIM of an all-zero neighbourhood (C1 C2 / (C1 C2) need not round to 1)
+    z = torch.zeros((3, 32, 32), device="cuda")
+    ssim0 = 1.0 - float(gau_loss_with_grad(z, z, 1.0, want_grad=False)[0])
+    lam, P, M = 0.2, 64, 20
+    torch.cuda.reset_peak_memory_stats()
+    for H, W in ((14563, 16384), (14567, 16381)):
+        rng = np.random.default_rng(H)
+        corners = [(0, 0), (H - P, W - P), (0, W - P), (H - P, 0),
+                   (H // 2 - 37, 128 * 60 - 29),           # row path: CTA boundary (128 columns)
+                   (16 * 401 - 31, 32 * 223 - 17),         # tiled: corners of 32 x 16 tiles
+                   (7 * H // 8 + 3, W // 3 + 5)]
+        img, gt = _patched_pair(H, W, corners, rng, P)
+        loss, grad = gau_loss_with_grad(img, gt, lam)
+        n_full = 3.0 * H * W
+        l1_sum = ss_sum = 0.0
+        n_crops = 0.0
+        for (y, x) in corners:
+            y0, y1, x0, x1 = max(0, y - M), min(H, y + P + M), max(0, x - M), min(W, x + P + M)
+            ci = img[:, y0:y1, x0:x1].cpu().numpy()
+            cg = gt[:, y0:y1, x0:x1].cpu().numpy()
+            ref = orc.gau_loss(ci, cg, lam)
+            n_crop = float(ci.size)
+            want = ref["dloss_dimage"] * (n_crop / n_full)
+            got = grad[:, y0:y1, x0:x1].cpu().numpy().astype(np.float64)
+            e = np.abs(got - want).max() / np.abs(want).max()
+            assert e < 3e-4, (H, W, y, x, e)   # the bound of test_gpu_gau_loss_vs_oracle
+            l1_sum += ref["l1"] * n_crop
+            ss_sum += ref["ssim"] * n_crop
+            n_crops += n_crop
+            grad[:, y0:y1, x0:x1] = 0
+        assert not bool(grad.any()), "gradient outside the patch crops (%d x %d)" % (H, W)
+        # the background counts at the kernels' SSIM of zero.  Tolerance: inside the crops the
+        # oracle's zero pixels have SSIM exactly 1 where the kernels have ssim0, and the kernels
+        # add fp32 per-pixel SSIMs in partial sums before the double accumulation: per pixel at
+        # most 1 - ssim0 plus a rounding of ~2^-24 per level of a (log-depth) shuffle tree, i.e.
+        # |d mean SSIM| <= |1 - ssim0| + 16 * 2^-24; L1 is exact outside the patches.
+        want_loss = (1 - lam) * l1_sum / n_full + lam * (1.0 - (ss_sum + (n_full - n_crops) * ssim0) / n_full)
+        tol = lam * (abs(1.0 - ssim0) + 16 * 2.0 ** -24) + 1e-5 * abs(want_loss)
+        assert abs(float(loss) - want_loss) <= tol, (H, W, float(loss), want_loss, tol)
+        # L1 alone (lambda = 0) has no background term: fp32 loss to a few ulps
+        l0, _ = gau_loss_with_grad(img, gt, 0.0, want_grad=False)
+        assert abs(float(l0) - l1_sum / n_full) <= 1e-5 * l1_sum / n_full, (H, W)
+        del img, gt, loss, grad, l0
+        torch.cuda.empty_cache()
+    print("peak device memory %.2f GB" % (torch.cuda.max_memory_allocated() / 2**30))
 
 
 @pytest.mark.gpu
