@@ -222,6 +222,15 @@ int gsb_gau_loss(int H, int W, const float *image, const float *gt_image, float 
   return launch_gau_loss(H, W, image, gt_image, loss_lambda, loss_out, dloss_dimage, ws, (cudaStream_t)stream);
 }
 
+// The rasterizer writes the three image planes with 16-byte stores and the binning writes the
+// tile ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h).
+static bool planes_aligned(const float *image, const int32_t *contrib, const float *final_tau,
+                           const int32_t *ranges) {
+  const uintptr_t planes = reinterpret_cast<uintptr_t>(image) | reinterpret_cast<uintptr_t>(contrib) |
+                           reinterpret_cast<uintptr_t>(final_tau);
+  return (planes & 15) == 0 && (reinterpret_cast<uintptr_t>(ranges) & 7) == 0;
+}
+
 size_t gsb_splat_bin_workspace_bytes(int N) { return bin_layout(N).bytes; }
 
 int gsb_splat_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
@@ -263,6 +272,7 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
                      int32_t *patch_range_per_tile, int32_t *gsid_per_patch, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splat: bad N/H/W/P");
   GSB_REQUIRE(image && contrib && final_tau && patch_range_per_tile, "splat: null output");
+  GSB_REQUIRE(planes_aligned(image, contrib, final_tau, patch_range_per_tile), "splat: misaligned output");
   GSB_REQUIRE(P == 0 || (us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch),
               "splat: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -293,6 +303,7 @@ static int splat_forward_impl(int H, int W, int N, const float *us, const float 
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad N/H/W/P_cap");
   GSB_REQUIRE(image && contrib && final_tau && patch_range_per_tile && gsid_per_patch && status_host && bin_ws && ws,
               "splat_forward: null pointer");
+  GSB_REQUIRE(planes_aligned(image, contrib, final_tau, patch_range_per_tile), "splat_forward: misaligned output");
   GSB_REQUIRE(N == 0 || (us && cinv2ds && alphas && depths && colors && areas), "splat_forward: null pointer");
   GSB_REQUIRE((reinterpret_cast<uintptr_t>(packed_records) & 15) == 0, "splat_forward: packed_records misaligned");
   cudaStream_t st = (cudaStream_t)stream;

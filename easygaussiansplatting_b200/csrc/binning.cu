@@ -19,6 +19,7 @@
 // Every pass is stable, so ties keep ascending Gaussian id exactly like thrust::sort_by_key.
 #include "common.cuh"
 #include "kernels.h"
+#include "tile_io.cuh"
 
 namespace gsb {
 
@@ -64,8 +65,8 @@ __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long
 constexpr int RS_CTA = 256, RS_ITEMS = 4, RS_SPAN = RS_CTA * RS_ITEMS;
 constexpr unsigned long long DESC_AGG = 1ull << 62, DESC_INC = 2ull << 62, DESC_VAL = (1ull << 62) - 1;
 
-__global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float2 *__restrict__ us,
-                                                       int2 *__restrict__ areas, float *__restrict__ depths,
+__global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__restrict__ us,
+                                                       int32_t *__restrict__ areas, float *__restrict__ depths,
                                                        int gx, int gy, uint2 *__restrict__ rects,
                                                        uint32_t *__restrict__ incl, uint32_t *__restrict__ total,
                                                        unsigned long long *__restrict__ desc,
@@ -88,8 +89,8 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float2 *__re
       uint2 rect = make_uint2(0u, 0u);
       const float d = depths[i];
       if (!(d < MIN_DEPTH)) {
-        const float2 u = __ldg(us + i);
-        const int2 ar = areas[i];
+        const float2 u = ld_pair(us, i);  // us / areas: any contiguous [N,2] view (tile_io.cuh)
+        const int2 ar = ld_pair_rw(areas, i);
         const float xs = (float)ar.x, ys = (float)ar.y;
         const int x0 = min(gx, max(0, (int)__fdiv_rn(__fsub_rn(u.x, xs), 16.0f)));
         const int y0 = min(gy, max(0, (int)__fdiv_rn(__fsub_rn(u.y, ys), 16.0f)));
@@ -98,7 +99,7 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float2 *__re
         n = (uint32_t)(y1 - y0) * (uint32_t)(x1 - x0);
         if (n == 0) {  // kernel.cu:114-119: in-place cull
           depths[i] = BAD_MARKER;
-          areas[i] = make_int2(0, 0);
+          st_pair(areas, i, 0, 0);
         } else {
           rect = make_uint2((uint32_t)x0 | ((uint32_t)x1 << 16), (uint32_t)y0 | ((uint32_t)y1 << 16));
           dkmax = max(dkmax, __float2uint_rz(__fmul_rn(d, 1000.0f)));  // kernel.cu:73
@@ -506,14 +507,14 @@ __global__ void __launch_bounds__(256) k_ranges(const uint32_t *__restrict__ P_d
 // Gathers the four per-Gaussian attribute arrays (all L2 resident: 36 B/Gaussian) into the
 // 48-B records the rasterizers gather with cp.async (gsid == nullptr: one record per Gaussian).
 __global__ void __launch_bounds__(256) k_pack(int64_t P, const int32_t *__restrict__ gsid,
-                                              const float2 *__restrict__ us,
+                                              const float *__restrict__ us,
                                               const float *__restrict__ cinv2ds,
                                               const float *__restrict__ alphas,
                                               const float *__restrict__ colors, Rec *__restrict__ recs) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
   const int g = gsid != nullptr ? __ldg(gsid + p) : (int)p;  // nullptr: one record per Gaussian
-  const float2 u = __ldg(us + g);
+  const float2 u = ld_pair(us, g);
   recs[p] = build_record(u.x, u.y, __ldg(cinv2ds + 3 * (size_t)g), __ldg(cinv2ds + 3 * (size_t)g + 1),
                          __ldg(cinv2ds + 3 * (size_t)g + 2), __ldg(alphas + g), __ldg(colors + 3 * (size_t)g),
                          __ldg(colors + 3 * (size_t)g + 1), __ldg(colors + 3 * (size_t)g + 2), g);
@@ -543,7 +544,7 @@ int launch_bin(int H, int W, int N, const float *us, float *depths, int32_t *are
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   ProfScope ps(K_RECTS, st);
   k_rects_scan<<<(N + RS_SPAN - 1) / RS_SPAN, RS_CTA, 0, st>>>(
-      N, reinterpret_cast<const float2 *>(us), reinterpret_cast<int2 *>(areas), depths, gx, gy,
+      N, us, areas, depths, gx, gy,
       reinterpret_cast<uint2 *>(b + L.rects), reinterpret_cast<uint32_t *>(b + L.offsets), total,
       reinterpret_cast<unsigned long long *>(b + L.scan_desc), total + 3);
   GSB_CUDA_TRY(cudaGetLastError());
@@ -580,8 +581,7 @@ int launch_pack_only(int64_t P, const int32_t *gsid_per_patch, const float *us, 
                      const float *alphas, const float *colors, Rec *recs, cudaStream_t st) {
   if (P <= 0) return 0;
   ProfScope ps(K_PACK, st);
-  k_pack<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(P, gsid_per_patch, reinterpret_cast<const float2 *>(us),
-                                                      cinv2ds, alphas, colors, recs);
+  k_pack<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(P, gsid_per_patch, us, cinv2ds, alphas, colors, recs);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -19,6 +19,7 @@
 // within an ulp of the reference's.
 #include "common.cuh"
 #include "kernels.h"
+#include "tile_io.cuh"
 
 namespace gsb {
 
@@ -32,11 +33,11 @@ struct Slot3 {  // exclusive counts of survivors / clones / splits before this G
 };
 // gsmodel.py:219-234.  init != 0 is the first call after a density update: the norm of every
 // Gaussian is stored and the counter starts from the mask (:228-229).
-__global__ void k_density_accumulate(int64_t N, const float2 *__restrict__ dus, const uint8_t *__restrict__ mask,
+__global__ void k_density_accumulate(int64_t N, const float *__restrict__ dus, const uint8_t *__restrict__ mask,
                                      float *__restrict__ acc, int32_t *__restrict__ cnt, int init) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  const float2 d = dus[i];
+  const float2 d = ld_pair(dus, i);  // any contiguous [N,2] view (tile_io.cuh)
   const float g = sqrtf(d.x * d.x + d.y * d.y);
   const bool m = mask[i] != 0;
   if (init) {
@@ -543,8 +544,7 @@ int launch_density_accumulate(int64_t N, const float *dloss_dus, const uint8_t *
                               int32_t *cunt, int init, cudaStream_t st) {
   if (N == 0) return 0;
   ProfScope ps(K_DENSITY_ACC, st);
-  k_density_accumulate<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(N, reinterpret_cast<const float2 *>(dloss_dus),
-                                                                     mask, grad_accum, cunt, init);
+  k_density_accumulate<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(N, dloss_dus, mask, grad_accum, cunt, init);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

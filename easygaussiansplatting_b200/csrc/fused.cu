@@ -71,10 +71,10 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
   if (valid) {
     pg::forward_one<K3>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
     const long long i = base + tid;
-    *reinterpret_cast<float2 *>(us + 2 * i) = make_float2(u[0], u[1]);
+    st_pair(us, i, u[0], u[1]);
     cinv2ds[3 * i] = conic[0]; cinv2ds[3 * i + 1] = conic[1]; cinv2ds[3 * i + 2] = conic[2];
     colors[3 * i] = col[0]; colors[3 * i + 1] = col[1]; colors[3 * i + 2] = col[2];
-    *reinterpret_cast<int2 *>(areas + 2 * i) = make_int2(area[0], area[1]);
+    st_pair(areas, i, area[0], area[1]);
     depths[i] = depth;
     // the rasterizers' per-Gaussian record, straight from registers (saves the k_pack pass)
     if (recs != nullptr)
@@ -127,12 +127,12 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
       gci[0] = -0.5f * m[2]; gci[1] = -m[3]; gci[2] = -0.5f * m[4];
       gcol[0] = m[6]; gcol[1] = m[7]; gcol[2] = m[8];
       galpha = m[5];
-      *reinterpret_cast<float2 *>(mi.dus_out + 2 * i) = make_float2(gu[0], gu[1]);
+      st_pair(mi.dus_out, i, gu[0], gu[1]);
       if (mi.dalphas_out != nullptr) mi.dalphas_out[i] = galpha;
     }
   } else if (valid) {
     const long long i = base + tid;
-    const float2 g2 = __ldg(reinterpret_cast<const float2 *>(g_us) + i);
+    const float2 g2 = ld_pair(g_us, i);
     gu[0] = g2.x; gu[1] = g2.y;
     gci[0] = __ldg(g_cinv2ds + 3 * i); gci[1] = __ldg(g_cinv2ds + 3 * i + 1); gci[2] = __ldg(g_cinv2ds + 3 * i + 2);
     gcol[0] = __ldg(g_colors + 3 * i); gcol[1] = __ldg(g_colors + 3 * i + 1); gcol[2] = __ldg(g_colors + 3 * i + 2);

@@ -138,7 +138,7 @@ __device__ __forceinline__ BwdEval bwd_eval(const float4 &q0, const float4 &q1, 
 }  // namespace
 
 __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
-    int W, int H, int gx, int T, const int2 *__restrict__ ranges, const Rec *__restrict__ recs,
+    int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ dloss_dgammas, float *__restrict__ moments, int *__restrict__ work) {
   __shared__ __align__(16) unsigned char s_ring[4][BWD_RING * BWD_CHUNK_BYTES];  // gathered records, per warp
@@ -179,7 +179,7 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
       const int code = ent & 7;
       tile = ent >> 3;
       whole_tile = code == 4;  // <= 32 patches: all four blocks from one gather
-      range = __ldg(ranges + tile);
+      range = ld_pair(ranges, tile);  // the caller's patch_range_per_tile: any alignment
       len = range.y - range.x;
       if (len <= 0) continue;
       blk = whole_tile ? 0 : code;
@@ -394,7 +394,7 @@ int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *
     const long long want = (long long)sms * DRAW_BWD_MINBLOCKS;
     const int grid = (int)(T < want ? T : want);
     ProfScope ps(K_DRAW_BWD, st);
-    k_draw_bwd<<<grid, 128, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, contrib,
+    k_draw_bwd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib,
                                      final_tau, dloss_dgammas, moments, work);
     GSB_CUDA_TRY(cudaGetLastError());
   }

@@ -13,6 +13,7 @@
 // Replaces reference kernel.cu:152-271 (draw).
 #include "common.cuh"
 #include "kernels.h"
+#include "tile_io.cuh"
 
 namespace gsb {
 
@@ -46,7 +47,7 @@ __device__ __forceinline__ float2 fwd_alpha(const float4 &q0, const float4 &q1, 
 // zeros itself with 16-byte stores -- one warp per empty tile -- so the sparse corner of BASELINE config 4
 // (50k Gaussians at 4K: 32 400 tiles, most of them empty) costs one streaming pass over the
 // frame instead of one queue item per 8x8 block.
-__global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, const int2 *__restrict__ ranges,
+__global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, const int32_t *__restrict__ ranges,
                                                    float *__restrict__ image, int32_t *__restrict__ contrib,
                                                    float *__restrict__ final_tau, int *__restrict__ work) {
   __shared__ unsigned s_empty[8];  // per warp: which of its 32 tiles have no patches
@@ -54,7 +55,7 @@ __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, 
   const int tile = blockIdx.x * 256 + threadIdx.x;  // phase 1: one thread per tile
   int len = 0;
   if (tile < T) {
-    const int2 r = __ldg(ranges + tile);
+    const int2 r = ld_pair(ranges, tile);  // splatB takes the ranges from its caller: any alignment
     len = r.y - r.x;
   }
   const bool has = len > 0;
@@ -117,7 +118,7 @@ int launch_tile_list(int H, int W, const int32_t *ranges, float *image, int32_t 
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   const int T = gx * gy;
   GSB_CUDA_TRY(cudaMemsetAsync(work, 0, 2 * sizeof(int), st));
-  k_tile_list<<<(T + 255) / 256, 256, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), image, contrib,
+  k_tile_list<<<(T + 255) / 256, 256, 0, st>>>(W, H, gx, T, ranges, image, contrib,
                                            final_tau, work);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
@@ -285,6 +286,8 @@ int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int3
   if (gx <= 0 || gy <= 0) return 0;
   const int T = gx * gy;
   if (work == nullptr) return set_arg_error("draw: work area missing");
+  // (k_draw reads `ranges` as int2: the splat entry points only accept an 8-byte aligned
+  // patch_range_per_tile, which the binning just wrote)
   // work list (and the zeros of the empty tiles) first; it also clears the item counter
   int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, work, st);
   if (rc) return rc;

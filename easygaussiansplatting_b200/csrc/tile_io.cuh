@@ -18,6 +18,41 @@ __device__ __forceinline__ bool aligned16(const void *p) {
   return (reinterpret_cast<uintptr_t>(p) & 15u) == 0;
 }
 
+__device__ __forceinline__ bool aligned8(const void *p) {
+  return (reinterpret_cast<uintptr_t>(p) & 7u) == 0;
+}
+
+// Row i of a caller's [N,2] array: one 8-byte access when the array is 8-byte aligned, two
+// scalar ones otherwise (a contiguous view at an odd float offset, e.g. a slice of a flat
+// buffer).  The test is on the base pointer, so the branch is uniform over a launch.
+__device__ __forceinline__ float2 ld_pair(const float *__restrict__ p, long long i) {
+  if (aligned8(p)) return __ldg(reinterpret_cast<const float2 *>(p) + i);
+  return make_float2(__ldg(p + 2 * i), __ldg(p + 2 * i + 1));
+}
+__device__ __forceinline__ int2 ld_pair(const int32_t *__restrict__ p, long long i) {
+  if (aligned8(p)) return __ldg(reinterpret_cast<const int2 *>(p) + i);
+  return make_int2(__ldg(p + 2 * i), __ldg(p + 2 * i + 1));
+}
+// (plain loads: for arrays a kernel also writes)
+__device__ __forceinline__ int2 ld_pair_rw(const int32_t *p, long long i) {
+  if (aligned8(p)) return reinterpret_cast<const int2 *>(p)[i];
+  return make_int2(p[2 * i], p[2 * i + 1]);
+}
+__device__ __forceinline__ void st_pair(float *p, long long i, float x, float y) {
+  if (aligned8(p)) {
+    reinterpret_cast<float2 *>(p)[i] = make_float2(x, y);
+  } else {
+    p[2 * i] = x; p[2 * i + 1] = y;
+  }
+}
+__device__ __forceinline__ void st_pair(int32_t *p, long long i, int x, int y) {
+  if (aligned8(p)) {
+    reinterpret_cast<int2 *>(p)[i] = make_int2(x, y);
+  } else {
+    p[2 * i] = x; p[2 * i + 1] = y;
+  }
+}
+
 // global [rows, K] (contiguous) -> smem tile
 template <int K>
 __device__ __forceinline__ void tile_fetch(const float *__restrict__ g, long long base_row,

@@ -471,6 +471,13 @@ def sh_grad_expand(pws, twcs, dloss_dcolors, sh_dim3, out=None):
         raise ValueError("sh_grad_expand: need twcs[V,3], dloss_dcolors[V,N,3], sh_dim3 in {1,4,9,16}")
     if out is None:
         out = torch.empty((N, 3 * k), dtype=torch.float32, device=pws.device)
+    else:  # the kernel writes N * 3k floats through out's data pointer
+        if not isinstance(out, torch.Tensor) or out.dtype != torch.float32:
+            raise TypeError("out must be a float32 torch.Tensor")
+        if out.device != pws.device:
+            raise ValueError("out must be on the device of pws")
+        if tuple(out.shape) != (N, 3 * k) or not out.is_contiguous():
+            raise ValueError("out must be a contiguous (%d, %d) tensor, got shape %s" % (N, 3 * k, tuple(out.shape)))
     lib = _L()
     with torch.cuda.device(pws.device):
         _lib.check(lib.gsb_sh_grad_expand(N, k, V, _ptr(pws), _ptr(twcs), _ptr(g), _ptr(out), _stream()), lib)

@@ -23,6 +23,12 @@
  *     kernel.cu:140-143; both are handled here).
  *   - "culled" Gaussians (depths[i] < 0.2) get all-zero outputs, exactly what the
  *     reference's zero-filled tensors hold for them.
+ *   - any float32 / int32 array may start at any 4-byte boundary (e.g. a slice of one flat
+ *     buffer at an odd offset): row-wise vector loads and stores are only used when the base
+ *     pointer is aligned for them.  The exceptions are buffers the caller allocates for the
+ *     call: packed_records must be 16-byte aligned, and so must gsb_splat_render's /
+ *     gsb_splat_forward's image, contrib and final_tau; their patch_range_per_tile must be
+ *     8-byte aligned.  A misaligned one is an argument error.
  */
 #ifndef GSPLAT_B200_H_
 #define GSPLAT_B200_H_

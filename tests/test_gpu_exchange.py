@@ -114,3 +114,63 @@ def test_exchange_argument_errors():
     assert rc != 0 and b"null region" in lib.gsb_last_error()
     rc = lib.gsb_grad_reduce_broadcast(1000, 16, 2, 0, regs, 0, None)
     assert rc != 0
+
+
+@pytest.mark.parametrize("world,N,k3", [(2, 3001, 1), (4, 3001, 9), (2, 20001, 9), (4, 20001, 1)])
+def test_exchange_with_moment_rows_equals_rank_ordered_sum(world, N, k3):
+    """push(moments=..., cinv2ds=...) -- the k_preprocess_bwd<K3, PUSH, MOM> kernel training runs
+    across GPUs -- against the rank-ordered sum of each rank's local preprocessB(moments=...), at
+    odd N (ragged last tile, padding rows in the slots); this rank's dL/du comes back unsummed."""
+    from easygaussiansplatting_b200 import ops
+    from easygaussiansplatting_b200.gsfunction import Camera
+    from easygaussiansplatting_b200.parallel import GradExchange
+    from easygaussiansplatting_b200.scene import ring_camera, synthetic_scene
+    W, H = 320, 200
+    sc = synthetic_scene(N, W, H, sh_dim=3 * k3, seed=world + 10)
+    pws, rots, scales, shs = t(sc["pws"]), t(sc["rots"] * 1.3), t(sc["scales"]), t(sc["shs"])
+    regions = [GradExchange.alloc_region(GradExchange.region_bytes(N, k3, world))[0] for _ in range(world)]
+    exs = [GradExchange(N, k3, world, r, regions, DEV, own_region=regions[r]) for r in range(world)]
+    streams = [torch.cuda.Stream() for _ in range(world)]
+    names = ("dpws", "dshs", "dscales", "drots", "dus", "dalphas")
+    try:
+        for step in range(3):
+            g = torch.Generator(device=DEV).manual_seed(1000 * world + step)
+            cams, ins, local = [], [], []
+            for r in range(world):
+                Rcw, tcw, twc = ring_camera(r + step, world + 2)
+                cams.append(Camera(W, H, sc["fx"], sc["fy"], sc["cx"], sc["cy"], t(Rcw), t(tcw), t(twc)))
+                cinv2ds = ops.preprocess(pws, rots, scales, shs, cams[r].Rcw, cams[r].tcw, cams[r].twc, sc["fx"],
+                                         sc["fy"], sc["cx"], sc["cy"], W, H)[1]
+                moments = torch.randn((N, 9), device=DEV, generator=g)
+                moments[torch.rand(N, device=DEV, generator=g) < 0.05, 0:2] = 0   # untouched rows
+                ins.append((moments, cinv2ds))
+                out = ops.preprocessB(pws, rots, scales, shs, cams[r].Rcw, cams[r].tcw, cams[r].twc, sc["fx"],
+                                      sc["fy"], sc["cx"], sc["cy"], W, H, None, None, None, moments=moments,
+                                      cinv2ds=cinv2ds)
+                local.append(dict(zip(names, out)))
+                local[-1]["dalphas"] = local[-1]["dalphas"].reshape(N, 1)
+            want = {k: local[0][k].clone() for k in names if k != "dus"}
+            for r in range(1, world):
+                for k in want:
+                    want[k] += local[r][k]
+            torch.cuda.synchronize()
+            dus = []
+            for r in range(world):
+                with torch.cuda.stream(streams[r]):
+                    dus.append(exs[r].push(pws, rots, scales, shs, cams[r], moments=ins[r][0], cinv2ds=ins[r][1]))
+            outs = []
+            for r in range(world):
+                with torch.cuda.stream(streams[r]):
+                    outs.append(exs[r].reduce())
+            torch.cuda.synchronize()
+            for r in range(world):
+                assert exs[r].status() == 0, "rank %d: a flag wait timed out" % r
+                assert torch.equal(dus[r], local[r]["dus"]), (step, r)
+                for k in want:
+                    assert outs[r][k].shape == want[k].shape
+                    err = float((outs[r][k] - want[k]).abs().max() / want[k].abs().max().clamp_min(1e-30))
+                    assert err <= 5e-6, (step, r, k, err)
+                assert torch.equal(outs[r]["dalphas"], want["dalphas"]), (step, r)
+    finally:
+        for ex in exs:
+            ex.close()
