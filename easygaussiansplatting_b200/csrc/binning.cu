@@ -1,7 +1,7 @@
 // Tile binning: per-Gaussian tile rectangles + exclusive offsets (one fused kernel with a
-// decoupled look-back scan), (tile | depth-mm) keys, a hand-written LSD radix sort (per pass: a
-// column scan of the per-tile digit counts + one rank-and-scatter kernel that also counts the
-// next pass's digits), per-tile ranges and the packed per-Gaussian record stream.
+// decoupled look-back scan), (tile | depth-mm) keys emitted warp-cooperatively, a hand-written
+// LSD radix sort (per pass: per-tile digit counts, one look-back scan of them, one
+// rank-and-scatter kernel), per-tile ranges and the packed per-Gaussian record stream.
 //
 // Replaces getRects / thrust::inclusive_scan / createKeys / thrust::sort_by_key / getRanges
 // (reference kernel.cu:46-150, gausplat.cu:50-91).  No library kernels: round 1 used CUB's
@@ -55,15 +55,44 @@ __device__ __forceinline__ unsigned long long ld_relaxed_u64(const unsigned long
   return v;
 }
 
+// Single-pass decoupled look-back of Merrill & Garland, shared by the two scans of this file
+// (k_rects_scan, k_colscan): a CTA publishes its aggregate, then its inclusive prefix, in one
+// 64-bit word (2 flag bits | value), and a warp walks back over its predecessors 32 at a time.
+// CTAs take their index `blk` from an atomic claim counter, so every predecessor is already
+// running: the walk cannot deadlock.  Called by one whole warp; returns the exclusive prefix.
+constexpr unsigned long long DESC_AGG = 1ull << 62, DESC_INC = 2ull << 62, DESC_VAL = (1ull << 62) - 1;
+__device__ unsigned long long scan_lookback(unsigned long long *desc, int blk, unsigned long long run) {
+  const int lane = threadIdx.x & 31;
+  unsigned long long excl = 0;
+  if (blk > 0) {
+    if (lane == 0) st_relaxed_u64(desc + blk, DESC_AGG | run);
+    int p = blk - 1;  // lane l inspects predecessor p - l
+    for (;;) {
+      const int q = p - lane;
+      unsigned long long v = DESC_INC;  // virtual predecessor before block 0: inclusive 0
+      if (q >= 0) {
+        do { v = ld_relaxed_u64(desc + q); } while ((v >> 62) == 0);
+      }
+      const unsigned inc_mask = __ballot_sync(0xffffffffu, (v >> 62) == 2);
+      const int first_inc = inc_mask ? __ffs(inc_mask) - 1 : 32;  // nearest predecessor with an inclusive value
+      unsigned long long part = (lane <= first_inc) ? (v & DESC_VAL) : 0ull;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+      excl += part;
+      if (inc_mask) break;
+      p -= 32;
+    }
+  }
+  if (lane == 0) st_relaxed_u64(desc + blk, DESC_INC | (excl + run));
+  return excl;
+}
+
 // =================================================================== phase 1: rects + scan
 // One CTA = 1024 consecutive Gaussians (4 per thread, strided so every access is coalesced).
 // Rectangle arithmetic: kernel.cu:105-110; DIV_ROUND_UP(X,16) on floats is ((X) + 16 - 1) / 16
 // (common.cuh:15).  Explicit _rn intrinsics: these decide the patch list, no contraction.
-// The inclusive prefix sum of the patch counts uses the single-pass decoupled look-back of
-// Merrill & Garland: a CTA publishes its aggregate, then its inclusive prefix, in one 64-bit
-// word (2 flag bits | value), and a warp walks back over its predecessors 32 at a time.
+// The inclusive prefix sum of the patch counts uses the decoupled look-back above.
 constexpr int RS_CTA = 256, RS_ITEMS = 4, RS_SPAN = RS_CTA * RS_ITEMS;
-constexpr unsigned long long DESC_AGG = 1ull << 62, DESC_INC = 2ull << 62, DESC_VAL = (1ull << 62) - 1;
 
 __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__restrict__ us,
                                                        int32_t *__restrict__ areas, float *__restrict__ depths,
@@ -134,28 +163,8 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__res
   }
   // look-back (warp 0): exclusive prefix of this CTA over all earlier CTAs
   if (warp == 0) {
-    unsigned long long excl = 0;
-    if (blk > 0) {
-      if (lane == 0) st_relaxed_u64(desc + blk, DESC_AGG | run);
-      int p = blk - 1;  // lane l inspects predecessor p - l
-      for (;;) {
-        const int q = p - lane;
-        unsigned long long v = DESC_INC;  // virtual predecessor before block 0: inclusive 0
-        if (q >= 0) {
-          do { v = ld_relaxed_u64(desc + q); } while ((v >> 62) == 0);
-        }
-        const unsigned inc_mask = __ballot_sync(0xffffffffu, (v >> 62) == 2);
-        const int first_inc = inc_mask ? __ffs(inc_mask) - 1 : 32;  // nearest predecessor with an inclusive value
-        unsigned long long part = (lane <= first_inc) ? (v & DESC_VAL) : 0ull;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        excl += part;
-        if (inc_mask) break;
-        p -= 32;
-      }
-    }
+    const unsigned long long excl = scan_lookback(desc, blk, run);
     if (lane == 0) {
-      st_relaxed_u64(desc + blk, DESC_INC | (excl + run));
       s_prefix = excl;
       if (blk == nblk - 1) total[0] = (uint32_t)min(excl + run, 0xffffffffull);  // P (saturating)
     }
@@ -210,152 +219,184 @@ static KeyPlan key_plan(int H, int W, uint32_t depth_key_max) {
   return p;
 }
 
-// One thread per Gaussian (grid-stride), serial over its rectangle (2.5 patches/Gaussian on the
-// benchmark scenes); rectangles of more than 32 tiles are emitted by the whole warp.  64-bit:
-// tile << 32 | dk (kernel.cu:71-74); 32-bit: tile << dbits | dk.  Also counts, for every sort
-// pass, the digit histogram of all keys (shared-memory counters, flushed once per CTA).
-// *status |= 2 when a Gaussian's patches do not fit the capacity, |= 4 when a depth key needs more
-// bits than the plan has (both only possible on the capacity-based path, gsb_splat_forward).
-constexpr int RX_THREADS = 256, RX_WARPS = RX_THREADS / 32, RX_IPT = 16, RX_TILE = RX_THREADS * RX_IPT;
+// Warp-cooperative: the patches of a warp's 32 consecutive Gaussians are one contiguous range
+// of the key array (exclusive offsets from the scan), and the lanes walk that range 32 keys at a
+// time.  Each lane finds the Gaussian that owns its position by a binary search over the warp's
+// 32 offsets (shuffles) and builds the key row-major inside that Gaussian's rectangle
+// (== reference order), so every store is coalesced and no lane waits for a large rectangle.
+// 64-bit: tile << 32 | dk (kernel.cu:71-74); 32-bit: tile << dbits | dk.
+// *status |= 2 when a Gaussian's patches do not fit the capacity (it is dropped whole and
+// nothing is written at or past `capacity`), |= 4 when a depth key needs more bits than the plan
+// has (both only possible on the capacity-based path, gsb_splat_forward).
 template <typename KeyT>
 __global__ void __launch_bounds__(256) k_keys(int N, const float *__restrict__ depths,
                                               const uint32_t *__restrict__ incl, const uint2 *__restrict__ rects,
-                                              int gx, int shift, const __grid_constant__ PassPlan pp,
-                                              uint32_t capacity,
+                                              int gx, int shift, uint32_t capacity,
                                               KeyT *__restrict__ keys, int32_t *__restrict__ vals,
-                                              uint32_t *__restrict__ hist, uint32_t *__restrict__ tile_hist,
                                               uint32_t *__restrict__ status) {
-  extern __shared__ uint32_t s_hist[];  // [pp.n][1 << pp.bits]
-  const int bins = 1 << pp.bits;
-  for (int i = threadIdx.x; i < pp.n * bins; i += blockDim.x) s_hist[i] = 0;
-  __syncthreads();
   const int lane = threadIdx.x & 31;
-  const uint32_t dmask = (uint32_t)bins - 1u;
-  auto emit = [&](uint32_t pos, KeyT key, int id) {
-    keys[pos] = key;
-    vals[pos] = id;
-    for (int p = 0; p < pp.n; p++) atomicAdd(&s_hist[p * bins + ((uint32_t)(key >> pp.shift[p]) & dmask)], 1u);
-    // digit counts of the first pass per sort tile (the passes count those of their successor)
-    if (pp.n > 0) atomicAdd(tile_hist + (size_t)(pos / RX_TILE) * bins + ((uint32_t)(key >> pp.shift[0]) & dmask), 1u);
-  };
-  const int stride = gridDim.x * blockDim.x;
-  for (int base = blockIdx.x * blockDim.x; base < N; base += stride) {  // (warp-uniform trip count)
-    const int i = base + threadIdx.x;
-    uint32_t off = 0, x0 = 0, x1 = 0, y0 = 0, y1 = 0;
-    KeyT dk = 0;
-    if (i < N) {
-      const float d = __ldg(depths + i);
-      if (!(d < MIN_DEPTH)) {
-        off = (i == 0) ? 0u : __ldg(incl + i - 1);
-        const uint2 r = __ldg(rects + i);
-        x0 = r.x & 0xffffu; x1 = r.x >> 16; y0 = r.y & 0xffffu; y1 = r.y >> 16;
-        dk = (KeyT)__float2uint_rz(__fmul_rn(d, 1000.0f));
-        if (sizeof(KeyT) == 4 && (dk >> shift) != 0) {  // deeper than the planned key width (capacity path)
-          atomicOr(status, 4u);
-          dk &= ((KeyT)1 << shift) - 1;
-        }
-      }
-    }
-    uint32_t w = x1 - x0, n = w * (y1 - y0);
-    if (n > 0 && (off > capacity || n > capacity - off)) {  // does not fit: drop, flag
-      atomicOr(status, 2u);
-      n = 0; w = 0; y1 = y0;
-    }
-    if (n <= 32) {
-      for (uint32_t y = y0; y < y1; y++)
-        for (uint32_t x = x0; x < x0 + w; x++) emit(off++, ((KeyT)(y * (uint32_t)gx + x) << shift) | dk, i);
-    }
-    unsigned big = __ballot_sync(0xffffffffu, n > 32);
-    while (big) {
-      const int src = __ffs(big) - 1;
-      big &= big - 1;
-      const uint32_t bn = __shfl_sync(0xffffffffu, n, src), bw = __shfl_sync(0xffffffffu, w, src);
-      const uint32_t bx0 = __shfl_sync(0xffffffffu, x0, src), by0 = __shfl_sync(0xffffffffu, y0, src);
-      const uint32_t boff = __shfl_sync(0xffffffffu, off, src);
-      const KeyT bdk = (KeyT)__shfl_sync(0xffffffffu, (unsigned long long)dk, src);
-      const int bi = __shfl_sync(0xffffffffu, i, src);
-      for (uint32_t t = lane; t < bn; t += 32) {  // row-major inside the rectangle == reference order
-        const uint32_t y = by0 + t / bw, x = bx0 + t % bw;
-        emit(boff + t, ((KeyT)(y * (uint32_t)gx + x) << shift) | bdk, bi);
+  const int first = (blockIdx.x * blockDim.x + threadIdx.x) & ~31;  // the warp's first Gaussian
+  if (first >= N) return;
+  const int i = first + lane;
+  const uint32_t inc = __ldg(incl + min(i, N - 1));  // lanes past N: no patches
+  uint32_t off = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) off = first == 0 ? 0u : __ldg(incl + first - 1);
+  uint32_t n = inc - off, rx = 0, ry = 0;
+  KeyT dk = 0;
+  if (i < N) {
+    const float d = __ldg(depths + i);
+    if (!(d < MIN_DEPTH)) {
+      const uint2 r = __ldg(rects + i);
+      rx = r.x; ry = r.y;  // (x0 | x1 << 16, y0 | y1 << 16)
+      dk = (KeyT)__float2uint_rz(__fmul_rn(d, 1000.0f));
+      if (sizeof(KeyT) == 4 && (dk >> shift) != 0) {  // deeper than the planned key width (capacity path)
+        atomicOr(status, 4u);
+        dk &= ((KeyT)1 << shift) - 1;
       }
     }
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < pp.n * bins; i += blockDim.x)
-    if (s_hist[i]) atomicAdd(hist + i, s_hist[i]);
+  if (n > 0 && (off > capacity || n > capacity - off)) {  // does not fit: drop, flag
+    atomicOr(status, 2u);
+    n = 0;
+  }
+  const uint32_t start = __shfl_sync(0xffffffffu, off, 0);
+  const uint32_t span = __shfl_sync(0xffffffffu, inc, 31) - start;
+  const uint32_t rel = off - start;  // non-decreasing over the lanes
+  // positions at or past the capacity belong to dropped Gaussians only
+  const uint32_t todo = start < capacity ? min(span, capacity - start) : 0u;
+  for (uint32_t t0 = 0; t0 < todo; t0 += 32) {
+    const uint32_t t = t0 + lane;
+    int o = 0;  // owner: the last lane whose range starts at or before t
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1)
+      if (__shfl_sync(0xffffffffu, rel, o + s) <= t) o += s;
+    const uint32_t on = __shfl_sync(0xffffffffu, n, o), orel = __shfl_sync(0xffffffffu, rel, o);
+    const uint32_t ox = __shfl_sync(0xffffffffu, rx, o), oy = __shfl_sync(0xffffffffu, ry, o);
+    const KeyT odk = __shfl_sync(0xffffffffu, dk, o);
+    const uint32_t local = t - orel;
+    if (t < todo && local < on) {
+      const uint32_t x0 = ox & 0xffffu, w = (ox >> 16) - x0;
+      const uint32_t y = (oy & 0xffffu) + local / w, x = x0 + local % w;
+      keys[start + t] = ((KeyT)(y * (uint32_t)gx + x) << shift) | odk;
+      vals[start + t] = first + o;
+    }
+  }
 }
 
 // =================================================================== phase 2: radix sort
-// LSD radix sort, one pass = two kernels, no inter-CTA waiting:
-//   k_colscan   turns the per-tile digit counts C[tile][digit] of the pass into scatter bases
-//               B[tile][digit] = (keys with a smaller digit) + (keys with this digit in earlier tiles);
-//   k_radix_pass  a CTA takes a tile of 4096 pairs, ranks its keys (stable: warps own contiguous
-//               512-element spans, the lanes of a round are ordered by ballots over the digit
-//               bits), scatters them to B + rank, and counts the NEXT pass's digit of every key
-//               into that pass's C at the key's new tile (one RED per key).
-// The first pass's C comes from k_keys.  (A single-kernel pass with decoupled look-back per digit
-// was tried first: with every CTA of a 2.5 M-pair pass starting in lockstep the look-back walked
-// ~40 tiles back on average -- 50 us per pass, slower than the library it replaced.)
-template <int BITS>
-__global__ void __launch_bounds__(1024) k_colscan(const uint32_t *__restrict__ P_dev, uint32_t capacity,
-                                                  const uint32_t *__restrict__ hist, uint32_t *__restrict__ C) {
-  constexpr int BINS = 1 << BITS, WARPS = 32;
-  __shared__ uint32_t s_g[BINS];
-  __shared__ uint32_t s_part[WARPS][32];
-  __shared__ uint32_t s_scan[WARPS];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (P_dev[2] != 0) return;  // [P, max key, flags]: capacity overflow, the frame is abandoned (see k_ranges)
-  const uint32_t P = min(*P_dev, capacity);
-  const int T = (int)((P + RX_TILE - 1) / RX_TILE);
-  {  // exclusive scan of the global digit histogram (BINS <= 1024 = one value per thread)
-    const uint32_t v = tid < BINS ? hist[tid] : 0u;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_scan[warp] = inc;
-    __syncthreads();
-    uint32_t run = inc - v;
-    for (int w = 0; w < warp; w++) run += s_scan[w];
-    if (tid < BINS) s_g[tid] = run;
-  }
-  // this CTA: digits [32 blockIdx.x, +32); warp w: tiles [w R, (w + 1) R); lane = digit
-  const int d = blockIdx.x * 32 + lane;
-  const int R = (T + WARPS - 1) / WARPS;
-  const int t0 = min(T, warp * R), t1 = min(T, t0 + R);
-  uint32_t *col = C + d;
-  uint32_t sum = 0;
-#pragma unroll 8
-  for (int t = t0; t < t1; t++) sum += col[(size_t)t * BINS];
-  s_part[warp][lane] = sum;
-  __syncthreads();
-  uint32_t run = s_g[d];
-  for (int w = 0; w < warp; w++) run += s_part[w][lane];
-#pragma unroll 8
-  for (int t = t0; t < t1; t++) {
-    const uint32_t c = col[(size_t)t * BINS];
-    col[(size_t)t * BINS] = run;
-    run += c;
-  }
-}
-
-#ifndef RX_UNROLL_OUT
-#define RX_UNROLL_OUT 0
-#endif
+// LSD radix sort over sort tiles of RX_TILE consecutive pairs; one pass = three kernels, no
+// global atomics and no inter-CTA waiting except the look-back of the scan:
+//   k_digit_counts  one CTA per sort tile counts the pass's digit of its keys in shared memory and
+//               writes the counts digit-major: C[digit][tile];
+//   k_colscan   one exclusive scan over all of C in that order turns it into the scatter bases
+//               B[digit][tile] = (keys with a smaller digit) + (keys with this digit in earlier
+//               tiles), spread over enough CTAs to use the whole GPU (decoupled look-back);
+//   k_radix_pass  one CTA per sort tile ranks its keys (stable: warps own contiguous 32 RX_IPT-
+//               element spans, the lanes of a round are ordered by ballots over the digit bits)
+//               and scatters them to B + rank.
+// k_digit_counts re-reads the keys the previous kernel has just written (L2 resident).  It
+// replaces one global RED per key and pass into the next pass's counts, which capped the
+// scatter kernel.  (A single-kernel pass with decoupled look-back per digit was tried before:
+// with every CTA of a 2.5 M-pair pass starting in lockstep the look-back walked ~40 tiles back
+// on average -- 50 us per pass, slower than the library it replaced.)
 #ifndef RX_MINBLOCKS
 #define RX_MINBLOCKS 3
 #endif
+// 4096-pair sort tiles: 614 tiles at config 2 (P = 2.51M).  Measured on an H100 80GB HBM3 (700 W
+// limit) against 2048-, 3072-, 5120- and 6144-pair tiles: 2048 and 3072 (at 4 or 6 CTAs per SM)
+// were slower; 5120 and 6144 sorted config 2 a few us per pass faster, but made the whole step
+// no faster and the 50k-Gaussian 4K frame slower.
+constexpr int RX_THREADS = 256, RX_WARPS = RX_THREADS / 32, RX_IPT = 16, RX_TILE = RX_THREADS * RX_IPT;
+constexpr int CS_CTA = 256, CS_ITEMS = 8, CS_SPAN = CS_CTA * CS_ITEMS;  // k_colscan: values per CTA
+
+template <typename KeyT, int BITS>
+__global__ void __launch_bounds__(RX_THREADS) k_digit_counts(const KeyT *__restrict__ keys,
+                                                             const uint32_t *__restrict__ P_dev, uint32_t capacity,
+                                                             int shift, uint32_t tiles, uint32_t *__restrict__ C,
+                                                             unsigned long long *__restrict__ desc, uint32_t ndesc,
+                                                             uint32_t *__restrict__ claim) {
+  constexpr int BINS = 1 << BITS;
+  __shared__ uint32_t s_cnt[BINS];
+  // reset the look-back state of the k_colscan that follows (ndesc <= tiles descriptors)
+  if (threadIdx.x == 0) {
+    if (blockIdx.x < ndesc) desc[blockIdx.x] = 0;
+    if (blockIdx.x == 0) *claim = 0;
+  }
+  if (P_dev[2] != 0) return;  // [P, max key, flags]: capacity overflow, the frame is abandoned (see k_ranges)
+  const uint32_t P = min(*P_dev, capacity);
+  const uint32_t tile = blockIdx.x;  // tiles past P (capacity path) write zero counts
+  for (int d = threadIdx.x; d < BINS; d += RX_THREADS) s_cnt[d] = 0;
+  KeyT key[RX_IPT];  // all loads in flight before the first count
+#pragma unroll
+  for (int r = 0; r < RX_IPT; r++) {
+    const uint32_t idx = tile * RX_TILE + r * RX_THREADS + threadIdx.x;
+    key[r] = idx < P ? keys[idx] : (KeyT)0;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < RX_IPT; r++)
+    if (tile * RX_TILE + r * RX_THREADS + threadIdx.x < P) atomicAdd(&s_cnt[(uint32_t)(key[r] >> shift) & (BINS - 1)], 1u);
+  __syncthreads();
+  for (int d = threadIdx.x; d < BINS; d += RX_THREADS) C[(size_t)d * tiles + tile] = s_cnt[d];
+}
+
+// In-place exclusive scan of n values (n a multiple of CS_ITEMS); claim / desc reset by k_digit_counts
+__global__ void __launch_bounds__(CS_CTA) k_colscan(const uint32_t *__restrict__ flags, uint32_t n,
+                                                    uint32_t *__restrict__ C, unsigned long long *__restrict__ desc,
+                                                    uint32_t *__restrict__ claim) {
+  __shared__ uint32_t s_warp[CS_CTA / 32];
+  __shared__ uint32_t s_prefix;
+  __shared__ int s_blk;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (*flags != 0) return;
+  if (tid == 0) s_blk = (int)atomicAdd(claim, 1u);
+  __syncthreads();
+  const int blk = s_blk;
+  const uint32_t i0 = (uint32_t)blk * CS_SPAN + tid * CS_ITEMS;  // this thread's CS_ITEMS consecutive values
+  uint4 v[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
+  if (i0 < n) {
+    v[0] = *reinterpret_cast<const uint4 *>(C + i0);
+    v[1] = *reinterpret_cast<const uint4 *>(C + i0 + 4);
+  }
+  const uint32_t sum = v[0].x + v[0].y + v[0].z + v[0].w + v[1].x + v[1].y + v[1].z + v[1].w;
+  uint32_t inc = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  uint32_t wbase = 0, run = 0;
+#pragma unroll
+  for (int w = 0; w < CS_CTA / 32; w++) {
+    const uint32_t t = s_warp[w];
+    if (w < warp) wbase += t;
+    run += t;
+  }
+  if (warp == 0) {
+    const unsigned long long excl = scan_lookback(desc, blk, run);
+    if (lane == 0) s_prefix = (uint32_t)excl;
+  }
+  __syncthreads();
+  if (i0 < n) {
+    uint32_t e = s_prefix + wbase + inc - sum;
+    uint4 o[2];
+    o[0].x = e; e += v[0].x; o[0].y = e; e += v[0].y; o[0].z = e; e += v[0].z; o[0].w = e; e += v[0].w;
+    o[1].x = e; e += v[1].x; o[1].y = e; e += v[1].y; o[1].z = e; e += v[1].z; o[1].w = e;
+    *reinterpret_cast<uint4 *>(C + i0) = o[0];
+    *reinterpret_cast<uint4 *>(C + i0 + 4) = o[1];
+  }
+}
+
 template <typename KeyT, int BITS>
 __global__ void __launch_bounds__(RX_THREADS, sizeof(KeyT) == 8 ? 2 : RX_MINBLOCKS) k_radix_pass(const KeyT *__restrict__ keys_in,
                                                               const int32_t *__restrict__ vals_in,
                                                               KeyT *__restrict__ keys_out,
                                                               int32_t *__restrict__ vals_out,
                                                               const uint32_t *__restrict__ P_dev,
-                                                              uint32_t capacity, int shift, int next_shift,
-                                                              const uint32_t *__restrict__ base,
-                                                              uint32_t *__restrict__ next_C) {
+                                                              uint32_t capacity, int shift, uint32_t tiles,
+                                                              const uint32_t *__restrict__ base) {
   constexpr int BINS = 1 << BITS, PER = BINS / RX_THREADS;
   __shared__ uint32_t s_whist[RX_WARPS][BINS];  // per-warp digit counts -> tile-local offsets
   __shared__ uint32_t s_gofs[BINS];             // global position of a digit's run minus its local start
@@ -368,120 +409,95 @@ __global__ void __launch_bounds__(RX_THREADS, sizeof(KeyT) == 8 ? 2 : RX_MINBLOC
   // positions could run past the buffers.  Nothing is sorted; k_ranges leaves every range empty.
   if (P_dev[2] != 0) return;
   const uint32_t P = min(*P_dev, capacity);
-  const int ntiles = (int)((P + RX_TILE - 1) / RX_TILE);
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    __syncthreads();  // previous tile's shared state is no longer read
-    for (int i = tid; i < RX_WARPS * BINS; i += RX_THREADS) (&s_whist[0][0])[i] = 0;
+  const uint32_t tile = blockIdx.x;  // one sort tile per CTA; tiles past P (capacity path) have nothing to do
+  if (tile * RX_TILE >= P) return;
+  for (int i = tid; i < RX_WARPS * BINS; i += RX_THREADS) (&s_whist[0][0])[i] = 0;
+  __syncthreads();
+  const uint32_t first = (uint32_t)tile * RX_TILE + warp * (32 * RX_IPT) + lane;
+  const uint32_t tile_n = min((uint32_t)RX_TILE, P - (uint32_t)tile * RX_TILE);
+  KeyT key[RX_IPT];
+  uint32_t rank[RX_IPT];
+#pragma unroll
+  for (int r = 0; r < RX_IPT; r++) {
+    const uint32_t idx = first + r * 32;
+    key[r] = idx < P ? keys_in[idx] : (KeyT)0;
+  }
+  uint32_t gbase[PER];  // scatter bases of this thread's digits (below), loaded under the ranking
+#pragma unroll
+  for (int k = 0; k < PER; k++) gbase[k] = base[(size_t)(tid * PER + k) * tiles + tile];
+#pragma unroll
+  for (int r = 0; r < RX_IPT; r++) {
+    const bool valid = first + r * 32 < P;
+    const uint32_t d = (uint32_t)(key[r] >> shift) & (BINS - 1);
+    // lanes of this round with the same digit (ballot per digit bit: __match_any_sync is a
+    // data-dependent loop in hardware)
+    unsigned peers = __ballot_sync(0xffffffffu, valid);
+#pragma unroll
+    for (int b = 0; b < BITS; b++) {
+      const bool bit = (d >> b) & 1u;
+      const unsigned m = __ballot_sync(0xffffffffu, bit);
+      peers &= bit ? m : ~m;
+    }
+    const int leader = __ffs(peers) - 1;
+    uint32_t old = 0;
+    if (valid && lane == leader) {
+      old = s_whist[warp][d];
+      s_whist[warp][d] = old + __popc(peers);
+    }
+    old = __shfl_sync(0xffffffffu, old, leader < 0 ? 0 : leader);
+    rank[r] = old + __popc(peers & ((1u << lane) - 1u));
+    __syncwarp();
+  }
+  __syncthreads();
+  {  // per digit (thread t owns digits [PER t, PER t + PER)): offsets of the warps, local start
+    uint32_t cnt[PER], sum = 0;
+#pragma unroll
+    for (int k = 0; k < PER; k++) {
+      const int d = tid * PER + k;
+      uint32_t run = 0;
+#pragma unroll
+      for (int w = 0; w < RX_WARPS; w++) {
+        const uint32_t t = s_whist[w][d];
+        s_whist[w][d] = run;
+        run += t;
+      }
+      cnt[k] = run;
+      sum += run;
+    }
+    uint32_t inc = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += t;
+    }
+    if (lane == 31) s_scan[warp] = inc;
     __syncthreads();
-    const uint32_t first = (uint32_t)tile * RX_TILE + warp * (32 * RX_IPT) + lane;
-    const uint32_t tile_n = min((uint32_t)RX_TILE, P - (uint32_t)tile * RX_TILE);
-    KeyT key[RX_IPT];
-    uint32_t rank[RX_IPT];
+    uint32_t start = inc - sum;  // tile-local start of this thread's first digit
+    for (int w = 0; w < warp; w++) start += s_scan[w];
 #pragma unroll
-    for (int r = 0; r < RX_IPT; r++) {
-      const uint32_t idx = first + r * 32;
-      key[r] = idx < P ? keys_in[idx] : (KeyT)0;
+    for (int k = 0; k < PER; k++) {
+      const int d = tid * PER + k;
+#pragma unroll
+      for (int w = 0; w < RX_WARPS; w++) s_whist[w][d] += start;
+      s_gofs[d] = gbase[k] - start;
+      start += cnt[k];
     }
+  }
+  __syncthreads();
 #pragma unroll
-    for (int r = 0; r < RX_IPT; r++) {
-      const bool valid = first + r * 32 < P;
-      const uint32_t d = (uint32_t)(key[r] >> shift) & (BINS - 1);
-      // lanes of this round with the same digit (ballot per digit bit: __match_any_sync is a
-      // data-dependent loop in hardware)
-      unsigned peers = __ballot_sync(0xffffffffu, valid);
-#pragma unroll
-      for (int b = 0; b < BITS; b++) {
-        const bool bit = (d >> b) & 1u;
-        const unsigned m = __ballot_sync(0xffffffffu, bit);
-        peers &= bit ? m : ~m;
-      }
-      const int leader = __ffs(peers) - 1;
-      uint32_t old = 0;
-      if (valid && lane == leader) {
-        old = s_whist[warp][d];
-        s_whist[warp][d] = old + __popc(peers);
-      }
-      old = __shfl_sync(0xffffffffu, old, leader < 0 ? 0 : leader);
-      rank[r] = old + __popc(peers & ((1u << lane) - 1u));
-      __syncwarp();
+  for (int r = 0; r < RX_IPT; r++) {
+    if (first + r * 32 < P) {
+      const uint32_t lp = s_whist[warp][(uint32_t)(key[r] >> shift) & (BINS - 1)] + rank[r];
+      s_keys[lp] = key[r];
+      s_vals[lp] = vals_in[first + r * 32];  // (read here, not held in registers through the ranking)
     }
-    __syncthreads();
-    {  // per digit (thread t owns digits [PER t, PER t + PER)): offsets of the warps, local start
-      uint32_t cnt[PER], sum = 0;
-#pragma unroll
-      for (int k = 0; k < PER; k++) {
-        const int d = tid * PER + k;
-        uint32_t run = 0;
-#pragma unroll
-        for (int w = 0; w < RX_WARPS; w++) {
-          const uint32_t t = s_whist[w][d];
-          s_whist[w][d] = run;
-          run += t;
-        }
-        cnt[k] = run;
-        sum += run;
-      }
-      uint32_t inc = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-      }
-      if (lane == 31) s_scan[warp] = inc;
-      __syncthreads();
-      uint32_t start = inc - sum;  // tile-local start of this thread's first digit
-      for (int w = 0; w < warp; w++) start += s_scan[w];
-#pragma unroll
-      for (int k = 0; k < PER; k++) {
-        const int d = tid * PER + k;
-#pragma unroll
-        for (int w = 0; w < RX_WARPS; w++) s_whist[w][d] += start;
-        s_gofs[d] = base[(size_t)tile * BINS + d] - start;
-        start += cnt[k];
-      }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int r = 0; r < RX_IPT; r++) {
-      if (first + r * 32 < P) {
-        const uint32_t lp = s_whist[warp][(uint32_t)(key[r] >> shift) & (BINS - 1)] + rank[r];
-        s_keys[lp] = key[r];
-        s_vals[lp] = vals_in[first + r * 32];  // (read here, not held in registers through the ranking)
-      }
-    }
-    __syncthreads();
-#if !RX_UNROLL_OUT
-    for (uint32_t j = tid; j < tile_n; j += RX_THREADS) {  // sorted order: runs of equal digits are contiguous
-      const KeyT k = s_keys[j];
-      const uint32_t pos = s_gofs[(uint32_t)(k >> shift) & (BINS - 1)] + j;
-      keys_out[pos] = k;
-      vals_out[pos] = s_vals[j];
-      if (next_C != nullptr)
-        atomicAdd(next_C + (size_t)(pos / RX_TILE) * BINS + ((uint32_t)(k >> next_shift) & (BINS - 1)), 1u);
-    }
-#else
-    {  // sorted order: runs of equal digits are contiguous.  Unrolled: 16 independent LDS -> STG chains
-      KeyT ko[RX_IPT];
-      int32_t vo[RX_IPT];
-#pragma unroll
-      for (int r = 0; r < RX_IPT; r++) {
-        const uint32_t j = tid + r * RX_THREADS;
-        ko[r] = j < tile_n ? s_keys[j] : (KeyT)0;
-        vo[r] = j < tile_n ? s_vals[j] : 0;
-      }
-#pragma unroll
-      for (int r = 0; r < RX_IPT; r++) {
-        const uint32_t j = tid + r * RX_THREADS;
-        if (j < tile_n) {
-          const uint32_t pos = s_gofs[(uint32_t)(ko[r] >> shift) & (BINS - 1)] + j;
-          keys_out[pos] = ko[r];
-          vals_out[pos] = vo[r];
-          if (next_C != nullptr)
-            atomicAdd(next_C + (size_t)(pos / RX_TILE) * BINS + ((uint32_t)(ko[r] >> next_shift) & (BINS - 1)), 1u);
-        }
-      }
-    }
-#endif
+  }
+  __syncthreads();
+  for (uint32_t j = tid; j < tile_n; j += RX_THREADS) {  // sorted order: runs of equal digits are contiguous
+    const KeyT k = s_keys[j];
+    const uint32_t pos = s_gofs[(uint32_t)(k >> shift) & (BINS - 1)] + j;
+    keys_out[pos] = k;
+    vals_out[pos] = s_vals[j];
   }
 }
 
@@ -565,13 +581,11 @@ int sort_layout(int N, int H, int W, int64_t P, SortLayout *out) {
   L.vals_b = o; o = align_up(o + n * sizeof(int32_t), 256);
   L.recs = o;   o = align_up(o + ng * sizeof(Rec), 256);  // one record per Gaussian
   L.counters = o; o = align_up(o + (4 * T + 2) * sizeof(int), 256);  // rasterizer work area (launch_tile_list)
-  // zeroed per call: [status | global digit histograms | per-tile digit counts of every pass]
+  // k_colscan's claim counter and look-back descriptors, reset before every pass by k_digit_counts
   L.sort_state = o;
-  L.hist = o + 64;
-  L.desc = L.hist + (size_t)MAX_PASSES * 512 * sizeof(uint32_t);
-  L.desc_stride = tiles * 512 * sizeof(uint32_t);
-  o = align_up(L.desc + (size_t)MAX_PASSES * L.desc_stride, 256);
-  L.sort_state_bytes = o - L.sort_state;
+  L.desc = o + 8;
+  o = align_up(L.desc + (tiles * 512 + CS_SPAN - 1) / CS_SPAN * sizeof(unsigned long long), 256);
+  L.counts = o; o = align_up(o + tiles * 512 * sizeof(uint32_t), 256);  // digit counts / scatter bases of a pass
   L.bytes = o;
   *out = L;
   return 0;
@@ -593,16 +607,15 @@ static int keys_sort_ranges(int N, int64_t P_cap, const float *depths, const uin
   const uint32_t *P_dev = total;
   KeyT *ka = reinterpret_cast<KeyT *>(b + SL.keys_a), *kb = reinterpret_cast<KeyT *>(b + SL.keys_b);
   int32_t *va = reinterpret_cast<int32_t *>(b + SL.vals_a), *vb = reinterpret_cast<int32_t *>(b + SL.vals_b);
-  uint32_t *state = reinterpret_cast<uint32_t *>(b + SL.sort_state);
-  uint32_t *hist = reinterpret_cast<uint32_t *>(b + SL.hist);
+  uint32_t *claim = reinterpret_cast<uint32_t *>(b + SL.sort_state);
+  unsigned long long *desc = reinterpret_cast<unsigned long long *>(b + SL.desc);
+  uint32_t *counts = reinterpret_cast<uint32_t *>(b + SL.counts);
   const PassPlan &pp = kp.pp;
-  const int bins = 1 << pp.bits;
   const int sms = sm_count();
-  // only the part of the state the passes of this call use is cleared
-  const size_t tiles = (size_t)((P_cap + RX_TILE - 1) / RX_TILE);
-  const size_t pass_bytes = tiles * bins * sizeof(uint32_t);  // (<= SL.desc_stride: laid out contiguously)
-  GSB_CUDA_TRY(cudaMemsetAsync(state, 0, (SL.desc - SL.sort_state) + (size_t)pp.n * pass_bytes, st));
-  auto tile_counts = [&](int p) { return reinterpret_cast<uint32_t *>(b + SL.desc + (size_t)p * pass_bytes); };
+  // one sort tile per CTA; sized for the capacity, the kernels skip the tiles past the device's P
+  const uint32_t tiles = (uint32_t)((P_cap + RX_TILE - 1) / RX_TILE);
+  const uint32_t nscan = tiles << pp.bits;  // values k_colscan scans (a multiple of CS_ITEMS)
+  const int scan_grid = (int)((nscan + CS_SPAN - 1) / CS_SPAN);
   // k_keys writes (ka, va); pass p reads what pass p-1 wrote; keys alternate ka <-> kb, values
   // va <-> vb except that the last pass (or k_keys itself when nothing has to be sorted) writes
   // the caller's gsid_per_patch
@@ -610,9 +623,8 @@ static int keys_sort_ranges(int N, int64_t P_cap, const float *depths, const uin
   int32_t *vin = pp.n == 0 ? gsid_per_patch : va;
   {
     ProfScope ps(K_KEYS, st);
-    const int grid = min((N + 255) / 256, sms * 4);
-    k_keys<KeyT><<<grid, 256, (size_t)(pp.n > 0 ? pp.n : 1) * bins * sizeof(uint32_t), st>>>(
-        N, depths, incl, rects, gx, kp.shift, pp, (uint32_t)P_cap, kin, vin, hist, tile_counts(0), total + 2);
+    k_keys<KeyT><<<(N + 255) / 256, 256, 0, st>>>(N, depths, incl, rects, gx, kp.shift, (uint32_t)P_cap, kin, vin,
+                                                  total + 2);
   }
   GSB_CUDA_TRY(cudaGetLastError());
   if (sr != nullptr) {  // everything the host has to validate is known now; the sort and the
@@ -622,27 +634,29 @@ static int keys_sort_ranges(int N, int64_t P_cap, const float *depths, const uin
   }
   {
     ProfScope ps(K_SORT, st);
-    const int grid = (int)(tiles < (size_t)sms * 4 ? tiles : (size_t)sms * 4);
     for (int p = 0; p < pp.n; p++) {
       KeyT *kout = (kin == ka) ? kb : ka;
       int32_t *vout = (p == pp.n - 1) ? gsid_per_patch : ((vin == va) ? vb : va);
-      uint32_t *next_C = p + 1 < pp.n ? tile_counts(p + 1) : nullptr;
-      const int next_shift = p + 1 < pp.n ? pp.shift[p + 1] : 0;
       constexpr size_t dyn = RX_TILE * (sizeof(KeyT) + sizeof(int32_t));  // staging of the sorted tile
-      if (pp.bits == 9) {
-        static const cudaError_t attr = cudaFuncSetAttribute(k_radix_pass<KeyT, 9>,
+      if (pp.bits == 9) {  // (only 32-bit plans use 9-bit digits: key_plan)
+        constexpr int B9 = sizeof(KeyT) == 4 ? 9 : 8;
+        static const cudaError_t attr = cudaFuncSetAttribute(k_radix_pass<KeyT, B9>,
                                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
         GSB_CUDA_TRY(attr);
-        k_colscan<9><<<512 / 32, 1024, 0, st>>>(P_dev, (uint32_t)P_cap, hist + p * bins, tile_counts(p));
-        k_radix_pass<KeyT, 9><<<grid, RX_THREADS, dyn, st>>>(kin, vin, kout, vout, P_dev, (uint32_t)P_cap,
-                                                             pp.shift[p], next_shift, tile_counts(p), next_C);
+        k_digit_counts<KeyT, B9><<<tiles, RX_THREADS, 0, st>>>(kin, P_dev, (uint32_t)P_cap, pp.shift[p], tiles, counts,
+                                                                 desc, (uint32_t)scan_grid, claim);
+        k_colscan<<<scan_grid, CS_CTA, 0, st>>>(total + 2, nscan, counts, desc, claim);
+        k_radix_pass<KeyT, B9><<<tiles, RX_THREADS, dyn, st>>>(kin, vin, kout, vout, P_dev, (uint32_t)P_cap,
+                                                              pp.shift[p], tiles, counts);
       } else {
         static const cudaError_t attr = cudaFuncSetAttribute(k_radix_pass<KeyT, 8>,
                                                              cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
         GSB_CUDA_TRY(attr);
-        k_colscan<8><<<256 / 32, 1024, 0, st>>>(P_dev, (uint32_t)P_cap, hist + p * bins, tile_counts(p));
-        k_radix_pass<KeyT, 8><<<grid, RX_THREADS, dyn, st>>>(kin, vin, kout, vout, P_dev, (uint32_t)P_cap,
-                                                             pp.shift[p], next_shift, tile_counts(p), next_C);
+        k_digit_counts<KeyT, 8><<<tiles, RX_THREADS, 0, st>>>(kin, P_dev, (uint32_t)P_cap, pp.shift[p], tiles, counts,
+                                                                 desc, (uint32_t)scan_grid, claim);
+        k_colscan<<<scan_grid, CS_CTA, 0, st>>>(total + 2, nscan, counts, desc, claim);
+        k_radix_pass<KeyT, 8><<<tiles, RX_THREADS, dyn, st>>>(kin, vin, kout, vout, P_dev, (uint32_t)P_cap,
+                                                              pp.shift[p], tiles, counts);
       }
       kin = kout;
       vin = vout;

@@ -133,7 +133,8 @@ int launch_bin(int H, int W, int N, const float *us, float *depths, int32_t *are
 
 struct SortLayout {  // carve-up of the phase-2 workspace
   size_t keys_a, keys_b, vals_a, vals_b, recs, counters;
-  size_t sort_state, sort_state_bytes, hist, desc, desc_stride;  // radix-sort state, zeroed per call
+  size_t sort_state, desc;  // radix-sort scan: claim counter, look-back descriptors (reset per pass)
+  size_t counts;            // [digit][sort tile] counts, then scatter bases
   size_t bytes;
 };
 int sort_layout(int N, int H, int W, int64_t P, SortLayout *out);
