@@ -231,11 +231,19 @@ static bool planes_aligned(const float *image, const int32_t *contrib, const flo
   return (planes & 15) == 0 && (reinterpret_cast<uintptr_t>(ranges) & 7) == 0;
 }
 
+// The binning packs a Gaussian's tile rectangle into 16-bit fields: x1 == 65536 would wrap to 0
+// and put its patches into the wrong tiles.
+static bool grid_fits(int H, int W) {
+  return ((int64_t)W + GSB_TILE - 1) / GSB_TILE <= GSB_MAX_GRID_TILES &&
+         ((int64_t)H + GSB_TILE - 1) / GSB_TILE <= GSB_MAX_GRID_TILES;
+}
+
 size_t gsb_splat_bin_workspace_bytes(int N) { return bin_layout(N).bytes; }
 
 int gsb_splat_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
                   size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0, "splat: bad N/H/W");
+  GSB_REQUIRE(grid_fits(H, W), "splat: more than 65535 tiles in a row or column");
   GSB_REQUIRE(P_host != nullptr && bin_ws != nullptr, "splat: null workspace / P_host");
   GSB_REQUIRE(N == 0 || (us && depths && areas), "splat: null pointer");
   const BinLayout L = bin_layout(N);
@@ -271,6 +279,7 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
                      void *ws, size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                      int32_t *patch_range_per_tile, int32_t *gsid_per_patch, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splat: bad N/H/W/P");
+  GSB_REQUIRE(grid_fits(H, W), "splat: more than 65535 tiles in a row or column");
   GSB_REQUIRE(image && contrib && final_tau && patch_range_per_tile, "splat: null output");
   GSB_REQUIRE(planes_aligned(image, contrib, final_tau, patch_range_per_tile), "splat: misaligned output");
   GSB_REQUIRE(P == 0 || (us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch),
@@ -301,6 +310,7 @@ static int splat_forward_impl(int H, int W, int N, const float *us, const float 
                               int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                               gsb_stream_t stream, bool wait) {
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad N/H/W/P_cap");
+  GSB_REQUIRE(grid_fits(H, W), "splat_forward: more than 65535 tiles in a row or column");
   GSB_REQUIRE(image && contrib && final_tau && patch_range_per_tile && gsid_per_patch && status_host && bin_ws && ws,
               "splat_forward: null pointer");
   GSB_REQUIRE(planes_aligned(image, contrib, final_tau, patch_range_per_tile), "splat_forward: misaligned output");

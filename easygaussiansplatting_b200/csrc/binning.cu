@@ -17,6 +17,8 @@
 // (tile, depth-mm, id) order with half the key traffic -- and only the digits that can be
 // non-zero are sorted (9-bit digits when that saves a pass: 27 bits at 1080p = 3 passes).
 // Every pass is stable, so ties keep ascending Gaussian id exactly like thrust::sort_by_key.
+#include <atomic>
+
 #include "common.cuh"
 #include "kernels.h"
 #include "tile_io.cuh"
@@ -134,7 +136,7 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__res
           dkmax = max(dkmax, __float2uint_rz(__fmul_rn(d, 1000.0f)));  // kernel.cu:73
         }
       }
-      rects[i] = rect;  // rect packed as (x0 | x1 << 16, y0 | y1 << 16); grids up to 65535 x 65535
+      rects[i] = rect;  // rect packed as (x0 | x1 << 16, y0 | y1 << 16); grids up to 65535 x 65535 (api.cu)
     }
     cnt[k] = n;
   }
@@ -195,8 +197,9 @@ struct PassPlan {
   int shift[MAX_PASSES];
 };
 struct KeyPlan {
-  bool narrow;  // 32-bit keys
-  int shift;    // tile field starts at this bit
+  bool narrow;     // 32-bit keys
+  int shift;       // tile field starts at this bit
+  int depth_bits;  // low bits of the depth key the passes order (32: all of it)
   PassPlan pp;
 };
 static KeyPlan key_plan(int H, int W, uint32_t depth_key_max) {
@@ -211,10 +214,12 @@ static KeyPlan key_plan(int H, int W, uint32_t depth_key_max) {
     const int end = dbits + tbits;
     pp.bits = (end > 0 && (end + 8) / 9 < (end + 7) / 8) ? 9 : 8;
     for (int s = 0; s < end; s += pp.bits) pp.shift[pp.n++] = s;
+    p.depth_bits = dbits;  // a deeper key would run into the tile field
   } else {  // 64-bit layout: depth bits [0, dbits), tile bits [32, 32 + tbits); the gap is all zero
     pp.bits = 8;
     for (int s = 0; s < dbits; s += 8) pp.shift[pp.n++] = s;
     for (int s = 0; s < tbits; s += 8) pp.shift[pp.n++] = 32 + s;
+    p.depth_bits = (dbits + 7) / 8 * 8;  // the depth passes cover whole digits
   }
   return p;
 }
@@ -226,12 +231,13 @@ static KeyPlan key_plan(int H, int W, uint32_t depth_key_max) {
 // (== reference order), so every store is coalesced and no lane waits for a large rectangle.
 // 64-bit: tile << 32 | dk (kernel.cu:71-74); 32-bit: tile << dbits | dk.
 // *status |= 2 when a Gaussian's patches do not fit the capacity (it is dropped whole and
-// nothing is written at or past `capacity`), |= 4 when a depth key needs more bits than the plan
-// has (both only possible on the capacity-based path, gsb_splat_forward).
+// nothing is written at or past `capacity`), |= 4 when a depth key needs more than the
+// `depth_bits` the passes order, in either layout (both only possible on the capacity-based
+// path, gsb_splat_forward, whose plan comes from an earlier frame's depth keys).
 template <typename KeyT>
 __global__ void __launch_bounds__(256) k_keys(int N, const float *__restrict__ depths,
                                               const uint32_t *__restrict__ incl, const uint2 *__restrict__ rects,
-                                              int gx, int shift, uint32_t capacity,
+                                              int gx, int shift, int depth_bits, uint32_t capacity,
                                               KeyT *__restrict__ keys, int32_t *__restrict__ vals,
                                               uint32_t *__restrict__ status) {
   const int lane = threadIdx.x & 31;
@@ -249,9 +255,9 @@ __global__ void __launch_bounds__(256) k_keys(int N, const float *__restrict__ d
       const uint2 r = __ldg(rects + i);
       rx = r.x; ry = r.y;  // (x0 | x1 << 16, y0 | y1 << 16)
       dk = (KeyT)__float2uint_rz(__fmul_rn(d, 1000.0f));
-      if (sizeof(KeyT) == 4 && (dk >> shift) != 0) {  // deeper than the planned key width (capacity path)
+      if (depth_bits < 32 && (dk >> depth_bits) != 0) {  // deeper than the plan sorts (capacity path)
         atomicOr(status, 4u);
-        dk &= ((KeyT)1 << shift) - 1;
+        dk &= ((KeyT)1 << depth_bits) - 1;  // (keeps the tile field of a 32-bit key intact)
       }
     }
   }
@@ -600,6 +606,22 @@ int launch_pack_only(int64_t P, const int32_t *gsid_per_patch, const float *us, 
   return 0;
 }
 
+// k_radix_pass stages its tile in dynamic shared memory, past the 48 KB default with 64-bit keys.
+// That opt-in is a function attribute of the device's context: set on each device before its
+// first pass (a process that sorts on two devices needs it twice).
+template <typename KeyT, int BITS>
+static cudaError_t radix_pass_smem_opt_in(int bytes) {
+  static std::atomic<unsigned long long> done{0};  // bit d: set on device d (devices past 63: every call)
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+  if (done.load(std::memory_order_relaxed) & bit) return cudaSuccess;
+  e = cudaFuncSetAttribute(k_radix_pass<KeyT, BITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) done.fetch_or(bit, std::memory_order_relaxed);
+  return e;
+}
+
 template <typename KeyT>
 static int keys_sort_ranges(int N, int64_t P_cap, const float *depths, const uint32_t *incl, const uint2 *rects,
                             uint32_t *total, int gx, int T, const KeyPlan &kp, char *b, const SortLayout &SL,
@@ -623,8 +645,8 @@ static int keys_sort_ranges(int N, int64_t P_cap, const float *depths, const uin
   int32_t *vin = pp.n == 0 ? gsid_per_patch : va;
   {
     ProfScope ps(K_KEYS, st);
-    k_keys<KeyT><<<(N + 255) / 256, 256, 0, st>>>(N, depths, incl, rects, gx, kp.shift, (uint32_t)P_cap, kin, vin,
-                                                  total + 2);
+    k_keys<KeyT><<<(N + 255) / 256, 256, 0, st>>>(N, depths, incl, rects, gx, kp.shift, kp.depth_bits,
+                                                  (uint32_t)P_cap, kin, vin, total + 2);
   }
   GSB_CUDA_TRY(cudaGetLastError());
   if (sr != nullptr) {  // everything the host has to validate is known now; the sort and the
@@ -640,18 +662,14 @@ static int keys_sort_ranges(int N, int64_t P_cap, const float *depths, const uin
       constexpr size_t dyn = RX_TILE * (sizeof(KeyT) + sizeof(int32_t));  // staging of the sorted tile
       if (pp.bits == 9) {  // (only 32-bit plans use 9-bit digits: key_plan)
         constexpr int B9 = sizeof(KeyT) == 4 ? 9 : 8;
-        static const cudaError_t attr = cudaFuncSetAttribute(k_radix_pass<KeyT, B9>,
-                                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-        GSB_CUDA_TRY(attr);
+        GSB_CUDA_TRY((radix_pass_smem_opt_in<KeyT, B9>((int)dyn)));
         k_digit_counts<KeyT, B9><<<tiles, RX_THREADS, 0, st>>>(kin, P_dev, (uint32_t)P_cap, pp.shift[p], tiles, counts,
                                                                  desc, (uint32_t)scan_grid, claim);
         k_colscan<<<scan_grid, CS_CTA, 0, st>>>(total + 2, nscan, counts, desc, claim);
         k_radix_pass<KeyT, B9><<<tiles, RX_THREADS, dyn, st>>>(kin, vin, kout, vout, P_dev, (uint32_t)P_cap,
                                                               pp.shift[p], tiles, counts);
       } else {
-        static const cudaError_t attr = cudaFuncSetAttribute(k_radix_pass<KeyT, 8>,
-                                                             cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-        GSB_CUDA_TRY(attr);
+        GSB_CUDA_TRY((radix_pass_smem_opt_in<KeyT, 8>((int)dyn)));
         k_digit_counts<KeyT, 8><<<tiles, RX_THREADS, 0, st>>>(kin, P_dev, (uint32_t)P_cap, pp.shift[p], tiles, counts,
                                                                  desc, (uint32_t)scan_grid, claim);
         k_colscan<<<scan_grid, CS_CTA, 0, st>>>(total + 2, nscan, counts, desc, claim);

@@ -42,6 +42,8 @@ extern "C" {
 
 #define GSB_ABI_VERSION 1
 #define GSB_TILE 16            /* reference common.cuh:13 BLOCK */
+#define GSB_MAX_GRID_TILES 65535 /* tiles per row and per column the binning entry points accept:
+                                  * W, H <= 1 048 560 pixels; larger frames are refused */
 #define GSB_RECORD_BYTES 48    /* packed per-Gaussian record, see DESIGN.md "data layout" */
 
 typedef void *gsb_stream_t; /* cudaStream_t */
@@ -129,7 +131,10 @@ int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float 
  * touch no tile get depths = -1, areas = 0).  Leaves rects/offsets in `bin_ws` for phase 2.
  * Writes the patch count to *P_host and the largest depth key (uint32)(depth*1000) of a
  * binned Gaussian to *depth_key_max_host (nullable) after synchronising `stream` (the one
- * host sync; the reference has the same read-back, gausplat.cu:67). */
+ * host sync; the reference has the same read-back, gausplat.cu:67).
+ * This and every other entry point that bins (gsb_splat_render, gsb_splat_forward,
+ * gsb_splat_forward_enqueue) return an argument error when ceil(W/16) or ceil(H/16) exceeds
+ * GSB_MAX_GRID_TILES, and when a frame has 2^30 patches or more. */
 size_t gsb_splat_bin_workspace_bytes(int N);
 int gsb_splat_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas,
                   void *bin_ws, size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host,
@@ -159,7 +164,8 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
  * gsb_splat_bin + gsb_splat_render stall the GPU while the host reads P back to size the sort
  * workspace (the reference does the same, gausplat.cu:64-67).  Here the caller provides CAPACITIES
  * instead -- an upper bound P_cap on the patch count (e.g. 1.25 x the previous frame's P) and on the
- * depth keys (depth_key_cap >= every (uint32)(depth*1000); it fixes the key width) -- all kernels
+ * depth keys (depth_key_cap >= every (uint32)(depth*1000); it fixes the key width and the depth
+ * bits the sort orders; a key needing more bits is reported, never sorted by its low bits) -- all kernels
  * read the actual P from device memory, and the host looks at [P, max depth key, flags] only
  * after the sort and the rasterizer have been enqueued behind the copy: no GPU bubble.
  * Workspaces: bin_ws as for gsb_splat_bin; ws >= gsb_splat_workspace_bytes(N, H, W, P_cap);
@@ -178,7 +184,8 @@ int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds
 
 /* Same, but only ENQUEUES (no host wait, no event): for capture into a CUDA graph.  status_host is
  * written by a stream-ordered copy; the caller reads it after the work has completed (flags bit 1:
- * P_cap exceeded, bit 2: depth_key_cap exceeded, or P > P_cap -> the frame's outputs are invalid). */
+ * P_cap exceeded, bit 2: a depth key wider than the sort depth_key_cap planned, or P > P_cap -> the
+ * frame's outputs are invalid). */
 int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
                               float *depths, const float *colors, int32_t *areas, const void *packed_records,
                               int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,

@@ -118,24 +118,34 @@ def inverse_cov2d(cov2ds, depths, calc_J=True):
 
 
 # ---------------------------------------------------------------- splat / splatB
-def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, margin=2e-5):
-    """gausplat.cu:24-112 + kernel.cu:46-271.  depths (f32) and areas (i32) are MODIFIED IN
-    PLACE like the device op.  Returns dict(image[3,H,W] f64, contrib[H,W] i32,
-    final_tau[H,W] f64, ranges[T,2] i32, gsid[P] i32, keys[P] u64, ambiguous[H,W] bool)."""
-    us, cinv2ds, colors = _f32(us), _f32(cinv2ds), _f32(colors)
-    alphas = _f32(alphas).reshape(-1)
+def bin(height, width, us, depths, areas):
+    """gausplat.cu:50-91 + kernel.cu:46-150: the binning alone (no compositing, so large frames
+    stay cheap).  depths (f32) and areas (i32) are MODIFIED IN PLACE like the device op.
+    -> (P, ranges[T,2] i32, gsid[P] i32, keys[P] u64 as (tile << 32 | depth key))"""
+    us = _f32(us)
     assert depths.dtype == np.float32 and depths.flags.c_contiguous
     assert areas.dtype == np.int32 and areas.flags.c_contiguous
     N = us.shape[0]
     H, W = int(height), int(width)
     T = ((W + 15) // 16) * ((H + 15) // 16)
     L = lib()
-    P = L.orc_bin(H, W, N, _p(us), _p(depths), _p(areas), None, None, None)
+    P = int(L.orc_bin(H, W, N, _p(us), _p(depths), _p(areas), None, None, None))
     ranges = np.zeros((T, 2), dtype=np.int32)
     gsid = np.empty(max(P, 1), dtype=np.int32)
     keys = np.empty(max(P, 1), dtype=np.uint64)
     L.orc_bin(H, W, N, _p(us), _p(depths), _p(areas), _p(ranges), _p(gsid), _p(keys))
-    gsid, keys = gsid[:P], keys[:P]
+    return P, ranges, gsid[:P], keys[:P]
+
+
+def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, margin=2e-5):
+    """gausplat.cu:24-112 + kernel.cu:46-271.  depths (f32) and areas (i32) are MODIFIED IN
+    PLACE like the device op.  Returns dict(image[3,H,W] f64, contrib[H,W] i32,
+    final_tau[H,W] f64, ranges[T,2] i32, gsid[P] i32, keys[P] u64, ambiguous[H,W] bool)."""
+    us, cinv2ds, colors = _f32(us), _f32(cinv2ds), _f32(colors)
+    alphas = _f32(alphas).reshape(-1)
+    H, W = int(height), int(width)
+    P, ranges, gsid, keys = bin(H, W, us, depths, areas)
+    L = lib()
     image = np.empty((3, H, W)); contrib = np.empty((H, W), dtype=np.int32)
     ftau = np.empty((H, W)); amb = np.empty((H, W), dtype=np.uint8)
     L.orc_draw(H, W, _p(ranges), _p(gsid), _p(us), _p(cinv2ds), _p(alphas), _p(colors),
