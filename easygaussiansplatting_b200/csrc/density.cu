@@ -49,14 +49,22 @@ __global__ void k_density_accumulate(int64_t N, const float *__restrict__ dus, c
   }
 }
 
-// gsmodel.py:238-262
+// max that returns NaN when either input is NaN, like torch.max (fmaxf drops the NaN)
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// gsmodel.py:238-262.  Both maxima propagate NaN: a row with a NaN scale is neither pruned for
+// size (NaN > thr is false) nor small enough to clone (NaN <= thr is false), as in the reference.
 __device__ __forceinline__ uint8_t classify_row(int64_t i, const float *__restrict__ alphas_raw,
                                                 const float *__restrict__ scales_raw, const float *__restrict__ acc,
                                                 const int32_t *__restrict__ cnt, float alpha_raw_min,
                                                 float scale_raw_max, float grad_min, float scale_clone_max) {
   const float a = alphas_raw[i];
   const float s0 = scales_raw[3 * i], s1 = scales_raw[3 * i + 1], s2 = scales_raw[3 * i + 2];
-  const float smax = fmaxf(s0, fmaxf(s1, s2));
+  const float smax = fmax_nan(s0, fmax_nan(s1, s2));
   uint8_t c;
   if (a < alpha_raw_min || smax > scale_raw_max) {
     c = CLS_PRUNE;
@@ -64,7 +72,7 @@ __device__ __forceinline__ uint8_t classify_row(int64_t i, const float *__restri
     float g = acc[i] / (float)cnt[i];
     if (isnan(g)) g = 0.f;
     // max over exp(s) (the reference compares the activated scales, :257)
-    const float big = fmaxf(expf(s0), fmaxf(expf(s1), expf(s2)));
+    const float big = fmax_nan(expf(s0), fmax_nan(expf(s1), expf(s2)));
     c = g >= grad_min ? (big <= scale_clone_max ? CLS_CLONE : CLS_SPLIT) : CLS_KEEP;
   }
   return c;

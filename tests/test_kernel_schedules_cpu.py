@@ -307,3 +307,87 @@ def test_density_row_group_schedule(N, seed):
                 if name in ("low_shs", "high_shs"): assert np.array_equal(got, ref[name]), name
                 else: # untransformed copies of the sources land in the right rows
                     assert np.array_equal(got[K:K + C], P[name][cls == CLONE]) and np.array_equal(got[K + C:], P[name][cls == SPLIT]), name
+
+
+# ------------------------------------------------------------------ csrc/density.cu, the plan's scan
+SC_THREADS, SC_PER = 256, 4
+SC_ROWS = SC_THREADS * SC_PER
+
+def warp_inclusive_scan(x, axis):
+    """the __shfl_up_sync ladder of both scan kernels along the 32-lane `axis`: a lane below the
+    offset keeps its value"""
+    x = np.moveaxis(x, axis, -1)
+    lane = np.arange(32)
+    for o in (1, 2, 4, 8, 16):
+        y = np.zeros_like(x)
+        y[..., o:] = x[..., :32 - o]
+        x = x + np.where(lane >= o, y, 0).astype(x.dtype)
+    return np.moveaxis(x, -1, axis)
+
+def classify_count(cls, nb):
+    """k_density_classify_count's per-CTA counts, through its (survivors | clones << 16) packing"""
+    c = np.full(nb * SC_ROWS, PRUNE, np.uint8)
+    c[:cls.size] = cls
+    c = c.reshape(nb, SC_ROWS)
+    kc = ((c != PRUNE).astype(np.uint32) + ((c == CLONE).astype(np.uint32) << 16)).sum(axis=1, dtype=np.uint32)
+    sp = (c == SPLIT).sum(axis=1, dtype=np.uint32)
+    return np.stack([kc & 0xffff, kc >> 16, sp], axis=1).astype(np.int32)
+
+def scan_blocks(block_counts):
+    """k_density_scan_blocks: one 1024-thread CTA walks the counts 1024 CTAs at a time; within a
+    pass, warp scans + the earlier warps' totals; across passes, the carry"""
+    nb = block_counts.shape[0]
+    out = block_counts.copy()
+    carry = np.zeros(3, np.int64)
+    tid = np.arange(1024)
+    for base in range(0, nb, 1024):
+        b = base + tid
+        ok = b < nb
+        v = np.zeros((1024, 3), np.int64)
+        v[ok] = block_counts[b[ok]]
+        inc = warp_inclusive_scan(v.reshape(32, 32, 3), 1).reshape(1024, 3)
+        warp_tot = inc.reshape(32, 32, 3)[:, 31]
+        before = carry + (np.cumsum(warp_tot, axis=0) - warp_tot)[tid >> 5]
+        c0 = before + inc - v
+        out[b[ok]] = c0[ok]
+        carry = c0[1023] + v[1023]
+    return out, carry
+
+def slots_kernel(cls, block_offsets):
+    """k_density_slots: 4 consecutive rows per thread, a packed warp scan, the earlier warps'
+    totals and the CTA's offset from scan_blocks"""
+    nb = block_offsets.shape[0]
+    c = np.full(nb * SC_ROWS, PRUNE, np.uint8)
+    c[:cls.size] = cls
+    c = c.reshape(nb, SC_THREADS // 32, 32, SC_PER)
+    kc = ((c != PRUNE).astype(np.uint32) + ((c == CLONE).astype(np.uint32) << 16)).sum(axis=3, dtype=np.uint32)
+    sp = (c == SPLIT).sum(axis=3, dtype=np.uint32)
+    ikc, isp = warp_inclusive_scan(kc, -1), warp_inclusive_scan(sp, -1)
+    wkc, wsp = ikc[:, :, 31], isp[:, :, 31]
+    bkc = ikc - kc + (np.cumsum(wkc, axis=1, dtype=np.uint32) - wkc)[:, :, None]
+    bsp = isp - sp + (np.cumsum(wsp, axis=1, dtype=np.uint32) - wsp)[:, :, None]
+    off = block_offsets.astype(np.int64)[:, None, None, :]
+    run = np.stack([bkc & 0xffff, bkc >> 16, bsp], axis=-1).astype(np.int64) + off
+    out = np.empty(c.shape + (3,), np.int64)
+    for j in range(SC_PER):
+        out[..., j, :] = run
+        run = run + np.stack([c[..., j] != PRUNE, c[..., j] == CLONE, c[..., j] == SPLIT], axis=-1)
+    return out.reshape(-1, 3)[:cls.size]
+
+@pytest.mark.parametrize("nb", [1, 33, 1024, 1025, 2050])
+def test_density_scan_schedule(nb):
+    """classify-count -> scan_blocks -> slots, against the prefix sums of the class flags.  1025
+    and 2050 CTAs need scan_blocks' carry from one 1024-CTA pass to the next; CTAs 0, 1023 and
+    1024 are all clones (1024 in both halves of the packed count), CTA 1 all splits"""
+    rng = np.random.default_rng(nb)
+    N = nb * SC_ROWS - (37 if nb > 1 else 24)
+    cls = rng.integers(0, 4, N).astype(np.uint8)
+    for b, c in ((0, CLONE), (1, SPLIT), (1023, CLONE), (1024, CLONE)):
+        cls[b * SC_ROWS:(b + 1) * SC_ROWS] = c
+    counts = classify_count(cls, nb)
+    offsets, totals = scan_blocks(counts)
+    slots = slots_kernel(cls, offsets)
+    flags = np.stack([cls != PRUNE, cls == CLONE, cls == SPLIT], axis=1).astype(np.int64)
+    assert np.array_equal(offsets, np.cumsum(counts, axis=0) - counts)
+    assert np.array_equal(totals, flags.sum(axis=0))
+    assert np.array_equal(slots, np.cumsum(flags, axis=0) - flags)
