@@ -222,14 +222,7 @@ int gsb_gau_loss(int H, int W, const float *image, const float *gt_image, float 
   return launch_gau_loss(H, W, image, gt_image, loss_lambda, loss_out, dloss_dimage, ws, (cudaStream_t)stream);
 }
 
-// The rasterizer writes the three image planes with 16-byte stores and the binning writes the
-// tile ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h).
-static bool planes_aligned(const float *image, const int32_t *contrib, const float *final_tau,
-                           const int32_t *ranges) {
-  const uintptr_t planes = reinterpret_cast<uintptr_t>(image) | reinterpret_cast<uintptr_t>(contrib) |
-                           reinterpret_cast<uintptr_t>(final_tau);
-  return (planes & 15) == 0 && (reinterpret_cast<uintptr_t>(ranges) & 7) == 0;
-}
+static bool aligned(const void *p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 // The binning packs a Gaussian's tile rectangle into 16-bit fields: x1 == 65536 would wrap to 0
 // and put its patches into the wrong tiles.
@@ -238,39 +231,73 @@ static bool grid_fits(int H, int W) {
          ((int64_t)H + GSB_TILE - 1) / GSB_TILE <= GSB_MAX_GRID_TILES;
 }
 
+// The checks of a frame every entry point that bins makes.  bin_ws holds uint2 rectangles and
+// 8-byte look-back descriptors (gsb_splat_render does not pass its size: SIZE_MAX).
+static int check_frame(int H, int W, int N, const void *bin_ws, size_t bin_ws_bytes) {
+  GSB_REQUIRE(N >= 0 && H > 0 && W > 0, "splat: bad N/H/W");
+  GSB_REQUIRE(grid_fits(H, W), "splat: more than 65535 tiles in a row or column");
+  GSB_REQUIRE(aligned(bin_ws, 16), "splat: bin_ws misaligned");
+  GSB_REQUIRE(bin_ws_bytes >= bin_layout(N).bytes, "splat: bin workspace too small");
+  return 0;
+}
+
 size_t gsb_splat_bin_workspace_bytes(int N) { return bin_layout(N).bytes; }
 
 int gsb_splat_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
                   size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0 && H > 0 && W > 0, "splat: bad N/H/W");
-  GSB_REQUIRE(grid_fits(H, W), "splat: more than 65535 tiles in a row or column");
+  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
+  if (rc) return rc;
   GSB_REQUIRE(P_host != nullptr && bin_ws != nullptr, "splat: null workspace / P_host");
   GSB_REQUIRE(N == 0 || (us && depths && areas), "splat: null pointer");
   const BinLayout L = bin_layout(N);
-  GSB_REQUIRE(bin_ws_bytes >= L.bytes, "splat: bin workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = launch_bin(H, W, N, us, depths, areas, bin_ws, L, st);
+  rc = launch_bin(H, W, N, us, depths, areas, bin_ws, L, st);
   if (rc) return rc;
   uint32_t total[3] = {0, 0, 0};  // [patch count, largest depth key, flags]
   GSB_CUDA_TRY(cudaMemcpyAsync(total, static_cast<char *>(bin_ws) + L.total, 3 * sizeof(uint32_t),
                                cudaMemcpyDeviceToHost, st));
   GSB_CUDA_TRY(cudaStreamSynchronize(st));
-  GSB_REQUIRE((total[2] & 1u) == 0 && total[0] < (1u << 30), "splat: more than 2^30 patches");
+  GSB_REQUIRE((total[2] & GSB_STATUS_TOO_MANY_PATCHES) == 0 && total[0] < (1u << 30), "splat: more than 2^30 patches");
   *P_host = (int64_t)total[0];
   if (depth_key_max_host) *depth_key_max_host = total[1];
   return 0;
 }
 
-size_t gsb_splat_records_offset(int N, int H, int W, int64_t P) {
-  SortLayout L;
-  if (sort_layout(N, H, W, P, &L)) return 0;
-  return L.recs;
-}
+size_t gsb_splat_records_offset(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).recs; }
 
-size_t gsb_splat_workspace_bytes(int N, int H, int W, int64_t P) {
-  SortLayout L;
-  if (sort_layout(N, H, W, P, &L)) return 0;
-  return L.bytes;
+size_t gsb_splat_workspace_bytes(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).bytes; }
+
+// A binned frame from the sort to the image, shared by both ways of rendering one: P is the patch
+// count (gsb_splat_render) or its capacity (gsb_splat_forward).  With `sr` (the capacity path) the
+// frame is binned here first, after every argument has been checked, and its status is copied to
+// sr->host behind the keys.
+static int render_frame(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                        const float *cinv2ds, const float *alphas, float *depths, const float *colors,
+                        int32_t *areas, const void *packed_records, void *bin_ws, void *ws, size_t ws_bytes,
+                        float *image, int32_t *contrib, float *final_tau, int32_t *ranges, int32_t *gsid,
+                        const StatusRead *sr, cudaStream_t st) {
+  GSB_REQUIRE(image && contrib && final_tau && ranges, "splat: null output");
+  // the rasterizer writes the three image planes with 16-byte stores and the binning writes the
+  // tile ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h)
+  GSB_REQUIRE(aligned(image, 16) && aligned(contrib, 16) && aligned(final_tau, 16) && aligned(ranges, 8),
+              "splat: misaligned output");
+  GSB_REQUIRE(aligned(packed_records, 16), "splat: packed_records misaligned");
+  // 64-bit keys at ws + 0, records gathered 16 bytes at a time (the layout's offsets are 256-B multiples)
+  GSB_REQUIRE(aligned(ws, 16), "splat: ws misaligned");
+  const SortLayout SL = sort_layout(N, H, W, P);
+  GSB_REQUIRE(ws != nullptr && ws_bytes >= SL.bytes, "splat: workspace too small");
+  const BinLayout BL = bin_layout(N);
+  int rc = sr ? launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st) : 0;
+  if (rc) return rc;
+  rc = launch_sort_and_pack(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
+                            ranges, gsid, packed_records == nullptr, sr, st);
+  if (rc) return rc;
+  char *b = static_cast<char *>(ws);
+  const Rec *recs =
+      packed_records ? static_cast<const Rec *>(packed_records) : reinterpret_cast<const Rec *>(b + SL.recs);
+  // with P == 0 (or N == 0) every tile is empty: the rasterizer only writes zeros
+  return launch_draw(H, W, ranges, P > 0 ? recs : nullptr, gsid, image, contrib, final_tau,
+                     reinterpret_cast<int *>(b + SL.counters), st);
 }
 
 int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
@@ -278,29 +305,15 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
                      const void *packed_records, const void *bin_ws,
                      void *ws, size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                      int32_t *patch_range_per_tile, int32_t *gsid_per_patch, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splat: bad N/H/W/P");
-  GSB_REQUIRE(grid_fits(H, W), "splat: more than 65535 tiles in a row or column");
-  GSB_REQUIRE(image && contrib && final_tau && patch_range_per_tile, "splat: null output");
-  GSB_REQUIRE(planes_aligned(image, contrib, final_tau, patch_range_per_tile), "splat: misaligned output");
+  int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
+  if (rc) return rc;
+  GSB_REQUIRE(P >= 0, "splat: bad P");
   GSB_REQUIRE(P == 0 || (us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch),
               "splat: null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  SortLayout SL{};
-  {
-    int rc = sort_layout(N, H, W, P, &SL);
-    if (rc) return rc;
-    GSB_REQUIRE(ws != nullptr && ws_bytes >= SL.bytes, "splat: workspace too small");
-  }
-  const BinLayout BL = bin_layout(N);
-  GSB_REQUIRE((reinterpret_cast<uintptr_t>(packed_records) & 15) == 0, "splat: packed_records misaligned");
-  int rc = launch_sort_and_pack(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
-                                patch_range_per_tile, gsid_per_patch, packed_records == nullptr, nullptr, st);
-  if (rc) return rc;
-  const Rec *recs = P > 0 ? reinterpret_cast<const Rec *>(static_cast<char *>(ws) + SL.recs) : nullptr;
-  if (P > 0 && packed_records != nullptr) recs = static_cast<const Rec *>(packed_records);
-  // with P == 0 every tile is empty: the rasterizer only writes zeros
-  int *work = reinterpret_cast<int *>(static_cast<char *>(ws) + SL.counters);
-  return launch_draw(H, W, patch_range_per_tile, recs, gsid_per_patch, image, contrib, final_tau, work, st);
+  // (without `sr` nothing is binned: depths and bin_ws are only read)
+  return render_frame(H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors, nullptr,
+                      packed_records, const_cast<void *>(bin_ws), ws, ws_bytes, image, contrib, final_tau,
+                      patch_range_per_tile, gsid_per_patch, nullptr, (cudaStream_t)stream);
 }
 
 static int splat_forward_impl(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -309,48 +322,28 @@ static int splat_forward_impl(int H, int W, int N, const float *us, const float 
                               size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                               int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                               gsb_stream_t stream, bool wait) {
-  GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad N/H/W/P_cap");
-  GSB_REQUIRE(grid_fits(H, W), "splat_forward: more than 65535 tiles in a row or column");
-  GSB_REQUIRE(image && contrib && final_tau && patch_range_per_tile && gsid_per_patch && status_host && bin_ws && ws,
-              "splat_forward: null pointer");
-  GSB_REQUIRE(planes_aligned(image, contrib, final_tau, patch_range_per_tile), "splat_forward: misaligned output");
-  GSB_REQUIRE(N == 0 || (us && cinv2ds && alphas && depths && colors && areas), "splat_forward: null pointer");
-  GSB_REQUIRE((reinterpret_cast<uintptr_t>(packed_records) & 15) == 0, "splat_forward: packed_records misaligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  const BinLayout BL = bin_layout(N);
-  GSB_REQUIRE(bin_ws_bytes >= BL.bytes, "splat_forward: bin workspace too small");
-  SortLayout SL{};
-  int rc = sort_layout(N, H, W, P_cap, &SL);
+  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
   if (rc) return rc;
-  GSB_REQUIRE(ws_bytes >= SL.bytes, "splat_forward: workspace too small");
+  GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad P_cap");
+  GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_forward: null pointer");
+  GSB_REQUIRE(N == 0 || (us && cinv2ds && alphas && depths && colors && areas), "splat_forward: null pointer");
   static thread_local cudaEvent_t ready_ev = nullptr;
   if (wait && ready_ev == nullptr) GSB_CUDA_TRY(cudaEventCreateWithFlags(&ready_ev, cudaEventDisableTiming));
-  cudaEvent_t ready = wait ? ready_ev : nullptr;
-  const StatusRead sr{status_host, ready};
+  const StatusRead sr{status_host, wait ? ready_ev : nullptr};
   if (wait) status_host[0] = status_host[1] = status_host[2] = 0;
-  rc = launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st);
-  if (rc) return rc;
-  if (N == 0) {  // nothing to bin: every tile is empty
-    GSB_CUDA_TRY(cudaMemsetAsync(patch_range_per_tile, 0,
-                                 sizeof(int32_t) * 2 * (size_t)((W + GSB_TILE - 1) / GSB_TILE) * ((H + GSB_TILE - 1) / GSB_TILE), st));
-    int *work = reinterpret_cast<int *>(static_cast<char *>(ws) + SL.counters);
-    return launch_draw(H, W, patch_range_per_tile, nullptr, gsid_per_patch, image, contrib, final_tau, work, st);
-  }
-  rc = launch_sort_and_pack(H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
-                            patch_range_per_tile, gsid_per_patch, packed_records == nullptr, &sr, st);
-  if (rc) return rc;
-  const Rec *recs = packed_records != nullptr ? static_cast<const Rec *>(packed_records)
-                                              : reinterpret_cast<const Rec *>(static_cast<char *>(ws) + SL.recs);
-  int *work = reinterpret_cast<int *>(static_cast<char *>(ws) + SL.counters);
-  rc = launch_draw(H, W, patch_range_per_tile, recs, gsid_per_patch, image, contrib, final_tau, work, st);
-  if (rc) return rc;
-  if (!wait) return 0;  // enqueue-only (CUDA graph capture): the caller inspects status_host later
-  // the sort and the rasterizer are queued; now look at what the binning found
-  GSB_CUDA_TRY(cudaEventSynchronize(ready));
-  if ((status_host[2] & 1u) != 0 || status_host[0] >= (1u << 30)) return set_arg_error("splat: more than 2^30 patches");
-  if ((status_host[2] & 6u) != 0 || (int64_t)status_host[0] > P_cap) {
-    snprintf(g_err, sizeof(g_err), "splat_forward: capacity exceeded (P = %u of %lld, flags %u)", status_host[0],
-             (long long)P_cap, status_host[2]);
+  rc = render_frame(H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas, packed_records, bin_ws,
+                    ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, &sr,
+                    (cudaStream_t)stream);
+  if (rc || !wait) return rc;  // enqueue-only (CUDA graph capture): the caller inspects status_host later
+  // the sort and the rasterizer are queued; now look at what the binning found (N == 0: nothing
+  // was copied, the zeros stand)
+  GSB_CUDA_TRY(cudaEventSynchronize(sr.ready));
+  const uint32_t P = status_host[0], flags = status_host[2];
+  if ((flags & GSB_STATUS_TOO_MANY_PATCHES) != 0 || P >= (1u << 30))
+    return set_arg_error("splat: more than 2^30 patches");
+  if ((flags & (GSB_STATUS_P_CAP | GSB_STATUS_DEPTH_KEY)) != 0 || (int64_t)P > P_cap) {
+    snprintf(g_err, sizeof(g_err), "splat_forward: capacity exceeded (P = %u of %lld, flags %u)", P,
+             (long long)P_cap, flags);
     return GSB_CAPACITY_EXCEEDED;
   }
   return 0;
@@ -378,13 +371,8 @@ int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float 
                             gsid_per_patch, status_host, stream, false);
 }
 
-size_t gsb_splat_backward_workspace_bytes(int N, int H, int W, int64_t P) {
-  // per-Gaussian records (256-B aligned; only when they have to be rebuilt, P > 0) + the [N,9]
-  // moment accumulators
-  const size_t T = (size_t)((W + GSB_TILE - 1) / GSB_TILE) * (size_t)((H + GSB_TILE - 1) / GSB_TILE);
-  return (size_t)(P > 0 && N > 0 ? N : 1) * sizeof(Rec) + 512 + (size_t)(N > 0 ? N : 1) * 9 * sizeof(float) + 512 +
-         (4 * T + 2) * sizeof(int);  // + the rasterizer's work area
-}
+// (a ws at any address: the size is the split from the worst start, 255 bytes short of a 256-B boundary)
+size_t gsb_splat_backward_workspace_bytes(int N, int H, int W, int64_t P) { return bwd_layout(N, H, W, P, 1).bytes; }
 
 int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
                        const float *alphas, const float *colors, const int32_t *contrib,
@@ -401,18 +389,17 @@ int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const fl
   // with the forward's records handed in, the workspace only has to hold the moment rows
   const int64_t P_ws = packed_records != nullptr ? 0 : P;
   GSB_REQUIRE(ws_bytes >= gsb_splat_backward_workspace_bytes(N, H, W, P_ws), "splatB: workspace too small");
-  // workspace: [records, 256-B aligned (cp.async needs 16 B)] [moment rows] [work area]
-  uintptr_t base = (reinterpret_cast<uintptr_t>(ws) + 255) & ~(uintptr_t)255;
-  Rec *recs = reinterpret_cast<Rec *>(base);
-  uintptr_t mbase = (base + (size_t)(P_ws > 0 ? N : 1) * sizeof(Rec) + 255) & ~(uintptr_t)255;
-  float *moments = moments_out != nullptr ? moments_out : reinterpret_cast<float *>(mbase);
-  int *work = reinterpret_cast<int *>((mbase + (size_t)N * 9 * sizeof(float) + 255) & ~(uintptr_t)255);
+  char *b = static_cast<char *>(ws);
+  const BwdLayout L = bwd_layout(N, H, W, P_ws, reinterpret_cast<uintptr_t>(ws));
+  Rec *recs = reinterpret_cast<Rec *>(b + L.recs);
+  float *moments = moments_out != nullptr ? moments_out : reinterpret_cast<float *>(b + L.moments);
+  int *work = reinterpret_cast<int *>(b + L.work);
   if (P > 0) {
     GSB_REQUIRE(us && alphas && colors && contrib && final_tau && patch_range_per_tile && gsid_per_patch &&
                     dloss_dgammas,
                 "splatB: null pointer");
     if (packed_records != nullptr) {  // the forward's record stream is still valid: skip the re-pack
-      GSB_REQUIRE((reinterpret_cast<uintptr_t>(packed_records) & 15) == 0, "splatB: packed_records misaligned");
+      GSB_REQUIRE(aligned(packed_records, 16), "splatB: packed_records misaligned");
       recs = const_cast<Rec *>(static_cast<const Rec *>(packed_records));
     } else {
       int rc = launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, recs, st);

@@ -19,6 +19,7 @@
 // Every pass is stable, so ties keep ascending Gaussian id exactly like thrust::sort_by_key.
 #include <atomic>
 
+#include "../../include/gsplat_b200.h"
 #include "common.cuh"
 #include "kernels.h"
 #include "tile_io.cuh"
@@ -185,7 +186,7 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__res
 #pragma unroll
     for (int w = 0; w < RS_CTA / 32; w++) m = max(m, s_max[w]);
     if (m > 0) atomicMax(total + 1, m);  // largest depth key of a binned Gaussian
-    if (s_prefix + run > 0xffffffffull) atomicOr(total + 2, 1u);  // P does not fit 32 bits
+    if (s_prefix + run > 0xffffffffull) atomicOr(total + 2, GSB_STATUS_TOO_MANY_PATCHES);  // P does not fit 32 bits
   }
 }
 
@@ -230,8 +231,8 @@ static KeyPlan key_plan(int H, int W, uint32_t depth_key_max) {
 // 32 offsets (shuffles) and builds the key row-major inside that Gaussian's rectangle
 // (== reference order), so every store is coalesced and no lane waits for a large rectangle.
 // 64-bit: tile << 32 | dk (kernel.cu:71-74); 32-bit: tile << dbits | dk.
-// *status |= 2 when a Gaussian's patches do not fit the capacity (it is dropped whole and
-// nothing is written at or past `capacity`), |= 4 when a depth key needs more than the
+// *status |= GSB_STATUS_P_CAP when a Gaussian's patches do not fit the capacity (it is dropped whole
+// and nothing is written at or past `capacity`), |= GSB_STATUS_DEPTH_KEY when a depth key needs more than the
 // `depth_bits` the passes order, in either layout (both only possible on the capacity-based
 // path, gsb_splat_forward, whose plan comes from an earlier frame's depth keys).
 template <typename KeyT>
@@ -256,13 +257,13 @@ __global__ void __launch_bounds__(256) k_keys(int N, const float *__restrict__ d
       rx = r.x; ry = r.y;  // (x0 | x1 << 16, y0 | y1 << 16)
       dk = (KeyT)__float2uint_rz(__fmul_rn(d, 1000.0f));
       if (depth_bits < 32 && (dk >> depth_bits) != 0) {  // deeper than the plan sorts (capacity path)
-        atomicOr(status, 4u);
+        atomicOr(status, GSB_STATUS_DEPTH_KEY);
         dk &= ((KeyT)1 << depth_bits) - 1;  // (keeps the tile field of a 32-bit key intact)
       }
     }
   }
   if (n > 0 && (off > capacity || n > capacity - off)) {  // does not fit: drop, flag
-    atomicOr(status, 2u);
+    atomicOr(status, GSB_STATUS_P_CAP);
     n = 0;
   }
   const uint32_t start = __shfl_sync(0xffffffffu, off, 0);
@@ -574,7 +575,7 @@ int launch_bin(int H, int W, int N, const float *us, float *depths, int32_t *are
 }
 
 // ---------------------------------------------------------------- phase 2 host side
-int sort_layout(int N, int H, int W, int64_t P, SortLayout *out) {
+SortLayout sort_layout(int N, int H, int W, int64_t P) {
   SortLayout L{};
   const size_t T = (size_t)((W + TILE - 1) / TILE) * (size_t)((H + TILE - 1) / TILE);
   const size_t n = (size_t)(P > 0 ? P : 1);
@@ -593,8 +594,17 @@ int sort_layout(int N, int H, int W, int64_t P, SortLayout *out) {
   o = align_up(L.desc + (tiles * 512 + CS_SPAN - 1) / CS_SPAN * sizeof(unsigned long long), 256);
   L.counts = o; o = align_up(o + tiles * 512 * sizeof(uint32_t), 256);  // digit counts / scatter bases of a pass
   L.bytes = o;
-  *out = L;
-  return 0;
+  return L;
+}
+
+BwdLayout bwd_layout(int N, int H, int W, int64_t P, uintptr_t base) {
+  BwdLayout L{};
+  const size_t T = (size_t)((W + TILE - 1) / TILE) * (size_t)((H + TILE - 1) / TILE);
+  L.recs = align_up(base, 256) - base;  // (cp.async gathers the records 16 bytes at a time)
+  L.moments = L.recs + align_up((size_t)(P > 0 && N > 0 ? N : 1) * sizeof(Rec), 256);
+  L.work = L.moments + align_up((size_t)(N > 0 ? N : 1) * 9 * sizeof(float), 256);
+  L.bytes = L.work + (4 * T + 2) * sizeof(int);  // launch_tile_list's work area
+  return L;
 }
 
 int launch_pack_only(int64_t P, const int32_t *gsid_per_patch, const float *us, const float *cinv2ds,

@@ -137,7 +137,14 @@ struct SortLayout {  // carve-up of the phase-2 workspace
   size_t counts;            // [digit][sort tile] counts, then scatter bases
   size_t bytes;
 };
-int sort_layout(int N, int H, int W, int64_t P, SortLayout *out);
+SortLayout sort_layout(int N, int H, int W, int64_t P);
+// carve-up of splatB's workspace, as offsets from `base`, the address it starts at (any byte):
+// [records, only when they are rebuilt (P > 0), 256-B aligned] [N x 9 moment rows] [rasterizer
+// work area].  bytes covers the split from that start.
+struct BwdLayout {
+  size_t recs, moments, work, bytes;
+};
+BwdLayout bwd_layout(int N, int H, int W, int64_t P, uintptr_t base);
 // capacity-based path: where to copy [P, max depth key, flags] for the host, and the event that
 // tells it the copy has landed (recorded right after the key kernel)
 struct StatusRead {

@@ -2,10 +2,10 @@
 per-kernel launch cost).
 
 Below ~500k Gaussians the step is bound by the host: ~25 launches and their Python wrappers per
-step can cost more than the kernels themselves.  The
-capacity-based rasterizer (`gsb_splat_forward_enqueue`) has no host decision inside the frame,
-so the whole forward (fused per-Gaussian stage, binning, sort, rasterizer) and the whole backward
-replay as two graphs over static buffers:
+step can cost more than the kernels themselves.  The capacity-based rasterizer, enqueue-only
+(`ops._capacity_frame`), has no host decision inside the frame, so the whole forward (fused
+per-Gaussian stage, binning, sort, rasterizer) and the whole backward replay as two graphs over
+static buffers:
 
     step = GraphedFusedStep(pws, shs, alphas, scales, rots, cam)    # learns capacities, captures
     image = step.forward()                 # static tensor; camera = step.cam (update its tensors in place)
@@ -16,11 +16,9 @@ The parameters are captured by address: an optimizer that updates them in place 
 next replay.  `forward()`'s outputs are validated lazily: `backward()` (or `check()`) reads the
 binning status of the frame; a frame that outgrew the captured capacities raises `CapacityError`
 after which `recapture()` (larger bounds) and a repeat of the step are due."""
-import ctypes as C
-
 import torch
 
-from . import _lib, ops
+from . import ops
 
 
 class CapacityError(RuntimeError):
@@ -43,54 +41,31 @@ class GraphedFusedStep:
         us, ci, col, dep, ar = ops.preprocess(p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc,
                                               cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height)
         out = ops.splat(cam.height, cam.width, us, ci, p["alphas"], dep, col, ar)
-        P = out[4].numel()
         dkmax = int((dep.max().clamp_min(0) * 1000).item()) + 1
-        return max(int(P * self.headroom) + 4096, 4096), (1 << max(dkmax, 1).bit_length()) - 1
+        return ops._next_capacity(out[4].numel(), dkmax, headroom=self.headroom)
 
     def _forward_body(self):
         cam, p = self.cam, self.p
-        lib = _lib.load()
         us, ci, col, dep, ar, rec = ops.preprocess(p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc,
                                                    cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height,
                                                    alphas=p["alphas"])
-        N, H, W, dev = us.shape[0], cam.height, cam.width, self.device
-        T = ((W + 15) // 16) * ((H + 15) // 16)
-        bin_bytes = lib.gsb_splat_bin_workspace_bytes(N)
-        ws_bytes = lib.gsb_splat_workspace_bytes(N, H, W, self.P_cap)
-        bin_ws = torch.empty((bin_bytes,), dtype=torch.uint8, device=dev)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        contrib = torch.empty((H, W), dtype=torch.int32, device=dev)
-        final_tau = torch.empty((H, W), dtype=torch.float32, device=dev)
-        ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
-        gsid = torch.empty((self.P_cap,), dtype=torch.int32, device=dev)
-        _lib.check(lib.gsb_splat_forward_enqueue(
-            H, W, N, ops._ptr(us), ops._ptr(ci), ops._ptr(p["alphas"]), ops._ptr(dep), ops._ptr(col), ops._ptr(ar),
-            ops._ptr(rec), self.P_cap, self.dk_cap, ops._ptr(bin_ws), bin_bytes, ops._ptr(ws), ws_bytes,
-            ops._ptr(image), ops._ptr(contrib), ops._ptr(final_tau), ops._ptr(ranges), ops._ptr(gsid),
-            self.status.data_ptr(), ops._stream()), lib)
-        self._keep = (bin_ws, ws)
+        _, self._keep, (image, contrib, final_tau, ranges, gsid) = ops._capacity_frame(
+            cam.height, cam.width, us, ci, p["alphas"], dep, col, ar, rec, self.P_cap, self.dk_cap, self.status,
+            enqueue=True)
         self._fwd = dict(us=us, cinv2ds=ci, colors=col, depths=dep, areas=ar, records=rec, contrib=contrib,
                          final_tau=final_tau, ranges=ranges, gsid=gsid)
         self.image = image
 
     def _backward_body(self):
         cam, p, f = self.cam, self.p, self._fwd
-        lib = _lib.load()
-        N, H, W, dev = f["us"].shape[0], cam.height, cam.width, self.device
-        k = p["shs"].shape[1] // 3
-        ws_bytes = lib.gsb_splat_backward_workspace_bytes(N, H, W, 0)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-        moments = torch.empty((N, 9), dtype=torch.float32, device=dev)
-        _lib.check(lib.gsb_splat_backward(
-            H, W, N, self.P_cap, ops._ptr(f["us"]), ops._ptr(f["cinv2ds"]), ops._ptr(p["alphas"]), ops._ptr(f["colors"]),
-            ops._ptr(f["contrib"]), ops._ptr(f["final_tau"]), ops._ptr(f["ranges"]), ops._ptr(f["gsid"]),
-            ops._ptr(self.dloss_dimage), ops._ptr(f["records"]), ops._ptr(ws), ws_bytes, None, None, None, None,
-            ops._ptr(moments), ops._stream()), lib)
+        # all P_cap patch slots: the replay's patch count is only known on the device
+        moments = ops.splatB(cam.height, cam.width, f["us"], f["cinv2ds"], p["alphas"], f["depths"], f["colors"],
+                             f["contrib"], f["final_tau"], f["ranges"], f["gsid"], self.dloss_dimage,
+                             moments_only=True, records=f["records"])
         gpw, gsh, gs, gq, dus, dal = ops.preprocessB(
             p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=f["cinv2ds"])
-        self._keep_b = (ws, moments)
+        self._keep_b = moments
         self.grads = dict(dpws=gpw, dshs=gsh, dscales=gs, drots=gq, dalphas=dal, dus=dus)
 
     def recapture(self, P_cap=None, dk_cap=None):
@@ -126,11 +101,11 @@ class GraphedFusedStep:
         if self._pending:
             self._done.synchronize()
             self._pending = False
-            P, flags = int(self.status[0]) & 0xffffffff, int(self.status[2])
-            if (flags & 6) or P > self.P_cap:
+            P, _, flags = ops._decode_status(self.status)
+            if (flags & (ops.GSB_STATUS_P_CAP | ops.GSB_STATUS_DEPTH_KEY)) or P > self.P_cap:
                 raise CapacityError("frame outgrew the captured capacities (P = %d of %d, flags %d): "
                                     "recapture() and repeat the step" % (P, self.P_cap, flags))
-        return int(self.status[0]) & 0xffffffff
+        return ops._decode_status(self.status)[0]
 
     def backward(self):
         self.check()

@@ -156,16 +156,65 @@ def inverseCov2D(cov2ds, depths, calc_J):
 
 
 GSB_CAPACITY_EXCEEDED = 2
+GSB_STATUS_P_CAP, GSB_STATUS_DEPTH_KEY = 2, 4  # flags of the status word (gsplat_b200.h GSB_STATUS_*)
 _CAPACITY = {}  # (device index, H, W, N) -> (P_cap, depth_key_cap) learnt from the previous frame
 _STATUS = {}    # device index -> pinned int32[4] for gsb_splat_forward's status read
 CAPACITY_STATS = {"capacity_frames": 0, "exact_frames": 0, "outgrown": 0}  # how the frames of `capacity=True` went
 
 
-def _next_capacity(P, dkmax):
-    """Bounds for the next frame of the same shape: 25 % head-room on the patch count, and the key
-    width the exact path would pick for this frame's largest depth key."""
+def _next_capacity(P, dkmax, headroom=1.25):
+    """Bounds for the next frame of the same shape: `headroom` on the patch count, and the key
+    width the exact path would pick for a largest depth key of `dkmax`."""
     bits = max(int(dkmax), 1).bit_length()
-    return int(P * 1.25) + 4096, (1 << bits) - 1
+    return int(P * headroom) + 4096, (1 << bits) - 1
+
+
+def _decode_status(status):
+    """the capacity path's status word [P, largest depth key, flags] (int32 storage) -> unsigned ints"""
+    return tuple(int(v) & 0xffffffff for v in status[:3].tolist())
+
+
+def _bytes(n, dev):
+    return torch.empty((n,), dtype=torch.uint8, device=dev)
+
+
+def _frame_buffers(lib, dev, H, W, N, P):
+    """the sort workspace for P patch slots and splat's five outputs"""
+    T = ((W + 15) // 16) * ((H + 15) // 16)
+    ws = _bytes(lib.gsb_splat_workspace_bytes(N, H, W, P), dev)
+    return ws, [torch.empty((3, H, W), dtype=torch.float32, device=dev),
+                torch.empty((H, W), dtype=torch.int32, device=dev),
+                torch.empty((H, W), dtype=torch.float32, device=dev),
+                torch.empty((T, 2), dtype=torch.int32, device=dev),
+                torch.empty((P,), dtype=torch.int32, device=dev)]
+
+
+def _capacity_frame(H, W, us, cinv2ds, alphas, depths, colors, areas, records, P_cap, dk_cap, status,
+                    enqueue=False):
+    """Bins, sorts and draws one frame with the sort sized from the bounds (P_cap, dk_cap):
+    gsb_splat_forward, or gsb_splat_forward_enqueue (no host wait: for CUDA graph capture).
+    -> (False when the frame outgrew a bound, its workspaces, the five outputs with P_cap
+    gsid slots); `status` (pinned int32[4]) receives the status word."""
+    lib, N, dev = _L(), us.shape[0], us.device
+    bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
+    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap)
+    forward = lib.gsb_splat_forward_enqueue if enqueue else lib.gsb_splat_forward
+    rc = forward(H, W, N, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors), _ptr(areas),
+                 _ptr(records), P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
+                 *[_ptr(o) for o in out], status.data_ptr(), _stream())
+    if rc != GSB_CAPACITY_EXCEEDED:
+        _lib.check(rc, lib)
+    return rc == 0, (bin_ws, ws), out
+
+
+def _attach_records(gsid, records, ws, N, H, W, P_slots, inputs):
+    """lets splatB reuse this frame's records: the caller's, or those packed into `ws`, the sort
+    workspace of P_slots patches"""
+    if gsid.numel() > 0:
+        if records is not None:
+            _remember_records(gsid, records, 0, inputs)
+        else:
+            _remember_records(gsid, ws, _L().gsb_splat_records_offset(N, H, W, P_slots), inputs)
 
 
 def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=None, capacity=False):
@@ -190,79 +239,46 @@ def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=Non
             and colors.shape[0] == N and areas.shape[0] == N):
         raise ValueError("splat inputs disagree on N")
     dev = us.device
-    T = ((W + 15) // 16) * ((H + 15) // 16)
     lib = _L()
     if records is not None:
         records = _chk(records, "records", last=12, ndim=2)
         if records.shape[0] != N:
             raise ValueError("records must be [N, 12]")
+    inputs = (us, cinv2ds, alphas, colors)
     cap_key = (dev.index, H, W, N)
-    if capacity and cap_key in _CAPACITY and N > 0:
-        P_cap, dk_cap = _CAPACITY[cap_key]
-        with torch.cuda.device(dev):
-            st = _stream()
+    # the workspaces are consumed by kernels already enqueued on the current stream; the caching
+    # allocator only reuses them for later work on the same stream
+    with torch.cuda.device(dev):
+        if capacity and cap_key in _CAPACITY and N > 0:
+            P_cap, dk_cap = _CAPACITY[cap_key]
             status = _STATUS.get(dev.index)
             if status is None:
                 status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
-            bin_bytes = lib.gsb_splat_bin_workspace_bytes(N)
-            bin_ws = torch.empty((bin_bytes,), dtype=torch.uint8, device=dev)
-            ws_bytes = lib.gsb_splat_workspace_bytes(N, H, W, P_cap)
-            ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-            image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-            contrib = torch.empty((H, W), dtype=torch.int32, device=dev)
-            final_tau = torch.empty((H, W), dtype=torch.float32, device=dev)
-            ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
-            gsid = torch.empty((P_cap,), dtype=torch.int32, device=dev)
-            rc = lib.gsb_splat_forward(H, W, N, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors),
-                                       _ptr(areas), _ptr(records), P_cap, dk_cap, _ptr(bin_ws), bin_bytes, _ptr(ws),
-                                       ws_bytes, _ptr(image), _ptr(contrib), _ptr(final_tau), _ptr(ranges),
-                                       _ptr(gsid), status.data_ptr(), st)
-            if rc == 0:
+            ok, (_, ws), out = _capacity_frame(H, W, us, cinv2ds, alphas, depths, colors, areas, records, P_cap,
+                                               dk_cap, status)
+            if ok:
                 CAPACITY_STATS["capacity_frames"] += 1
-                P, dkmax = int(status[0]) & 0xffffffff, int(status[1]) & 0xffffffff
+                P, dkmax, _ = _decode_status(status)
                 _CAPACITY[cap_key] = _next_capacity(P, dkmax)
-                gsid = gsid[:P]
-                if P > 0:
-                    if records is not None:
-                        _remember_records(gsid, records, 0, (us, cinv2ds, alphas, colors))
-                    else:
-                        _remember_records(gsid, ws, lib.gsb_splat_records_offset(N, H, W, P_cap),
-                                          (us, cinv2ds, alphas, colors))
-                return [image, contrib, final_tau, ranges, gsid]
-            if rc != GSB_CAPACITY_EXCEEDED:
-                _lib.check(rc, lib)
+                out[4] = out[4][:P]
+                _attach_records(out[4], records, ws, N, H, W, P_cap, inputs)
+                return out
             CAPACITY_STATS["outgrown"] += 1
             del _CAPACITY[cap_key]  # outgrown: this frame the exact way (the in-place culls are idempotent)
-    with torch.cuda.device(dev):
-        st = _stream()
-        bin_bytes = lib.gsb_splat_bin_workspace_bytes(N)
-        bin_ws = torch.empty((bin_bytes,), dtype=torch.uint8, device=dev)
+        bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
         P, dkmax = C.c_int64(0), C.c_uint32(0)
-        _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_bytes,
-                                     C.byref(P), C.byref(dkmax), st), lib)
+        _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
+                                     C.byref(P), C.byref(dkmax), _stream()), lib)
         P = int(P.value)
-        ws_bytes = lib.gsb_splat_workspace_bytes(N, H, W, P)
-        ws = torch.empty((max(ws_bytes, 1),), dtype=torch.uint8, device=dev)
-        image = torch.empty((3, H, W), dtype=torch.float32, device=dev)
-        contrib = torch.empty((H, W), dtype=torch.int32, device=dev)
-        final_tau = torch.empty((H, W), dtype=torch.float32, device=dev)
-        ranges = torch.empty((T, 2), dtype=torch.int32, device=dev)
-        gsid = torch.empty((P,), dtype=torch.int32, device=dev)
+        ws, out = _frame_buffers(lib, dev, H, W, N, P)
         if capacity:
             CAPACITY_STATS["exact_frames"] += 1
             _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
         _lib.check(lib.gsb_splat_render(H, W, N, P, dkmax.value, _ptr(us), _ptr(cinv2ds), _ptr(alphas),
-                                        _ptr(depths), _ptr(colors), _ptr(records), _ptr(bin_ws), _ptr(ws), ws_bytes,
-                                        _ptr(image), _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid),
-                                        st), lib)
-        # the workspaces are consumed by kernels already enqueued on `st`; the caching
-        # allocator only reuses them for later work on the same stream
-        if P > 0:
-            if records is not None:
-                _remember_records(gsid, records, 0, (us, cinv2ds, alphas, colors))
-            else:
-                _remember_records(gsid, ws, lib.gsb_splat_records_offset(N, H, W, P), (us, cinv2ds, alphas, colors))
-    return [image, contrib, final_tau, ranges, gsid]
+                                        _ptr(depths), _ptr(colors), _ptr(records), _ptr(bin_ws), _ptr(ws), ws.numel(),
+                                        *[_ptr(o) for o in out], _stream()), lib)
+        _attach_records(out[4], records, ws, N, H, W, P, inputs)
+    return out
 
 
 # The forward leaves the packed per-Gaussian records in its workspace (or got them from
@@ -311,11 +327,14 @@ def clear_record_cache():
 
 
 def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau,
-           patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=False):
+           patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=False, records=None):
     """ext.cpp:20-32.  -> [dloss_dus[N,1,2], dloss_dcinv2ds[N,1,3], dloss_dalphas[N,1,1],
     dloss_dcolors[N,1,3]]   (`depths` is accepted and unused, as in the reference)
     moments_only (extension): -> the raw moment rows [N,9] for `preprocessB(..., moments=...)`;
-    the conversion pass to the four tensors is skipped."""
+    the conversion pass to the four tensors is skipped.
+    records (extension): the forward's packed per-Gaussian records [N,12] (what `splat` was given,
+    or its own); they are used as they are instead of those `splat` attached to gsid_per_patch,
+    and nothing is re-packed."""
     H, W = int(height), int(width)
     us = _chk(us, "us", last=2, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
     alphas = _chk(alphas, "alphas"); colors = _chk(colors, "colors", last=3, ndim=2)
@@ -332,6 +351,11 @@ def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_ta
         raise ValueError("patch_range_per_tile does not match the tile grid")
     if not (cinv2ds.shape[0] == N and alphas.numel() == N and colors.shape[0] == N):
         raise ValueError("splatB inputs disagree on N")
+    if records is not None:
+        records = _chk(records, "records", last=12, ndim=2)
+        _same_device(us, records)
+        if records.shape[0] != N:
+            raise ValueError("records must be [N, 12]")
     P = gsid.numel()
     dev = us.device
     o = dict(dtype=torch.float32, device=dev)
@@ -344,13 +368,15 @@ def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_ta
         moments = None
     lib = _L()
     with torch.cuda.device(dev):
-        recs = _cached_records(gsid, (us, cinv2ds, alphas, colors)) if P > 0 else None
+        if records is not None:
+            recs = records.data_ptr()
+        else:
+            recs = _cached_records(gsid, (us, cinv2ds, alphas, colors)) if P > 0 else None
         # with cached records only the [N,9] moment rows are needed from the workspace
-        ws_bytes = lib.gsb_splat_backward_workspace_bytes(N, H, W, 0 if recs else P)
-        ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        ws = _bytes(lib.gsb_splat_backward_workspace_bytes(N, H, W, 0 if recs else P), dev)
         _lib.check(lib.gsb_splat_backward(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
                                           _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
-                                          recs, _ptr(ws), ws_bytes, _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol),
+                                          recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol),
                                           _ptr(moments), _stream()), lib)
     if moments_only:
         return moments

@@ -27,8 +27,10 @@
  *     buffer at an odd offset): row-wise vector loads and stores are only used when the base
  *     pointer is aligned for them.  The exceptions are buffers the caller allocates for the
  *     call: packed_records must be 16-byte aligned, and so must gsb_splat_render's /
- *     gsb_splat_forward's image, contrib and final_tau; their patch_range_per_tile must be
- *     8-byte aligned.  A misaligned one is an argument error.
+ *     gsb_splat_forward's image, contrib and final_tau, the sort workspace `ws` of those and of
+ *     gsb_splat_forward_enqueue, and the binning workspace `bin_ws` of those and of
+ *     gsb_splat_bin; their patch_range_per_tile must be 8-byte aligned.  A misaligned one is
+ *     an argument error.  (gsb_splat_backward's `ws` may start anywhere.)
  */
 #ifndef GSPLAT_B200_H_
 #define GSPLAT_B200_H_
@@ -170,11 +172,14 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
  * after the sort and the rasterizer have been enqueued behind the copy: no GPU bubble.
  * Workspaces: bin_ws as for gsb_splat_bin; ws >= gsb_splat_workspace_bytes(N, H, W, P_cap);
  * gsid_per_patch[P_cap] (the first P entries are valid).  status_host[3] (pinned memory for a truly
- * asynchronous copy) receives P, the largest depth key and the flags.
+ * asynchronous copy) receives P, the largest depth key and the flags (GSB_STATUS_*).
  * Returns 0, or GSB_CAPACITY_EXCEEDED when a bound was too small: the outputs are then undefined and
  * the caller repeats the frame with gsb_splat_bin / gsb_splat_render (or larger capacities);
  * depths / areas have been culled in place exactly as gsb_splat_bin does, which is idempotent. */
 #define GSB_CAPACITY_EXCEEDED 2
+#define GSB_STATUS_TOO_MANY_PATCHES 1u /* flags bit 0: 2^32 patches or more (P saturated) */
+#define GSB_STATUS_P_CAP 2u            /* flags bit 1: the patches did not fit P_cap */
+#define GSB_STATUS_DEPTH_KEY 4u        /* flags bit 2: a depth key wider than depth_key_cap plans */
 int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
                       float *depths, const float *colors, int32_t *areas, const void *packed_records,
                       int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
@@ -183,9 +188,8 @@ int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds
                       gsb_stream_t stream);
 
 /* Same, but only ENQUEUES (no host wait, no event): for capture into a CUDA graph.  status_host is
- * written by a stream-ordered copy; the caller reads it after the work has completed (flags bit 1:
- * P_cap exceeded, bit 2: a depth key wider than the sort depth_key_cap planned, or P > P_cap -> the
- * frame's outputs are invalid). */
+ * written by a stream-ordered copy; the caller reads it after the work has completed (any
+ * GSB_STATUS_* flag, or P > P_cap -> the frame's outputs are invalid). */
 int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
                               float *depths, const float *colors, int32_t *areas, const void *packed_records,
                               int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
