@@ -167,6 +167,29 @@ int gsb_preprocess_forward(int N, int sh_dim3, const float *pws, const float *ro
                                (cudaStream_t)stream);
 }
 
+// Checks shared by the fused backward's two entry points: N, sh_dim3, the parameter and camera
+// pointers, and the upstream gradients -- the moment rows with the forward's conics and the dL/du
+// output, or the plain dL/du, dL/dconic and dL/dcolor.  `who` prefixes the error message.
+static int check_preprocess_backward(const char *who, int N, int sh_dim3, const float *pws, const float *rots,
+                                     const float *scales, const float *shs, const float *Rcw, const float *tcw,
+                                     const float *twc, const float *dloss_dus, const float *dloss_dcinv2ds,
+                                     const float *dloss_dcolors, const float *moments, const float *cinv2ds,
+                                     const float *dloss_dus_out) {
+  const char *err = nullptr;
+  if (N < 0)
+    err = "N < 0";
+  else if (!(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16))
+    err = "shs.shape[1]/3 must be 1, 4, 9 or 16";
+  else if (N > 0 && !(pws && rots && scales && shs && Rcw && tcw && twc))
+    err = "null pointer";
+  else if (N > 0 && !(moments ? (cinv2ds && dloss_dus_out) : (dloss_dus && dloss_dcinv2ds && dloss_dcolors)))
+    err = "null upstream gradient";
+  if (err == nullptr) return 0;
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", who, err);
+  return set_arg_error(msg);
+}
+
 int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
                             const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                             float fy, float cx, float cy, float width, float height, const float *dloss_dus,
@@ -174,26 +197,17 @@ int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *r
                             float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
                             const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                             gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0, "preprocessB: N < 0");
-  if (moments != nullptr) {  // upstream gradients as moment rows (gsb_splat_backward with moments_out)
-    GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-                "preprocessB: shs.shape[1]/3 must be 1, 4, 9 or 16");
-    GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && cinv2ds && dloss_dus_out &&
-                           dloss_dalphas_out && dloss_dpws && dloss_dscales && dloss_drots),
-                "preprocessB: null pointer");  // (dloss_dshs may be NULL: see gsb_sh_grad_expand)
-    const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
-    return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                                 nullptr, nullptr, nullptr, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, &mi,
-                                 (cudaStream_t)stream);
-  }
-  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-              "preprocessB: shs.shape[1]/3 must be 1, 4, 9 or 16");
-  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && dloss_dus && dloss_dcinv2ds &&
-                         dloss_dcolors && dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots),
+  if (int rc = check_preprocess_backward("preprocessB", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, dloss_dus,
+                                          dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dus_out))
+    return rc;
+  // with moments, dloss_dshs may be NULL (see gsb_sh_grad_expand) and dL/dalpha is an output
+  GSB_REQUIRE(N == 0 || (dloss_dpws && dloss_dscales && dloss_drots &&
+                         (moments ? dloss_dalphas_out != nullptr : dloss_dshs != nullptr)),
               "preprocessB: null pointer");
+  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, (cudaStream_t)stream);
+                               dloss_drots, nullptr, moments ? &mi : nullptr, (cudaStream_t)stream);
 }
 
 int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float *twcs, const float *dloss_dcolors,
@@ -556,13 +570,13 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
                                  const float *dloss_dalphas, const float *moments, const float *cinv2ds,
                                  float *dloss_dus_out, int world, int rank, void *const *regions_host,
                                  uint32_t epoch, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0, "preprocess_backward_push: N < 0");
+  if (int rc = check_preprocess_backward("preprocess_backward_push", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw,
+                                          twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds,
+                                          dloss_dus_out))
+    return rc;
+  GSB_REQUIRE(N == 0 || moments || dloss_dalphas, "preprocess_backward_push: null upstream gradient");
   GSB_REQUIRE(world >= 1 && world <= kMaxWorld && rank >= 0 && rank < world && regions_host && epoch != 0,
               "preprocess_backward_push: bad world / rank / regions / epoch");
-  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc), "preprocess_backward_push: null pointer");
-  GSB_REQUIRE(N == 0 || (moments ? (cinv2ds && dloss_dus_out)
-                                 : (dloss_dus && dloss_dcinv2ds && dloss_dcolors && dloss_dalphas)),
-              "preprocess_backward_push: null upstream gradient");
   const ExchangeGeom G = exchange_geom(N, sh_dim3, world);
   GradPush gp{};
   for (int p = 0; p < world; p++) {
@@ -581,9 +595,9 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
   gp.rank = rank;
   gp.epoch = epoch;
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, nullptr};
-  return launch_preprocess_bwd_push(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                                    dloss_dus, dloss_dcinv2ds, dloss_dcolors, gp, moments ? &mi : nullptr,
-                                    (cudaStream_t)stream);
+  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
+                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, nullptr, nullptr, nullptr, &gp,
+                               moments ? &mi : nullptr, (cudaStream_t)stream);
 }
 
 int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *const *regions_host, uint32_t epoch,

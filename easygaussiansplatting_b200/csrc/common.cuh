@@ -4,10 +4,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "pg_fused_math.h"
+
 namespace gsb {
 
 constexpr int TILE = 16;              // reference common.cuh:13
-constexpr float MIN_DEPTH = 0.2f;     // kernel.cu:10: (float)z < 0.2 (double)  <=>  z < 0.2f
+constexpr float MIN_DEPTH = pg::kMinDepth;
 constexpr float BAD_MARKER = -1.0f;   // kernel.cu:11
 constexpr float ALPHA_CLAMP = 0.99f;  // kernel.cu:245
 constexpr float ALPHA_SKIP = 0.002f;  // kernel.cu:246

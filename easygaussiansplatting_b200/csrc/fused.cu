@@ -210,12 +210,10 @@ __global__ void __launch_bounds__(PG) k_sh_expand(int N, int V, const float *__r
       const float *gc = gcols + ((size_t)v * N + i) * 3;
       const float g0 = __ldg(gc), g1 = __ldg(gc + 1), g2 = __ldg(gc + 2);
       float Y[K3], dY[K3][3];
-      float r[3] = {0.f, 0.f, 0.f};
+      float d[3], r[3] = {0.f, 0.f, 0.f};
       if (K3 > 1) {
-        const float d0 = pw[0] - __ldg(twcs + 3 * v), d1 = pw[1] - __ldg(twcs + 3 * v + 1),
-                    d2 = pw[2] - __ldg(twcs + 3 * v + 2);
-        const float ninv = 1.0f / sqrtf(d0 * d0 + d1 * d1 + d2 * d2);
-        r[0] = d0 * ninv; r[1] = d1 * ninv; r[2] = d2 * ninv;
+        const float twc[3] = {__ldg(twcs + 3 * v), __ldg(twcs + 3 * v + 1), __ldg(twcs + 3 * v + 2)};
+        pg::view_dir(pw, twc, d, r);
       }
       pg::sh_basis<K3>(r[0], r[1], r[2], Y, dY);
 #pragma unroll
@@ -272,42 +270,28 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
-                          float *g_scales, float *g_rots, const MomentsIn *mi, cudaStream_t st) {
+                          float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
+                          cudaStream_t st) {
   if (N <= 0) return 0;
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = (N + PG - 1) / PG;
+  const GradPush p = gp ? *gp : GradPush{};
+  const MomentsIn m = mi ? *mi : MomentsIn{};
   ProfScope ps(K_PRE_BWD, st);
-  if (mi != nullptr) {
-    GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, false, true><<<nb, PG, 0, st>>>(
-                            N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, nullptr, nullptr, nullptr,
-                            g_pws, g_shs, g_scales, g_rots, GradPush{}, *mi)));
+#define GSB_PRE_BWD(PUSH, MOM)                                                                                  \
+  GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM><<<nb, PG, 0, st>>>(                                      \
+                          N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us, g_cinv2ds, \
+                          g_colors, g_pws, g_shs, g_scales, g_rots, p, m)))
+  if (gp != nullptr && mi != nullptr) {
+    GSB_PRE_BWD(true, true);
+  } else if (gp != nullptr) {
+    GSB_PRE_BWD(true, false);
+  } else if (mi != nullptr) {
+    GSB_PRE_BWD(false, true);
   } else {
-    GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, false, false><<<nb, PG, 0, st>>>(
-                            N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us, g_cinv2ds, g_colors,
-                            g_pws, g_shs, g_scales, g_rots, GradPush{}, MomentsIn{})));
+    GSB_PRE_BWD(false, false);
   }
-  GSB_CUDA_TRY(cudaGetLastError());
-  return 0;
-}
-
-int launch_preprocess_bwd_push(int N, int k3, const float *pws, const float *rots, const float *scales,
-                               const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                               float fy, float cx, float cy, float width, float height, const float *g_us,
-                               const float *g_cinv2ds, const float *g_colors, const GradPush &gp,
-                               const MomentsIn *mi, cudaStream_t st) {
-  if (N <= 0) return 0;
-  const float tfx = width / (2 * fx), tfy = height / (2 * fy);
-  const int nb = (N + PG - 1) / PG;
-  ProfScope ps(K_PRE_BWD, st);
-  if (mi != nullptr) {
-    GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, true, true><<<nb, PG, 0, st>>>(
-                            N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, nullptr, nullptr, nullptr,
-                            nullptr, nullptr, nullptr, nullptr, gp, *mi)));
-  } else {
-    GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, true, false><<<nb, PG, 0, st>>>(
-                            N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us, g_cinv2ds, g_colors,
-                            nullptr, nullptr, nullptr, nullptr, gp, MomentsIn{})));
-  }
+#undef GSB_PRE_BWD
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -51,11 +51,16 @@ struct MomentsIn {
   float *dus_out;        // [N,2]  dL/du, still needed by the caller
   float *dalphas_out;    // [N]    dL/dalpha (nullable: the push variant forwards it instead)
 };
+struct GradPush;
+// gp == nullptr: the gradients go to g_pws, g_shs, g_scales, g_rots; otherwise into the exchange
+// staging slots gp describes (the g_* outputs are unused).  mi == nullptr: the upstream gradients
+// are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.
 int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
-                          float *g_scales, float *g_rots, const MomentsIn *mi, cudaStream_t st);
+                          float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
+                          cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,
@@ -88,11 +93,6 @@ struct GradPush {
   int world, rank;
   uint32_t epoch;
 };
-int launch_preprocess_bwd_push(int N, int k3, const float *pws, const float *rots, const float *scales,
-                               const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                               float fy, float cx, float cy, float width, float height, const float *g_us,
-                               const float *g_cinv2ds, const float *g_colors, const GradPush &gp,
-                               const MomentsIn *mi, cudaStream_t st);
 int launch_grad_reduce_bcast(const ExchangeGeom &G, int rank, void *const *regions, uint32_t epoch,
                              cudaStream_t st);
 

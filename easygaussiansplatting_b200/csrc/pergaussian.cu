@@ -8,10 +8,14 @@
 // float4 loads/stores.  Culled Gaussians write their zeros in-kernel, so outputs can be
 // torch.empty (the reference pre-fills every output with torch::full, gausplat.cu:176-178).
 //
-// Math follows docs/forward.md F.1-F.5.3 and docs/backward.md B.1-B.5.3 of the reference;
-// each kernel cites the reference kernel it replaces.
+// The values (means, covariances, colours, conics, radii) are computed by the stage functions of
+// pg_fused_math.h, the same ones the fused kernels (fused.cu) compose; each kernel here adds only
+// its shared-memory staging, the gate on the caller's depths and its Jacobian outputs, whose math
+// follows docs/backward.md B.1-B.5.3 of the reference.  Each kernel cites the reference kernel it
+// replaces.
 #include "common.cuh"
 #include "kernels.h"
+#include "pg_fused_math.h"
 #include "tile_io.cuh"
 
 namespace gsb {
@@ -33,37 +37,39 @@ __global__ void __launch_bounds__(PG) k_project(int N, const float *__restrict__
   const bool valid = tid < nv;
   tile_fetch<3>(pws, base, nv, sm, tid);
   __syncthreads();
-  float x = 0.f, y = 0.f, z = 0.f;
+  float pc[3] = {0.f, 0.f, 0.f};
+  bool keep = false;
   if (valid) {
-    const float *r = ROW(3);
-    float px = r[0], py = r[1], pz = r[2];
-    x = fmaf(__ldg(Rcw + 0), px, fmaf(__ldg(Rcw + 1), py, fmaf(__ldg(Rcw + 2), pz, __ldg(tcw + 0))));
-    y = fmaf(__ldg(Rcw + 3), px, fmaf(__ldg(Rcw + 4), py, fmaf(__ldg(Rcw + 5), pz, __ldg(tcw + 1))));
-    z = fmaf(__ldg(Rcw + 6), px, fmaf(__ldg(Rcw + 7), py, fmaf(__ldg(Rcw + 8), pz, __ldg(tcw + 2))));
+    float R[9], t[3];
+#pragma unroll
+    for (int k = 0; k < 9; k++) R[k] = __ldg(Rcw + k);
+#pragma unroll
+    for (int k = 0; k < 3; k++) t[k] = __ldg(tcw + k);
+    keep = pg::camera_point(R, t, ROW(3), pc);
   }
-  const bool keep = valid && !(z < MIN_DEPTH);
-  float zi = 0.f, xf = 0.f, yf = 0.f;
+  float zi = 0.f, xf = 0.f, yf = 0.f, u[2] = {0.f, 0.f};
   if (keep) {
-    zi = 1.0f / z;
-    xf = x * fx;
-    yf = y * fy;
+    zi = 1.0f / pc[2];
+    xf = pc[0] * fx;  // for du/dpc; the same products project_mean forms
+    yf = pc[1] * fy;
+    pg::project_mean(pc, zi, fx, fy, cx, cy, u);
   }
   __syncthreads();
   {  // pcs
     float *r = ROW(3);
-    r[0] = keep ? x : 0.f; r[1] = keep ? y : 0.f; r[2] = keep ? z : 0.f;
+    r[0] = keep ? pc[0] : 0.f; r[1] = keep ? pc[1] : 0.f; r[2] = keep ? pc[2] : 0.f;
   }
   __syncthreads();
   tile_flush<3>(pcs, base, nv, sm, tid);
   __syncthreads();
   {  // us
     float *r = ROW(2);
-    r[0] = keep ? fmaf(xf, zi, cx) : 0.f;
-    r[1] = keep ? fmaf(yf, zi, cy) : 0.f;
+    r[0] = u[0];
+    r[1] = u[1];
   }
   __syncthreads();
   tile_flush<2>(us, base, nv, sm, tid);
-  if (valid) depths[base + tid] = keep ? z : BAD_MARKER;
+  if (valid) depths[base + tid] = keep ? pc[2] : BAD_MARKER;
   if (du_dpcs != nullptr) {
     __syncthreads();
     float *r = ROW(6);
@@ -104,33 +110,21 @@ __global__ void __launch_bounds__(PG) k_cov3d(int N, const float *__restrict__ r
       q[0] = __ldg(rq); q[1] = __ldg(rq + 1); q[2] = __ldg(rq + 2); q[3] = __ldg(rq + 3);
     }
   }
-  const float w = q[0], x = q[1], y = q[2], z = q[3];
-  float R[9] = {1.f - 2.f * (y * y + z * z), 2.f * (x * y - z * w), 2.f * (x * z + y * w),
-                2.f * (x * y + z * w), 1.f - 2.f * (x * x + z * z), 2.f * (y * z - x * w),
-                2.f * (x * z - y * w), 2.f * (y * z + x * w), 1.f - 2.f * (x * x + y * y)};
-  float M[9];
-#pragma unroll
-  for (int r = 0; r < 3; r++)
-#pragma unroll
-    for (int c = 0; c < 3; c++) M[3 * r + c] = R[3 * r + c] * s[c];
+  float R[9], M[9], S6[6];
+  pg::cov3d(q, s, R, M, S6);
   __syncthreads();
   {
     float *o = ROW(6);
-    int n = 0;
 #pragma unroll
-    for (int r = 0; r < 3; r++)
-#pragma unroll
-      for (int c = r; c < 3; c++) {
-        float v = M[3 * r] * M[3 * c] + M[3 * r + 1] * M[3 * c + 1] + M[3 * r + 2] * M[3 * c + 2];
-        o[n++] = keep ? v : 0.f;
-      }
+    for (int n = 0; n < 6; n++) o[n] = keep ? S6[n] : 0.f;
   }
   __syncthreads();
   tile_flush<6>(cov3ds, base, nv, sm, tid);
   if (dcov3d_drots == nullptr || dcov3d_dscales == nullptr) return;
   __syncthreads();
   {
-    // dR/dq_p (times 2), rows as in quat_R above
+    // dR/dq_p (times 2), rows as in pg::quat_to_R
+    const float w = q[0], x = q[1], y = q[2], z = q[3];
     const float dR[4][9] = {{0.f, -z, y, z, 0.f, -x, -y, x, 0.f},
                             {0.f, y, z, y, -2.f * x, -w, z, w, -2.f * x},
                             {-2.f * y, x, w, x, 0.f, z, -w, z, -2.f * y},
@@ -214,35 +208,17 @@ __global__ void __launch_bounds__(PG) k_cov2d(int N, const float *__restrict__ c
     const float *r = ROW(3);
     pc[0] = r[0]; pc[1] = r[1]; pc[2] = r[2];
   }
-  if (!keep) { pc[0] = 0.f; pc[1] = 0.f; pc[2] = 1.f; }
   float R[9];
 #pragma unroll
   for (int k = 0; k < 9; k++) R[k] = __ldg(Rcw + k);
-  const float z = pc[2];
-  const float limx = 1.3f * tan_fovx, limy = 1.3f * tan_fovy;
-  const float x = fminf(limx, fmaxf(-limx, pc[0] / z)) * z;
-  const float y = fminf(limy, fmaxf(-limy, pc[1] / z)) * z;
-  const float zi = 1.0f / z, zi2 = zi * zi, zi3 = zi2 * zi;
-  const float J02 = -(fx * x) * zi2, J12 = -(fy * y) * zi2, J00 = fx * zi, J11 = fy * zi;
-  float M[6];
-#pragma unroll
-  for (int c = 0; c < 3; c++) {
-    M[c] = fmaf(J00, R[c], J02 * R[6 + c]);
-    M[3 + c] = fmaf(J11, R[3 + c], J12 * R[6 + c]);
-  }
-  const float S[9] = {c3[0], c3[1], c3[2], c3[1], c3[3], c3[4], c3[2], c3[4], c3[5]};
-  float MS[6];
-#pragma unroll
-  for (int a = 0; a < 2; a++)
-#pragma unroll
-    for (int c = 0; c < 3; c++)
-      MS[3 * a + c] = M[3 * a] * S[c] + M[3 * a + 1] * S[3 + c] + M[3 * a + 2] * S[6 + c];
+  pg::Cov2d g;
+  pg::cov2d(pc, keep, c3, R, fx, fy, tan_fovx, tan_fovy, g);
+  const float *M = g.M, *MS = g.MS;
+  const float x = g.xc, y = g.yc, zi2 = g.zi * g.zi, zi3 = zi2 * g.zi;
   __syncthreads();
   {
     float *o = ROW(3);
-    o[0] = keep ? MS[0] * M[0] + MS[1] * M[1] + MS[2] * M[2] + 0.3f : 0.f;
-    o[1] = keep ? MS[0] * M[3] + MS[1] * M[4] + MS[2] * M[5] : 0.f;
-    o[2] = keep ? MS[3] * M[3] + MS[4] * M[4] + MS[5] * M[5] + 0.3f : 0.f;
+    o[0] = keep ? g.c2[0] : 0.f; o[1] = keep ? g.c2[1] : 0.f; o[2] = keep ? g.c2[2] : 0.f;
   }
   __syncthreads();
   tile_flush<3>(cov2ds, base, nv, sm, tid);
@@ -298,13 +274,6 @@ __global__ void __launch_bounds__(PG) k_cov2d(int N, const float *__restrict__ c
 
 // ------------------------------------------------------------------ sh2Color
 // replaces kernel.cu:619-807.  K3 = coefficients per channel (1,4,9,16).
-__constant__ float SHC1[3] = {-0.4886025119029199f, 0.4886025119029199f, -0.4886025119029199f};
-__constant__ float SHC2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                              -1.0925484305920792f, 0.5462742152960396f};
-__constant__ float SHC3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                              0.3731763325901154f, -0.4570457994644658f, 1.445305721320277f,
-                              -0.5900435899266435f};
-
 template <int K3>
 __global__ void __launch_bounds__(PG) k_sh2color(int N, const float *__restrict__ shs,
                                                  const float *__restrict__ pws,
@@ -319,61 +288,24 @@ __global__ void __launch_bounds__(PG) k_sh2color(int N, const float *__restrict_
   const long long base = (long long)blockIdx.x * PG;
   const int nv = min(PG, (int)(N - base));
   const bool valid = tid < nv;
-  float d[3] = {0.f, 0.f, 1.f};
+  float pw[3] = {0.f, 0.f, 1.f}, tw[3] = {0.f, 0.f, 0.f};
   if (K3 > 1) {
     tile_fetch<3>(pws, base, nv, sm, tid);
     __syncthreads();
     if (valid) {
       const float *r = ROW(3);
-      d[0] = r[0] - __ldg(twc + 0); d[1] = r[1] - __ldg(twc + 1); d[2] = r[2] - __ldg(twc + 2);
+#pragma unroll
+      for (int k = 0; k < 3; k++) { pw[k] = r[k]; tw[k] = __ldg(twc + k); }
     }
     __syncthreads();
   }
   tile_fetch<KS>(shs, base, nv, sm, tid);
   __syncthreads();
   const float *sh = ROW(KS);  // [coef][rgb]
-  float Y[K3];
-  float dY[K3][3];
-#pragma unroll
-  for (int l = 0; l < K3; l++) { Y[l] = 0.f; dY[l][0] = dY[l][1] = dY[l][2] = 0.f; }
-  Y[0] = 0.28209479177387814f;
-  float ninv = 1.f, x = 0.f, y = 0.f, z = 0.f;
-  if (K3 > 1) {
-    ninv = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-    x = d[0] * ninv; y = d[1] * ninv; z = d[2] * ninv;
-    Y[1 % K3] = SHC1[0] * y; dY[1 % K3][1] = SHC1[0];
-    Y[2 % K3] = SHC1[1] * z; dY[2 % K3][2] = SHC1[1];
-    Y[3 % K3] = SHC1[2] * x; dY[3 % K3][0] = SHC1[2];
-  }
-  if (K3 > 4) {
-    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-    Y[4 % K3] = SHC2[0] * xy; dY[4 % K3][0] = SHC2[0] * y; dY[4 % K3][1] = SHC2[0] * x;
-    Y[5 % K3] = SHC2[1] * yz; dY[5 % K3][1] = SHC2[1] * z; dY[5 % K3][2] = SHC2[1] * y;
-    Y[6 % K3] = SHC2[2] * (2.f * zz - xx - yy);
-    dY[6 % K3][0] = -2.f * SHC2[2] * x; dY[6 % K3][1] = -2.f * SHC2[2] * y; dY[6 % K3][2] = 4.f * SHC2[2] * z;
-    Y[7 % K3] = SHC2[3] * xz; dY[7 % K3][0] = SHC2[3] * z; dY[7 % K3][2] = SHC2[3] * x;
-    Y[8 % K3] = SHC2[4] * (xx - yy); dY[8 % K3][0] = 2.f * SHC2[4] * x; dY[8 % K3][1] = -2.f * SHC2[4] * y;
-    if (K3 > 9) {
-      Y[9 % K3] = SHC3[0] * y * (3.f * xx - yy);
-      dY[9 % K3][0] = SHC3[0] * 6.f * xy; dY[9 % K3][1] = SHC3[0] * (3.f * xx - 3.f * yy);
-      Y[10 % K3] = SHC3[1] * xy * z;
-      dY[10 % K3][0] = SHC3[1] * yz; dY[10 % K3][1] = SHC3[1] * xz; dY[10 % K3][2] = SHC3[1] * xy;
-      Y[11 % K3] = SHC3[2] * y * (4.f * zz - xx - yy);
-      dY[11 % K3][0] = SHC3[2] * (-2.f * xy); dY[11 % K3][1] = SHC3[2] * (4.f * zz - xx - 3.f * yy);
-      dY[11 % K3][2] = SHC3[2] * 8.f * yz;
-      Y[12 % K3] = SHC3[3] * z * (2.f * zz - 3.f * xx - 3.f * yy);
-      dY[12 % K3][0] = SHC3[3] * (-6.f * xz); dY[12 % K3][1] = SHC3[3] * (-6.f * yz);
-      dY[12 % K3][2] = SHC3[3] * (6.f * zz - 3.f * xx - 3.f * yy);
-      Y[13 % K3] = SHC3[4] * x * (4.f * zz - xx - yy);
-      dY[13 % K3][0] = SHC3[4] * (4.f * zz - 3.f * xx - yy); dY[13 % K3][1] = SHC3[4] * (-2.f * xy);
-      dY[13 % K3][2] = SHC3[4] * 8.f * xz;
-      Y[14 % K3] = SHC3[5] * z * (xx - yy);
-      dY[14 % K3][0] = SHC3[5] * 2.f * xz; dY[14 % K3][1] = SHC3[5] * (-2.f * yz);
-      dY[14 % K3][2] = SHC3[5] * (xx - yy);
-      Y[15 % K3] = SHC3[6] * x * (xx - 3.f * yy);
-      dY[15 % K3][0] = SHC3[6] * (3.f * xx - 3.f * yy); dY[15 % K3][1] = SHC3[6] * (-6.f * xy);
-    }
-  }
+  float d[3], r[3] = {0.f, 0.f, 0.f}, ninv = 1.f;
+  if (K3 > 1) ninv = pg::view_dir<K3 == 16>(pw, tw, d, r);
+  float Y[K3], dY[K3][3];
+  pg::sh_basis<K3>(r[0], r[1], r[2], Y, dY);
   float col[3] = {0.5f, 0.5f, 0.5f};
   float dc_dr[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   if (valid) {
@@ -429,8 +361,7 @@ __global__ void __launch_bounds__(PG) k_sh2color(int N, const float *__restrict_
 }
 
 // ------------------------------------------------------------------ inverseCov2D
-// replaces kernel.cu:274-324.  radius in fp32 exactly as the reference: IEEE sqrt, one
-// multiply, ceil, truncate (decides the tile rectangle, so it has to be bit-identical).
+// replaces kernel.cu:274-324
 __global__ void __launch_bounds__(PG) k_inv_cov2d(int N, const float *__restrict__ cov2ds,
                                                   float *__restrict__ depths,
                                                   float *__restrict__ cinv2ds,
@@ -444,14 +375,13 @@ __global__ void __launch_bounds__(PG) k_inv_cov2d(int N, const float *__restrict
   tile_fetch<3>(cov2ds, base, nv, sm, tid);
   __syncthreads();
   bool keep = false;
-  float a = 1.f, b = 0.f, c = 1.f, di = 0.f;
+  float c2[3] = {1.f, 0.f, 1.f}, di = 0.f, cn[3];
   if (valid) {
     keep = !(depths[base + tid] < MIN_DEPTH);
     const float *r = ROW(3);
     if (keep) {
-      a = r[0]; b = r[1]; c = r[2];
-      di = 1.0f / (a * c - b * b);
-      if (isnan(di)) {
+      c2[0] = r[0]; c2[1] = r[1]; c2[2] = r[2];
+      if (!pg::conic(c2, di, cn)) {
         depths[base + tid] = BAD_MARKER;
         keep = false;
       }
@@ -460,19 +390,16 @@ __global__ void __launch_bounds__(PG) k_inv_cov2d(int N, const float *__restrict
   __syncthreads();
   {
     float *o = ROW(3);
-    o[0] = keep ? di * c : 0.f; o[1] = keep ? -di * b : 0.f; o[2] = keep ? di * a : 0.f;
+    o[0] = keep ? cn[0] : 0.f; o[1] = keep ? cn[1] : 0.f; o[2] = keep ? cn[2] : 0.f;
   }
   __syncthreads();
   tile_flush<3>(cinv2ds, base, nv, sm, tid);
   __syncthreads();
   {
     float *o = ROW(2);
-    int ax = 0, ay = 0;
-    if (keep) {
-      ax = (int)ceilf(__fmul_rn(3.0f, __fsqrt_rn(fabsf(a))));
-      ay = (int)ceilf(__fmul_rn(3.0f, __fsqrt_rn(fabsf(c))));
-    }
-    o[0] = __int_as_float(ax); o[1] = __int_as_float(ay);
+    int area[2] = {0, 0};
+    if (keep) pg::radius(c2, area);
+    o[0] = __int_as_float(area[0]); o[1] = __int_as_float(area[1]);
   }
   __syncthreads();
   tile_flush<2>(reinterpret_cast<float *>(areas), base, nv, sm, tid);
@@ -480,7 +407,7 @@ __global__ void __launch_bounds__(PG) k_inv_cov2d(int N, const float *__restrict
   __syncthreads();
   {
     float *o = ROW(9);
-    const float d2 = di * di;
+    const float a = c2[0], b = c2[1], c = c2[2], d2 = di * di;
     o[0] = keep ? -c * c * d2 : 0.f;      o[1] = keep ? 2.f * b * c * d2 : 0.f;       o[2] = keep ? di - a * c * d2 : 0.f;
     o[3] = keep ? b * c * d2 : 0.f;       o[4] = keep ? -di - 2.f * b * b * d2 : 0.f; o[5] = keep ? a * b * d2 : 0.f;
     o[6] = keep ? di - a * c * d2 : 0.f;  o[7] = keep ? 2.f * a * b * d2 : 0.f;       o[8] = keep ? -a * a * d2 : 0.f;

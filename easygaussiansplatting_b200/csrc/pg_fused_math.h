@@ -1,6 +1,8 @@
-// Per-Gaussian math of the fused preprocess path, shared by the CUDA kernels (fused.cu) and a
-// host build used only by tests (tests/host_shim/fused_host.cpp) -- hence host+device, no
-// CUDA-only intrinsics.
+// Per-Gaussian math, shared by the operator kernels (pergaussian.cu), the fused kernels
+// (fused.cu) and a host build used only by tests (tests/host_shim/fused_host.cpp) -- hence
+// host+device, no CUDA-only intrinsics.  Each formula is stated once, as a stage function
+// (camera_point, project_mean, cov3d, cov2d, conic, radius, view_dir, sh_basis); the operator
+// kernels call the stages one by one and add their Jacobians, the fused path composes them:
 //
 // forward : (pw, q, s, sh) -> u, conic, colour, depth, radius   == project + computeCov3D +
 //           computeCov2D + sh2Color + inverseCov2D of the reference (kernel.cu:274-807) without
@@ -32,13 +34,101 @@ struct Cam {
   float fx, fy, cx, cy, tan_fovx, tan_fovy;
 };
 
-constexpr float kMinDepth = 0.2f;
+constexpr float kMinDepth = 0.2f;  // kernel.cu:10: (float)z < 0.2 (double)  <=>  z < 0.2f
+
+// camera transform pc = Rcw pw + tcw; false when the Gaussian is nearer than kMinDepth (culled)
+GSB_HD bool camera_point(const float R[9], const float t[3], const float pw[3], float pc[3]) {
+  pc[0] = fmaf(R[0], pw[0], fmaf(R[1], pw[1], fmaf(R[2], pw[2], t[0])));
+  pc[1] = fmaf(R[3], pw[0], fmaf(R[4], pw[1], fmaf(R[5], pw[2], t[1])));
+  pc[2] = fmaf(R[6], pw[0], fmaf(R[7], pw[1], fmaf(R[8], pw[2], t[2])));
+  return !(pc[2] < kMinDepth);
+}
+
+// projected mean u = (fx x/z + cx, fy y/z + cy) of a kept Gaussian; zi = 1/z
+GSB_HD void project_mean(const float pc[3], float zi, float fx, float fy, float cx, float cy, float u[2]) {
+  u[0] = fmaf(pc[0] * fx, zi, cx);
+  u[1] = fmaf(pc[1] * fy, zi, cy);
+}
 
 GSB_HD void quat_to_R(const float q[4], float R[9]) {
   const float w = q[0], x = q[1], y = q[2], z = q[3];
   R[0] = 1.f - 2.f * (y * y + z * z); R[1] = 2.f * (x * y - z * w);       R[2] = 2.f * (x * z + y * w);
   R[3] = 2.f * (x * y + z * w);       R[4] = 1.f - 2.f * (x * x + z * z); R[5] = 2.f * (y * z - x * w);
   R[6] = 2.f * (x * z - y * w);       R[7] = 2.f * (y * z + x * w);       R[8] = 1.f - 2.f * (x * x + y * y);
+}
+
+// cov3d: R3 = R(q), M3 = R3 diag(s), S6 = upper triangle of Sigma = M3 M3^T
+GSB_HD void cov3d(const float q[4], const float s[3], float R3[9], float M3[9], float S6[6]) {
+  quat_to_R(q, R3);
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) M3[3 * r + c] = R3[3 * r + c] * s[c];
+  int n = 0;
+  for (int r = 0; r < 3; r++)
+    for (int c = r; c < 3; c++)
+      S6[n++] = M3[3 * r] * M3[3 * c] + M3[3 * r + 1] * M3[3 * c + 1] + M3[3 * r + 2] * M3[3 * c + 2];
+}
+
+// cov2d = M Sigma M^T + 0.3 I with M = J Rcw.  A culled Gaussian (keep false) is evaluated at
+// pc = (0, 0, 1) so that nothing divides by its depth.
+struct Cov2d {
+  float xc, yc;  // x, y after the 1.3*tan_fov clamp (kernel.cu:458-461)
+  float zi;      // 1/z
+  float M[6];    // J Rcw (2x3)
+  float MS[6];   // M Sigma
+  float c2[3];   // cov2d (a, b, c) with the +0.3 blur
+};
+
+GSB_HD void cov2d(const float pc[3], bool keep, const float S6[6], const float R[9], float fx, float fy,
+                  float tan_fovx, float tan_fovy, Cov2d &o) {
+  const float z = keep ? pc[2] : 1.0f;
+  o.zi = 1.0f / z;
+  const float limx = 1.3f * tan_fovx, limy = 1.3f * tan_fovy;
+  const float px = keep ? pc[0] : 0.f, py = keep ? pc[1] : 0.f;
+  o.xc = fminf(limx, fmaxf(-limx, px / z)) * z;
+  o.yc = fminf(limy, fmaxf(-limy, py / z)) * z;
+  const float zi2 = o.zi * o.zi;
+  const float J00 = fx * o.zi, J11 = fy * o.zi;
+  const float J02 = -(fx * o.xc) * zi2, J12 = -(fy * o.yc) * zi2;
+  for (int c = 0; c < 3; c++) {
+    o.M[c] = fmaf(J00, R[c], J02 * R[6 + c]);
+    o.M[3 + c] = fmaf(J11, R[3 + c], J12 * R[6 + c]);
+  }
+  const float S[9] = {S6[0], S6[1], S6[2], S6[1], S6[3], S6[4], S6[2], S6[4], S6[5]};
+  for (int a = 0; a < 2; a++)
+    for (int c = 0; c < 3; c++)
+      o.MS[3 * a + c] = o.M[3 * a] * S[c] + o.M[3 * a + 1] * S[3 + c] + o.M[3 * a + 2] * S[6 + c];
+  o.c2[0] = o.MS[0] * o.M[0] + o.MS[1] * o.M[1] + o.MS[2] * o.M[2] + 0.3f;
+  o.c2[1] = o.MS[0] * o.M[3] + o.MS[1] * o.M[4] + o.MS[2] * o.M[5];
+  o.c2[2] = o.MS[3] * o.M[3] + o.MS[4] * o.M[4] + o.MS[5] * o.M[5] + 0.3f;
+}
+
+// conic = cov2d^-1 with di = 1/det; false when di is NaN: such a Gaussian is culled (kernel.cu:301-305)
+GSB_HD bool conic(const float c2[3], float &di, float cn[3]) {
+  di = 1.0f / (c2[0] * c2[2] - c2[1] * c2[1]);
+  cn[0] = di * c2[2];
+  cn[1] = -di * c2[1];
+  cn[2] = di * c2[0];
+  return di == di;
+}
+
+// 3-sigma radius in pixels, exactly as the reference (IEEE sqrt, one multiply, ceil, truncate):
+// it decides the tile rectangle, so it has to be bit-identical
+GSB_HD void radius(const float c2[3], int area[2]) {
+  area[0] = (int)ceilf(3.0f * sqrtf(fabsf(c2[0])));
+  area[1] = (int)ceilf(3.0f * sqrtf(fabsf(c2[2])));
+}
+
+// view direction r = d / |d| with d = pw - twc; returns ninv = 1 / |d|.  FMA_NORM: |d|^2 as
+// fma(d2, d2, fma(d0, d0, d1 d1)), the rounding k_sh2color<16> has always had (the compiler
+// contracted it there and nowhere else)
+template <bool FMA_NORM = false>
+GSB_HD float view_dir(const float pw[3], const float twc[3], float d[3], float r[3]) {
+  d[0] = pw[0] - twc[0]; d[1] = pw[1] - twc[1]; d[2] = pw[2] - twc[2];
+  const float n2 = FMA_NORM ? fmaf(d[2], d[2], fmaf(d[0], d[0], d[1] * d[1]))
+                            : d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
+  const float ninv = 1.0f / sqrtf(n2);
+  r[0] = d[0] * ninv; r[1] = d[1] * ninv; r[2] = d[2] * ninv;
+  return ninv;
 }
 
 // real SH basis up to degree 3 and its partial derivatives wrt the (unit) direction, with
@@ -77,88 +167,46 @@ GSB_HD void sh_basis(float x, float y, float z, float Y[K3], float dY[K3][3]) {
 
 // Everything the backward needs again is recomputed from the parameters by this same
 // function, so forward and backward see identical intermediates.
-struct Geo {
+struct Geo : Cov2d {
   float pc[3];        // camera-frame position
-  float xc, yc;       // x, y after the 1.3*tan_fov clamp (kernel.cu:458-461)
-  float zi;           // 1/z
   float R3[9], M3[9]; // R(q), R(q) diag(s)
   float S6[6];        // cov3d upper triangle
-  float M[6];         // J Rcw (2x3)
-  float MS[6];        // M Sigma
-  float c2[3];        // cov2d (a, b, c) with the +0.3 blur
   float di;           // 1 / det(cov2d)
+  float cn[3];        // conic
   bool keep;          // z >= 0.2 and 1/det not NaN
 };
 
 GSB_HD void geometry(const float pw[3], const float q[4], const float s[3], const Cam &cam, Geo &g) {
-  const float *R = cam.R;
-  g.pc[0] = fmaf(R[0], pw[0], fmaf(R[1], pw[1], fmaf(R[2], pw[2], cam.t[0])));
-  g.pc[1] = fmaf(R[3], pw[0], fmaf(R[4], pw[1], fmaf(R[5], pw[2], cam.t[1])));
-  g.pc[2] = fmaf(R[6], pw[0], fmaf(R[7], pw[1], fmaf(R[8], pw[2], cam.t[2])));
-  g.keep = !(g.pc[2] < kMinDepth);
-  const float z = g.keep ? g.pc[2] : 1.0f;
-  g.zi = 1.0f / z;
-  quat_to_R(q, g.R3);
-  for (int r = 0; r < 3; r++)
-    for (int c = 0; c < 3; c++) g.M3[3 * r + c] = g.R3[3 * r + c] * s[c];
-  int n = 0;
-  for (int r = 0; r < 3; r++)
-    for (int c = r; c < 3; c++)
-      g.S6[n++] = g.M3[3 * r] * g.M3[3 * c] + g.M3[3 * r + 1] * g.M3[3 * c + 1] + g.M3[3 * r + 2] * g.M3[3 * c + 2];
-  const float limx = 1.3f * cam.tan_fovx, limy = 1.3f * cam.tan_fovy;
-  const float px = g.keep ? g.pc[0] : 0.f, py = g.keep ? g.pc[1] : 0.f;
-  g.xc = fminf(limx, fmaxf(-limx, px / z)) * z;
-  g.yc = fminf(limy, fmaxf(-limy, py / z)) * z;
-  const float zi2 = g.zi * g.zi;
-  const float J00 = cam.fx * g.zi, J11 = cam.fy * g.zi;
-  const float J02 = -(cam.fx * g.xc) * zi2, J12 = -(cam.fy * g.yc) * zi2;
-  for (int c = 0; c < 3; c++) {
-    g.M[c] = fmaf(J00, R[c], J02 * R[6 + c]);
-    g.M[3 + c] = fmaf(J11, R[3 + c], J12 * R[6 + c]);
-  }
-  const float S[9] = {g.S6[0], g.S6[1], g.S6[2], g.S6[1], g.S6[3], g.S6[4], g.S6[2], g.S6[4], g.S6[5]};
-  for (int a = 0; a < 2; a++)
-    for (int c = 0; c < 3; c++)
-      g.MS[3 * a + c] = g.M[3 * a] * S[c] + g.M[3 * a + 1] * S[3 + c] + g.M[3 * a + 2] * S[6 + c];
-  g.c2[0] = g.MS[0] * g.M[0] + g.MS[1] * g.M[1] + g.MS[2] * g.M[2] + 0.3f;
-  g.c2[1] = g.MS[0] * g.M[3] + g.MS[1] * g.M[4] + g.MS[2] * g.M[5];
-  g.c2[2] = g.MS[3] * g.M[3] + g.MS[4] * g.M[4] + g.MS[5] * g.M[5] + 0.3f;
-  g.di = 1.0f / (g.c2[0] * g.c2[2] - g.c2[1] * g.c2[1]);
-  if (g.di != g.di) g.keep = false;  // NaN determinant: culled (kernel.cu:301-305)
+  g.keep = camera_point(cam.R, cam.t, pw, g.pc);
+  cov3d(q, s, g.R3, g.M3, g.S6);
+  cov2d(g.pc, g.keep, g.S6, cam.R, cam.fx, cam.fy, cam.tan_fovx, cam.tan_fovy, g);
+  if (!conic(g.c2, g.di, g.cn)) g.keep = false;
 }
 
-// forward outputs for one Gaussian.  areas exactly as inverseCov2D (IEEE sqrt, *3, ceil).
+// forward outputs for one Gaussian
 template <int K3>
 GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], const float *sh /*[K3][3]*/,
-                        const Cam &cam, float u[2], float conic[3], float col[3], float *depth, int area[2]) {
+                        const Cam &cam, float u[2], float cn[3], float col[3], float *depth, int area[2]) {
   Geo g;
   geometry(pw, q, s, cam, g);
   // colour is not gated by depth in the reference (kernel.cu:619-726)
   float Y[K3], dY[K3][3];
-  float x = 0.f, y = 0.f, z = 0.f;
-  if (K3 > 1) {
-    const float d0 = pw[0] - cam.twc[0], d1 = pw[1] - cam.twc[1], d2 = pw[2] - cam.twc[2];
-    const float ninv = 1.0f / sqrtf(d0 * d0 + d1 * d1 + d2 * d2);
-    x = d0 * ninv; y = d1 * ninv; z = d2 * ninv;
-  }
-  sh_basis<K3>(x, y, z, Y, dY);
+  float d[3], r[3] = {0.f, 0.f, 0.f};
+  if (K3 > 1) view_dir(pw, cam.twc, d, r);
+  sh_basis<K3>(r[0], r[1], r[2], Y, dY);
   col[0] = col[1] = col[2] = 0.5f;
   for (int l = 0; l < K3; l++)
     for (int c = 0; c < 3; c++) col[c] = fmaf(Y[l], sh[3 * l + c], col[c]);
   if (!g.keep) {
     u[0] = u[1] = 0.f;
-    conic[0] = conic[1] = conic[2] = 0.f;
+    cn[0] = cn[1] = cn[2] = 0.f;
     area[0] = area[1] = 0;
     *depth = -1.0f;
     return;
   }
-  u[0] = fmaf(g.pc[0] * cam.fx, g.zi, cam.cx);
-  u[1] = fmaf(g.pc[1] * cam.fy, g.zi, cam.cy);
-  conic[0] = g.di * g.c2[2];
-  conic[1] = -g.di * g.c2[1];
-  conic[2] = g.di * g.c2[0];
-  area[0] = (int)ceilf(3.0f * sqrtf(fabsf(g.c2[0])));
-  area[1] = (int)ceilf(3.0f * sqrtf(fabsf(g.c2[2])));
+  project_mean(g.pc, g.zi, cam.fx, cam.fy, cam.cx, cam.cy, u);
+  cn[0] = g.cn[0]; cn[1] = g.cn[1]; cn[2] = g.cn[2];
+  radius(g.c2, area);
   *depth = g.pc[2];
 }
 
@@ -170,12 +218,8 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
                          float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/) {
   // ---- colour branch (independent of the depth cull, like sh2Color)
   float Y[K3], dY[K3][3];
-  float d[3] = {0.f, 0.f, 1.f}, ninv = 1.f, r[3] = {0.f, 0.f, 0.f};
-  if (K3 > 1) {
-    d[0] = pw[0] - cam.twc[0]; d[1] = pw[1] - cam.twc[1]; d[2] = pw[2] - cam.twc[2];
-    ninv = 1.0f / sqrtf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-    r[0] = d[0] * ninv; r[1] = d[1] * ninv; r[2] = d[2] * ninv;
-  }
+  float d[3], ninv = 1.f, r[3] = {0.f, 0.f, 0.f};
+  if (K3 > 1) ninv = view_dir(pw, cam.twc, d, r);
   sh_basis<K3>(r[0], r[1], r[2], Y, dY);
   float gdir[3] = {0.f, 0.f, 0.f};
   for (int l = 0; l < K3; l++) {

@@ -48,6 +48,32 @@ def _same_device(ref, *ts):
             raise ValueError("all tensors must be on the same device")
 
 
+def _shs(shs, N, ref):
+    """shs[N, 3k] with k in {1,4,9,16}, on the device of `ref` -> (shs contiguous, k)"""
+    shs = _chk(shs, "shs", ndim=2)
+    _same_device(ref, shs)
+    if shs.shape[0] != N or shs.shape[1] % 3 != 0 or shs.shape[1] // 3 not in (1, 4, 9, 16):
+        raise ValueError("shs must be [N, 3k] with k in {1,4,9,16}, got %s" % (tuple(shs.shape),))
+    return shs, shs.shape[1] // 3
+
+
+def _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc):
+    """Checks the per-Gaussian parameters and the camera the fused kernels read: float32 CUDA
+    tensors on one device, pws[N,3], rots[N,4], scales[N,3], shs[N,3k] with k in {1,4,9,16},
+    Rcw 9, tcw 3 and twc 3 elements.  -> ((the seven tensors, contiguous), N, k)"""
+    pws = _chk(pws, "pws", last=3, ndim=2); rots = _chk(rots, "rots", last=4, ndim=2)
+    scales = _chk(scales, "scales", last=3, ndim=2)
+    Rcw = _chk(Rcw, "Rcw"); tcw = _chk(tcw, "tcw"); twc = _chk(twc, "twc")
+    _same_device(pws, rots, scales, Rcw, tcw, twc)
+    N = pws.shape[0]
+    if rots.shape[0] != N or scales.shape[0] != N:
+        raise ValueError("pws, rots, scales disagree on N")
+    shs, k = _shs(shs, N, pws)
+    if Rcw.numel() != 9 or tcw.numel() != 3 or twc.numel() != 3:
+        raise ValueError("Rcw must have 9, tcw and twc 3 elements")
+    return (pws, rots, scales, shs, Rcw, tcw, twc), N, k
+
+
 def _ptr(t):
     return None if t is None else t.data_ptr()
 
@@ -117,14 +143,12 @@ def computeCov2D(cov3ds, pcs, Rcw, depths, focal_x, focal_y, width, height, calc
 def sh2Color(shs, pws, twc, calc_J):
     """ext.cpp:63-66.  shs[N,3k], k in {1,4,9,16}.
     -> [colors[N,3]] (+ dcolor_dshs[N,1,k], dcolor_dpws[N,3,3])"""
-    shs = _chk(shs, "shs", ndim=2); pws = _chk(pws, "pws", last=3, ndim=2); twc = _chk(twc, "twc")
-    _same_device(pws, shs, twc)
+    pws = _chk(pws, "pws", last=3, ndim=2); twc = _chk(twc, "twc")
+    _same_device(pws, twc)
     N = pws.shape[0]
-    if shs.shape[0] != N or shs.shape[1] % 3 != 0 or shs.shape[1] // 3 not in (1, 4, 9, 16):
-        raise ValueError("shs must be [N, 3k] with k in {1,4,9,16}, got %s" % (tuple(shs.shape),))
+    shs, k = _shs(shs, N, pws)
     if twc.numel() != 3:
         raise ValueError("twc must have 3 elements")
-    k = shs.shape[1] // 3
     o = dict(dtype=torch.float32, device=pws.device)
     col = torch.empty((N, 3), **o)
     Js = torch.empty((N, 1, k), **o) if calc_J else None
@@ -392,18 +416,7 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
     kernel.  -> [us[N,2], cinv2ds[N,3], colors[N,3], depths[N], areas[N,2] int32], ready for
     `splat`.  With alphas[N] a sixth output: the packed per-Gaussian records [N,12] for
     `splat(..., records=...)`."""
-    pws = _chk(pws, "pws", last=3, ndim=2); rots = _chk(rots, "rots", last=4, ndim=2)
-    scales = _chk(scales, "scales", last=3, ndim=2); shs = _chk(shs, "shs", ndim=2)
-    Rcw = _chk(Rcw, "Rcw"); tcw = _chk(tcw, "tcw"); twc = _chk(twc, "twc")
-    _same_device(pws, rots, scales, shs, Rcw, tcw, twc)
-    N = pws.shape[0]
-    if not (rots.shape[0] == N and scales.shape[0] == N and shs.shape[0] == N):
-        raise ValueError("preprocess inputs disagree on N")
-    if shs.shape[1] % 3 != 0 or shs.shape[1] // 3 not in (1, 4, 9, 16):
-        raise ValueError("shs must be [N, 3k] with k in {1,4,9,16}, got %s" % (tuple(shs.shape),))
-    if Rcw.numel() != 9 or tcw.numel() != 3 or twc.numel() != 3:
-        raise ValueError("Rcw must have 9, tcw and twc 3 elements")
-    k = shs.shape[1] // 3
+    (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     o = dict(dtype=torch.float32, device=pws.device)
     us = torch.empty((N, 2), **o); cinv = torch.empty((N, 3), **o); col = torch.empty((N, 3), **o)
     depths = torch.empty((N,), **o); areas = torch.empty((N, 2), dtype=torch.int32, device=pws.device)
@@ -432,27 +445,19 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     compact (with moments): dloss_dshs is not produced (None) -- the caller expands it from the
     views' dL/dcolor = moments[:, 6:9] with `sh_grad_expand` -- and the other gradients share one
     flat bucket [dpws | dscales | drots | dalphas] of 11 N floats (one collective sums it)."""
-    pws = _chk(pws, "pws", last=3, ndim=2); rots = _chk(rots, "rots", last=4, ndim=2)
-    scales = _chk(scales, "scales", last=3, ndim=2); shs = _chk(shs, "shs", ndim=2)
-    Rcw = _chk(Rcw, "Rcw"); tcw = _chk(tcw, "tcw"); twc = _chk(twc, "twc")
-    N = pws.shape[0]
+    (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     if moments is not None:
         moments = _chk(moments, "moments", last=9, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
-        _same_device(pws, rots, scales, shs, Rcw, tcw, twc, moments, cinv2ds)
+        _same_device(pws, moments, cinv2ds)
         if moments.shape[0] != N or cinv2ds.shape[0] != N:
             raise ValueError("moments / cinv2ds must have N rows")
         gu = gc = gcol = None
     else:
         gu = _chk(dloss_dus, "dloss_dus", last=2); gc = _chk(dloss_dcinv2ds, "dloss_dcinv2ds", last=3)
         gcol = _chk(dloss_dcolors, "dloss_dcolors", last=3)
-        _same_device(pws, rots, scales, shs, Rcw, tcw, twc, gu, gc, gcol)
+        _same_device(pws, gu, gc, gcol)
         if not (gu.numel() == 2 * N and gc.numel() == 3 * N and gcol.numel() == 3 * N):
             raise ValueError("preprocessB inputs disagree on N")
-    if not (rots.shape[0] == N and scales.shape[0] == N and shs.shape[0] == N):
-        raise ValueError("preprocessB inputs disagree on N")
-    if shs.shape[1] % 3 != 0 or shs.shape[1] // 3 not in (1, 4, 9, 16):
-        raise ValueError("shs must be [N, 3k] with k in {1,4,9,16}, got %s" % (tuple(shs.shape),))
-    k = shs.shape[1] // 3
     o = dict(dtype=torch.float32, device=pws.device)
     # one flat bucket [dshs | drots | dpws | dscales]: a multi-GPU caller can all-reduce the four
     # gradients in place with a single collective (parallel.allreduce_grads); every view starts

@@ -169,11 +169,10 @@ class GradExchange:
         `splatB(..., moments_only=True)`) + the forward's cinv2ds -- then this view's own
         dloss_dus[N,2] is returned (it is not part of the exchange)."""
         from . import _lib
-        from .ops import _chk, _ptr, _stream
-        pws = _chk(pws, "pws", last=3, ndim=2); rots = _chk(rots, "rots", last=4, ndim=2)
-        scales = _chk(scales, "scales", last=3, ndim=2); shs = _chk(shs, "shs", ndim=2)
-        N = pws.shape[0]
-        if N != self.N or shs.shape[1] != 3 * self.k3:
+        from .ops import _chk, _gaussian_params, _ptr, _stream
+        (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, cam.Rcw, cam.tcw,
+                                                                         cam.twc)
+        if N != self.N or k != self.k3:
             raise ValueError("GradExchange was built for N=%d, sh_dim3=%d" % (self.N, self.k3))
         gu = gc = gcol = ga = dus = None
         if moments is not None:
@@ -189,9 +188,8 @@ class GradExchange:
         self.epoch += 1
         with torch.cuda.device(pws.device):
             _lib.check(self.lib.gsb_preprocess_backward_push(
-                N, self.k3, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(_chk(cam.Rcw, "Rcw")),
-                _ptr(_chk(cam.tcw, "tcw")), _ptr(_chk(cam.twc, "twc")), float(cam.fx), float(cam.fy), float(cam.cx),
-                float(cam.cy), float(cam.width), float(cam.height), _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(ga),
+                N, self.k3, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
+                float(cam.fx), float(cam.fy), float(cam.cx), float(cam.cy), float(cam.width), float(cam.height), _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(ga),
                 _ptr(moments), _ptr(cinv2ds), _ptr(dus), self.world, self.rank, self.regions, self.epoch, _stream()),
                 self.lib)
         return dus

@@ -114,6 +114,31 @@ def test_exchange_argument_errors():
     assert rc != 0 and b"null region" in lib.gsb_last_error()
     rc = lib.gsb_grad_reduce_broadcast(1000, 16, 2, 0, regs, 0, None)
     assert rc != 0
+    # push checks the parameter set like preprocessB: rots / scales with N - 1 rows or a short
+    # camera tensor raise before any launch (the kernel reads N rows and 9 / 3 floats)
+    from easygaussiansplatting_b200.gsfunction import Camera
+    from easygaussiansplatting_b200.parallel import GradExchange
+    from easygaussiansplatting_b200.scene import synthetic_scene
+    N, k3 = 1000, 16
+    sc = synthetic_scene(N, 64, 64, sh_dim=3 * k3, seed=5)
+    P = {k: t(sc[k]) for k in ("pws", "rots", "scales", "shs")}
+    region, _ = GradExchange.alloc_region(GradExchange.region_bytes(N, k3, 1))
+    ex = GradExchange(N, k3, 1, 0, [region], DEV, own_region=region)
+    cam = dict(Rcw=t(sc["Rcw"]), tcw=t(sc["tcw"]), twc=t(sc["twc"]))
+    ins = [torch.zeros((N, k), device=DEV) for k in (2, 3, 3, 1)]
+    try:
+        torch.cuda.synchronize()
+        launches = lib.gsb_profile_launches(-1)
+        for name, short in (("rots", P["rots"][:-1]), ("scales", P["scales"][:-1]),
+                            ("Rcw", cam["Rcw"].reshape(-1)[:8]), ("tcw", cam["tcw"][:2]), ("twc", cam["twc"][:2])):
+            p, c = dict(P), dict(cam)
+            (p if name in p else c)[name] = short
+            with pytest.raises(ValueError):
+                ex.push(p["pws"], p["rots"], p["scales"], p["shs"],
+                        Camera(64, 64, sc["fx"], sc["fy"], sc["cx"], sc["cy"], c["Rcw"], c["tcw"], c["twc"]), *ins)
+        assert lib.gsb_profile_launches(-1) == launches
+    finally:
+        ex.close()
 
 
 @pytest.mark.parametrize("world,N,k3", [(2, 3001, 1), (4, 3001, 9), (2, 20001, 9), (4, 20001, 1)])

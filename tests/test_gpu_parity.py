@@ -468,6 +468,21 @@ def test_input_validation_raises():
                   torch.zeros(3, device=DEV), 1, 1, 0, 0, True)
     with pytest.raises(ValueError):
         g.sh2Color(torch.zeros(4, 15, device=DEV), torch.zeros(4, 3, device=DEV), torch.zeros(3, device=DEV), False)
+    # preprocessB checks the camera like preprocess: a short Rcw / tcw never reaches the kernel,
+    # which reads 9 and 3 floats from them
+    from easygaussiansplatting_b200 import _lib, ops
+    sc = synthetic_scene(64, 64, 64, sh_dim=48, seed=3)
+    P = [t(sc[k]) for k in ("pws", "rots", "scales", "shs")]
+    cam = [t(sc[k]) for k in ("Rcw", "tcw", "twc")] + [sc["fx"], sc["fy"], sc["cx"], sc["cy"], 64, 64]
+    grads = [torch.zeros(64, k, device=DEV) for k in (2, 3, 3)]
+    torch.cuda.synchronize()
+    launches = _lib.load().gsb_profile_launches(-1)
+    for i, short in ((0, t(sc["Rcw"]).reshape(-1)[:8]), (1, t(sc["tcw"])[:2])):
+        bad = list(cam)
+        bad[i] = short
+        with pytest.raises(ValueError):
+            ops.preprocessB(*P, *bad, *grads)
+    assert _lib.load().gsb_profile_launches(-1) == launches
 
 
 def test_non_contiguous_inputs():
