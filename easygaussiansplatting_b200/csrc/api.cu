@@ -38,7 +38,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "small_bmm", "density_accumulate", "density_classify",
                                              "density_scan", "density_apply", "reset_alpha",
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
-                                             "grad_reduce_broadcast", "sh_grad_expand"};
+                                             "grad_reduce_broadcast", "sh_grad_expand", "draw_rgbd",
+                                             "draw_backward_rgbd"};
 
 ProfScope::ProfScope(int id, cudaStream_t st) : id_(id), st_(st), stop_(nullptr) {
   std::lock_guard<std::mutex> lk(g_prof_mu);
@@ -190,14 +191,16 @@ static int check_preprocess_backward(const char *who, int N, int sh_dim3, const 
   return set_arg_error(msg);
 }
 
-int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
-                            const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                            float fy, float cx, float cy, float width, float height, const float *dloss_dus,
-                            const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
-                            float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
-                            const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
-                            gsb_stream_t stream) {
-  if (int rc = check_preprocess_backward("preprocessB", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, dloss_dus,
+// gsb_preprocess_backward and its RGB-D form (dloss_ddepths != NULL)
+static int preprocess_backward_impl(const char *who, int N, int sh_dim3, const float *pws, const float *rots,
+                                    const float *scales, const float *shs, const float *Rcw, const float *tcw,
+                                    const float *twc, float fx, float fy, float cx, float cy, float width,
+                                    float height, const float *dloss_dus, const float *dloss_dcinv2ds,
+                                    const float *dloss_dcolors, const float *dloss_ddepths, float *dloss_dpws,
+                                    float *dloss_dshs, float *dloss_dscales, float *dloss_drots,
+                                    const float *moments, const float *cinv2ds, float *dloss_dus_out,
+                                    float *dloss_dalphas_out, gsb_stream_t stream) {
+  if (int rc = check_preprocess_backward(who, N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, dloss_dus,
                                           dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dus_out))
     return rc;
   // with moments, dloss_dshs may be NULL (see gsb_sh_grad_expand) and dL/dalpha is an output
@@ -207,7 +210,34 @@ int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *r
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, moments ? &mi : nullptr, (cudaStream_t)stream);
+                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, (cudaStream_t)stream);
+}
+
+int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                            const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                            float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                            const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                            float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                            const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                            gsb_stream_t stream) {
+  return preprocess_backward_impl("preprocessB", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy,
+                                  width, height, dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, dloss_dpws,
+                                  dloss_dshs, dloss_dscales, dloss_drots, moments, cinv2ds, dloss_dus_out,
+                                  dloss_dalphas_out, stream);
+}
+
+int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                                 const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                                 float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                                 const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                                 const float *dloss_ddepths, gsb_stream_t stream) {
+  GSB_REQUIRE(N <= 0 || dloss_ddepths != nullptr, "preprocessB_rgbd: null dloss_ddepths");
+  return preprocess_backward_impl("preprocessB_rgbd", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx,
+                                  cy, width, height, dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_ddepths,
+                                  dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, moments, cinv2ds, dloss_dus_out,
+                                  dloss_dalphas_out, stream);
 }
 
 int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float *twcs, const float *dloss_dcolors,
@@ -289,8 +319,11 @@ static int render_frame(int H, int W, int N, int64_t P, uint32_t depth_key_max, 
                         const float *cinv2ds, const float *alphas, float *depths, const float *colors,
                         int32_t *areas, const void *packed_records, void *bin_ws, void *ws, size_t ws_bytes,
                         float *image, int32_t *contrib, float *final_tau, int32_t *ranges, int32_t *gsid,
-                        const StatusRead *sr, cudaStream_t st) {
+                        float *depth_image, float *alpha_image, const StatusRead *sr, cudaStream_t st) {
   GSB_REQUIRE(image && contrib && final_tau && ranges, "splat: null output");
+  // RGB-D frames (the *_rgbd entry points pass both planes, written like the image planes)
+  GSB_REQUIRE((depth_image == nullptr) == (alpha_image == nullptr), "splat: depth_image and alpha_image go together");
+  GSB_REQUIRE(aligned(depth_image, 16) && aligned(alpha_image, 16), "splat: misaligned depth_image / alpha_image");
   // the rasterizer writes the three image planes with 16-byte stores and the binning writes the
   // tile ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h)
   GSB_REQUIRE(aligned(image, 16) && aligned(contrib, 16) && aligned(final_tau, 16) && aligned(ranges, 8),
@@ -310,15 +343,15 @@ static int render_frame(int H, int W, int N, int64_t P, uint32_t depth_key_max, 
   const Rec *recs =
       packed_records ? static_cast<const Rec *>(packed_records) : reinterpret_cast<const Rec *>(b + SL.recs);
   // with P == 0 (or N == 0) every tile is empty: the rasterizer only writes zeros
-  return launch_draw(H, W, ranges, P > 0 ? recs : nullptr, gsid, image, contrib, final_tau,
+  return launch_draw(H, W, ranges, P > 0 ? recs : nullptr, gsid, image, contrib, final_tau, depth_image, alpha_image,
                      reinterpret_cast<int *>(b + SL.counters), st);
 }
 
-int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
-                     const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
-                     const void *packed_records, const void *bin_ws,
-                     void *ws, size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
-                     int32_t *patch_range_per_tile, int32_t *gsid_per_patch, gsb_stream_t stream) {
+static int splat_render_impl(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                             const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                             const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
+                             int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                             int32_t *gsid_per_patch, float *depth_image, float *alpha_image, gsb_stream_t stream) {
   int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
   if (rc) return rc;
   GSB_REQUIRE(P >= 0, "splat: bad P");
@@ -327,7 +360,28 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
   // (without `sr` nothing is binned: depths and bin_ws are only read)
   return render_frame(H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors, nullptr,
                       packed_records, const_cast<void *>(bin_ws), ws, ws_bytes, image, contrib, final_tau,
-                      patch_range_per_tile, gsid_per_patch, nullptr, (cudaStream_t)stream);
+                      patch_range_per_tile, gsid_per_patch, depth_image, alpha_image, nullptr, (cudaStream_t)stream);
+}
+
+int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                     const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                     const void *packed_records, const void *bin_ws,
+                     void *ws, size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                     int32_t *patch_range_per_tile, int32_t *gsid_per_patch, gsb_stream_t stream) {
+  return splat_render_impl(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, packed_records, bin_ws, ws,
+                           ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, nullptr, nullptr,
+                           stream);
+}
+
+int gsb_splat_render_rgbd(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                          const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                          const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
+                          int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                          float *depth_image, float *alpha_image, gsb_stream_t stream) {
+  GSB_REQUIRE(depth_image && alpha_image, "splat_rgbd: null depth_image / alpha_image");
+  return splat_render_impl(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, packed_records, bin_ws, ws,
+                           ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, depth_image,
+                           alpha_image, stream);
 }
 
 static int splat_forward_impl(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -335,7 +389,7 @@ static int splat_forward_impl(int H, int W, int N, const float *us, const float 
                               int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
                               size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                               int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
-                              gsb_stream_t stream, bool wait) {
+                              float *depth_image, float *alpha_image, gsb_stream_t stream, bool wait) {
   int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
   if (rc) return rc;
   GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad P_cap");
@@ -346,8 +400,8 @@ static int splat_forward_impl(int H, int W, int N, const float *us, const float 
   const StatusRead sr{status_host, wait ? ready_ev : nullptr};
   if (wait) status_host[0] = status_host[1] = status_host[2] = 0;
   rc = render_frame(H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas, packed_records, bin_ws,
-                    ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, &sr,
-                    (cudaStream_t)stream);
+                    ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, depth_image,
+                    alpha_image, &sr, (cudaStream_t)stream);
   if (rc || !wait) return rc;  // enqueue-only (CUDA graph capture): the caller inspects status_host later
   // the sort and the rasterizer are queued; now look at what the binning found (N == 0: nothing
   // was copied, the zeros stand)
@@ -371,7 +425,19 @@ int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds
                       gsb_stream_t stream) {
   return splat_forward_impl(H, W, N, us, cinv2ds, alphas, depths, colors, areas, packed_records, P_cap, depth_key_cap,
                             bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
-                            gsid_per_patch, status_host, stream, true);
+                            gsid_per_patch, status_host, nullptr, nullptr, stream, true);
+}
+
+int gsb_splat_forward_rgbd(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
+                           float *depths, const float *colors, int32_t *areas, const void *packed_records,
+                           int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
+                           size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                           int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
+                           float *depth_image, float *alpha_image, gsb_stream_t stream) {
+  GSB_REQUIRE(depth_image && alpha_image, "splat_forward_rgbd: null depth_image / alpha_image");
+  return splat_forward_impl(H, W, N, us, cinv2ds, alphas, depths, colors, areas, packed_records, P_cap, depth_key_cap,
+                            bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
+                            gsid_per_patch, status_host, depth_image, alpha_image, stream, true);
 }
 
 int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -382,18 +448,20 @@ int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float 
                               gsb_stream_t stream) {
   return splat_forward_impl(H, W, N, us, cinv2ds, alphas, depths, colors, areas, packed_records, P_cap, depth_key_cap,
                             bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
-                            gsid_per_patch, status_host, stream, false);
+                            gsid_per_patch, status_host, nullptr, nullptr, stream, false);
 }
 
 // (a ws at any address: the size is the split from the worst start, 255 bytes short of a 256-B boundary)
 size_t gsb_splat_backward_workspace_bytes(int N, int H, int W, int64_t P) { return bwd_layout(N, H, W, P, 1).bytes; }
 
-int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
-                       const float *alphas, const float *colors, const int32_t *contrib,
-                       const float *final_tau, const int32_t *patch_range_per_tile,
-                       const int32_t *gsid_per_patch, const float *dloss_dgammas,
-                       const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus, float *dloss_dcinv2ds, float *dloss_dalphas,
-                       float *dloss_dcolors, float *moments_out, gsb_stream_t stream) {
+// gsb_splat_backward and, with dg, its RGB-D form (depths: the re-pack's depth words)
+static int splat_backward_impl(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                               const float *alphas, const float *colors, const float *depths, const int32_t *contrib,
+                               const float *final_tau, const int32_t *patch_range_per_tile,
+                               const int32_t *gsid_per_patch, const float *dloss_dgammas, const DepthGrads *dg,
+                               const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
+                               float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
+                               gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splatB: bad N/H/W/P");
   GSB_REQUIRE(N == 0 || moments_out || (dloss_dus && dloss_dcinv2ds && dloss_dalphas && dloss_dcolors),
               "splatB: null output");
@@ -412,18 +480,47 @@ int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const fl
     GSB_REQUIRE(us && alphas && colors && contrib && final_tau && patch_range_per_tile && gsid_per_patch &&
                     dloss_dgammas,
                 "splatB: null pointer");
+    GSB_REQUIRE(dg == nullptr || (depths && dg->dloss_ddepth_image && dg->dloss_dalpha_image),
+                "splatB_rgbd: null pointer");
     if (packed_records != nullptr) {  // the forward's record stream is still valid: skip the re-pack
       GSB_REQUIRE(aligned(packed_records, 16), "splatB: packed_records misaligned");
       recs = const_cast<Rec *>(static_cast<const Rec *>(packed_records));
     } else {
-      int rc = launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, recs, st);
+      int rc = launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, depths, recs, st);
       if (rc) return rc;
     }
   }
   // P == 0: nothing was drawn; the zeroed moment rows finalise to all-zero gradients
   return launch_draw_backward(H, W, N, patch_range_per_tile, P > 0 ? recs : nullptr, gsid_per_patch, contrib, final_tau,
-                              dloss_dgammas, cinv2ds, moments, work, dloss_dus, dloss_dcinv2ds, dloss_dalphas,
+                              dloss_dgammas, dg, cinv2ds, moments, work, dloss_dus, dloss_dcinv2ds, dloss_dalphas,
                               dloss_dcolors, moments_out == nullptr, st);
+}
+
+int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                       const float *alphas, const float *colors, const int32_t *contrib,
+                       const float *final_tau, const int32_t *patch_range_per_tile,
+                       const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                       const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus, float *dloss_dcinv2ds, float *dloss_dalphas,
+                       float *dloss_dcolors, float *moments_out, gsb_stream_t stream) {
+  // (the re-pack leaves the records' depth word 0: k_draw_bwd never reads it)
+  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
+                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws,
+                             ws_bytes, dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, stream);
+}
+
+int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                            const float *alphas, const float *colors, const float *depths, const int32_t *contrib,
+                            const float *final_tau, const int32_t *patch_range_per_tile,
+                            const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                            const float *dloss_ddepth_image, const float *dloss_dalpha_image,
+                            const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
+                            float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
+                            float *dloss_ddepths, gsb_stream_t stream) {
+  GSB_REQUIRE(N <= 0 || dloss_ddepths != nullptr, "splatB_rgbd: null dloss_ddepths");
+  const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
+  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
+                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
+                             dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, stream);
 }
 
 // ---- density control + record conversion (density.cu)
@@ -597,7 +694,7 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, nullptr};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, nullptr, nullptr, nullptr, &gp,
-                               moments ? &mi : nullptr, (cudaStream_t)stream);
+                               moments ? &mi : nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *const *regions_host, uint32_t epoch,

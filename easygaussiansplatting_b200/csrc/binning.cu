@@ -528,19 +528,22 @@ __global__ void __launch_bounds__(256) k_ranges(const uint32_t *__restrict__ P_d
 }
 
 // Gathers the four per-Gaussian attribute arrays (all L2 resident: 36 B/Gaussian) into the
-// 48-B records the rasterizers gather with cp.async (gsid == nullptr: one record per Gaussian).
+// 48-B records the rasterizers gather with cp.async (gsid == nullptr: one record per Gaussian);
+// the depth word is depths[g], or 0 when depths is NULL (only the RGB-D rasterizers read it).
 __global__ void __launch_bounds__(256) k_pack(int64_t P, const int32_t *__restrict__ gsid,
                                               const float *__restrict__ us,
                                               const float *__restrict__ cinv2ds,
                                               const float *__restrict__ alphas,
-                                              const float *__restrict__ colors, Rec *__restrict__ recs) {
+                                              const float *__restrict__ colors,
+                                              const float *__restrict__ depths, Rec *__restrict__ recs) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
   const int g = gsid != nullptr ? __ldg(gsid + p) : (int)p;  // nullptr: one record per Gaussian
   const float2 u = ld_pair(us, g);
   recs[p] = build_record(u.x, u.y, __ldg(cinv2ds + 3 * (size_t)g), __ldg(cinv2ds + 3 * (size_t)g + 1),
                          __ldg(cinv2ds + 3 * (size_t)g + 2), __ldg(alphas + g), __ldg(colors + 3 * (size_t)g),
-                         __ldg(colors + 3 * (size_t)g + 1), __ldg(colors + 3 * (size_t)g + 2), g);
+                         __ldg(colors + 3 * (size_t)g + 1), __ldg(colors + 3 * (size_t)g + 2),
+                         depths != nullptr ? __ldg(depths + g) : 0.0f, g);
 }
 
 // ---------------------------------------------------------------- phase 1 host side
@@ -608,10 +611,10 @@ BwdLayout bwd_layout(int N, int H, int W, int64_t P, uintptr_t base) {
 }
 
 int launch_pack_only(int64_t P, const int32_t *gsid_per_patch, const float *us, const float *cinv2ds,
-                     const float *alphas, const float *colors, Rec *recs, cudaStream_t st) {
+                     const float *alphas, const float *colors, const float *depths, Rec *recs, cudaStream_t st) {
   if (P <= 0) return 0;
   ProfScope ps(K_PACK, st);
-  k_pack<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(P, gsid_per_patch, us, cinv2ds, alphas, colors, recs);
+  k_pack<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(P, gsid_per_patch, us, cinv2ds, alphas, colors, depths, recs);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -722,7 +725,7 @@ int launch_sort_and_pack(int H, int W, int N, int64_t P, uint32_t depth_key_max,
                      : keys_sort_ranges<uint64_t>(N, P, depths, incl, rects, total, gx, gx * gy, kp, b, SL, ranges,
                                                   gsid_per_patch, sr, st);
   if (rc || !pack) return rc;  // !pack: the caller already holds the per-Gaussian records
-  return launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, reinterpret_cast<Rec *>(b + SL.recs), st);
+  return launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, depths, reinterpret_cast<Rec *>(b + SL.recs), st);
 }
 
 }  // namespace gsb

@@ -24,7 +24,8 @@ constexpr float LOG2E = 1.4426950408889634f;
 //                              -0.5*log2e, -log2e, -0.5*log2e); thr = log2(alpha / 0.002) (+margin):
 //                              a pixel can reach alpha' >= 0.002 only where -log2(g) <= thr
 //                              (+inf: never cull, -inf: never contributes)
-//   q2 = (r, g, b, 0)
+//   q2 = (r, g, b, z)          colour; camera-frame depth (the `depths` value), read only by the
+//                              RGB-D rasterizers (k_draw_rgbd, k_draw_bwd_rgbd)
 struct __align__(16) Rec {
   float4 q0, q1, q2;
 };
@@ -104,7 +105,7 @@ __device__ __forceinline__ bool rec_can_touch(const float4 &q0, const float4 &q1
 // warp-level culling test (rec_can_touch); the positive-definiteness check carries a safety
 // factor against fp32 cancellation in A C - B^2.
 __device__ __forceinline__ Rec build_record(float ux, float uy, float A, float B, float C, float al, float cr,
-                                            float cg, float cb, int id) {
+                                            float cg, float cb, float z, int id) {
   float thr = INFINITY;  // never cull unless the conic is a proper positive definite form
   if (al < ALPHA_SKIP) {
     thr = -INFINITY;  // alpha * g < 0.002 everywhere: never contributes
@@ -119,7 +120,7 @@ __device__ __forceinline__ Rec build_record(float ux, float uy, float A, float B
   Rec r;
   r.q0 = make_float4(ux, uy, __int_as_float(id), al);
   r.q1 = make_float4(-0.5f * LOG2E * A, -LOG2E * B, -0.5f * LOG2E * C, thr);
-  r.q2 = make_float4(cr, cg, cb, 0.f);
+  r.q2 = make_float4(cr, cg, cb, z);
   return r;
 }
 

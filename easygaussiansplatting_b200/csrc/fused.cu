@@ -78,7 +78,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
     depths[i] = depth;
     // the rasterizers' per-Gaussian record, straight from registers (saves the k_pack pass)
     if (recs != nullptr)
-      recs[i] = build_record(u[0], u[1], conic[0], conic[1], conic[2], __ldg(alphas + i), col[0], col[1], col[2], (int)i);
+      recs[i] = build_record(u[0], u[1], conic[0], conic[1], conic[2], __ldg(alphas + i), col[0], col[1], col[2], depth,
+                             (int)i);
   }
 }
 
@@ -93,14 +94,15 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
 // dL/dconic = (-Sxx/2, -Sxy, -Syy/2), dL/dcolor, dL/dalpha) happens here in registers, dL/du and
 // dL/dalpha are still written out (the caller's densification statistics / alpha gradient), and
 // the separate finalize pass with its 36 B/Gaussian round trip disappears.
-template <int K3, bool PUSH, bool MOM>
+// DEPTH = the RGB-D rasterizer's dL/dz[N] (g_depths) is a fourth upstream gradient (not with PUSH).
+template <int K3, bool PUSH, bool MOM, bool DEPTH>
 __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
     const float *__restrict__ shs, const float *__restrict__ Rcw, const float *__restrict__ tcw,
     const float *__restrict__ twc, float fx, float fy, float cx, float cy, float tan_fovx, float tan_fovy,
     const float *__restrict__ g_us, const float *__restrict__ g_cinv2ds, const float *__restrict__ g_colors,
     float *__restrict__ g_pws, float *__restrict__ g_shs, float *__restrict__ g_scales,
-    float *__restrict__ g_rots, GradPush gp, MomentsIn mi) {
+    float *__restrict__ g_rots, GradPush gp, MomentsIn mi, const float *__restrict__ g_depths) {
   constexpr int KS = 3 * K3;
   constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
   __shared__ float sm[SMF];
@@ -141,7 +143,12 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   __syncthreads();
   float gpw[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f};
   // dL/dsh overwrites the thread's own SH row in place, then the tile is flushed
-  if (valid) pg::backward_one<K3>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS));
+  if (DEPTH) {
+    const float gz = valid ? __ldg(g_depths + base + tid) : 0.f;
+    if (valid) pg::backward_one<K3, true>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), gz);
+  } else if (valid) {
+    pg::backward_one<K3>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS));
+  }
   __syncthreads();
   long long drow = base;
   if (PUSH) {  // destination = slot `rank` on the owner of this tile, rows relative to its range
@@ -271,25 +278,32 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          cudaStream_t st) {
+                          const float *g_depths, cudaStream_t st) {
   if (N <= 0) return 0;
+  if (g_depths != nullptr && gp != nullptr) return set_arg_error("preprocessB: no depth gradient with the exchange");
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = (N + PG - 1) / PG;
   const GradPush p = gp ? *gp : GradPush{};
   const MomentsIn m = mi ? *mi : MomentsIn{};
   ProfScope ps(K_PRE_BWD, st);
-#define GSB_PRE_BWD(PUSH, MOM)                                                                                  \
-  GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM><<<nb, PG, 0, st>>>(                                      \
+#define GSB_PRE_BWD(PUSH, MOM, DEPTH)                                                                           \
+  GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH><<<nb, PG, 0, st>>>(                               \
                           N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us, g_cinv2ds, \
-                          g_colors, g_pws, g_shs, g_scales, g_rots, p, m)))
+                          g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths)))
   if (gp != nullptr && mi != nullptr) {
-    GSB_PRE_BWD(true, true);
+    GSB_PRE_BWD(true, true, false);
   } else if (gp != nullptr) {
-    GSB_PRE_BWD(true, false);
+    GSB_PRE_BWD(true, false, false);
   } else if (mi != nullptr) {
-    GSB_PRE_BWD(false, true);
+    if (g_depths != nullptr) {
+      GSB_PRE_BWD(false, true, true);
+    } else {
+      GSB_PRE_BWD(false, true, false);
+    }
+  } else if (g_depths != nullptr) {
+    GSB_PRE_BWD(false, false, true);
   } else {
-    GSB_PRE_BWD(false, false);
+    GSB_PRE_BWD(false, false, false);
   }
 #undef GSB_PRE_BWD
   GSB_CUDA_TRY(cudaGetLastError());

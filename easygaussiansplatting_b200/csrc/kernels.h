@@ -15,7 +15,7 @@ enum KernelId {
   K_PROJECT = 0, K_COV3D, K_COV2D, K_SH2COLOR, K_INVCOV, K_RECTS, K_SCAN, K_KEYS, K_SORT, K_RANGES,
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
-  K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_COUNT
+  K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -54,13 +54,14 @@ struct MomentsIn {
 struct GradPush;
 // gp == nullptr: the gradients go to g_pws, g_shs, g_scales, g_rots; otherwise into the exchange
 // staging slots gp describes (the g_* outputs are unused).  mi == nullptr: the upstream gradients
-// are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.
+// are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.  g_depths: NULL, or dL/dz[N]
+// of the RGB-D rasterizer (not with gp).
 int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          cudaStream_t st);
+                          const float *g_depths, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,
@@ -156,20 +157,32 @@ int launch_sort_and_pack(int H, int W, int N, int64_t P, uint32_t depth_key_max,
                          const void *bin_ws, const BinLayout &BL, void *ws, const SortLayout &SL,
                          int32_t *ranges, int32_t *gsid_per_patch, bool pack, const StatusRead *sr,
                          cudaStream_t st);
+// depths: nullable; the records' depth word (q2.w) is 0 without them
 int launch_pack_only(int64_t P, const int32_t *gsid_per_patch, const float *us, const float *cinv2ds,
-                     const float *alphas, const float *colors, Rec *recs, cudaStream_t st);
+                     const float *alphas, const float *colors, const float *depths, Rec *recs, cudaStream_t st);
 
 // ---- rasterizer (raster_fwd.cu, raster_bwd.cu).  recs: one 48-byte record per Gaussian; gsid: the
 // sorted patch list -- the kernels gather records through it.  work = [item counter, #entries,
 // entries ...] (2 + 4 * tiles ints, see k_tile_list); with outputs given the empty tiles are
 // zero-filled there.
+// depth_image / alpha_image: both NULL (colour frame), or the RGB-D frame's D and A planes [H,W]
+// (k_draw_rgbd; the records' depth word must hold z).
 int launch_tile_list(int H, int W, const int32_t *ranges, float *image, int32_t *contrib, float *final_tau,
-                     int *work, cudaStream_t st);
+                     float *depth_image, float *alpha_image, int *work, cudaStream_t st);
 int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int32_t *gsid, float *image,
-                int32_t *contrib, float *final_tau, int *work, cudaStream_t st);
+                int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, int *work,
+                cudaStream_t st);
+// the RGB-D backward's extra upstream planes [H,W] and its dL/dz output [N] (zeroed here)
+struct DepthGrads {
+  const float *dloss_ddepth_image;
+  const float *dloss_dalpha_image;
+  float *ddepths;
+};
+// dg == nullptr: k_draw_bwd; otherwise k_draw_bwd_rgbd
 int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
                          const int32_t *contrib, const float *final_tau, const float *dloss_dgammas,
-                         const float *cinv2ds, float *moments, int *work, float *dloss_dus, float *dloss_dcinv2ds,
-                         float *dloss_dalphas, float *dloss_dcolors, bool finalize, cudaStream_t st);
+                         const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
+                         float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
+                         cudaStream_t st);
 
 }  // namespace gsb

@@ -1,5 +1,5 @@
 // Per-Gaussian math, shared by the operator kernels (pergaussian.cu), the fused kernels
-// (fused.cu) and a host build used only by tests (tests/host_shim/fused_host.cpp) -- hence
+// (fused.cu) and host builds used only by tests (tests/host_shim/) -- hence
 // host+device, no CUDA-only intrinsics.  Each formula is stated once, as a stage function
 // (camera_point, project_mean, cov3d, cov2d, conic, radius, view_dir, sh_basis); the operator
 // kernels call the stages one by one and add their Jacobians, the fused path composes them:
@@ -211,11 +211,12 @@ GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], c
 }
 
 // backward for one Gaussian.  gu[2], gconic[3], gcol[3] are the splatB outputs for it.
-// gsh may alias sh (row-private in-place update).
-template <int K3>
+// gsh may alias sh (row-private in-place update).  DEPTH: gdepth = dL/dz from the RGB-D
+// rasterizer; z = pc[2], so it adds to dL/dpc[2] and reaches dL/dpw through Rcw[2,:].
+template <int K3, bool DEPTH = false>
 GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], const float *sh,
                          const Cam &cam, const float gu[2], const float gconic[3], const float gcol[3],
-                         float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/) {
+                         float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f) {
   // ---- colour branch (independent of the depth cull, like sh2Color)
   float Y[K3], dY[K3][3];
   float d[3], ninv = 1.f, r[3] = {0.f, 0.f, 0.f};
@@ -244,7 +245,8 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
   // ---- geometry branch
   Geo g;
   geometry(pw, q, s, cam, g);
-  const bool any = (gu[0] != 0.f) || (gu[1] != 0.f) || (gconic[0] != 0.f) || (gconic[1] != 0.f) || (gconic[2] != 0.f);
+  const bool any = (gu[0] != 0.f) || (gu[1] != 0.f) || (gconic[0] != 0.f) || (gconic[1] != 0.f) || (gconic[2] != 0.f) ||
+                   (DEPTH && gdepth != 0.f);
   if (!g.keep || !any) return;
   const float a = g.c2[0], b = g.c2[1], c = g.c2[2], di = g.di, d2 = di * di;
   // dL/dcov2d = dL/dconic . dconic/dcov2d   (B.5.3)
@@ -291,6 +293,7 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
   gpc[0] += gu[0] * (cam.fx * zi);
   gpc[1] += gu[1] * (cam.fy * zi);
   gpc[2] += -(gu[0] * (g.pc[0] * cam.fx) + gu[1] * (g.pc[1] * cam.fy)) * zi2;
+  if (DEPTH) gpc[2] += gdepth;  // depth z = pc[2]
   for (int j = 0; j < 3; j++) gpw[j] += gpc[0] * R[j] + gpc[1] * R[3 + j] + gpc[2] * R[6 + j];
   // cov3d: dL/dM3 = 2 sym(g3) M3
   const float G3[9] = {g3[0], 0.5f * g3[1], 0.5f * g3[2], 0.5f * g3[1], g3[3], 0.5f * g3[4],

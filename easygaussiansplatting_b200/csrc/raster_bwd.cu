@@ -39,6 +39,9 @@ constexpr int BWD_CHUNK_BYTES = 32 * 48;
 #ifndef DRAW_BWD_MINBLOCKS
 #define DRAW_BWD_MINBLOCKS 6
 #endif
+#ifndef DRAW_BWD_RGBD_MINBLOCKS
+#define DRAW_BWD_RGBD_MINBLOCKS 5
+#endif
 
 namespace {
 __device__ __forceinline__ void sts64(uint32_t a, float2 v) {
@@ -52,8 +55,12 @@ __device__ __forceinline__ float2 hi(const float4 &v) { return make_float2(v.z, 
 //   inf = record word q0 = (u_x, u_y, gaussian id, alpha) of the lane's slot.  It travels in registers:
 //   shared-memory wavefronts are this kernel's scarcest resource, and a 16-byte shared store
 //   costs 4 of them even from one lane (benchmarks/micro/redux_bench.cu).
+//   RGBD: a tenth sum, wc dL/dD = dL/dz, over a fourth dL/d-plane at dl_addr + 768; it goes to
+//   ddepths[id] from the part-3 lane (which carries only one other reduction).
+template <bool RGBD>
 __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, uint32_t dl_addr, int nslots,
-                                          float fbx0, float fby0, float *__restrict__ moments, int lane) {
+                                          float fbx0, float fby0, float *__restrict__ moments,
+                                          float *__restrict__ ddepths, int lane) {
   const int slot = lane >> 2, part = lane & 3;
   const float U = inf.x - (fbx0 + (float)((part & 1) * 4));
   const float V = inf.y - (fby0 + (float)(part >> 1));
@@ -61,7 +68,7 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
   const uint32_t a = w_addr + slot * BWD_SLOT_BYTES + part * 16;
   const uint32_t d = dl_addr + part * 16;
   float2 m0 = p2s(0.f), m1 = p2s(0.f), m2 = p2s(0.f), m3 = p2s(0.f), m4 = p2s(0.f), m5 = p2s(0.f),
-         m6 = p2s(0.f), m7 = p2s(0.f), m8 = p2s(0.f);
+         m6 = p2s(0.f), m7 = p2s(0.f), m8 = p2s(0.f), m9 = p2s(0.f);
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     const float dy = V - (float)(2 * j);
@@ -86,6 +93,11 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
     m7 = fma2_rn(hi(wc), hi(dg), m7);
     m8 = fma2_rn(lo(wc), lo(db), m8);
     m8 = fma2_rn(hi(wc), hi(db), m8);
+    if (RGBD) {
+      const float4 dd = lds128(d + 768 + j * 64);
+      m9 = fma2_rn(lo(wc), lo(dd), m9);
+      m9 = fma2_rn(hi(wc), hi(dd), m9);
+    }
   }
   // sum dL/dalpha' g = (sum w) / alpha; records above the clamp were reduced in phase A
   const float inv_alpha = inf.w <= ALPHA_CLAMP ? __fdividef(1.0f, inf.w) : 0.0f;
@@ -108,6 +120,12 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
     atomicAdd(row, b[0]);
     if (part != 3) atomicAdd(row + 1, b[1]);
     if (!u2) atomicAdd(row + 2, b[2]);
+  }
+  if (RGBD) {
+    float z = m9.x + m9.y;
+    z += __shfl_xor_sync(F, z, 1);
+    z += __shfl_xor_sync(F, z, 2);
+    if (slot < nslots && part == 3) atomicAdd(ddepths + __float_as_int(inf.z), z);
   }
 }
 
@@ -137,13 +155,21 @@ __device__ __forceinline__ BwdEval bwd_eval(const float4 &q0, const float4 &q1, 
 }
 }  // namespace
 
-__global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
+// The backward's body, shared by k_draw_bwd and k_draw_bwd_rgbd.  RGBD: the upstream gradient of a
+// pixel also has dL/dD and dL/dA, so in phase A dL/dalpha' gains (dL/dD z + dL/dA) next to
+// dL/dgamma . c (the sdot recurrence carries the sum of all five channels), and phase B sums
+// wc dL/dD into dL/dz from a fourth per-pixel table.  dL/dA needs no table: opacity has no
+// per-Gaussian value to differentiate.
+template <bool RGBD>
+__device__ __forceinline__ void draw_bwd_body(
     int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
-    const float *__restrict__ dloss_dgammas, float *__restrict__ moments, int *__restrict__ work) {
+    const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
+    const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
+    int *__restrict__ work) {
   __shared__ __align__(16) unsigned char s_ring[4][BWD_RING * BWD_CHUNK_BYTES];  // gathered records, per warp
   __shared__ __align__(16) unsigned char s_w[4][BWD_W_BYTES];                   // weight rows, per warp
-  __shared__ __align__(16) float s_dl[4][3][64];                               // dL/dgamma of the block
+  __shared__ __align__(16) float s_dl[4][RGBD ? 4 : 3][64];                    // dL/dgamma (dL/dD) of the block
   __shared__ __align__(16) uint2 s_list[4][34];  // (record address, patch index) of a chunk's survivors
   __shared__ __align__(16) Rec s_dummy;          // all-zero record: pads an odd survivor count
 
@@ -206,6 +232,11 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
 
     int cont0 = 0, cont1 = 0;
     float2 tau = p2s(0.f), dlr = p2s(0.f), dlg = p2s(0.f), dlb = p2s(0.f);
+    float2 dld = p2s(0.f), dla = p2s(0.f);  // RGBD only: dL/dD, dL/dA
+    if (RGBD) {
+      if (in0) { dld.x = __ldg(dloss_ddepth_image + pix); dla.x = __ldg(dloss_dalpha_image + pix); }
+      if (in1) { dld.y = __ldg(dloss_ddepth_image + pix + 1); dla.y = __ldg(dloss_dalpha_image + pix + 1); }
+    }
     if (in0) {
       cont0 = min(__ldg(contrib + pix), len);
       tau.x = __ldg(final_tau + pix);
@@ -229,6 +260,7 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
     sts64(dl_addr + lane * 8, dlr);
     sts64(dl_addr + 256 + lane * 8, dlg);
     sts64(dl_addr + 512 + lane * 8, dlb);
+    if (RGBD) sts64(dl_addr + 768 + lane * 8, dld);
 
     const int nch = (wmax + 31) >> 5;  // chunks [0, nch) hold the records any pixel replays
     const int32_t *ids = gsid + range.x;
@@ -276,7 +308,7 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
       for (int i = 0; i < n; i += 2) {
         if (wa > wa_pair_limit) {  // no room for a pair
           __syncwarp();
-          bwd_flush(w_addr, inf, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, lane);
+          bwd_flush<RGBD>(w_addr, inf, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, ddepths, lane);
           __syncwarp();
           wa = w_addr + lane * 8;
           to_my_slot = lane >> 2;
@@ -287,8 +319,14 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
         const float4 q2a = lds128(ent.x + 32), q2b = lds128(ent.z + 32);
         const BwdEval A = bwd_eval(q0a, q1a, npx, fpy, (int)ent.y, cont0, cont1);
         const BwdEval B = bwd_eval(q0b, q1b, npx, fpy, (int)ent.w, cont0, cont1);
-        const float2 dca = fma2_rn(dlr, p2s(q2a.x), fma2_rn(dlg, p2s(q2a.y), mul2_rn(dlb, p2s(q2a.z))));
-        const float2 dcb = fma2_rn(dlr, p2s(q2b.x), fma2_rn(dlg, p2s(q2b.y), mul2_rn(dlb, p2s(q2b.z))));
+        float2 dca, dcb;
+        if (RGBD) {  // dL/dgamma . c + dL/dD z + dL/dA
+          dca = fma2_rn(dlr, p2s(q2a.x), fma2_rn(dlg, p2s(q2a.y), fma2_rn(dlb, p2s(q2a.z), fma2_rn(dld, p2s(q2a.w), dla))));
+          dcb = fma2_rn(dlr, p2s(q2b.x), fma2_rn(dlg, p2s(q2b.y), fma2_rn(dlb, p2s(q2b.z), fma2_rn(dld, p2s(q2b.w), dla))));
+        } else {
+          dca = fma2_rn(dlr, p2s(q2a.x), fma2_rn(dlg, p2s(q2a.y), mul2_rn(dlb, p2s(q2a.z))));
+          dcb = fma2_rn(dlr, p2s(q2b.x), fma2_rn(dlg, p2s(q2b.y), mul2_rn(dlb, p2s(q2b.z))));
+        }
         // first record
         tau = mul2_rn(tau, A.rc);
         const float2 diffa = add2_rn(dca, p2(-sdot.x, -sdot.y));
@@ -328,10 +366,28 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
     cp_async_wait<0>();
     if (wa != w_addr + lane * 8) {
       __syncwarp();
-      bwd_flush(w_addr, inf, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, lane);
+      bwd_flush<RGBD>(w_addr, inf, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, ddepths, lane);
     }
     __syncwarp();  // the flush has read s_dl / s_w before the next block rewrites them
   }
+}
+
+__global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
+    int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    const float *__restrict__ dloss_dgammas, float *__restrict__ moments, int *__restrict__ work) {
+  draw_bwd_body<false>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr, moments,
+                       nullptr, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_BWD_RGBD_MINBLOCKS) k_draw_bwd_rgbd(
+    int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
+    const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
+    int *__restrict__ work) {
+  draw_bwd_body<true>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
+                      dloss_dalpha_image, moments, ddepths, work);
 }
 
 constexpr int MOM = 9;  // floats per moment row
@@ -378,24 +434,35 @@ __global__ void __launch_bounds__(PG) k_finalize_grads(int N, const float *__res
 
 int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
                          const int32_t *contrib, const float *final_tau, const float *dloss_dgammas,
-                         const float *cinv2ds, float *moments, int *work, float *dloss_dus, float *dloss_dcinv2ds,
-                         float *dloss_dalphas, float *dloss_dcolors, bool finalize, cudaStream_t st) {
+                         const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
+                         float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
+                         cudaStream_t st) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0 || N <= 0) return 0;
   GSB_CUDA_TRY(cudaMemsetAsync(moments, 0, sizeof(float) * MOM * (size_t)N, st));
+  if (dg != nullptr) GSB_CUDA_TRY(cudaMemsetAsync(dg->ddepths, 0, sizeof(float) * (size_t)N, st));
   if (recs != nullptr) {
     const int T = gx * gy;
     if (work == nullptr) return set_arg_error("drawB: work area missing");
-    int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, work, st);  // tiles with patches
+    int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);  // tiles with patches
     if (rc) return rc;
     int dev = 0, sms = 132;
     GSB_CUDA_TRY(cudaGetDevice(&dev));
     GSB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const long long want = (long long)sms * DRAW_BWD_MINBLOCKS;
-    const int grid = (int)(T < want ? T : want);
-    ProfScope ps(K_DRAW_BWD, st);
-    k_draw_bwd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib,
-                                     final_tau, dloss_dgammas, moments, work);
+    if (dg != nullptr) {
+      const long long want = (long long)sms * DRAW_BWD_RGBD_MINBLOCKS;
+      const int grid = (int)(T < want ? T : want);
+      ProfScope ps(K_DRAW_BWD_RGBD, st);
+      k_draw_bwd_rgbd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
+                                            dg->dloss_ddepth_image, dg->dloss_dalpha_image, moments, dg->ddepths,
+                                            work);
+    } else {
+      const long long want = (long long)sms * DRAW_BWD_MINBLOCKS;
+      const int grid = (int)(T < want ? T : want);
+      ProfScope ps(K_DRAW_BWD, st);
+      k_draw_bwd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib,
+                                       final_tau, dloss_dgammas, moments, work);
+    }
     GSB_CUDA_TRY(cudaGetLastError());
   }
   if (finalize) {  // otherwise the caller consumes the moment rows (gsb_preprocess_backward)

@@ -49,7 +49,8 @@ __device__ __forceinline__ float2 fwd_alpha(const float4 &q0, const float4 &q1, 
 // frame instead of one queue item per 8x8 block.
 __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, const int32_t *__restrict__ ranges,
                                                    float *__restrict__ image, int32_t *__restrict__ contrib,
-                                                   float *__restrict__ final_tau, int *__restrict__ work) {
+                                                   float *__restrict__ final_tau, float *__restrict__ depth_image,
+                                                   float *__restrict__ alpha_image, int *__restrict__ work) {
   __shared__ unsigned s_empty[8];  // per warp: which of its 32 tiles have no patches
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int tile = blockIdx.x * 256 + threadIdx.x;  // phase 1: one thread per tile
@@ -101,12 +102,17 @@ __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, 
           *reinterpret_cast<float4 *>(image + 2 * HW + pix + 4 * h) = z;
           *reinterpret_cast<int4 *>(contrib + pix + 4 * h) = make_int4(0, 0, 0, 0);
           *reinterpret_cast<float4 *>(final_tau + pix + 4 * h) = z;
+          if (depth_image != nullptr) {  // (the RGB-D frame's D and A planes: zero too)
+            *reinterpret_cast<float4 *>(depth_image + pix + 4 * h) = z;
+            *reinterpret_cast<float4 *>(alpha_image + pix + 4 * h) = z;
+          }
         }
       } else {
         for (int x = x0; x < min(x0 + 8, W); x++) {
           const size_t q = (size_t)y * W + x;
           image[q] = 0.f; image[HW + q] = 0.f; image[2 * HW + q] = 0.f;
           contrib[q] = 0; final_tau[q] = 0.f;
+          if (depth_image != nullptr) { depth_image[q] = 0.f; alpha_image[q] = 0.f; }
         }
       }
     }
@@ -114,24 +120,26 @@ __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, 
 }
 
 int launch_tile_list(int H, int W, const int32_t *ranges, float *image, int32_t *contrib, float *final_tau,
-                     int *work, cudaStream_t st) {
+                     float *depth_image, float *alpha_image, int *work, cudaStream_t st) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   const int T = gx * gy;
   GSB_CUDA_TRY(cudaMemsetAsync(work, 0, 2 * sizeof(int), st));
   k_tile_list<<<(T + 255) / 256, 256, 0, st>>>(W, H, gx, T, ranges, image, contrib,
-                                           final_tau, work);
+                                           final_tau, depth_image, alpha_image, work);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
-__global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int gx, int T,
-                                                              const int2 *__restrict__ ranges,
-                                                              const Rec *__restrict__ recs,
-                                                              const int32_t *__restrict__ gsid,
-                                                              float *__restrict__ image,
-                                                              int32_t *__restrict__ contrib,
-                                                              float *__restrict__ final_tau,
-                                                              int *__restrict__ work) {
+// The rasterizer's body, shared by the colour kernel (k_draw) and the RGB-D kernel (k_draw_rgbd).
+// RGBD: depth and opacity composite like two more colour channels whose per-record values are
+// z = q2.w and 1 -- D = sum w z, A = sum w with the image's weights w = tau alpha' -- two more
+// pair accumulators and two more [H,W] planes.
+template <bool RGBD>
+__device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int2 *__restrict__ ranges,
+                                          const Rec *__restrict__ recs, const int32_t *__restrict__ gsid,
+                                          float *__restrict__ image, int32_t *__restrict__ contrib,
+                                          float *__restrict__ final_tau, float *__restrict__ depth_image,
+                                          float *__restrict__ alpha_image, int *__restrict__ work) {
   __shared__ __align__(16) unsigned char s_ring[4][FWD_RING * FWD_CHUNK_BYTES];  // gathered records, per warp
   __shared__ __align__(16) uint2 s_list[4][34];  // (record address, patch index + 1) of a chunk's survivors
   __shared__ __align__(16) Rec s_dummy;          // all-zero record (alpha = 0): pads an odd survivor count
@@ -178,6 +186,7 @@ __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int 
     const size_t pix = (size_t)py * W + px;
 
     float2 tau = p2s(0.f), cr = p2s(0.f), cg = p2s(0.f), cb = p2s(0.f);
+    float2 cd = p2s(0.f), ca = p2s(0.f);  // RGBD only: D and A
     int cont0 = 0, cont1 = 0;
     if (len > 0) {  // (a tile without patches keeps image 0, contrib 0, tau 0: kernel.cu:182-183)
       const int nch = (len + 31) >> 5;
@@ -233,6 +242,10 @@ __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int 
             cr = fma2_rn(w, p2s(q2a.x), cr);
             cg = fma2_rn(w, p2s(q2a.y), cg);
             cb = fma2_rn(w, p2s(q2a.z), cb);
+            if (RGBD) {
+              cd = fma2_rn(w, p2s(q2a.w), cd);
+              ca = add2_rn(ca, w);
+            }
             tau = mul2_rn(tau, add2_rn(p2s(1.0f), p2(-e.x, -e.y)));
             if (c0) cont0 = (int)ent.y;
             if (c1) cont1 = (int)ent.y;
@@ -245,6 +258,10 @@ __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int 
             cr = fma2_rn(w, p2s(q2b.x), cr);
             cg = fma2_rn(w, p2s(q2b.y), cg);
             cb = fma2_rn(w, p2s(q2b.z), cb);
+            if (RGBD) {
+              cd = fma2_rn(w, p2s(q2b.w), cd);
+              ca = add2_rn(ca, w);
+            }
             tau = mul2_rn(tau, add2_rn(p2s(1.0f), p2(-e.x, -e.y)));
             if (c0) cont0 = (int)ent.w;
             if (c1) cont1 = (int)ent.w;
@@ -266,22 +283,53 @@ __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int 
       *reinterpret_cast<float2 *>(image + 2 * HW + pix) = cb;
       *reinterpret_cast<int2 *>(contrib + pix) = make_int2(cont0, cont1);
       *reinterpret_cast<float2 *>(final_tau + pix) = tau;
+      if (RGBD) {
+        *reinterpret_cast<float2 *>(depth_image + pix) = cd;
+        *reinterpret_cast<float2 *>(alpha_image + pix) = ca;
+      }
     } else {
       if (in0) {
         image[pix] = cr.x; image[HW + pix] = cg.x; image[2 * HW + pix] = cb.x;
         contrib[pix] = cont0; final_tau[pix] = tau.x;
+        if (RGBD) { depth_image[pix] = cd.x; alpha_image[pix] = ca.x; }
       }
       if (in1) {
         image[pix + 1] = cr.y; image[HW + pix + 1] = cg.y; image[2 * HW + pix + 1] = cb.y;
         contrib[pix + 1] = cont1; final_tau[pix + 1] = tau.y;
+        if (RGBD) { depth_image[pix + 1] = cd.y; alpha_image[pix + 1] = ca.y; }
       }
     }
    }  // blocks of the entry
   }
 }
 
+__global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int gx, int T,
+                                                              const int2 *__restrict__ ranges,
+                                                              const Rec *__restrict__ recs,
+                                                              const int32_t *__restrict__ gsid,
+                                                              float *__restrict__ image,
+                                                              int32_t *__restrict__ contrib,
+                                                              float *__restrict__ final_tau,
+                                                              int *__restrict__ work) {
+  draw_body<false>(W, H, gx, T, ranges, recs, gsid, image, contrib, final_tau, nullptr, nullptr, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw_rgbd(int W, int H, int gx, int T,
+                                                                   const int2 *__restrict__ ranges,
+                                                                   const Rec *__restrict__ recs,
+                                                                   const int32_t *__restrict__ gsid,
+                                                                   float *__restrict__ image,
+                                                                   int32_t *__restrict__ contrib,
+                                                                   float *__restrict__ final_tau,
+                                                                   float *__restrict__ depth_image,
+                                                                   float *__restrict__ alpha_image,
+                                                                   int *__restrict__ work) {
+  draw_body<true>(W, H, gx, T, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image, work);
+}
+
 int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int32_t *gsid, float *image,
-                int32_t *contrib, float *final_tau, int *work, cudaStream_t st) {
+                int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, int *work,
+                cudaStream_t st) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0) return 0;
   const int T = gx * gy;
@@ -289,16 +337,22 @@ int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int3
   // (k_draw reads `ranges` as int2: the splat entry points only accept an 8-byte aligned
   // patch_range_per_tile, which the binning just wrote)
   // work list (and the zeros of the empty tiles) first; it also clears the item counter
-  int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, work, st);
+  int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st);
   if (rc) return rc;
   int dev = 0, sms = 132;
   GSB_CUDA_TRY(cudaGetDevice(&dev));
   GSB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long want = (long long)sms * DRAW_MINBLOCKS;
   const int grid = (int)(T < want ? T : want);
-  ProfScope ps(K_DRAW, st);
-  k_draw<<<grid, 128, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, image, contrib,
-                               final_tau, work);
+  if (depth_image != nullptr) {
+    ProfScope ps(K_DRAW_RGBD, st);
+    k_draw_rgbd<<<grid, 128, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, image,
+                                      contrib, final_tau, depth_image, alpha_image, work);
+  } else {
+    ProfScope ps(K_DRAW, st);
+    k_draw<<<grid, 128, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, image, contrib,
+                                 final_tau, work);
+  }
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

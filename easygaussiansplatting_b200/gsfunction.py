@@ -135,3 +135,42 @@ class GSFunctionFused(torch.autograd.Function):
             pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds)
         return (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus, None)
+
+
+class GSFunctionFusedRGBD(torch.autograd.Function):
+    """GSFunctionFused with depth and opacity: the same arguments and gradient slots, outputs
+    (image[3,H,W], depth[H,W], alpha[H,W], depths > 0.2) with
+        depth[p] = sum_i w_i(p) z_i,   alpha[p] = sum_i w_i(p)
+    (w = tau alpha', the image's compositing weights; z = camera-frame depth).  depth is not
+    normalised: depth / alpha is the expected depth.  Gradients of all three images flow to pws,
+    shs, alphas, scales, rots and us; the depth term reaches pws through z = (Rcw pw + tcw)[2]."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam):
+        from . import ops
+        # the fused forward's records carry z in their depth word, as the RGB-D rasterizer needs
+        us, cinv2ds, colors, depths, areas, records = ops.preprocess(
+            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+            cam.width, cam.height, alphas=alphas)
+        image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, depth, alpha = ops.splat_rgbd(
+            cam.height, cam.width, us, cinv2ds, alphas, depths, colors, areas, records=records, capacity=True)
+        ctx.cam = cam
+        ctx.alpha_shape = alphas.shape
+        ctx.save_for_backward(pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib,
+                              final_tau, patch_range_per_tile, gsid_per_patch)
+        return image, depth, alpha, depths > 0.2
+
+    @staticmethod
+    def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
+        from . import ops
+        cam = ctx.cam
+        (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau,
+         patch_range_per_tile, gsid_per_patch) = ctx.saved_tensors
+        # (autograd hands zeros for an output the loss does not use: all three planes are given)
+        moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib,
+                                           final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas,
+                                           dloss_ddepth, dloss_dalpha, moments_only=True)
+        dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = ops.preprocessB(
+            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths)
+        return (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus, None)

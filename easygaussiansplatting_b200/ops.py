@@ -202,30 +202,38 @@ def _bytes(n, dev):
     return torch.empty((n,), dtype=torch.uint8, device=dev)
 
 
-def _frame_buffers(lib, dev, H, W, N, P):
-    """the sort workspace for P patch slots and splat's five outputs"""
+def _frame_buffers(lib, dev, H, W, N, P, rgbd=False):
+    """the sort workspace for P patch slots and splat's five outputs (+ the depth and alpha planes)"""
     T = ((W + 15) // 16) * ((H + 15) // 16)
     ws = _bytes(lib.gsb_splat_workspace_bytes(N, H, W, P), dev)
+    planes = [torch.empty((H, W), dtype=torch.float32, device=dev) for _ in range(2)] if rgbd else []
     return ws, [torch.empty((3, H, W), dtype=torch.float32, device=dev),
                 torch.empty((H, W), dtype=torch.int32, device=dev),
                 torch.empty((H, W), dtype=torch.float32, device=dev),
                 torch.empty((T, 2), dtype=torch.int32, device=dev),
-                torch.empty((P,), dtype=torch.int32, device=dev)]
+                torch.empty((P,), dtype=torch.int32, device=dev)] + planes
 
 
 def _capacity_frame(H, W, us, cinv2ds, alphas, depths, colors, areas, records, P_cap, dk_cap, status,
-                    enqueue=False):
+                    enqueue=False, rgbd=False):
     """Bins, sorts and draws one frame with the sort sized from the bounds (P_cap, dk_cap):
-    gsb_splat_forward, or gsb_splat_forward_enqueue (no host wait: for CUDA graph capture).
+    gsb_splat_forward, or gsb_splat_forward_enqueue (no host wait: for CUDA graph capture), or
+    with rgbd gsb_splat_forward_rgbd.
     -> (False when the frame outgrew a bound, its workspaces, the five outputs with P_cap
-    gsid slots); `status` (pinned int32[4]) receives the status word."""
+    gsid slots, + depth and alpha with rgbd); `status` (pinned int32[4]) receives the status word."""
     lib, N, dev = _L(), us.shape[0], us.device
+    if rgbd and enqueue:
+        raise ValueError("the RGB-D frame has no enqueue-only form")
     bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
-    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap)
-    forward = lib.gsb_splat_forward_enqueue if enqueue else lib.gsb_splat_forward
-    rc = forward(H, W, N, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors), _ptr(areas),
-                 _ptr(records), P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
-                 *[_ptr(o) for o in out], status.data_ptr(), _stream())
+    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap, rgbd)
+    args = (H, W, N, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors), _ptr(areas),
+            _ptr(records), P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
+            *[_ptr(o) for o in out[:5]], status.data_ptr())
+    if rgbd:
+        rc = lib.gsb_splat_forward_rgbd(*args, _ptr(out[5]), _ptr(out[6]), _stream())
+    else:
+        forward = lib.gsb_splat_forward_enqueue if enqueue else lib.gsb_splat_forward
+        rc = forward(*args, _stream())
     if rc != GSB_CAPACITY_EXCEEDED:
         _lib.check(rc, lib)
     return rc == 0, (bin_ws, ws), out
@@ -250,6 +258,20 @@ def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=Non
     capacity (extension): size the sort from the previous frame of the same shape
     (gsb_splat_forward) instead of reading the patch count back in the middle of the frame; a
     frame that outgrows the bound is transparently redone the exact way."""
+    return _splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records, capacity, False)
+
+
+def splat_rgbd(height, width, us, cinv2ds, alphas, depths, colors, areas, records=None, capacity=False):
+    """`splat` (same arguments, same five outputs, bit-identical) plus two [H,W] planes composited
+    with the image's weights w = tau alpha':  depth D = sum w z  and  alpha A = sum w,  z = the
+    Gaussian's `depths` value.  D is not normalised (the expected depth is D / A); pixels of empty
+    tiles get D = A = 0.  -> [image, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+    depth[H,W], alpha[H,W]].  Its backward is `splatB_rgbd`."""
+    return _splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records, capacity, True)
+
+
+def _splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records, capacity, rgbd):
+    """the one frame driver of `splat` and `splat_rgbd`"""
     H, W = int(height), int(width)
     if H <= 0 or W <= 0:
         raise ValueError("height and width must be positive")
@@ -268,7 +290,9 @@ def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=Non
         records = _chk(records, "records", last=12, ndim=2)
         if records.shape[0] != N:
             raise ValueError("records must be [N, 12]")
-    inputs = (us, cinv2ds, alphas, colors)
+    # the record cache key: what the records are packed from (depths last: only the RGB-D
+    # backward reads the records' depth word, and it looks the records up with depths included)
+    inputs = (us, cinv2ds, alphas, colors, depths)
     cap_key = (dev.index, H, W, N)
     # the workspaces are consumed by kernels already enqueued on the current stream; the caching
     # allocator only reuses them for later work on the same stream
@@ -279,7 +303,7 @@ def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=Non
             if status is None:
                 status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
             ok, (_, ws), out = _capacity_frame(H, W, us, cinv2ds, alphas, depths, colors, areas, records, P_cap,
-                                               dk_cap, status)
+                                               dk_cap, status, rgbd=rgbd)
             if ok:
                 CAPACITY_STATS["capacity_frames"] += 1
                 P, dkmax, _ = _decode_status(status)
@@ -294,13 +318,13 @@ def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=Non
         _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
                                      C.byref(P), C.byref(dkmax), _stream()), lib)
         P = int(P.value)
-        ws, out = _frame_buffers(lib, dev, H, W, N, P)
+        ws, out = _frame_buffers(lib, dev, H, W, N, P, rgbd)
         if capacity:
             CAPACITY_STATS["exact_frames"] += 1
             _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
-        _lib.check(lib.gsb_splat_render(H, W, N, P, dkmax.value, _ptr(us), _ptr(cinv2ds), _ptr(alphas),
-                                        _ptr(depths), _ptr(colors), _ptr(records), _ptr(bin_ws), _ptr(ws), ws.numel(),
-                                        *[_ptr(o) for o in out], _stream()), lib)
+        render = lib.gsb_splat_render_rgbd if rgbd else lib.gsb_splat_render
+        _lib.check(render(H, W, N, P, dkmax.value, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors),
+                          _ptr(records), _ptr(bin_ws), _ptr(ws), ws.numel(), *[_ptr(o) for o in out], _stream()), lib)
         _attach_records(out[4], records, ws, N, H, W, P, inputs)
     return out
 
@@ -312,7 +336,9 @@ def splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records=Non
 # caching allocator may hand out again, and the workspace lives exactly as long as that tensor.
 # The inputs must still be the very tensors the forward saw, unmodified (data_ptr + torch's
 # in-place version counter); writes that bypass the counter (`.data`, foreign kernels) are the
-# caller's to announce with `forget_records(gsid)`.
+# caller's to announce with `forget_records(gsid)`.  The key covers us, cinv2ds, alphas, colors
+# and depths; `splatB` matches the first four (its kernel never reads the depth word), `splatB_rgbd`
+# all five, so it never uses records whose depth word is stale.
 _RECORDS_ATTR = "_gsb_records"
 
 
@@ -334,7 +360,8 @@ def _cached_records(gsid, inputs):
     if h is None:
         return None
     ws, offset, key, gptr, P = h
-    if gptr != gsid.data_ptr() or P != gsid.numel() or key != _input_key(inputs):
+    want = _input_key(inputs)
+    if gptr != gsid.data_ptr() or P != gsid.numel() or want is None or key is None or key[:len(want)] != want:
         return None
     return ws.data_ptr() + offset
 
@@ -359,6 +386,28 @@ def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_ta
     records (extension): the forward's packed per-Gaussian records [N,12] (what `splat` was given,
     or its own); they are used as they are instead of those `splat` attached to gsid_per_patch,
     and nothing is re-packed."""
+    return _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
+                   gsid_per_patch, dloss_dgammas, None, None, moments_only, records)
+
+
+def splatB_rgbd(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
+                gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only=False, records=None):
+    """Backward of `splat_rgbd`: `splatB`'s arguments plus dloss_ddepth[H,W] and dloss_dalpha[H,W]
+    (dL/dD, dL/dA); `depths` is read (the records' depth words).
+    -> [dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors] as `splatB`, + dloss_ddepths[N]
+    (dL/dz of every Gaussian's `depths` value); with moments_only: [moments[N,9], dloss_ddepths]
+    for `preprocessB(..., moments=..., dloss_ddepths=...)`.
+    records: as for `splatB`; they must carry z, as those `preprocess(..., alphas=...)` returns do.
+    Records `splat` / `splat_rgbd` attached to gsid_per_patch are used only while `depths` is
+    unchanged too; otherwise they are re-packed from the arguments."""
+    return _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
+                   gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only, records)
+
+
+def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
+            gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only, records):
+    """`splatB`, or `splatB_rgbd` when dloss_ddepth is given"""
+    rgbd = dloss_ddepth is not None
     H, W = int(height), int(width)
     us = _chk(us, "us", last=2, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
     alphas = _chk(alphas, "alphas"); colors = _chk(colors, "colors", last=3, ndim=2)
@@ -375,6 +424,14 @@ def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_ta
         raise ValueError("patch_range_per_tile does not match the tile grid")
     if not (cinv2ds.shape[0] == N and alphas.numel() == N and colors.shape[0] == N):
         raise ValueError("splatB inputs disagree on N")
+    if rgbd:
+        depths = _chk(depths, "depths")
+        dld = _chk(dloss_ddepth, "dloss_ddepth"); dla = _chk(dloss_dalpha, "dloss_dalpha")
+        _same_device(us, depths, dld, dla)
+        if depths.numel() != N:
+            raise ValueError("splatB_rgbd inputs disagree on N")
+        if dld.numel() != H * W or dla.numel() != H * W:
+            raise ValueError("dloss_ddepth / dloss_dalpha do not match height x width")
     if records is not None:
         records = _chk(records, "records", last=12, ndim=2)
         _same_device(us, records)
@@ -390,22 +447,31 @@ def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_ta
         du = torch.empty((N, 1, 2), **o); dc = torch.empty((N, 1, 3), **o)
         da = torch.empty((N, 1, 1), **o); dcol = torch.empty((N, 1, 3), **o)
         moments = None
+    ddepths = torch.empty((N,), **o) if rgbd else None
     lib = _L()
     with torch.cuda.device(dev):
         if records is not None:
             recs = records.data_ptr()
         else:
-            recs = _cached_records(gsid, (us, cinv2ds, alphas, colors)) if P > 0 else None
+            key = (us, cinv2ds, alphas, colors, depths) if rgbd else (us, cinv2ds, alphas, colors)
+            recs = _cached_records(gsid, key) if P > 0 else None
         # with cached records only the [N,9] moment rows are needed from the workspace
         ws = _bytes(lib.gsb_splat_backward_workspace_bytes(N, H, W, 0 if recs else P), dev)
-        _lib.check(lib.gsb_splat_backward(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
-                                          _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
-                                          recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol),
-                                          _ptr(moments), _stream()), lib)
+        if rgbd:
+            _lib.check(lib.gsb_splat_backward_rgbd(
+                H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
+                _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dld), _ptr(dla), recs, _ptr(ws), ws.numel(),
+                _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol), _ptr(moments), _ptr(ddepths), _stream()), lib)
+        else:
+            _lib.check(lib.gsb_splat_backward(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
+                                              _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
+                                              recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol),
+                                              _ptr(moments), _stream()), lib)
     if moments_only:
-        return moments
+        return [moments, ddepths] if rgbd else moments
     # tagged so that the reference's `dloss_d* @ jacobian` chain takes the streaming matmul
-    return [_jac(du), _jac(dc), _jac(da), _jac(dcol)]
+    out = [_jac(du), _jac(dc), _jac(da), _jac(dcol)]
+    return out + [ddepths] if rgbd else out
 
 
 # ---------------------------------------------------------------------------------------
@@ -436,7 +502,8 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
 
 
 def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
-                dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False):
+                dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False,
+                dloss_ddepths=None):
     """Vector-Jacobian products of the five per-Gaussian stages (== the torch.bmm chain of
     gsmodel.py:72-85).  -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4]]
     With moments[N,9] (from `splatB(..., moments_only=True)`) and the forward's cinv2ds[N,3] the
@@ -444,7 +511,9 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     dloss_dus[N,2], dloss_dalphas[N].
     compact (with moments): dloss_dshs is not produced (None) -- the caller expands it from the
     views' dL/dcolor = moments[:, 6:9] with `sh_grad_expand` -- and the other gradients share one
-    flat bucket [dpws | dscales | drots | dalphas] of 11 N floats (one collective sums it)."""
+    flat bucket [dpws | dscales | drots | dalphas] of 11 N floats (one collective sums it).
+    dloss_ddepths[N] (from `splatB_rgbd`): dL/dz of the Gaussians' depths; dloss_dpws gains
+    dloss_ddepths Rcw[2,:] (0 for culled Gaussians).  None: exactly the colour-only call."""
     (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     if moments is not None:
         moments = _chk(moments, "moments", last=9, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
@@ -458,6 +527,11 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
         _same_device(pws, gu, gc, gcol)
         if not (gu.numel() == 2 * N and gc.numel() == 3 * N and gcol.numel() == 3 * N):
             raise ValueError("preprocessB inputs disagree on N")
+    if dloss_ddepths is not None:
+        dloss_ddepths = _chk(dloss_ddepths, "dloss_ddepths")
+        _same_device(pws, dloss_ddepths)
+        if dloss_ddepths.numel() != N:
+            raise ValueError("dloss_ddepths must have N elements")
     o = dict(dtype=torch.float32, device=pws.device)
     # one flat bucket [dshs | drots | dpws | dscales]: a multi-GPU caller can all-reduce the four
     # gradients in place with a single collective (parallel.allreduce_grads); every view starts
@@ -482,11 +556,14 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     dus = torch.empty((N, 2), **o) if moments is not None else None
     lib = _L()
     with torch.cuda.device(pws.device):
-        _lib.check(lib.gsb_preprocess_backward(
-            N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
-            float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
-            _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(moments), _ptr(cinv2ds),
-            _ptr(dus), _ptr(dal), _stream()), lib)
+        args = (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
+                float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
+                _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(moments), _ptr(cinv2ds),
+                _ptr(dus), _ptr(dal))
+        if dloss_ddepths is not None:
+            _lib.check(lib.gsb_preprocess_backward_rgbd(*args, _ptr(dloss_ddepths), _stream()), lib)
+        else:
+            _lib.check(lib.gsb_preprocess_backward(*args, _stream()), lib)
     return [gpw, gsh, gs, gq] + ([dus, dal] if moments is not None else [])
 
 

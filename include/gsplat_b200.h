@@ -116,6 +116,16 @@ int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *r
                             float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
                             const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                             gsb_stream_t stream);
+/* RGB-D form (extension): the same, plus dloss_ddepths[N] = dL/dz from gsb_splat_backward_rgbd.
+ * z = (Rcw pw + tcw)[2], so dL/dpws gains dloss_ddepths Rcw[2,:]; a culled Gaussian (z < 0.2)
+ * gets 0, as for every other gradient. */
+int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                                 const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                                 float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                                 const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                                 const float *dloss_ddepths, gsb_stream_t stream);
 
 /* dL/dsh from per-view dL/dcolor (extension; multi-view data parallelism, SURVEY 8e).
  * colour = 0.5 + sum_l Y_l(dir) sh_l is linear in sh and never clamped (kernel.cu:735-774), so
@@ -162,6 +172,22 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
                      int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
                      int32_t *gsid_per_patch, gsb_stream_t stream);
 
+/* ---- RGB-D rendering (extension).  The *_rgbd forms of gsb_splat_render / gsb_splat_forward also
+ * write two more [H,W] planes, 16-byte aligned like `image` (a misaligned one is an argument error):
+ *   depth_image D[p] = sum_i w_i(p) z_i,   alpha_image A[p] = sum_i w_i(p),
+ * with the image's compositing weights w_i = tau_i alpha'_i (same clamp, skip and stop rules) and
+ * z_i the Gaussian's camera-frame depth, i.e. its `depths` value.  Pixels of tiles without patches
+ * get D = A = 0.  D is not normalised: the expected depth is D / A.  Every other output is
+ * bit-identical to the colour entry point's.
+ * The packed records carry z in their last word (q2.w): those gsb_preprocess_forward writes and
+ * those the render entry points pack (from `depths`) both do, and only the RGB-D rasterizers
+ * read it. */
+int gsb_splat_render_rgbd(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                          const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                          const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
+                          int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                          float *depth_image, float *alpha_image, gsb_stream_t stream);
+
 /* ---- splat, both phases without the mid-way host round trip (extension).
  * gsb_splat_bin + gsb_splat_render stall the GPU while the host reads P back to size the sort
  * workspace (the reference does the same, gausplat.cu:64-67).  Here the caller provides CAPACITIES
@@ -186,6 +212,13 @@ int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds
                       size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                       int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                       gsb_stream_t stream);
+/* RGB-D form: the same, plus depth_image / alpha_image as for gsb_splat_render_rgbd. */
+int gsb_splat_forward_rgbd(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
+                           float *depths, const float *colors, int32_t *areas, const void *packed_records,
+                           int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
+                           size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                           int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
+                           float *depth_image, float *alpha_image, gsb_stream_t stream);
 
 /* Same, but only ENQUEUES (no host wait, no event): for capture into a CUDA graph.  status_host is
  * written by a stream-ordered copy; the caller reads it after the work has completed (any
@@ -213,6 +246,19 @@ int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const fl
                        const void *packed_records, void *ws,
                        size_t ws_bytes, float *dloss_dus, float *dloss_dcinv2ds,
                        float *dloss_dalphas, float *dloss_dcolors, float *moments_out, gsb_stream_t stream);
+/* RGB-D form (extension): the backward of gsb_splat_render_rgbd / gsb_splat_forward_rgbd.  Extra inputs:
+ * depths[N] (the depth words of the records it re-packs when packed_records is NULL),
+ * dloss_ddepth_image[H,W] and dloss_dalpha_image[H,W] (any 4-byte alignment, like dloss_dgammas);
+ * extra output dloss_ddepths[N] = dL/dz (every element written; 0 for Gaussians no pixel replays).
+ * packed_records, when given, must carry z (gsb_preprocess_forward's, or the forward's own). */
+int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                            const float *alphas, const float *colors, const float *depths, const int32_t *contrib,
+                            const float *final_tau, const int32_t *patch_range_per_tile,
+                            const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                            const float *dloss_ddepth_image, const float *dloss_dalpha_image,
+                            const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
+                            float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
+                            float *dloss_ddepths, gsb_stream_t stream);
 
 /* ---- batched tiny matmul (extension).  C[b] = A[b] (m x k) . B[b] (k x n), or B shared by all
  * batches when b_shared != 0; dense row-major f32.  This is the product the reference's
