@@ -168,14 +168,17 @@ int gsb_preprocess_forward(int N, int sh_dim3, const float *pws, const float *ro
                                (cudaStream_t)stream);
 }
 
-// Checks shared by the fused backward's two entry points: N, sh_dim3, the parameter and camera
+static bool aligned(const void *p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+// Checks shared by the fused backward's entry points: N, sh_dim3, the parameter and camera
 // pointers, and the upstream gradients -- the moment rows with the forward's conics and the dL/du
 // output, or the plain dL/du, dL/dconic and dL/dcolor.  `who` prefixes the error message.
+// pose_only (gsb_preprocess_backward_pose without per-Gaussian outputs): no dL/du output either.
 static int check_preprocess_backward(const char *who, int N, int sh_dim3, const float *pws, const float *rots,
                                      const float *scales, const float *shs, const float *Rcw, const float *tcw,
                                      const float *twc, const float *dloss_dus, const float *dloss_dcinv2ds,
                                      const float *dloss_dcolors, const float *moments, const float *cinv2ds,
-                                     const float *dloss_dus_out) {
+                                     const float *dloss_dus_out, bool pose_only = false) {
   const char *err = nullptr;
   if (N < 0)
     err = "N < 0";
@@ -183,7 +186,8 @@ static int check_preprocess_backward(const char *who, int N, int sh_dim3, const 
     err = "shs.shape[1]/3 must be 1, 4, 9 or 16";
   else if (N > 0 && !(pws && rots && scales && shs && Rcw && tcw && twc))
     err = "null pointer";
-  else if (N > 0 && !(moments ? (cinv2ds && dloss_dus_out) : (dloss_dus && dloss_dcinv2ds && dloss_dcolors)))
+  else if (N > 0 && !(moments ? (cinv2ds && (pose_only || dloss_dus_out))
+                              : (dloss_dus && dloss_dcinv2ds && dloss_dcolors)))
     err = "null upstream gradient";
   if (err == nullptr) return 0;
   char msg[128];
@@ -210,7 +214,8 @@ static int preprocess_backward_impl(const char *who, int N, int sh_dim3, const f
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, (cudaStream_t)stream);
+                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, nullptr,
+                               (cudaStream_t)stream);
 }
 
 int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -240,6 +245,39 @@ int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const flo
                                   dloss_dalphas_out, stream);
 }
 
+size_t gsb_preprocess_backward_pose_workspace_bytes(int N) { return pose_workspace_bytes(N); }
+
+int gsb_preprocess_backward_pose(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                                 const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                                 float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                                 const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                                 const float *dloss_ddepths, float *dloss_dcamera, void *ws, size_t ws_bytes,
+                                 gsb_stream_t stream) {
+  const bool pose_only = dloss_dpws == nullptr;
+  if (int rc = check_preprocess_backward("preprocessB_pose", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc,
+                                          dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dus_out,
+                                          pose_only))
+    return rc;
+  GSB_REQUIRE(dloss_dcamera != nullptr, "preprocessB_pose: null dloss_dcamera");
+  // the per-Gaussian outputs all go together: all of them (pose and parameters) or none (pose only)
+  const bool all = dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots &&
+                   (moments == nullptr || (dloss_dus_out && dloss_dalphas_out));
+  const bool none = !dloss_dpws && !dloss_dshs && !dloss_dscales && !dloss_drots &&
+                    (moments == nullptr || (!dloss_dus_out && !dloss_dalphas_out));
+  GSB_REQUIRE(N == 0 || all || none, "preprocessB_pose: per-Gaussian outputs must be all set or all null");
+  GSB_REQUIRE(aligned(ws, 16), "preprocessB_pose: workspace misaligned");
+  GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
+              "preprocessB_pose: workspace too small");
+  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
+  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
+  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
+                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, &po,
+                               (cudaStream_t)stream);
+}
+
 int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float *twcs, const float *dloss_dcolors,
                        float *dloss_dshs, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && V >= 1, "sh_grad_expand: bad N / V");
@@ -265,8 +303,6 @@ int gsb_gau_loss(int H, int W, const float *image, const float *gt_image, float 
   GSB_REQUIRE(ws_bytes >= gau_loss_workspace_bytes(H, W), "gau_loss: workspace too small");
   return launch_gau_loss(H, W, image, gt_image, loss_lambda, loss_out, dloss_dimage, ws, (cudaStream_t)stream);
 }
-
-static bool aligned(const void *p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 // The binning packs a Gaussian's tile rectangle into 16-bit fields: x1 == 65536 would wrap to 0
 // and put its patches into the wrong tiles.
@@ -694,7 +730,7 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, nullptr};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, nullptr, nullptr, nullptr, &gp,
-                               moments ? &mi : nullptr, nullptr, (cudaStream_t)stream);
+                               moments ? &mi : nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *const *regions_host, uint32_t epoch,

@@ -95,14 +95,22 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
 // dL/dalpha are still written out (the caller's densification statistics / alpha gradient), and
 // the separate finalize pass with its 36 B/Gaussian round trip disappears.
 // DEPTH = the RGB-D rasterizer's dL/dz[N] (g_depths) is a fourth upstream gradient (not with PUSH).
-template <int K3, bool PUSH, bool MOM, bool DEPTH>
+// POSE = the camera gradient instead of the per-Gaussian ones (not with PUSH): everything is read
+// as before, the CTA sums its threads' 15 contributions (pg::backward_one) -- warp shuffles, then
+// the 4 warps through shared memory, fp32 -- into row blockIdx.x of pose_part[nb][16] (summed by
+// k_pose_reduce), and no per-Gaussian gradient (nor, with MOM, dL/du or dL/dalpha) is written, nor
+// the SH tile flushed.  A caller that wants both runs the non-POSE form as well: the compiler
+// fuses multiply-adds differently in a kernel that also carries the camera terms, and the
+// per-Gaussian gradients have to be the same bits with and without the pose.
+template <int K3, bool PUSH, bool MOM, bool DEPTH, bool POSE>
 __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
     const float *__restrict__ shs, const float *__restrict__ Rcw, const float *__restrict__ tcw,
     const float *__restrict__ twc, float fx, float fy, float cx, float cy, float tan_fovx, float tan_fovy,
     const float *__restrict__ g_us, const float *__restrict__ g_cinv2ds, const float *__restrict__ g_colors,
     float *__restrict__ g_pws, float *__restrict__ g_shs, float *__restrict__ g_scales,
-    float *__restrict__ g_rots, GradPush gp, MomentsIn mi, const float *__restrict__ g_depths) {
+    float *__restrict__ g_rots, GradPush gp, MomentsIn mi, const float *__restrict__ g_depths,
+    float *__restrict__ pose_part) {
   constexpr int KS = 3 * K3;
   constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
   __shared__ float sm[SMF];
@@ -129,8 +137,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
       gci[0] = -0.5f * m[2]; gci[1] = -m[3]; gci[2] = -0.5f * m[4];
       gcol[0] = m[6]; gcol[1] = m[7]; gcol[2] = m[8];
       galpha = m[5];
-      st_pair(mi.dus_out, i, gu[0], gu[1]);
-      if (mi.dalphas_out != nullptr) mi.dalphas_out[i] = galpha;
+      if (!POSE) st_pair(mi.dus_out, i, gu[0], gu[1]);
+      if (!POSE && mi.dalphas_out != nullptr) mi.dalphas_out[i] = galpha;
     }
   } else if (valid) {
     const long long i = base + tid;
@@ -142,6 +150,36 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   tile_fetch<KS>(shs, base, nv, sm, tid);
   __syncthreads();
   float gpw[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f};
+  if (POSE) {
+    float gcam[15];
+#pragma unroll
+    for (int e = 0; e < 15; e++) gcam[e] = 0.f;
+    if (valid) {
+      const float gz = DEPTH ? __ldg(g_depths + base + tid) : 0.f;
+      float xpw[3], xq[4], xs[3], xsh[KS];  // the per-Gaussian outputs: not written by this form
+      pg::backward_one<K3, DEPTH, true>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam);
+    }
+    __shared__ float red[PG / 32][16];
+#pragma unroll
+    for (int e = 0; e < 15; e++) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) gcam[e] += __shfl_down_sync(0xffffffffu, gcam[e], o);
+    }
+    if ((tid & 31) == 0) {
+#pragma unroll
+      for (int e = 0; e < 15; e++) red[tid >> 5][e] = gcam[e];
+    }
+    __syncthreads();
+    if (tid < 16) {
+      float v = 0.f;
+      if (tid < 15) {
+#pragma unroll
+        for (int w = 0; w < PG / 32; w++) v += red[w][tid];
+      }
+      pose_part[(size_t)blockIdx.x * 16 + tid] = v;
+    }
+    return;  // nothing per Gaussian leaves the CTA
+  }
   // dL/dsh overwrites the thread's own SH row in place, then the tile is flushed
   if (DEPTH) {
     const float gz = valid ? __ldg(g_depths + base + tid) : 0.f;
@@ -187,6 +225,45 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
         for (int p = 0; p < gp.world; p++) st_release_sys(gp.flags[p] + gp.rank, gp.epoch);
       }
     }
+  }
+}
+
+// The camera gradient: the nrows partial rows of k_preprocess_bwd<..., POSE> summed in fp64 by
+// one CTA in a fixed order (thread t takes rows t, t + PR, ...; then a fixed shuffle tree and the
+// warps in index order), so the result is the same bits on every run.  nrows == 0 writes zeros.
+constexpr int PR = 512;
+__global__ void __launch_bounds__(PR) k_pose_reduce(int nrows, const float *__restrict__ part,
+                                                    float *__restrict__ gcam) {
+  const int tid = threadIdx.x;
+  double acc[15];
+#pragma unroll
+  for (int e = 0; e < 15; e++) acc[e] = 0.0;
+  for (int r = tid; r < nrows; r += PR) {
+    const float4 *row = reinterpret_cast<const float4 *>(part + (size_t)r * 16);
+    float v[16];
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      const float4 x = __ldg(row + c);
+      v[4 * c] = x.x; v[4 * c + 1] = x.y; v[4 * c + 2] = x.z; v[4 * c + 3] = x.w;
+    }
+#pragma unroll
+    for (int e = 0; e < 15; e++) acc[e] += (double)v[e];
+  }
+#pragma unroll
+  for (int e = 0; e < 15; e++) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[e] += __shfl_down_sync(0xffffffffu, acc[e], o);
+  }
+  __shared__ double red[PR / 32][15];
+  if ((tid & 31) == 0) {
+#pragma unroll
+    for (int e = 0; e < 15; e++) red[tid >> 5][e] = acc[e];
+  }
+  __syncthreads();
+  if (tid < 15) {
+    double t = 0.0;
+    for (int w = 0; w < PR / 32; w++) t += red[w][tid];
+    gcam[tid] = (float)t;
   }
 }
 
@@ -278,32 +355,54 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, cudaStream_t st) {
-  if (N <= 0) return 0;
+                          const float *g_depths, const PoseOut *po, cudaStream_t st) {
+  if (po != nullptr && gp != nullptr) return set_arg_error("preprocessB: no camera gradient with the exchange");
+  if (N <= 0 && po == nullptr) return 0;
   if (g_depths != nullptr && gp != nullptr) return set_arg_error("preprocessB: no depth gradient with the exchange");
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
-  const int nb = (N + PG - 1) / PG;
+  const int nb = N > 0 ? (N + PG - 1) / PG : 0;
   const GradPush p = gp ? *gp : GradPush{};
   const MomentsIn m = mi ? *mi : MomentsIn{};
+  float *part = po ? po->part : nullptr;
   ProfScope ps(K_PRE_BWD, st);
-#define GSB_PRE_BWD(PUSH, MOM, DEPTH)                                                                           \
-  GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH><<<nb, PG, 0, st>>>(                               \
+#define GSB_PRE_BWD(PUSH, MOM, DEPTH, POSE)                                                                     \
+  GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE><<<nb, PG, 0, st>>>(                         \
                           N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us, g_cinv2ds, \
-                          g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths)))
-  if (gp != nullptr && mi != nullptr) {
-    GSB_PRE_BWD(true, true, false);
-  } else if (gp != nullptr) {
-    GSB_PRE_BWD(true, false, false);
-  } else if (mi != nullptr) {
-    if (g_depths != nullptr) {
-      GSB_PRE_BWD(false, true, true);
-    } else {
-      GSB_PRE_BWD(false, true, false);
+                          g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part)))
+  // the camera gradient; then, unless g_pws is NULL (pose only), the per-Gaussian gradients from
+  // the unchanged kernel below
+  if (po != nullptr) {
+    if (nb > 0) {
+      if (mi != nullptr) {
+        if (g_depths != nullptr) {
+          GSB_PRE_BWD(false, true, true, true);
+        } else {
+          GSB_PRE_BWD(false, true, false, true);
+        }
+      } else if (g_depths != nullptr) {
+        GSB_PRE_BWD(false, false, true, true);
+      } else {
+        GSB_PRE_BWD(false, false, false, true);
+      }
     }
-  } else if (g_depths != nullptr) {
-    GSB_PRE_BWD(false, false, true);
-  } else {
-    GSB_PRE_BWD(false, false, false);
+    k_pose_reduce<<<1, PR, 0, st>>>(nb, part, po->gcam);
+  }
+  if (nb > 0 && (po == nullptr || g_pws != nullptr)) {
+    if (gp != nullptr && mi != nullptr) {
+      GSB_PRE_BWD(true, true, false, false);
+    } else if (gp != nullptr) {
+      GSB_PRE_BWD(true, false, false, false);
+    } else if (mi != nullptr) {
+      if (g_depths != nullptr) {
+        GSB_PRE_BWD(false, true, true, false);
+      } else {
+        GSB_PRE_BWD(false, true, false, false);
+      }
+    } else if (g_depths != nullptr) {
+      GSB_PRE_BWD(false, false, true, false);
+    } else {
+      GSB_PRE_BWD(false, false, false, false);
+    }
   }
 #undef GSB_PRE_BWD
   GSB_CUDA_TRY(cudaGetLastError());

@@ -52,16 +52,25 @@ struct MomentsIn {
   float *dalphas_out;    // [N]    dL/dalpha (nullable: the push variant forwards it instead)
 };
 struct GradPush;
+// the camera gradient (fused.cu, POSE variants): gcam[15] = dL/dRcw (9), dL/dtcw (3), dL/dtwc (3);
+// part = ceil(N/128) partial rows of 16 floats (16-byte aligned), one per CTA
+struct PoseOut {
+  float *gcam;
+  float *part;
+};
+constexpr size_t pose_workspace_bytes(int N) { return N > 0 ? (size_t)((N + 127) / 128) * 16 * sizeof(float) : 0; }
 // gp == nullptr: the gradients go to g_pws, g_shs, g_scales, g_rots; otherwise into the exchange
 // staging slots gp describes (the g_* outputs are unused).  mi == nullptr: the upstream gradients
 // are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.  g_depths: NULL, or dL/dz[N]
-// of the RGB-D rasterizer (not with gp).
+// of the RGB-D rasterizer (not with gp).  po: NULL, or also the camera gradient (not with gp; a
+// pass of its own); then g_pws == NULL (with g_shs, g_scales, g_rots and mi's outputs NULL) writes
+// only that.
 int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, cudaStream_t st);
+                          const float *g_depths, const PoseOut *po, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,

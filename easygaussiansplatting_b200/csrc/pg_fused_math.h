@@ -213,10 +213,17 @@ GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], c
 // backward for one Gaussian.  gu[2], gconic[3], gcol[3] are the splatB outputs for it.
 // gsh may alias sh (row-private in-place update).  DEPTH: gdepth = dL/dz from the RGB-D
 // rasterizer; z = pc[2], so it adds to dL/dpc[2] and reaches dL/dpw through Rcw[2,:].
-template <int K3, bool DEPTH = false>
+// POSE: this Gaussian's contribution to the camera gradient, gcam[15] = dL/dRcw (row-major 9),
+// dL/dtcw (3), dL/dtwc (3):
+//   dL/dtcw = gpc;  dL/dRcw = gpc (x) pw + J^T dL/dM  (pc = Rcw pw + tcw, M = J Rcw);
+//   dL/dtwc = -(colour part of dL/dpw)  (the view direction is pw - twc).
+// gpc is the vector rotated into dL/dpw (x, y taken as unclamped, as above); a culled Gaussian
+// contributes through its colour branch only, as it does to dL/dpw.
+template <int K3, bool DEPTH = false, bool POSE = false>
 GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], const float *sh,
                          const Cam &cam, const float gu[2], const float gconic[3], const float gcol[3],
-                         float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f) {
+                         float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f,
+                         float *gcam = nullptr /*[15], POSE only*/) {
   // ---- colour branch (independent of the depth cull, like sh2Color)
   float Y[K3], dY[K3][3];
   float d[3], ninv = 1.f, r[3] = {0.f, 0.f, 0.f};
@@ -238,6 +245,10 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
   if (K3 > 1) {
     const float rg = r[0] * gdir[0] + r[1] * gdir[1] + r[2] * gdir[2];
     for (int a = 0; a < 3; a++) gpw[a] = (gdir[a] - r[a] * rg) * ninv;
+  }
+  if (POSE) {
+    for (int e = 0; e < 12; e++) gcam[e] = 0.f;
+    for (int a = 0; a < 3; a++) gcam[12 + a] = -gpw[a];
   }
   gq[0] = gq[1] = gq[2] = gq[3] = 0.f;
   gs[0] = gs[1] = gs[2] = 0.f;
@@ -295,6 +306,17 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
   gpc[2] += -(gu[0] * (g.pc[0] * cam.fx) + gu[1] * (g.pc[1] * cam.fy)) * zi2;
   if (DEPTH) gpc[2] += gdepth;  // depth z = pc[2]
   for (int j = 0; j < 3; j++) gpw[j] += gpc[0] * R[j] + gpc[1] * R[3 + j] + gpc[2] * R[6 + j];
+  if (POSE) {
+    // J = [[J00, 0, J02], [0, J11, J12]] exactly as cov2d() evaluated it
+    const float J00 = cam.fx * zi, J11 = cam.fy * zi;
+    const float J02 = -(cam.fx * g.xc) * zi2, J12 = -(cam.fy * g.yc) * zi2;
+    for (int k = 0; k < 3; k++) {
+      gcam[k] = fmaf(gpc[0], pw[k], J00 * dM[k]);
+      gcam[3 + k] = fmaf(gpc[1], pw[k], J11 * dM[3 + k]);
+      gcam[6 + k] = fmaf(gpc[2], pw[k], fmaf(J02, dM[k], J12 * dM[3 + k]));
+      gcam[9 + k] = gpc[k];
+    }
+  }
   // cov3d: dL/dM3 = 2 sym(g3) M3
   const float G3[9] = {g3[0], 0.5f * g3[1], 0.5f * g3[2], 0.5f * g3[1], g3[3], 0.5f * g3[4],
                        0.5f * g3[2], 0.5f * g3[4], g3[5]};

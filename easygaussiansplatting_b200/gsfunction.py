@@ -174,3 +174,85 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
             pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths)
         return (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus, None)
+
+
+def _pose_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
+    from . import ops
+    if getattr(cam, "grad_exchange", None) is not None:
+        raise ValueError("camera gradients are single-view: cam.grad_exchange must not be set")
+    Rcw, tcw, twc = Rcw.detach(), tcw.detach(), twc.detach()
+    us, cinv2ds, colors, depths, areas, records = ops.preprocess(
+        pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, alphas=alphas)
+    splat = ops.splat_rgbd if rgbd else ops.splat
+    out = splat(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, areas, records=records, capacity=True)
+    ctx.cam = cam
+    ctx.alpha_shape = alphas.shape
+    ctx.cam_shapes = (Rcw.shape, tcw.shape, twc.shape)
+    ctx.save_for_backward(pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, *out[1:5], Rcw, tcw, twc)
+    mask = depths > 0.2
+    return (out[0], out[5], out[6], mask) if rgbd else (out[0], mask)
+
+
+def _pose_backward(ctx, rgbd, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None):
+    from . import ops
+    cam = ctx.cam
+    (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau, patch_range_per_tile,
+     gsid_per_patch, Rcw, tcw, twc) = ctx.saved_tensors
+    need_map = any(ctx.needs_input_grad[:6])
+    need_cam = any(ctx.needs_input_grad[6:9])
+    ddepths = None
+    if rgbd:
+        moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib,
+                                           final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas,
+                                           dloss_ddepth, dloss_dalpha, moments_only=True)
+    else:
+        moments = ops.splatB(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib, final_tau,
+                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True)
+    # the frozen-map case (tracking) takes the pose-only kernel: no per-Gaussian gradient is written
+    out = ops.preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
+                          cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths,
+                          camera_grad=need_cam, pose_only=need_cam and not need_map)
+    if need_cam:
+        sr, st, sw = ctx.cam_shapes
+        dR, dt, dw = out[6]
+        cam_grads = (dR.reshape(sr), dt.reshape(st), dw.reshape(sw))
+    else:
+        cam_grads = (None, None, None)
+    if need_map:
+        dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = out[:6]
+        map_grads = (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus)
+    else:
+        map_grads = (None,) * 6
+    return map_grads + cam_grads + (None,)
+
+
+class GSFunctionFusedPose(torch.autograd.Function):
+    """GSFunctionFused with a differentiable camera pose:
+    `apply(pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)` -> (image, depths > 0.2).
+    The camera tensors replace cam.Rcw, cam.tcw, cam.twc (cam supplies the size and intrinsics)
+    and get dL/dRcw, dL/dtcw, dL/dtwc as independent inputs: a caller that builds twc from Rcw
+    and tcw with torch ops has autograd chain it.  What runs follows ctx.needs_input_grad:
+    only the camera -> the pose-only kernel (a frozen map: tracking); no camera -> exactly
+    GSFunctionFused's backward.  Intrinsics are not differentiated; single view only."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
+        return _pose_forward(ctx, False, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)
+
+    @staticmethod
+    def backward(ctx, dloss_dgammas, _):
+        return _pose_backward(ctx, False, dloss_dgammas)
+
+
+class GSFunctionFusedRGBDPose(torch.autograd.Function):
+    """GSFunctionFusedRGBD with a differentiable camera pose, as GSFunctionFusedPose:
+    `apply(pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)` -> (image, depth, alpha,
+    depths > 0.2).  The depth plane's gradient reaches the pose through z = (Rcw pw + tcw)[2]."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
+        return _pose_forward(ctx, True, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)
+
+    @staticmethod
+    def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
+        return _pose_backward(ctx, True, dloss_dgammas, dloss_ddepth, dloss_dalpha)

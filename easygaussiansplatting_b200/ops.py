@@ -503,7 +503,7 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
 
 def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
                 dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False,
-                dloss_ddepths=None):
+                dloss_ddepths=None, camera_grad=False, pose_only=False):
     """Vector-Jacobian products of the five per-Gaussian stages (== the torch.bmm chain of
     gsmodel.py:72-85).  -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4]]
     With moments[N,9] (from `splatB(..., moments_only=True)`) and the forward's cinv2ds[N,3] the
@@ -513,7 +513,16 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     views' dL/dcolor = moments[:, 6:9] with `sh_grad_expand` -- and the other gradients share one
     flat bucket [dpws | dscales | drots | dalphas] of 11 N floats (one collective sums it).
     dloss_ddepths[N] (from `splatB_rgbd`): dL/dz of the Gaussians' depths; dloss_dpws gains
-    dloss_ddepths Rcw[2,:] (0 for culled Gaussians).  None: exactly the colour-only call."""
+    dloss_ddepths Rcw[2,:] (0 for culled Gaussians).  None: exactly the colour-only call.
+    camera_grad: one more output follows, the camera gradient (dRcw[3,3], dtcw[3], dtwc[3]) --
+    views of one 15-float tensor, summed over the Gaussians in a fixed order (gsb_preprocess_backward_pose;
+    Rcw, tcw, twc taken as independent inputs).  The per-Gaussian outputs are the same bits as
+    without it.  pose_only (with camera_grad): the map is frozen; the per-Gaussian gradients
+    (and dloss_dus, dloss_dalphas) are not computed and come back as None."""
+    if pose_only and not camera_grad:
+        raise ValueError("pose_only=True needs camera_grad=True")
+    if camera_grad and compact:
+        raise ValueError("camera_grad does not combine with compact")
     (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     if moments is not None:
         moments = _chk(moments, "moments", last=9, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
@@ -537,7 +546,9 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     # gradients in place with a single collective (parallel.allreduce_grads); every view starts
     # 16-byte aligned (3k*N and 4*N floats are multiples of 4 elements when N % 4 == 0; the
     # kernels fall back to scalar stores otherwise)
-    if compact:
+    if pose_only:
+        bucket = gsh = gpw = gs = gq = dal = None
+    elif compact:
         if moments is None:
             raise ValueError("compact=True needs the moment rows")
         bucket = torch.empty((N * 11,), **o)
@@ -553,18 +564,27 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
         gpw = bucket[N * (3 * k + 4):N * (3 * k + 7)].view(N, 3)
         gs = bucket[N * (3 * k + 7):].view(N, 3)
         dal = torch.empty((N,), **o) if moments is not None else None
-    dus = torch.empty((N, 2), **o) if moments is not None else None
+    dus = torch.empty((N, 2), **o) if moments is not None and not pose_only else None
     lib = _L()
     with torch.cuda.device(pws.device):
         args = (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
                 float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
                 _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(moments), _ptr(cinv2ds),
                 _ptr(dus), _ptr(dal))
-        if dloss_ddepths is not None:
+        if camera_grad:
+            gcam = torch.empty((15,), **o)
+            ws_bytes = int(lib.gsb_preprocess_backward_pose_workspace_bytes(N))
+            ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
+            _lib.check(lib.gsb_preprocess_backward_pose(*args, _ptr(dloss_ddepths), _ptr(gcam), _ptr(ws), ws_bytes,
+                                                        _stream()), lib)
+        elif dloss_ddepths is not None:
             _lib.check(lib.gsb_preprocess_backward_rgbd(*args, _ptr(dloss_ddepths), _stream()), lib)
         else:
             _lib.check(lib.gsb_preprocess_backward(*args, _stream()), lib)
-    return [gpw, gsh, gs, gq] + ([dus, dal] if moments is not None else [])
+    out = [gpw, gsh, gs, gq] + ([dus, dal] if moments is not None else [])
+    if camera_grad:
+        out.append((gcam[:9].view(3, 3), gcam[9:12], gcam[12:15]))
+    return out
 
 
 def sh_grad_expand(pws, twcs, dloss_dcolors, sh_dim3, out=None):

@@ -127,6 +127,31 @@ int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const flo
                                  const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                  const float *dloss_ddepths, gsb_stream_t stream);
 
+/* Camera gradient (extension; pose refinement and RGB-D tracking).  The arguments of
+ * gsb_preprocess_backward_rgbd, where dloss_ddepths may be NULL (colour only), plus
+ * dloss_dcamera[15] = dL/dRcw (row-major 3x3), dL/dtcw (3), dL/dtwc (3), summed over the N
+ * Gaussians:  dL/dtcw = sum dL/dpc,  dL/dRcw = sum dL/dpc (x) pw + J^T dL/d(J Rcw),
+ * dL/dtwc = -sum (colour part of dL/dpw) (0 at SH degree 0).  dL/dpc is the vector the backward
+ * rotates into dloss_dpws (x, y differentiated as if unclamped, as there); a culled Gaussian
+ * contributes through its colour only.  Intrinsics are not differentiated, and Rcw, tcw, twc
+ * are independent inputs (twc = -Rcw^T tcw is the caller's relation to chain).
+ * dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots (and with moments dloss_dus_out,
+ * dloss_dalphas_out) are all set -- the same per-Gaussian outputs as gsb_preprocess_backward,
+ * bit for bit (they come from the same kernel, after a pass that computes the camera gradient)
+ * -- or all NULL: pose only, for a frozen map; one pass, nothing per Gaussian is written.
+ * ws: caller-owned, 16-byte aligned, at least gsb_preprocess_backward_pose_workspace_bytes(N)
+ * bytes.  The CTAs' partial sums are added in a fixed order in fp64 (no atomics): the same
+ * inputs give the same bits on every run.  N = 0 writes zeros. */
+size_t gsb_preprocess_backward_pose_workspace_bytes(int N);
+int gsb_preprocess_backward_pose(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                                 const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                                 float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                                 const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                                 const float *dloss_ddepths, float *dloss_dcamera, void *ws, size_t ws_bytes,
+                                 gsb_stream_t stream);
+
 /* dL/dsh from per-view dL/dcolor (extension; multi-view data parallelism, SURVEY 8e).
  * colour = 0.5 + sum_l Y_l(dir) sh_l is linear in sh and never clamped (kernel.cu:735-774), so
  * dloss_dshs[n, l, c] = sum_v Y_l((pws[n] - twcs[v]) / |.|) * dloss_dcolors[v, n, c].
