@@ -170,25 +170,46 @@ int gsb_preprocess_forward(int N, int sh_dim3, const float *pws, const float *ro
 
 static bool aligned(const void *p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
-// Checks shared by the fused backward's entry points: N, sh_dim3, the parameter and camera
-// pointers, and the upstream gradients -- the moment rows with the forward's conics and the dL/du
-// output, or the plain dL/du, dL/dconic and dL/dcolor.  `who` prefixes the error message.
-// pose_only (gsb_preprocess_backward_pose without per-Gaussian outputs): no dL/du output either.
-static int check_preprocess_backward(const char *who, int N, int sh_dim3, const float *pws, const float *rots,
-                                     const float *scales, const float *shs, const float *Rcw, const float *tcw,
-                                     const float *twc, const float *dloss_dus, const float *dloss_dcinv2ds,
-                                     const float *dloss_dcolors, const float *moments, const float *cinv2ds,
-                                     const float *dloss_dus_out, bool pose_only = false) {
+// Which per-Gaussian outputs an entry point of the fused backward writes: dloss_dpws, dloss_dshs,
+// dloss_dscales, dloss_drots and, with the moment rows, dloss_dus_out and dloss_dalphas_out.
+enum class GradOutputs {
+  kAll,        // all of them (plain and RGB-D); with the moment rows dloss_dshs may be NULL (gsb_sh_grad_expand)
+  kAllOrNone,  // all of them, or none: the camera gradient only (pose)
+  kNone,       // none: the gradients go to the exchange; with the moment rows dloss_dus_out still does (push)
+};
+
+// Every check the fused backward's entry points share: N, sh_dim3, the parameter and camera
+// pointers, the upstream gradients (the moment rows with the forward's conics, or the plain dL/du,
+// dL/dconic and dL/dcolor) and the per-Gaussian outputs `outs` asks for.  `who` prefixes the error
+// message.  An entry point checks its own further arguments after this.
+static int check_preprocess_backward(const char *who, GradOutputs outs, int N, int sh_dim3, const float *pws,
+                                     const float *rots, const float *scales, const float *shs, const float *Rcw,
+                                     const float *tcw, const float *twc, const float *dloss_dus,
+                                     const float *dloss_dcinv2ds, const float *dloss_dcolors, const float *moments,
+                                     const float *cinv2ds, const float *dloss_dpws, const float *dloss_dshs,
+                                     const float *dloss_dscales, const float *dloss_drots,
+                                     const float *dloss_dus_out, const float *dloss_dalphas_out) {
+  const bool mom = moments != nullptr;
+  const bool all_but_shs = dloss_dpws && dloss_dscales && dloss_drots && (!mom || (dloss_dus_out && dloss_dalphas_out));
+  const bool none = !dloss_dpws && !dloss_dshs && !dloss_dscales && !dloss_drots &&
+                    (!mom || (!dloss_dus_out && !dloss_dalphas_out));
   const char *err = nullptr;
   if (N < 0)
     err = "N < 0";
   else if (!(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16))
     err = "shs.shape[1]/3 must be 1, 4, 9 or 16";
-  else if (N > 0 && !(pws && rots && scales && shs && Rcw && tcw && twc))
+  else if (N == 0)
+    return 0;
+  else if (!(pws && rots && scales && shs && Rcw && tcw && twc))
     err = "null pointer";
-  else if (N > 0 && !(moments ? (cinv2ds && (pose_only || dloss_dus_out))
-                              : (dloss_dus && dloss_dcinv2ds && dloss_dcolors)))
+  else if (!(mom ? cinv2ds != nullptr : (dloss_dus && dloss_dcinv2ds && dloss_dcolors)))
     err = "null upstream gradient";
+  else if (outs == GradOutputs::kAll && !(all_but_shs && (mom || dloss_dshs)))
+    err = "null output";
+  else if (outs == GradOutputs::kAllOrNone && !((all_but_shs && dloss_dshs) || none))
+    err = "per-Gaussian outputs must be all set or all null";
+  else if (outs == GradOutputs::kNone && mom && !dloss_dus_out)
+    err = "null output";
   if (err == nullptr) return 0;
   char msg[128];
   snprintf(msg, sizeof(msg), "%s: %s", who, err);
@@ -204,13 +225,10 @@ static int preprocess_backward_impl(const char *who, int N, int sh_dim3, const f
                                     float *dloss_dshs, float *dloss_dscales, float *dloss_drots,
                                     const float *moments, const float *cinv2ds, float *dloss_dus_out,
                                     float *dloss_dalphas_out, gsb_stream_t stream) {
-  if (int rc = check_preprocess_backward(who, N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, dloss_dus,
-                                          dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dus_out))
+  if (int rc = check_preprocess_backward(who, GradOutputs::kAll, N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc,
+                                          dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dpws,
+                                          dloss_dshs, dloss_dscales, dloss_drots, dloss_dus_out, dloss_dalphas_out))
     return rc;
-  // with moments, dloss_dshs may be NULL (see gsb_sh_grad_expand) and dL/dalpha is an output
-  GSB_REQUIRE(N == 0 || (dloss_dpws && dloss_dscales && dloss_drots &&
-                         (moments ? dloss_dalphas_out != nullptr : dloss_dshs != nullptr)),
-              "preprocessB: null pointer");
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
@@ -255,18 +273,12 @@ int gsb_preprocess_backward_pose(int N, int sh_dim3, const float *pws, const flo
                                  const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                  const float *dloss_ddepths, float *dloss_dcamera, void *ws, size_t ws_bytes,
                                  gsb_stream_t stream) {
-  const bool pose_only = dloss_dpws == nullptr;
-  if (int rc = check_preprocess_backward("preprocessB_pose", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc,
-                                          dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dus_out,
-                                          pose_only))
+  if (int rc = check_preprocess_backward("preprocessB_pose", GradOutputs::kAllOrNone, N, sh_dim3, pws, rots, scales,
+                                          shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
+                                          cinv2ds, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, dloss_dus_out,
+                                          dloss_dalphas_out))
     return rc;
   GSB_REQUIRE(dloss_dcamera != nullptr, "preprocessB_pose: null dloss_dcamera");
-  // the per-Gaussian outputs all go together: all of them (pose and parameters) or none (pose only)
-  const bool all = dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots &&
-                   (moments == nullptr || (dloss_dus_out && dloss_dalphas_out));
-  const bool none = !dloss_dpws && !dloss_dshs && !dloss_dscales && !dloss_drots &&
-                    (moments == nullptr || (!dloss_dus_out && !dloss_dalphas_out));
-  GSB_REQUIRE(N == 0 || all || none, "preprocessB_pose: per-Gaussian outputs must be all set or all null");
   GSB_REQUIRE(aligned(ws, 16), "preprocessB_pose: workspace misaligned");
   GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
               "preprocessB_pose: workspace too small");
@@ -703,9 +715,9 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
                                  const float *dloss_dalphas, const float *moments, const float *cinv2ds,
                                  float *dloss_dus_out, int world, int rank, void *const *regions_host,
                                  uint32_t epoch, gsb_stream_t stream) {
-  if (int rc = check_preprocess_backward("preprocess_backward_push", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw,
-                                          twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds,
-                                          dloss_dus_out))
+  if (int rc = check_preprocess_backward("preprocess_backward_push", GradOutputs::kNone, N, sh_dim3, pws, rots, scales,
+                                          shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
+                                          cinv2ds, nullptr, nullptr, nullptr, nullptr, dloss_dus_out, nullptr))
     return rc;
   GSB_REQUIRE(N == 0 || moments || dloss_dalphas, "preprocess_backward_push: null upstream gradient");
   GSB_REQUIRE(world >= 1 && world <= kMaxWorld && rank >= 0 && rank < world && regions_host && epoch != 0,

@@ -7,6 +7,8 @@
 // (SH degree 3).  The 192-byte SH rows go through the coalescing shared-memory tile of
 // tile_io.cuh; the 3/4-float rows are read and written straight from registers, so all loads
 // of a CTA are in flight at once.
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.h"
 #include "pg_fused_math.h"
@@ -350,61 +352,56 @@ int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, 
   return 0;
 }
 
+// f(std::bool_constant<b>...) for the runtime flags b...: each flag becomes a compile-time constant
+template <class F>
+static int with_flags(F &&f) { return f(); }
+template <class F, class... B>
+static int with_flags(F &&f, bool b, B... rest) {
+  const auto bind = [&](auto c) { return with_flags([&](auto... cs) { return f(c, cs...); }, rest...); };
+  return b ? bind(std::true_type{}) : bind(std::false_type{});
+}
+
 int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
                           const float *g_depths, const PoseOut *po, cudaStream_t st) {
-  if (po != nullptr && gp != nullptr) return set_arg_error("preprocessB: no camera gradient with the exchange");
   if (N <= 0 && po == nullptr) return 0;
-  if (g_depths != nullptr && gp != nullptr) return set_arg_error("preprocessB: no depth gradient with the exchange");
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = N > 0 ? (N + PG - 1) / PG : 0;
   const GradPush p = gp ? *gp : GradPush{};
   const MomentsIn m = mi ? *mi : MomentsIn{};
   float *part = po ? po->part : nullptr;
+  // one pass of k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE>, PUSH, MOM and DEPTH set by which optional
+  // inputs are given.  The exchange carries neither a depth nor a camera gradient, so no PUSH form
+  // with DEPTH or POSE exists (api.cu never asks for one).
+  const auto pass = [&](auto pose) {
+    return with_flags(
+        [&](auto push, auto mom, auto depth) -> int {
+          constexpr bool PUSH = decltype(push)::value, MOM = decltype(mom)::value, DEPTH = decltype(depth)::value,
+                         POSE = decltype(pose)::value;
+          if constexpr (PUSH && (DEPTH || POSE)) {
+            return set_arg_error("preprocessB: no depth or camera gradient with the exchange");
+          } else {
+            GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE><<<nb, PG, 0, st>>>(
+                                    N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us,
+                                    g_cinv2ds, g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part)));
+            return 0;
+          }
+        },
+        gp != nullptr, mi != nullptr, g_depths != nullptr);
+  };
   ProfScope ps(K_PRE_BWD, st);
-#define GSB_PRE_BWD(PUSH, MOM, DEPTH, POSE)                                                                     \
-  GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE><<<nb, PG, 0, st>>>(                         \
-                          N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us, g_cinv2ds, \
-                          g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part)))
-  // the camera gradient; then, unless g_pws is NULL (pose only), the per-Gaussian gradients from
-  // the unchanged kernel below
+  // the camera gradient first; then, unless g_pws is NULL (pose only), the per-Gaussian gradients
+  // from the form without POSE
   if (po != nullptr) {
-    if (nb > 0) {
-      if (mi != nullptr) {
-        if (g_depths != nullptr) {
-          GSB_PRE_BWD(false, true, true, true);
-        } else {
-          GSB_PRE_BWD(false, true, false, true);
-        }
-      } else if (g_depths != nullptr) {
-        GSB_PRE_BWD(false, false, true, true);
-      } else {
-        GSB_PRE_BWD(false, false, false, true);
-      }
-    }
+    if (nb > 0)
+      if (int rc = pass(std::true_type{})) return rc;
     k_pose_reduce<<<1, PR, 0, st>>>(nb, part, po->gcam);
   }
-  if (nb > 0 && (po == nullptr || g_pws != nullptr)) {
-    if (gp != nullptr && mi != nullptr) {
-      GSB_PRE_BWD(true, true, false, false);
-    } else if (gp != nullptr) {
-      GSB_PRE_BWD(true, false, false, false);
-    } else if (mi != nullptr) {
-      if (g_depths != nullptr) {
-        GSB_PRE_BWD(false, true, true, false);
-      } else {
-        GSB_PRE_BWD(false, true, false, false);
-      }
-    } else if (g_depths != nullptr) {
-      GSB_PRE_BWD(false, false, true, false);
-    } else {
-      GSB_PRE_BWD(false, false, false, false);
-    }
-  }
-#undef GSB_PRE_BWD
+  if (nb > 0 && (po == nullptr || g_pws != nullptr))
+    if (int rc = pass(std::false_type{})) return rc;
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

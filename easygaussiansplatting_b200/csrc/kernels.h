@@ -64,7 +64,7 @@ constexpr size_t pose_workspace_bytes(int N) { return N > 0 ? (size_t)((N + 127)
 // are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.  g_depths: NULL, or dL/dz[N]
 // of the RGB-D rasterizer (not with gp).  po: NULL, or also the camera gradient (not with gp; a
 // pass of its own); then g_pws == NULL (with g_shs, g_scales, g_rots and mi's outputs NULL) writes
-// only that.
+// only that.  The arguments are checked by the entry points (api.cu check_preprocess_backward).
 int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,

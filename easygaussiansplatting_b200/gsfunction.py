@@ -98,43 +98,11 @@ class GSFunctionFused(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pws, shs, alphas, scales, rots, us, cam):
-        from . import ops
-        # the per-Gaussian records of the rasterizers come straight out of the fused forward
-        us, cinv2ds, colors, depths, areas, records = ops.preprocess(
-            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, alphas=alphas)
-        image, contrib, final_tau, patch_range_per_tile, gsid_per_patch = ops.splat(
-            cam.height, cam.width, us, cinv2ds, alphas, depths, colors, areas, records=records, capacity=True)
-        ctx.cam = cam
-        ctx.alpha_shape = alphas.shape
-        ctx.save_for_backward(pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib,
-                              final_tau, patch_range_per_tile, gsid_per_patch)
-        return image, depths > 0.2
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
-        from . import ops
-        cam = ctx.cam
-        (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau,
-         patch_range_per_tile, gsid_per_patch) = ctx.saved_tensors
-        # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward
-        # converts them in registers (no finalize pass, no 32 B/Gaussian round trip)
-        moments = ops.splatB(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib, final_tau,
-                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True)
-        ex = getattr(cam, "grad_exchange", None)
-        if ex is not None:
-            # multi-view data parallel (parallel.GradExchange): the per-Gaussian backward pushes
-            # its tiles into peer memory and the gradients come back already summed over ranks
-            # (dloss_dus stays this view's own: it only feeds the densification statistics)
-            g = ex.backward(pws, rots, scales, shs, cam, moments=moments, cinv2ds=cinv2ds)
-            # the result region is overwritten by the next step's broadcast: hand autograd its own
-            # copies (AccumulateGrad may keep a returned tensor, and so may hooks / retain_grad)
-            return (g["dpws"].clone(), g["dshs"].clone(), g["dalphas"].clone().reshape(ctx.alpha_shape),
-                    g["dscales"].clone(), g["drots"].clone(), g["dus"], None)
-        dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = ops.preprocessB(
-            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds)
-        return (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus, None)
+        return _fused_backward(ctx, False, False, dloss_dgammas)
 
 
 class GSFunctionFusedRGBD(torch.autograd.Function):
@@ -147,59 +115,54 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pws, shs, alphas, scales, rots, us, cam):
-        from . import ops
-        # the fused forward's records carry z in their depth word, as the RGB-D rasterizer needs
-        us, cinv2ds, colors, depths, areas, records = ops.preprocess(
-            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, alphas=alphas)
-        image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, depth, alpha = ops.splat_rgbd(
-            cam.height, cam.width, us, cinv2ds, alphas, depths, colors, areas, records=records, capacity=True)
-        ctx.cam = cam
-        ctx.alpha_shape = alphas.shape
-        ctx.save_for_backward(pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib,
-                              final_tau, patch_range_per_tile, gsid_per_patch)
-        return image, depth, alpha, depths > 0.2
+        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
-        from . import ops
-        cam = ctx.cam
-        (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau,
-         patch_range_per_tile, gsid_per_patch) = ctx.saved_tensors
-        # (autograd hands zeros for an output the loss does not use: all three planes are given)
-        moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib,
-                                           final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas,
-                                           dloss_ddepth, dloss_dalpha, moments_only=True)
-        dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = ops.preprocessB(
-            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths)
-        return (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus, None)
+        return _fused_backward(ctx, True, False, dloss_dgammas, dloss_ddepth, dloss_dalpha)
 
 
-def _pose_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
+def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None):
+    """The forward of the four fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
+    camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward."""
     from . import ops
-    if getattr(cam, "grad_exchange", None) is not None:
-        raise ValueError("camera gradients are single-view: cam.grad_exchange must not be set")
-    Rcw, tcw, twc = Rcw.detach(), tcw.detach(), twc.detach()
+    if pose is None:
+        Rcw, tcw, twc = cam.Rcw, cam.tcw, cam.twc
+    else:
+        if getattr(cam, "grad_exchange", None) is not None:
+            raise ValueError("camera gradients are single-view: cam.grad_exchange must not be set")
+        Rcw, tcw, twc = (x.detach() for x in pose)
+    # the per-Gaussian records of the rasterizers come straight out of the fused forward (with z in
+    # their depth word, as the RGB-D rasterizer needs)
     us, cinv2ds, colors, depths, areas, records = ops.preprocess(
         pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, alphas=alphas)
     splat = ops.splat_rgbd if rgbd else ops.splat
     out = splat(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, areas, records=records, capacity=True)
     ctx.cam = cam
     ctx.alpha_shape = alphas.shape
-    ctx.cam_shapes = (Rcw.shape, tcw.shape, twc.shape)
-    ctx.save_for_backward(pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, *out[1:5], Rcw, tcw, twc)
+    saved = (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, *out[1:5])
+    if pose is not None:
+        ctx.cam_shapes = (Rcw.shape, tcw.shape, twc.shape)
+        saved += (Rcw, tcw, twc)
+    ctx.save_for_backward(*saved)
     mask = depths > 0.2
     return (out[0], out[5], out[6], mask) if rgbd else (out[0], mask)
 
 
-def _pose_backward(ctx, rgbd, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None):
+def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None):
+    """The backward of the four fused classes -> the gradients of the map inputs (pws, shs, alphas,
+    scales, rots, us), with pose those of Rcw, tcw, twc, and None for cam.  What runs follows
+    ctx.needs_input_grad: the pose alone takes the pose-only kernel (a frozen map: tracking)."""
     from . import ops
     cam = ctx.cam
     (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau, patch_range_per_tile,
-     gsid_per_patch, Rcw, tcw, twc) = ctx.saved_tensors
+     gsid_per_patch, *cam_saved) = ctx.saved_tensors
+    Rcw, tcw, twc = cam_saved if pose else (cam.Rcw, cam.tcw, cam.twc)
     need_map = any(ctx.needs_input_grad[:6])
-    need_cam = any(ctx.needs_input_grad[6:9])
+    need_cam = pose and any(ctx.needs_input_grad[6:9])
+    # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward converts
+    # them in registers (no finalize pass, no 32 B/Gaussian round trip).  (autograd hands zeros for
+    # an RGB-D output the loss does not use: all three planes are given)
     ddepths = None
     if rgbd:
         moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib,
@@ -208,22 +171,29 @@ def _pose_backward(ctx, rgbd, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=Non
     else:
         moments = ops.splatB(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib, final_tau,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True)
-    # the frozen-map case (tracking) takes the pose-only kernel: no per-Gaussian gradient is written
+    ex = None if rgbd or pose else getattr(cam, "grad_exchange", None)
+    if ex is not None:
+        # multi-view data parallel (parallel.GradExchange): the per-Gaussian backward pushes
+        # its tiles into peer memory and the gradients come back already summed over ranks
+        # (dloss_dus stays this view's own: it only feeds the densification statistics)
+        g = ex.backward(pws, rots, scales, shs, cam, moments=moments, cinv2ds=cinv2ds)
+        # the result region is overwritten by the next step's broadcast: hand autograd its own
+        # copies (AccumulateGrad may keep a returned tensor, and so may hooks / retain_grad)
+        return (g["dpws"].clone(), g["dshs"].clone(), g["dalphas"].clone().reshape(ctx.alpha_shape),
+                g["dscales"].clone(), g["drots"].clone(), g["dus"], None)
     out = ops.preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
                           cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths,
                           camera_grad=need_cam, pose_only=need_cam and not need_map)
-    if need_cam:
-        sr, st, sw = ctx.cam_shapes
-        dR, dt, dw = out[6]
-        cam_grads = (dR.reshape(sr), dt.reshape(st), dw.reshape(sw))
-    else:
-        cam_grads = (None, None, None)
     if need_map:
         dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = out[:6]
-        map_grads = (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus)
+        grads = (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus)
     else:
-        map_grads = (None,) * 6
-    return map_grads + cam_grads + (None,)
+        grads = (None,) * 6
+    if need_cam:
+        grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
+    elif pose:
+        grads += (None, None, None)
+    return grads + (None,)
 
 
 class GSFunctionFusedPose(torch.autograd.Function):
@@ -237,11 +207,11 @@ class GSFunctionFusedPose(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
-        return _pose_forward(ctx, False, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc))
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
-        return _pose_backward(ctx, False, dloss_dgammas)
+        return _fused_backward(ctx, False, True, dloss_dgammas)
 
 
 class GSFunctionFusedRGBDPose(torch.autograd.Function):
@@ -251,8 +221,8 @@ class GSFunctionFusedRGBDPose(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
-        return _pose_forward(ctx, True, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)
+        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc))
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
-        return _pose_backward(ctx, True, dloss_dgammas, dloss_ddepth, dloss_dalpha)
+        return _fused_backward(ctx, True, True, dloss_dgammas, dloss_ddepth, dloss_dalpha)

@@ -74,6 +74,25 @@ def _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc):
     return (pws, rots, scales, shs, Rcw, tcw, twc), N, k
 
 
+def _upstream_grads(N, ref, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds):
+    """Checks the upstream gradients the fused backward reads, float32 CUDA tensors on the device
+    of `ref`: moments[N,9] with the forward's cinv2ds[N,3] or, when moments is None, dloss_dus,
+    dloss_dcinv2ds, dloss_dcolors (2N, 3N, 3N elements, last dim 2, 3, 3).
+    -> (dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds), contiguous, the unused ones None"""
+    if moments is not None:
+        moments = _chk(moments, "moments", last=9, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
+        _same_device(ref, moments, cinv2ds)
+        if moments.shape[0] != N or cinv2ds.shape[0] != N:
+            raise ValueError("moments / cinv2ds must have N rows")
+        return None, None, None, moments, cinv2ds
+    gu = _chk(dloss_dus, "dloss_dus", last=2); gc = _chk(dloss_dcinv2ds, "dloss_dcinv2ds", last=3)
+    gcol = _chk(dloss_dcolors, "dloss_dcolors", last=3)
+    _same_device(ref, gu, gc, gcol)
+    if not (gu.numel() == 2 * N and gc.numel() == 3 * N and gcol.numel() == 3 * N):
+        raise ValueError("upstream gradients disagree on N")
+    return gu, gc, gcol, None, None
+
+
 def _ptr(t):
     return None if t is None else t.data_ptr()
 
@@ -524,18 +543,8 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     if camera_grad and compact:
         raise ValueError("camera_grad does not combine with compact")
     (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
-    if moments is not None:
-        moments = _chk(moments, "moments", last=9, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
-        _same_device(pws, moments, cinv2ds)
-        if moments.shape[0] != N or cinv2ds.shape[0] != N:
-            raise ValueError("moments / cinv2ds must have N rows")
-        gu = gc = gcol = None
-    else:
-        gu = _chk(dloss_dus, "dloss_dus", last=2); gc = _chk(dloss_dcinv2ds, "dloss_dcinv2ds", last=3)
-        gcol = _chk(dloss_dcolors, "dloss_dcolors", last=3)
-        _same_device(pws, gu, gc, gcol)
-        if not (gu.numel() == 2 * N and gc.numel() == 3 * N and gcol.numel() == 3 * N):
-            raise ValueError("preprocessB inputs disagree on N")
+    gu, gc, gcol, moments, cinv2ds = _upstream_grads(N, pws, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
+                                                     cinv2ds)
     if dloss_ddepths is not None:
         dloss_ddepths = _chk(dloss_ddepths, "dloss_ddepths")
         _same_device(pws, dloss_ddepths)

@@ -169,22 +169,21 @@ class GradExchange:
         `splatB(..., moments_only=True)`) + the forward's cinv2ds -- then this view's own
         dloss_dus[N,2] is returned (it is not part of the exchange)."""
         from . import _lib
-        from .ops import _chk, _gaussian_params, _ptr, _stream
+        from .ops import _chk, _gaussian_params, _ptr, _same_device, _stream, _upstream_grads
         (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, cam.Rcw, cam.tcw,
                                                                          cam.twc)
         if N != self.N or k != self.k3:
             raise ValueError("GradExchange was built for N=%d, sh_dim3=%d" % (self.N, self.k3))
-        gu = gc = gcol = ga = dus = None
+        gu, gc, gcol, moments, cinv2ds = _upstream_grads(N, pws, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
+                                                         cinv2ds)
+        ga = dus = None
         if moments is not None:
-            moments = _chk(moments, "moments", last=9, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
-            if moments.shape[0] != N or cinv2ds.shape[0] != N:
-                raise ValueError("moments / cinv2ds must have N rows")
             dus = torch.empty((N, 2), dtype=torch.float32, device=pws.device)
-        else:
-            gu = _chk(dloss_dus, "dloss_dus", last=2); gc = _chk(dloss_dcinv2ds, "dloss_dcinv2ds", last=3)
-            gcol = _chk(dloss_dcolors, "dloss_dcolors", last=3); ga = _chk(dloss_dalphas, "dloss_dalphas")
-            if ga.numel() != N or gu.numel() != 2 * N:
-                raise ValueError("upstream gradients disagree on N")
+        else:  # dL/dalpha goes into the exchange as it is
+            ga = _chk(dloss_dalphas, "dloss_dalphas")
+            _same_device(pws, ga)
+            if ga.numel() != N:
+                raise ValueError("dloss_dalphas must have N elements")
         self.epoch += 1
         with torch.cuda.device(pws.device):
             _lib.check(self.lib.gsb_preprocess_backward_push(

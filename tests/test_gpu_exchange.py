@@ -136,6 +136,14 @@ def test_exchange_argument_errors():
             with pytest.raises(ValueError):
                 ex.push(p["pws"], p["rots"], p["scales"], p["shs"],
                         Camera(64, 64, sc["fx"], sc["fy"], sc["cx"], sc["cy"], c["Rcw"], c["tcw"], c["twc"]), *ins)
+        # so are the upstream gradients: a dloss_dcinv2ds or dloss_dcolors with N - 1 rows (3N floats read)
+        for i in (1, 2):
+            short = list(ins)
+            short[i] = ins[i][:-1]
+            with pytest.raises(ValueError):
+                ex.push(P["pws"], P["rots"], P["scales"], P["shs"],
+                        Camera(64, 64, sc["fx"], sc["fy"], sc["cx"], sc["cy"], cam["Rcw"], cam["tcw"], cam["twc"]),
+                        *short)
         assert lib.gsb_profile_launches(-1) == launches
     finally:
         ex.close()
