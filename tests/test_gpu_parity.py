@@ -259,19 +259,25 @@ def op_inputs(parts):
     return f32(cols[0]), f32(cols[1]), f32(cols[2]), f32(cols[3]), f32(cols[4]), t(cols[5], torch.int32)
 
 
-def test_splat_patch_count_and_survivor_boundaries():
-    """Scenes built at the op surface so that every tile's patch count is exactly what was put
-    there: whole-tile entries (<= 32 patches) against four-entry tiles (>= 33) and the 32-record
-    chunk edges at 32/33, 64/65; 6-9 and 16-17 survivors in one 8x8 block (the backward's phase-B
-    flushes); opacities 0.99, nextafter(0.99, 1) and 1.0 at list positions 30-33 (above the clamp:
-    the backward's shuffle path); and near-opaque stacks whose last composited record is list
-    index 31, 32 or 33."""
-    rng = np.random.default_rng(7)
-    gx, parts, expect = 8, [], {}
+BOUNDARY_GX = 8  # tiles per row of boundary_scene's frame
+
+
+def boundary_scene(rng, z0s=None):
+    """Op-surface scene whose every tile's patch count is exactly what was put there: whole-tile
+    entries (<= 32 patches) against four-entry tiles (>= 33) and the 32-record chunk edges at
+    32/33, 64/65; 6-9 and 16-17 survivors in one 8x8 block (the backward's phase-B flushes);
+    opacities 0.99, nextafter(0.99, 1) and 1.0 at list positions 30-33 (above the clamp: the
+    backward's shuffle path); and near-opaque stacks whose last composited record is list index
+    31, 32 or 33.  z0s[i]: the depth offset of tile i (default 1.0 everywhere).  The frame is
+    BOUNDARY_GX tiles wide and as many rows high as the tiles need.
+    -> (parts, expect {tile: patches}, survivor_tiles {tile: survivors}, stack_tiles {tile: contrib})"""
+    gx, parts, expect = BOUNDARY_GX, [], {}
     tile = iter(range(1000))
 
     def add(k, **kw):
         i = next(tile)
+        if z0s is not None:
+            kw["z0"] = float(z0s[i])
         parts.append(gaussians_in_tile(i % gx, i // gx, k, rng, **kw))
         expect[i] = k
         return i, parts[-1]
@@ -295,7 +301,19 @@ def test_splat_patch_count_and_survivor_boundaries():
         i, p = add(40, sigma=(200.0, 200.0), alpha=(0.05, 0.05))
         p[2][m:] = 1.0
         stack_tiles[i] = m + 2
-    W, H = 16 * gx, 16 * ((len(expect) + gx - 1) // gx)
+    return parts, expect, survivor_tiles, stack_tiles
+
+
+def boundary_frame(expect):
+    """(W, H) of boundary_scene's frame"""
+    return 16 * BOUNDARY_GX, 16 * ((len(expect) + BOUNDARY_GX - 1) // BOUNDARY_GX)
+
+
+def test_splat_patch_count_and_survivor_boundaries():
+    """boundary_scene: patch counts, survivor blocks and stack contribs as built"""
+    gx = BOUNDARY_GX
+    parts, expect, survivor_tiles, stack_tiles = boundary_scene(np.random.default_rng(7))
+    W, H = boundary_frame(expect)
     (image, contrib, ftau, ranges, gsid), ref = check_splat_vs_oracle(H, W, *op_inputs(parts), seed=7)
     lens = ref["ranges"][:, 1] - ref["ranges"][:, 0]
     for i, k in expect.items():
@@ -311,15 +329,14 @@ def test_splat_patch_count_and_survivor_boundaries():
         assert (con[16 * (i // gx):16 * (i // gx) + 16, 16 * (i % gx):16 * (i % gx) + 16] == c).all(), i
 
 
-def test_splat_dead_sparse_tiles_and_64bit_keys():
-    """3840x2160 with 1-3 patches in every tile: the backward's whole-tile entries alternate between
-    live tiles and dead ones whose patches all have alpha 0.0015 (no pixel composites anything,
-    so all four blocks skip after the tile's record gather was issued), about ten entries per
-    resident warp in a row.  A tenth of the Gaussians sit near 1 km: depth keys of ~20 bits plus
-    15 tile bits need the 64-bit sort key layout."""
-    rng = np.random.default_rng(11)
-    W, H = 3840, 2160
-    gx, gy = W // 16, H // 16
+DEAD_W, DEAD_H = 3840, 2160
+
+
+def dead_sparse_scene(rng):
+    """3840x2160 with 1-3 patches in every tile; tile (tx, ty) with tx + ty odd is dead (alpha
+    0.0015 everywhere: nothing composites); a tenth of the tiles' Gaussians sit near 1 km.
+    -> parts, one per tile in row-major tile order"""
+    gx, gy = DEAD_W // 16, DEAD_H // 16
     parts = []
     for ty in range(gy):
         for tx in range(gx):
@@ -331,6 +348,18 @@ def test_splat_dead_sparse_tiles_and_64bit_keys():
     for p, f in zip(parts, far):
         if f:
             p[3][:] = rng.uniform(900.0, 1100.0) + 0.01 * np.arange(len(p[3]))
+    return parts
+
+
+def test_splat_dead_sparse_tiles_and_64bit_keys():
+    """3840x2160 with 1-3 patches in every tile: the backward's whole-tile entries alternate between
+    live tiles and dead ones whose patches all have alpha 0.0015 (no pixel composites anything,
+    so all four blocks skip after the tile's record gather was issued), about ten entries per
+    resident warp in a row.  A tenth of the Gaussians sit near 1 km: depth keys of ~20 bits plus
+    15 tile bits need the 64-bit sort key layout."""
+    W, H = DEAD_W, DEAD_H
+    gx, gy = W // 16, H // 16
+    parts = dead_sparse_scene(np.random.default_rng(11))
     (image, contrib, ftau, ranges, gsid), ref = check_splat_vs_oracle(H, W, *op_inputs(parts), seed=11)
     lens = ref["ranges"][:, 1] - ref["ranges"][:, 0]
     assert lens.min() >= 1 and lens.max() <= 3
@@ -343,31 +372,45 @@ def test_splat_dead_sparse_tiles_and_64bit_keys():
     assert depth_bits >= 20 and tile_bits == 15 and depth_bits + tile_bits > 32
 
 
-def test_splat_dense_early_termination():
-    """many opaque layers: every pixel reaches tau < 1e-4 long before the list ends, and a
-    tile's list spans several shared-memory batches"""
+def dense_scene():
+    """96x64, 6000 Gaussians of alpha 0.6-0.99 at three times the scale: many opaque layers"""
     W, H, N = 96, 64, 6000
     sc = synthetic_scene(N, W, H, sh_dim=3, seed=11)
     sc["alphas"][:] = np.random.default_rng(1).uniform(0.6, 0.99, N).astype(np.float32)
     sc["scales"] *= 3.0
+    return sc
+
+
+def test_splat_dense_early_termination():
+    """many opaque layers: every pixel reaches tau < 1e-4 long before the list ends, and a
+    tile's list spans several shared-memory batches"""
+    sc = dense_scene()
+    N, W, H = len(sc["pws"]), sc["width"], sc["height"]
     _, _, (image, contrib, ftau, ranges, gsid), ref = run_splat_case(N, W, H, sc=sc, seed=11)
     lens = ref["ranges"][:, 1] - ref["ranges"][:, 0]
     assert lens.max() > 300 and (ref["final_tau"] < 1e-4).mean() > 0.5
     assert ref["contrib"].max() < lens.max()
 
 
-def test_splat_alpha_clamp_and_tiny_alpha():
+def clamp_scene():
+    """80x80, 400 Gaussians: every third of opacity 1.0 (alpha' clamps at 0.99 near the centre,
+    kernel.cu:245), rows of 0.001 (can never reach 0.002) and of 0.002"""
     W, H, N = 80, 80, 400
     sc = synthetic_scene(N, W, H, sh_dim=3, seed=2)
-    sc["alphas"][::3] = 1.0          # alpha' clamps at 0.99 near the centre (kernel.cu:245)
-    sc["alphas"][1::7] = 0.001       # can never reach 0.002
+    sc["alphas"][::3] = 1.0
+    sc["alphas"][1::7] = 0.001
     sc["alphas"][2::11] = 0.002
-    run_splat_case(N, W, H, sc=sc, seed=2)
+    return sc
 
 
-def test_splat_huge_and_needle_gaussians():
-    """footprints covering hundreds of tiles, extreme anisotropy (needles at 45 degrees) and
-    Gaussians centred far outside the frame whose 3-sigma box still reaches it"""
+def test_splat_alpha_clamp_and_tiny_alpha():
+    sc = clamp_scene()
+    run_splat_case(len(sc["pws"]), sc["width"], sc["height"], sc=sc, seed=2)
+
+
+def huge_needle_scene():
+    """400x304, 3000 Gaussians: 40 with sigma up to ~200 px, 300 needles of 100:1 anisotropy and
+    100 centred off-screen with boxes that still reach the frame"""
     W, H, N = 400, 304, 3000
     sc = synthetic_scene(N, W, H, sh_dim=3, seed=13)
     rng = np.random.default_rng(13)
@@ -380,6 +423,14 @@ def test_splat_huge_and_needle_gaussians():
     sc["pws"][far, 0] *= 1.6                                                   # centres off-screen
     sc["scales"][far] *= 15.0
     sc["alphas"][big] = rng.uniform(0.02, 0.3, 40).astype(np.float32)
+    return sc
+
+
+def test_splat_huge_and_needle_gaussians():
+    """footprints covering hundreds of tiles, extreme anisotropy (needles at 45 degrees) and
+    Gaussians centred far outside the frame whose 3-sigma box still reaches it"""
+    sc = huge_needle_scene()
+    N, W, H = len(sc["pws"]), sc["width"], sc["height"]
     # Integer side (culls, ranges, patch order, contrib) stays bit-exact.  The float side gets
     # 20x the usual bound: along a 100:1 needle the terms a*dx^2, c*dy^2, 2b*dx*dy reach ~1e5
     # and cancel to O(10), so ANY fp32 evaluation (the reference's included) carries ~1e-2

@@ -48,9 +48,22 @@ def upstream(W, H, seed, zmax):
     return dl, dld, dla
 
 
-def check_rgbd(H, W, us_d, ci_d, al_d, d_d, col_d, ar_d, seed=0, records=None, capacity=False, tol_scale=1.0):
+def tile_zmax(H, W, ref):
+    """[H,W]: the largest |z| in the patch list of each pixel's tile (0 on empty tiles), from the
+    oracle forward's ranges / gsid / z"""
+    gx, gy = (W + 15) // 16, (H + 15) // 16
+    lens = ref["ranges"][:, 1] - ref["ranges"][:, 0]
+    zt = np.zeros(gx * gy)
+    np.maximum.at(zt, np.repeat(np.arange(gx * gy), lens), np.abs(ref["z"][ref["gsid"]]))
+    return np.repeat(np.repeat(zt.reshape(gy, gx), 16, axis=0), 16, axis=1)[:H, :W]
+
+
+def check_rgbd(H, W, us_d, ci_d, al_d, d_d, col_d, ar_d, seed=0, records=None, capacity=False, tol_scale=1.0,
+               tile_z=False):
     """splat_rgbd (+ splatB_rgbd) against splat / splatB and the oracle.  d_d / ar_d are culled
-    in place.  -> (the seven outputs, the oracle forward, the five gradients)"""
+    in place.  tile_z: D is bounded per pixel by the largest z of its own tile's list instead of
+    the frame's (for scenes whose depths span orders of magnitude).
+    -> (the seven outputs, the oracle forward, the five gradients)"""
     o = ops()
     us, ci, col, al = n(us_d), n(ci_d), n(col_d), n(al_d)
     d_in, a_in = n(d_d).copy(), n(ar_d).copy()
@@ -68,8 +81,13 @@ def check_rgbd(H, W, us_d, ci_d, al_d, d_d, col_d, ar_d, seed=0, records=None, c
     eA = np.abs(n(out[6]).astype(np.float64) - ref["alpha"])
     eD = np.abs(n(out[5]).astype(np.float64) - ref["depth"])
     assert eA[~amb].max(initial=0) <= 5e-5 * tol_scale, "alpha err %.3e" % eA[~amb].max()
-    assert eD[~amb].max(initial=0) <= 5e-5 * tol_scale * zmax, "depth err %.3e of %g" % (eD[~amb].max(), zmax)
-    assert eA.max(initial=0) <= 1e-2 and eD.max(initial=0) <= 1e-2 * zmax
+    if tile_z:
+        eD = eD / np.maximum(tile_zmax(H, W, ref), 1.0)
+        assert eD[~amb].max(initial=0) <= 5e-5 * tol_scale, "depth err %.3e of the tile's max z" % eD[~amb].max()
+        assert eA.max(initial=0) <= 1e-2 and eD.max(initial=0) <= 1e-2
+    else:
+        assert eD[~amb].max(initial=0) <= 5e-5 * tol_scale * zmax, "depth err %.3e of %g" % (eD[~amb].max(), zmax)
+        assert eA.max(initial=0) <= 1e-2 and eD.max(initial=0) <= 1e-2 * zmax
     # backward: all five per-Gaussian gradients against the oracle
     dl, dld, dla = upstream(W, H, seed, zmax)
     g5 = o.splatB_rgbd(H, W, us_d, ci_d, al_d, d_d, col_d, out[1], out[2], out[3], out[4], t(dl), t(dld), t(dla),
