@@ -51,6 +51,8 @@ SIGNATURES = {
     "gsb_splat_backward_rgbd": (_i, [_i, _i, _i, _i64] + [_vp] * 14 + [_sz] + [_vp] * 7),
     "gsb_preprocess_backward_pose_workspace_bytes": (_sz, [_i]),
     "gsb_preprocess_backward_pose": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 14 + [_sz, _vp]),
+    "gsb_preprocess_forward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 9),
+    "gsb_preprocess_backward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 15 + [_sz, _vp]),
     "gsb_sh_grad_expand": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gsb_small_bmm": (_i, [C.c_longlong, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "gsb_gau_loss_workspace_bytes": (_sz, [_i, _i]),

@@ -164,7 +164,24 @@ int gsb_preprocess_forward(int N, int sh_dim3, const float *pws, const float *ro
                          depths && areas),
               "preprocess: null pointer");
   return launch_preprocess_fwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records),
+                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), nullptr,
+                               (cudaStream_t)stream);
+}
+
+int gsb_preprocess_forward_aa(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                              const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                              float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
+                              float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
+                              float *alphas_eff, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0, "preprocess_aa: N < 0");
+  GSB_REQUIRE((reinterpret_cast<uintptr_t>(records) & 15) == 0, "preprocess_aa: records misaligned");
+  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
+              "preprocess_aa: shs.shape[1]/3 must be 1, 4, 9 or 16");
+  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && us && cinv2ds && colors &&
+                         depths && areas && alphas && alphas_eff),
+              "preprocess_aa: null pointer");
+  return launch_preprocess_fwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
+                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), alphas_eff,
                                (cudaStream_t)stream);
 }
 
@@ -232,7 +249,7 @@ static int preprocess_backward_impl(const char *who, int N, int sh_dim3, const f
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, nullptr,
+                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, nullptr, nullptr,
                                (cudaStream_t)stream);
 }
 
@@ -286,7 +303,38 @@ int gsb_preprocess_backward_pose(int N, int sh_dim3, const float *pws, const flo
   const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, &po,
+                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, &po, nullptr,
+                               (cudaStream_t)stream);
+}
+
+int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                               const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                               float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                               const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                               float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                               const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                               const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
+                               size_t ws_bytes, gsb_stream_t stream) {
+  const char *who = "preprocessB_aa";
+  const bool pose = dloss_dcamera != nullptr;
+  if (int rc = check_preprocess_backward(who, pose ? GradOutputs::kAllOrNone : GradOutputs::kAll, N, sh_dim3, pws,
+                                          rots, scales, shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors,
+                                          moments, cinv2ds, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots,
+                                          dloss_dus_out, dloss_dalphas_out))
+    return rc;
+  GSB_REQUIRE(N == 0 || moments != nullptr, "preprocessB_aa: antialiasing takes the moment rows");
+  GSB_REQUIRE(N == 0 || alphas != nullptr, "preprocessB_aa: null alphas");
+  if (pose) {
+    GSB_REQUIRE(aligned(ws, 16), "preprocessB_aa: workspace misaligned");
+    GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
+                "preprocessB_aa: workspace too small");
+  }
+  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
+  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
+  // (N == 0 launches no per-Gaussian pass: only the camera gradient's zeros, with dloss_dcamera)
+  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
+                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                               dloss_drots, nullptr, &mi, dloss_ddepths, pose ? &po : nullptr, alphas,
                                (cudaStream_t)stream);
 }
 
@@ -742,7 +790,7 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
   const MomentsIn mi{moments, cinv2ds, dloss_dus_out, nullptr};
   return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, nullptr, nullptr, nullptr, &gp,
-                               moments ? &mi : nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                               moments ? &mi : nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *const *regions_host, uint32_t epoch,

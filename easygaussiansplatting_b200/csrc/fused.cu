@@ -44,14 +44,17 @@ __device__ __forceinline__ void load_small_rows(const float *__restrict__ pws, c
   }
 }
 
-template <int K3>
+// AA = antialiasing (pg::aa_scale): alphas is read, alpha_eff = rho alpha goes to alphas_eff[N]
+// and into the record's alpha word (so its culling threshold follows); every other output is the
+// non-AA kernel's.
+template <int K3, bool AA>
 __global__ void __launch_bounds__(PG) k_preprocess_fwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
     const float *__restrict__ shs, const float *__restrict__ Rcw, const float *__restrict__ tcw,
     const float *__restrict__ twc, float fx, float fy, float cx, float cy, float tan_fovx, float tan_fovy,
     float *__restrict__ us, float *__restrict__ cinv2ds, float *__restrict__ colors,
     float *__restrict__ depths, int32_t *__restrict__ areas, const float *__restrict__ alphas,
-    Rec *__restrict__ recs) {
+    Rec *__restrict__ recs, float *__restrict__ alphas_eff) {
   constexpr int KS = 3 * K3;
   constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
   __shared__ float sm[SMF];
@@ -71,17 +74,22 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
   float u[2] = {0.f, 0.f}, conic[3] = {0.f, 0.f, 0.f}, col[3] = {0.f, 0.f, 0.f}, depth = -1.f;
   int area[2] = {0, 0};
   if (valid) {
-    pg::forward_one<K3>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
+    const float rho = pg::forward_one<K3, AA>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
     const long long i = base + tid;
     st_pair(us, i, u[0], u[1]);
     cinv2ds[3 * i] = conic[0]; cinv2ds[3 * i + 1] = conic[1]; cinv2ds[3 * i + 2] = conic[2];
     colors[3 * i] = col[0]; colors[3 * i + 1] = col[1]; colors[3 * i + 2] = col[2];
     st_pair(areas, i, area[0], area[1]);
     depths[i] = depth;
+    float al = 0.f;
+    if (AA) {
+      al = rho * __ldg(alphas + i);
+      alphas_eff[i] = al;
+    }
     // the rasterizers' per-Gaussian record, straight from registers (saves the k_pack pass)
     if (recs != nullptr)
-      recs[i] = build_record(u[0], u[1], conic[0], conic[1], conic[2], __ldg(alphas + i), col[0], col[1], col[2], depth,
-                             (int)i);
+      recs[i] = build_record(u[0], u[1], conic[0], conic[1], conic[2], AA ? al : __ldg(alphas + i), col[0], col[1],
+                             col[2], depth, (int)i);
   }
 }
 
@@ -104,7 +112,10 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
 // the SH tile flushed.  A caller that wants both runs the non-POSE form as well: the compiler
 // fuses multiply-adds differently in a kernel that also carries the camera terms, and the
 // per-Gaussian gradients have to be the same bits with and without the pose.
-template <int K3, bool PUSH, bool MOM, bool DEPTH, bool POSE>
+// AA = antialiasing (only with MOM, not with PUSH): the moment rows' dL/dalpha is dL/dalpha_eff of
+// the forward's alpha_eff = rho alpha; alphas (raw, 4 B/Gaussian) is read, dL/dalpha = rho m[5]
+// is written and alpha m[5] drho feeds the geometry (and camera) gradients (pg::backward_one).
+template <int K3, bool PUSH, bool MOM, bool DEPTH, bool POSE, bool AA>
 __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
     const float *__restrict__ shs, const float *__restrict__ Rcw, const float *__restrict__ tcw,
@@ -112,7 +123,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     const float *__restrict__ g_us, const float *__restrict__ g_cinv2ds, const float *__restrict__ g_colors,
     float *__restrict__ g_pws, float *__restrict__ g_shs, float *__restrict__ g_scales,
     float *__restrict__ g_rots, GradPush gp, MomentsIn mi, const float *__restrict__ g_depths,
-    float *__restrict__ pose_part) {
+    float *__restrict__ pose_part, const float *__restrict__ alphas) {
+  static_assert(!AA || (MOM && !PUSH), "antialiasing takes the moment rows and no exchange");
   constexpr int KS = 3 * K3;
   constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
   __shared__ float sm[SMF];
@@ -124,7 +136,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
   float gu[2] = {0.f, 0.f}, gci[3] = {0.f, 0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
   load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);  // see k_preprocess_fwd
-  float galpha = 0.f;
+  float galpha = 0.f, al = 0.f;
   if (MOM) {
     if (valid) {
       const long long i = base + tid;
@@ -139,8 +151,9 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
       gci[0] = -0.5f * m[2]; gci[1] = -m[3]; gci[2] = -0.5f * m[4];
       gcol[0] = m[6]; gcol[1] = m[7]; gcol[2] = m[8];
       galpha = m[5];
+      if (AA) al = __ldg(alphas + i);  // in flight with the moment row
       if (!POSE) st_pair(mi.dus_out, i, gu[0], gu[1]);
-      if (!POSE && mi.dalphas_out != nullptr) mi.dalphas_out[i] = galpha;
+      if (!POSE && !AA && mi.dalphas_out != nullptr) mi.dalphas_out[i] = galpha;  // AA: after the math
     }
   } else if (valid) {
     const long long i = base + tid;
@@ -159,7 +172,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     if (valid) {
       const float gz = DEPTH ? __ldg(g_depths + base + tid) : 0.f;
       float xpw[3], xq[4], xs[3], xsh[KS];  // the per-Gaussian outputs: not written by this form
-      pg::backward_one<K3, DEPTH, true>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam);
+      pg::backward_one<K3, DEPTH, true, AA>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam,
+                                            galpha, al);
     }
     __shared__ float red[PG / 32][16];
 #pragma unroll
@@ -183,12 +197,17 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     return;  // nothing per Gaussian leaves the CTA
   }
   // dL/dsh overwrites the thread's own SH row in place, then the tile is flushed
+  float gal = galpha;
   if (DEPTH) {
     const float gz = valid ? __ldg(g_depths + base + tid) : 0.f;
-    if (valid) pg::backward_one<K3, true>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), gz);
+    if (valid)
+      gal = pg::backward_one<K3, true, false, AA>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), gz,
+                                                  nullptr, galpha, al);
   } else if (valid) {
-    pg::backward_one<K3>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS));
+    gal = pg::backward_one<K3, false, false, AA>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), 0.f,
+                                                 nullptr, galpha, al);
   }
+  if (AA && valid && mi.dalphas_out != nullptr) mi.dalphas_out[base + tid] = gal;
   __syncthreads();
   long long drow = base;
   if (PUSH) {  // destination = slot `rank` on the owner of this tile, rows relative to its range
@@ -330,14 +349,20 @@ int launch_preprocess_fwd(int N, int k3, const float *pws, const float *rots, co
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
                           float *colors, float *depths, int32_t *areas, const float *alphas, Rec *recs,
-                          cudaStream_t st) {
+                          float *alphas_eff, cudaStream_t st) {
   if (N <= 0) return 0;
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = (N + PG - 1) / PG;
   ProfScope ps(K_PRE_FWD, st);
-  GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3><<<nb, PG, 0, st>>>(N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx,
-                                                                cy, tfx, tfy, us, cinv2ds, colors, depths, areas,
-                                                                alphas, recs)));
+  if (alphas_eff != nullptr) {
+    GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3, true><<<nb, PG, 0, st>>>(N, pws, rots, scales, shs, Rcw, tcw, twc, fx,
+                                                                        fy, cx, cy, tfx, tfy, us, cinv2ds, colors,
+                                                                        depths, areas, alphas, recs, alphas_eff)));
+  } else {
+    GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3, false><<<nb, PG, 0, st>>>(N, pws, rots, scales, shs, Rcw, tcw, twc, fx,
+                                                                         fy, cx, cy, tfx, tfy, us, cinv2ds, colors,
+                                                                         depths, areas, alphas, recs, nullptr)));
+  }
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -366,31 +391,35 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, const PoseOut *po, cudaStream_t st) {
+                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st) {
   if (N <= 0 && po == nullptr) return 0;
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = N > 0 ? (N + PG - 1) / PG : 0;
   const GradPush p = gp ? *gp : GradPush{};
   const MomentsIn m = mi ? *mi : MomentsIn{};
   float *part = po ? po->part : nullptr;
-  // one pass of k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE>, PUSH, MOM and DEPTH set by which optional
-  // inputs are given.  The exchange carries neither a depth nor a camera gradient, so no PUSH form
-  // with DEPTH or POSE exists (api.cu never asks for one).
+  // one pass of k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA>, PUSH, MOM, DEPTH and AA set by
+  // which optional inputs are given.  The exchange carries neither a depth nor a camera gradient,
+  // so no PUSH form with DEPTH or POSE exists (api.cu never asks for one); AA exists only with the
+  // moment rows and without the exchange.
   const auto pass = [&](auto pose) {
     return with_flags(
-        [&](auto push, auto mom, auto depth) -> int {
+        [&](auto push, auto mom, auto depth, auto aa) -> int {
           constexpr bool PUSH = decltype(push)::value, MOM = decltype(mom)::value, DEPTH = decltype(depth)::value,
-                         POSE = decltype(pose)::value;
+                         POSE = decltype(pose)::value, AA = decltype(aa)::value;
           if constexpr (PUSH && (DEPTH || POSE)) {
             return set_arg_error("preprocessB: no depth or camera gradient with the exchange");
+          } else if constexpr (AA && (PUSH || !MOM)) {
+            return set_arg_error("preprocessB: antialiasing needs the moment rows and no exchange");
           } else {
-            GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE><<<nb, PG, 0, st>>>(
+            GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA><<<nb, PG, 0, st>>>(
                                     N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us,
-                                    g_cinv2ds, g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part)));
+                                    g_cinv2ds, g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part,
+                                    alphas)));
             return 0;
           }
         },
-        gp != nullptr, mi != nullptr, g_depths != nullptr);
+        gp != nullptr, mi != nullptr, g_depths != nullptr, alphas != nullptr);
   };
   ProfScope ps(K_PRE_BWD, st);
   // the camera gradient first; then, unless g_pws is NULL (pose only), the per-Gaussian gradients

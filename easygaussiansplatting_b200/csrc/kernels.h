@@ -43,7 +43,8 @@ int launch_preprocess_fwd(int N, int k3, const float *pws, const float *rots, co
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
                           float *colors, float *depths, int32_t *areas, const float *alphas, Rec *recs,
-                          cudaStream_t st);
+                          float *alphas_eff, cudaStream_t st);
+// alphas_eff: NULL, or antialiasing (alphas required): alphas_eff[N] = rho alpha, also in recs
 // upstream gradients given as the rasterizer backward's moment rows (fused.cu, MOM variants)
 struct MomentsIn {
   const float *moments;  // [N,9]
@@ -64,13 +65,15 @@ constexpr size_t pose_workspace_bytes(int N) { return N > 0 ? (size_t)((N + 127)
 // are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.  g_depths: NULL, or dL/dz[N]
 // of the RGB-D rasterizer (not with gp).  po: NULL, or also the camera gradient (not with gp; a
 // pass of its own); then g_pws == NULL (with g_shs, g_scales, g_rots and mi's outputs NULL) writes
-// only that.  The arguments are checked by the entry points (api.cu check_preprocess_backward).
+// only that.  alphas: NULL, or antialiasing (the raw opacities; only with mi, not with gp): the
+// moment rows' dL/dalpha is dL/dalpha_eff.  The arguments are checked by the entry points (api.cu
+// check_preprocess_backward).
 int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, const PoseOut *po, cudaStream_t st);
+                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,

@@ -35,6 +35,7 @@ struct Cam {
 };
 
 constexpr float kMinDepth = 0.2f;  // kernel.cu:10: (float)z < 0.2 (double)  <=>  z < 0.2f
+constexpr float kBlur = 0.3f;      // the low-pass filter the reference adds to every cov2d
 
 // camera transform pc = Rcw pw + tcw; false when the Gaussian is nearer than kMinDepth (culled)
 GSB_HD bool camera_point(const float R[9], const float t[3], const float pw[3], float pc[3]) {
@@ -76,6 +77,7 @@ struct Cov2d {
   float M[6];    // J Rcw (2x3)
   float MS[6];   // M Sigma
   float c2[3];   // cov2d (a, b, c) with the +0.3 blur
+  float raw[2];  // its diagonal (a, c) before the blur (antialiasing only; dead code otherwise)
 };
 
 GSB_HD void cov2d(const float pc[3], bool keep, const float S6[6], const float R[9], float fx, float fy,
@@ -97,9 +99,28 @@ GSB_HD void cov2d(const float pc[3], bool keep, const float S6[6], const float R
   for (int a = 0; a < 2; a++)
     for (int c = 0; c < 3; c++)
       o.MS[3 * a + c] = o.M[3 * a] * S[c] + o.M[3 * a + 1] * S[3 + c] + o.M[3 * a + 2] * S[6 + c];
-  o.c2[0] = o.MS[0] * o.M[0] + o.MS[1] * o.M[1] + o.MS[2] * o.M[2] + 0.3f;
+  o.c2[0] = o.MS[0] * o.M[0] + o.MS[1] * o.M[1] + o.MS[2] * o.M[2] + kBlur;
   o.c2[1] = o.MS[0] * o.M[3] + o.MS[1] * o.M[4] + o.MS[2] * o.M[5];
-  o.c2[2] = o.MS[3] * o.M[3] + o.MS[4] * o.M[4] + o.MS[5] * o.M[5] + 0.3f;
+  o.c2[2] = o.MS[3] * o.M[3] + o.MS[4] * o.M[4] + o.MS[5] * o.M[5] + kBlur;
+  // the same sums without the blur, after c2 so that code which never reads them compiles as before
+  o.raw[0] = o.MS[0] * o.M[0] + o.MS[1] * o.M[1] + o.MS[2] * o.M[2];
+  o.raw[1] = o.MS[3] * o.M[3] + o.MS[4] * o.M[4] + o.MS[5] * o.M[5];
+}
+
+// Antialiasing (2D-filter opacity compensation, Mip-Splatting; gsplat's rasterize_mode
+// "antialiased"): the blur spreads a Gaussian's mass, so its opacity is scaled by
+//   rho = sqrt(max(kAaMinR, r)),  r = det(Sigma) / det(Sigma + kBlur I) = (a c - b^2) di
+// with (a, b, c) the pre-blur cov2d and di = 1 / det of the blurred one (conic()).  r is the
+// ratio the rasterizers would otherwise over-draw a sub-pixel Gaussian by.
+constexpr float kAaMinR = 2.5e-5f;
+GSB_HD void aa_scale(float a, float b, float c, float di, float &rho, float &r) {
+  r = (a * c - b * b) * di;
+  const float x = fmaxf(kAaMinR, r);
+#ifdef __CUDA_ARCH__
+  rho = x * rsqrtf(x);  // x >= kAaMinR is a normal number: no slow-path call (and no stack frame)
+#else
+  rho = sqrtf(x);
+#endif
 }
 
 // conic = cov2d^-1 with di = 1/det; false when di is NaN: such a Gaussian is culled (kernel.cu:301-305)
@@ -183,10 +204,11 @@ GSB_HD void geometry(const float pw[3], const float q[4], const float s[3], cons
   if (!conic(g.c2, g.di, g.cn)) g.keep = false;
 }
 
-// forward outputs for one Gaussian
-template <int K3>
-GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], const float *sh /*[K3][3]*/,
-                        const Cam &cam, float u[2], float cn[3], float col[3], float *depth, int area[2]) {
+// forward outputs for one Gaussian.  Returns rho (aa_scale) with AA, 1 without or when culled:
+// the caller composites rho * alpha.  Every output is the same with and without AA.
+template <int K3, bool AA = false>
+GSB_HD float forward_one(const float pw[3], const float q[4], const float s[3], const float *sh /*[K3][3]*/,
+                         const Cam &cam, float u[2], float cn[3], float col[3], float *depth, int area[2]) {
   Geo g;
   geometry(pw, q, s, cam, g);
   // colour is not gated by depth in the reference (kernel.cu:619-726)
@@ -202,12 +224,18 @@ GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], c
     cn[0] = cn[1] = cn[2] = 0.f;
     area[0] = area[1] = 0;
     *depth = -1.0f;
-    return;
+    return 1.f;
   }
   project_mean(g.pc, g.zi, cam.fx, cam.fy, cam.cx, cam.cy, u);
   cn[0] = g.cn[0]; cn[1] = g.cn[1]; cn[2] = g.cn[2];
   radius(g.c2, area);
   *depth = g.pc[2];
+  float rho = 1.f;
+  if (AA) {
+    float r;
+    aa_scale(g.raw[0], g.c2[1], g.raw[1], g.di, rho, r);
+  }
+  return rho;
 }
 
 // backward for one Gaussian.  gu[2], gconic[3], gcol[3] are the splatB outputs for it.
@@ -219,11 +247,18 @@ GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], c
 //   dL/dtwc = -(colour part of dL/dpw)  (the view direction is pw - twc).
 // gpc is the vector rotated into dL/dpw (x, y taken as unclamped, as above); a culled Gaussian
 // contributes through its colour branch only, as it does to dL/dpw.
-template <int K3, bool DEPTH = false, bool POSE = false>
-GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], const float *sh,
-                         const Cam &cam, const float gu[2], const float gconic[3], const float gcol[3],
-                         float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f,
-                         float *gcam = nullptr /*[15], POSE only*/) {
+// AA: the rasterizers composited alpha_eff = rho alpha (forward_one<K3, true>); galpha =
+// dL/dalpha_eff, alpha the raw opacity.  Returns dL/dalpha = rho galpha (galpha without AA) and
+// adds alpha galpha drho/d(a, b, c) to dL/dcov2d, from where it reaches every geometry gradient
+// (and gcam) like the conic's.  With w = kBlur, D = 1/di = det of the blurred cov2d (a', b, c'):
+//   dr/da = w (c c' + b^2) di^2,  dr/db = -2 w b (w + a + c) di^2,  dr/dc = w (a a' + b^2) di^2,
+// drho = dr / (2 rho), and 0 where the clamp holds (r <= kAaMinR).  galpha != 0 alone makes the
+// Gaussian's geometry gradient non-zero, so it joins the zero-gradient gate.
+template <int K3, bool DEPTH = false, bool POSE = false, bool AA = false>
+GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3], const float *sh,
+                          const Cam &cam, const float gu[2], const float gconic[3], const float gcol[3],
+                          float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f,
+                          float *gcam = nullptr /*[15], POSE only*/, float galpha = 0.f, float alpha = 0.f) {
   // ---- colour branch (independent of the depth cull, like sh2Color)
   float Y[K3], dY[K3][3];
   float d[3], ninv = 1.f, r[3] = {0.f, 0.f, 0.f};
@@ -257,13 +292,32 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
   Geo g;
   geometry(pw, q, s, cam, g);
   const bool any = (gu[0] != 0.f) || (gu[1] != 0.f) || (gconic[0] != 0.f) || (gconic[1] != 0.f) || (gconic[2] != 0.f) ||
-                   (DEPTH && gdepth != 0.f);
-  if (!g.keep || !any) return;
+                   (DEPTH && gdepth != 0.f) || (AA && galpha != 0.f);
+  if (!g.keep || !any) return galpha;  // rho = 1 when culled; rho * 0 otherwise
   const float a = g.c2[0], b = g.c2[1], c = g.c2[2], di = g.di, d2 = di * di;
   // dL/dcov2d = dL/dconic . dconic/dcov2d   (B.5.3)
-  const float ga = gconic[0] * (-c * c * d2) + gconic[1] * (b * c * d2) + gconic[2] * (di - a * c * d2);
-  const float gb = gconic[0] * (2.f * b * c * d2) + gconic[1] * (-di - 2.f * b * b * d2) + gconic[2] * (2.f * a * b * d2);
-  const float gc = gconic[0] * (di - a * c * d2) + gconic[1] * (a * b * d2) + gconic[2] * (-a * a * d2);
+  float ga = gconic[0] * (-c * c * d2) + gconic[1] * (b * c * d2) + gconic[2] * (di - a * c * d2);
+  float gb = gconic[0] * (2.f * b * c * d2) + gconic[1] * (-di - 2.f * b * b * d2) + gconic[2] * (2.f * a * b * d2);
+  float gc = gconic[0] * (di - a * c * d2) + gconic[1] * (a * b * d2) + gconic[2] * (-a * a * d2);
+  float galpha_raw = galpha;
+  if (AA) {
+    const float ar = g.raw[0], cr = g.raw[1];
+    float rho, r;
+    aa_scale(ar, b, cr, di, rho, r);
+    galpha_raw = rho * galpha;
+    if (r > kAaMinR) {
+      // drho/dr = 1 / (2 rho), rho in [0.005, 1]: the fast division is exact to 2 ulp there and
+      // adds no slow-path call (whose register saves cost the K3 = 16 kernel a stack frame)
+#ifdef __CUDA_ARCH__
+      const float k = alpha * galpha * (kBlur * d2) * __fdividef(0.5f, rho);
+#else
+      const float k = alpha * galpha * (kBlur * d2) * (0.5f / rho);
+#endif
+      ga += k * (cr * c + b * b);
+      gb += k * (-2.f * b * (kBlur + ar + cr));
+      gc += k * (ar * a + b * b);
+    }
+  }
   // G = [[ga, gb/2], [gb/2, gc]]
   const float G00 = ga, G01 = 0.5f * gb, G11 = gc;
   const float *M = g.M;
@@ -334,6 +388,7 @@ GSB_HD void backward_one(const float pw[3], const float q[4], const float s[3], 
   gq[1] = 2.f * (y * dR[1] + z * dR[2] + y * dR[3] - 2.f * x * dR[4] - w * dR[5] + z * dR[6] + w * dR[7] - 2.f * x * dR[8]);
   gq[2] = 2.f * (-2.f * y * dR[0] + x * dR[1] + w * dR[2] + x * dR[3] + z * dR[5] - w * dR[6] + z * dR[7] - 2.f * y * dR[8]);
   gq[3] = 2.f * (-2.f * z * dR[0] - w * dR[1] + x * dR[2] + w * dR[3] - 2.f * z * dR[4] + y * dR[5] + x * dR[6] + y * dR[7]);
+  return galpha_raw;
 }
 
 }  // namespace pg

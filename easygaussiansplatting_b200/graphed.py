@@ -12,6 +12,9 @@ static buffers:
     step.dloss_dimage.copy_(...)           # the loss lives between the two graphs
     grads = step.backward()                # dict dpws dshs dalphas dscales drots dus (static tensors)
 
+With cam.antialiased the captured frame composites alpha_eff = rho * alpha (ops.preprocess) and the
+backward returns dL/dalpha of the raw alphas; binning, hence the captured capacities, is the same.
+
 The parameters are captured by address: an optimizer that updates them in place is seen by the
 next replay.  `forward()`'s outputs are validated lazily: `backward()` (or `check()`) reads the
 binning status of the frame; a frame that outgrew the captured capacities raises `CapacityError`
@@ -46,25 +49,28 @@ class GraphedFusedStep:
 
     def _forward_body(self):
         cam, p = self.cam, self.p
-        us, ci, col, dep, ar, rec = ops.preprocess(p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc,
-                                                   cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height,
-                                                   alphas=p["alphas"])
+        aa = bool(getattr(cam, "antialiased", False))
+        pre = ops.preprocess(p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
+                             cam.cx, cam.cy, cam.width, cam.height, alphas=p["alphas"], antialiased=aa)
+        us, ci, col, dep, ar, rec = pre[:6]
+        drawn = pre[6] if aa else p["alphas"]  # antialiased: the rasterizers composite alpha_eff
         _, self._keep, (image, contrib, final_tau, ranges, gsid) = ops._capacity_frame(
-            cam.height, cam.width, us, ci, p["alphas"], dep, col, ar, rec, self.P_cap, self.dk_cap, self.status,
+            cam.height, cam.width, us, ci, drawn, dep, col, ar, rec, self.P_cap, self.dk_cap, self.status,
             enqueue=True)
         self._fwd = dict(us=us, cinv2ds=ci, colors=col, depths=dep, areas=ar, records=rec, contrib=contrib,
-                         final_tau=final_tau, ranges=ranges, gsid=gsid)
+                         final_tau=final_tau, ranges=ranges, gsid=gsid, alphas=drawn, aa=aa)
         self.image = image
 
     def _backward_body(self):
         cam, p, f = self.cam, self.p, self._fwd
         # all P_cap patch slots: the replay's patch count is only known on the device
-        moments = ops.splatB(cam.height, cam.width, f["us"], f["cinv2ds"], p["alphas"], f["depths"], f["colors"],
+        moments = ops.splatB(cam.height, cam.width, f["us"], f["cinv2ds"], f["alphas"], f["depths"], f["colors"],
                              f["contrib"], f["final_tau"], f["ranges"], f["gsid"], self.dloss_dimage,
                              moments_only=True, records=f["records"])
         gpw, gsh, gs, gq, dus, dal = ops.preprocessB(
             p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=f["cinv2ds"])
+            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=f["cinv2ds"], antialiased=f["aa"],
+            alphas=p["alphas"] if f["aa"] else None)
         self._keep_b = moments
         self.grads = dict(dpws=gpw, dshs=gsh, dscales=gs, drots=gq, dalphas=dal, dus=dus)
 

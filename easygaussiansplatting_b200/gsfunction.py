@@ -10,13 +10,16 @@ import torch
 
 
 class Camera:
-    """Fields of gsplat/gausplat_dataset.py:14-27 that the rasterizer reads."""
+    """Fields of gsplat/gausplat_dataset.py:14-27 that the rasterizer reads.  antialiased (an
+    extension, read by the fused classes, GraphedFusedStep and MultiViewStep): render with the
+    2D-filter opacity compensation, alpha_eff = rho * alpha (ops.preprocess)."""
 
-    def __init__(self, width, height, fx, fy, cx, cy, Rcw, tcw, twc=None):
+    def __init__(self, width, height, fx, fy, cx, cy, Rcw, tcw, twc=None, antialiased=False):
         self.width, self.height = int(width), int(height)
         self.fx, self.fy, self.cx, self.cy = float(fx), float(fy), float(cx), float(cy)
         self.Rcw, self.tcw = Rcw, tcw
         self.twc = twc if twc is not None else -torch.linalg.inv(Rcw) @ tcw
+        self.antialiased = bool(antialiased)
 
 
 def build_gsfunction(gsc):
@@ -39,6 +42,8 @@ def build_gsfunction(gsc):
 class _Impl:
     @staticmethod
     def forward(gsc, ctx, pws, shs, alphas, scales, rots, us, cam):
+        if getattr(cam, "antialiased", False):
+            raise ValueError("GSFunction (the seven-operator surface) has no antialiased mode: use GSFunctionFused")
         us, pcs, depths, du_dpcs = gsc.project(pws, cam.Rcw, cam.tcw, cam.fx, cam.fy, cam.cx, cam.cy, True)
         cov3ds, dcov3d_drots, dcov3d_dscales = gsc.computeCov3D(rots, scales, depths, True)
         cov2ds, dcov2d_dcov3ds, dcov2d_dpcs = gsc.computeCov2D(
@@ -124,23 +129,30 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
 
 def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None):
     """The forward of the four fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
-    camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward."""
+    camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward.
+    cam.antialiased (absent: False): the rasterizers composite alpha_eff = rho * alpha."""
     from . import ops
+    aa = bool(getattr(cam, "antialiased", False))
     if pose is None:
         Rcw, tcw, twc = cam.Rcw, cam.tcw, cam.twc
+        if aa and not rgbd and getattr(cam, "grad_exchange", None) is not None:
+            raise ValueError("the gradient exchange has no antialiased form: cam.grad_exchange must not be set")
     else:
         if getattr(cam, "grad_exchange", None) is not None:
             raise ValueError("camera gradients are single-view: cam.grad_exchange must not be set")
         Rcw, tcw, twc = (x.detach() for x in pose)
     # the per-Gaussian records of the rasterizers come straight out of the fused forward (with z in
     # their depth word, as the RGB-D rasterizer needs)
-    us, cinv2ds, colors, depths, areas, records = ops.preprocess(
-        pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height, alphas=alphas)
+    pre = ops.preprocess(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
+                         cam.height, alphas=alphas, antialiased=aa)
+    us, cinv2ds, colors, depths, areas, records = pre[:6]
+    drawn = pre[6] if aa else alphas  # the opacities the rasterizers composite
     splat = ops.splat_rgbd if rgbd else ops.splat
-    out = splat(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, areas, records=records, capacity=True)
+    out = splat(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, areas, records=records, capacity=True)
     ctx.cam = cam
+    ctx.aa = aa
     ctx.alpha_shape = alphas.shape
-    saved = (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, *out[1:5])
+    saved = (pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths, colors, *out[1:5])
     if pose is not None:
         ctx.cam_shapes = (Rcw.shape, tcw.shape, twc.shape)
         saved += (Rcw, tcw, twc)
@@ -155,21 +167,22 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
     ctx.needs_input_grad: the pose alone takes the pose-only kernel (a frozen map: tracking)."""
     from . import ops
     cam = ctx.cam
-    (pws, shs, alphas, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau, patch_range_per_tile,
+    (pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau, patch_range_per_tile,
      gsid_per_patch, *cam_saved) = ctx.saved_tensors
     Rcw, tcw, twc = cam_saved if pose else (cam.Rcw, cam.tcw, cam.twc)
     need_map = any(ctx.needs_input_grad[:6])
     need_cam = pose and any(ctx.needs_input_grad[6:9])
     # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward converts
     # them in registers (no finalize pass, no 32 B/Gaussian round trip).  (autograd hands zeros for
-    # an RGB-D output the loss does not use: all three planes are given)
+    # an RGB-D output the loss does not use: all three planes are given)  With antialiasing the
+    # rasterizer replays alpha_eff (`drawn`), and the per-Gaussian backward takes the raw alphas.
     ddepths = None
     if rgbd:
-        moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib,
+        moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib,
                                            final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas,
                                            dloss_ddepth, dloss_dalpha, moments_only=True)
     else:
-        moments = ops.splatB(cam.height, cam.width, us, cinv2ds, alphas, depths, colors, contrib, final_tau,
+        moments = ops.splatB(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True)
     ex = None if rgbd or pose else getattr(cam, "grad_exchange", None)
     if ex is not None:
@@ -183,7 +196,8 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
                 g["dscales"].clone(), g["drots"].clone(), g["dus"], None)
     out = ops.preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
                           cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths,
-                          camera_grad=need_cam, pose_only=need_cam and not need_map)
+                          camera_grad=need_cam, pose_only=need_cam and not need_map, antialiased=ctx.aa,
+                          alphas=alphas if ctx.aa else None)
     if need_map:
         dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = out[:6]
         grads = (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus)

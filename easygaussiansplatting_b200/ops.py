@@ -496,33 +496,44 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
 # ---------------------------------------------------------------------------------------
 # Extensions (not in the reference module): the fused per-Gaussian path, SURVEY 8f row N1.
 def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
-               alphas=None):
+               alphas=None, antialiased=False):
     """project + computeCov3D + computeCov2D + sh2Color + inverseCov2D (calc_J=False) in one
     kernel.  -> [us[N,2], cinv2ds[N,3], colors[N,3], depths[N], areas[N,2] int32], ready for
     `splat`.  With alphas[N] a sixth output: the packed per-Gaussian records [N,12] for
-    `splat(..., records=...)`."""
+    `splat(..., records=...)`.
+    antialiased (alphas required): a seventh output alphas_eff[N] = rho * alphas, the opacity
+    scaled by how much the 0.3 px blur spread each Gaussian (gsb_preprocess_forward_aa); the records
+    carry it.  Render with alphas_eff; the other outputs are the same bits as without."""
     (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    if antialiased and alphas is None:
+        raise ValueError("antialiased=True needs alphas")
     o = dict(dtype=torch.float32, device=pws.device)
     us = torch.empty((N, 2), **o); cinv = torch.empty((N, 3), **o); col = torch.empty((N, 3), **o)
     depths = torch.empty((N,), **o); areas = torch.empty((N, 2), dtype=torch.int32, device=pws.device)
     records = None
     if alphas is not None:
         alphas = _chk(alphas, "alphas")
+        if antialiased:
+            _same_device(pws, alphas)
         if alphas.numel() != N:
             raise ValueError("alphas must have N elements")
         records = torch.empty((N, 12), **o)
     lib = _L()
     with torch.cuda.device(pws.device):
-        _lib.check(lib.gsb_preprocess_forward(
-            N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
-            float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
-            _ptr(us), _ptr(cinv), _ptr(col), _ptr(depths), _ptr(areas), _ptr(alphas), _ptr(records), _stream()), lib)
+        args = (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
+                float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
+                _ptr(us), _ptr(cinv), _ptr(col), _ptr(depths), _ptr(areas), _ptr(alphas), _ptr(records))
+        if antialiased:
+            alphas_eff = torch.empty((N,), **o)
+            _lib.check(lib.gsb_preprocess_forward_aa(*args, _ptr(alphas_eff), _stream()), lib)
+            return [us, cinv, col, depths, areas, records, alphas_eff]
+        _lib.check(lib.gsb_preprocess_forward(*args, _stream()), lib)
     return [us, cinv, col, depths, areas] + ([records] if records is not None else [])
 
 
 def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
                 dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False,
-                dloss_ddepths=None, camera_grad=False, pose_only=False):
+                dloss_ddepths=None, camera_grad=False, pose_only=False, antialiased=False, alphas=None):
     """Vector-Jacobian products of the five per-Gaussian stages (== the torch.bmm chain of
     gsmodel.py:72-85).  -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4]]
     With moments[N,9] (from `splatB(..., moments_only=True)`) and the forward's cinv2ds[N,3] the
@@ -537,14 +548,26 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     views of one 15-float tensor, summed over the Gaussians in a fixed order (gsb_preprocess_backward_pose;
     Rcw, tcw, twc taken as independent inputs).  The per-Gaussian outputs are the same bits as
     without it.  pose_only (with camera_grad): the map is frozen; the per-Gaussian gradients
-    (and dloss_dus, dloss_dalphas) are not computed and come back as None."""
+    (and dloss_dus, dloss_dalphas) are not computed and come back as None.
+    antialiased (with moments and the raw alphas[N]): the frame was rendered with
+    `preprocess(..., antialiased=True)`'s alphas_eff, so the moment rows' dL/dalpha is dL/dalphas_eff;
+    dloss_dalphas = rho * dL/dalphas_eff and the geometry (and camera) gradients gain the term
+    through rho (gsb_preprocess_backward_aa).  Combines with compact, dloss_ddepths, camera_grad
+    and pose_only."""
     if pose_only and not camera_grad:
         raise ValueError("pose_only=True needs camera_grad=True")
     if camera_grad and compact:
         raise ValueError("camera_grad does not combine with compact")
+    if antialiased and (moments is None or alphas is None):
+        raise ValueError("antialiased=True needs the moment rows and alphas")
     (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     gu, gc, gcol, moments, cinv2ds = _upstream_grads(N, pws, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
                                                      cinv2ds)
+    if antialiased:
+        alphas = _chk(alphas, "alphas")
+        _same_device(pws, alphas)
+        if alphas.numel() != N:
+            raise ValueError("alphas must have N elements")
     if dloss_ddepths is not None:
         dloss_ddepths = _chk(dloss_ddepths, "dloss_ddepths")
         _same_device(pws, dloss_ddepths)
@@ -580,10 +603,16 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
                 float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
                 _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(moments), _ptr(cinv2ds),
                 _ptr(dus), _ptr(dal))
+        gcam = ws = None
+        ws_bytes = 0
         if camera_grad:
             gcam = torch.empty((15,), **o)
             ws_bytes = int(lib.gsb_preprocess_backward_pose_workspace_bytes(N))
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
+        if antialiased:
+            _lib.check(lib.gsb_preprocess_backward_aa(*args, _ptr(dloss_ddepths), _ptr(alphas), _ptr(gcam), _ptr(ws),
+                                                      ws_bytes, _stream()), lib)
+        elif camera_grad:
             _lib.check(lib.gsb_preprocess_backward_pose(*args, _ptr(dloss_ddepths), _ptr(gcam), _ptr(ws), ws_bytes,
                                                         _stream()), lib)
         elif dloss_ddepths is not None:

@@ -170,6 +170,8 @@ class GradExchange:
         dloss_dus[N,2] is returned (it is not part of the exchange)."""
         from . import _lib
         from .ops import _chk, _gaussian_params, _ptr, _same_device, _stream, _upstream_grads
+        if getattr(cam, "antialiased", False):
+            raise ValueError("GradExchange has no antialiased form (cam.antialiased): use MultiViewStep")
         (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, cam.Rcw, cam.tcw,
                                                                          cam.twc)
         if N != self.N or k != self.k3:
@@ -262,19 +264,22 @@ class MultiViewStep:
 
     def render(self, cam):
         from . import ops
-        us, cinv2ds, colors, depths, areas, records = ops.preprocess(
-            self.pws, self.rots, self.scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, alphas=self.alphas)
-        image, contrib, final_tau, ranges, gsid = ops.splat(cam.height, cam.width, us, cinv2ds, self.alphas, depths,
+        aa = bool(getattr(cam, "antialiased", False))
+        pre = ops.preprocess(self.pws, self.rots, self.scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
+                             cam.cx, cam.cy, cam.width, cam.height, alphas=self.alphas, antialiased=aa)
+        us, cinv2ds, colors, depths, areas, records = pre[:6]
+        drawn = pre[6] if aa else self.alphas  # antialiased: the rasterizers composite alpha_eff
+        image, contrib, final_tau, ranges, gsid = ops.splat(cam.height, cam.width, us, cinv2ds, drawn, depths,
                                                             colors, areas, records=records, capacity=True)
-        return image, (cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid)
+        return image, (cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid, drawn)
 
     def backward(self, ctx, dloss_dimage, last=False):
         """last=True (the rank's final view of the step): the all-gather of the views' dL/dcolor
         starts here, right after the rasterizer backward, and runs under the per-Gaussian backward."""
         from . import ops
-        cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid = ctx
-        moments = ops.splatB(cam.height, cam.width, us, cinv2ds, self.alphas, depths, colors, contrib, final_tau,
+        cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid, drawn = ctx
+        aa = bool(getattr(cam, "antialiased", False))
+        moments = ops.splatB(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
                              ranges, gsid, dloss_dimage, moments_only=True)
         self._colors.append(moments[:, 6:9])          # dL/dcolor of this view
         self._twcs.append(cam.twc.reshape(1, 3))
@@ -282,7 +287,8 @@ class MultiViewStep:
             self._early = _start_gathers(torch.stack(self._colors), torch.cat(self._twcs).contiguous(), self.group)
         gpw, _, gs, gq, dus, dal = ops.preprocessB(
             self.pws, self.rots, self.scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
-            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, compact=True)
+            cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, compact=True, antialiased=aa,
+            alphas=self.alphas if aa else None)
         bucket = torch.as_strided(gpw, (gpw.shape[0] * 11,), (1,), gpw.storage_offset())  # [dpws|dscales|drots|dalphas]
         self._small = bucket if self._small is None else self._small.add_(bucket)
         self._dus.append(dus)

@@ -152,6 +152,35 @@ int gsb_preprocess_backward_pose(int N, int sh_dim3, const float *pws, const flo
                                  const float *dloss_ddepths, float *dloss_dcamera, void *ws, size_t ws_bytes,
                                  gsb_stream_t stream);
 
+/* Antialiasing (extension; the 2D-filter opacity compensation of Mip-Splatting, gsplat's
+ * rasterize_mode="antialiased").  The rasterizers keep drawing cov2d + 0.3 I, and each Gaussian's
+ * opacity is scaled by how much that blur spread it:
+ *     r = det(cov2d) / det(cov2d + 0.3 I)  (pre-blur over blurred),  rho = sqrt(max(2.5e-5, r)),
+ *     alpha_eff = rho * alpha               (rho = 1 for a culled Gaussian).
+ * gsb_preprocess_forward_aa: gsb_preprocess_forward's arguments with alphas required, plus
+ * alphas_eff[N] (output).  The records (optional) carry alpha_eff; every other output is
+ * bit-identical to gsb_preprocess_forward's.  Render with alphas_eff.
+ * gsb_preprocess_backward_aa: gsb_preprocess_backward_pose's arguments plus the raw alphas[N];
+ * the moment rows are required (they come from a splat backward run on alphas_eff, so their
+ * dL/dalpha is dL/dalpha_eff).  dloss_dalphas_out = rho dL/dalpha_eff, and alpha dL/dalpha_eff
+ * drho/dcov2d joins the geometry gradients (0 where the 2.5e-5 clamp holds).  dloss_ddepths
+ * may be NULL (colour only); dloss_dcamera NULL (ws ignored) is the plain or (dloss_dshs NULL)
+ * compact call, otherwise the camera gradient as in gsb_preprocess_backward_pose, with the
+ * per-Gaussian outputs all set or all NULL (pose only). */
+int gsb_preprocess_forward_aa(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                              const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                              float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
+                              float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
+                              float *alphas_eff, gsb_stream_t stream);
+int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                               const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                               float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                               const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                               float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                               const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                               const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
+                               size_t ws_bytes, gsb_stream_t stream);
+
 /* dL/dsh from per-view dL/dcolor (extension; multi-view data parallelism, SURVEY 8e).
  * colour = 0.5 + sum_l Y_l(dir) sh_l is linear in sh and never clamped (kernel.cu:735-774), so
  * dloss_dshs[n, l, c] = sum_v Y_l((pws[n] - twcs[v]) / |.|) * dloss_dcolors[v, n, c].
