@@ -54,6 +54,10 @@ SIGNATURES = {
     "gsb_preprocess_forward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 9),
     "gsb_preprocess_backward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 15 + [_sz, _vp]),
     "gsb_sh_grad_expand": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    "gsb_filter3d_workspace_bytes": (_sz, [_i, _i]),
+    "gsb_filter3d": (_i, [_i, _vp, _i, _vp, _f, _vp, _vp, _sz, _vp]),
+    "gsb_filter3d_apply": (_i, [_i] + [_vp] * 6),
+    "gsb_filter3d_backward": (_i, [_i] + [_vp] * 8),
     "gsb_small_bmm": (_i, [C.c_longlong, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "gsb_gau_loss_workspace_bytes": (_sz, [_i, _i]),
     "gsb_gau_loss": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),

@@ -38,7 +38,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "small_bmm", "density_accumulate", "density_classify",
                                              "density_scan", "density_apply", "reset_alpha",
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
-                                             "grad_reduce_broadcast", "sh_grad_expand", "draw_rgbd",
+                                             "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
+                                             "filter3d_apply", "filter3d_backward", "draw_rgbd",
                                              "draw_backward_rgbd"};
 
 ProfScope::ProfScope(int id, cudaStream_t st) : id_(id), st_(st), stop_(nullptr) {
@@ -336,6 +337,44 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
                                dloss_drots, nullptr, &mi, dloss_ddepths, pose ? &po : nullptr, alphas,
                                (cudaStream_t)stream);
+}
+
+// ---- Mip-Splatting 3D smoothing filter (filter3d.cu)
+static_assert(F3_CHUNK == GSB_FILTER3D_CHUNK, "gsplat_b200.h and kernels.h disagree on the camera chunk");
+
+size_t gsb_filter3d_workspace_bytes(int N, int C) {
+  (void)N;
+  (void)C;
+  return filter3d_workspace_bytes();
+}
+
+int gsb_filter3d(int N, const float *pws, int C, const float *cams, float variance, float *filter3d, void *ws,
+                 size_t ws_bytes, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && C >= 0, "filter3d: N < 0 or C < 0");
+  GSB_REQUIRE(isfinite(variance) && variance >= 0.f, "filter3d: variance must be finite and >= 0");
+  if (N == 0) return 0;
+  GSB_REQUIRE(pws && filter3d && (C == 0 || cams), "filter3d: null pointer");
+  GSB_REQUIRE(aligned(ws, 16), "filter3d: workspace misaligned");
+  GSB_REQUIRE(ws != nullptr && ws_bytes >= filter3d_workspace_bytes(), "filter3d: workspace too small");
+  return launch_filter3d(N, pws, C, cams, variance, filter3d, static_cast<unsigned int *>(ws), (cudaStream_t)stream);
+}
+
+int gsb_filter3d_apply(int N, const float *scales, const float *alphas, const float *filter3d, float *scales_f,
+                       float *alphas_f, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0, "filter3d_apply: N < 0");
+  GSB_REQUIRE(N == 0 || (scales && alphas && filter3d && scales_f && alphas_f), "filter3d_apply: null pointer");
+  return launch_filter3d_apply(N, scales, alphas, filter3d, scales_f, alphas_f, (cudaStream_t)stream);
+}
+
+int gsb_filter3d_backward(int N, const float *scales, const float *alphas, const float *filter3d,
+                          const float *dloss_dscales_f, const float *dloss_dalphas_f, float *dloss_dscales,
+                          float *dloss_dalphas, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0, "filter3d_backward: N < 0");
+  GSB_REQUIRE(N == 0 || (scales && alphas && filter3d && dloss_dscales_f && dloss_dalphas_f && dloss_dscales &&
+                         dloss_dalphas),
+              "filter3d_backward: null pointer");
+  return launch_filter3d_bwd(N, scales, alphas, filter3d, dloss_dscales_f, dloss_dalphas_f, dloss_dscales,
+                             dloss_dalphas, (cudaStream_t)stream);
 }
 
 int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float *twcs, const float *dloss_dcolors,

@@ -15,7 +15,8 @@ enum KernelId {
   K_PROJECT = 0, K_COV3D, K_COV2D, K_SH2COLOR, K_INVCOV, K_RECTS, K_SCAN, K_KEYS, K_SORT, K_RANGES,
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
-  K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
+  K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -78,6 +79,19 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,
                      cudaStream_t st);
+
+// ---- Mip-Splatting 3D smoothing filter (filter3d.cu; the math is pg_fused_math.h filter3d_*).
+// cams: the [C][20] training-camera table (pg::kCamRow); ws: 2 words, zeroed here.  C == 0 gives
+// zeros.  The backward's outputs may alias dscales_f / dalphas_f.
+constexpr int F3_CHUNK = 64;  // cameras k_filter3d_depth stages in shared memory at once (GSB_FILTER3D_CHUNK)
+constexpr size_t filter3d_workspace_bytes() { return 16; }
+int launch_filter3d(int N, const float *pws, int C, const float *cams, float variance, float *filter3d,
+                    unsigned int *ws, cudaStream_t st);
+int launch_filter3d_apply(int N, const float *scales, const float *alphas, const float *filter3d, float *scales_f,
+                          float *alphas_f, cudaStream_t st);
+int launch_filter3d_bwd(int N, const float *scales, const float *alphas, const float *filter3d,
+                        const float *dscales_f, const float *dalphas_f, float *dscales, float *dalphas,
+                        cudaStream_t st);
 
 // ---- multi-GPU gradient exchange (comm.cu; the producer is the PUSH variant in fused.cu).
 // Every rank owns one region of peer-mapped memory:

@@ -391,5 +391,65 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
   return galpha_raw;
 }
 
+// ---- Mip-Splatting's 3D smoothing filter (filter3d.cu).  A training camera row is 20 floats:
+// Rcw (row-major 9), tcw (3), fx, fy, cx, cy, W, H, 2 pad (kCamRow).  Camera k sees a Gaussian
+// when camera_point keeps it (z >= kMinDepth, the rasterizers' cull) and its projected mean lies
+// within 15 % of the frame on every side.  Mip-Splatting's compute_3D_filter projects with
+// cx = W/2, cy = H/2 and culls z > 0.2; this uses the camera's own cx, cy and the z >= 0.2f cull.
+constexpr int kCamRow = 20;
+constexpr float kFilterMargin = 0.15f;
+
+// true when the camera `c` (one row) sees pw; z = its camera-frame depth then
+GSB_HD bool filter3d_sees(const float *c, const float pw[3], float &z) {
+  float pc[3];
+  if (!camera_point(c, c + 9, pw, pc)) return false;
+  float u[2];
+  project_mean(pc, 1.0f / pc[2], c[12], c[13], c[14], c[15], u);
+  const float W = c[16], H = c[17];
+  z = pc[2];
+  return u[0] >= -kFilterMargin * W && u[0] <= (1.0f + kFilterMargin) * W && u[1] >= -kFilterMargin * H &&
+         u[1] <= (1.0f + kFilterMargin) * H;
+}
+
+// filter3d = sqrt(variance) d / f_max, with d the nearest depth at which a camera sees the Gaussian
+GSB_HD float filter3d_value(float d, float fmax, float variance) { return sqrtf(variance) * d / fmax; }
+
+// Apply: s'_j = sqrt(s_j^2 + f^2), t_j = s_j / s'_j, alpha' = c alpha with c = t_0 t_1 t_2 (the
+// filtered Gaussian keeps the mass alpha prod s).  f == 0 passes s through and returns c = 1
+// exactly (s = f = 0 divides nothing).  t[3] receives t_j (1 when f == 0).
+GSB_HD float filter3d_apply(const float s[3], float f, float sf[3], float t[3]) {
+  if (f == 0.f) {
+    for (int j = 0; j < 3; j++) { sf[j] = s[j]; t[j] = 1.f; }
+    return 1.f;
+  }
+  const float f2 = f * f;
+  for (int j = 0; j < 3; j++) {
+    sf[j] = sqrtf(fmaf(s[j], s[j], f2));
+    t[j] = s[j] / sf[j];
+  }
+  return t[0] * t[1] * t[2];
+}
+
+// Backward of filter3d_apply (f is a constant):
+//   dL/ds_j = dL/ds'_j t_j + alpha dL/dalpha' (prod_{k != j} t_k) f^2 / s'_j^3,   dL/dalpha = c dL/dalpha'
+// with f^2 / s'^3 evaluated as (f / s')^2 / s' (no underflow of s'^3).  f == 0 passes both through.
+// gs may alias gsf (row-private in-place update).  Returns dL/dalpha.
+GSB_HD float filter3d_backward(const float s[3], float alpha, float f, const float gsf[3], float galpha_f,
+                               float gs[3]) {
+  if (f == 0.f) {
+    for (int j = 0; j < 3; j++) gs[j] = gsf[j];
+    return galpha_f;
+  }
+  float sf[3], t[3];
+  const float c = filter3d_apply(s, f, sf, t);
+  const float a = alpha * galpha_f;
+  const float other[3] = {t[1] * t[2], t[0] * t[2], t[0] * t[1]};
+  for (int j = 0; j < 3; j++) {
+    const float q = f / sf[j];
+    gs[j] = fmaf(gsf[j], t[j], a * other[j] * (q * q / sf[j]));
+  }
+  return c * galpha_f;
+}
+
 }  // namespace pg
 }  // namespace gsb

@@ -134,6 +134,20 @@ def params_to_gs_rows(training_params):
     return rows
 
 
+def bake_filter3d(training_params, filter3d):
+    """The plain 3DGS parameters of a model trained with the Mip-Splatting 3D filter: the six raw
+    training tensors whose activated scales and opacities are the filtered s' = sqrt(s^2 + f^2) and
+    alpha' = alpha prod s / s' (ops.filter3d_apply), so a renderer, viewer or PLY consumer that
+    knows nothing of the filter draws the filtered model.  Bake before saving.
+    -> dict of the six raw tensors (new leaves with requires_grad, as gs_rows_to_params)."""
+    from . import ops
+    rows = params_to_gs_rows(training_params)  # activated: pw 3 | rot 4 | scale 3 | alpha 1 | sh 48
+    sf, af = ops.filter3d_apply(rows[:, 7:10], rows[:, 10], filter3d)
+    rows[:, 7:10] = sf
+    rows[:, 10] = af
+    return gs_rows_to_params(rows, 48)
+
+
 def _rows_to_recarray(rows, sh_dim):
     host = rows.cpu().numpy()
     return np.rec.array(np.ascontiguousarray(host).view(np.dtype(gsdata_type(sh_dim))).reshape(-1))

@@ -14,6 +14,10 @@ static buffers:
 
 With cam.antialiased the captured frame composites alpha_eff = rho * alpha (ops.preprocess) and the
 backward returns dL/dalpha of the raw alphas; binning, hence the captured capacities, is the same.
+With filter3d[N] (ops.filter3d, the Mip-Splatting 3D filter) the forward graph starts with the
+filter's apply pass (s', alpha') and the backward graph ends with its backward, so the gradients
+are those of the unfiltered scales and alphas; the filter is captured by address like the
+parameters (recompute it in place).
 
 The parameters are captured by address: an optimizer that updates them in place is seen by the
 next replay.  `forward()`'s outputs are validated lazily: `backward()` (or `check()`) reads the
@@ -29,9 +33,10 @@ class CapacityError(RuntimeError):
 
 
 class GraphedFusedStep:
-    def __init__(self, pws, shs, alphas, scales, rots, cam, headroom=1.5):
+    def __init__(self, pws, shs, alphas, scales, rots, cam, headroom=1.5, filter3d=None):
         self.p = dict(pws=pws.detach(), shs=shs.detach(), alphas=alphas.detach(), scales=scales.detach(),
                       rots=rots.detach())
+        self.filter3d = filter3d.detach() if filter3d is not None else None
         self.cam, self.headroom = cam, float(headroom)
         self.device = pws.device
         self.status = torch.zeros(4, dtype=torch.int32).pin_memory()
@@ -39,26 +44,36 @@ class GraphedFusedStep:
         self.recapture()
 
     # ------------------------------------------------------------------ capture
+    def _drawn_params(self):
+        """the scales and alphas the frame is rendered from: s', alpha' with the filter"""
+        p = self.p
+        if self.filter3d is None:
+            return p["scales"], p["alphas"]
+        return ops.filter3d_apply(p["scales"], p["alphas"], self.filter3d)
+
     def _learn_capacities(self):
         cam, p = self.cam, self.p
-        us, ci, col, dep, ar = ops.preprocess(p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc,
+        scales, alphas = self._drawn_params()
+        us, ci, col, dep, ar = ops.preprocess(p["pws"], p["rots"], scales, p["shs"], cam.Rcw, cam.tcw, cam.twc,
                                               cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height)
-        out = ops.splat(cam.height, cam.width, us, ci, p["alphas"], dep, col, ar)
+        out = ops.splat(cam.height, cam.width, us, ci, alphas, dep, col, ar)
         dkmax = int((dep.max().clamp_min(0) * 1000).item()) + 1
         return ops._next_capacity(out[4].numel(), dkmax, headroom=self.headroom)
 
     def _forward_body(self):
         cam, p = self.cam, self.p
         aa = bool(getattr(cam, "antialiased", False))
-        pre = ops.preprocess(p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
-                             cam.cx, cam.cy, cam.width, cam.height, alphas=p["alphas"], antialiased=aa)
+        scales, alphas = self._drawn_params()
+        pre = ops.preprocess(p["pws"], p["rots"], scales, p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
+                             cam.cx, cam.cy, cam.width, cam.height, alphas=alphas, antialiased=aa)
         us, ci, col, dep, ar, rec = pre[:6]
-        drawn = pre[6] if aa else p["alphas"]  # antialiased: the rasterizers composite alpha_eff
+        drawn = pre[6] if aa else alphas  # antialiased: the rasterizers composite alpha_eff
         _, self._keep, (image, contrib, final_tau, ranges, gsid) = ops._capacity_frame(
             cam.height, cam.width, us, ci, drawn, dep, col, ar, rec, self.P_cap, self.dk_cap, self.status,
             enqueue=True)
         self._fwd = dict(us=us, cinv2ds=ci, colors=col, depths=dep, areas=ar, records=rec, contrib=contrib,
-                         final_tau=final_tau, ranges=ranges, gsid=gsid, alphas=drawn, aa=aa)
+                         final_tau=final_tau, ranges=ranges, gsid=gsid, alphas=drawn, aa=aa, scales_f=scales,
+                         alphas_f=alphas)
         self.image = image
 
     def _backward_body(self):
@@ -68,9 +83,11 @@ class GraphedFusedStep:
                              f["contrib"], f["final_tau"], f["ranges"], f["gsid"], self.dloss_dimage,
                              moments_only=True, records=f["records"])
         gpw, gsh, gs, gq, dus, dal = ops.preprocessB(
-            p["pws"], p["rots"], p["scales"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+            p["pws"], p["rots"], f["scales_f"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=f["cinv2ds"], antialiased=f["aa"],
-            alphas=p["alphas"] if f["aa"] else None)
+            alphas=f["alphas_f"] if f["aa"] else None)
+        if self.filter3d is not None:  # dL/ds', dL/dalpha' -> dL/ds, dL/dalpha, in place
+            ops.filter3d_backward(p["scales"], p["alphas"], self.filter3d, gs, dal, inplace=True)
         self._keep_b = moments
         self.grads = dict(dpws=gpw, dshs=gsh, dscales=gs, drots=gq, dalphas=dal, dus=dus)
 

@@ -99,11 +99,14 @@ class GSFunctionFused(torch.autograd.Function):
     stages run as one fused forward kernel and one fused backward kernel (ops.preprocess /
     ops.preprocessB) instead of five Jacobian-materialising ops + the torch.bmm chain.
     Swap-in: `from easygaussiansplatting_b200.gsfunction import GSFunctionFused as GSFunction`
-    in gsplat/gsmodel.py."""
+    in gsplat/gsmodel.py.
+    All four fused classes take an optional trailing `filter3d[N]` (ops.filter3d; after `cam`):
+    the Mip-Splatting 3D filter, a constant that gets no gradient.  The frame is then rendered from
+    s', alpha' (ops.filter3d_apply) and the scale and opacity gradients are taken back through it."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, cam):
-        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam)
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None):
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
@@ -119,19 +122,27 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
     shs, alphas, scales, rots and us; the depth term reaches pws through z = (Rcw pw + tcw)[2]."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, cam):
-        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam)
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None):
+        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
         return _fused_backward(ctx, True, False, dloss_dgammas, dloss_ddepth, dloss_dalpha)
 
 
-def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None):
+def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None, filter3d=None):
     """The forward of the four fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
     camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward.
-    cam.antialiased (absent: False): the rasterizers composite alpha_eff = rho * alpha."""
+    cam.antialiased (absent: False): the rasterizers composite alpha_eff = rho * alpha.
+    filter3d: None, or the Mip-Splatting 3D filter[N] (ops.filter3d, a constant): the frame is
+    rendered from s' = sqrt(s^2 + f^2) and alpha' = alpha prod s / s' (ops.filter3d_apply)."""
     from . import ops
+    ctx.filtered = filter3d is not None
+    raw = ()
+    if ctx.filtered:
+        filter3d = filter3d.detach()
+        raw = (scales, alphas, filter3d)
+        scales, alphas = ops.filter3d_apply(scales, alphas, filter3d)
     aa = bool(getattr(cam, "antialiased", False))
     if pose is None:
         Rcw, tcw, twc = cam.Rcw, cam.tcw, cam.twc
@@ -156,20 +167,37 @@ def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None
     if pose is not None:
         ctx.cam_shapes = (Rcw.shape, tcw.shape, twc.shape)
         saved += (Rcw, tcw, twc)
-    ctx.save_for_backward(*saved)
+    ctx.save_for_backward(*(saved + raw))  # (with the filter, scales and alphas above are s', alpha')
     mask = depths > 0.2
     return (out[0], out[5], out[6], mask) if rgbd else (out[0], mask)
 
 
 def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None):
     """The backward of the four fused classes -> the gradients of the map inputs (pws, shs, alphas,
-    scales, rots, us), with pose those of Rcw, tcw, twc, and None for cam.  What runs follows
-    ctx.needs_input_grad: the pose alone takes the pose-only kernel (a frozen map: tracking)."""
+    scales, rots, us), with pose those of Rcw, tcw, twc, and None for cam (and filter3d).  What runs
+    follows ctx.needs_input_grad: the pose alone takes the pose-only kernel (a frozen map: tracking)."""
     from . import ops
     cam = ctx.cam
     (pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau, patch_range_per_tile,
-     gsid_per_patch, *cam_saved) = ctx.saved_tensors
-    Rcw, tcw, twc = cam_saved if pose else (cam.Rcw, cam.tcw, cam.twc)
+     gsid_per_patch, *rest) = ctx.saved_tensors
+    Rcw, tcw, twc = rest[:3] if pose else (cam.Rcw, cam.tcw, cam.twc)
+    raw = rest[3:] if pose else rest  # (scales, alphas, filter3d) of a filtered frame
+    grads = _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds,
+                                 depths, colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw,
+                                 twc, dloss_dgammas, dloss_ddepth, dloss_dalpha)
+    if ctx.filtered and grads[3] is not None:
+        # the gradients are those of s', alpha' (summed over the ranks with the exchange: the filter's
+        # backward is linear with per-Gaussian coefficients, so it applies after the sum as well)
+        dscales, dalphas = ops.filter3d_backward(*raw, grads[3], grads[2], inplace=True)
+        grads = grads[:2] + (dalphas, dscales) + grads[4:]
+    # one gradient per input apply received (cam, and filter3d when passed -- also as None -- get None)
+    return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
+
+
+def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths,
+                         colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw, twc,
+                         dloss_dgammas, dloss_ddepth, dloss_dalpha):
+    """the gradients of the inputs the frame was rendered from, up to and including the pose's"""
     need_map = any(ctx.needs_input_grad[:6])
     need_cam = pose and any(ctx.needs_input_grad[6:9])
     # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward converts
@@ -193,7 +221,7 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
         # the result region is overwritten by the next step's broadcast: hand autograd its own
         # copies (AccumulateGrad may keep a returned tensor, and so may hooks / retain_grad)
         return (g["dpws"].clone(), g["dshs"].clone(), g["dalphas"].clone().reshape(ctx.alpha_shape),
-                g["dscales"].clone(), g["drots"].clone(), g["dus"], None)
+                g["dscales"].clone(), g["drots"].clone(), g["dus"])
     out = ops.preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
                           cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths,
                           camera_grad=need_cam, pose_only=need_cam and not need_map, antialiased=ctx.aa,
@@ -207,7 +235,7 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
         grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
     elif pose:
         grads += (None, None, None)
-    return grads + (None,)
+    return grads
 
 
 class GSFunctionFusedPose(torch.autograd.Function):
@@ -220,8 +248,8 @@ class GSFunctionFusedPose(torch.autograd.Function):
     GSFunctionFused's backward.  Intrinsics are not differentiated; single view only."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
-        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc))
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None):
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
@@ -234,8 +262,8 @@ class GSFunctionFusedRGBDPose(torch.autograd.Function):
     depths > 0.2).  The depth plane's gradient reaches the pose through z = (Rcw pw + tcw)[2]."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam):
-        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc))
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None):
+        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):

@@ -12,6 +12,7 @@ libgsplat_b200.so.  Differences from the reference, all deliberate:
   * N == 0 and P <= 1 are handled (SURVEY 8b "degenerate inputs").
 """
 import ctypes as C
+import math
 
 import torch
 
@@ -623,6 +624,117 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     if camera_grad:
         out.append((gcam[:9].view(3, 3), gcam[9:12], gcam[12:15]))
     return out
+
+
+# ---------------------------------------------------------------------------------------
+# Mip-Splatting's 3D smoothing filter (gsb_filter3d*): a per-Gaussian lower bound on the size,
+# from the sampling rate of the training views.  scales / alphas are the activated values.
+FILTER3D_CHUNK = 64   # cameras the filter kernel stages in shared memory at once (GSB_FILTER3D_CHUNK)
+CAMERA_ROW = 20       # Rcw (row-major 9), tcw (3), fx, fy, cx, cy, W, H, 2 unused
+
+
+def camera_table(cams, device=None):
+    """Packs training cameras -- any objects with the reference Camera's fields width, height, fx,
+    fy, cx, cy, Rcw[3,3], tcw[3] (gsplat/gausplat_dataset.py Camera, gsfunction.Camera) -- into the
+    [C, 20] float32 device table `filter3d` reads.  W, H > 0 and finite intrinsics with fx > 0 are
+    checked here, on the host.  device: where the table goes (default: that of the first
+    camera's Rcw when it is a CUDA tensor, else the current CUDA device)."""
+    cams = list(cams)
+    rows = torch.zeros((len(cams), CAMERA_ROW), dtype=torch.float64)
+    for k, c in enumerate(cams):
+        w, h = float(c.width), float(c.height)
+        intr = [float(c.fx), float(c.fy), float(c.cx), float(c.cy)]
+        if not (w > 0 and h > 0):
+            raise ValueError("camera %d: width and height must be positive" % k)
+        if not all(math.isfinite(x) for x in intr) or intr[0] <= 0:
+            raise ValueError("camera %d: fx, fy, cx, cy must be finite and fx > 0" % k)
+        R = torch.as_tensor(c.Rcw).detach().reshape(-1).to("cpu", torch.float64)
+        t = torch.as_tensor(c.tcw).detach().reshape(-1).to("cpu", torch.float64)
+        if R.numel() != 9 or t.numel() != 3:
+            raise ValueError("camera %d: Rcw must have 9 and tcw 3 elements" % k)
+        rows[k, :9], rows[k, 9:12] = R, t
+        rows[k, 12:18] = torch.tensor(intr + [w, h], dtype=torch.float64)
+    if device is None:
+        R0 = cams[0].Rcw if cams else None
+        device = R0.device if isinstance(R0, torch.Tensor) and R0.is_cuda else torch.device("cuda")
+    return rows.to(torch.float32).to(device)
+
+
+def filter3d(pws, cams_or_table, variance=0.2):
+    """The 3D filter of every Gaussian from the training cameras (gsb_filter3d): camera k sees
+    Gaussian i when its camera-frame depth z >= 0.2 and its projected mean lies within 15 % of the
+    frame on every side; d_i = the smallest such z (the largest d of the seen Gaussians when no
+    camera sees i), and filter3d_i = sqrt(variance) d_i / max_k fx_k (the largest positive fx; a
+    table given as a tensor is not checked on the host).  All 0 when nothing is seen or no camera
+    has fx > 0.
+    cams_or_table: camera objects (`camera_table`) or such a [C, 20] table.  -> filter3d[N]"""
+    pws = _chk(pws, "pws", last=3, ndim=2)
+    if isinstance(cams_or_table, torch.Tensor):
+        table = _chk(cams_or_table, "camera table", last=CAMERA_ROW, ndim=2)
+    else:
+        table = camera_table(cams_or_table, device=pws.device)
+    _same_device(pws, table)
+    variance = float(variance)
+    if not (math.isfinite(variance) and variance >= 0):
+        raise ValueError("variance must be finite and >= 0")
+    N, Cn = pws.shape[0], table.shape[0]
+    out = torch.empty((N,), dtype=torch.float32, device=pws.device)
+    lib = _L()
+    nbytes = int(lib.gsb_filter3d_workspace_bytes(N, Cn))
+    ws = _bytes(max(nbytes, 16), pws.device)
+    with torch.cuda.device(pws.device):
+        _lib.check(lib.gsb_filter3d(N, _ptr(pws), Cn, _ptr(table), variance, _ptr(out), _ptr(ws), nbytes, _stream()),
+                   lib)
+    return out
+
+
+def _filter3d_rows(scales, alphas, filter3d):
+    scales = _chk(scales, "scales", last=3, ndim=2); alphas = _chk(alphas, "alphas")
+    filter3d = _chk(filter3d, "filter3d")
+    _same_device(scales, alphas, filter3d)
+    N = scales.shape[0]
+    if alphas.numel() != N or filter3d.numel() != N:
+        raise ValueError("scales[N,3], alphas[N] and filter3d[N] disagree on N")
+    return scales, alphas, filter3d, N
+
+
+def filter3d_apply(scales, alphas, filter3d):
+    """(scales[N,3], alphas) -> (scales_f, alphas_f) (gsb_filter3d_apply): s'_j = sqrt(s_j^2 + f^2)
+    and alpha' = alpha prod_j s_j / s'_j, which keeps each Gaussian's mass; f == 0 copies exactly.
+    alphas_f has the shape of alphas.  Render with these; the filter itself is not differentiated."""
+    shape = alphas.shape if isinstance(alphas, torch.Tensor) else None
+    scales, alphas, filter3d, N = _filter3d_rows(scales, alphas, filter3d)
+    sf = torch.empty_like(scales); af = torch.empty(shape, dtype=torch.float32, device=scales.device)
+    lib = _L()
+    with torch.cuda.device(scales.device):
+        _lib.check(lib.gsb_filter3d_apply(N, _ptr(scales), _ptr(alphas), _ptr(filter3d), _ptr(sf), _ptr(af),
+                                          _stream()), lib)
+    return sf, af
+
+
+def filter3d_backward(scales, alphas, filter3d, dloss_dscales_f, dloss_dalphas_f, inplace=False):
+    """Backward of `filter3d_apply` (gsb_filter3d_backward): dL/ds' [N,3] and dL/dalpha' -> (dL/ds,
+    dL/dalpha) of the unfiltered scales and alphas.  inplace: written over the two gradient inputs
+    (which must then be contiguous float32 CUDA tensors) and those are returned."""
+    scales, alphas, filter3d, N = _filter3d_rows(scales, alphas, filter3d)
+    if inplace and not (isinstance(dloss_dscales_f, torch.Tensor) and dloss_dscales_f.is_contiguous() and
+                        isinstance(dloss_dalphas_f, torch.Tensor) and dloss_dalphas_f.is_contiguous()):
+        raise ValueError("inplace=True needs contiguous gradient tensors")
+    gs = _chk(dloss_dscales_f, "dloss_dscales_f", last=3, ndim=2)
+    ga_shape = dloss_dalphas_f.shape if isinstance(dloss_dalphas_f, torch.Tensor) else None
+    ga = _chk(dloss_dalphas_f, "dloss_dalphas_f")
+    _same_device(scales, gs, ga)
+    if gs.shape[0] != N or ga.numel() != N:
+        raise ValueError("dloss_dscales_f[N,3] and dloss_dalphas_f[N] disagree with scales on N")
+    if inplace:
+        ds, da = gs, ga
+    else:
+        ds = torch.empty_like(gs); da = torch.empty(ga_shape, dtype=torch.float32, device=gs.device)
+    lib = _L()
+    with torch.cuda.device(scales.device):
+        _lib.check(lib.gsb_filter3d_backward(N, _ptr(scales), _ptr(alphas), _ptr(filter3d), _ptr(gs), _ptr(ga),
+                                             _ptr(ds), _ptr(da), _stream()), lib)
+    return ds, da
 
 
 def sh_grad_expand(pws, twcs, dloss_dcolors, sh_dim3, out=None):

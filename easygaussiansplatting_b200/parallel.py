@@ -252,32 +252,44 @@ class MultiViewStep:
 
     The collectives go through torch.distributed (NCCL on GPUs); the all-gather of the colours
     is started before the expansion of the local result needs it and the all-reduce of the small
-    bucket overlaps that expansion.  world == 1 (or no process group) degenerates to local sums."""
+    bucket overlaps that expansion.  world == 1 (or no process group) degenerates to local sums.
 
-    def __init__(self, pws, rots, scales, shs, alphas, group=None):
+    filter3d[N] (ops.filter3d, the Mip-Splatting 3D filter): every view renders s', alpha'
+    (ops.filter3d_apply, computed by the step's first `render` and reused by its other views: the
+    parameters do not change inside a step) and `reduce` takes the summed dL/ds', dL/dalpha' back through the filter
+    once -- it is linear with per-Gaussian coefficients, so once after the sum equals once per view."""
+
+    def __init__(self, pws, rots, scales, shs, alphas, group=None, filter3d=None):
         self.pws, self.rots, self.scales, self.shs, self.alphas = pws, rots, scales, shs, alphas
+        self.filter3d = filter3d
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.k3 = shs.shape[1] // 3
         self._small, self._colors, self._twcs, self._dus = None, [], [], []
         self._early = None
+        self._filtered = None  # this step's (s', alpha')
 
     def render(self, cam):
         from . import ops
         aa = bool(getattr(cam, "antialiased", False))
-        pre = ops.preprocess(self.pws, self.rots, self.scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
-                             cam.cx, cam.cy, cam.width, cam.height, alphas=self.alphas, antialiased=aa)
+        scales, alphas = self.scales, self.alphas
+        if self.filter3d is not None:  # render s', alpha' (once per step)
+            if self._filtered is None:
+                self._filtered = ops.filter3d_apply(scales, alphas, self.filter3d)
+            scales, alphas = self._filtered
+        pre = ops.preprocess(self.pws, self.rots, scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
+                             cam.cx, cam.cy, cam.width, cam.height, alphas=alphas, antialiased=aa)
         us, cinv2ds, colors, depths, areas, records = pre[:6]
-        drawn = pre[6] if aa else self.alphas  # antialiased: the rasterizers composite alpha_eff
+        drawn = pre[6] if aa else alphas  # antialiased: the rasterizers composite alpha_eff
         image, contrib, final_tau, ranges, gsid = ops.splat(cam.height, cam.width, us, cinv2ds, drawn, depths,
                                                             colors, areas, records=records, capacity=True)
-        return image, (cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid, drawn)
+        return image, (cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid, drawn, scales, alphas)
 
     def backward(self, ctx, dloss_dimage, last=False):
         """last=True (the rank's final view of the step): the all-gather of the views' dL/dcolor
         starts here, right after the rasterizer backward, and runs under the per-Gaussian backward."""
         from . import ops
-        cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid, drawn = ctx
+        cam, us, cinv2ds, depths, colors, contrib, final_tau, ranges, gsid, drawn, scales, alphas = ctx
         aa = bool(getattr(cam, "antialiased", False))
         moments = ops.splatB(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
                              ranges, gsid, dloss_dimage, moments_only=True)
@@ -286,9 +298,9 @@ class MultiViewStep:
         if last and self.world > 1 and _EARLY_GATHER:
             self._early = _start_gathers(torch.stack(self._colors), torch.cat(self._twcs).contiguous(), self.group)
         gpw, _, gs, gq, dus, dal = ops.preprocessB(
-            self.pws, self.rots, self.scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+            self.pws, self.rots, scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, compact=True, antialiased=aa,
-            alphas=self.alphas if aa else None)
+            alphas=alphas if aa else None)
         bucket = torch.as_strided(gpw, (gpw.shape[0] * 11,), (1,), gpw.storage_offset())  # [dpws|dscales|drots|dalphas]
         self._small = bucket if self._small is None else self._small.add_(bucket)
         self._dus.append(dus)
@@ -304,11 +316,15 @@ class MultiViewStep:
             colors = torch.stack(self._colors)                   # [V_local, N, 3] (contiguous copy)
             twcs = torch.cat(self._twcs).contiguous()            # [V_local, 3]
             small, dshs = factorised_sum(self._small, colors, twcs, self.group, expand)
+        if self.filter3d is not None:  # the summed dL/ds', dL/dalpha' -> dL/ds, dL/dalpha, in place
+            ops.filter3d_backward(self.scales, self.alphas, self.filter3d, small[3 * N:6 * N].view(N, 3),
+                                  small[10 * N:], inplace=True)
         out = {"dpws": small[:3 * N].view(N, 3), "dscales": small[3 * N:6 * N].view(N, 3),
                "drots": small[6 * N:10 * N].view(N, 4), "dalphas": small[10 * N:], "dshs": dshs, "dus": self._dus,
                "bytes_per_rank": int(small.numel() * 4 + colors.numel() * 4)}
         self._small, self._colors, self._twcs, self._dus = None, [], [], []
         self._early = None
+        self._filtered = None
         return out
 
 

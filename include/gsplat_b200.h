@@ -191,6 +191,38 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
 int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float *twcs, const float *dloss_dcolors,
                        float *dloss_dshs, gsb_stream_t stream);
 
+/* Mip-Splatting 3D smoothing filter (extension).  Bounds each Gaussian's size from below by the
+ * sampling rate of the training views, so that a scene rendered closer or at a higher resolution
+ * than it was trained at shows no high-frequency erosion.  scales and alphas are the ACTIVATED
+ * values (exp of the raw scales, sigmoid of the raw opacities), as the fused path takes them.
+ * gsb_filter3d: pws[N,3] and the training cameras cams[C,20] (row: Rcw row-major 9, tcw 3, fx,
+ * fy, cx, cy, W, H, 2 unused) -> filter3d[N]:
+ *     camera k sees Gaussian i  iff  z = (Rcw pw + tcw)[2] >= 0.2f (the rasterizers' cull) and the
+ *       projected mean u = (fx x/z + cx, fy y/z + cy) lies in [-0.15 W, 1.15 W] x [-0.15 H, 1.15 H];
+ *     d_i = min z over the cameras that see i, or the largest d of the seen Gaussians if none does;
+ *     filter3d_i = sqrt(variance) d_i / max_k fx_k (the largest POSITIVE fx; the table is not
+ *       checked on the host, so a camera with fx <= 0 or NaN only drops out of that maximum);
+ *     all 0 when no Gaussian is seen, when C == 0, or when no camera has fx > 0.
+ * (Mip-Splatting's compute_3D_filter with the camera's own cx, cy instead of W/2, H/2, and the
+ * z >= 0.2f cull instead of z > 0.2.)  The cameras are staged GSB_FILTER3D_CHUNK at a time; any
+ * C works.  ws: 16-byte aligned, gsb_filter3d_workspace_bytes(N, C) bytes.  Deterministic.
+ * gsb_filter3d_apply: (scales[N,3], alphas[N]) -> scales_f[N,3], alphas_f[N] with
+ *     s'_j = sqrt(s_j^2 + f^2),  alpha' = alpha prod_j s_j / s'_j    (f = filter3d_i);
+ *     f == 0 copies both exactly.  Render (and run the fused backward) with s', alpha'.
+ * gsb_filter3d_backward: dL/ds' (dloss_dscales_f[N,3]) and dL/dalpha' (dloss_dalphas_f[N]) ->
+ *     dL/ds = dL/ds'_j s_j/s'_j + alpha dL/dalpha' prod_{k!=j}(s_k/s'_k) f^2/s'_j^3,
+ *     dL/dalpha = prod_j (s_j/s'_j) dL/dalpha'   (f is a constant; f == 0 passes both through).
+ *     The outputs may be the inputs (in place). */
+#define GSB_FILTER3D_CHUNK 64
+size_t gsb_filter3d_workspace_bytes(int N, int C);
+int gsb_filter3d(int N, const float *pws, int C, const float *cams, float variance, float *filter3d, void *ws,
+                 size_t ws_bytes, gsb_stream_t stream);
+int gsb_filter3d_apply(int N, const float *scales, const float *alphas, const float *filter3d, float *scales_f,
+                       float *alphas_f, gsb_stream_t stream);
+int gsb_filter3d_backward(int N, const float *scales, const float *alphas, const float *filter3d,
+                          const float *dloss_dscales_f, const float *dloss_dalphas_f, float *dloss_dscales,
+                          float *dloss_dalphas, gsb_stream_t stream);
+
 /* ---- splat, phase 1: tile rectangles + patch count.
  * Replaces getRects + thrust::inclusive_scan + the D2H read of the total
  * (gausplat.cu:54-67, kernel.cu:82-122).  depths and areas are READ-WRITE (Gaussians that
