@@ -40,6 +40,29 @@ def scale(c2, keep):
                 near=keep & (np.abs(r - R_MIN) <= 1e-4 * R_MIN))
 
 
+def rel_tol(s):
+    """relative tolerance of an fp32 rho against the oracle's (s: `scale`): r = (a c - b^2) / D loses kappa
+    times the relative error of the fp32 cov2d entries (a few ulps: they come through cov3d and J), and
+    rho = sqrt(r) halves it; 2^-19 kappa bounds the measured error with margin"""
+    return 2e-5 + 2.0 ** -19 * np.nan_to_num(s["kappa"], nan=1.0)  # nan: a = b = c = 0 (clamped)
+
+
+def thin(scales):
+    """rows whose 3D covariance has thin axes fp32 cannot resolve next to its long one: the cov3d entries
+    round at 2^-24 s_max^2, so whatever depends on the thin axes keeps few digits once s_max^2 / s_min^2
+    nears 2^24 (r here; the conic and its gradients, and the pixels' exponent, on every path)"""
+    sc3 = np.abs(np.asarray(scales, np.float64)).reshape(-1, 3)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        k3d = np.nan_to_num((sc3.max(1) / sc3.min(1)) ** 2, nan=1.0, posinf=np.inf)
+    return k3d > 1e4
+
+
+def flagged(scales, s):
+    """rows an fp32 AA gradient is bounded separately on: at the clamp, an ill-conditioned 2D determinant,
+    or `thin`.  scales: those drawn."""
+    return s["near"] | (rel_tol(s) > 1e-3) | thin(scales)
+
+
 def dcov2d_addend(c2, keep, alphas, dloss_dalphas_eff):
     """alpha dL/dalpha_eff drho/d(a, b, c) -> [N,3] (0 on culled and clamped rows)"""
     c2 = np.asarray(c2, np.float64).reshape(-1, 3)

@@ -38,7 +38,11 @@ def edge_scene(k3, seed, n=3000):
     """_scene (culled rows, fov-clamped rows, a general camera) with the AA edge rows at its head:
     0-3 zero scale (r = 0: the clamp holds), 4-7 needles (large kappa), 8-11 huge (rho -> 1),
     12-15 culled (rho = 1).  -> (scene, dict of row index arrays)"""
-    sc = _scene(n, k3, seed=seed)
+    return aa_edge_rows(_scene(n, k3, seed=seed))
+
+
+def aa_edge_rows(sc):
+    """edge_scene's head rows written into any scene (in place) -> (scene, dict of row index arrays)"""
     pc_mid = sc["pws"][sc["pws"][:, 2] > 0][:16]
     sc["pws"][:16] = pc_mid
     sc["scales"][0:4] = 0.0
@@ -116,11 +120,7 @@ def upstream(sc, k3, seed, rows=None):
     return gu, gci, gcol, gz, gal
 
 
-def rel_tol(s):
-    """relative tolerance of an fp32 rho against the oracle's: r = (a c - b^2) / D loses kappa times
-    the relative error of the fp32 cov2d entries (a few ulps: they come through cov3d and J), and
-    rho = sqrt(r) halves it; 2^-19 kappa bounds the measured error with margin"""
-    return 2e-5 + 2.0 ** -19 * np.nan_to_num(s["kappa"], nan=1.0)  # nan: a = b = c = 0 (clamped)
+rel_tol = oaa.rel_tol  # (the tolerance of an fp32 rho, shared with oracle/step_oracle.py)
 
 
 # ---------------------------------------------------------------- the oracle itself

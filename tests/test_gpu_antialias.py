@@ -37,13 +37,8 @@ def _params(sc):
 
 
 def flagged(sc, s):
-    """rows bounded separately: at the clamp, an ill-conditioned 2D determinant, or a 3D covariance
-    whose thin axes fp32 cannot resolve next to its long one (the cov3d entries round at
-    2^-24 s_max^2, so r keeps no digits once s_max^2 / s_min^2 nears 2^24)"""
-    sc3 = np.abs(np.asarray(sc["scales"], np.float64))
-    with np.errstate(divide="ignore", invalid="ignore"):
-        k3d = np.nan_to_num((sc3.max(1) / sc3.min(1)) ** 2, nan=1.0, posinf=np.inf)
-    return s["near"] | (rel_tol(s) > 1e-3) | (k3d > 1e4)
+    """rows bounded separately (aa_oracle.flagged: the clamp, ill-conditioned 2D or 3D covariances)"""
+    return oaa.flagged(sc["scales"], s)
 
 
 def _grid_scene(N, k3):
