@@ -39,7 +39,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "density_scan", "density_apply", "reset_alpha",
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
                                              "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
-                                             "filter3d_apply", "filter3d_backward", "draw_rgbd",
+                                             "filter3d_apply", "filter3d_backward", "density_apply_rows",
+                                             "draw_features", "draw_backward_features", "draw_rgbd",
                                              "draw_backward_rgbd"};
 
 ProfScope::ProfScope(int id, cudaStream_t st) : id_(id), st_(st), stop_(nullptr) {
@@ -658,6 +659,87 @@ int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, con
                              dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, stream);
 }
 
+// ---- feature rendering (raster_feat.cu)
+
+size_t gsb_splat_features_workspace_bytes(int N, int H, int W, int64_t P) {
+  return feat_layout(N, H, W, P, 1).bytes;  // (a ws at any address: the split from the worst start)
+}
+
+// The checks both feature entry points make, and the records they replay: packed_records, or
+// those packed into ws from us / cinv2ds / alphas / colors.  -> 0 and *recs (NULL without patches)
+static int feature_frame(const char *who, int H, int W, int N, int64_t P, int D, const float *us, const float *cinv2ds,
+                         const float *alphas, const float *colors, const float *features, const int32_t *contrib,
+                         const int32_t *ranges, const int32_t *gsid, const void *packed_records, void *ws,
+                         size_t ws_bytes, const Rec **recs, int **work, cudaStream_t st) {
+  char msg[160];
+  const char *err = nullptr;
+  const int64_t P_ws = packed_records != nullptr ? 0 : P;
+  if (N < 0 || H <= 0 || W <= 0 || P < 0)
+    err = "bad N/H/W/P";
+  else if (D < 1)
+    err = "D < 1";
+  else if (!grid_fits(H, W))
+    err = "more than 65535 tiles in a row or column";
+  else if (!aligned(packed_records, 16))
+    err = "packed_records misaligned";
+  else if (!(contrib && ranges && ws))
+    err = "null pointer";
+  else if (P > 0 && !(features && gsid && (packed_records || (us && cinv2ds && alphas && colors))))
+    err = "null pointer";
+  else if (ws_bytes < feat_layout(N, H, W, P_ws, 1).bytes)
+    err = "workspace too small";
+  if (err) {
+    snprintf(msg, sizeof(msg), "%s: %s", who, err);
+    return set_arg_error(msg);
+  }
+  char *b = static_cast<char *>(ws);
+  const FeatLayout L = feat_layout(N, H, W, P_ws, reinterpret_cast<uintptr_t>(ws));
+  *work = reinterpret_cast<int *>(b + L.work);
+  *recs = nullptr;
+  if (P == 0 || N == 0) return 0;
+  if (packed_records != nullptr) {
+    *recs = static_cast<const Rec *>(packed_records);
+    return 0;
+  }
+  Rec *r = reinterpret_cast<Rec *>(b + L.recs);
+  *recs = r;
+  return launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, nullptr, r, st);
+}
+
+int gsb_splat_features(int H, int W, int N, int64_t P, int D, const float *us, const float *cinv2ds,
+                       const float *alphas, const float *colors, const float *features, const void *packed_records,
+                       const int32_t *contrib, const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                       void *ws, size_t ws_bytes, float *feature_image, gsb_stream_t stream) {
+  GSB_REQUIRE(feature_image != nullptr, "splat_features: null feature_image");
+  GSB_REQUIRE(aligned(feature_image, 16), "splat_features: misaligned feature_image");
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rec *recs = nullptr;
+  int *work = nullptr;
+  if (int rc = feature_frame("splat_features", H, W, N, P, D, us, cinv2ds, alphas, colors, features, contrib,
+                             patch_range_per_tile, gsid_per_patch, packed_records, ws, ws_bytes, &recs, &work, st))
+    return rc;
+  return launch_draw_features(H, W, D, patch_range_per_tile, recs, gsid_per_patch, contrib, features, feature_image,
+                              work, st);
+}
+
+int gsb_splat_features_backward(int H, int W, int N, int64_t P, int D, const float *us, const float *cinv2ds,
+                                const float *alphas, const float *colors, const float *features,
+                                const void *packed_records, const int32_t *contrib, const float *final_tau,
+                                const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                                const float *dloss_dfeature_image, void *ws, size_t ws_bytes, float *moments,
+                                float *dloss_dfeatures, gsb_stream_t stream) {
+  GSB_REQUIRE(N == 0 || (moments && dloss_dfeatures), "splat_features_backward: null output");
+  GSB_REQUIRE(P == 0 || (final_tau && dloss_dfeature_image), "splat_features_backward: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rec *recs = nullptr;
+  int *work = nullptr;
+  if (int rc = feature_frame("splat_features_backward", H, W, N, P, D, us, cinv2ds, alphas, colors, features, contrib,
+                             patch_range_per_tile, gsid_per_patch, packed_records, ws, ws_bytes, &recs, &work, st))
+    return rc;
+  return launch_draw_features_backward(H, W, N, D, patch_range_per_tile, recs, gsid_per_patch, contrib, final_tau,
+                                       features, dloss_dfeature_image, moments, dloss_dfeatures, work, st);
+}
+
 // ---- density control + record conversion (density.cu)
 
 static bool gau_complete(const gsb_gaussians *g) {
@@ -711,6 +793,18 @@ int gsb_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64
   return launch_density_apply(N, cls, slots, K, C, gau_ptrs(src), state ? gau_ptrs(src_m) : nullptr,
                               state ? gau_ptrs(src_v) : nullptr, z, gau_ptrs(dst), state ? gau_ptrs(dst_m) : nullptr,
                               state ? gau_ptrs(dst_v) : nullptr, (cudaStream_t)stream);
+}
+
+int gsb_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C, int64_t S,
+                           int D, const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
+                           float *dst_v, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && K >= 0 && C >= 0 && S >= 0 && K <= N && C + S <= K && D >= 1, "density_apply_rows: bad counts");
+  if (N == 0 || K + C + S == 0) return 0;
+  GSB_REQUIRE(cls && slots && src && dst, "density_apply_rows: null pointer");
+  const bool state = src_m != nullptr;
+  GSB_REQUIRE((src_v != nullptr) == state && (dst_m != nullptr) == state && (dst_v != nullptr) == state,
+              "density_apply_rows: Adam moments must be all given or all NULL");
+  return launch_density_apply_rows(N, cls, slots, K, C, D, src, src_m, src_v, dst, dst_m, dst_v, (cudaStream_t)stream);
 }
 
 int gsb_reset_alpha(int64_t N, float *alphas_raw, float *exp_avg, float *exp_avg_sq, float reset_raw,

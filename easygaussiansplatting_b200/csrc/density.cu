@@ -442,6 +442,36 @@ __global__ void __launch_bounds__(32 * DG_WARPS) k_density_apply_rows(int N, con
 #undef GSB_JOB
 }
 
+// gsb_density_apply_rows: the plan applied to one more [N, D] tensor of any width D (per-Gaussian
+// features), blockIdx.y = the set (parameter, exp_avg, exp_avg_sq).  Grid-stride over the N D
+// elements; a survivor's element moves to its compacted row, a clone's or split's element is also
+// written at its new row -- a copy for the parameter, 0 for an Adam moment.  Elements of pruned
+// Gaussians are not loaded.
+__global__ void __launch_bounds__(256) k_density_copy_rows(int64_t N, int D, const uint8_t *__restrict__ cls,
+                                                           const Slot3 *__restrict__ slots, int64_t K, int64_t C,
+                                                           const float *__restrict__ src0,
+                                                           const float *__restrict__ src1,
+                                                           const float *__restrict__ src2, float *__restrict__ dst0,
+                                                           float *__restrict__ dst1, float *__restrict__ dst2) {
+  const int set = blockIdx.y;
+  const float *__restrict__ src = set == 0 ? src0 : (set == 1 ? src1 : src2);
+  float *__restrict__ dst = set == 0 ? dst0 : (set == 1 ? dst1 : dst2);
+  if (src == nullptr) return;
+  const int64_t total = N * D, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += stride) {
+    const int64_t i = e / D;
+    const int c = (int)(e - i * D);
+    const uint8_t cl = cls[i];
+    if (cl == CLS_PRUNE) continue;
+    const Slot3 sl = slots[i];
+    const float v = src[e];
+    dst[(int64_t)sl.k * D + c] = v;
+    if (cl == CLS_KEEP) continue;
+    const int64_t r = cl == CLS_SPLIT ? K + C + sl.s : K + sl.c;
+    dst[r * D + c] = set == 0 ? v : 0.f;
+  }
+}
+
 // gsmodel.py:320-331
 __global__ void k_reset_alpha(int64_t N, float *__restrict__ alphas_raw, float *__restrict__ m,
                               float *__restrict__ v, float val) {
@@ -611,6 +641,18 @@ int launch_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, in
   }
   dim3 grid(stream_grid((N * 45 + 3) / 4, 256), 18);
   k_density_apply<<<grid, 256, 0, st>>>(N, cls, reinterpret_cast<const Slot3 *>(slots), K, C, S, z);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C, int D,
+                              const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
+                              float *dst_v, cudaStream_t st) {
+  if (N == 0 || D == 0) return 0;
+  ProfScope ps(K_DENSITY_ROWS, st);
+  const dim3 grid(stream_grid(N * D, 256), 3);
+  k_density_copy_rows<<<grid, 256, 0, st>>>(N, D, cls, reinterpret_cast<const Slot3 *>(slots), K, C, src, src_m, src_v,
+                                            dst, dst_m, dst_v);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

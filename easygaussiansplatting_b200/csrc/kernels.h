@@ -16,7 +16,7 @@ enum KernelId {
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
-  K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -144,6 +144,11 @@ int launch_density_plan(int64_t N, const float *alphas_raw, const float *scales_
 int launch_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C,
                          float *const *src, float *const *src_m, float *const *src_v, const float *z,
                          float *const *dst, float *const *dst_m, float *const *dst_v, cudaStream_t st);
+// the same plan applied to one more [N, D] tensor and its Adam moments (src_m .. dst_v: all NULL or
+// all set): survivors, then clones, then splits, each new row a copy of its source (moments: 0)
+int launch_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C, int D,
+                              const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
+                              float *dst_v, cudaStream_t st);
 int launch_reset_alpha(int64_t N, float *alphas_raw, float *m, float *v, float val, cudaStream_t st);
 int launch_ply_rows_to_gs(int64_t N, int stride, int sh_dim, const float *rows, const int32_t *colmap, float *gs,
                           cudaStream_t st);
@@ -210,5 +215,24 @@ int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *
                          const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
                          float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
                          cudaStream_t st);
+
+// ---- feature rasterizers (raster_feat.cu): replays of the colour forward's binning that composite
+// features[N,D] (row stride D, any 4-byte alignment) with the image's weights.  ranges: any
+// alignment; work: the 2 + 4 * tiles ints of launch_tile_list.  recs == nullptr: no patches.
+// The forward writes every element of feature_image[D,H,W] (16-byte aligned).  The backward ADDS
+// its terms to moment rows 0-5 of moments[N,9] and writes every element of dloss_dfeatures[N,D].
+int launch_draw_features(int H, int W, int D, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
+                         const int32_t *contrib, const float *features, float *feature_image, int *work,
+                         cudaStream_t st);
+int launch_draw_features_backward(int H, int W, int N, int D, const int32_t *ranges, const Rec *recs,
+                                  const int32_t *gsid, const int32_t *contrib, const float *final_tau,
+                                  const float *features, const float *dloss_dfeature_image, float *moments,
+                                  float *dloss_dfeatures, int *work, cudaStream_t st);
+// carve-up of the feature passes' workspace from `base` (any byte): [records, only when they are
+// rebuilt (P > 0), 256-B aligned] [rasterizer work area]
+struct FeatLayout {
+  size_t recs, work, bytes;
+};
+FeatLayout feat_layout(int N, int H, int W, int64_t P, uintptr_t base);
 
 }  // namespace gsb

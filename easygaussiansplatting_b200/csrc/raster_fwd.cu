@@ -13,6 +13,7 @@
 // Replaces reference kernel.cu:152-271 (draw).
 #include "common.cuh"
 #include "kernels.h"
+#include "raster_eval.cuh"
 #include "tile_io.cuh"
 
 namespace gsb {
@@ -22,20 +23,6 @@ constexpr int FWD_CHUNK_BYTES = 32 * 48;
 #ifndef DRAW_MINBLOCKS
 #define DRAW_MINBLOCKS 8
 #endif
-
-namespace {
-// alpha' = min(0.99, alpha * exp2(a dx^2 + b dx dy + c dy^2)) at the lane's two pixels
-// (kernel.cu:236-245; same operation sequence as bwd_eval in raster_bwd.cu)
-__device__ __forceinline__ float2 fwd_alpha(const float4 &q0, const float4 &q1, const float2 &npx, float fpy) {
-  const float2 dx = add2_rn(p2s(q0.x), npx);
-  const float dy = q0.y - fpy;
-  const float cdy2 = (q1.z * dy) * dy;
-  const float2 t = fma2_rn(p2s(q1.y), p2s(dy), mul2_rn(p2s(q1.x), dx));
-  const float2 p = fma2_rn(t, dx, p2s(cdy2));
-  const float2 ag = mul2_rn(p2s(q0.w), p2(ex2_approx(fminf(p.x, 0.0f)), ex2_approx(fminf(p.y, 0.0f))));
-  return p2(fminf(ALPHA_CLAMP, ag.x), fminf(ALPHA_CLAMP, ag.y));
-}
-}  // namespace
 
 // Work list of the two rasterizers (work[0] = the kernels' item counter, work[1] = number of
 // entries, work[2..] = entries): a tile with more than 32 patches contributes four entries

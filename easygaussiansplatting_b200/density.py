@@ -122,6 +122,21 @@ def apply(cls, slots, counts, src, src_m, src_v, z):
     return dst, dst_m, dst_v
 
 
+def apply_rows(cls, slots, counts, src, src_m=None, src_v=None):
+    """gsb_density_apply_rows on one [N, D] tensor (and its Adam moments, both or neither)
+    -> (dst, dst_m, dst_v) fresh [K + C + S, D] tensors (the moments None without them)"""
+    lib = _lib.load()
+    K, Cn, S = counts
+    N, D = src.shape
+    dev = cls.device
+    fresh = lambda: torch.empty((K + Cn + S, D), dtype=torch.float32, device=dev)  # noqa: E731
+    dst = fresh()
+    dst_m, dst_v = (fresh(), fresh()) if src_m is not None else (None, None)
+    _lib.check(lib.gsb_density_apply_rows(N, _ptr(cls), _ptr(slots), K, Cn, S, D, _ptr(src), _ptr(src_m), _ptr(src_v),
+                                          _ptr(dst), _ptr(dst_m), _ptr(dst_v), _stream()), lib)
+    return dst, dst_m, dst_v
+
+
 class DensityController:
     """the density-control half of gsplat.gsmodel.GSModel (gsmodel.py:168-331), same attribute
     names (`grad_accum`, `cunt`) and the same printed report"""
@@ -147,17 +162,33 @@ class DensityController:
         accumulate(dloss_dus, mask, self.grad_accum, self.cunt, first)
 
     @torch.no_grad()
-    def update_gaussian_density(self, params, optimizer, generator=None):
+    def update_gaussian_density(self, params, optimizer, generator=None, extra=()):
         """gsmodel.py:236-318 with prune_params / update_params (:132-166) fused in.  Mutates
-        `params` and the optimizer's groups / state like the reference; returns the report."""
+        `params` and the optimizer's groups / state like the reference; returns the report.
+        extra: names of further per-Gaussian [N, D] entries of `params` (per-Gaussian features),
+        each with an optimizer group of that name; they are rebuilt by the same plan (survivors in
+        order, then clones, then splits, every new row a copy of its source row, with zero Adam
+        moments) by gsb_density_apply_rows.  extra=() is exactly the six-tensor update."""
         if self.cunt is None:
             raise RuntimeError("update_gaussian_density needs at least one update_density_info call")
         N, src = check_params(params)
+        extra = tuple(extra)
+        for k in extra:
+            if k in GAUSSIAN_TENSORS:
+                raise ValueError("extra names a built-in tensor: %r" % (k,))
+            t = params[k]
+            if not (isinstance(t, torch.Tensor) and t.dim() == 2 and t.shape[0] == N and t.shape[1] >= 1):
+                raise ValueError("params[%r] must be [N, D] with N = %d and D >= 1" % (k, N))
+            src[k] = _check(t.detach(), "params[%r]" % (k,), tuple(t.shape))
         groups = {g["name"]: g for g in optimizer.param_groups}
-        states = {k: optimizer.state.get(groups[k]["params"][0], None) for k in GAUSSIAN_TENSORS}
+        names = GAUSSIAN_TENSORS + extra
+        missing = [k for k in names if k not in groups]
+        if missing:
+            raise ValueError("the optimizer has no param group named %s" % ", ".join(map(repr, missing)))
+        states = {k: optimizer.state.get(groups[k]["params"][0], None) for k in names}
         have = [s is not None and "exp_avg" in s for s in states.values()]
         if any(have) and not all(have):
-            raise ValueError("optimizer state must exist for all six groups or for none")
+            raise ValueError("optimizer state must exist for all groups or for none")
         src_m = src_v = None
         if all(have):
             src_m = {k: _check(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape) for k in GAUSSIAN_TENSORS}
@@ -166,7 +197,15 @@ class DensityController:
         # the reference's torch.normal(mean=zeros(S,3), std=scales[split]) (:276-277)
         z = torch.empty((S, 3), dtype=torch.float32, device=src["pws"].device).normal_(0, 1, generator=generator)
         dst, dst_m, dst_v = apply(cls, slots, (K, Cn, S), src, src_m, src_v, z)
-        for k in GAUSSIAN_TENSORS:
+        for k in extra:
+            m = v = None
+            if src_m is not None:
+                m = _check(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape)
+                v = _check(states[k]["exp_avg_sq"], "exp_avg_sq[%r]" % k, src[k].shape)
+            dst[k], dm, dv = apply_rows(cls, slots, (K, Cn, S), src[k], m, v)
+            if dst_m is not None:
+                dst_m[k], dst_v[k] = dm, dv
+        for k in names:
             group = groups[k]
             old = group["params"][0]
             new = torch.nn.Parameter(dst[k].requires_grad_(True))

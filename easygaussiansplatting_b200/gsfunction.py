@@ -130,12 +130,14 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
         return _fused_backward(ctx, True, False, dloss_dgammas, dloss_ddepth, dloss_dalpha)
 
 
-def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None, filter3d=None):
-    """The forward of the four fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
+def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None, filter3d=None, features=None):
+    """The forward of the fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
     camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward.
     cam.antialiased (absent: False): the rasterizers composite alpha_eff = rho * alpha.
     filter3d: None, or the Mip-Splatting 3D filter[N] (ops.filter3d, a constant): the frame is
-    rendered from s' = sqrt(s^2 + f^2) and alpha' = alpha prod s / s' (ops.filter3d_apply)."""
+    rendered from s' = sqrt(s^2 + f^2) and alpha' = alpha prod s / s' (ops.filter3d_apply).
+    features: None, or [N, D]: the feature map [D, H, W] follows the image (ops.splat_features,
+    from the same records) and features is saved last."""
     from . import ops
     ctx.filtered = filter3d is not None
     raw = ()
@@ -167,37 +169,53 @@ def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None
     if pose is not None:
         ctx.cam_shapes = (Rcw.shape, tcw.shape, twc.shape)
         saved += (Rcw, tcw, twc)
-    ctx.save_for_backward(*(saved + raw))  # (with the filter, scales and alphas above are s', alpha')
+    feat = ()
+    if features is not None:
+        feat = (features,)
+        fmap = ops.splat_features(cam.height, cam.width, features, out[1], out[3], out[4], records=records)
+    ctx.save_for_backward(*(saved + raw + feat))  # (with the filter, scales and alphas above are s', alpha')
     mask = depths > 0.2
+    if features is not None:
+        return out[0], fmap, mask
     return (out[0], out[5], out[6], mask) if rgbd else (out[0], mask)
 
 
-def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None):
-    """The backward of the four fused classes -> the gradients of the map inputs (pws, shs, alphas,
-    scales, rots, us), with pose those of Rcw, tcw, twc, and None for cam (and filter3d).  What runs
-    follows ctx.needs_input_grad: the pose alone takes the pose-only kernel (a frozen map: tracking)."""
+def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None, featured=False,
+                    dloss_dfeatures_map=None):
+    """The backward of the fused classes -> the gradients of the map inputs (pws, shs, alphas,
+    scales, rots, us), with pose those of Rcw, tcw, twc, with features (featured) that of features,
+    and None for cam (and filter3d).  What runs follows ctx.needs_input_grad: the pose alone takes
+    the pose-only kernel (a frozen map: tracking)."""
     from . import ops
     cam = ctx.cam
     (pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths, colors, contrib, final_tau, patch_range_per_tile,
      gsid_per_patch, *rest) = ctx.saved_tensors
+    if featured:
+        feat = (rest.pop(), dloss_dfeatures_map)
     Rcw, tcw, twc = rest[:3] if pose else (cam.Rcw, cam.tcw, cam.twc)
     raw = rest[3:] if pose else rest  # (scales, alphas, filter3d) of a filtered frame
     grads = _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds,
                                  depths, colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw,
-                                 twc, dloss_dgammas, dloss_ddepth, dloss_dalpha)
+                                 twc, dloss_dgammas, dloss_ddepth, dloss_dalpha, feat if featured else None)
+    if featured:  # dL/dfeatures goes right after the map inputs (the pose classes take no features)
+        grads, dfeat = grads[:-1], grads[-1]
     if ctx.filtered and grads[3] is not None:
         # the gradients are those of s', alpha' (summed over the ranks with the exchange: the filter's
         # backward is linear with per-Gaussian coefficients, so it applies after the sum as well)
         dscales, dalphas = ops.filter3d_backward(*raw, grads[3], grads[2], inplace=True)
         grads = grads[:2] + (dalphas, dscales) + grads[4:]
+    if featured:
+        grads = grads + (dfeat,)
     # one gradient per input apply received (cam, and filter3d when passed -- also as None -- get None)
     return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
 def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths,
                          colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw, twc,
-                         dloss_dgammas, dloss_ddepth, dloss_dalpha):
-    """the gradients of the inputs the frame was rendered from, up to and including the pose's"""
+                         dloss_dgammas, dloss_ddepth, dloss_dalpha, feat=None):
+    """the gradients of the inputs the frame was rendered from, up to and including the pose's;
+    feat: None, or (features, dL/dfeature map or None) -> dL/dfeatures (None when no map gradient
+    came) appended"""
     need_map = any(ctx.needs_input_grad[:6])
     need_cam = pose and any(ctx.needs_input_grad[6:9])
     # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward converts
@@ -209,9 +227,17 @@ def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, sca
         moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib,
                                            final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas,
                                            dloss_ddepth, dloss_dalpha, moments_only=True)
+    elif dloss_dgammas is None:  # (the feature class: no image gradient, no colour replay)
+        moments = torch.zeros((pws.shape[0], 9), dtype=torch.float32, device=pws.device)
     else:
         moments = ops.splatB(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True)
+    dfeat = None
+    if feat is not None and feat[1] is not None:
+        # the feature map's terms are added to moment rows 0-5: the conversion below sums both losses
+        moments, dfeat = ops.splatB_features(cam.height, cam.width, feat[0], contrib, final_tau, patch_range_per_tile,
+                                             gsid_per_patch, feat[1], moments=moments, us=us, cinv2ds=cinv2ds,
+                                             alphas=drawn, colors=colors)
     ex = None if rgbd or pose else getattr(cam, "grad_exchange", None)
     if ex is not None:
         # multi-view data parallel (parallel.GradExchange): the per-Gaussian backward pushes
@@ -235,7 +261,32 @@ def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, sca
         grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
     elif pose:
         grads += (None, None, None)
-    return grads
+    return grads + (dfeat,) if feat is not None else grads
+
+
+class GSFunctionFusedFeatures(torch.autograd.Function):
+    """GSFunctionFused with per-Gaussian features: `apply(pws, shs, alphas, scales, rots, us, features, cam,
+    filter3d=None)` -> (image[3,H,W], feature_map[D,H,W], depths > 0.2) with
+        feature_map[c, p] = sum_i w_i(p) features[i, c]
+    (w = tau alpha', the image's compositing weights; any width D >= 1; not view-dependent, no
+    offset).  Semantic or instance labels, distilled 2D features, normals, uncertainty.  Gradients
+    of both maps reach features and, through the rasterizers' moment rows, pws, alphas, scales,
+    rots and us (which feeds DensityController.update_density_info as for colour).  Composes with
+    Camera(..., antialiased=True) and filter3d.  A map the loss does not use costs nothing in the
+    backward: without an image gradient the colour replay is skipped, without a feature-map
+    gradient the feature replay.  Single view: cam.grad_exchange is refused."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, features, cam, filter3d=None):
+        if getattr(cam, "grad_exchange", None) is not None:
+            raise ValueError("GSFunctionFusedFeatures is single-view: cam.grad_exchange must not be set")
+        ctx.set_materialize_grads(False)
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d,
+                              features=features)
+
+    @staticmethod
+    def backward(ctx, dloss_dgammas, dloss_dfeature_map, _):
+        return _fused_backward(ctx, False, False, dloss_dgammas, featured=True, dloss_dfeatures_map=dloss_dfeature_map)
 
 
 class GSFunctionFusedPose(torch.autograd.Function):

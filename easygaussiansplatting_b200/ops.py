@@ -495,6 +495,103 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
 
 
 # ---------------------------------------------------------------------------------------
+# Feature rendering (extension): per-Gaussian feature vectors composited with the image's weights.
+def _feature_frame(height, width, features, contrib, patch_range_per_tile, gsid_per_patch, records, us, cinv2ds,
+                   alphas, colors):
+    """the checks both feature operators make -> (H, W, N, D, P, features, contrib, ranges, gsid,
+    the record pointer or None, (us, cinv2ds, alphas, colors) for a re-pack), on the device of features"""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    features = _chk(features, "features", ndim=2)
+    if features.shape[1] < 1:
+        raise ValueError("features must be [N, D] with D >= 1, got shape %s" % (tuple(features.shape),))
+    N, D = features.shape
+    contrib = _chk(contrib, "contrib", dtype=torch.int32)
+    ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
+    gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
+    _same_device(features, contrib, ranges, gsid)
+    if contrib.numel() != H * W:
+        raise ValueError("contrib does not match height x width")
+    if ranges.shape[0] != ((W + 15) // 16) * ((H + 15) // 16):
+        raise ValueError("patch_range_per_tile does not match the tile grid")
+    P = gsid.numel()
+    attrs = (None,) * 4
+    recs = None
+    if records is not None:
+        records = _chk(records, "records", last=12, ndim=2)
+        _same_device(features, records)
+        if records.shape[0] != N:
+            raise ValueError("records must be [N, 12]")
+        recs = records.data_ptr()
+    elif P > 0:
+        if any(x is None for x in (us, cinv2ds, alphas, colors)):
+            raise ValueError("give the forward's records, or us, cinv2ds, alphas and colors to find or re-pack them")
+        us = _chk(us, "us", last=2, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
+        alphas = _chk(alphas, "alphas"); colors = _chk(colors, "colors", last=3, ndim=2)
+        _same_device(features, us, cinv2ds, alphas, colors)
+        if not (us.shape[0] == N and cinv2ds.shape[0] == N and alphas.numel() == N and colors.shape[0] == N):
+            raise ValueError("features, us, cinv2ds, alphas and colors disagree on N")
+        attrs = (us, cinv2ds, alphas, colors)
+        recs = _cached_records(gsid, attrs)  # those `splat` attached, while its inputs are unchanged
+    return H, W, N, D, P, features, contrib, ranges, gsid, recs, attrs
+
+
+def splat_features(height, width, features, contrib, patch_range_per_tile, gsid_per_patch, records=None, us=None,
+                   cinv2ds=None, alphas=None, colors=None):
+    """The feature map of a frame `splat` (or `splat_rgbd`) drew (gsb_splat_features):
+        feature_map[c, p] = sum_i w_i(p) features[i, c],   w = tau alpha', the image's weights
+    features[N, D] (any D >= 1; f = the colours gives the image's bits).  contrib,
+    patch_range_per_tile, gsid_per_patch: that frame's outputs.  records: the forward's packed
+    records [N,12] (`preprocess(..., alphas=...)`'s, as given to `splat`); otherwise those `splat`
+    attached to gsid_per_patch are used while us, cinv2ds, alphas and colors (then required) are
+    the tensors it saw, unchanged, and re-packed from them if not.  -> feature_map[D, H, W]
+    (0 on tiles without patches).  Its backward is `splatB_features`."""
+    H, W, N, D, P, features, contrib, ranges, gsid, recs, attrs = _feature_frame(
+        height, width, features, contrib, patch_range_per_tile, gsid_per_patch, records, us, cinv2ds, alphas, colors)
+    dev = features.device
+    out = torch.empty((D, H, W), dtype=torch.float32, device=dev)
+    lib = _L()
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_splat_features_workspace_bytes(N, H, W, 0 if recs else P), dev)
+        _lib.check(lib.gsb_splat_features(H, W, N, P, D, *[_ptr(a) for a in attrs], _ptr(features), recs, _ptr(contrib),
+                                          _ptr(ranges), _ptr(gsid), _ptr(ws), ws.numel(), _ptr(out), _stream()), lib)
+    return out
+
+
+def splatB_features(height, width, features, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                    dloss_dfeature_map, moments=None, records=None, us=None, cinv2ds=None, alphas=None, colors=None):
+    """Backward of `splat_features` (gsb_splat_features_backward): dloss_dfeature_map[D, H, W] ->
+    (moments[N, 9], dloss_dfeatures[N, D]).  The feature map's dL/dalpha' enters moment rows 0-5,
+    the form `splatB(..., moments_only=True)` returns, so `preprocessB(..., moments=...)` turns
+    them into the geometry and opacity gradients.  moments: None (fresh rows, rows 6-8 zero), or
+    such rows (contiguous float32 [N, 9]) to ADD to in place -- chain it after
+    `splatB(..., moments_only=True)` / `splatB_rgbd` for a loss on both maps.  records, us,
+    cinv2ds, alphas, colors: as for `splat_features`."""
+    H, W, N, D, P, features, contrib, ranges, gsid, recs, attrs = _feature_frame(
+        height, width, features, contrib, patch_range_per_tile, gsid_per_patch, records, us, cinv2ds, alphas, colors)
+    final_tau = _chk(final_tau, "final_tau")
+    dl = _chk(dloss_dfeature_map, "dloss_dfeature_map")
+    _same_device(features, final_tau, dl)
+    if final_tau.numel() != H * W or dl.numel() != D * H * W:
+        raise ValueError("final_tau / dloss_dfeature_map do not match D x height x width")
+    dev = features.device
+    if moments is None:
+        moments = torch.zeros((N, 9), dtype=torch.float32, device=dev)
+    elif not (isinstance(moments, torch.Tensor) and moments.is_cuda and moments.dtype == torch.float32 and
+              tuple(moments.shape) == (N, 9) and moments.is_contiguous() and moments.device == dev):
+        raise ValueError("moments must be a contiguous float32 [N, 9] tensor on the device of features")
+    dfeat = torch.empty((N, D), dtype=torch.float32, device=dev)
+    lib = _L()
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_splat_features_workspace_bytes(N, H, W, 0 if recs else P), dev)
+        _lib.check(lib.gsb_splat_features_backward(
+            H, W, N, P, D, *[_ptr(a) for a in attrs], _ptr(features), recs, _ptr(contrib), _ptr(final_tau), _ptr(ranges),
+            _ptr(gsid), _ptr(dl), _ptr(ws), ws.numel(), _ptr(moments), _ptr(dfeat), _stream()), lib)
+    return moments, dfeat
+
+
+# ---------------------------------------------------------------------------------------
 # Extensions (not in the reference module): the fused per-Gaussian path, SURVEY 8f row N1.
 def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
                alphas=None, antialiased=False):

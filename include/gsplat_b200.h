@@ -346,6 +346,39 @@ int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, con
                             float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
                             float *dloss_ddepths, gsb_stream_t stream);
 
+/* ---- feature rendering (extension).  Composites per-Gaussian feature vectors features[N,D]
+ * (row-major, row stride D, any 4-byte alignment; D >= 1) with the image's weights:
+ *   feature_image[c, p] = sum_i w_i(p) features[i, c],   w_i = tau_i alpha'_i
+ * (the same clamp, skip and stop rules and the same fp32 operations as the colour image: a feature
+ * column equal to a colour channel composites to that image plane's bits).  Both calls replay a
+ * frame the colour forward binned and drew: its contrib, patch_range_per_tile (any alignment) and
+ * gsid_per_patch (P entries), and final_tau for the backward; the colour entry points are not
+ * involved.  packed_records: the forward's record array, or NULL -- the records are then packed
+ * into `ws` from us, cinv2ds, alphas and colors, as gsb_splat_backward does.  With P == 0 (or
+ * N == 0) nothing was drawn.  ws: gsb_splat_features_workspace_bytes(N, H, W, P) bytes, any
+ * alignment (P = 0 when packed_records is given); one workspace serves both calls.
+ * gsb_splat_features: -> feature_image[D,H,W] planar, 16-byte aligned like `image` (a misaligned
+ *   one is an argument error); every element written, 0 on tiles without patches.
+ * gsb_splat_features_backward: dloss_dfeature_image[D,H,W] (any 4-byte alignment) ->
+ *   moments[N,9] READ-MODIFY-WRITE: rows 0-5 (the geometry and opacity moments gsb_splat_backward
+ *     leaves with moments_out) are ADDED to, rows 6-8 are left alone, so the conversion of
+ *     gsb_splat_backward / gsb_preprocess_backward* yields the gradients of the sum of both losses;
+ *   dloss_dfeatures[N,D] = sum_p tau alpha' dL/dF(p) (every element written; 0 for Gaussians no
+ *     pixel replays, culled ones included; summed with float atomics).
+ * Argument errors: D < 1, a misaligned feature_image, and the tile-grid limit of the splat entry
+ * points (GSB_MAX_GRID_TILES). */
+size_t gsb_splat_features_workspace_bytes(int N, int H, int W, int64_t P);
+int gsb_splat_features(int H, int W, int N, int64_t P, int D, const float *us, const float *cinv2ds,
+                       const float *alphas, const float *colors, const float *features, const void *packed_records,
+                       const int32_t *contrib, const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                       void *ws, size_t ws_bytes, float *feature_image, gsb_stream_t stream);
+int gsb_splat_features_backward(int H, int W, int N, int64_t P, int D, const float *us, const float *cinv2ds,
+                                const float *alphas, const float *colors, const float *features,
+                                const void *packed_records, const int32_t *contrib, const float *final_tau,
+                                const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                                const float *dloss_dfeature_image, void *ws, size_t ws_bytes, float *moments,
+                                float *dloss_dfeatures, gsb_stream_t stream);
+
 /* ---- batched tiny matmul (extension).  C[b] = A[b] (m x k) . B[b] (k x n), or B shared by all
  * batches when b_shared != 0; dense row-major f32.  This is the product the reference's
  * GSFunction.backward applies ~12 times over the per-Gaussian Jacobians (gsmodel.py:72-85);
@@ -412,6 +445,14 @@ int gsb_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64
                       const gsb_gaussians *src, const gsb_gaussians *src_m, const gsb_gaussians *src_v,
                       const float *z, const gsb_gaussians *dst, const gsb_gaussians *dst_m,
                       const gsb_gaussians *dst_v, gsb_stream_t stream);
+
+/* The same plan applied to one more per-Gaussian tensor of any width D >= 1 (features[N,D],
+ * row-major f32): dst[K + C + S, D] gets the survivors in order, then the clones, then the
+ * splits, each new row a copy of its source row; src_m/src_v (Adam moments, same shape) -> dst_m/
+ * dst_v with zero rows for the new Gaussians.  src_m/src_v/dst_m/dst_v: NULL, or all four set. */
+int gsb_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C, int64_t S,
+                           int D, const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
+                           float *dst_v, gsb_stream_t stream);
 
 /* reset_alpha (:320-331): alphas_raw = min(alphas_raw, reset_raw); the alpha group's Adam
  * moments (nullable) are zeroed. */
