@@ -70,6 +70,14 @@ SIGNATURES = {
     "gsb_density_plan": (_i, [_i64, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _vp, _sz, _vp, _vp, C.POINTER(_i64), _vp]),
     "gsb_density_apply": (_i, [_i64, _vp, _vp, _i64, _i64, _i64, _gp, _gp, _gp, _vp, _gp, _gp, _gp, _vp]),
     "gsb_reset_alpha": (_i, [_i64, _vp, _vp, _vp, _f, _vp]),
+    "gsb_mcmc_workspace_bytes": (_sz, [_i64, _i64]),
+    "gsb_mcmc_plan": (_i, [_i64, _vp, _f, _i, _vp, _sz, C.POINTER(_i64), _vp]),
+    "gsb_mcmc_sample": (_i, [_i64, _i64, _vp, _vp, _sz, _vp, _vp]),
+    "gsb_mcmc_relocate": (_i, [_i64, _i64, _vp, _vp, _sz, C.c_double, _i, _gp, _gp, _gp, _vp]),
+    "gsb_mcmc_relocate_rows": (_i, [_i64, _i64, _vp, _vp, _sz, _i, _vp, _vp, _vp, _vp]),
+    "gsb_mcmc_grow": (_i, [_i64, _i64, _vp, _vp, _sz, C.c_double, _i, _gp, _gp, _gp, _gp, _gp, _gp, _vp]),
+    "gsb_mcmc_grow_rows": (_i, [_i64, _i64, _vp, _vp, _sz, _i] + [_vp] * 7),
+    "gsb_mcmc_noise": (_i, [_i64] + [_vp] * 5 + [_f, _f, _f, _vp]),
     "gsb_ply_rows_to_gs": (_i, [_i64, _i, _i, _vp, _vp, _vp, _vp]),
     "gsb_gs_to_params": (_i, [_i64, _i, _vp, _gp, _vp]),
     "gsb_params_to_gs": (_i, [_i64, _gp, _vp, _vp]),

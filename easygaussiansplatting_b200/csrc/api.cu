@@ -40,7 +40,9 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
                                              "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
-                                             "draw_features", "draw_backward_features", "draw_rgbd",
+                                             "draw_features", "draw_backward_features", "mcmc_scan",
+                                             "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
+                                             "mcmc_noise", "draw_rgbd",
                                              "draw_backward_rgbd"};
 
 ProfScope::ProfScope(int id, cudaStream_t st) : id_(id), st_(st), stop_(nullptr) {
@@ -812,6 +814,111 @@ int gsb_reset_alpha(int64_t N, float *alphas_raw, float *exp_avg, float *exp_avg
   GSB_REQUIRE(N >= 0, "reset_alpha: N < 0");
   GSB_REQUIRE(N == 0 || alphas_raw, "reset_alpha: null pointer");
   return launch_reset_alpha(N, alphas_raw, exp_avg, exp_avg_sq, reset_raw, (cudaStream_t)stream);
+}
+
+// ---- MCMC densification (density.cu)
+
+static const int64_t kMcmcMaxN = (int64_t)1 << 31;  // row ids are int32
+
+size_t gsb_mcmc_workspace_bytes(int64_t N, int64_t n) {
+  return mcmc_workspace_bytes(N < 0 ? 0 : N, n < 0 ? 0 : n);
+}
+
+#define GSB_MCMC_WS(ws, ws_bytes, N, n, what)                                                   \
+  do {                                                                                          \
+    GSB_REQUIRE(ws != nullptr && aligned(ws, 16), what ": workspace null or misaligned");      \
+    GSB_REQUIRE(ws_bytes >= mcmc_workspace_bytes(N, n), what ": workspace too small");          \
+  } while (0)
+
+int gsb_mcmc_plan(int64_t N, const float *alphas_raw, float alpha_raw_min, int mode, void *ws, size_t ws_bytes,
+                  int64_t *counts_host, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && N < kMcmcMaxN, "mcmc_plan: N out of range");
+  GSB_REQUIRE(mode == 0 || mode == 1, "mcmc_plan: mode must be 0 (relocate) or 1 (grow)");
+  GSB_REQUIRE(counts_host != nullptr, "mcmc_plan: counts_host is null");
+  if (N == 0) return counts_host[0] = counts_host[1] = 0, 0;
+  GSB_REQUIRE(alphas_raw != nullptr, "mcmc_plan: null pointer");
+  GSB_MCMC_WS(ws, ws_bytes, N, 0, "mcmc_plan");
+  return launch_mcmc_plan(N, alphas_raw, alpha_raw_min, mode, ws, counts_host, (cudaStream_t)stream);
+}
+
+int gsb_mcmc_sample(int64_t N, int64_t n, const double *u, void *ws, size_t ws_bytes, int32_t *sampled,
+                    gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && N < kMcmcMaxN && n >= 0, "mcmc_sample: bad counts");
+  GSB_REQUIRE(n == 0 || N > 0, "mcmc_sample: draws from no rows");
+  if (n == 0) return 0;
+  GSB_REQUIRE(u && sampled, "mcmc_sample: null pointer");
+  GSB_MCMC_WS(ws, ws_bytes, N, 0, "mcmc_sample");
+  return launch_mcmc_sample(N, n, u, ws, sampled, (cudaStream_t)stream);
+}
+
+static bool mcmc_moments_ok(const gsb_gaussians *m, const gsb_gaussians *v) {
+  return (m == nullptr) == (v == nullptr) && (m == nullptr || (gau_complete(m) && gau_complete(v)));
+}
+
+int gsb_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, size_t ws_bytes, double min_opacity,
+                      int n_max, const gsb_gaussians *params, const gsb_gaussians *exp_avg,
+                      const gsb_gaussians *exp_avg_sq, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && N < kMcmcMaxN && n >= 0 && n <= N, "mcmc_relocate: bad counts");
+  GSB_REQUIRE(n_max >= 1 && n_max <= 51, "mcmc_relocate: n_max must be in [1, 51]");
+  GSB_REQUIRE(min_opacity > 0.0 && min_opacity < 1.0, "mcmc_relocate: min_opacity must be in (0, 1)");
+  if (n == 0) return 0;
+  GSB_REQUIRE(sampled && gau_complete(params), "mcmc_relocate: null pointer");
+  GSB_REQUIRE(mcmc_moments_ok(exp_avg, exp_avg_sq), "mcmc_relocate: Adam moments must be both given or both NULL");
+  GSB_MCMC_WS(ws, ws_bytes, N, n, "mcmc_relocate");
+  return launch_mcmc_relocate(N, n, sampled, ws, min_opacity, n_max, gau_ptrs(params),
+                              exp_avg ? gau_ptrs(exp_avg) : nullptr, exp_avg_sq ? gau_ptrs(exp_avg_sq) : nullptr,
+                              (cudaStream_t)stream);
+}
+
+int gsb_mcmc_relocate_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, size_t ws_bytes, int D,
+                           float *x, float *exp_avg, float *exp_avg_sq, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && N < kMcmcMaxN && n >= 0 && n <= N && D >= 1, "mcmc_relocate_rows: bad counts");
+  if (n == 0) return 0;
+  GSB_REQUIRE(sampled && x, "mcmc_relocate_rows: null pointer");
+  GSB_REQUIRE((exp_avg == nullptr) == (exp_avg_sq == nullptr),
+              "mcmc_relocate_rows: Adam moments must be both given or both NULL");
+  GSB_MCMC_WS(ws, ws_bytes, N, 0, "mcmc_relocate_rows");
+  return launch_mcmc_relocate_rows(N, n, sampled, ws, D, x, exp_avg, exp_avg_sq, (cudaStream_t)stream);
+}
+
+int gsb_mcmc_grow(int64_t N, int64_t n, const int32_t *sampled, void *ws, size_t ws_bytes, double min_opacity,
+                  int n_max, const gsb_gaussians *src, const gsb_gaussians *src_m, const gsb_gaussians *src_v,
+                  const gsb_gaussians *dst, const gsb_gaussians *dst_m, const gsb_gaussians *dst_v,
+                  gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && n >= 0 && N + n < kMcmcMaxN, "mcmc_grow: bad counts");
+  GSB_REQUIRE(n_max >= 1 && n_max <= 51, "mcmc_grow: n_max must be in [1, 51]");
+  GSB_REQUIRE(min_opacity > 0.0 && min_opacity < 1.0, "mcmc_grow: min_opacity must be in (0, 1)");
+  GSB_REQUIRE(n == 0 || N > 0, "mcmc_grow: draws from no rows");
+  if (N == 0) return 0;
+  GSB_REQUIRE(gau_complete(src) && gau_complete(dst) && (n == 0 || sampled), "mcmc_grow: null pointer");
+  const bool state = src_m != nullptr;
+  GSB_REQUIRE(mcmc_moments_ok(src_m, src_v) && mcmc_moments_ok(dst_m, dst_v) && (dst_m != nullptr) == state,
+              "mcmc_grow: Adam moments must be all given or all NULL");
+  GSB_MCMC_WS(ws, ws_bytes, N, n, "mcmc_grow");
+  return launch_mcmc_grow(N, n, sampled, ws, min_opacity, n_max, gau_ptrs(src), state ? gau_ptrs(src_m) : nullptr,
+                          state ? gau_ptrs(src_v) : nullptr, gau_ptrs(dst), state ? gau_ptrs(dst_m) : nullptr,
+                          state ? gau_ptrs(dst_v) : nullptr, (cudaStream_t)stream);
+}
+
+int gsb_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, size_t ws_bytes, int D,
+                       const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
+                       float *dst_v, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && n >= 0 && N + n < kMcmcMaxN && D >= 1, "mcmc_grow_rows: bad counts");
+  GSB_REQUIRE(n == 0 || N > 0, "mcmc_grow_rows: draws from no rows");
+  if (N == 0) return 0;
+  GSB_REQUIRE(src && dst && (n == 0 || sampled), "mcmc_grow_rows: null pointer");
+  const bool state = src_m != nullptr;
+  GSB_REQUIRE((src_v != nullptr) == state && (dst_m != nullptr) == state && (dst_v != nullptr) == state,
+              "mcmc_grow_rows: Adam moments must be all given or all NULL");
+  GSB_MCMC_WS(ws, ws_bytes, N, 0, "mcmc_grow_rows");
+  return launch_mcmc_grow_rows(N, n, sampled, ws, D, src, src_m, src_v, dst, dst_m, dst_v, (cudaStream_t)stream);
+}
+
+int gsb_mcmc_noise(int64_t N, float *pws, const float *alphas_raw, const float *scales_raw, const float *rots_raw,
+                   const float *z, float scale, float k, float x0, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0, "mcmc_noise: N < 0");
+  GSB_REQUIRE(N == 0 || (pws && alphas_raw && scales_raw && rots_raw && z), "mcmc_noise: null pointer");
+  return launch_mcmc_noise(N, pws, alphas_raw, scales_raw, rots_raw, z, scale, k, x0, (cudaStream_t)stream);
 }
 
 static bool sh_dim_ok(int d) { return d == 3 || d == 12 || d == 27 || d == 48; }

@@ -19,6 +19,7 @@
 // within an ulp of the reference's.
 #include "common.cuh"
 #include "kernels.h"
+#include "pg_fused_math.h"
 #include "tile_io.cuh"
 
 namespace gsb {
@@ -571,6 +572,395 @@ inline int stream_grid(int64_t total, int block) {
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
+// ---- MCMC densification (Kheradmand et al. 2024): relocate dead Gaussians onto live ones, grow
+// to a budget, covariance-shaped position noise.  DESIGN 3.11.
+//
+// The sampler is integer arithmetic so that its ids do not depend on summation order: row i has
+// the weight q_i = floor(o_i 2^32) (o_i = sigmoid of the fp32 raw value, in fp64; 0 for excluded
+// rows), W = the uint64 inclusive prefix sum, and a uniform u picks the first i with
+// W_i > floor(u W_total).  The scan has the density scan's three-kernel shape:
+//   k_mcmc_weight_count  per-CTA weight sum and dead count of 1024 rows;
+//   k_mcmc_scan_blocks   one CTA turns them into exclusive offsets and the totals;
+//   k_mcmc_prefix        every CTA rescans its rows, writes W, the dead-row list, and clears the
+//                        per-row sample counts.
+enum : int { MCMC_RELOCATE = 0, MCMC_GROW = 1 };
+
+// relocate samples alive rows (dead = !(a > alpha_raw_min), NaN included); grow samples every
+// row that is not NaN
+__device__ __forceinline__ uint64_t mcmc_weight(float a, float alpha_raw_min, int mode, bool &dead) {
+  dead = !(a > alpha_raw_min);
+  if (isnan(a) || (mode == MCMC_RELOCATE && dead)) return 0;
+  const double o = 1.0 / (1.0 + exp(-(double)a));
+  return (uint64_t)floor(o * 4294967296.0);
+}
+
+__device__ __forceinline__ uint64_t warp_sum_u64(uint64_t x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  return x;
+}
+
+__global__ void __launch_bounds__(SC_THREADS) k_mcmc_weight_count(int64_t N, const float *__restrict__ alphas_raw,
+                                                                   float alpha_raw_min, int mode,
+                                                                   uint64_t *__restrict__ block_w,
+                                                                   int32_t *__restrict__ block_dead) {
+  __shared__ uint64_t red_w[SC_THREADS / 32];
+  __shared__ uint32_t red_d[SC_THREADS / 32];
+  uint64_t w = 0;
+  uint32_t d = 0;
+#pragma unroll
+  for (int j = 0; j < SC_PER; j++) {
+    const int64_t i = (int64_t)blockIdx.x * SC_ROWS + j * SC_THREADS + threadIdx.x;
+    if (i < N) {
+      bool dd;
+      w += mcmc_weight(alphas_raw[i], alpha_raw_min, mode, dd);
+      d += dd;
+    }
+  }
+  w = warp_sum_u64(w);
+  d = __reduce_add_sync(0xffffffffu, d);
+  if ((threadIdx.x & 31) == 0) red_w[threadIdx.x >> 5] = w, red_d[threadIdx.x >> 5] = d;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint64_t a = 0;
+    uint32_t b = 0;
+#pragma unroll
+    for (int k = 0; k < SC_THREADS / 32; k++) a += red_w[k], b += red_d[k];
+    block_w[blockIdx.x] = a;
+    block_dead[blockIdx.x] = (int32_t)b;
+  }
+}
+
+// in place: block sums -> the sums before each CTA; totals = (W_total, dead count)
+__global__ void __launch_bounds__(1024) k_mcmc_scan_blocks(int nb, uint64_t *__restrict__ block_w,
+                                                           int32_t *__restrict__ block_dead,
+                                                           int64_t *__restrict__ totals) {
+  __shared__ uint64_t tot_w[32];
+  __shared__ int tot_d[32];
+  __shared__ uint64_t carry_w;
+  __shared__ int carry_d;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (threadIdx.x == 0) carry_w = 0, carry_d = 0;
+  __syncthreads();
+  for (int base = 0; base < nb; base += 1024) {
+    const int b = base + threadIdx.x;
+    const uint64_t vw = b < nb ? block_w[b] : 0;
+    const int vd = b < nb ? block_dead[b] : 0;
+    uint64_t iw = vw;
+    int id = vd;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint64_t yw = __shfl_up_sync(0xffffffffu, iw, o);
+      const int yd = __shfl_up_sync(0xffffffffu, id, o);
+      if (lane >= o) iw += yw, id += yd;
+    }
+    if (lane == 31) tot_w[wid] = iw, tot_d[wid] = id;
+    __syncthreads();
+    uint64_t ew = carry_w + iw - vw;
+    int ed = carry_d + id - vd;
+    for (int k = 0; k < wid; k++) ew += tot_w[k], ed += tot_d[k];
+    if (b < nb) block_w[b] = ew, block_dead[b] = ed;
+    __syncthreads();
+    if (threadIdx.x == 1023) carry_w = ew + vw, carry_d = ed + vd;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) totals[0] = (int64_t)carry_w, totals[1] = carry_d;
+}
+
+__global__ void __launch_bounds__(SC_THREADS) k_mcmc_prefix(int64_t N, const float *__restrict__ alphas_raw,
+                                                             float alpha_raw_min, int mode,
+                                                             const uint64_t *__restrict__ block_w,
+                                                             const int32_t *__restrict__ block_dead,
+                                                             uint64_t *__restrict__ W, int32_t *__restrict__ dead,
+                                                             int32_t *__restrict__ count) {
+  __shared__ uint64_t tot_w[SC_THREADS / 32];
+  __shared__ uint32_t tot_d[SC_THREADS / 32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int64_t row0 = (int64_t)blockIdx.x * SC_ROWS + (int64_t)threadIdx.x * SC_PER;
+  uint64_t w[SC_PER], sw = 0;
+  bool dd[SC_PER];
+  uint32_t sd = 0;
+#pragma unroll
+  for (int j = 0; j < SC_PER; j++) {
+    w[j] = 0, dd[j] = false;
+    if (row0 + j < N) w[j] = mcmc_weight(alphas_raw[row0 + j], alpha_raw_min, mode, dd[j]);
+    sw += w[j], sd += dd[j];
+  }
+  uint64_t iw = sw;
+  uint32_t id = sd;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint64_t a = __shfl_up_sync(0xffffffffu, iw, o);
+    const uint32_t b = __shfl_up_sync(0xffffffffu, id, o);
+    if (lane >= o) iw += a, id += b;
+  }
+  if (lane == 31) tot_w[wid] = iw, tot_d[wid] = id;
+  __syncthreads();
+  uint64_t rw = block_w[blockIdx.x] + iw - sw;
+  int rd = block_dead[blockIdx.x] + (int)(id - sd);
+  for (int k = 0; k < wid; k++) rw += tot_w[k], rd += (int)tot_d[k];
+#pragma unroll
+  for (int j = 0; j < SC_PER; j++) {
+    const int64_t i = row0 + j;
+    if (i >= N) break;
+    rw += w[j];
+    W[i] = rw;
+    count[i] = 0;
+    if (mode == MCMC_RELOCATE && dd[j]) dead[rd++] = (int)i;
+  }
+}
+
+// sampled[j] = the first i with W_i > t_j, t_j = min(floor(u_j W_total), W_total - 1); count[i] =
+// how many draws hit row i
+__global__ void k_mcmc_sample(int64_t N, int64_t n, const double *__restrict__ u, const uint64_t *__restrict__ W,
+                              const int64_t *__restrict__ totals, int32_t *__restrict__ sampled,
+                              int32_t *__restrict__ count) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint64_t total = (uint64_t)totals[0];
+  uint64_t t = (uint64_t)floor(u[j] * (double)total);
+  if (t >= total) t = total - 1;
+  int64_t lo = 0, hi = N - 1;  // W_{N-1} = total > t: the answer is in [lo, hi]
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (W[mid] > t) hi = mid;
+    else lo = mid + 1;
+  }
+  sampled[j] = (int32_t)lo;
+  atomicAdd(count + lo, 1);
+}
+
+// The relocation value of a source hit c times, in fp64 (DESIGN 3.11): r = min(c + 1, n_max) copies
+// share its opacity, o' = 1 - (1 - o)^(1/r), and its scale shrinks by o / sum_m C(r,m) (-1)^(m+1)
+// o'^m / sqrt(m), so that the r copies together render what the source did.  The alternating sum's
+// terms reach ~2e5 at r = 51 against a result of order 1: an fp32 evaluation would lose most of
+// its digits.  Each output is rounded to fp32 once.
+__device__ __forceinline__ float4 relocation_value(float a, const float *__restrict__ s3, int c, double min_opacity,
+                                                   int n_max) {
+  const int r = min(c + 1, n_max);
+  // o and 1 - o each from its own sigmoid: 1 - o formed from o would keep no digits of a nearly
+  // opaque source's transparency, and o' and logit(o') are made from it
+  const double o = 1.0 / (1.0 + exp(-(double)a)), om = 1.0 / (1.0 + exp((double)a));
+  double op = o, q = om;  // o' and 1 - o'; r = 1 keeps o exactly (the scale factor is then 1)
+  if (r > 1) q = pow(om, 1.0 / r), op = 1.0 - q;
+  if (op < min_opacity) op = min_opacity, q = 1.0 - min_opacity;
+  else if (q < 0x1p-23) q = 0x1p-23, op = 1.0 - 0x1p-23;
+  double denom = 0.0, binom = 1.0, p = 1.0;
+  for (int m = 1; m <= r; m++) {
+    binom = binom * (double)(r - m + 1) / (double)m;  // C(r, m), exact for r <= 51
+    p *= op;
+    const double term = binom * p / sqrt((double)m);
+    denom += (m & 1) ? term : -term;
+  }
+  const double f = log(o / denom);
+  return make_float4((float)log(op / q), (float)((double)s3[0] + f), (float)((double)s3[1] + f),
+                     (float)((double)s3[2] + f));
+}
+
+// vals[j] = the relocation value of sampled[j], from the unmodified source, before any row moves
+__global__ void k_mcmc_values(int64_t n, const int32_t *__restrict__ sampled, const int32_t *__restrict__ count,
+                              const float *__restrict__ alphas_raw, const float *__restrict__ scales_raw,
+                              double min_opacity, int n_max, float4 *__restrict__ vals) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const int64_t i = sampled[j];
+  vals[j] = relocation_value(alphas_raw[i], scales_raw + 3 * i, count[i], min_opacity, n_max);
+}
+
+// One more per-Gaussian tensor [N, D] and its Adam moments (m, v: both or neither) for the
+// row-moving kernels below; the six training tensors are jobs 0-5 (kWidth), an extra tensor job 6.
+struct McmcJob {
+  const float *p, *m, *v;  // sources
+  float *dp, *dm, *dv;     // destinations (grow: fresh [N + n] tensors; relocate: the sources)
+  int w;
+};
+struct McmcJobs {
+  McmcJob j[6];
+};
+
+// the value a sampled source row gets at column c (alphas_raw, scales_raw: the relocation value)
+template <int A>
+__device__ __forceinline__ float source_value(const float *__restrict__ p, int64_t src, int c, int w,
+                                              const float4 &val) {
+  if (A == 3) return val.x;
+  if (A == 4) return c == 0 ? val.y : (c == 1 ? val.z : val.w);
+  return p[src * w + c];
+}
+
+// relocate, in place: the source's opacity and scale become the relocation value, dead row dead[j]
+// becomes a copy of the updated source sampled[j]; the moments of both rows are zeroed.  The new
+// values come from vals[] and every other column of a source is only read (a source is alive, a
+// destination dead), so several dead rows may copy one source in any order.
+template <int A>
+__device__ __forceinline__ void relocate_job(int64_t n, const int32_t *__restrict__ sampled,
+                                             const int32_t *__restrict__ dead, const float4 *__restrict__ vals,
+                                             const McmcJob &J) {
+  const int w = A < 6 ? kWidth[A < 6 ? A : 0] : J.w;
+  const int64_t total = n * w, stride = (int64_t)gridDim.x * blockDim.x;
+  float *__restrict__ p = J.dp;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += stride) {
+    const int64_t j = e / w;
+    const int c = (int)(e - j * w);
+    const int64_t src = sampled[j], dst = dead[j];
+    float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (A == 3 || A == 4) val = vals[j];
+    const float x = source_value<A>(p, src, c, w, val);
+    p[dst * w + c] = x;
+    if (A == 3 || A == 4) p[src * w + c] = x;
+    if (J.dm) {
+      J.dm[src * w + c] = 0.f, J.dm[dst * w + c] = 0.f;
+      J.dv[src * w + c] = 0.f, J.dv[dst * w + c] = 0.f;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) k_mcmc_relocate(int64_t n, const int32_t *__restrict__ sampled,
+                                                       const int32_t *__restrict__ dead,
+                                                       const float4 *__restrict__ vals,
+                                                       const __grid_constant__ McmcJobs J) {
+  switch (blockIdx.y) {
+    case 0: relocate_job<0>(n, sampled, dead, vals, J.j[0]); break;
+    case 1: relocate_job<1>(n, sampled, dead, vals, J.j[1]); break;
+    case 2: relocate_job<2>(n, sampled, dead, vals, J.j[2]); break;
+    case 3: relocate_job<3>(n, sampled, dead, vals, J.j[3]); break;
+    case 4: relocate_job<4>(n, sampled, dead, vals, J.j[4]); break;
+    case 5: relocate_job<5>(n, sampled, dead, vals, J.j[5]); break;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_mcmc_relocate_rows(int64_t n, const int32_t *__restrict__ sampled,
+                                                            const int32_t *__restrict__ dead,
+                                                            const __grid_constant__ McmcJob J) {
+  relocate_job<6>(n, sampled, dead, nullptr, J);
+}
+
+// grow, part 1: rows [0, N) of the fresh tensors are the old rows; a sampled source (count > 0)
+// gets zero moments.  blockIdx.y = the set (parameter, exp_avg, exp_avg_sq); four independent
+// elements in flight per thread.
+template <int A>
+__device__ __forceinline__ void grow_copy_job(int64_t N, const int32_t *__restrict__ count, const McmcJob &J,
+                                              int set) {
+  const int w = A < 6 ? kWidth[A < 6 ? A : 0] : J.w;
+  const float *__restrict__ src = set == 0 ? J.p : (set == 1 ? J.m : J.v);
+  float *__restrict__ dst = set == 0 ? J.dp : (set == 1 ? J.dm : J.dv);
+  if (src == nullptr) return;
+  constexpr int U = 4;
+  const int64_t total = N * w, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e0 < total; e0 += stride * U) {
+    float x[U];
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      const int64_t e = e0 + u * stride;
+      x[u] = 0.f;
+      if (e < total && (set == 0 || count[e / w] == 0)) x[u] = src[e];
+    }
+#pragma unroll
+    for (int u = 0; u < U; u++) {
+      const int64_t e = e0 + u * stride;
+      if (e < total) dst[e] = x[u];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) k_mcmc_grow_copy(int64_t N, const int32_t *__restrict__ count,
+                                                        const __grid_constant__ McmcJobs J) {
+  const int set = blockIdx.y % 3;
+  switch (blockIdx.y / 3) {
+    case 0: grow_copy_job<0>(N, count, J.j[0], set); break;
+    case 1: grow_copy_job<1>(N, count, J.j[1], set); break;
+    case 2: grow_copy_job<2>(N, count, J.j[2], set); break;
+    case 3: grow_copy_job<3>(N, count, J.j[3], set); break;
+    case 4: grow_copy_job<4>(N, count, J.j[4], set); break;
+    case 5: grow_copy_job<5>(N, count, J.j[5], set); break;
+  }
+}
+
+// grow, part 2 (after part 1): row N + j is a copy of the updated source sampled[j] with zero
+// moments, and the source row itself gets the relocation value
+template <int A>
+__device__ __forceinline__ void grow_append_job(int64_t N, int64_t n, const int32_t *__restrict__ sampled,
+                                                const float4 *__restrict__ vals, const McmcJob &J) {
+  const int w = A < 6 ? kWidth[A < 6 ? A : 0] : J.w;
+  const int64_t total = n * w, stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += stride) {
+    const int64_t j = e / w;
+    const int c = (int)(e - j * w);
+    const int64_t src = sampled[j], dst = N + j;
+    float4 val = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (A == 3 || A == 4) val = vals[j];
+    const float x = source_value<A>(J.p, src, c, w, val);
+    J.dp[dst * w + c] = x;
+    if (A == 3 || A == 4) J.dp[src * w + c] = x;
+    if (J.dm) J.dm[dst * w + c] = 0.f, J.dv[dst * w + c] = 0.f;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_mcmc_grow_append(int64_t N, int64_t n, const int32_t *__restrict__ sampled,
+                                                          const float4 *__restrict__ vals,
+                                                          const __grid_constant__ McmcJobs J) {
+  switch (blockIdx.y) {
+    case 0: grow_append_job<0>(N, n, sampled, vals, J.j[0]); break;
+    case 1: grow_append_job<1>(N, n, sampled, vals, J.j[1]); break;
+    case 2: grow_append_job<2>(N, n, sampled, vals, J.j[2]); break;
+    case 3: grow_append_job<3>(N, n, sampled, vals, J.j[3]); break;
+    case 4: grow_append_job<4>(N, n, sampled, vals, J.j[4]); break;
+    case 5: grow_append_job<5>(N, n, sampled, vals, J.j[5]); break;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *__restrict__ count,
+                                                        const int32_t *__restrict__ sampled,
+                                                        const __grid_constant__ McmcJob J, int part) {
+  if (part == 0) grow_copy_job<6>(N, count, J, blockIdx.y);
+  else if (blockIdx.y == 0) grow_append_job<6>(N, n, sampled, nullptr, J);
+}
+
+// pws += Sigma(q, s) z * scale / (1 + exp(-k ((1 - o) - x0))), Sigma = R S^2 R^T of the normalised
+// quaternion and the raw scales (pg_fused_math.h), scale = lr * noise_lr.  68 B per Gaussian.
+__global__ void __launch_bounds__(256) k_mcmc_noise(int64_t N, float *__restrict__ pws,
+                                                    const float *__restrict__ alphas_raw,
+                                                    const float *__restrict__ scales_raw,
+                                                    const float *__restrict__ rots_raw, const float *__restrict__ z,
+                                                    float scale, float k, float x0) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  // the gate in fp64: it is steep (slope k / 4) where 1 - o crosses x0, so an fp32 1 - o would
+  // carry ~1e-5 relative error into it; ~40 fp64 operations per Gaussian are hidden by the loads
+  const double one_minus_o = 1.0 / (1.0 + exp((double)alphas_raw[i]));
+  const float gate = (float)(1.0 / (1.0 + exp(-(double)k * (one_minus_o - (double)x0))));
+  float q[4] = {rots_raw[4 * i], rots_raw[4 * i + 1], rots_raw[4 * i + 2], rots_raw[4 * i + 3]};
+  const float nq = fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
+#pragma unroll
+  for (int c = 0; c < 4; c++) q[c] /= nq;
+  const float s[3] = {expf(scales_raw[3 * i]), expf(scales_raw[3 * i + 1]), expf(scales_raw[3 * i + 2])};
+  float R3[9], M3[9], S6[6];
+  pg::cov3d(q, s, R3, M3, S6);
+  const float z0 = z[3 * i], z1 = z[3 * i + 1], z2 = z[3 * i + 2];
+  const float f = scale * gate;
+  pws[3 * i] += f * (S6[0] * z0 + S6[1] * z1 + S6[2] * z2);
+  pws[3 * i + 1] += f * (S6[1] * z0 + S6[3] * z1 + S6[4] * z2);
+  pws[3 * i + 2] += f * (S6[2] * z0 + S6[4] * z1 + S6[5] * z2);
+}
+
+// [totals: W_total, dead count; 256 B][block weight sums: nb u64][block dead counts: nb i32, 256-B
+// padded][W: N u64][count: N i32][dead: N i32][vals: n float4]
+struct McmcLayout {
+  size_t block_w, block_dead, W, count, dead, vals, bytes;
+};
+inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
+McmcLayout mcmc_layout(int64_t N, int64_t n) {
+  McmcLayout L;
+  const size_t nb = (size_t)((N + SC_ROWS - 1) / SC_ROWS) + 1;
+  L.block_w = 256;
+  L.block_dead = up256(L.block_w + nb * 8);
+  L.W = up256(L.block_dead + nb * 4);
+  L.count = up256(L.W + (size_t)N * 8);
+  L.dead = up256(L.count + (size_t)N * 4);
+  L.vals = up256(L.dead + (size_t)N * 4);
+  L.bytes = up256(L.vals + (size_t)n * 16);
+  return L;
+}
+
 }  // namespace
 
 size_t density_workspace_bytes(int64_t N) {
@@ -688,6 +1078,136 @@ int launch_params_to_gs(int64_t N, float *const *src, float *gs, cudaStream_t st
   if (N == 0) return 0;
   ProfScope ps(K_PARAMS_TO_GS, st);
   k_params_to_gs<<<stream_grid(N * 59, 256), 256, 0, st>>>(N, src[0], src[1], src[2], src[3], src[4], src[5], gs);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// ---- MCMC densification
+size_t mcmc_workspace_bytes(int64_t N, int64_t n) { return mcmc_layout(N, n).bytes; }
+
+int launch_mcmc_plan(int64_t N, const float *alphas_raw, float alpha_raw_min, int mode, void *ws,
+                     int64_t *counts_host, cudaStream_t st) {
+  counts_host[0] = counts_host[1] = 0;
+  if (N == 0) return 0;
+  const McmcLayout L = mcmc_layout(N, 0);
+  char *b = static_cast<char *>(ws);
+  int64_t *totals = reinterpret_cast<int64_t *>(b);
+  uint64_t *block_w = reinterpret_cast<uint64_t *>(b + L.block_w);
+  int32_t *block_dead = reinterpret_cast<int32_t *>(b + L.block_dead);
+  const int nb = (int)((N + SC_ROWS - 1) / SC_ROWS);
+  {
+    ProfScope ps(K_MCMC_SCAN, st);
+    k_mcmc_weight_count<<<nb, SC_THREADS, 0, st>>>(N, alphas_raw, alpha_raw_min, mode, block_w, block_dead);
+    k_mcmc_scan_blocks<<<1, 1024, 0, st>>>(nb, block_w, block_dead, totals);
+    k_mcmc_prefix<<<nb, SC_THREADS, 0, st>>>(N, alphas_raw, alpha_raw_min, mode, block_w, block_dead,
+                                             reinterpret_cast<uint64_t *>(b + L.W),
+                                             reinterpret_cast<int32_t *>(b + L.dead),
+                                             reinterpret_cast<int32_t *>(b + L.count));
+    GSB_CUDA_TRY(cudaGetLastError());
+  }
+  GSB_CUDA_TRY(cudaMemcpyAsync(counts_host, totals, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  GSB_CUDA_TRY(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int launch_mcmc_sample(int64_t N, int64_t n, const double *u, void *ws, int32_t *sampled, cudaStream_t st) {
+  if (n == 0) return 0;
+  const McmcLayout L = mcmc_layout(N, 0);
+  char *b = static_cast<char *>(ws);
+  ProfScope ps(K_MCMC_SAMPLE, st);
+  k_mcmc_sample<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(N, n, u, reinterpret_cast<const uint64_t *>(b + L.W),
+                                                             reinterpret_cast<const int64_t *>(b), sampled,
+                                                             reinterpret_cast<int32_t *>(b + L.count));
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+static int launch_mcmc_values(int64_t N, int64_t n, const int32_t *sampled, void *ws, const float *alphas_raw,
+                              const float *scales_raw, double min_opacity, int n_max, cudaStream_t st) {
+  const McmcLayout L = mcmc_layout(N, n);
+  char *b = static_cast<char *>(ws);
+  k_mcmc_values<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, sampled, reinterpret_cast<const int32_t *>(b + L.count),
+                                                             alphas_raw, scales_raw, min_opacity, n_max,
+                                                             reinterpret_cast<float4 *>(b + L.vals));
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+static McmcJobs mcmc_jobs(float *const *src, float *const *src_m, float *const *src_v, float *const *dst,
+                          float *const *dst_m, float *const *dst_v) {
+  McmcJobs J;
+  for (int a = 0; a < 6; a++)
+    J.j[a] = McmcJob{src[a], src_m ? src_m[a] : nullptr, src_v ? src_v[a] : nullptr, dst[a],
+                     dst_m ? dst_m[a] : nullptr, dst_v ? dst_v[a] : nullptr, kWidth[a]};
+  return J;
+}
+
+int launch_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, double min_opacity, int n_max,
+                         float *const *p, float *const *m, float *const *v, cudaStream_t st) {
+  if (n == 0) return 0;
+  ProfScope ps(K_MCMC_RELOCATE, st);
+  if (int rc = launch_mcmc_values(N, n, sampled, ws, p[3], p[4], min_opacity, n_max, st)) return rc;
+  const McmcLayout L = mcmc_layout(N, n);
+  char *b = static_cast<char *>(ws);
+  const dim3 grid(stream_grid(n * 45, 256), 6);
+  k_mcmc_relocate<<<grid, 256, 0, st>>>(n, sampled, reinterpret_cast<const int32_t *>(b + L.dead),
+                                        reinterpret_cast<const float4 *>(b + L.vals), mcmc_jobs(p, m, v, p, m, v));
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_mcmc_relocate_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, int D, float *x,
+                              float *m, float *v, cudaStream_t st) {
+  if (n == 0) return 0;
+  ProfScope ps(K_MCMC_ROWS, st);
+  const McmcLayout L = mcmc_layout(N, 0);
+  const McmcJob J{x, m, v, x, m, v, D};
+  k_mcmc_relocate_rows<<<stream_grid(n * D, 256), 256, 0, st>>>(
+      n, sampled, reinterpret_cast<const int32_t *>(static_cast<const char *>(ws) + L.dead), J);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_mcmc_grow(int64_t N, int64_t n, const int32_t *sampled, void *ws, double min_opacity, int n_max,
+                     float *const *src, float *const *src_m, float *const *src_v, float *const *dst,
+                     float *const *dst_m, float *const *dst_v, cudaStream_t st) {
+  if (N == 0) return 0;
+  ProfScope ps(K_MCMC_GROW, st);
+  const McmcLayout L = mcmc_layout(N, n);
+  char *b = static_cast<char *>(ws);
+  const McmcJobs J = mcmc_jobs(src, src_m, src_v, dst, dst_m, dst_v);
+  const dim3 grid(stream_grid((N * 45 + 3) / 4, 256), 18);
+  k_mcmc_grow_copy<<<grid, 256, 0, st>>>(N, reinterpret_cast<const int32_t *>(b + L.count), J);
+  GSB_CUDA_TRY(cudaGetLastError());
+  if (n == 0) return 0;
+  if (int rc = launch_mcmc_values(N, n, sampled, ws, src[3], src[4], min_opacity, n_max, st)) return rc;
+  k_mcmc_grow_append<<<dim3(stream_grid(n * 45, 256), 6), 256, 0, st>>>(
+      N, n, sampled, reinterpret_cast<const float4 *>(b + L.vals), J);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, int D, const float *src,
+                          const float *src_m, const float *src_v, float *dst, float *dst_m, float *dst_v,
+                          cudaStream_t st) {
+  if (N == 0) return 0;
+  ProfScope ps(K_MCMC_ROWS, st);
+  const McmcLayout L = mcmc_layout(N, 0);
+  const int32_t *count = reinterpret_cast<const int32_t *>(static_cast<const char *>(ws) + L.count);
+  const McmcJob J{src, src_m, src_v, dst, dst_m, dst_v, D};
+  k_mcmc_grow_rows<<<dim3(stream_grid((N * D + 3) / 4, 256), 3), 256, 0, st>>>(N, n, count, sampled, J, 0);
+  GSB_CUDA_TRY(cudaGetLastError());
+  if (n == 0) return 0;
+  k_mcmc_grow_rows<<<stream_grid(n * D, 256), 256, 0, st>>>(N, n, count, sampled, J, 1);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_mcmc_noise(int64_t N, float *pws, const float *alphas_raw, const float *scales_raw, const float *rots_raw,
+                      const float *z, float scale, float k, float x0, cudaStream_t st) {
+  if (N == 0) return 0;
+  ProfScope ps(K_MCMC_NOISE, st);
+  k_mcmc_noise<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(N, pws, alphas_raw, scales_raw, rots_raw, z, scale, k, x0);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -16,7 +16,8 @@ enum KernelId {
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
-  K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
+  K_MCMC_ROWS, K_MCMC_NOISE, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -150,6 +151,25 @@ int launch_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slot
                               const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
                               float *dst_v, cudaStream_t st);
 int launch_reset_alpha(int64_t N, float *alphas_raw, float *m, float *v, float val, cudaStream_t st);
+// MCMC densification (density.cu, DESIGN 3.11).  ws: mcmc_workspace_bytes(N, n) bytes, 256-B
+// aligned, shared by the calls of one relocate / grow; mode 0 samples alive rows (relocate) and
+// lists the dead ones, mode 1 samples every non-NaN row (grow).  counts_host <- (W_total, dead count).
+size_t mcmc_workspace_bytes(int64_t N, int64_t n);
+int launch_mcmc_plan(int64_t N, const float *alphas_raw, float alpha_raw_min, int mode, void *ws,
+                     int64_t *counts_host, cudaStream_t st);
+int launch_mcmc_sample(int64_t N, int64_t n, const double *u, void *ws, int32_t *sampled, cudaStream_t st);
+int launch_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, double min_opacity, int n_max,
+                         float *const *p, float *const *m, float *const *v, cudaStream_t st);
+int launch_mcmc_relocate_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, int D, float *x,
+                              float *m, float *v, cudaStream_t st);
+int launch_mcmc_grow(int64_t N, int64_t n, const int32_t *sampled, void *ws, double min_opacity, int n_max,
+                     float *const *src, float *const *src_m, float *const *src_v, float *const *dst,
+                     float *const *dst_m, float *const *dst_v, cudaStream_t st);
+int launch_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, int D, const float *src,
+                          const float *src_m, const float *src_v, float *dst, float *dst_m, float *dst_v,
+                          cudaStream_t st);
+int launch_mcmc_noise(int64_t N, float *pws, const float *alphas_raw, const float *scales_raw, const float *rots_raw,
+                      const float *z, float scale, float k, float x0, cudaStream_t st);
 int launch_ply_rows_to_gs(int64_t N, int stride, int sh_dim, const float *rows, const int32_t *colmap, float *gs,
                           cudaStream_t st);
 int launch_gs_to_params(int64_t N, int sh_dim, const float *gs, float *const *dst, cudaStream_t st);

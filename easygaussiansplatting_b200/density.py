@@ -243,3 +243,216 @@ class DensityController:
         if st is not None and "exp_avg" in st:
             m, v = _check(st["exp_avg"], "exp_avg"), _check(st["exp_avg_sq"], "exp_avg_sq")
         _lib.check(lib.gsb_reset_alpha(a.shape[0], _ptr(a), _ptr(m), _ptr(v), val, _stream()), lib)
+
+
+# ----------------------------------------------------------------------------- MCMC densification
+
+MCMC_RELOCATE, MCMC_GROW = 0, 1
+
+
+def mcmc_plan(alphas_raw, alpha_raw_min, mode, n_draws):
+    """gsb_mcmc_plan -> (workspace for up to n_draws draws, W_total, dead count).  Waits for the
+    two counts (one D2H)."""
+    lib = _lib.load()
+    N = alphas_raw.shape[0]
+    nbytes = lib.gsb_mcmc_workspace_bytes(N, n_draws)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=alphas_raw.device)
+    counts = (C.c_int64 * 2)()
+    _lib.check(lib.gsb_mcmc_plan(N, _ptr(alphas_raw), float(alpha_raw_min), mode, _ptr(ws), nbytes, counts,
+                                 _stream()), lib)
+    return ws, int(counts[0]), int(counts[1])
+
+
+def mcmc_sample(ws, N, u):
+    """gsb_mcmc_sample: fp64 uniforms u[n] -> int32 row ids [n] (after mcmc_plan on ws)"""
+    lib = _lib.load()
+    u = _check(u, "u", (u.shape[0],), torch.float64)
+    sampled = torch.empty(u.shape[0], dtype=torch.int32, device=u.device)
+    _lib.check(lib.gsb_mcmc_sample(N, u.shape[0], _ptr(u), _ptr(ws), ws.numel(), _ptr(sampled), _stream()), lib)
+    return sampled
+
+
+def _in_place(t, name, shape):
+    """the tensor itself (contiguous float32 CUDA of `shape`): the kernels write through its pointer"""
+    c = _check(t.detach(), name, shape)
+    if c.data_ptr() != t.data_ptr():
+        raise ValueError("%s must be contiguous (it is updated in place)" % name)
+    return c
+
+
+class MCMCController:
+    """MCMC densification (Kheradmand et al., "3D Gaussian Splatting as Markov Chain Monte Carlo",
+    2024; gsplat's MCMCStrategy): at most `cap_max` Gaussians, dead ones (opacity <= min_opacity)
+    moved onto live ones instead of pruned, and covariance-shaped position noise every step.
+
+        ctl = MCMCController(cap_max=1_000_000)
+        optimizer.step(); ctl.inject_noise(params, optimizer)     # every step
+        ctl.relocate(params, optimizer); ctl.grow(params, optimizer)  # every refinement interval
+
+    `params` / `optimizer` are those of DensityController (six raw tensors, Adam groups named after
+    them).  Sources are drawn in proportion to their opacity with an integer sampler whose ids do not
+    depend on the GPU's summation order; the uniforms and normals come from `generator` (a CUDA
+    torch.Generator, or the default one), so ranks that seed it alike stay identical.  A source hit
+    c times shares its opacity among r = min(c + 1, n_max) copies with a scale that keeps the
+    rendered footprint (DESIGN 3.11); the Adam moments of every row a call writes are zeroed."""
+
+    NOISE_K, NOISE_X0 = 100.0, 0.995
+
+    def __init__(self, cap_max, min_opacity=0.005, n_max=51, grow_rate=0.05, noise_lr=5e5, verbose=True):
+        if not 1 <= int(n_max) <= 51:
+            raise ValueError("n_max must be in [1, 51]")
+        if not 0.0 < min_opacity < 1.0:
+            raise ValueError("min_opacity must be in (0, 1)")
+        self.cap_max = int(cap_max)
+        self.min_opacity = float(min_opacity)
+        self.n_max = int(n_max)
+        self.grow_rate = float(grow_rate)
+        self.noise_lr = float(noise_lr)
+        self.verbose = verbose
+        # the fp32 logit the kernels compare alphas_raw with, as raw_thresholds computes it
+        self.alpha_raw_min = float(np.float32(np.log(self.min_opacity / (1 - self.min_opacity))))
+
+    def _state(self, params, optimizer, extra, in_place):
+        """checked (N, tensors, moments m / v or None, groups) for the six tensors and `extra`"""
+        N = params["pws"].shape[0]
+        take = _in_place if in_place else (lambda t, name, shape: _check(t.detach(), name, shape))
+        src = {}
+        for k, w in zip(GAUSSIAN_TENSORS, GAUSSIAN_WIDTHS):
+            src[k] = take(params[k], "params[%r]" % k, (N, w))
+        for k in extra:
+            if k in GAUSSIAN_TENSORS:
+                raise ValueError("extra names a built-in tensor: %r" % (k,))
+            t = params[k]
+            if not (isinstance(t, torch.Tensor) and t.dim() == 2 and t.shape[0] == N and t.shape[1] >= 1):
+                raise ValueError("params[%r] must be [N, D] with N = %d and D >= 1" % (k, N))
+            src[k] = take(t, "params[%r]" % (k,), tuple(t.shape))
+        groups = {g["name"]: g for g in optimizer.param_groups}
+        names = GAUSSIAN_TENSORS + tuple(extra)
+        missing = [k for k in names if k not in groups]
+        if missing:
+            raise ValueError("the optimizer has no param group named %s" % ", ".join(map(repr, missing)))
+        states = {k: optimizer.state.get(groups[k]["params"][0], None) for k in names}
+        have = [s is not None and "exp_avg" in s for s in states.values()]
+        if any(have) and not all(have):
+            raise ValueError("optimizer state must exist for all groups or for none")
+        m = v = None
+        if all(have):
+            m = {k: take(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape) for k in names}
+            v = {k: take(states[k]["exp_avg_sq"], "exp_avg_sq[%r]" % k, src[k].shape) for k in names}
+        return N, src, m, v, groups
+
+    def _report(self, title, rows):
+        if self.verbose:
+            print("---------------------")
+            print("gaussian %s report" % title)
+            for name, val in rows:
+                print("%s: " % name, val)
+            print("---------------------")
+
+    @torch.no_grad()
+    def relocate(self, params, optimizer, generator=None, extra=()):
+        """Moves every dead Gaussian (!(alphas_raw > logit(min_opacity)), NaN included) onto a live
+        one drawn by opacity, in place: N and the Parameter objects stay.  The sources get their
+        relocation value, dead row dead[j] (ascending) becomes a copy of the updated source j, and the
+        Adam moments of sources and destinations are zeroed.  extra: names of further [N, D]
+        entries of `params` with optimizer groups of those names (copied along).  HOST
+        SYNCHRONISATION: one read of the dead count.  -> dict(relocated, total)"""
+        lib = _lib.load()
+        extra = tuple(extra)
+        N, src, m, v, _ = self._state(params, optimizer, extra, in_place=True)
+        n = 0
+        if N:
+            ws, w_total, n = mcmc_plan(src["alphas_raw"], self.alpha_raw_min, MCMC_RELOCATE, N)
+            if w_total == 0:
+                n = 0  # nothing alive to copy from
+        if n:
+            u = torch.rand(n, dtype=torch.float64, device=src["pws"].device, generator=generator)
+            sampled = mcmc_sample(ws, N, u)
+            g, keep = gaussians_struct(src)
+            gm, keep_m = gaussians_struct(m) if m is not None else (None, None)
+            gv, keep_v = gaussians_struct(v) if m is not None else (None, None)
+            _lib.check(lib.gsb_mcmc_relocate(N, n, _ptr(sampled), _ptr(ws), ws.numel(), self.min_opacity, self.n_max,
+                                             C.byref(g), C.byref(gm) if gm is not None else None,
+                                             C.byref(gv) if gv is not None else None, _stream()), lib)
+            for k in extra:
+                _lib.check(lib.gsb_mcmc_relocate_rows(N, n, _ptr(sampled), _ptr(ws), ws.numel(), src[k].shape[1],
+                                                      _ptr(src[k]), _ptr(m[k] if m else None),
+                                                      _ptr(v[k] if v else None), _stream()), lib)
+        report = dict(relocated=n, total=N)
+        self._report("relocation", [("relocated num", n), ("total gaussian number", N)])
+        return report
+
+    @torch.no_grad()
+    def grow(self, params, optimizer, generator=None, extra=()):
+        """Adds n = max(0, min(cap_max, int(N (1 + grow_rate))) - N) Gaussians drawn by opacity over
+        every non-NaN row: rows [0, N) keep their order with the sources updated to their relocation
+        value, rows [N, N + n) copy the updated sources in draw order.  Moments are carried, except
+        zero for the sources and the new rows.  The Parameters are replaced and the optimizer
+        groups / state moved, as DensityController.update_gaussian_density does (a captured
+        GraphedFusedStep does not survive this call).  HOST SYNCHRONISATION: one read of the weight
+        total.  -> dict(added, total)"""
+        lib = _lib.load()
+        extra = tuple(extra)
+        N, src, m, v, groups = self._state(params, optimizer, extra, in_place=False)
+        n = max(0, min(self.cap_max, int(N * (1.0 + self.grow_rate))) - N)
+        if n:
+            ws, w_total, _ = mcmc_plan(src["alphas_raw"], self.alpha_raw_min, MCMC_GROW, n)
+            if w_total == 0:
+                n = 0
+        if n:
+            dev = src["pws"].device
+            u = torch.rand(n, dtype=torch.float64, device=dev, generator=generator)
+            sampled = mcmc_sample(ws, N, u)
+            fresh = lambda k: torch.empty((N + n,) + tuple(src[k].shape[1:]), dtype=torch.float32, device=dev)  # noqa: E731
+            dst = {k: fresh(k) for k in src}
+            dst_m = {k: fresh(k) for k in src} if m is not None else None
+            dst_v = {k: fresh(k) for k in src} if m is not None else None
+            structs, keep = [], []
+            for d in (src, m, v, dst, dst_m, dst_v):
+                if d is None:
+                    structs.append(None)
+                else:
+                    g, ka = gaussians_struct(d)
+                    keep.append((g, ka))
+                    structs.append(C.byref(g))
+            _lib.check(lib.gsb_mcmc_grow(N, n, _ptr(sampled), _ptr(ws), ws.numel(), self.min_opacity, self.n_max,
+                                         *structs, _stream()), lib)
+            for k in extra:
+                mk = lambda d: _ptr(d[k] if d is not None else None)  # noqa: E731
+                _lib.check(lib.gsb_mcmc_grow_rows(N, n, _ptr(sampled), _ptr(ws), ws.numel(), src[k].shape[1],
+                                                  _ptr(src[k]), mk(m), mk(v), _ptr(dst[k]), mk(dst_m), mk(dst_v),
+                                                  _stream()), lib)
+            for k in GAUSSIAN_TENSORS + extra:
+                group = groups[k]
+                old = group["params"][0]
+                new = torch.nn.Parameter(dst[k].requires_grad_(True))
+                st = optimizer.state.pop(old, None)
+                if st is not None and dst_m is not None:
+                    st["exp_avg"], st["exp_avg_sq"] = dst_m[k], dst_v[k]
+                    optimizer.state[new] = st
+                group["params"][0] = new
+                params[k] = new
+        report = dict(added=n, total=N + n)
+        self._report("growth", [("added num", n), ("total gaussian number", N + n)])
+        return report
+
+    @torch.no_grad()
+    def inject_noise(self, params, optimizer, generator=None):
+        """pws += Sigma(q, s) z * lr * noise_lr / (1 + exp(-100 ((1 - o) - 0.995))), in place, with
+        z ~ N(0, I) [N, 3] from `generator`, lr the current lr of the "pws" group and Sigma = R S^2 R^T
+        of the normalised rots_raw and exp(scales_raw) (no 3D filter, no antialiasing).  Runs after
+        optimizer.step(); pointers stay, so a captured GraphedFusedStep stays valid."""
+        lib = _lib.load()
+        N = params["pws"].shape[0]
+        pws = _in_place(params["pws"], "params['pws']", (N, 3))
+        a = _check(params["alphas_raw"].detach(), "params['alphas_raw']", (N, 1))
+        s = _check(params["scales_raw"].detach(), "params['scales_raw']", (N, 3))
+        q = _check(params["rots_raw"].detach(), "params['rots_raw']", (N, 4))
+        groups = [g for g in optimizer.param_groups if g.get("name") == "pws"]
+        if not groups:
+            raise ValueError("the optimizer has no param group named 'pws'")
+        lr = float(groups[0]["lr"])
+        z = torch.empty((N, 3), dtype=torch.float32, device=pws.device).normal_(0, 1, generator=generator)
+        _lib.check(lib.gsb_mcmc_noise(N, _ptr(pws), _ptr(a), _ptr(s), _ptr(q), _ptr(z), lr * self.noise_lr,
+                                      self.NOISE_K, self.NOISE_X0, _stream()), lib)
+        return z

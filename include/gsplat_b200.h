@@ -459,6 +459,59 @@ int gsb_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slots, 
 int gsb_reset_alpha(int64_t N, float *alphas_raw, float *exp_avg, float *exp_avg_sq, float reset_raw,
                     gsb_stream_t stream);
 
+/* ---- MCMC densification (extension; Kheradmand et al., "3D Gaussian Splatting as Markov Chain
+ * Monte Carlo", 2024; DESIGN 3.11).  A fixed Gaussian budget: dead Gaussians are moved onto live
+ * ones instead of pruned, growth samples existing Gaussians, and positions get noise shaped by each
+ * Gaussian's covariance.  o = sigmoid(alphas_raw), N < 2^31.
+ *
+ * Sampler: row i weighs q_i = floor(o_i 2^32) (o_i in fp64 from the fp32 raw value; 0 for rows
+ * the mode excludes), W = its uint64 inclusive prefix sum, and a draw u in [0, 1) picks the first i
+ * with W_i > min(floor(u W_total), W_total - 1).  Integer sums do not depend on the order of
+ * summation, so the ids are reproducible.  mode 0 (relocate): a row is dead when
+ * !(alphas_raw > alpha_raw_min) (NaN included); only alive rows are sampled, and the dead rows are
+ * listed in ascending order.  mode 1 (grow): every row but NaN ones is sampled.
+ *
+ * ws: gsb_mcmc_workspace_bytes(N, n) bytes, 16-byte aligned, for n draws; one workspace carries a
+ * plan through its sample and relocate / grow calls.  gsb_mcmc_plan -> counts_host[2] =
+ * (W_total, dead count).  HOST SYNCHRONISATION: waits for the two counts; the caller sizes the draws
+ * (relocate: n = dead count) and skips a call with W_total == 0 (nothing can be sampled).
+ * gsb_mcmc_sample: u[n] fp64 uniforms -> sampled[n] int32 row ids (plus the per-row hit counts c,
+ * kept in ws).
+ *
+ * Relocation value of a source hit c times, in fp64: r = min(c + 1, n_max),
+ *   o' = clamp(1 - (1 - o)^(1/r), min_opacity, 1 - 2^-23),
+ *   denom = sum_{m=1..r} C(r,m) (-1)^(m+1) o'^m / sqrt(m),
+ *   alphas_raw' = (float) logit(o'),  scales_raw' = (float)((double) scales_raw + log(o / denom)).
+ * gsb_mcmc_relocate (in place, mode 0 plan): every source gets its relocation value, dead row j of
+ *   the list becomes a copy of the updated source sampled[j]; the Adam moments (exp_avg /
+ *   exp_avg_sq: NULL, or both set) of every source and destination row are zeroed.
+ * gsb_mcmc_grow (mode 1 plan): dst [N + n rows] = the src rows with the sources updated, then
+ *   row N + j = a copy of the updated source sampled[j]; moments carried, except zero for the
+ *   sources and the new rows.  src_m/src_v/dst_m/dst_v: NULL, or all four set.
+ * The _rows variants do the same to one more per-Gaussian tensor [N, D] (features): a plain copy.
+ * gsb_mcmc_noise: pws += Sigma(q, s) z * scale / (1 + exp(-k ((1 - o) - x0))) with Sigma = R S^2
+ *   R^T of q = normalize(rots_raw), s = exp(scales_raw), z[N,3] the caller's unit normals and
+ *   scale = lr * noise_lr; in place. */
+size_t gsb_mcmc_workspace_bytes(int64_t N, int64_t n);
+int gsb_mcmc_plan(int64_t N, const float *alphas_raw, float alpha_raw_min, int mode, void *ws, size_t ws_bytes,
+                  int64_t *counts_host, gsb_stream_t stream);
+int gsb_mcmc_sample(int64_t N, int64_t n, const double *u, void *ws, size_t ws_bytes, int32_t *sampled,
+                    gsb_stream_t stream);
+int gsb_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, size_t ws_bytes, double min_opacity,
+                      int n_max, const gsb_gaussians *params, const gsb_gaussians *exp_avg,
+                      const gsb_gaussians *exp_avg_sq, gsb_stream_t stream);
+int gsb_mcmc_relocate_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, size_t ws_bytes, int D,
+                           float *x, float *exp_avg, float *exp_avg_sq, gsb_stream_t stream);
+int gsb_mcmc_grow(int64_t N, int64_t n, const int32_t *sampled, void *ws, size_t ws_bytes, double min_opacity,
+                  int n_max, const gsb_gaussians *src, const gsb_gaussians *src_m, const gsb_gaussians *src_v,
+                  const gsb_gaussians *dst, const gsb_gaussians *dst_m, const gsb_gaussians *dst_v,
+                  gsb_stream_t stream);
+int gsb_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const void *ws, size_t ws_bytes, int D,
+                       const float *src, const float *src_m, const float *src_v, float *dst, float *dst_m,
+                       float *dst_v, gsb_stream_t stream);
+int gsb_mcmc_noise(int64_t N, float *pws, const float *alphas_raw, const float *scales_raw, const float *rots_raw,
+                   const float *z, float scale, float k, float x0, gsb_stream_t stream);
+
 /* ---- Gaussian record conversion (extension; SURVEY 8f row N3, gsplat/gau_io.py).  A "gs row"
  * is the reference's .npy record (gau_io.py:7-12): pw[3] rot[4] scale[3] alpha sh[sh_dim],
  * 11 + sh_dim floats, activated values.
