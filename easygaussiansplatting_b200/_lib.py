@@ -19,6 +19,12 @@ class Gaussians(C.Structure):
 
 _gp = C.POINTER(Gaussians)
 
+
+class AdamTensor(C.Structure):
+    """gsb_adam_tensor: one row of gsb_adam_step's table"""
+    _fields_ = [("param", _vp), ("grad", _vp), ("exp_avg", _vp), ("exp_avg_sq", _vp), ("numel", _i64),
+                ("D", C.c_int32), ("step_size", _f), ("bc2_sqrt", _f)]
+
 # name -> (restype, argtypes); mirrors include/gsplat_b200.h one to one
 SIGNATURES = {
     "gsb_abi_version": (_i, []),
@@ -78,6 +84,7 @@ SIGNATURES = {
     "gsb_mcmc_grow": (_i, [_i64, _i64, _vp, _vp, _sz, C.c_double, _i, _gp, _gp, _gp, _gp, _gp, _gp, _vp]),
     "gsb_mcmc_grow_rows": (_i, [_i64, _i64, _vp, _vp, _sz, _i] + [_vp] * 7),
     "gsb_mcmc_noise": (_i, [_i64] + [_vp] * 5 + [_f, _f, _f, _vp]),
+    "gsb_adam_step": (_i, [_i, C.POINTER(AdamTensor), _i64, _vp, C.c_double, C.c_double, C.c_double, _vp]),
     "gsb_ply_rows_to_gs": (_i, [_i64, _i, _i, _vp, _vp, _vp, _vp]),
     "gsb_gs_to_params": (_i, [_i64, _i, _vp, _gp, _vp]),
     "gsb_params_to_gs": (_i, [_i64, _gp, _vp, _vp]),

@@ -42,7 +42,7 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
                                              "draw_features", "draw_backward_features", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
-                                             "mcmc_noise", "draw_rgbd",
+                                             "mcmc_noise", "adam", "draw_rgbd",
                                              "draw_backward_rgbd"};
 
 ProfScope::ProfScope(int id, cudaStream_t st) : id_(id), st_(st), stop_(nullptr) {
@@ -919,6 +919,30 @@ int gsb_mcmc_noise(int64_t N, float *pws, const float *alphas_raw, const float *
   GSB_REQUIRE(N >= 0, "mcmc_noise: N < 0");
   GSB_REQUIRE(N == 0 || (pws && alphas_raw && scales_raw && rots_raw && z), "mcmc_noise: null pointer");
   return launch_mcmc_noise(N, pws, alphas_raw, scales_raw, rots_raw, z, scale, k, x0, (cudaStream_t)stream);
+}
+
+int gsb_adam_step(int n_tensors, const gsb_adam_tensor *table, int64_t N, const uint8_t *visibility, double beta1,
+                  double beta2, double eps, gsb_stream_t stream) {
+  GSB_REQUIRE(n_tensors >= 0 && N >= 0, "adam_step: negative count");
+  GSB_REQUIRE(n_tensors == 0 || table != nullptr, "adam_step: null table");
+  GSB_REQUIRE(visibility != nullptr || N == 0, "adam_step: N > 0 without a visibility mask");
+  GSB_REQUIRE(beta1 >= 0.0 && beta1 < 1.0 && beta2 >= 0.0 && beta2 < 1.0, "adam_step: betas must be in [0, 1)");
+  GSB_REQUIRE(eps >= 0.0 && isfinite(eps), "adam_step: eps must be finite and >= 0");
+  bool work = false;
+  for (int i = 0; i < n_tensors; i++) {
+    const gsb_adam_tensor &a = table[i];
+    GSB_REQUIRE(a.numel >= 0, "adam_step: negative numel");
+    if (visibility) {
+      GSB_REQUIRE(a.D >= 1 && a.numel == N * (int64_t)a.D, "adam_step: a tensor's numel is not N * D");
+    }
+    if (a.numel == 0) continue;
+    GSB_REQUIRE(a.param && a.grad && a.exp_avg && a.exp_avg_sq, "adam_step: null pointer");
+    GSB_REQUIRE(aligned(a.param, 4) && aligned(a.grad, 4) && aligned(a.exp_avg, 4) && aligned(a.exp_avg_sq, 4),
+                "adam_step: misaligned tensor");
+    work = true;
+  }
+  if (!work) return 0;
+  return launch_adam(n_tensors, table, visibility, beta1, beta2, eps, (cudaStream_t)stream);
 }
 
 static bool sh_dim_ok(int d) { return d == 3 || d == 12 || d == 27 || d == 48; }

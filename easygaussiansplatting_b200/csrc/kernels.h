@@ -4,6 +4,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+struct gsb_adam_tensor;
+
 namespace gsb {
 
 struct Rec;
@@ -17,7 +19,7 @@ enum KernelId {
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
   K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
-  K_MCMC_ROWS, K_MCMC_NOISE, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_MCMC_ROWS, K_MCMC_NOISE, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -174,6 +176,11 @@ int launch_ply_rows_to_gs(int64_t N, int stride, int sh_dim, const float *rows, 
                           cudaStream_t st);
 int launch_gs_to_params(int64_t N, int sh_dim, const float *gs, float *const *dst, cudaStream_t st);
 int launch_params_to_gs(int64_t N, float *const *src, float *gs, cudaStream_t st);
+
+// ---- fused Adam step (adam.cu, DESIGN 3.12): the table of gsb_adam_step, checked by the entry
+// point; visibility NULL is dense Adam
+int launch_adam(int n_tensors, const gsb_adam_tensor *table, const uint8_t *visibility, double beta1, double beta2,
+                double eps, cudaStream_t st);
 
 // ---- binning (binning.cu)
 struct BinLayout {  // carve-up of the phase-1 workspace

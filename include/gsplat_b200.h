@@ -512,6 +512,31 @@ int gsb_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const void 
 int gsb_mcmc_noise(int64_t N, float *pws, const float *alphas_raw, const float *scales_raw, const float *rots_raw,
                    const float *z, float scale, float k, float x0, gsb_stream_t stream);
 
+/* ---- fused Adam step (extension; DESIGN 3.12).  One launch updates every tensor of the table in
+ * place, with torch.optim.Adam's foreach arithmetic in fp32 and in its order:
+ *   m = lerp(m, g, 1 - beta1);  v = v * beta2 + (1 - beta2) * g * g;
+ *   denom = sqrt(v) / bc2_sqrt + eps;  p = p - step_size * m / denom.
+ * step_size = lr / (1 - beta1^t) and bc2_sqrt = sqrt(1 - beta2^t) are per tensor (the caller
+ * forms them in double and rounds once).  beta1, beta2 and eps come as doubles so that 1 - beta1
+ * and 1 - beta2 are formed in double and rounded once, as torch does.  numel == 0 rows are skipped.
+ * Any 4-byte alignment; tensors whose four pointers share their offset mod 16 use 16-byte accesses.
+ * Selective mode (visibility != NULL, uint8 [N]): every tensor has numel == N * D (D >= 1) and row
+ * r = element / D is updated only where visibility[r] != 0; other rows' p, g, m and v are neither
+ * read (beyond the 16-byte quads a visible row shares) nor written.  Dense mode: visibility NULL,
+ * N = 0.  An empty table, or N = 0 in selective mode, is a no-op. */
+typedef struct gsb_adam_tensor {
+  float *param;
+  const float *grad;
+  float *exp_avg;
+  float *exp_avg_sq;
+  int64_t numel;
+  int32_t D;       /* row width (selective mode) */
+  float step_size; /* lr / (1 - beta1^t) */
+  float bc2_sqrt;  /* sqrt(1 - beta2^t) */
+} gsb_adam_tensor;
+int gsb_adam_step(int n_tensors, const gsb_adam_tensor *table, int64_t N, const uint8_t *visibility, double beta1,
+                  double beta2, double eps, gsb_stream_t stream);
+
 /* ---- Gaussian record conversion (extension; SURVEY 8f row N3, gsplat/gau_io.py).  A "gs row"
  * is the reference's .npy record (gau_io.py:7-12): pw[3] rot[4] scale[3] alpha sh[sh_dim],
  * 11 + sh_dim floats, activated values.
