@@ -1,13 +1,8 @@
 // Backward tile rasterizer ("drawB").  Replaces reference kernel.cu:809-950.
 //
-// Same work list and record gather as the forward (raster_fwd.cu): a work item is one 8x8 pixel
-// block of a tile, and every warp of the persistent grid pulls items from a global counter and
-// streams the tile's record list itself (32-record chunks, one cp.async gather of 48 bytes per
-// lane, double buffered with cp.async groups + __syncwarp; no __syncthreads after start-up).  The
-// list is walked back to front from the last chunk any pixel of the block replays (max contrib),
-// so a warp stops at its own block's last contributing record, not the tile's.  The records are
-// read 4x (once per block) instead of once per tile; they come from L2.  Records that cannot touch
-// the block are culled by the forward's exact test (rec_can_touch).
+// The record walk of raster_walk.cuh, back to front from the last chunk any pixel of the block
+// replays (max contrib), so a warp stops at its own block's last contributing record, not the
+// tile's.  The records are read 4x (once per block) instead of once per tile; they come from L2.
 //
 // Phase A, pixel-parallel replay: each pixel replays its saved (final_tau, contrib) state:
 // tau <- tau / (1 - alpha'), dL/dalpha' = tau (c - gamma_next) . dL/dgamma, with gamma_next kept as
@@ -25,18 +20,11 @@
 //   dL/du = -(A Sx + B Sy, B Sx + C Sy),  dL/dconic = (-Sxx/2, -Sxy, -Syy/2).
 #include "common.cuh"
 #include "kernels.h"
-#include "raster_eval.cuh"
+#include "raster_walk.cuh"
 #include "tile_io.cuh"
 
 namespace gsb {
 
-constexpr int BWD_SLOTS = 8;
-// slot = 2 weight rows of 64 floats + 16 floats of padding: a stride of 16 (mod 32) floats makes the
-// phase-B 128-bit reads (2 slots x 4 parts per 8-lane wavefront) conflict-free
-constexpr int BWD_SLOT_BYTES = (2 * 64 + 16) * 4;      // 576
-constexpr int BWD_W_BYTES = BWD_SLOTS * BWD_SLOT_BYTES;  // 4608
-constexpr int BWD_RING = 2;                              // 32-record chunks in flight per warp
-constexpr int BWD_CHUNK_BYTES = 32 * 48;
 #ifndef DRAW_BWD_MINBLOCKS
 #define DRAW_BWD_MINBLOCKS 6
 #endif
@@ -45,12 +33,6 @@ constexpr int BWD_CHUNK_BYTES = 32 * 48;
 #endif
 
 namespace {
-__device__ __forceinline__ void sts64(uint32_t a, float2 v) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y) : "memory");
-}
-__device__ __forceinline__ float2 lo(const float4 &v) { return make_float2(v.x, v.y); }
-__device__ __forceinline__ float2 hi(const float4 &v) { return make_float2(v.z, v.w); }
-
 // Phase B: moment sums of up to 8 records over the warp's 8x8 block.
 //   lane = slot * 4 + part; part covers x in [4 (part & 1), +4) of rows (part >> 1) + {0, 2, 4, 6}.
 //   inf = record word q0 = (u_x, u_y, gaussian id, alpha) of the lane's slot.  It travels in registers:
@@ -66,7 +48,7 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
   const float U = inf.x - (fbx0 + (float)((part & 1) * 4));
   const float V = inf.y - (fby0 + (float)(part >> 1));
   const float2 dx01 = p2(U, U - 1.0f), dx23 = p2(U - 2.0f, U - 3.0f);
-  const uint32_t a = w_addr + slot * BWD_SLOT_BYTES + part * 16;
+  const uint32_t a = w_addr + slot * WALK_SLOT_BYTES + part * 16;
   const uint32_t d = dl_addr + part * 16;
   float2 m0 = p2s(0.f), m1 = p2s(0.f), m2 = p2s(0.f), m3 = p2s(0.f), m4 = p2s(0.f), m5 = p2s(0.f),
          m6 = p2s(0.f), m7 = p2s(0.f), m8 = p2s(0.f), m9 = p2s(0.f);
@@ -143,8 +125,8 @@ __device__ __forceinline__ void draw_bwd_body(
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
     int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][BWD_RING * BWD_CHUNK_BYTES];  // gathered records, per warp
-  __shared__ __align__(16) unsigned char s_w[4][BWD_W_BYTES];                   // weight rows, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_w[4][WALK_W_BYTES];                   // weight rows, per warp
   __shared__ __align__(16) float s_dl[4][RGBD ? 4 : 3][64];                    // dL/dgamma (dL/dD) of the block
   __shared__ __align__(16) uint2 s_list[4][34];  // (record address, patch index) of a chunk's survivors
   __shared__ __align__(16) Rec s_dummy;          // all-zero record: pads an odd survivor count
@@ -156,8 +138,7 @@ __device__ __forceinline__ void draw_bwd_body(
   const uint32_t dl_addr = opaque_u32(smem_u32(&s_dl[warp][0][0]));
   const uint32_t list_addr = opaque_u32(smem_u32(&s_list[warp][0]));
   const uint32_t dummy_addr = smem_u32(&s_dummy);
-  if (threadIdx.x < 12) reinterpret_cast<float *>(&s_dummy)[threadIdx.x] = 0.0f;
-  __syncthreads();  // (the only CTA-wide barrier: start-up)
+  zero_dummy(s_dummy);
   (void)T;
   const int items = work[1];  // entries of the work list (k_tile_list, raster_fwd.cu)
   const int *__restrict__ entries = work + 2;
@@ -169,13 +150,10 @@ __device__ __forceinline__ void draw_bwd_body(
   int2 range = make_int2(0, 0);
   for (;;) {
     if (blk == blk_end) {
-      int item = 0;
-      if (lane == 0) item = atomicAdd(work, 1);
-      item = __shfl_sync(0xffffffffu, item, 0);
+      const int item = pull_item(work, lane);
       // a whole-tile gather whose four blocks all skipped (outside the image / nothing composited)
       // was never waited for: drain it before the next gather reuses the ring, or the warp exits
-      cp_async_wait<0>();
-      __syncwarp();
+      walk_drain();
       if (item >= items) break;
       const int ent = __ldg(entries + item);
       const int code = ent & 7;
@@ -186,17 +164,7 @@ __device__ __forceinline__ void draw_bwd_body(
       if (len <= 0) continue;
       blk = whole_tile ? 0 : code;
       blk_end = whole_tile ? 4 : code + 1;
-      if (whole_tile) {  // the tile's single chunk, gathered once (two groups: see the wait below)
-        if (lane < len) {
-          const char *src = reinterpret_cast<const char *>(recs + __ldg(gsid + range.x + lane));
-          const uint32_t dst = ring_addr + lane * 48;
-          cp_async16_sa(dst, src);
-          cp_async16_sa(dst + 16, src + 16);
-          cp_async16_sa(dst + 32, src + 32);
-        }
-        cp_async_commit();
-        cp_async_commit();
-      }
+      if (whole_tile) gather_whole_tile(ring_addr, recs, gsid + range.x, len, lane);
     }
     const int cur = blk++;
     const int tx = tile % gx, ty = tile / gx;
@@ -242,21 +210,16 @@ __device__ __forceinline__ void draw_bwd_body(
     const int32_t *ids = gsid + range.x;
     // gather of chunk c: lane j copies the record of patch 32 c + j (if below wmax) into ring slot c & 1
     auto issue = [&](int c, int id) {
-      if (c >= 0 && c * 32 + lane < wmax) {
-        const char *src = reinterpret_cast<const char *>(recs + id);
-        const uint32_t dst = ring_addr + (c & (BWD_RING - 1)) * BWD_CHUNK_BYTES + lane * 48;
-        cp_async16_sa(dst, src);
-        cp_async16_sa(dst + 16, src + 16);
-        cp_async16_sa(dst + 32, src + 32);
-      }
+      if (c >= 0 && c * 32 + lane < wmax)
+        gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
       cp_async_commit();
     };
     auto load_id = [&](int c) { return (c >= 0 && c * 32 + lane < wmax) ? __ldg(ids + c * 32 + lane) : 0; };
     int id_next = 0;
     if (!whole_tile) {
 #pragma unroll
-      for (int r = 0; r < BWD_RING; r++) issue(nch - 1 - r, load_id(nch - 1 - r));
-      id_next = load_id(nch - 1 - BWD_RING);  // id of the chunk the first refill gathers
+      for (int r = 0; r < WALK_RING; r++) issue(nch - 1 - r, load_id(nch - 1 - r));
+      id_next = load_id(nch - 1 - WALK_RING);  // id of the chunk the first refill gathers
     }
 
     const float2 npx = p2(-(float)px, -(float)(px + 1));
@@ -264,18 +227,17 @@ __device__ __forceinline__ void draw_bwd_body(
     const float bx0 = (float)rx0, bx1 = (float)(rx0 + 7), by0 = (float)ry0, by1 = (float)(ry0 + 7);
     float2 sdot = p2s(0.f);  // dL/dgamma . gamma_next, per pixel
     uint32_t wa = w_addr + lane * 8;  // where the next record's weight rows go
-    const uint32_t wa_pair_limit = w_addr + lane * 8 + (BWD_SLOTS - 2) * BWD_SLOT_BYTES;
+    const uint32_t wa_pair_limit = w_addr + lane * 8 + (WALK_SLOTS - 2) * WALK_SLOT_BYTES;
     int to_my_slot = lane >> 2;  // free slots before the one whose moments this lane sums in phase B
     float4 inf = make_float4(0.f, 0.f, 0.f, 1.f);
 
     for (int c = nch - 1; c >= 0; c--) {
-      cp_async_wait<BWD_RING - 1>();  // this lane's copy of chunk c has landed ...
-      __syncwarp();                  // ... and so have the other lanes'
-      const uint32_t my_rec = ring_addr + (c & (BWD_RING - 1)) * BWD_CHUNK_BYTES + lane * 48;
+      // survivors of the chunk, back to front, as (record address, patch index); the pad's index
+      // lies beyond every contrib
+      const uint32_t my_rec = wait_chunk(ring_addr, c, lane);
       const int my_idx = c * 32 + lane;
       bool hit = false;
       if (my_idx < wmax) hit = rec_can_touch(lds128(my_rec), lds128(my_rec + 16), bx0, bx1, by0, by1);
-      // survivors of the chunk, back to front, as a list of (record address, patch index)
       const unsigned mask = __ballot_sync(0xffffffffu, hit);
       const int n = __popc(mask);
       if (hit) sts64u(list_addr + __popc(mask & ~((2u << lane) - 1u)) * 8, my_rec, (uint32_t)my_idx);
@@ -316,8 +278,8 @@ __device__ __forceinline__ void draw_bwd_body(
         const float2 diffb = add2_rn(dcb, p2(-sdot.x, -sdot.y));
         sdot = fma2_rn(B.e, diffb, sdot);
         const float2 dapb = mul2_rn(tau, diffb);
-        sts64(wa + BWD_SLOT_BYTES, mul2_rn(dapb, B.e));
-        sts64(wa + BWD_SLOT_BYTES + 256, mul2_rn(B.e, tau));
+        sts64(wa + WALK_SLOT_BYTES, mul2_rn(dapb, B.e));
+        sts64(wa + WALK_SLOT_BYTES + 256, mul2_rn(B.e, tau));
         if (to_my_slot == 1) inf = q0b;
         if (fmaxf(q0a.w, q0b.w) > ALPHA_CLAMP) {  // opacity above the clamp (rare):
           // sum dL/dalpha' g is not (sum w) / alpha on clamped pixels -- reduce it with shuffles
@@ -332,12 +294,12 @@ __device__ __forceinline__ void draw_bwd_body(
           if (lane == 0 && vb != 0.0f) atomicAdd(moments + (size_t)__float_as_int(q0b.z) * 9 + 5, vb);
         }
         const bool pair = i + 2 <= n;  // false: the second record was the pad, its slot is reused
-        wa += pair ? 2 * BWD_SLOT_BYTES : BWD_SLOT_BYTES;
+        wa += pair ? 2 * WALK_SLOT_BYTES : WALK_SLOT_BYTES;
         to_my_slot -= pair ? 2 : 1;
       }
       __syncwarp();  // every lane is done with this ring slot and with the list
-      issue(c - BWD_RING, id_next);
-      id_next = load_id(c - BWD_RING - 1);
+      issue(c - WALK_RING, id_next);
+      id_next = load_id(c - WALK_RING - 1);
     }
     cp_async_wait<0>();
     if (wa != w_addr + lane * 8) {
@@ -422,19 +384,15 @@ int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *
     if (work == nullptr) return set_arg_error("drawB: work area missing");
     int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);  // tiles with patches
     if (rc) return rc;
-    int dev = 0, sms = 132;
-    GSB_CUDA_TRY(cudaGetDevice(&dev));
-    GSB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    int grid = 0;
+    rc = persistent_grid(T, dg != nullptr ? DRAW_BWD_RGBD_MINBLOCKS : DRAW_BWD_MINBLOCKS, grid);
+    if (rc) return rc;
     if (dg != nullptr) {
-      const long long want = (long long)sms * DRAW_BWD_RGBD_MINBLOCKS;
-      const int grid = (int)(T < want ? T : want);
       ProfScope ps(K_DRAW_BWD_RGBD, st);
       k_draw_bwd_rgbd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
                                             dg->dloss_ddepth_image, dg->dloss_dalpha_image, moments, dg->ddepths,
                                             work);
     } else {
-      const long long want = (long long)sms * DRAW_BWD_MINBLOCKS;
-      const int grid = (int)(T < want ? T : want);
       ProfScope ps(K_DRAW_BWD, st);
       k_draw_bwd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib,
                                        final_tau, dloss_dgammas, moments, work);

@@ -6,12 +6,9 @@
 // channels (G = 8, or 4 for a last group of at most 4 channels), so D channels take ceil(D / 8)
 // replays or fewer.
 //
-// Mapping: the rasterizers' own.  Work items from k_tile_list (one 8x8 block, or all four blocks
-// of a tile with <= 32 patches), every warp of the persistent grid pulls items from a global
-// counter, a lane owns two horizontally adjacent pixels, records are gathered 32 at a time with
-// three 16-byte cp.async per lane (double buffered) and culled per block by rec_can_touch.  A
-// surviving record's G feature floats are then loaded by the lane that gathered it into a small
-// per-warp shared table next to the survivor list.
+// Mapping: the rasterizers' own, through the record walk of raster_walk.cuh.  A surviving record's
+// G feature floats are loaded by the lane that gathered it into a small per-warp shared table next
+// to the survivor list.
 //
 // Weights: a record contributes to a pixel exactly when its patch index is below the pixel's
 // contrib and alpha' >= 0.002 -- the forward's skip and stop rules, since tau >= 1e-4 holds for every
@@ -30,19 +27,12 @@
 // dL/dfeatures[id, c] with scalar float atomics (DESIGN 3.10).
 #include "common.cuh"
 #include "kernels.h"
-#include "raster_eval.cuh"
+#include "raster_walk.cuh"
 #include "tile_io.cuh"
 
 namespace gsb {
 
-constexpr int FEAT_RING = 2;  // 32-record chunks in flight per warp
-constexpr int FEAT_CHUNK_BYTES = 32 * 48;
 constexpr int FEAT_G = 8;     // channels per replay (a last group of <= 4 channels takes the G = 4 form)
-// weight rows of phase B: the layout of k_draw_bwd (2 rows of 64 floats + 16 floats of padding per
-// slot: conflict-free 128-bit reads)
-constexpr int FEAT_SLOTS = 8;
-constexpr int FEAT_SLOT_BYTES = (2 * 64 + 16) * 4;
-constexpr int FEAT_W_BYTES = FEAT_SLOTS * FEAT_SLOT_BYTES;
 // CTAs per SM, the most that build without spills (-Xptxas -v): the forward at 71 / 68 registers
 // (G = 8 / 4); the backward keeps dL/dF of both pixels in registers through phase A and its 6 + G
 // sums in phase B (152 / 121 registers)
@@ -53,14 +43,9 @@ template <int G>
 constexpr int feat_bwd_minblocks() { return G == 4 ? 4 : 3; }
 
 namespace {
-__device__ __forceinline__ void sts64f(uint32_t a, float2 v) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v.x), "f"(v.y) : "memory");
-}
 __device__ __forceinline__ void sts128f(uint32_t a, float x, float y, float z, float w) {
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
 }
-__device__ __forceinline__ float2 lo(const float4 &v) { return make_float2(v.x, v.y); }
-__device__ __forceinline__ float2 hi(const float4 &v) { return make_float2(v.z, v.w); }
 
 // channels c0 .. c0 + G - 1 of Gaussian `id` (0 past D) into the feature table entry at `dst`
 template <int G>
@@ -136,7 +121,7 @@ __device__ __forceinline__ void feat_flush(uint32_t w_addr, const float4 &inf, u
   const float U = inf.x - (fbx0 + (float)((part & 1) * 4));
   const float V = inf.y - (fby0 + (float)(part >> 1));
   const float2 dx01 = p2(U, U - 1.0f), dx23 = p2(U - 2.0f, U - 3.0f);
-  const uint32_t a = w_addr + slot * FEAT_SLOT_BYTES + part * 16;
+  const uint32_t a = w_addr + slot * WALK_SLOT_BYTES + part * 16;
   const uint32_t d = dl_addr + part * 16;
   float2 m0 = p2s(0.f), m1 = p2s(0.f), m2 = p2s(0.f), m3 = p2s(0.f), m4 = p2s(0.f), m5 = p2s(0.f);
   float2 mf[G];
@@ -197,7 +182,7 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
     int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ features, int D,
     int c0, float *__restrict__ feature_image, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][FEAT_RING * FEAT_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
   __shared__ __align__(16) uint2 s_list[4][34];       // (record address, patch index) of a chunk's survivors
   __shared__ __align__(16) float s_feat[4][34][G];    // their features, same order
   __shared__ __align__(16) Rec s_dummy;               // all-zero record: pads an odd survivor count
@@ -209,36 +194,21 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
   const uint32_t list_addr = opaque_u32(smem_u32(&s_list[warp][0]));
   const uint32_t feat_addr = opaque_u32(smem_u32(&s_feat[warp][0][0]));
   const uint32_t dummy_addr = smem_u32(&s_dummy);
-  if (threadIdx.x < 12) reinterpret_cast<float *>(&s_dummy)[threadIdx.x] = 0.0f;
-  __syncthreads();  // (the only CTA-wide barrier: start-up)
+  zero_dummy(s_dummy);
   zero_empty_tiles<G>(W, H, gx, T, D, c0, ranges, feature_image);
   const int items = work[1];
   const int *__restrict__ entries = work + 2;
 
   for (;;) {
-    int item = 0;
-    if (lane == 0) item = atomicAdd(work, 1);
-    item = __shfl_sync(0xffffffffu, item, 0);
-    // a whole-tile gather whose blocks all had nothing to composite was never waited for
-    cp_async_wait<0>();
-    __syncwarp();
+    const int item = pull_item(work, lane);
+    walk_drain();  // a whole-tile gather whose blocks all had nothing to composite was never waited for
     if (item >= items) break;
     const int ent = __ldg(entries + item);
     const int tile = ent >> 3, code = ent & 7;
     const bool whole_tile = code == 4;
     const int2 range = ld_pair(ranges, tile);
     const int len = range.y - range.x;
-    if (whole_tile) {  // the tile's single chunk, gathered once (two groups: see the wait below)
-      if (lane < len) {
-        const char *src = reinterpret_cast<const char *>(recs + __ldg(gsid + range.x + lane));
-        const uint32_t dst = ring_addr + lane * 48;
-        cp_async16_sa(dst, src);
-        cp_async16_sa(dst + 16, src + 16);
-        cp_async16_sa(dst + 32, src + 32);
-      }
-      cp_async_commit();
-      cp_async_commit();
-    }
+    if (whole_tile) gather_whole_tile(ring_addr, recs, gsid + range.x, len, lane);
     for (int blk = whole_tile ? 0 : code; blk < (whole_tile ? 4 : code + 1); blk++) {
       const int tx = tile % gx, ty = tile / gx;
       const int rx0 = tx * TILE + (blk & 1) * 8, ry0 = ty * TILE + (blk >> 1) * 8;
@@ -259,21 +229,16 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
         const int nch = (wmax + 31) >> 5;  // chunks [0, nch) hold every record a pixel of the block composites
         const int32_t *ids = gsid + range.x;
         auto issue = [&](int c, int id) {
-          if (c < nch && c * 32 + lane < wmax) {
-            const char *src = reinterpret_cast<const char *>(recs + id);
-            const uint32_t dst = ring_addr + (c & (FEAT_RING - 1)) * FEAT_CHUNK_BYTES + lane * 48;
-            cp_async16_sa(dst, src);
-            cp_async16_sa(dst + 16, src + 16);
-            cp_async16_sa(dst + 32, src + 32);
-          }
+          if (c < nch && c * 32 + lane < wmax)
+            gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
           cp_async_commit();
         };
         auto load_id = [&](int c) { return (c < nch && c * 32 + lane < wmax) ? __ldg(ids + c * 32 + lane) : 0; };
         int id_next = 0;
         if (!whole_tile) {
 #pragma unroll
-          for (int r = 0; r < FEAT_RING; r++) issue(r, load_id(r));
-          id_next = load_id(FEAT_RING);
+          for (int r = 0; r < WALK_RING; r++) issue(r, load_id(r));
+          id_next = load_id(WALK_RING);
         }
         const float2 npx = p2(-(float)px, -(float)(px + 1));
         const float fpy = (float)py;
@@ -281,29 +246,15 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
         float2 tau = p2s(1.0f);
 
         for (int c = 0; c < nch; c++) {
-          cp_async_wait<FEAT_RING - 1>();  // this lane's copy of chunk c has landed ...
-          __syncwarp();                   // ... and so have the other lanes'
-          const uint32_t my_rec = ring_addr + (c & (FEAT_RING - 1)) * FEAT_CHUNK_BYTES + lane * 48;
-          const int my_idx = c * 32 + lane;
-          bool hit = false;
-          float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (my_idx < wmax) {
-            q0 = lds128(my_rec);
-            hit = rec_can_touch(q0, lds128(my_rec + 16), bx0, bx1, by0, by1);
-          }
-          // survivors front to back: (record address, patch index) and their G features
-          const unsigned mask = __ballot_sync(0xffffffffu, hit);
-          const int n = __popc(mask);
-          if (hit) {
-            const int pos = __popc(mask & ((1u << lane) - 1u));
-            sts64u(list_addr + pos * 8, my_rec, (uint32_t)my_idx);
-            load_features<G>(feat_addr + pos * G * 4, features, D, c0, __float_as_int(q0.z));
-          }
-          if (lane == 0) {  // pad: alpha 0, an index beyond every contrib, zero features
-            sts64u(list_addr + n * 8, dummy_addr, 0x7fffffffu);
-            zero_features<G>(feat_addr + n * G * 4);
-          }
-          __syncwarp();
+          // survivors front to back: (record address, patch index) and their G features; the pad has
+          // alpha 0, an index beyond every contrib and zero features
+          const int n = cull_compact(
+              wait_chunk(ring_addr, c, lane), c * 32 + lane, wmax, bx0, bx1, by0, by1, list_addr, dummy_addr, 0u,
+              0x7fffffffu, lane,
+              [&](int pos, const float4 &q0) {
+                load_features<G>(feat_addr + pos * G * 4, features, D, c0, __float_as_int(q0.z));
+              },
+              [&](int n) { zero_features<G>(feat_addr + n * G * 4); });
           for (int i = 0; i < n; i += 2) {
             const uint4 ent2 = lds128u(list_addr + i * 8);
             const float4 q0a = lds128(ent2.x), q0b = lds128(ent2.z);
@@ -342,11 +293,10 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
             }
           }
           __syncwarp();  // every lane is done with this ring slot, the list and the features
-          issue(c + FEAT_RING, id_next);
-          id_next = load_id(c + FEAT_RING + 1);
+          issue(c + WALK_RING, id_next);
+          id_next = load_id(c + WALK_RING + 1);
         }
-        cp_async_wait<0>();
-        __syncwarp();
+        walk_drain();
       }
       store_pixels<G>(feature_image, HW, pix, D, c0, in0, in1, vec2, acc);
     }
@@ -359,8 +309,8 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ features, int D, int c0, const float *__restrict__ dloss_dfeature_image,
     float *__restrict__ moments, float *__restrict__ dfeat, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][FEAT_RING * FEAT_CHUNK_BYTES];  // gathered records, per warp
-  __shared__ __align__(16) unsigned char s_w[4][FEAT_W_BYTES];                    // weight rows, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_w[4][WALK_W_BYTES];                    // weight rows, per warp
   __shared__ __align__(16) float s_dl[4][G][64];       // dL/dF of the block, channel-major
   __shared__ __align__(16) uint2 s_list[4][34];        // (record address, patch index) of a chunk's survivors
   __shared__ __align__(16) float s_feat[4][34][G];     // their features, same order
@@ -374,8 +324,7 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
   const uint32_t list_addr = opaque_u32(smem_u32(&s_list[warp][0]));
   const uint32_t feat_addr = opaque_u32(smem_u32(&s_feat[warp][0][0]));
   const uint32_t dummy_addr = smem_u32(&s_dummy);
-  if (threadIdx.x < 12) reinterpret_cast<float *>(&s_dummy)[threadIdx.x] = 0.0f;
-  __syncthreads();  // (the only CTA-wide barrier: start-up)
+  zero_dummy(s_dummy);
   const int items = work[1];
   const int *__restrict__ entries = work + 2;
 
@@ -385,11 +334,8 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
   int2 range = make_int2(0, 0);
   for (;;) {
     if (blk == blk_end) {
-      int item = 0;
-      if (lane == 0) item = atomicAdd(work, 1);
-      item = __shfl_sync(0xffffffffu, item, 0);
-      cp_async_wait<0>();  // (an unused whole-tile gather: drained before the ring is reused)
-      __syncwarp();
+      const int item = pull_item(work, lane);
+      walk_drain();  // (an unused whole-tile gather: drained before the ring is reused)
       if (item >= items) break;
       const int ent = __ldg(entries + item);
       const int code = ent & 7;
@@ -400,17 +346,7 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
       if (len <= 0) continue;
       blk = whole_tile ? 0 : code;
       blk_end = whole_tile ? 4 : code + 1;
-      if (whole_tile) {
-        if (lane < len) {
-          const char *src = reinterpret_cast<const char *>(recs + __ldg(gsid + range.x + lane));
-          const uint32_t dst = ring_addr + lane * 48;
-          cp_async16_sa(dst, src);
-          cp_async16_sa(dst + 16, src + 16);
-          cp_async16_sa(dst + 32, src + 32);
-        }
-        cp_async_commit();
-        cp_async_commit();
-      }
+      if (whole_tile) gather_whole_tile(ring_addr, recs, gsid + range.x, len, lane);
     }
     const int cur = blk++;
     const int tx = tile % gx, ty = tile / gx;
@@ -437,27 +373,22 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
         if (in0) dl[k].x = __ldg(plane + pix);
         if (in1) dl[k].y = __ldg(plane + pix + 1);
       }
-      sts64f(dl_addr + k * 256 + lane * 8, dl[k]);  // phase B's table; the flush's __syncwarp orders it
+      sts64(dl_addr + k * 256 + lane * 8, dl[k]);  // phase B's table; the flush's __syncwarp orders it
     }
 
     const int nch = (wmax + 31) >> 5;
     const int32_t *ids = gsid + range.x;
     auto issue = [&](int c, int id) {
-      if (c >= 0 && c * 32 + lane < wmax) {
-        const char *src = reinterpret_cast<const char *>(recs + id);
-        const uint32_t dst = ring_addr + (c & (FEAT_RING - 1)) * FEAT_CHUNK_BYTES + lane * 48;
-        cp_async16_sa(dst, src);
-        cp_async16_sa(dst + 16, src + 16);
-        cp_async16_sa(dst + 32, src + 32);
-      }
+      if (c >= 0 && c * 32 + lane < wmax)
+        gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
       cp_async_commit();
     };
     auto load_id = [&](int c) { return (c >= 0 && c * 32 + lane < wmax) ? __ldg(ids + c * 32 + lane) : 0; };
     int id_next = 0;
     if (!whole_tile) {
 #pragma unroll
-      for (int r = 0; r < FEAT_RING; r++) issue(nch - 1 - r, load_id(nch - 1 - r));
-      id_next = load_id(nch - 1 - FEAT_RING);
+      for (int r = 0; r < WALK_RING; r++) issue(nch - 1 - r, load_id(nch - 1 - r));
+      id_next = load_id(nch - 1 - WALK_RING);
     }
 
     const float2 npx = p2(-(float)px, -(float)(px + 1));
@@ -465,14 +396,12 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
     const float bx0 = (float)rx0, bx1 = (float)(rx0 + 7), by0 = (float)ry0, by1 = (float)(ry0 + 7);
     float2 sdot = p2s(0.f);  // dL/dF . F_next, per pixel
     uint32_t wa = w_addr + lane * 8;
-    const uint32_t wa_pair_limit = w_addr + lane * 8 + (FEAT_SLOTS - 2) * FEAT_SLOT_BYTES;
+    const uint32_t wa_pair_limit = w_addr + lane * 8 + (WALK_SLOTS - 2) * WALK_SLOT_BYTES;
     int to_my_slot = lane >> 2;
     float4 inf = make_float4(0.f, 0.f, 0.f, 1.f);
 
     for (int c = nch - 1; c >= 0; c--) {
-      cp_async_wait<FEAT_RING - 1>();
-      __syncwarp();
-      const uint32_t my_rec = ring_addr + (c & (FEAT_RING - 1)) * FEAT_CHUNK_BYTES + lane * 48;
+      const uint32_t my_rec = wait_chunk(ring_addr, c, lane);
       const int my_idx = c * 32 + lane;
       bool hit = false;
       float4 q0 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -527,16 +456,16 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
         const float2 diffa = add2_rn(dfa, p2(-sdot.x, -sdot.y));
         sdot = fma2_rn(A.e, diffa, sdot);
         const float2 dapa = mul2_rn(tau, diffa);
-        sts64f(wa, mul2_rn(dapa, A.e));       // w
-        sts64f(wa + 256, mul2_rn(A.e, tau));  // wc
+        sts64(wa, mul2_rn(dapa, A.e));       // w
+        sts64(wa + 256, mul2_rn(A.e, tau));  // wc
         if (to_my_slot == 0) inf = q0a;
         // second record (the all-zero pad record when the count is odd: e = 0, weights 0)
         tau = mul2_rn(tau, B.rc);
         const float2 diffb = add2_rn(dfb, p2(-sdot.x, -sdot.y));
         sdot = fma2_rn(B.e, diffb, sdot);
         const float2 dapb = mul2_rn(tau, diffb);
-        sts64f(wa + FEAT_SLOT_BYTES, mul2_rn(dapb, B.e));
-        sts64f(wa + FEAT_SLOT_BYTES + 256, mul2_rn(B.e, tau));
+        sts64(wa + WALK_SLOT_BYTES, mul2_rn(dapb, B.e));
+        sts64(wa + WALK_SLOT_BYTES + 256, mul2_rn(B.e, tau));
         if (to_my_slot == 1) inf = q0b;
         if (fmaxf(q0a.w, q0b.w) > ALPHA_CLAMP) {  // opacity above the clamp: row 5 reduced here
           float va = q0a.w > ALPHA_CLAMP ? fmaf(A.e.x > 0.f ? dapa.x : 0.f, A.gg.x, (A.e.y > 0.f ? dapa.y : 0.f) * A.gg.y) : 0.0f;
@@ -550,12 +479,12 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
           if (lane == 0 && vb != 0.0f) atomicAdd(moments + (size_t)__float_as_int(q0b.z) * 9 + 5, vb);
         }
         const bool pair = i + 2 <= n;
-        wa += pair ? 2 * FEAT_SLOT_BYTES : FEAT_SLOT_BYTES;
+        wa += pair ? 2 * WALK_SLOT_BYTES : WALK_SLOT_BYTES;
         to_my_slot -= pair ? 2 : 1;
       }
       __syncwarp();  // every lane is done with this ring slot, the list and the features
-      issue(c - FEAT_RING, id_next);
-      id_next = load_id(c - FEAT_RING - 1);
+      issue(c - WALK_RING, id_next);
+      id_next = load_id(c - WALK_RING - 1);
     }
     cp_async_wait<0>();
     if (wa != w_addr + lane * 8) {
@@ -576,14 +505,6 @@ FeatLayout feat_layout(int N, int H, int W, int64_t P, uintptr_t base) {
   return L;
 }
 
-static int grid_for(int T, int per_sm) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    return -1;
-  const long long want = (long long)sms * per_sm;
-  return (int)(T < want ? T : want);
-}
-
 int launch_draw_features(int H, int W, int D, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
                          const int32_t *contrib, const float *features, float *feature_image, int *work,
                          cudaStream_t st) {
@@ -597,8 +518,9 @@ int launch_draw_features(int H, int W, int D, const int32_t *ranges, const Rec *
   }
   int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);
   if (rc) return rc;
-  const int grid = grid_for(T, DRAW_FEAT_MINBLOCKS);
-  if (grid < 0) return set_arg_error("draw_features: no device");
+  int grid = 0;
+  rc = persistent_grid(T, DRAW_FEAT_MINBLOCKS, grid);
+  if (rc) return rc;
   for (int c0 = 0; c0 < D; c0 += FEAT_G) {
     if (c0 > 0) GSB_CUDA_TRY(cudaMemsetAsync(work, 0, sizeof(int), st));  // the item counter, per replay
     ProfScope ps(K_DRAW_FEAT, st);
@@ -625,8 +547,10 @@ int launch_draw_features_backward(int H, int W, int N, int D, const int32_t *ran
   if (work == nullptr) return set_arg_error("draw_features_backward: work area missing");
   int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);
   if (rc) return rc;
-  const int grid4 = grid_for(T, feat_bwd_minblocks<4>()), grid = grid_for(T, feat_bwd_minblocks<FEAT_G>());
-  if (grid < 0 || grid4 < 0) return set_arg_error("draw_features_backward: no device");
+  int grid4 = 0, grid = 0;
+  rc = persistent_grid(T, feat_bwd_minblocks<4>(), grid4);
+  if (rc == 0) rc = persistent_grid(T, feat_bwd_minblocks<FEAT_G>(), grid);
+  if (rc) return rc;
   for (int c0 = 0; c0 < D; c0 += FEAT_G) {
     if (c0 > 0) GSB_CUDA_TRY(cudaMemsetAsync(work, 0, sizeof(int), st));
     ProfScope ps(K_DRAW_FEAT_BWD, st);

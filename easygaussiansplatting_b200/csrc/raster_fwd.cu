@@ -1,25 +1,19 @@
 // Forward tile rasterizer: warp-autonomous 8x8 blocks and a list-driven two-record loop.
 //
-// A work item is one 8x8 pixel block of a 16x16 tile (reference BLOCK); every warp of the
-// persistent grid pulls items from a global counter and streams the tile's record list itself:
-// 32-record chunks, lane j gathers the 48-byte record of patch 32 c + j with three 16-byte
-// cp.async (double buffered, cp.async groups + __syncwarp -- no CTA barrier anywhere), tests it
-// against the block (rec_can_touch: exact, so image / contrib / final_tau are unaffected), and the
-// surviving records go into a small shared-memory list that the compositing loop walks two at a
-// time (two independent alpha' chains in flight per warp).  A lane owns two horizontally adjacent
-// pixels; the quadratic form, the alpha multiply and the compositing update are fp32 pair ops (common.cuh).
-// The backward (raster_bwd.cu) has the same structure and replays alpha' with the same operation
-// sequence, so both take identical skip decisions.
+// Every warp of the persistent grid walks its blocks' records by the protocol of raster_walk.cuh
+// (work list, cp.async chunk ring, exact culling into a survivor list); the compositing loop walks
+// the survivors two at a time (two independent alpha' chains in flight per warp).  A lane owns two
+// horizontally adjacent pixels; the quadratic form, the alpha multiply and the compositing update
+// are fp32 pair ops (common.cuh).  The backward (raster_bwd.cu) replays alpha' with the same
+// operation sequence (raster_eval.cuh), so both take identical skip decisions.
 // Replaces reference kernel.cu:152-271 (draw).
 #include "common.cuh"
 #include "kernels.h"
-#include "raster_eval.cuh"
+#include "raster_walk.cuh"
 #include "tile_io.cuh"
 
 namespace gsb {
 
-constexpr int FWD_RING = 2;  // 32-record chunks in flight per warp
-constexpr int FWD_CHUNK_BYTES = 32 * 48;
 #ifndef DRAW_MINBLOCKS
 #define DRAW_MINBLOCKS 8
 #endif
@@ -127,7 +121,7 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
                                           float *__restrict__ image, int32_t *__restrict__ contrib,
                                           float *__restrict__ final_tau, float *__restrict__ depth_image,
                                           float *__restrict__ alpha_image, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][FWD_RING * FWD_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
   __shared__ __align__(16) uint2 s_list[4][34];  // (record address, patch index + 1) of a chunk's survivors
   __shared__ __align__(16) Rec s_dummy;          // all-zero record (alpha = 0): pads an odd survivor count
 
@@ -137,33 +131,20 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
   const uint32_t ring_addr = opaque_u32(smem_u32(&s_ring[warp][0]));
   const uint32_t list_addr = opaque_u32(smem_u32(&s_list[warp][0]));
   const uint32_t dummy_addr = smem_u32(&s_dummy);
-  if (threadIdx.x < 12) reinterpret_cast<float *>(&s_dummy)[threadIdx.x] = 0.0f;
-  __syncthreads();  // (the only CTA-wide barrier: start-up)
+  zero_dummy(s_dummy);
   (void)T;
   const int items = work[1];  // entries of the work list (k_tile_list)
   const int *__restrict__ entries = work + 2;
 
   for (;;) {
-    int item = 0;
-    if (lane == 0) item = atomicAdd(work, 1);
-    item = __shfl_sync(0xffffffffu, item, 0);
+    const int item = pull_item(work, lane);
     if (item >= items) break;
     const int ent = __ldg(entries + item);
     const int tile = ent >> 3, code = ent & 7;
     const bool whole_tile = code == 4;  // <= 32 patches: this warp renders all four blocks from one gather
     const int2 range = __ldg(ranges + tile);
     const int len = range.y - range.x;
-    if (whole_tile) {  // the tile's single chunk, gathered once (two groups: see the wait below)
-      if (lane < len) {
-        const char *src = reinterpret_cast<const char *>(recs + __ldg(gsid + range.x + lane));
-        const uint32_t dst = ring_addr + lane * 48;
-        cp_async16_sa(dst, src);
-        cp_async16_sa(dst + 16, src + 16);
-        cp_async16_sa(dst + 32, src + 32);
-      }
-      cp_async_commit();
-      cp_async_commit();
-    }
+    if (whole_tile) gather_whole_tile(ring_addr, recs, gsid + range.x, len, lane);
    for (int blk = whole_tile ? 0 : code; blk < (whole_tile ? 4 : code + 1); blk++) {
     const int tx = tile % gx, ty = tile / gx;
     const int rx0 = tx * TILE + (blk & 1) * 8, ry0 = ty * TILE + (blk >> 1) * 8;
@@ -179,21 +160,16 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
       const int nch = (len + 31) >> 5;
       const int32_t *ids = gsid + range.x;
       auto issue = [&](int c, int id) {
-        if (c < nch && c * 32 + lane < len) {
-          const char *src = reinterpret_cast<const char *>(recs + id);
-          const uint32_t dst = ring_addr + (c & (FWD_RING - 1)) * FWD_CHUNK_BYTES + lane * 48;
-          cp_async16_sa(dst, src);
-          cp_async16_sa(dst + 16, src + 16);
-          cp_async16_sa(dst + 32, src + 32);
-        }
+        if (c < nch && c * 32 + lane < len)
+          gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
         cp_async_commit();
       };
       auto load_id = [&](int c) { return (c < nch && c * 32 + lane < len) ? __ldg(ids + c * 32 + lane) : 0; };
       int id_next = 0;
       if (!whole_tile) {
 #pragma unroll
-        for (int r = 0; r < FWD_RING; r++) issue(r, load_id(r));
-        id_next = load_id(FWD_RING);
+        for (int r = 0; r < WALK_RING; r++) issue(r, load_id(r));
+        id_next = load_id(WALK_RING);
       }
 
       const float2 npx = p2(-(float)px, -(float)(px + 1));
@@ -203,18 +179,10 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
       tau = p2(in0 ? 1.0f : 0.0f, in1 ? 1.0f : 0.0f);
 
       for (int c = 0; c < nch; c++) {
-        cp_async_wait<FWD_RING - 1>();  // this lane's copy of chunk c has landed ...
-        __syncwarp();                  // ... and so have the other lanes'
-        const uint32_t my_rec = ring_addr + (c & (FWD_RING - 1)) * FWD_CHUNK_BYTES + lane * 48;
-        const int my_idx = c * 32 + lane;
-        bool hit = false;
-        if (my_idx < len) hit = rec_can_touch(lds128(my_rec), lds128(my_rec + 16), bx0, bx1, by0, by1);
-        // survivors of the chunk, front to back, as a list of (record address, patch index + 1)
-        const unsigned mask = __ballot_sync(0xffffffffu, hit);
-        const int n = __popc(mask);
-        if (hit) sts64u(list_addr + __popc(mask & ((1u << lane) - 1u)) * 8, my_rec, (uint32_t)my_idx + 1u);
-        if (lane == 0) sts64u(list_addr + n * 8, dummy_addr, 0u);  // pad (alpha = 0: never contributes)
-        __syncwarp();
+        // survivors of the chunk, front to back, as (record address, patch index + 1); the pad
+        // record has alpha = 0 and never contributes
+        const int n = cull_compact(wait_chunk(ring_addr, c, lane), c * 32 + lane, len, bx0, bx1, by0, by1,
+                                          list_addr, dummy_addr, 1u, 0u, lane, no_hit_work, no_pad_work);
         for (int i = 0; i < n; i += 2) {
           const uint4 ent = lds128u(list_addr + i * 8);
           const float4 q0a = lds128(ent.x), q0b = lds128(ent.z);
@@ -258,11 +226,10 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
         const bool done = __all_sync(0xffffffffu, tau.x < TAU_STOP && tau.y < TAU_STOP);
         if (done) break;
         __syncwarp();  // every lane is done with this ring slot and with the list
-        issue(c + FWD_RING, id_next);
-        id_next = load_id(c + FWD_RING + 1);
+        issue(c + WALK_RING, id_next);
+        id_next = load_id(c + WALK_RING + 1);
       }
-      cp_async_wait<0>();
-      __syncwarp();
+      walk_drain();
     }
     if (in0 && in1 && vec2) {
       *reinterpret_cast<float2 *>(image + pix) = cr;
@@ -326,11 +293,9 @@ int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int3
   // work list (and the zeros of the empty tiles) first; it also clears the item counter
   int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st);
   if (rc) return rc;
-  int dev = 0, sms = 132;
-  GSB_CUDA_TRY(cudaGetDevice(&dev));
-  GSB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long want = (long long)sms * DRAW_MINBLOCKS;
-  const int grid = (int)(T < want ? T : want);
+  int grid = 0;
+  rc = persistent_grid(T, DRAW_MINBLOCKS, grid);
+  if (rc) return rc;
   if (depth_image != nullptr) {
     ProfScope ps(K_DRAW_RGBD, st);
     k_draw_rgbd<<<grid, 128, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, image,
