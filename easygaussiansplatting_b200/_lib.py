@@ -55,6 +55,8 @@ SIGNATURES = {
     "gsb_splat_forward_rgbd": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_uint32, _vp, _sz, _vp,
                                     _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "gsb_splat_backward_rgbd": (_i, [_i, _i, _i, _i64] + [_vp] * 14 + [_sz] + [_vp] * 7),
+    "gsb_splat_backward_abs": (_i, [_i, _i, _i, _i64] + [_vp] * 11 + [_sz] + [_vp] * 7),
+    "gsb_splat_backward_rgbd_abs": (_i, [_i, _i, _i, _i64] + [_vp] * 14 + [_sz] + [_vp] * 8),
     "gsb_preprocess_backward_pose_workspace_bytes": (_sz, [_i]),
     "gsb_preprocess_backward_pose": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 14 + [_sz, _vp]),
     "gsb_preprocess_forward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 9),

@@ -42,7 +42,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
                                              "draw_features", "draw_backward_features", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
-                                             "mcmc_noise", "adam", "draw_rgbd",
+                                             "mcmc_noise", "draw_backward_abs", "draw_backward_rgbd_abs",
+                                             "adam", "draw_rgbd",
                                              "draw_backward_rgbd"};
 
 ProfScope::ProfScope(int id, cudaStream_t st) : id_(id), st_(st), stop_(nullptr) {
@@ -599,7 +600,7 @@ static int splat_backward_impl(int H, int W, int N, int64_t P, const float *us, 
                                const int32_t *gsid_per_patch, const float *dloss_dgammas, const DepthGrads *dg,
                                const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
                                float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
-                               gsb_stream_t stream) {
+                               float *dloss_dus_abs, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splatB: bad N/H/W/P");
   GSB_REQUIRE(N == 0 || moments_out || (dloss_dus && dloss_dcinv2ds && dloss_dalphas && dloss_dcolors),
               "splatB: null output");
@@ -631,7 +632,7 @@ static int splat_backward_impl(int H, int W, int N, int64_t P, const float *us, 
   // P == 0: nothing was drawn; the zeroed moment rows finalise to all-zero gradients
   return launch_draw_backward(H, W, N, patch_range_per_tile, P > 0 ? recs : nullptr, gsid_per_patch, contrib, final_tau,
                               dloss_dgammas, dg, cinv2ds, moments, work, dloss_dus, dloss_dcinv2ds, dloss_dalphas,
-                              dloss_dcolors, moments_out == nullptr, st);
+                              dloss_dcolors, moments_out == nullptr, dloss_dus_abs, st);
 }
 
 int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -643,7 +644,8 @@ int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const fl
   // (the re-pack leaves the records' depth word 0: k_draw_bwd never reads it)
   return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws,
-                             ws_bytes, dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, stream);
+                             ws_bytes, dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, nullptr,
+                             stream);
 }
 
 int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -658,7 +660,37 @@ int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, con
   const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
   return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
-                             dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, stream);
+                             dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, nullptr, stream);
+}
+
+int gsb_splat_backward_abs(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                           const float *alphas, const float *colors, const int32_t *contrib, const float *final_tau,
+                           const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                           const float *dloss_dgammas, const void *packed_records, void *ws, size_t ws_bytes,
+                           float *dloss_dus, float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors,
+                           float *moments_out, float *dloss_dus_abs, gsb_stream_t stream) {
+  GSB_REQUIRE(N <= 0 || dloss_dus_abs != nullptr, "splatB_abs: null dloss_dus_abs");
+  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
+                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws,
+                             ws_bytes, dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out,
+                             dloss_dus_abs, stream);
+}
+
+int gsb_splat_backward_rgbd_abs(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                                const float *alphas, const float *colors, const float *depths, const int32_t *contrib,
+                                const float *final_tau, const int32_t *patch_range_per_tile,
+                                const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                                const float *dloss_ddepth_image, const float *dloss_dalpha_image,
+                                const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
+                                float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
+                                float *dloss_ddepths, float *dloss_dus_abs, gsb_stream_t stream) {
+  GSB_REQUIRE(N <= 0 || dloss_dus_abs != nullptr, "splatB_rgbd_abs: null dloss_dus_abs");
+  GSB_REQUIRE(N <= 0 || dloss_ddepths != nullptr, "splatB_rgbd: null dloss_ddepths");
+  const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
+  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
+                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
+                             dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, dloss_dus_abs,
+                             stream);
 }
 
 // ---- feature rendering (raster_feat.cu)

@@ -19,7 +19,7 @@ enum KernelId {
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
   K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
-  K_MCMC_ROWS, K_MCMC_NOISE, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_MCMC_ROWS, K_MCMC_NOISE, K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -236,12 +236,14 @@ struct DepthGrads {
   const float *dloss_dalpha_image;
   float *ddepths;
 };
-// dg == nullptr: k_draw_bwd; otherwise k_draw_bwd_rgbd
+// dg == nullptr: k_draw_bwd; otherwise k_draw_bwd_rgbd.  dus_abs: NULL, or [N,2] (any 4-byte
+// alignment, zeroed here) for the per-pixel absolute sums of dL/du: then k_draw_bwd_abs /
+// k_draw_bwd_rgbd_abs
 int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
                          const int32_t *contrib, const float *final_tau, const float *dloss_dgammas,
                          const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
                          float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
-                         cudaStream_t st);
+                         float *dus_abs, cudaStream_t st);
 
 // ---- feature rasterizers (raster_feat.cu): replays of the colour forward's binning that composite
 // features[N,D] (row stride D, any 4-byte alignment) with the image's weights.  ranges: any

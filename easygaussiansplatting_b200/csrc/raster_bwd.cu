@@ -18,6 +18,11 @@
 // and add them into the Gaussian's contiguous 9-float moment row (red.global.add).
 // k_finalize_grads turns moment rows into the four gradient tensors:
 //   dL/du = -(A Sx + B Sy, B Sx + C Sy),  dL/dconic = (-Sxx/2, -Sxy, -Syy/2).
+//
+// The _abs kernels (absolute-gradient densification, DESIGN 3.13) also sum, per Gaussian, the
+// absolute value of every pixel's term of dL/du: sum_p |w (A dx + B dy)|, sum_p |w (B dx + C dy)|.
+// |.| is not linear, so these cannot come from the moment rows; phase B forms them from the same
+// w it reads for the moments.
 #include "common.cuh"
 #include "kernels.h"
 #include "raster_walk.cuh"
@@ -31,8 +36,18 @@ namespace gsb {
 #ifndef DRAW_BWD_RGBD_MINBLOCKS
 #define DRAW_BWD_RGBD_MINBLOCKS 5
 #endif
+// the _abs kernels: 96 registers and a small spill at 5 CTAs/SM, measured faster than 128
+// registers without spills at 4 (DESIGN 3.13)
+#ifndef DRAW_BWD_ABS_MINBLOCKS
+#define DRAW_BWD_ABS_MINBLOCKS 5
+#endif
+#ifndef DRAW_BWD_RGBD_ABS_MINBLOCKS
+#define DRAW_BWD_RGBD_ABS_MINBLOCKS 5
+#endif
 
 namespace {
+__device__ __forceinline__ float2 abs2(float2 a) { return make_float2(fabsf(a.x), fabsf(a.y)); }
+
 // Phase B: moment sums of up to 8 records over the warp's 8x8 block.
 //   lane = slot * 4 + part; part covers x in [4 (part & 1), +4) of rows (part >> 1) + {0, 2, 4, 6}.
 //   inf = record word q0 = (u_x, u_y, gaussian id, alpha) of the lane's slot.  It travels in registers:
@@ -40,10 +55,13 @@ namespace {
 //   costs 4 of them even from one lane (benchmarks/micro/redux_bench.cu).
 //   RGBD: a tenth sum, wc dL/dD = dL/dz, over a fourth dL/d-plane at dl_addr + 768; it goes to
 //   ddepths[id] from the part-3 lane (which carries only one other reduction).
-template <bool RGBD>
-__device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, uint32_t dl_addr, int nslots,
-                                          float fbx0, float fby0, float *__restrict__ moments,
-                                          float *__restrict__ ddepths, int lane) {
+//   ABS: cq = record word q1 = log2e (-A/2, -B, -C/2) of the slot, carried next to inf; two more sums
+//   sum |w| |2 q1.x dx + q1.y dy|, sum |w| |q1.y dx + 2 q1.z dy|, scaled by 1/log2e once, go to
+//   dus_abs[id] from the part-2 (x) and part-3 (y) lanes, which carry the fewest other reductions.
+template <bool RGBD, bool ABS>
+__device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, const float4 &cq, uint32_t dl_addr,
+                                          int nslots, float fbx0, float fby0, float *__restrict__ moments,
+                                          float *__restrict__ ddepths, float *__restrict__ dus_abs, int lane) {
   const int slot = lane >> 2, part = lane & 3;
   const float U = inf.x - (fbx0 + (float)((part & 1) * 4));
   const float V = inf.y - (fby0 + (float)(part >> 1));
@@ -52,6 +70,8 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
   const uint32_t d = dl_addr + part * 16;
   float2 m0 = p2s(0.f), m1 = p2s(0.f), m2 = p2s(0.f), m3 = p2s(0.f), m4 = p2s(0.f), m5 = p2s(0.f),
          m6 = p2s(0.f), m7 = p2s(0.f), m8 = p2s(0.f), m9 = p2s(0.f);
+  float2 ax = p2s(0.f), ay = p2s(0.f);  // ABS only
+  const float cx2 = 2.0f * cq.x, cz2 = 2.0f * cq.z;
 #pragma unroll
   for (int j = 0; j < 4; j++) {
     const float dy = V - (float)(2 * j);
@@ -80,6 +100,13 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
       const float4 dd = lds128(d + 768 + j * 64);
       m9 = fma2_rn(lo(wc), lo(dd), m9);
       m9 = fma2_rn(hi(wc), hi(dd), m9);
+    }
+    if (ABS) {
+      const float2 bx = p2s(cq.y * dy), by = p2s(cz2 * dy);
+      ax = add2_rn(ax, abs2(mul2_rn(lo(w), fma2_rn(p2s(cx2), dx01, bx))));
+      ax = add2_rn(ax, abs2(mul2_rn(hi(w), fma2_rn(p2s(cx2), dx23, bx))));
+      ay = add2_rn(ay, abs2(mul2_rn(lo(w), fma2_rn(p2s(cq.y), dx01, by))));
+      ay = add2_rn(ay, abs2(mul2_rn(hi(w), fma2_rn(p2s(cq.y), dx23, by))));
     }
   }
   // sum dL/dalpha' g = (sum w) / alpha; records above the clamp were reduced in phase A
@@ -110,6 +137,13 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
     z += __shfl_xor_sync(F, z, 2);
     if (slot < nslots && part == 3) atomicAdd(ddepths + __float_as_int(inf.z), z);
   }
+  if (ABS) {  // parts 0 and 2 gather the x sums, parts 1 and 3 the y sums
+    const float sx = ax.x + ax.y, sy = ay.x + ay.y;
+    float h = (u1 ? sy : sx) + __shfl_xor_sync(F, u1 ? sx : sy, 1);
+    h += __shfl_xor_sync(F, h, 2);
+    if (slot < nslots && u2)
+      atomicAdd(dus_abs + (size_t)__float_as_int(inf.z) * 2 + (part & 1), h * (1.0f / LOG2E));
+  }
 }
 }  // namespace
 
@@ -117,14 +151,15 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, ui
 // pixel also has dL/dD and dL/dA, so in phase A dL/dalpha' gains (dL/dD z + dL/dA) next to
 // dL/dgamma . c (the sdot recurrence carries the sum of all five channels), and phase B sums
 // wc dL/dD into dL/dz from a fourth per-pixel table.  dL/dA needs no table: opacity has no
-// per-Gaussian value to differentiate.
-template <bool RGBD>
+// per-Gaussian value to differentiate.  ABS: the _abs kernels; phase A also keeps the lane's slot's
+// record word q1 (the conic) for bwd_flush's absolute sums into dus_abs.
+template <bool RGBD, bool ABS>
 __device__ __forceinline__ void draw_bwd_body(
     int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
-    int *__restrict__ work) {
+    float *__restrict__ dus_abs, int *__restrict__ work) {
   __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
   __shared__ __align__(16) unsigned char s_w[4][WALK_W_BYTES];                   // weight rows, per warp
   __shared__ __align__(16) float s_dl[4][RGBD ? 4 : 3][64];                    // dL/dgamma (dL/dD) of the block
@@ -230,6 +265,7 @@ __device__ __forceinline__ void draw_bwd_body(
     const uint32_t wa_pair_limit = w_addr + lane * 8 + (WALK_SLOTS - 2) * WALK_SLOT_BYTES;
     int to_my_slot = lane >> 2;  // free slots before the one whose moments this lane sums in phase B
     float4 inf = make_float4(0.f, 0.f, 0.f, 1.f);
+    float4 cq = make_float4(0.f, 0.f, 0.f, 0.f);  // ABS only
 
     for (int c = nch - 1; c >= 0; c--) {
       // survivors of the chunk, back to front, as (record address, patch index); the pad's index
@@ -246,7 +282,8 @@ __device__ __forceinline__ void draw_bwd_body(
       for (int i = 0; i < n; i += 2) {
         if (wa > wa_pair_limit) {  // no room for a pair
           __syncwarp();
-          bwd_flush<RGBD>(w_addr, inf, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, ddepths, lane);
+          bwd_flush<RGBD, ABS>(w_addr, inf, cq, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, ddepths,
+                               dus_abs, lane);
           __syncwarp();
           wa = w_addr + lane * 8;
           to_my_slot = lane >> 2;
@@ -273,6 +310,7 @@ __device__ __forceinline__ void draw_bwd_body(
         sts64(wa, mul2_rn(dapa, A.e));        // w
         sts64(wa + 256, mul2_rn(A.e, tau));   // wc
         if (to_my_slot == 0) inf = q0a;
+        if (ABS && to_my_slot == 0) cq = q1a;
         // second record (the all-zero pad record when the count is odd: e = 0, weights 0)
         tau = mul2_rn(tau, B.rc);
         const float2 diffb = add2_rn(dcb, p2(-sdot.x, -sdot.y));
@@ -281,6 +319,7 @@ __device__ __forceinline__ void draw_bwd_body(
         sts64(wa + WALK_SLOT_BYTES, mul2_rn(dapb, B.e));
         sts64(wa + WALK_SLOT_BYTES + 256, mul2_rn(B.e, tau));
         if (to_my_slot == 1) inf = q0b;
+        if (ABS && to_my_slot == 1) cq = q1b;
         if (fmaxf(q0a.w, q0b.w) > ALPHA_CLAMP) {  // opacity above the clamp (rare):
           // sum dL/dalpha' g is not (sum w) / alpha on clamped pixels -- reduce it with shuffles
           float va = q0a.w > ALPHA_CLAMP ? fmaf(A.e.x > 0.f ? dapa.x : 0.f, A.gg.x, (A.e.y > 0.f ? dapa.y : 0.f) * A.gg.y) : 0.0f;
@@ -304,7 +343,8 @@ __device__ __forceinline__ void draw_bwd_body(
     cp_async_wait<0>();
     if (wa != w_addr + lane * 8) {
       __syncwarp();
-      bwd_flush<RGBD>(w_addr, inf, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, ddepths, lane);
+      bwd_flush<RGBD, ABS>(w_addr, inf, cq, dl_addr, (lane >> 2) - to_my_slot, bx0, by0, moments, ddepths, dus_abs,
+                           lane);
     }
     __syncwarp();  // the flush has read s_dl / s_w before the next block rewrites them
   }
@@ -314,8 +354,8 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
     int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ dloss_dgammas, float *__restrict__ moments, int *__restrict__ work) {
-  draw_bwd_body<false>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr, moments,
-                       nullptr, work);
+  draw_bwd_body<false, false>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr,
+                              moments, nullptr, nullptr, work);
 }
 
 __global__ void __launch_bounds__(128, DRAW_BWD_RGBD_MINBLOCKS) k_draw_bwd_rgbd(
@@ -324,8 +364,27 @@ __global__ void __launch_bounds__(128, DRAW_BWD_RGBD_MINBLOCKS) k_draw_bwd_rgbd(
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
     int *__restrict__ work) {
-  draw_bwd_body<true>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
-                      dloss_dalpha_image, moments, ddepths, work);
+  draw_bwd_body<true, false>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
+                             dloss_dalpha_image, moments, ddepths, nullptr, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_BWD_ABS_MINBLOCKS) k_draw_bwd_abs(
+    int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    const float *__restrict__ dloss_dgammas, float *__restrict__ moments, float *__restrict__ dus_abs,
+    int *__restrict__ work) {
+  draw_bwd_body<false, true>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr,
+                             moments, nullptr, dus_abs, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_BWD_RGBD_ABS_MINBLOCKS) k_draw_bwd_rgbd_abs(
+    int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
+    const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
+    float *__restrict__ dus_abs, int *__restrict__ work) {
+  draw_bwd_body<true, true>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
+                            dloss_dalpha_image, moments, ddepths, dus_abs, work);
 }
 
 constexpr int MOM = 9;  // floats per moment row
@@ -374,20 +433,32 @@ int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *
                          const int32_t *contrib, const float *final_tau, const float *dloss_dgammas,
                          const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
                          float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
-                         cudaStream_t st) {
+                         float *dus_abs, cudaStream_t st) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0 || N <= 0) return 0;
   GSB_CUDA_TRY(cudaMemsetAsync(moments, 0, sizeof(float) * MOM * (size_t)N, st));
   if (dg != nullptr) GSB_CUDA_TRY(cudaMemsetAsync(dg->ddepths, 0, sizeof(float) * (size_t)N, st));
+  if (dus_abs != nullptr) GSB_CUDA_TRY(cudaMemsetAsync(dus_abs, 0, sizeof(float) * 2 * (size_t)N, st));
   if (recs != nullptr) {
     const int T = gx * gy;
     if (work == nullptr) return set_arg_error("drawB: work area missing");
     int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);  // tiles with patches
     if (rc) return rc;
     int grid = 0;
-    rc = persistent_grid(T, dg != nullptr ? DRAW_BWD_RGBD_MINBLOCKS : DRAW_BWD_MINBLOCKS, grid);
+    const int per_sm = dus_abs != nullptr ? (dg != nullptr ? DRAW_BWD_RGBD_ABS_MINBLOCKS : DRAW_BWD_ABS_MINBLOCKS)
+                                          : (dg != nullptr ? DRAW_BWD_RGBD_MINBLOCKS : DRAW_BWD_MINBLOCKS);
+    rc = persistent_grid(T, per_sm, grid);
     if (rc) return rc;
-    if (dg != nullptr) {
+    if (dus_abs != nullptr && dg != nullptr) {
+      ProfScope ps(K_DRAW_BWD_RGBD_ABS, st);
+      k_draw_bwd_rgbd_abs<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
+                                                dg->dloss_ddepth_image, dg->dloss_dalpha_image, moments, dg->ddepths,
+                                                dus_abs, work);
+    } else if (dus_abs != nullptr) {
+      ProfScope ps(K_DRAW_BWD_ABS, st);
+      k_draw_bwd_abs<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, moments,
+                                           dus_abs, work);
+    } else if (dg != nullptr) {
       ProfScope ps(K_DRAW_BWD_RGBD, st);
       k_draw_bwd_rgbd<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
                                             dg->dloss_ddepth_image, dg->dloss_dalpha_image, moments, dg->ddepths,

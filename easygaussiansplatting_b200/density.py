@@ -139,10 +139,17 @@ def apply_rows(cls, slots, counts, src, src_m=None, src_v=None):
 
 class DensityController:
     """the density-control half of gsplat.gsmodel.GSModel (gsmodel.py:168-331), same attribute
-    names (`grad_accum`, `cunt`) and the same printed report"""
+    names (`grad_accum`, `cunt`) and the same printed report.
 
-    def __init__(self, sense_size, verbose=True):
-        self.grad_threshold = 4e-7
+    grad_threshold: the mean per-view |statistic| at or above which a Gaussian is cloned or split
+    (the reference's 4e-7 by default).  Absolute-gradient densification (AbsGS) feeds
+    update_density_info the `us_abs.grad` of the fused classes instead of `us.grad`; each view's
+    norm is then >= the signed one, so the default threshold densifies more.  gsplat raises its
+    threshold 4x for absgrad; no threshold for the absolute statistic has been measured with this
+    library, so tune it for the scene."""
+
+    def __init__(self, sense_size, verbose=True, grad_threshold=4e-7):
+        self.grad_threshold = grad_threshold
         self.scale_threshold = 0.01 * sense_size
         self.alpha_threshold = 0.005
         self.big_threshold = 0.1 * sense_size
@@ -153,7 +160,8 @@ class DensityController:
         self.verbose = verbose
 
     def update_density_info(self, dloss_dus, mask):
-        """gsmodel.py:219-234 (the caller passes us.grad and the GSFunction mask)"""
+        """gsmodel.py:219-234 (the caller passes us.grad -- or, for absolute-gradient
+        densification, us_abs.grad of the fused classes -- and the GSFunction mask)"""
         N = dloss_dus.shape[0]
         first = self.cunt is None
         if first:

@@ -102,11 +102,17 @@ class GSFunctionFused(torch.autograd.Function):
     in gsplat/gsmodel.py.
     All four fused classes take an optional trailing `filter3d[N]` (ops.filter3d; after `cam`):
     the Mip-Splatting 3D filter, a constant that gets no gradient.  The frame is then rendered from
-    s', alpha' (ops.filter3d_apply) and the scale and opacity gradients are taken back through it."""
+    s', alpha' (ops.filter3d_apply) and the scale and opacity gradients are taken back through it.
+    They also take an optional `us_abs[N,2]` after filter3d (absolute-gradient densification, AbsGS):
+    a dummy input, normally zeros with requires_grad=True, whose gradient is the per-pixel absolute
+    sum of dL/du (ops.splatB(..., absgrad=True)), as `us` is the dummy whose gradient is dL/du.
+    `DensityController.update_density_info(us_abs.grad, mask)` then densifies on it.  The
+    rasterizer's _abs kernel runs only when us_abs requires a gradient; every other gradient is the
+    one the call without us_abs returns.  Single view: refused with cam.grad_exchange."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None):
-        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d)
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None, us_abs=None):
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d, us_abs=us_abs)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
@@ -119,26 +125,41 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
         depth[p] = sum_i w_i(p) z_i,   alpha[p] = sum_i w_i(p)
     (w = tau alpha', the image's compositing weights; z = camera-frame depth).  depth is not
     normalised: depth / alpha is the expected depth.  Gradients of all three images flow to pws,
-    shs, alphas, scales, rots and us; the depth term reaches pws through z = (Rcw pw + tcw)[2]."""
+    shs, alphas, scales, rots and us; the depth term reaches pws through z = (Rcw pw + tcw)[2].
+    us_abs (after filter3d) as for GSFunctionFused: its gradient sums the per-pixel terms of all
+    three planes."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None):
-        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d)
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None, us_abs=None):
+        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, filter3d=filter3d, us_abs=us_abs)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
         return _fused_backward(ctx, True, False, dloss_dgammas, dloss_ddepth, dloss_dalpha)
 
 
-def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None, filter3d=None, features=None):
+def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None, filter3d=None, features=None,
+                   us_abs=None):
     """The forward of the fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
     camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward.
     cam.antialiased (absent: False): the rasterizers composite alpha_eff = rho * alpha.
     filter3d: None, or the Mip-Splatting 3D filter[N] (ops.filter3d, a constant): the frame is
     rendered from s' = sqrt(s^2 + f^2) and alpha' = alpha prod s / s' (ops.filter3d_apply).
     features: None, or [N, D]: the feature map [D, H, W] follows the image (ops.splat_features,
-    from the same records) and features is saved last."""
+    from the same records) and features is saved last.
+    us_abs: None, or the [N,2] dummy input whose gradient is the absolute-gradient statistic; its
+    gradient slot (after cam and filter3d) is kept in ctx.abs_slot."""
     from . import ops
+    ctx.abs_slot = None
+    if us_abs is not None:
+        if getattr(cam, "grad_exchange", None) is not None:
+            raise ValueError("us_abs is single-view: cam.grad_exchange must not be set")
+        if not isinstance(us_abs, torch.Tensor) or tuple(us_abs.shape) != (pws.shape[0], 2):
+            raise ValueError("us_abs must be a [N, 2] tensor (N = %d), got %s"
+                             % (pws.shape[0], tuple(getattr(us_abs, "shape", ()))))
+        if us_abs.device != pws.device:
+            raise ValueError("us_abs must be on the device of pws (%s), got %s" % (pws.device, us_abs.device))
+        ctx.abs_slot = 6 + (3 if pose is not None else 0) + 2
     ctx.filtered = filter3d is not None
     raw = ()
     if ctx.filtered:
@@ -194,9 +215,13 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
         feat = (rest.pop(), dloss_dfeatures_map)
     Rcw, tcw, twc = rest[:3] if pose else (cam.Rcw, cam.tcw, cam.twc)
     raw = rest[3:] if pose else rest  # (scales, alphas, filter3d) of a filtered frame
+    need_abs = ctx.abs_slot is not None and ctx.needs_input_grad[ctx.abs_slot]
     grads = _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds,
                                  depths, colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw,
-                                 twc, dloss_dgammas, dloss_ddepth, dloss_dalpha, feat if featured else None)
+                                 twc, dloss_dgammas, dloss_ddepth, dloss_dalpha, feat if featured else None,
+                                 absgrad=need_abs)
+    if need_abs:
+        grads, dabs = grads[:-1], grads[-1]
     if featured:  # dL/dfeatures goes right after the map inputs (the pose classes take no features)
         grads, dfeat = grads[:-1], grads[-1]
     if ctx.filtered and grads[3] is not None:
@@ -206,29 +231,39 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
         grads = grads[:2] + (dalphas, dscales) + grads[4:]
     if featured:
         grads = grads + (dfeat,)
+    if need_abs:  # cam and filter3d get None, us_abs the statistic
+        grads = grads + (None,) * (ctx.abs_slot - len(grads)) + (dabs,)
     # one gradient per input apply received (cam, and filter3d when passed -- also as None -- get None)
     return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
 def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths,
                          colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw, twc,
-                         dloss_dgammas, dloss_ddepth, dloss_dalpha, feat=None):
+                         dloss_dgammas, dloss_ddepth, dloss_dalpha, feat=None, absgrad=False):
     """the gradients of the inputs the frame was rendered from, up to and including the pose's;
     feat: None, or (features, dL/dfeature map or None) -> dL/dfeatures (None when no map gradient
-    came) appended"""
+    came) appended; absgrad: the rasterizer's _abs kernel runs and its dloss_dus_abs[N,2] is
+    appended last (not with feat)"""
     need_map = any(ctx.needs_input_grad[:6])
     need_cam = pose and any(ctx.needs_input_grad[6:9])
     # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward converts
     # them in registers (no finalize pass, no 32 B/Gaussian round trip).  (autograd hands zeros for
     # an RGB-D output the loss does not use: all three planes are given)  With antialiasing the
     # rasterizer replays alpha_eff (`drawn`), and the per-Gaussian backward takes the raw alphas.
-    ddepths = None
+    ddepths = dabs = None
     if rgbd:
-        moments, ddepths = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib,
-                                           final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas,
-                                           dloss_ddepth, dloss_dalpha, moments_only=True)
+        rb = ops.splatB_rgbd(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
+                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha,
+                             moments_only=True, absgrad=absgrad)
+        moments, ddepths = rb[:2]
+        if absgrad:
+            dabs = rb[2]
     elif dloss_dgammas is None:  # (the feature class: no image gradient, no colour replay)
         moments = torch.zeros((pws.shape[0], 9), dtype=torch.float32, device=pws.device)
+    elif absgrad:
+        moments, dabs = ops.splatB(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
+                                   patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True,
+                                   absgrad=True)
     else:
         moments = ops.splatB(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=True)
@@ -261,6 +296,8 @@ def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, sca
         grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
     elif pose:
         grads += (None, None, None)
+    if absgrad:
+        return grads + (dabs,)
     return grads + (dfeat,) if feat is not None else grads
 
 
@@ -296,11 +333,13 @@ class GSFunctionFusedPose(torch.autograd.Function):
     and get dL/dRcw, dL/dtcw, dL/dtwc as independent inputs: a caller that builds twc from Rcw
     and tcw with torch ops has autograd chain it.  What runs follows ctx.needs_input_grad:
     only the camera -> the pose-only kernel (a frozen map: tracking); no camera -> exactly
-    GSFunctionFused's backward.  Intrinsics are not differentiated; single view only."""
+    GSFunctionFused's backward.  Intrinsics are not differentiated; single view only.  us_abs (after
+    filter3d) as for GSFunctionFused, also with the pose-only backward."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None):
-        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d)
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None, us_abs=None):
+        return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d,
+                              us_abs=us_abs)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
@@ -310,11 +349,13 @@ class GSFunctionFusedPose(torch.autograd.Function):
 class GSFunctionFusedRGBDPose(torch.autograd.Function):
     """GSFunctionFusedRGBD with a differentiable camera pose, as GSFunctionFusedPose:
     `apply(pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)` -> (image, depth, alpha,
-    depths > 0.2).  The depth plane's gradient reaches the pose through z = (Rcw pw + tcw)[2]."""
+    depths > 0.2).  The depth plane's gradient reaches the pose through z = (Rcw pw + tcw)[2].
+    us_abs (after filter3d) as for GSFunctionFusedRGBD."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None):
-        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d)
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None, us_abs=None):
+        return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d,
+                              us_abs=us_abs)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):

@@ -398,20 +398,24 @@ def clear_record_cache():
 
 
 def splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau,
-           patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=False, records=None):
+           patch_range_per_tile, gsid_per_patch, dloss_dgammas, moments_only=False, records=None, absgrad=False):
     """ext.cpp:20-32.  -> [dloss_dus[N,1,2], dloss_dcinv2ds[N,1,3], dloss_dalphas[N,1,1],
     dloss_dcolors[N,1,3]]   (`depths` is accepted and unused, as in the reference)
     moments_only (extension): -> the raw moment rows [N,9] for `preprocessB(..., moments=...)`;
     the conversion pass to the four tensors is skipped.
     records (extension): the forward's packed per-Gaussian records [N,12] (what `splat` was given,
     or its own); they are used as they are instead of those `splat` attached to gsid_per_patch,
-    and nothing is re-packed."""
+    and nothing is re-packed.
+    absgrad (extension; AbsGS): dloss_dus_abs[N,2], the per-pixel absolute sums of dL/du
+    (gsb_splat_backward_abs), is appended to what the call returns otherwise; every other output
+    is the same."""
     return _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
-                   gsid_per_patch, dloss_dgammas, None, None, moments_only, records)
+                   gsid_per_patch, dloss_dgammas, None, None, moments_only, records, absgrad)
 
 
 def splatB_rgbd(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
-                gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only=False, records=None):
+                gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only=False, records=None,
+                absgrad=False):
     """Backward of `splat_rgbd`: `splatB`'s arguments plus dloss_ddepth[H,W] and dloss_dalpha[H,W]
     (dL/dD, dL/dA); `depths` is read (the records' depth words).
     -> [dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors] as `splatB`, + dloss_ddepths[N]
@@ -419,14 +423,15 @@ def splatB_rgbd(height, width, us, cinv2ds, alphas, depths, colors, contrib, fin
     for `preprocessB(..., moments=..., dloss_ddepths=...)`.
     records: as for `splatB`; they must carry z, as those `preprocess(..., alphas=...)` returns do.
     Records `splat` / `splat_rgbd` attached to gsid_per_patch are used only while `depths` is
-    unchanged too; otherwise they are re-packed from the arguments."""
+    unchanged too; otherwise they are re-packed from the arguments.
+    absgrad: as for `splatB`, appended last (the upstream gradient of all three planes enters it)."""
     return _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
-                   gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only, records)
+                   gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only, records, absgrad)
 
 
 def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
-            gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only, records):
-    """`splatB`, or `splatB_rgbd` when dloss_ddepth is given"""
+            gsid_per_patch, dloss_dgammas, dloss_ddepth, dloss_dalpha, moments_only, records, absgrad=False):
+    """`splatB`, or `splatB_rgbd` when dloss_ddepth is given; absgrad: the _abs entry points"""
     rgbd = dloss_ddepth is not None
     H, W = int(height), int(width)
     us = _chk(us, "us", last=2, ndim=2); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=2)
@@ -468,6 +473,7 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
         da = torch.empty((N, 1, 1), **o); dcol = torch.empty((N, 1, 3), **o)
         moments = None
     ddepths = torch.empty((N,), **o) if rgbd else None
+    dabs = torch.empty((N, 2), **o) if absgrad else None
     lib = _L()
     with torch.cuda.device(dev):
         if records is not None:
@@ -477,21 +483,35 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
             recs = _cached_records(gsid, key) if P > 0 else None
         # with cached records only the [N,9] moment rows are needed from the workspace
         ws = _bytes(lib.gsb_splat_backward_workspace_bytes(N, H, W, 0 if recs else P), dev)
-        if rgbd:
+        if rgbd and absgrad:
+            _lib.check(lib.gsb_splat_backward_rgbd_abs(
+                H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
+                _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dld), _ptr(dla), recs, _ptr(ws), ws.numel(),
+                _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol), _ptr(moments), _ptr(ddepths), _ptr(dabs), _stream()), lib)
+        elif rgbd:
             _lib.check(lib.gsb_splat_backward_rgbd(
                 H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
                 _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dld), _ptr(dla), recs, _ptr(ws), ws.numel(),
                 _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol), _ptr(moments), _ptr(ddepths), _stream()), lib)
+        elif absgrad:
+            _lib.check(lib.gsb_splat_backward_abs(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
+                                                  _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
+                                                  recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da),
+                                                  _ptr(dcol), _ptr(moments), _ptr(dabs), _stream()), lib)
         else:
             _lib.check(lib.gsb_splat_backward(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
                                               _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
                                               recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol),
                                               _ptr(moments), _stream()), lib)
     if moments_only:
-        return [moments, ddepths] if rgbd else moments
-    # tagged so that the reference's `dloss_d* @ jacobian` chain takes the streaming matmul
-    out = [_jac(du), _jac(dc), _jac(da), _jac(dcol)]
-    return out + [ddepths] if rgbd else out
+        out = [moments, ddepths] if rgbd else moments
+    else:
+        # tagged so that the reference's `dloss_d* @ jacobian` chain takes the streaming matmul
+        out = [_jac(du), _jac(dc), _jac(da), _jac(dcol)]
+        out = out + [ddepths] if rgbd else out
+    if not absgrad:
+        return out
+    return (out if isinstance(out, list) else [out]) + [dabs]
 
 
 # ---------------------------------------------------------------------------------------

@@ -346,6 +346,31 @@ int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, con
                             float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
                             float *dloss_ddepths, gsb_stream_t stream);
 
+/* Absolute-gradient densification (extension; AbsGS, gsplat's absgrad=True).  The arguments of
+ * gsb_splat_backward / gsb_splat_backward_rgbd, plus one output dloss_dus_abs[N,2] (any 4-byte
+ * alignment; every element written, 0 for Gaussians no pixel replays):
+ *     dloss_dus_abs[i] = ( sum_p |g_ip.x| , sum_p |g_ip.y| ),   dloss_dus[i] = sum_p g_ip,
+ *     g_ip = -w_ip (A dx + B dy, B dx + C dy),  w_ip = dL/dalpha'_ip alpha'_ip,  (dx, dy) = u_i - p,
+ * with (A, B, C) = cinv2ds[i] and dL/dalpha' that of the colour (RGB-D form: colour, depth and
+ * alpha) planes -- the per-pixel terms whose sum is dL/du.  Per-pixel gradients of opposite sign
+ * cancel in dL/du but not here, so a Gaussian that covers a large, textured region gets a large
+ * statistic to densify on.  Every other output (moments_out included) is that of the plain call.
+ * A NULL dloss_dus_abs is an argument error (unless N == 0). */
+int gsb_splat_backward_abs(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                           const float *alphas, const float *colors, const int32_t *contrib, const float *final_tau,
+                           const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                           const float *dloss_dgammas, const void *packed_records, void *ws, size_t ws_bytes,
+                           float *dloss_dus, float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors,
+                           float *moments_out, float *dloss_dus_abs, gsb_stream_t stream);
+int gsb_splat_backward_rgbd_abs(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                                const float *alphas, const float *colors, const float *depths, const int32_t *contrib,
+                                const float *final_tau, const int32_t *patch_range_per_tile,
+                                const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                                const float *dloss_ddepth_image, const float *dloss_dalpha_image,
+                                const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
+                                float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
+                                float *dloss_ddepths, float *dloss_dus_abs, gsb_stream_t stream);
+
 /* ---- feature rendering (extension).  Composites per-Gaussian feature vectors features[N,D]
  * (row-major, row stride D, any 4-byte alignment; D >= 1) with the image's weights:
  *   feature_image[c, p] = sum_i w_i(p) features[i, c],   w_i = tau_i alpha'_i
