@@ -61,6 +61,8 @@ SIGNATURES = {
     "gsb_preprocess_backward_pose": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 14 + [_sz, _vp]),
     "gsb_preprocess_forward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 9),
     "gsb_preprocess_backward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 15 + [_sz, _vp]),
+    "gsb_preprocess_forward_model": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 10),
+    "gsb_preprocess_backward_model": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 15 + [_sz, _vp, _vp]),
     "gsb_sh_grad_expand": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gsb_filter3d_workspace_bytes": (_sz, [_i, _i]),
     "gsb_filter3d": (_i, [_i, _vp, _i, _vp, _f, _vp, _vp, _sz, _vp]),

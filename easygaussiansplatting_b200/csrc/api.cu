@@ -3,6 +3,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
 #include <mutex>
 #include <vector>
 
@@ -341,6 +342,90 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
                                dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
                                dloss_drots, nullptr, &mi, dloss_ddepths, pose ? &po : nullptr, alphas,
                                (cudaStream_t)stream);
+}
+
+// ---- camera models (DESIGN 3.14).  NULL or PINHOLE passes no CamLens: the kernels of the
+// entry points above.
+static int camera_lens(const char *who, const gsb_camera_model *cm, float fx, float fy, CamLens &out,
+                       const CamLens *&lens) {
+  lens = nullptr;
+  if (cm == nullptr) return 0;
+  const char *err = nullptr;
+  const bool fin = std::isfinite(cm->k[0]) && std::isfinite(cm->k[1]) && std::isfinite(cm->k[2]) &&
+                   std::isfinite(cm->k[3]);
+  const bool k0 = cm->k[0] == 0.f && cm->k[1] == 0.f && cm->k[2] == 0.f && cm->k[3] == 0.f;
+  if (cm->model != GSB_CAMERA_PINHOLE && cm->model != GSB_CAMERA_ORTHO && cm->model != GSB_CAMERA_FISHEYE)
+    err = "unknown camera model";
+  else if (!fin)
+    err = "non-finite radial coefficient";
+  else if (cm->model != GSB_CAMERA_FISHEYE && !k0)
+    err = "radial coefficients are for the fisheye model only";
+  else if (cm->model != GSB_CAMERA_PINHOLE && !(fx > 0.f && fy > 0.f))
+    err = "fx and fy must be > 0";
+  if (err != nullptr) {
+    char msg[128];
+    snprintf(msg, sizeof(msg), "%s: %s", who, err);
+    return set_arg_error(msg);
+  }
+  if (cm->model == GSB_CAMERA_PINHOLE) return 0;
+  out.model = cm->model;
+  for (int i = 0; i < 4; i++) out.k[i] = cm->k[i];
+  lens = &out;
+  return 0;
+}
+
+int gsb_preprocess_forward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
+                                 float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
+                                 float *alphas_eff, const gsb_camera_model *camera_model, gsb_stream_t stream) {
+  CamLens cl;
+  const CamLens *lens;
+  if (int rc = camera_lens("preprocess_model", camera_model, fx, fy, cl, lens)) return rc;
+  GSB_REQUIRE(N >= 0, "preprocess_model: N < 0");
+  GSB_REQUIRE(alphas_eff != nullptr || (alphas == nullptr) == (records == nullptr),
+              "preprocess_model: alphas and records go together");
+  GSB_REQUIRE((reinterpret_cast<uintptr_t>(records) & 15) == 0, "preprocess_model: records misaligned");
+  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
+              "preprocess_model: shs.shape[1]/3 must be 1, 4, 9 or 16");
+  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && us && cinv2ds && colors &&
+                         depths && areas && (alphas_eff == nullptr || alphas)),
+              "preprocess_model: null pointer");
+  return launch_preprocess_fwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
+                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), alphas_eff,
+                               (cudaStream_t)stream, lens);
+}
+
+int gsb_preprocess_backward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                  const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                  float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                                  const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                                  float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                                  const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                                  const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
+                                  size_t ws_bytes, const gsb_camera_model *camera_model, gsb_stream_t stream) {
+  const char *who = "preprocessB_model";
+  CamLens cl;
+  const CamLens *lens;
+  if (int rc = camera_lens(who, camera_model, fx, fy, cl, lens)) return rc;
+  const bool pose = dloss_dcamera != nullptr;
+  if (int rc = check_preprocess_backward(who, pose ? GradOutputs::kAllOrNone : GradOutputs::kAll, N, sh_dim3, pws,
+                                          rots, scales, shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors,
+                                          moments, cinv2ds, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots,
+                                          dloss_dus_out, dloss_dalphas_out))
+    return rc;
+  GSB_REQUIRE(N == 0 || moments != nullptr, "preprocessB_model: the camera models take the moment rows");
+  if (pose) {
+    GSB_REQUIRE(aligned(ws, 16), "preprocessB_model: workspace misaligned");
+    GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
+                "preprocessB_model: workspace too small");
+  }
+  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
+  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
+  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
+                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                               dloss_drots, nullptr, &mi, dloss_ddepths, pose ? &po : nullptr, alphas,
+                               (cudaStream_t)stream, lens);
 }
 
 // ---- Mip-Splatting 3D smoothing filter (filter3d.cu)

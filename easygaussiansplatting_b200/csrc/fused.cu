@@ -47,14 +47,15 @@ __device__ __forceinline__ void load_small_rows(const float *__restrict__ pws, c
 // AA = antialiasing (pg::aa_scale): alphas is read, alpha_eff = rho alpha goes to alphas_eff[N]
 // and into the record's alpha word (so its culling threshold follows); every other output is the
 // non-AA kernel's.
-template <int K3, bool AA>
+// MODEL = pg::CamModel; lk = FISHEYE's k1..k4 (unread by the other models)
+template <int K3, bool AA, int MODEL>
 __global__ void __launch_bounds__(PG) k_preprocess_fwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
     const float *__restrict__ shs, const float *__restrict__ Rcw, const float *__restrict__ tcw,
     const float *__restrict__ twc, float fx, float fy, float cx, float cy, float tan_fovx, float tan_fovy,
     float *__restrict__ us, float *__restrict__ cinv2ds, float *__restrict__ colors,
     float *__restrict__ depths, int32_t *__restrict__ areas, const float *__restrict__ alphas,
-    Rec *__restrict__ recs, float *__restrict__ alphas_eff) {
+    Rec *__restrict__ recs, float *__restrict__ alphas_eff, float4 lk) {
   constexpr int KS = 3 * K3;
   constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
   __shared__ float sm[SMF];
@@ -62,7 +63,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
   const long long base = (long long)blockIdx.x * PG;
   const int nv = min(PG, (int)(N - base));
   const bool valid = tid < nv;
-  const pg::Cam cam = load_cam(Rcw, tcw, twc, fx, fy, cx, cy, tan_fovx, tan_fovy);
+  pg::Cam cam = load_cam(Rcw, tcw, twc, fx, fy, cx, cy, tan_fovx, tan_fovy);
+  if (MODEL == pg::FISHEYE) { cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w; }
   float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
   // The 10 floats of position / scale / rotation go straight from global memory to registers
   // (a warp's strided loads use every byte of the sectors they touch; L1 serves the repeats) and
@@ -74,7 +76,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
   float u[2] = {0.f, 0.f}, conic[3] = {0.f, 0.f, 0.f}, col[3] = {0.f, 0.f, 0.f}, depth = -1.f;
   int area[2] = {0, 0};
   if (valid) {
-    const float rho = pg::forward_one<K3, AA>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
+    const float rho = pg::forward_one<K3, AA, MODEL>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
     const long long i = base + tid;
     st_pair(us, i, u[0], u[1]);
     cinv2ds[3 * i] = conic[0]; cinv2ds[3 * i + 1] = conic[1]; cinv2ds[3 * i + 2] = conic[2];
@@ -115,7 +117,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
 // AA = antialiasing (only with MOM, not with PUSH): the moment rows' dL/dalpha is dL/dalpha_eff of
 // the forward's alpha_eff = rho alpha; alphas (raw, 4 B/Gaussian) is read, dL/dalpha = rho m[5]
 // is written and alpha m[5] drho feeds the geometry (and camera) gradients (pg::backward_one).
-template <int K3, bool PUSH, bool MOM, bool DEPTH, bool POSE, bool AA>
+// MODEL, lk: as for k_preprocess_fwd (ORTHO and FISHEYE only with MOM, not with PUSH).
+template <int K3, bool PUSH, bool MOM, bool DEPTH, bool POSE, bool AA, int MODEL>
 __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
     const float *__restrict__ shs, const float *__restrict__ Rcw, const float *__restrict__ tcw,
@@ -123,8 +126,9 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     const float *__restrict__ g_us, const float *__restrict__ g_cinv2ds, const float *__restrict__ g_colors,
     float *__restrict__ g_pws, float *__restrict__ g_shs, float *__restrict__ g_scales,
     float *__restrict__ g_rots, GradPush gp, MomentsIn mi, const float *__restrict__ g_depths,
-    float *__restrict__ pose_part, const float *__restrict__ alphas) {
+    float *__restrict__ pose_part, const float *__restrict__ alphas, float4 lk) {
   static_assert(!AA || (MOM && !PUSH), "antialiasing takes the moment rows and no exchange");
+  static_assert(MODEL == pg::PINHOLE || (MOM && !PUSH), "camera models take the moment rows and no exchange");
   constexpr int KS = 3 * K3;
   constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
   __shared__ float sm[SMF];
@@ -132,7 +136,8 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   const long long base = (long long)blockIdx.x * PG;
   const int nv = min(PG, (int)(N - base));
   const bool valid = tid < nv;
-  const pg::Cam cam = load_cam(Rcw, tcw, twc, fx, fy, cx, cy, tan_fovx, tan_fovy);
+  pg::Cam cam = load_cam(Rcw, tcw, twc, fx, fy, cx, cy, tan_fovx, tan_fovy);
+  if (MODEL == pg::FISHEYE) { cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w; }
   float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
   float gu[2] = {0.f, 0.f}, gci[3] = {0.f, 0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
   load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);  // see k_preprocess_fwd
@@ -172,7 +177,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     if (valid) {
       const float gz = DEPTH ? __ldg(g_depths + base + tid) : 0.f;
       float xpw[3], xq[4], xs[3], xsh[KS];  // the per-Gaussian outputs: not written by this form
-      pg::backward_one<K3, DEPTH, true, AA>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam,
+      pg::backward_one<K3, DEPTH, true, AA, MODEL>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam,
                                             galpha, al);
     }
     __shared__ float red[PG / 32][16];
@@ -201,10 +206,10 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   if (DEPTH) {
     const float gz = valid ? __ldg(g_depths + base + tid) : 0.f;
     if (valid)
-      gal = pg::backward_one<K3, true, false, AA>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), gz,
+      gal = pg::backward_one<K3, true, false, AA, MODEL>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), gz,
                                                   nullptr, galpha, al);
   } else if (valid) {
-    gal = pg::backward_one<K3, false, false, AA>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), 0.f,
+    gal = pg::backward_one<K3, false, false, AA, MODEL>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, gpw, gq, gs, ROWK(KS), 0.f,
                                                  nullptr, galpha, al);
   }
   if (AA && valid && mi.dalphas_out != nullptr) mi.dalphas_out[base + tid] = gal;
@@ -349,20 +354,30 @@ int launch_preprocess_fwd(int N, int k3, const float *pws, const float *rots, co
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
                           float *colors, float *depths, int32_t *areas, const float *alphas, Rec *recs,
-                          float *alphas_eff, cudaStream_t st) {
+                          float *alphas_eff, cudaStream_t st, const CamLens *lens) {
   if (N <= 0) return 0;
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = (N + PG - 1) / PG;
+  const int model = lens ? lens->model : pg::PINHOLE;
+  const float4 lk = lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
   ProfScope ps(K_PRE_FWD, st);
-  if (alphas_eff != nullptr) {
-    GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3, true><<<nb, PG, 0, st>>>(N, pws, rots, scales, shs, Rcw, tcw, twc, fx,
-                                                                        fy, cx, cy, tfx, tfy, us, cinv2ds, colors,
-                                                                        depths, areas, alphas, recs, alphas_eff)));
-  } else {
-    GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3, false><<<nb, PG, 0, st>>>(N, pws, rots, scales, shs, Rcw, tcw, twc, fx,
-                                                                         fy, cx, cy, tfx, tfy, us, cinv2ds, colors,
-                                                                         depths, areas, alphas, recs, nullptr)));
-  }
+  const auto launch = [&](auto aa, auto mdl) -> int {
+    constexpr bool AA = decltype(aa)::value;
+    constexpr int MODEL = decltype(mdl)::value;
+    GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3, AA, MODEL><<<nb, PG, 0, st>>>(
+                            N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, us, cinv2ds, colors,
+                            depths, areas, alphas, recs, AA ? alphas_eff : nullptr, lk)));
+    return 0;
+  };
+  const auto with_model = [&](auto aa) -> int {
+    switch (model) {
+      case pg::PINHOLE: return launch(aa, std::integral_constant<int, pg::PINHOLE>{});
+      case pg::ORTHO: return launch(aa, std::integral_constant<int, pg::ORTHO>{});
+      case pg::FISHEYE: return launch(aa, std::integral_constant<int, pg::FISHEYE>{});
+      default: return set_arg_error("preprocess: unknown camera model");
+    }
+  };
+  if (int rc = alphas_eff != nullptr ? with_model(std::true_type{}) : with_model(std::false_type{})) return rc;
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -391,35 +406,49 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st) {
+                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st,
+                          const CamLens *lens) {
   if (N <= 0 && po == nullptr) return 0;
   const float tfx = width / (2 * fx), tfy = height / (2 * fy);
   const int nb = N > 0 ? (N + PG - 1) / PG : 0;
   const GradPush p = gp ? *gp : GradPush{};
   const MomentsIn m = mi ? *mi : MomentsIn{};
   float *part = po ? po->part : nullptr;
+  const int model = lens ? lens->model : pg::PINHOLE;
+  const float4 lk = lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
   // one pass of k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA>, PUSH, MOM, DEPTH and AA set by
   // which optional inputs are given.  The exchange carries neither a depth nor a camera gradient,
   // so no PUSH form with DEPTH or POSE exists (api.cu never asks for one); AA exists only with the
-  // moment rows and without the exchange.
-  const auto pass = [&](auto pose) {
+  // moment rows and without the exchange, and so do the camera models other than PINHOLE.
+  const auto pass_model = [&](auto pose, auto mdl) {
     return with_flags(
         [&](auto push, auto mom, auto depth, auto aa) -> int {
           constexpr bool PUSH = decltype(push)::value, MOM = decltype(mom)::value, DEPTH = decltype(depth)::value,
                          POSE = decltype(pose)::value, AA = decltype(aa)::value;
+          constexpr int MODEL = decltype(mdl)::value;
           if constexpr (PUSH && (DEPTH || POSE)) {
             return set_arg_error("preprocessB: no depth or camera gradient with the exchange");
           } else if constexpr (AA && (PUSH || !MOM)) {
             return set_arg_error("preprocessB: antialiasing needs the moment rows and no exchange");
+          } else if constexpr (MODEL != pg::PINHOLE && (PUSH || !MOM)) {
+            return set_arg_error("preprocessB: camera models need the moment rows and no exchange");
           } else {
-            GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA><<<nb, PG, 0, st>>>(
+            GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA, MODEL><<<nb, PG, 0, st>>>(
                                     N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us,
                                     g_cinv2ds, g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part,
-                                    alphas)));
+                                    alphas, lk)));
             return 0;
           }
         },
         gp != nullptr, mi != nullptr, g_depths != nullptr, alphas != nullptr);
+  };
+  const auto pass = [&](auto pose) -> int {
+    switch (model) {
+      case pg::PINHOLE: return pass_model(pose, std::integral_constant<int, pg::PINHOLE>{});
+      case pg::ORTHO: return pass_model(pose, std::integral_constant<int, pg::ORTHO>{});
+      case pg::FISHEYE: return pass_model(pose, std::integral_constant<int, pg::FISHEYE>{});
+      default: return set_arg_error("preprocessB: unknown camera model");
+    }
   };
   ProfScope ps(K_PRE_BWD, st);
   // the camera gradient first; then, unless g_pws is NULL (pose only), the per-Gaussian gradients

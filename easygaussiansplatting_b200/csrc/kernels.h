@@ -43,12 +43,19 @@ int launch_inv_cov2d(int N, const float *cov2ds, float *depths, float *cinv2ds, 
                      float *J, cudaStream_t st);
 
 // ---- fused per-Gaussian path (fused.cu)
+// camera model of the fused per-Gaussian kernels (gsb_camera_model)
+struct CamLens {
+  int model;   // pg::CamModel
+  float k[4];  // FISHEYE's k1..k4
+};
 int launch_preprocess_fwd(int N, int k3, const float *pws, const float *rots, const float *scales,
                           const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                           float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
                           float *colors, float *depths, int32_t *areas, const float *alphas, Rec *recs,
-                          float *alphas_eff, cudaStream_t st);
+                          float *alphas_eff, cudaStream_t st, const CamLens *lens = nullptr);
 // alphas_eff: NULL, or antialiasing (alphas required): alphas_eff[N] = rho alpha, also in recs
+// lens: NULL or PINHOLE (the reference's projection), or ORTHO / FISHEYE with the fisheye's k1..k4
+// (pg_fused_math.h; the backward's non-pinhole forms take the moment rows and no exchange)
 // upstream gradients given as the rasterizer backward's moment rows (fused.cu, MOM variants)
 struct MomentsIn {
   const float *moments;  // [N,9]
@@ -77,7 +84,8 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
                           float fy, float cx, float cy, float width, float height, const float *g_us,
                           const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
                           float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st);
+                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st,
+                          const CamLens *lens = nullptr);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,

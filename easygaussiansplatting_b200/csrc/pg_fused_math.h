@@ -29,9 +29,15 @@
 namespace gsb {
 namespace pg {
 
+// Camera models (DESIGN 3.14).  PINHOLE is the reference's projection; ORTHO and FISHEYE
+// (Kannala-Brandt, COLMAP's OPENCV_FISHEYE) only change the mean u and the Jacobian J of the
+// EWA splat -- everything after cov2d is model-independent.
+enum CamModel : int { PINHOLE = 0, ORTHO = 1, FISHEYE = 2 };
+
 struct Cam {
   float R[9], t[3], twc[3];
   float fx, fy, cx, cy, tan_fovx, tan_fovy;
+  float k[4];  // FISHEYE: theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8)
 };
 
 constexpr float kMinDepth = 0.2f;  // kernel.cu:10: (float)z < 0.2 (double)  <=>  z < 0.2f
@@ -105,6 +111,113 @@ GSB_HD void cov2d(const float pc[3], bool keep, const float S6[6], const float R
   // the same sums without the blur, after c2 so that code which never reads them compiles as before
   o.raw[0] = o.MS[0] * o.M[0] + o.MS[1] * o.M[1] + o.MS[2] * o.M[2];
   o.raw[1] = o.MS[3] * o.M[3] + o.MS[4] * o.M[4] + o.MS[5] * o.M[5];
+}
+
+// ---- ORTHO and FISHEYE.  Lens holds the projection of pc and what its derivatives need:
+//   ORTHO   u = (fx x + cx, fy y + cy),  J = [[fx, 0, 0], [0, fy, 0]]
+//   FISHEYE r = |(x, y)|, theta = atan2(r, z), theta_d = theta P(theta^2), s = theta_d / r,
+//           u = (fx s x + cx, fy s y + cy),  g = (1/r) ds/dr,  h = -ds/dz = theta_d' / (r^2 + z^2),
+//           J = [[fx (s + x^2 g), fx x y g, -fx x h], [fy x y g, fy (s + y^2 g), -fy y h]]
+//   and for the backward's dJ/dpc: G = (1/r) dg/dr, H = (1/r) dh/dr (= -dg/dz), hz = dh/dz.
+// s, g and G cancel to nothing as t = r/z -> 0 (0/0 on the axis): below kFishSeries they come
+// from their series in t^2,  s = (1 + a1 t^2 + a2 t^4) / z, g = (2 a1 + 4 a2 t^2) / z^3,
+// G = 8 a2 / z^5  with a1 = k1 - 1/3, a2 = 1/5 - k1 + k2.  The direct forms lose ~eps/t of dJ/dpc
+// and the truncated series ~t^4 (relative), which meet near t = 0.03.
+constexpr float kFishSeries = 0.03f;
+
+struct Lens {
+  float J[6];           // du/dpc (2x3, row-major)
+  float s, g, h;        // FISHEYE
+  float G, H, hz;       // FISHEYE, backward only
+};
+
+// false when the Gaussian lies beyond the range where the fisheye's theta_d increases
+// (theta_d' <= 0): culled like z < 0.2.  A culled Gaussian (keep false) is evaluated at (0, 0, 1).
+template <int MODEL>
+GSB_HD bool lens(const float pc_in[3], bool keep, const Cam &cam, Lens &L) {
+  if constexpr (MODEL == ORTHO) {
+    L.J[0] = cam.fx; L.J[1] = 0.f; L.J[2] = 0.f;
+    L.J[3] = 0.f; L.J[4] = cam.fy; L.J[5] = 0.f;
+    return true;
+  } else {
+    static_assert(MODEL == FISHEYE, "unknown camera model");
+    const float x = keep ? pc_in[0] : 0.f, y = keep ? pc_in[1] : 0.f, z = keep ? pc_in[2] : 1.f;
+    const float *k = cam.k;
+    const float r2 = x * x + y * y, r = sqrtf(r2), q = fmaf(z, z, r2), qi = 1.0f / q, zi = 1.0f / z;
+    const float t = r * zi;
+    const float th = atan2f(r, z), th2 = th * th;
+    // theta_d / theta, theta_d' and theta_d'' / theta, polynomials in theta^2
+    const float P = fmaf(th2, fmaf(th2, fmaf(th2, fmaf(th2, k[3], k[2]), k[1]), k[0]), 1.f);
+    const float P1 = fmaf(th2, fmaf(th2, fmaf(th2, fmaf(th2, 9.f * k[3], 7.f * k[2]), 5.f * k[1]), 3.f * k[0]), 1.f);
+    const float P2 = fmaf(th2, fmaf(th2, fmaf(th2, 72.f * k[3], 42.f * k[2]), 20.f * k[1]), 6.f * k[0]);
+    float tht;  // theta / t
+    if (t < kFishSeries) {
+      const float t2 = t * t, a1 = k[0] - (1.f / 3.f), a2 = 0.2f - k[0] + k[1];
+      const float zi2 = zi * zi, zi3 = zi2 * zi;
+      L.s = zi * fmaf(t2, fmaf(t2, a2, a1), 1.f);
+      L.g = zi3 * fmaf(4.f * a2, t2, 2.f * a1);
+      L.G = zi3 * zi2 * (8.f * a2);
+      tht = fmaf(t2, -1.f / 3.f, 1.f);
+    } else {
+      tht = th / t;
+      L.s = P * th / r;
+      L.g = (P1 * z * qi - L.s) / r2;
+      const float A = r * z * qi, sn2 = r2 * qi;       // sin(theta) cos(theta), sin^2(theta)
+      const float F = P1 * A - P * th;                   // g r^3
+      const float Fp = P2 * th * A - 2.f * P1 * sn2;     // dF/dtheta
+      L.G = (A * Fp - 3.f * F) / (r2 * r2 * r);
+    }
+    L.h = P1 * qi;
+    L.H = (P2 * tht - 2.f * P1) * qi * qi;
+    L.hz = -(P2 * th * r + 2.f * z * P1) * qi * qi;
+    const float fx = cam.fx, fy = cam.fy, xyg = x * y * L.g;
+    L.J[0] = fx * fmaf(x * x, L.g, L.s); L.J[1] = fx * xyg; L.J[2] = -fx * x * L.h;
+    L.J[3] = fy * xyg; L.J[4] = fy * fmaf(y * y, L.g, L.s); L.J[5] = -fy * y * L.h;
+    return P1 > 0.f;
+  }
+}
+
+// projected mean of a kept Gaussian under ORTHO / FISHEYE (PINHOLE: project_mean)
+template <int MODEL>
+GSB_HD void lens_mean(const float pc[3], const Cam &cam, const Lens &L, float u[2]) {
+  if constexpr (MODEL == ORTHO) {
+    u[0] = fmaf(cam.fx, pc[0], cam.cx);
+    u[1] = fmaf(cam.fy, pc[1], cam.cy);
+  } else {
+    u[0] = fmaf(cam.fx * L.s, pc[0], cam.cx);
+    u[1] = fmaf(cam.fy * L.s, pc[1], cam.cy);
+  }
+}
+
+// cov2d (Cov2d's M, MS, c2, raw; not xc, yc, zi) under ORTHO / FISHEYE: M = J Rcw with J = L.J
+GSB_HD void cov2d_lens(const Lens &L, const float S6[6], const float R[9], Cov2d &o) {
+  for (int a = 0; a < 2; a++)
+    for (int c = 0; c < 3; c++)
+      o.M[3 * a + c] = fmaf(L.J[3 * a], R[c], fmaf(L.J[3 * a + 1], R[3 + c], L.J[3 * a + 2] * R[6 + c]));
+  const float S[9] = {S6[0], S6[1], S6[2], S6[1], S6[3], S6[4], S6[2], S6[4], S6[5]};
+  for (int a = 0; a < 2; a++)
+    for (int c = 0; c < 3; c++)
+      o.MS[3 * a + c] = o.M[3 * a] * S[c] + o.M[3 * a + 1] * S[3 + c] + o.M[3 * a + 2] * S[6 + c];
+  o.raw[0] = o.MS[0] * o.M[0] + o.MS[1] * o.M[1] + o.MS[2] * o.M[2];
+  o.raw[1] = o.MS[3] * o.M[3] + o.MS[4] * o.M[4] + o.MS[5] * o.M[5];
+  o.c2[0] = o.raw[0] + kBlur;
+  o.c2[1] = o.MS[0] * o.M[3] + o.MS[1] * o.M[4] + o.MS[2] * o.M[5];
+  o.c2[2] = o.raw[1] + kBlur;
+}
+
+// dL/dpc of the cov2d term under FISHEYE: sum_ab dL/dJ_ab dJ_ab/dpc (ORTHO: J is constant)
+GSB_HD void lens_dJ_dpc(const float pc[3], const Cam &cam, const Lens &L, const float dJ[6], float gpc[3]) {
+  const float x = pc[0], y = pc[1], fx = cam.fx, fy = cam.fy;
+  const float g = L.g, G = L.G, h = L.h, H = L.H, xx = x * x, yy = y * y, xy = x * y;
+  // row 0: J00 = fx (s + x^2 g), J01 = fx x y g, J02 = -fx x h
+  const float a0 = dJ[0] * fx, a1 = dJ[1] * fx, a2 = dJ[2] * fx;
+  const float b0 = dJ[3] * fy, b1 = dJ[4] * fy, b2 = dJ[5] * fy;
+  gpc[0] = a0 * x * fmaf(xx, G, 3.f * g) + a1 * y * fmaf(xx, G, g) - a2 * fmaf(xx, H, h) +
+           b0 * y * fmaf(xx, G, g) + b1 * x * fmaf(yy, G, g) - b2 * xy * H;
+  gpc[1] = a0 * y * fmaf(xx, G, g) + a1 * x * fmaf(yy, G, g) - a2 * xy * H +
+           b0 * x * fmaf(yy, G, g) + b1 * y * fmaf(yy, G, 3.f * g) - b2 * fmaf(yy, H, h);
+  gpc[2] = -a0 * fmaf(xx, H, h) - a1 * xy * H - a2 * x * L.hz -
+           b0 * xy * H - b1 * fmaf(yy, H, h) - b2 * y * L.hz;
 }
 
 // Antialiasing (2D-filter opacity compensation, Mip-Splatting; gsplat's rasterize_mode
@@ -194,23 +307,30 @@ struct Geo : Cov2d {
   float S6[6];        // cov3d upper triangle
   float di;           // 1 / det(cov2d)
   float cn[3];        // conic
-  bool keep;          // z >= 0.2 and 1/det not NaN
+  bool keep;          // z >= 0.2 and 1/det not NaN (FISHEYE: and theta_d' > 0)
+  Lens L;             // ORTHO / FISHEYE only
 };
 
+template <int MODEL = PINHOLE>
 GSB_HD void geometry(const float pw[3], const float q[4], const float s[3], const Cam &cam, Geo &g) {
   g.keep = camera_point(cam.R, cam.t, pw, g.pc);
   cov3d(q, s, g.R3, g.M3, g.S6);
-  cov2d(g.pc, g.keep, g.S6, cam.R, cam.fx, cam.fy, cam.tan_fovx, cam.tan_fovy, g);
+  if constexpr (MODEL == PINHOLE) {
+    cov2d(g.pc, g.keep, g.S6, cam.R, cam.fx, cam.fy, cam.tan_fovx, cam.tan_fovy, g);
+  } else {
+    if (!lens<MODEL>(g.pc, g.keep, cam, g.L)) g.keep = false;
+    cov2d_lens(g.L, g.S6, cam.R, g);
+  }
   if (!conic(g.c2, g.di, g.cn)) g.keep = false;
 }
 
 // forward outputs for one Gaussian.  Returns rho (aa_scale) with AA, 1 without or when culled:
 // the caller composites rho * alpha.  Every output is the same with and without AA.
-template <int K3, bool AA = false>
+template <int K3, bool AA = false, int MODEL = PINHOLE>
 GSB_HD float forward_one(const float pw[3], const float q[4], const float s[3], const float *sh /*[K3][3]*/,
                          const Cam &cam, float u[2], float cn[3], float col[3], float *depth, int area[2]) {
   Geo g;
-  geometry(pw, q, s, cam, g);
+  geometry<MODEL>(pw, q, s, cam, g);
   // colour is not gated by depth in the reference (kernel.cu:619-726)
   float Y[K3], dY[K3][3];
   float d[3], r[3] = {0.f, 0.f, 0.f};
@@ -226,7 +346,10 @@ GSB_HD float forward_one(const float pw[3], const float q[4], const float s[3], 
     *depth = -1.0f;
     return 1.f;
   }
-  project_mean(g.pc, g.zi, cam.fx, cam.fy, cam.cx, cam.cy, u);
+  if constexpr (MODEL == PINHOLE)
+    project_mean(g.pc, g.zi, cam.fx, cam.fy, cam.cx, cam.cy, u);
+  else
+    lens_mean<MODEL>(g.pc, cam, g.L, u);
   cn[0] = g.cn[0]; cn[1] = g.cn[1]; cn[2] = g.cn[2];
   radius(g.c2, area);
   *depth = g.pc[2];
@@ -254,7 +377,7 @@ GSB_HD float forward_one(const float pw[3], const float q[4], const float s[3], 
 //   dr/da = w (c c' + b^2) di^2,  dr/db = -2 w b (w + a + c) di^2,  dr/dc = w (a a' + b^2) di^2,
 // drho = dr / (2 rho), and 0 where the clamp holds (r <= kAaMinR).  galpha != 0 alone makes the
 // Gaussian's geometry gradient non-zero, so it joins the zero-gradient gate.
-template <int K3, bool DEPTH = false, bool POSE = false, bool AA = false>
+template <int K3, bool DEPTH = false, bool POSE = false, bool AA = false, int MODEL = PINHOLE>
 GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3], const float *sh,
                           const Cam &cam, const float gu[2], const float gconic[3], const float gcol[3],
                           float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f,
@@ -290,7 +413,7 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
 
   // ---- geometry branch
   Geo g;
-  geometry(pw, q, s, cam, g);
+  geometry<MODEL>(pw, q, s, cam, g);
   const bool any = (gu[0] != 0.f) || (gu[1] != 0.f) || (gconic[0] != 0.f) || (gconic[1] != 0.f) || (gconic[2] != 0.f) ||
                    (DEPTH && gdepth != 0.f) || (AA && galpha != 0.f);
   if (!g.keep || !any) return galpha;  // rho = 1 when culled; rho * 0 otherwise
@@ -348,27 +471,48 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
   for (int a2 = 0; a2 < 2; a2++)
     for (int k = 0; k < 3; k++)
       dJ[3 * a2 + k] = dM[3 * a2] * R[3 * k] + dM[3 * a2 + 1] * R[3 * k + 1] + dM[3 * a2 + 2] * R[3 * k + 2];
-  const float zi = g.zi, zi2 = zi * zi, zi3 = zi2 * zi;
   float gpc[3];
-  gpc[0] = dJ[2] * (-cam.fx * zi2);
-  gpc[1] = dJ[5] * (-cam.fy * zi2);
-  gpc[2] = dJ[0] * (-cam.fx * zi2) + dJ[2] * (2.f * cam.fx * g.xc * zi3) + dJ[4] * (-cam.fy * zi2) +
-           dJ[5] * (2.f * cam.fy * g.yc * zi3);
-  // projection u = (fx x/z + cx, fy y/z + cy)   (B.1.2, unclamped x, y)
-  gpc[0] += gu[0] * (cam.fx * zi);
-  gpc[1] += gu[1] * (cam.fy * zi);
-  gpc[2] += -(gu[0] * (g.pc[0] * cam.fx) + gu[1] * (g.pc[1] * cam.fy)) * zi2;
-  if (DEPTH) gpc[2] += gdepth;  // depth z = pc[2]
-  for (int j = 0; j < 3; j++) gpw[j] += gpc[0] * R[j] + gpc[1] * R[3 + j] + gpc[2] * R[6 + j];
-  if (POSE) {
-    // J = [[J00, 0, J02], [0, J11, J12]] exactly as cov2d() evaluated it
-    const float J00 = cam.fx * zi, J11 = cam.fy * zi;
-    const float J02 = -(cam.fx * g.xc) * zi2, J12 = -(cam.fy * g.yc) * zi2;
-    for (int k = 0; k < 3; k++) {
-      gcam[k] = fmaf(gpc[0], pw[k], J00 * dM[k]);
-      gcam[3 + k] = fmaf(gpc[1], pw[k], J11 * dM[3 + k]);
-      gcam[6 + k] = fmaf(gpc[2], pw[k], fmaf(J02, dM[k], J12 * dM[3 + k]));
-      gcam[9 + k] = gpc[k];
+  if constexpr (MODEL == PINHOLE) {
+    const float zi = g.zi, zi2 = zi * zi, zi3 = zi2 * zi;
+    gpc[0] = dJ[2] * (-cam.fx * zi2);
+    gpc[1] = dJ[5] * (-cam.fy * zi2);
+    gpc[2] = dJ[0] * (-cam.fx * zi2) + dJ[2] * (2.f * cam.fx * g.xc * zi3) + dJ[4] * (-cam.fy * zi2) +
+             dJ[5] * (2.f * cam.fy * g.yc * zi3);
+    // projection u = (fx x/z + cx, fy y/z + cy)   (B.1.2, unclamped x, y)
+    gpc[0] += gu[0] * (cam.fx * zi);
+    gpc[1] += gu[1] * (cam.fy * zi);
+    gpc[2] += -(gu[0] * (g.pc[0] * cam.fx) + gu[1] * (g.pc[1] * cam.fy)) * zi2;
+    if (DEPTH) gpc[2] += gdepth;  // depth z = pc[2]
+    for (int j = 0; j < 3; j++) gpw[j] += gpc[0] * R[j] + gpc[1] * R[3 + j] + gpc[2] * R[6 + j];
+    if (POSE) {
+      // J = [[J00, 0, J02], [0, J11, J12]] exactly as cov2d() evaluated it
+      const float J00 = cam.fx * zi, J11 = cam.fy * zi;
+      const float J02 = -(cam.fx * g.xc) * zi2, J12 = -(cam.fy * g.yc) * zi2;
+      for (int k = 0; k < 3; k++) {
+        gcam[k] = fmaf(gpc[0], pw[k], J00 * dM[k]);
+        gcam[3 + k] = fmaf(gpc[1], pw[k], J11 * dM[3 + k]);
+        gcam[6 + k] = fmaf(gpc[2], pw[k], fmaf(J02, dM[k], J12 * dM[3 + k]));
+        gcam[9 + k] = gpc[k];
+      }
+    }
+  } else {
+    // ORTHO / FISHEYE: u has the exact Jacobian J (no clamp), and the cov2d term goes through dJ/dpc
+    // (0 for ORTHO, whose J is constant)
+    const float *J = g.L.J;
+    if constexpr (MODEL == FISHEYE) {
+      lens_dJ_dpc(g.pc, cam, g.L, dJ, gpc);
+    } else {
+      gpc[0] = gpc[1] = gpc[2] = 0.f;
+    }
+    for (int k = 0; k < 3; k++) gpc[k] = fmaf(gu[0], J[k], fmaf(gu[1], J[3 + k], gpc[k]));
+    if (DEPTH) gpc[2] += gdepth;
+    for (int j = 0; j < 3; j++) gpw[j] += gpc[0] * R[j] + gpc[1] * R[3 + j] + gpc[2] * R[6 + j];
+    if (POSE) {
+      // dL/dRcw = gpc (x) pw + J^T dL/dM
+      for (int a2 = 0; a2 < 3; a2++)
+        for (int k = 0; k < 3; k++)
+          gcam[3 * a2 + k] = fmaf(gpc[a2], pw[k], fmaf(J[a2], dM[k], J[3 + a2] * dM[3 + k]));
+      for (int k = 0; k < 3; k++) gcam[9 + k] = gpc[k];
     }
   }
   // cov3d: dL/dM3 = 2 sym(g3) M3

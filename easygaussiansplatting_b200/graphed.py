@@ -26,6 +26,7 @@ after which `recapture()` (larger bounds) and a repeat of the step are due."""
 import torch
 
 from . import ops
+from .gsfunction import camera_model_kwargs
 
 
 class CapacityError(RuntimeError):
@@ -55,7 +56,8 @@ class GraphedFusedStep:
         cam, p = self.cam, self.p
         scales, alphas = self._drawn_params()
         us, ci, col, dep, ar = ops.preprocess(p["pws"], p["rots"], scales, p["shs"], cam.Rcw, cam.tcw, cam.twc,
-                                              cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height)
+                                              cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height,
+                                              **camera_model_kwargs(cam))
         out = ops.splat(cam.height, cam.width, us, ci, alphas, dep, col, ar)
         dkmax = int((dep.max().clamp_min(0) * 1000).item()) + 1
         return ops._next_capacity(out[4].numel(), dkmax, headroom=self.headroom)
@@ -65,7 +67,8 @@ class GraphedFusedStep:
         aa = bool(getattr(cam, "antialiased", False))
         scales, alphas = self._drawn_params()
         pre = ops.preprocess(p["pws"], p["rots"], scales, p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
-                             cam.cx, cam.cy, cam.width, cam.height, alphas=alphas, antialiased=aa)
+                             cam.cx, cam.cy, cam.width, cam.height, alphas=alphas, antialiased=aa,
+                             **camera_model_kwargs(cam))
         us, ci, col, dep, ar, rec = pre[:6]
         drawn = pre[6] if aa else alphas  # antialiased: the rasterizers composite alpha_eff
         _, self._keep, (image, contrib, final_tau, ranges, gsid) = ops._capacity_frame(
@@ -85,7 +88,7 @@ class GraphedFusedStep:
         gpw, gsh, gs, gq, dus, dal = ops.preprocessB(
             p["pws"], p["rots"], f["scales_f"], p["shs"], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=f["cinv2ds"], antialiased=f["aa"],
-            alphas=f["alphas_f"] if f["aa"] else None)
+            alphas=f["alphas_f"] if f["aa"] else None, **camera_model_kwargs(cam))
         if self.filter3d is not None:  # dL/ds', dL/dalpha' -> dL/ds, dL/dalpha, in place
             ops.filter3d_backward(p["scales"], p["alphas"], self.filter3d, gs, dal, inplace=True)
         self._keep_b = moments

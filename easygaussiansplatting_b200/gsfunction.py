@@ -12,14 +12,35 @@ import torch
 class Camera:
     """Fields of gsplat/gausplat_dataset.py:14-27 that the rasterizer reads.  antialiased (an
     extension, read by the fused classes, GraphedFusedStep and MultiViewStep): render with the
-    2D-filter opacity compensation, alpha_eff = rho * alpha (ops.preprocess)."""
+    2D-filter opacity compensation, alpha_eff = rho * alpha (ops.preprocess).
+    camera_model (an extension, read by the same classes): "pinhole" (the reference's projection),
+    "ortho" (u = (fx x + cx, fy y + cy)) or "fisheye" (Kannala-Brandt, COLMAP's OPENCV_FISHEYE, with
+    radial_coeffs = (k1, k2, k3, k4); None = the equidistant lens).  The seven-operator GSFunction,
+    GradExchange and the 3D filter's camera table take pinhole cameras only."""
 
-    def __init__(self, width, height, fx, fy, cx, cy, Rcw, tcw, twc=None, antialiased=False):
+    def __init__(self, width, height, fx, fy, cx, cy, Rcw, tcw, twc=None, antialiased=False, camera_model="pinhole",
+                 radial_coeffs=None):
+        from .ops import camera_model_args
         self.width, self.height = int(width), int(height)
         self.fx, self.fy, self.cx, self.cy = float(fx), float(fy), float(cx), float(cy)
         self.Rcw, self.tcw = Rcw, tcw
         self.twc = twc if twc is not None else -torch.linalg.inv(Rcw) @ tcw
         self.antialiased = bool(antialiased)
+        self.camera_model, k = camera_model_args(camera_model, radial_coeffs)
+        self.radial_coeffs = k if radial_coeffs is not None else None
+        if self.camera_model != "pinhole" and not (self.fx > 0 and self.fy > 0):
+            raise ValueError("camera_model=%r needs fx, fy > 0" % self.camera_model)
+
+
+def camera_model_kwargs(cam):
+    """ops.preprocess / preprocessB keywords of a camera; one without the fields (the reference's
+    dataset Camera) is pinhole"""
+    return dict(camera_model=getattr(cam, "camera_model", "pinhole"), radial_coeffs=getattr(cam, "radial_coeffs", None))
+
+
+def _pinhole_only(cam, what):
+    if getattr(cam, "camera_model", "pinhole") != "pinhole":
+        raise ValueError("%s takes pinhole cameras only, got camera_model=%r" % (what, cam.camera_model))
 
 
 def build_gsfunction(gsc):
@@ -44,6 +65,7 @@ class _Impl:
     def forward(gsc, ctx, pws, shs, alphas, scales, rots, us, cam):
         if getattr(cam, "antialiased", False):
             raise ValueError("GSFunction (the seven-operator surface) has no antialiased mode: use GSFunctionFused")
+        _pinhole_only(cam, "GSFunction (the seven-operator surface; use GSFunctionFused)")
         us, pcs, depths, du_dpcs = gsc.project(pws, cam.Rcw, cam.tcw, cam.fx, cam.fy, cam.cx, cam.cy, True)
         cov3ds, dcov3d_drots, dcov3d_dscales = gsc.computeCov3D(rots, scales, depths, True)
         cov2ds, dcov2d_dcov3ds, dcov2d_dpcs = gsc.computeCov2D(
@@ -151,6 +173,8 @@ def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None
     gradient slot (after cam and filter3d) is kept in ctx.abs_slot."""
     from . import ops
     ctx.abs_slot = None
+    if getattr(cam, "grad_exchange", None) is not None:
+        _pinhole_only(cam, "the gradient exchange (cam.grad_exchange)")
     if us_abs is not None:
         if getattr(cam, "grad_exchange", None) is not None:
             raise ValueError("us_abs is single-view: cam.grad_exchange must not be set")
@@ -178,7 +202,7 @@ def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None
     # the per-Gaussian records of the rasterizers come straight out of the fused forward (with z in
     # their depth word, as the RGB-D rasterizer needs)
     pre = ops.preprocess(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
-                         cam.height, alphas=alphas, antialiased=aa)
+                         cam.height, alphas=alphas, antialiased=aa, **camera_model_kwargs(cam))
     us, cinv2ds, colors, depths, areas, records = pre[:6]
     drawn = pre[6] if aa else alphas  # the opacities the rasterizers composite
     splat = ops.splat_rgbd if rgbd else ops.splat
@@ -286,7 +310,7 @@ def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, sca
     out = ops.preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
                           cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths,
                           camera_grad=need_cam, pose_only=need_cam and not need_map, antialiased=ctx.aa,
-                          alphas=alphas if ctx.aa else None)
+                          alphas=alphas if ctx.aa else None, **camera_model_kwargs(cam))
     if need_map:
         dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = out[:6]
         grads = (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus)

@@ -613,15 +613,52 @@ def splatB_features(height, width, features, contrib, final_tau, patch_range_per
 
 # ---------------------------------------------------------------------------------------
 # Extensions (not in the reference module): the fused per-Gaussian path, SURVEY 8f row N1.
+CAMERA_MODELS = ("pinhole", "ortho", "fisheye")  # GSB_CAMERA_PINHOLE, _ORTHO, _FISHEYE
+
+
+class _CameraModel(C.Structure):
+    _fields_ = [("model", C.c_int32), ("k", C.c_float * 4)]
+
+
+def camera_model_args(camera_model="pinhole", radial_coeffs=None):
+    """Checks a camera model on the host -> (name, (k1, k2, k3, k4) as floats).  camera_model is
+    "pinhole", "ortho" or "fisheye"; radial_coeffs (k1..k4 of the Kannala-Brandt lens, COLMAP's
+    OPENCV_FISHEYE; None = all 0) is accepted only with "fisheye" and must be finite."""
+    if camera_model not in CAMERA_MODELS:
+        raise ValueError("camera_model must be one of %s, got %r" % (CAMERA_MODELS, camera_model))
+    if radial_coeffs is None:
+        return camera_model, (0.0, 0.0, 0.0, 0.0)
+    if camera_model != "fisheye":
+        raise ValueError("radial_coeffs are for camera_model='fisheye' only")
+    k = tuple(float(x) for x in radial_coeffs)
+    if len(k) != 4 or not all(math.isfinite(x) for x in k):
+        raise ValueError("radial_coeffs must be four finite numbers (k1, k2, k3, k4)")
+    return camera_model, k
+
+
+def _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y):
+    """-> None for pinhole (today's entry points), else the gsb_camera_model to pass by pointer"""
+    name, k = camera_model_args(camera_model, radial_coeffs)
+    if name == "pinhole":
+        return None
+    if not (float(focal_x) > 0 and float(focal_y) > 0):
+        raise ValueError("camera_model=%r needs focal_x, focal_y > 0" % name)
+    return C.pointer(_CameraModel(CAMERA_MODELS.index(name), (C.c_float * 4)(*k)))
+
+
 def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
-               alphas=None, antialiased=False):
+               alphas=None, antialiased=False, camera_model="pinhole", radial_coeffs=None):
     """project + computeCov3D + computeCov2D + sh2Color + inverseCov2D (calc_J=False) in one
     kernel.  -> [us[N,2], cinv2ds[N,3], colors[N,3], depths[N], areas[N,2] int32], ready for
     `splat`.  With alphas[N] a sixth output: the packed per-Gaussian records [N,12] for
     `splat(..., records=...)`.
     antialiased (alphas required): a seventh output alphas_eff[N] = rho * alphas, the opacity
     scaled by how much the 0.3 px blur spread each Gaussian (gsb_preprocess_forward_aa); the records
-    carry it.  Render with alphas_eff; the other outputs are the same bits as without."""
+    carry it.  Render with alphas_eff; the other outputs are the same bits as without.
+    camera_model ("pinhole", "ortho" or "fisheye") and radial_coeffs (fisheye's k1..k4): the
+    projection (gsb_preprocess_forward_model; pinhole runs the calls above).  width/height feed
+    only pinhole's fov clamp."""
+    cm = _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y)
     (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     if antialiased and alphas is None:
         raise ValueError("antialiased=True needs alphas")
@@ -641,17 +678,22 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
         args = (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
                 float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
                 _ptr(us), _ptr(cinv), _ptr(col), _ptr(depths), _ptr(areas), _ptr(alphas), _ptr(records))
-        if antialiased:
-            alphas_eff = torch.empty((N,), **o)
+        alphas_eff = torch.empty((N,), **o) if antialiased else None
+        if cm is not None:
+            _lib.check(lib.gsb_preprocess_forward_model(*args, _ptr(alphas_eff), cm, _stream()), lib)
+        elif antialiased:
             _lib.check(lib.gsb_preprocess_forward_aa(*args, _ptr(alphas_eff), _stream()), lib)
+        else:
+            _lib.check(lib.gsb_preprocess_forward(*args, _stream()), lib)
+        if antialiased:
             return [us, cinv, col, depths, areas, records, alphas_eff]
-        _lib.check(lib.gsb_preprocess_forward(*args, _stream()), lib)
     return [us, cinv, col, depths, areas] + ([records] if records is not None else [])
 
 
 def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
                 dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False,
-                dloss_ddepths=None, camera_grad=False, pose_only=False, antialiased=False, alphas=None):
+                dloss_ddepths=None, camera_grad=False, pose_only=False, antialiased=False, alphas=None,
+                camera_model="pinhole", radial_coeffs=None):
     """Vector-Jacobian products of the five per-Gaussian stages (== the torch.bmm chain of
     gsmodel.py:72-85).  -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4]]
     With moments[N,9] (from `splatB(..., moments_only=True)`) and the forward's cinv2ds[N,3] the
@@ -671,7 +713,12 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     `preprocess(..., antialiased=True)`'s alphas_eff, so the moment rows' dL/dalpha is dL/dalphas_eff;
     dloss_dalphas = rho * dL/dalphas_eff and the geometry (and camera) gradients gain the term
     through rho (gsb_preprocess_backward_aa).  Combines with compact, dloss_ddepths, camera_grad
-    and pose_only."""
+    and pose_only.
+    camera_model, radial_coeffs: as for `preprocess` (gsb_preprocess_backward_model); a model other
+    than pinhole needs the moment rows and combines with everything above."""
+    cm = _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y)
+    if cm is not None and moments is None:
+        raise ValueError("camera_model=%r needs the moment rows" % camera_model)
     if pose_only and not camera_grad:
         raise ValueError("pose_only=True needs camera_grad=True")
     if camera_grad and compact:
@@ -727,7 +774,10 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
             gcam = torch.empty((15,), **o)
             ws_bytes = int(lib.gsb_preprocess_backward_pose_workspace_bytes(N))
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
-        if antialiased:
+        if cm is not None:
+            _lib.check(lib.gsb_preprocess_backward_model(*args, _ptr(dloss_ddepths), _ptr(alphas if antialiased else None),
+                                                         _ptr(gcam), _ptr(ws), ws_bytes, cm, _stream()), lib)
+        elif antialiased:
             _lib.check(lib.gsb_preprocess_backward_aa(*args, _ptr(dloss_ddepths), _ptr(alphas), _ptr(gcam), _ptr(ws),
                                                       ws_bytes, _stream()), lib)
         elif camera_grad:
@@ -759,6 +809,10 @@ def camera_table(cams, device=None):
     cams = list(cams)
     rows = torch.zeros((len(cams), CAMERA_ROW), dtype=torch.float64)
     for k, c in enumerate(cams):
+        if getattr(c, "camera_model", "pinhole") != "pinhole":
+            # the visibility test and the d / f sampling rate are pinhole formulas
+            raise ValueError("camera %d: the 3D filter is computed from pinhole cameras only, got camera_model=%r"
+                             % (k, c.camera_model))
         w, h = float(c.width), float(c.height)
         intr = [float(c.fx), float(c.fy), float(c.cx), float(c.cy)]
         if not (w > 0 and h > 0):

@@ -15,6 +15,8 @@ import ctypes as C
 import torch
 import torch.distributed as dist
 
+from .gsfunction import camera_model_kwargs
+
 
 def view_index(step, rank, world):
     """camera index rendered by `rank` at `step` (8 cameras/step at world=8, config 5)"""
@@ -172,6 +174,9 @@ class GradExchange:
         from .ops import _chk, _gaussian_params, _ptr, _same_device, _stream, _upstream_grads
         if getattr(cam, "antialiased", False):
             raise ValueError("GradExchange has no antialiased form (cam.antialiased): use MultiViewStep")
+        if getattr(cam, "camera_model", "pinhole") != "pinhole":
+            raise ValueError("GradExchange takes pinhole cameras only (camera_model=%r): use MultiViewStep"
+                             % cam.camera_model)
         (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, cam.Rcw, cam.tcw,
                                                                          cam.twc)
         if N != self.N or k != self.k3:
@@ -278,7 +283,8 @@ class MultiViewStep:
                 self._filtered = ops.filter3d_apply(scales, alphas, self.filter3d)
             scales, alphas = self._filtered
         pre = ops.preprocess(self.pws, self.rots, scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
-                             cam.cx, cam.cy, cam.width, cam.height, alphas=alphas, antialiased=aa)
+                             cam.cx, cam.cy, cam.width, cam.height, alphas=alphas, antialiased=aa,
+                             **camera_model_kwargs(cam))
         us, cinv2ds, colors, depths, areas, records = pre[:6]
         drawn = pre[6] if aa else alphas  # antialiased: the rasterizers composite alpha_eff
         image, contrib, final_tau, ranges, gsid = ops.splat(cam.height, cam.width, us, cinv2ds, drawn, depths,
@@ -300,7 +306,7 @@ class MultiViewStep:
         gpw, _, gs, gq, dus, dal = ops.preprocessB(
             self.pws, self.rots, scales, self.shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
             cam.width, cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, compact=True, antialiased=aa,
-            alphas=alphas if aa else None)
+            alphas=alphas if aa else None, **camera_model_kwargs(cam))
         bucket = torch.as_strided(gpw, (gpw.shape[0] * 11,), (1,), gpw.storage_offset())  # [dpws|dscales|drots|dalphas]
         self._small = bucket if self._small is None else self._small.add_(bucket)
         self._dus.append(dus)

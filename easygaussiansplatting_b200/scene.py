@@ -55,3 +55,49 @@ def ring_camera(k, n_views, radius=0.6):
     twc = np.array([radius * math.cos(a), radius * math.sin(a) * 0.5, 0.0])
     tcw = -Rcw @ twc
     return Rcw.astype(np.float32), tcw.astype(np.float32), twc.astype(np.float32)
+
+
+COLMAP_LIKE_FISHEYE_K = (0.05, -0.01, 0.002, -0.0005)  # k1..k4 of a typical OPENCV_FISHEYE calibration
+
+
+def camera_model_scene(N, width, height, camera_model="pinhole", radial_coeffs=None, sh_dim=48, seed=0):
+    """synthetic_scene with its target pixels unprojected through a camera model instead of the pinhole,
+    so that scenes of different models cover the frame alike.  pinhole: synthetic_scene itself.
+    ortho: fx = fy = W / 16 (16 world units across); pw = ((u - cx) / fx, (v - cy) / fy, z).
+    fisheye (Kannala-Brandt k1..k4 = radial_coeffs, default 0): fx = fy = W / pi, 180 degrees across the
+    width; the pixel's ray (theta_d -> theta by Newton) at distance z.  Targets beyond theta = 90 degrees (the
+    corners) land behind the camera and are culled.  Scales: the pixel sigma times the metres per pixel at
+    the Gaussian (z / fx; 1 / fx for ortho).  -> the dict of synthetic_scene plus camera_model, radial_coeffs"""
+    sc = synthetic_scene(N, width, height, sh_dim=sh_dim, seed=seed)
+    sc["camera_model"], sc["radial_coeffs"] = camera_model, radial_coeffs
+    if camera_model == "pinhole":
+        return sc
+    rng = np.random.default_rng(seed)  # the same draws as synthetic_scene
+    W, H = int(width), int(height)
+    cx, cy = W / 2.0, H / 2.0
+    z = rng.uniform(2.0, 12.0, N)
+    u = rng.uniform(-0.05 * W, 1.05 * W, N)
+    v = rng.uniform(-0.05 * H, 1.05 * H, N)
+    sig = np.exp(rng.uniform(math.log(0.5), math.log(4.0), (N, 3)))
+    if camera_model == "ortho":
+        f = W / 16.0
+        pws = np.stack([(u - cx) / f, (v - cy) / f, z], axis=1)
+        scales = sig / f
+    elif camera_model == "fisheye":
+        f = W / math.pi
+        k1, k2, k3, k4 = radial_coeffs if radial_coeffs is not None else (0.0, 0.0, 0.0, 0.0)
+        mx, my = (u - cx) / f, (v - cy) / f
+        td = np.hypot(mx, my)
+        th = td.copy()
+        for _ in range(30):
+            t2 = th * th
+            fth = th * (1 + t2 * (k1 + t2 * (k2 + t2 * (k3 + t2 * k4)))) - td
+            th -= fth / (1 + t2 * (3 * k1 + t2 * (5 * k2 + t2 * (7 * k3 + t2 * 9 * k4))))
+        phi = np.arctan2(my, mx)
+        pws = np.stack([z * np.sin(th) * np.cos(phi), z * np.sin(th) * np.sin(phi), z * np.cos(th)], axis=1)
+        scales = sig * z[:, None] / f
+    else:
+        raise ValueError("unknown camera model %r" % (camera_model,))
+    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+    sc.update(pws=f32(pws), scales=f32(scales), fx=float(f), fy=float(f))
+    return sc

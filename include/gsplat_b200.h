@@ -181,6 +181,43 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
                                const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
                                size_t ws_bytes, gsb_stream_t stream);
 
+/* Camera models (extension; gsplat's camera_model="pinhole" | "ortho" | "fisheye").  Only the
+ * projected mean u and the Jacobian J of the EWA splat change; everything after cov2d (conic,
+ * radius, records, the rasterizers) is the same.  Depth stays the camera-frame z, and every model
+ * culls z < 0.2.
+ *   PINHOLE  u = (fx x/z + cx, fy y/z + cy), J with the +-1.3 tan_fov clamp: the entry points above.
+ *   ORTHO    u = (fx x + cx, fy y + cy),  J = [[fx, 0, 0], [0, fy, 0]];  no clamp.
+ *   FISHEYE  Kannala-Brandt (COLMAP's OPENCV_FISHEYE; k = 0 is the equidistant lens):
+ *            theta = atan2(|(x, y)|, z),  theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6
+ *            + k4 theta^8),  u = (fx theta_d x / r + cx, fy theta_d y / r + cy), J its exact
+ *            Jacobian; no clamp.  A Gaussian where d theta_d / d theta <= 0 is culled like z < 0.2.
+ * k must be 0 for the models other than FISHEYE; fx, fy > 0 for ORTHO and FISHEYE.
+ * gsb_preprocess_forward_model: gsb_preprocess_forward_aa's arguments with alphas_eff nullable
+ * (NULL: no antialiasing, and then alphas and records go together as in gsb_preprocess_forward).
+ * gsb_preprocess_backward_model: gsb_preprocess_backward_aa's arguments with alphas nullable (NULL:
+ * no antialiasing) and the moment rows required.  A NULL camera_model, or PINHOLE, runs the
+ * kernels the entry points above run.  width/height feed only PINHOLE's clamp. */
+#define GSB_CAMERA_PINHOLE 0
+#define GSB_CAMERA_ORTHO 1
+#define GSB_CAMERA_FISHEYE 2
+typedef struct gsb_camera_model {
+  int32_t model; /* GSB_CAMERA_* */
+  float k[4];    /* FISHEYE: k1..k4 */
+} gsb_camera_model;
+int gsb_preprocess_forward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
+                                 float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
+                                 float *alphas_eff, const gsb_camera_model *camera_model, gsb_stream_t stream);
+int gsb_preprocess_backward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                  const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                  float fy, float cx, float cy, float width, float height, const float *dloss_dus,
+                                  const float *dloss_dcinv2ds, const float *dloss_dcolors, float *dloss_dpws,
+                                  float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
+                                  const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
+                                  const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
+                                  size_t ws_bytes, const gsb_camera_model *camera_model, gsb_stream_t stream);
+
 /* dL/dsh from per-view dL/dcolor (extension; multi-view data parallelism, SURVEY 8e).
  * colour = 0.5 + sum_l Y_l(dir) sh_l is linear in sh and never clamped (kernel.cu:735-774), so
  * dloss_dshs[n, l, c] = sum_v Y_l((pws[n] - twcs[v]) / |.|) * dloss_dcolors[v, n, c].
