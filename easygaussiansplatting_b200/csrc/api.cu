@@ -72,6 +72,9 @@ using namespace gsb;
     if (!(cond)) return set_arg_error(msg); \
   } while (0)
 
+// shs.shape[1] / 3 of SH degrees 0 to 3
+static bool sh_dim3_ok(int sh_dim3) { return sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16; }
+
 extern "C" {
 
 int gsb_abi_version(void) { return GSB_ABI_VERSION; }
@@ -108,8 +111,7 @@ int gsb_compute_cov2d(int N, const float *cov3ds, const float *pcs, const float 
 int gsb_sh2color(int N, int sh_dim3, const float *shs, const float *pws, const float *twc,
                  float *colors, float *dcolor_dshs, float *dcolor_dpws, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0, "sh2Color: N < 0");
-  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-              "sh2Color: shs.shape[1]/3 must be 1, 4, 9 or 16");
+  GSB_REQUIRE(sh_dim3_ok(sh_dim3), "sh2Color: shs.shape[1]/3 must be 1, 4, 9 or 16");
   GSB_REQUIRE(N == 0 || (shs && pws && twc && colors), "sh2Color: null pointer");
   GSB_REQUIRE((dcolor_dshs == nullptr) == (dcolor_dpws == nullptr),
               "sh2Color: Jacobian outputs must be both set or both null");
@@ -156,22 +158,62 @@ int gsb_profile_read(int id, double *ms_total, long long *timed_launches) {
   return 0;
 }
 
+static bool aligned(const void *p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+// "<who>: <err>" as the argument error
+static int arg_error(const char *who, const char *err) {
+  char msg[128];
+  snprintf(msg, sizeof(msg), "%s: %s", who, err);
+  return set_arg_error(msg);
+}
+
+// ---- camera models (DESIGN 3.14).  NULL or PINHOLE passes no CamLens: the kernels of the
+// entry points without a model.
+static int camera_lens(const char *who, const gsb_camera_model *cm, float fx, float fy, CamLens &out,
+                       const CamLens *&lens) {
+  lens = nullptr;
+  if (cm == nullptr) return 0;
+  const bool fin = std::isfinite(cm->k[0]) && std::isfinite(cm->k[1]) && std::isfinite(cm->k[2]) &&
+                   std::isfinite(cm->k[3]);
+  const bool k0 = cm->k[0] == 0.f && cm->k[1] == 0.f && cm->k[2] == 0.f && cm->k[3] == 0.f;
+  if (cm->model != GSB_CAMERA_PINHOLE && cm->model != GSB_CAMERA_ORTHO && cm->model != GSB_CAMERA_FISHEYE)
+    return arg_error(who, "unknown camera model");
+  if (!fin) return arg_error(who, "non-finite radial coefficient");
+  if (cm->model != GSB_CAMERA_FISHEYE && !k0)
+    return arg_error(who, "radial coefficients are for the fisheye model only");
+  if (cm->model != GSB_CAMERA_PINHOLE && !(fx > 0.f && fy > 0.f)) return arg_error(who, "fx and fy must be > 0");
+  if (cm->model == GSB_CAMERA_PINHOLE) return 0;
+  out.model = cm->model;
+  for (int i = 0; i < 4; i++) out.k[i] = cm->k[i];
+  lens = &out;
+  return 0;
+}
+
+// The fused forward behind its three entry points.  antialiased: alphas and alphas_eff are
+// required; otherwise alphas and records go together.
+static int preprocess_forward(const char *who, bool antialiased, const gsb_camera_model *camera_model, FusedScene sc,
+                              const FusedFwd &f, gsb_stream_t stream) {
+  CamLens cl;
+  if (int rc = camera_lens(who, camera_model, sc.fx, sc.fy, cl, sc.lens)) return rc;
+  if (sc.N < 0) return arg_error(who, "N < 0");
+  if (!antialiased && (f.alphas == nullptr) != (f.recs == nullptr))
+    return arg_error(who, "alphas and records go together");
+  if (!aligned(f.recs, 16)) return arg_error(who, "records misaligned");
+  if (!sh_dim3_ok(sc.k3)) return arg_error(who, "shs.shape[1]/3 must be 1, 4, 9 or 16");
+  if (!(sc.N == 0 || (sc.pws && sc.rots && sc.scales && sc.shs && sc.Rcw && sc.tcw && sc.twc && f.us && f.cinv2ds &&
+                      f.colors && f.depths && f.areas && (!antialiased || (f.alphas && f.alphas_eff)))))
+    return arg_error(who, "null pointer");
+  return launch_preprocess_fwd(sc, f, (cudaStream_t)stream);
+}
+
 int gsb_preprocess_forward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
                            const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
                            float fy, float cx, float cy, float width, float height, float *us,
                            float *cinv2ds, float *colors, float *depths, int32_t *areas, const float *alphas,
                            void *records, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0, "preprocess: N < 0");
-  GSB_REQUIRE((alphas == nullptr) == (records == nullptr), "preprocess: alphas and records go together");
-  GSB_REQUIRE((reinterpret_cast<uintptr_t>(records) & 15) == 0, "preprocess: records misaligned");
-  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-              "preprocess: shs.shape[1]/3 must be 1, 4, 9 or 16");
-  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && us && cinv2ds && colors &&
-                         depths && areas),
-              "preprocess: null pointer");
-  return launch_preprocess_fwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), nullptr,
-                               (cudaStream_t)stream);
+  return preprocess_forward("preprocess", false, nullptr,
+                            {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                            {us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), nullptr}, stream);
 }
 
 int gsb_preprocess_forward_aa(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -179,19 +221,22 @@ int gsb_preprocess_forward_aa(int N, int sh_dim3, const float *pws, const float 
                               float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
                               float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
                               float *alphas_eff, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0, "preprocess_aa: N < 0");
-  GSB_REQUIRE((reinterpret_cast<uintptr_t>(records) & 15) == 0, "preprocess_aa: records misaligned");
-  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-              "preprocess_aa: shs.shape[1]/3 must be 1, 4, 9 or 16");
-  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && us && cinv2ds && colors &&
-                         depths && areas && alphas && alphas_eff),
-              "preprocess_aa: null pointer");
-  return launch_preprocess_fwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), alphas_eff,
-                               (cudaStream_t)stream);
+  return preprocess_forward("preprocess_aa", true, nullptr,
+                            {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                            {us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), alphas_eff},
+                            stream);
 }
 
-static bool aligned(const void *p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+int gsb_preprocess_forward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                 float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
+                                 float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
+                                 float *alphas_eff, const gsb_camera_model *camera_model, gsb_stream_t stream) {
+  return preprocess_forward("preprocess_model", alphas_eff != nullptr, camera_model,
+                            {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                            {us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), alphas_eff},
+                            stream);
+}
 
 // Which per-Gaussian outputs an entry point of the fused backward writes: dloss_dpws, dloss_dshs,
 // dloss_dscales, dloss_drots and, with the moment rows, dloss_dus_out and dloss_dalphas_out.
@@ -205,58 +250,52 @@ enum class GradOutputs {
 // pointers, the upstream gradients (the moment rows with the forward's conics, or the plain dL/du,
 // dL/dconic and dL/dcolor) and the per-Gaussian outputs `outs` asks for.  `who` prefixes the error
 // message.  An entry point checks its own further arguments after this.
-static int check_preprocess_backward(const char *who, GradOutputs outs, int N, int sh_dim3, const float *pws,
-                                     const float *rots, const float *scales, const float *shs, const float *Rcw,
-                                     const float *tcw, const float *twc, const float *dloss_dus,
-                                     const float *dloss_dcinv2ds, const float *dloss_dcolors, const float *moments,
-                                     const float *cinv2ds, const float *dloss_dpws, const float *dloss_dshs,
-                                     const float *dloss_dscales, const float *dloss_drots,
-                                     const float *dloss_dus_out, const float *dloss_dalphas_out) {
-  const bool mom = moments != nullptr;
-  const bool all_but_shs = dloss_dpws && dloss_dscales && dloss_drots && (!mom || (dloss_dus_out && dloss_dalphas_out));
-  const bool none = !dloss_dpws && !dloss_dshs && !dloss_dscales && !dloss_drots &&
-                    (!mom || (!dloss_dus_out && !dloss_dalphas_out));
-  const char *err = nullptr;
-  if (N < 0)
-    err = "N < 0";
-  else if (!(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16))
-    err = "shs.shape[1]/3 must be 1, 4, 9 or 16";
-  else if (N == 0)
-    return 0;
-  else if (!(pws && rots && scales && shs && Rcw && tcw && twc))
-    err = "null pointer";
-  else if (!(mom ? cinv2ds != nullptr : (dloss_dus && dloss_dcinv2ds && dloss_dcolors)))
-    err = "null upstream gradient";
-  else if (outs == GradOutputs::kAll && !(all_but_shs && (mom || dloss_dshs)))
-    err = "null output";
-  else if (outs == GradOutputs::kAllOrNone && !((all_but_shs && dloss_dshs) || none))
-    err = "per-Gaussian outputs must be all set or all null";
-  else if (outs == GradOutputs::kNone && mom && !dloss_dus_out)
-    err = "null output";
-  if (err == nullptr) return 0;
-  char msg[128];
-  snprintf(msg, sizeof(msg), "%s: %s", who, err);
-  return set_arg_error(msg);
+static int check_preprocess_backward(const char *who, GradOutputs outs, const FusedScene &sc, const FusedBwd &b) {
+  const bool mom = b.mi.moments != nullptr;
+  const bool all_but_shs = b.g_pws && b.g_scales && b.g_rots && (!mom || (b.mi.dus_out && b.mi.dalphas_out));
+  const bool none = !b.g_pws && !b.g_shs && !b.g_scales && !b.g_rots && (!mom || (!b.mi.dus_out && !b.mi.dalphas_out));
+  if (sc.N < 0) return arg_error(who, "N < 0");
+  if (!sh_dim3_ok(sc.k3)) return arg_error(who, "shs.shape[1]/3 must be 1, 4, 9 or 16");
+  if (sc.N == 0) return 0;
+  if (!(sc.pws && sc.rots && sc.scales && sc.shs && sc.Rcw && sc.tcw && sc.twc)) return arg_error(who, "null pointer");
+  if (!(mom ? b.mi.cinv2ds != nullptr : (b.g_us && b.g_cinv2ds && b.g_colors)))
+    return arg_error(who, "null upstream gradient");
+  if (outs == GradOutputs::kAll && !(all_but_shs && (mom || b.g_shs))) return arg_error(who, "null output");
+  if (outs == GradOutputs::kAllOrNone && !((all_but_shs && b.g_shs) || none))
+    return arg_error(who, "per-Gaussian outputs must be all set or all null");
+  if (outs == GradOutputs::kNone && mom && !b.mi.dus_out) return arg_error(who, "null output");
+  return 0;
 }
 
-// gsb_preprocess_backward and its RGB-D form (dloss_ddepths != NULL)
-static int preprocess_backward_impl(const char *who, int N, int sh_dim3, const float *pws, const float *rots,
-                                    const float *scales, const float *shs, const float *Rcw, const float *tcw,
-                                    const float *twc, float fx, float fy, float cx, float cy, float width,
-                                    float height, const float *dloss_dus, const float *dloss_dcinv2ds,
-                                    const float *dloss_dcolors, const float *dloss_ddepths, float *dloss_dpws,
-                                    float *dloss_dshs, float *dloss_dscales, float *dloss_drots,
-                                    const float *moments, const float *cinv2ds, float *dloss_dus_out,
-                                    float *dloss_dalphas_out, gsb_stream_t stream) {
-  if (int rc = check_preprocess_backward(who, GradOutputs::kAll, N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc,
-                                          dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds, dloss_dpws,
-                                          dloss_dshs, dloss_dscales, dloss_drots, dloss_dus_out, dloss_dalphas_out))
-    return rc;
-  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
-  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, nullptr, nullptr,
-                               (cudaStream_t)stream);
+// What an entry point of the fused backward requires beyond check_preprocess_backward
+enum : unsigned { kNeedDepths = 1, kNeedCamera = 2, kNeedAlphas = 4 };
+
+// The fused backward behind its five local entry points.  needs: the kNeed* the entry point
+// requires; need_moments: NULL, or why it requires the moment rows (the refusal's text).
+// dloss_dcamera (with its workspace): NULL, or also the camera gradient; then the per-Gaussian
+// outputs may be all NULL (pose only).
+static int preprocess_backward(const char *who, unsigned needs, const char *need_moments,
+                               const gsb_camera_model *camera_model, FusedScene sc, FusedBwd b, float *dloss_dcamera,
+                               void *ws, size_t ws_bytes, gsb_stream_t stream) {
+  CamLens cl;
+  if (int rc = camera_lens(who, camera_model, sc.fx, sc.fy, cl, sc.lens)) return rc;
+  const int N = sc.N;
+  if ((needs & kNeedDepths) && N > 0 && b.g_depths == nullptr) return arg_error(who, "null dloss_ddepths");
+  const bool pose = dloss_dcamera != nullptr;
+  const GradOutputs outs = (needs & kNeedCamera) || pose ? GradOutputs::kAllOrNone : GradOutputs::kAll;
+  if (int rc = check_preprocess_backward(who, outs, sc, b)) return rc;
+  if ((needs & kNeedCamera) && !pose) return arg_error(who, "null dloss_dcamera");
+  if (need_moments && N != 0 && b.mi.moments == nullptr) return arg_error(who, need_moments);
+  if ((needs & kNeedAlphas) && N != 0 && b.alphas == nullptr) return arg_error(who, "null alphas");
+  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
+  if (pose) {
+    if (!aligned(ws, 16)) return arg_error(who, "workspace misaligned");
+    if (!(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr)))
+      return arg_error(who, "workspace too small");
+    // (N == 0 launches no per-Gaussian pass: only the camera gradient's zeros)
+    b.po = &po;
+  }
+  return launch_preprocess_bwd(sc, b, (cudaStream_t)stream);
 }
 
 int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -266,10 +305,11 @@ int gsb_preprocess_backward(int N, int sh_dim3, const float *pws, const float *r
                             float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
                             const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                             gsb_stream_t stream) {
-  return preprocess_backward_impl("preprocessB", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy,
-                                  width, height, dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, dloss_dpws,
-                                  dloss_dshs, dloss_dscales, dloss_drots, moments, cinv2ds, dloss_dus_out,
-                                  dloss_dalphas_out, stream);
+  return preprocess_backward("preprocessB", 0, nullptr, nullptr,
+                             {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                             {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                              dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}},
+                             nullptr, nullptr, 0, stream);
 }
 
 int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -279,11 +319,11 @@ int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const flo
                                  float *dloss_dshs, float *dloss_dscales, float *dloss_drots, const float *moments,
                                  const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                  const float *dloss_ddepths, gsb_stream_t stream) {
-  GSB_REQUIRE(N <= 0 || dloss_ddepths != nullptr, "preprocessB_rgbd: null dloss_ddepths");
-  return preprocess_backward_impl("preprocessB_rgbd", N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx,
-                                  cy, width, height, dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_ddepths,
-                                  dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, moments, cinv2ds, dloss_dus_out,
-                                  dloss_dalphas_out, stream);
+  return preprocess_backward("preprocessB_rgbd", kNeedDepths, nullptr, nullptr,
+                             {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                             {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                              dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}, dloss_ddepths},
+                             nullptr, nullptr, 0, stream);
 }
 
 size_t gsb_preprocess_backward_pose_workspace_bytes(int N) { return pose_workspace_bytes(N); }
@@ -296,21 +336,11 @@ int gsb_preprocess_backward_pose(int N, int sh_dim3, const float *pws, const flo
                                  const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                  const float *dloss_ddepths, float *dloss_dcamera, void *ws, size_t ws_bytes,
                                  gsb_stream_t stream) {
-  if (int rc = check_preprocess_backward("preprocessB_pose", GradOutputs::kAllOrNone, N, sh_dim3, pws, rots, scales,
-                                          shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
-                                          cinv2ds, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, dloss_dus_out,
-                                          dloss_dalphas_out))
-    return rc;
-  GSB_REQUIRE(dloss_dcamera != nullptr, "preprocessB_pose: null dloss_dcamera");
-  GSB_REQUIRE(aligned(ws, 16), "preprocessB_pose: workspace misaligned");
-  GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
-              "preprocessB_pose: workspace too small");
-  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
-  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
-  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, moments ? &mi : nullptr, dloss_ddepths, &po, nullptr,
-                               (cudaStream_t)stream);
+  return preprocess_backward("preprocessB_pose", kNeedCamera, nullptr, nullptr,
+                             {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                             {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                              dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}, dloss_ddepths},
+                             dloss_dcamera, ws, ws_bytes, stream);
 }
 
 int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -321,79 +351,11 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
                                const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
                                size_t ws_bytes, gsb_stream_t stream) {
-  const char *who = "preprocessB_aa";
-  const bool pose = dloss_dcamera != nullptr;
-  if (int rc = check_preprocess_backward(who, pose ? GradOutputs::kAllOrNone : GradOutputs::kAll, N, sh_dim3, pws,
-                                          rots, scales, shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors,
-                                          moments, cinv2ds, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots,
-                                          dloss_dus_out, dloss_dalphas_out))
-    return rc;
-  GSB_REQUIRE(N == 0 || moments != nullptr, "preprocessB_aa: antialiasing takes the moment rows");
-  GSB_REQUIRE(N == 0 || alphas != nullptr, "preprocessB_aa: null alphas");
-  if (pose) {
-    GSB_REQUIRE(aligned(ws, 16), "preprocessB_aa: workspace misaligned");
-    GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
-                "preprocessB_aa: workspace too small");
-  }
-  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
-  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
-  // (N == 0 launches no per-Gaussian pass: only the camera gradient's zeros, with dloss_dcamera)
-  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, &mi, dloss_ddepths, pose ? &po : nullptr, alphas,
-                               (cudaStream_t)stream);
-}
-
-// ---- camera models (DESIGN 3.14).  NULL or PINHOLE passes no CamLens: the kernels of the
-// entry points above.
-static int camera_lens(const char *who, const gsb_camera_model *cm, float fx, float fy, CamLens &out,
-                       const CamLens *&lens) {
-  lens = nullptr;
-  if (cm == nullptr) return 0;
-  const char *err = nullptr;
-  const bool fin = std::isfinite(cm->k[0]) && std::isfinite(cm->k[1]) && std::isfinite(cm->k[2]) &&
-                   std::isfinite(cm->k[3]);
-  const bool k0 = cm->k[0] == 0.f && cm->k[1] == 0.f && cm->k[2] == 0.f && cm->k[3] == 0.f;
-  if (cm->model != GSB_CAMERA_PINHOLE && cm->model != GSB_CAMERA_ORTHO && cm->model != GSB_CAMERA_FISHEYE)
-    err = "unknown camera model";
-  else if (!fin)
-    err = "non-finite radial coefficient";
-  else if (cm->model != GSB_CAMERA_FISHEYE && !k0)
-    err = "radial coefficients are for the fisheye model only";
-  else if (cm->model != GSB_CAMERA_PINHOLE && !(fx > 0.f && fy > 0.f))
-    err = "fx and fy must be > 0";
-  if (err != nullptr) {
-    char msg[128];
-    snprintf(msg, sizeof(msg), "%s: %s", who, err);
-    return set_arg_error(msg);
-  }
-  if (cm->model == GSB_CAMERA_PINHOLE) return 0;
-  out.model = cm->model;
-  for (int i = 0; i < 4; i++) out.k[i] = cm->k[i];
-  lens = &out;
-  return 0;
-}
-
-int gsb_preprocess_forward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
-                                 const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                                 float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
-                                 float *colors, float *depths, int32_t *areas, const float *alphas, void *records,
-                                 float *alphas_eff, const gsb_camera_model *camera_model, gsb_stream_t stream) {
-  CamLens cl;
-  const CamLens *lens;
-  if (int rc = camera_lens("preprocess_model", camera_model, fx, fy, cl, lens)) return rc;
-  GSB_REQUIRE(N >= 0, "preprocess_model: N < 0");
-  GSB_REQUIRE(alphas_eff != nullptr || (alphas == nullptr) == (records == nullptr),
-              "preprocess_model: alphas and records go together");
-  GSB_REQUIRE((reinterpret_cast<uintptr_t>(records) & 15) == 0, "preprocess_model: records misaligned");
-  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-              "preprocess_model: shs.shape[1]/3 must be 1, 4, 9 or 16");
-  GSB_REQUIRE(N == 0 || (pws && rots && scales && shs && Rcw && tcw && twc && us && cinv2ds && colors &&
-                         depths && areas && (alphas_eff == nullptr || alphas)),
-              "preprocess_model: null pointer");
-  return launch_preprocess_fwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records), alphas_eff,
-                               (cudaStream_t)stream, lens);
+  return preprocess_backward("preprocessB_aa", kNeedAlphas, "antialiasing takes the moment rows", nullptr,
+                             {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                             {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                              dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}, dloss_ddepths, alphas},
+                             dloss_dcamera, ws, ws_bytes, stream);
 }
 
 int gsb_preprocess_backward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -404,28 +366,11 @@ int gsb_preprocess_backward_model(int N, int sh_dim3, const float *pws, const fl
                                   const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                   const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
                                   size_t ws_bytes, const gsb_camera_model *camera_model, gsb_stream_t stream) {
-  const char *who = "preprocessB_model";
-  CamLens cl;
-  const CamLens *lens;
-  if (int rc = camera_lens(who, camera_model, fx, fy, cl, lens)) return rc;
-  const bool pose = dloss_dcamera != nullptr;
-  if (int rc = check_preprocess_backward(who, pose ? GradOutputs::kAllOrNone : GradOutputs::kAll, N, sh_dim3, pws,
-                                          rots, scales, shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors,
-                                          moments, cinv2ds, dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots,
-                                          dloss_dus_out, dloss_dalphas_out))
-    return rc;
-  GSB_REQUIRE(N == 0 || moments != nullptr, "preprocessB_model: the camera models take the moment rows");
-  if (pose) {
-    GSB_REQUIRE(aligned(ws, 16), "preprocessB_model: workspace misaligned");
-    GSB_REQUIRE(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr),
-                "preprocessB_model: workspace too small");
-  }
-  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, dloss_dalphas_out};
-  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
-  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
-                               dloss_drots, nullptr, &mi, dloss_ddepths, pose ? &po : nullptr, alphas,
-                               (cudaStream_t)stream, lens);
+  return preprocess_backward("preprocessB_model", 0, "the camera models take the moment rows", camera_model,
+                             {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                             {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                              dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}, dloss_ddepths, alphas},
+                             dloss_dcamera, ws, ws_bytes, stream);
 }
 
 // ---- Mip-Splatting 3D smoothing filter (filter3d.cu)
@@ -469,8 +414,7 @@ int gsb_filter3d_backward(int N, const float *scales, const float *alphas, const
 int gsb_sh_grad_expand(int N, int sh_dim3, int V, const float *pws, const float *twcs, const float *dloss_dcolors,
                        float *dloss_dshs, gsb_stream_t stream) {
   GSB_REQUIRE(N >= 0 && V >= 1, "sh_grad_expand: bad N / V");
-  GSB_REQUIRE(sh_dim3 == 1 || sh_dim3 == 4 || sh_dim3 == 9 || sh_dim3 == 16,
-              "sh_grad_expand: sh_dim3 must be 1, 4, 9 or 16");
+  GSB_REQUIRE(sh_dim3_ok(sh_dim3), "sh_grad_expand: sh_dim3 must be 1, 4, 9 or 16");
   GSB_REQUIRE(N == 0 || (pws && twcs && dloss_dcolors && dloss_dshs), "sh_grad_expand: null pointer");
   return launch_sh_expand(N, sh_dim3, V, pws, twcs, dloss_dcolors, dloss_dshs, (cudaStream_t)stream);
 }
@@ -1144,10 +1088,10 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
                                  const float *dloss_dalphas, const float *moments, const float *cinv2ds,
                                  float *dloss_dus_out, int world, int rank, void *const *regions_host,
                                  uint32_t epoch, gsb_stream_t stream) {
-  if (int rc = check_preprocess_backward("preprocess_backward_push", GradOutputs::kNone, N, sh_dim3, pws, rots, scales,
-                                          shs, Rcw, tcw, twc, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
-                                          cinv2ds, nullptr, nullptr, nullptr, nullptr, dloss_dus_out, nullptr))
-    return rc;
+  const FusedScene sc{N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height};
+  FusedBwd b{dloss_dus, dloss_dcinv2ds, dloss_dcolors};
+  b.mi = {moments, cinv2ds, dloss_dus_out, nullptr};
+  if (int rc = check_preprocess_backward("preprocess_backward_push", GradOutputs::kNone, sc, b)) return rc;
   GSB_REQUIRE(N == 0 || moments || dloss_dalphas, "preprocess_backward_push: null upstream gradient");
   GSB_REQUIRE(world >= 1 && world <= kMaxWorld && rank >= 0 && rank < world && regions_host && epoch != 0,
               "preprocess_backward_push: bad world / rank / regions / epoch");
@@ -1168,10 +1112,8 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
   gp.world = world;
   gp.rank = rank;
   gp.epoch = epoch;
-  const MomentsIn mi{moments, cinv2ds, dloss_dus_out, nullptr};
-  return launch_preprocess_bwd(N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height,
-                               dloss_dus, dloss_dcinv2ds, dloss_dcolors, nullptr, nullptr, nullptr, nullptr, &gp,
-                               moments ? &mi : nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+  b.gp = &gp;
+  return launch_preprocess_bwd(sc, b, (cudaStream_t)stream);
 }
 
 int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *const *regions_host, uint32_t epoch,

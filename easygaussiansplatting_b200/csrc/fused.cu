@@ -350,34 +350,51 @@ __global__ void __launch_bounds__(PG) k_sh_expand(int N, int V, const float *__r
     default: return set_arg_error("sh_dim3 must be 1, 4, 9 or 16");         \
   }
 
-int launch_preprocess_fwd(int N, int k3, const float *pws, const float *rots, const float *scales,
-                          const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                          float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
-                          float *colors, float *depths, int32_t *areas, const float *alphas, Rec *recs,
-                          float *alphas_eff, cudaStream_t st, const CamLens *lens) {
+// f(std::bool_constant<b>...) for the runtime flags b...: each flag becomes a compile-time constant
+template <class F>
+static int with_flags(F &&f) { return f(); }
+template <class F, class... B>
+static int with_flags(F &&f, bool b, B... rest) {
+  const auto bind = [&](auto c) { return with_flags([&](auto... cs) { return f(c, cs...); }, rest...); };
+  return b ? bind(std::true_type{}) : bind(std::false_type{});
+}
+// f(std::integral_constant<int, pg::CamModel>) for the camera model of lens (NULL: PINHOLE).  The
+// deduced return type has the compiler instantiate f, and its kernels, where this is called: the
+// forward's kernels stay ahead of k_sh_expand in the cubin.
+template <class F>
+static auto with_model(const CamLens *lens, const char *unknown, F &&f) {
+  switch (lens ? lens->model : pg::PINHOLE) {
+    case pg::PINHOLE: return f(std::integral_constant<int, pg::PINHOLE>{});
+    case pg::ORTHO: return f(std::integral_constant<int, pg::ORTHO>{});
+    case pg::FISHEYE: return f(std::integral_constant<int, pg::FISHEYE>{});
+    default: return set_arg_error(unknown);
+  }
+}
+// the kernels' lk
+static float4 lens_k(const CamLens *lens) {
+  return lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+int launch_preprocess_fwd(const FusedScene &sc, const FusedFwd &f, cudaStream_t st) {
+  const int N = sc.N;
   if (N <= 0) return 0;
-  const float tfx = width / (2 * fx), tfy = height / (2 * fy);
+  const float tfx = sc.width / (2 * sc.fx), tfy = sc.height / (2 * sc.fy);
   const int nb = (N + PG - 1) / PG;
-  const int model = lens ? lens->model : pg::PINHOLE;
-  const float4 lk = lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4 lk = lens_k(sc.lens);
   ProfScope ps(K_PRE_FWD, st);
-  const auto launch = [&](auto aa, auto mdl) -> int {
-    constexpr bool AA = decltype(aa)::value;
-    constexpr int MODEL = decltype(mdl)::value;
-    GSB_DISPATCH_K3(k3, (k_preprocess_fwd<K3, AA, MODEL><<<nb, PG, 0, st>>>(
-                            N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, us, cinv2ds, colors,
-                            depths, areas, alphas, recs, AA ? alphas_eff : nullptr, lk)));
-    return 0;
+  const auto launch = [&](auto aa) {
+    return with_model(sc.lens, "preprocess: unknown camera model", [&](auto mdl) -> int {
+      constexpr bool AA = decltype(aa)::value;
+      constexpr int MODEL = decltype(mdl)::value;
+      GSB_DISPATCH_K3(sc.k3, (k_preprocess_fwd<K3, AA, MODEL><<<nb, PG, 0, st>>>(
+                                 N, sc.pws, sc.rots, sc.scales, sc.shs, sc.Rcw, sc.tcw, sc.twc, sc.fx, sc.fy, sc.cx,
+                                 sc.cy, tfx, tfy, f.us, f.cinv2ds, f.colors, f.depths, f.areas, f.alphas, f.recs,
+                                 AA ? f.alphas_eff : nullptr, lk)));
+      return 0;
+    });
   };
-  const auto with_model = [&](auto aa) -> int {
-    switch (model) {
-      case pg::PINHOLE: return launch(aa, std::integral_constant<int, pg::PINHOLE>{});
-      case pg::ORTHO: return launch(aa, std::integral_constant<int, pg::ORTHO>{});
-      case pg::FISHEYE: return launch(aa, std::integral_constant<int, pg::FISHEYE>{});
-      default: return set_arg_error("preprocess: unknown camera model");
-    }
-  };
-  if (int rc = alphas_eff != nullptr ? with_model(std::true_type{}) : with_model(std::false_type{})) return rc;
+  const int rc = f.alphas_eff != nullptr ? launch(std::true_type{}) : launch(std::false_type{});
+  if (rc) return rc;
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -392,63 +409,44 @@ int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, 
   return 0;
 }
 
-// f(std::bool_constant<b>...) for the runtime flags b...: each flag becomes a compile-time constant
-template <class F>
-static int with_flags(F &&f) { return f(); }
-template <class F, class... B>
-static int with_flags(F &&f, bool b, B... rest) {
-  const auto bind = [&](auto c) { return with_flags([&](auto... cs) { return f(c, cs...); }, rest...); };
-  return b ? bind(std::true_type{}) : bind(std::false_type{});
-}
-
-int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
-                          const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                          float fy, float cx, float cy, float width, float height, const float *g_us,
-                          const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
-                          float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st,
-                          const CamLens *lens) {
+int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t st) {
+  const int N = sc.N;
+  const PoseOut *po = b.po;
   if (N <= 0 && po == nullptr) return 0;
-  const float tfx = width / (2 * fx), tfy = height / (2 * fy);
+  const float tfx = sc.width / (2 * sc.fx), tfy = sc.height / (2 * sc.fy);
   const int nb = N > 0 ? (N + PG - 1) / PG : 0;
-  const GradPush p = gp ? *gp : GradPush{};
-  const MomentsIn m = mi ? *mi : MomentsIn{};
+  const bool moments = b.mi.moments != nullptr;
+  const GradPush p = b.gp ? *b.gp : GradPush{};
+  const MomentsIn m = moments ? b.mi : MomentsIn{};
   float *part = po ? po->part : nullptr;
-  const int model = lens ? lens->model : pg::PINHOLE;
-  const float4 lk = lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
-  // one pass of k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA>, PUSH, MOM, DEPTH and AA set by
-  // which optional inputs are given.  The exchange carries neither a depth nor a camera gradient,
+  const float4 lk = lens_k(sc.lens);
+  // one pass of k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA, MODEL>, PUSH, MOM, DEPTH and AA set
+  // by which optional inputs are given.  The exchange carries neither a depth nor a camera gradient,
   // so no PUSH form with DEPTH or POSE exists (api.cu never asks for one); AA exists only with the
   // moment rows and without the exchange, and so do the camera models other than PINHOLE.
-  const auto pass_model = [&](auto pose, auto mdl) {
-    return with_flags(
-        [&](auto push, auto mom, auto depth, auto aa) -> int {
-          constexpr bool PUSH = decltype(push)::value, MOM = decltype(mom)::value, DEPTH = decltype(depth)::value,
-                         POSE = decltype(pose)::value, AA = decltype(aa)::value;
-          constexpr int MODEL = decltype(mdl)::value;
-          if constexpr (PUSH && (DEPTH || POSE)) {
-            return set_arg_error("preprocessB: no depth or camera gradient with the exchange");
-          } else if constexpr (AA && (PUSH || !MOM)) {
-            return set_arg_error("preprocessB: antialiasing needs the moment rows and no exchange");
-          } else if constexpr (MODEL != pg::PINHOLE && (PUSH || !MOM)) {
-            return set_arg_error("preprocessB: camera models need the moment rows and no exchange");
-          } else {
-            GSB_DISPATCH_K3(k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA, MODEL><<<nb, PG, 0, st>>>(
-                                    N, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, tfx, tfy, g_us,
-                                    g_cinv2ds, g_colors, g_pws, g_shs, g_scales, g_rots, p, m, g_depths, part,
-                                    alphas, lk)));
-            return 0;
-          }
-        },
-        gp != nullptr, mi != nullptr, g_depths != nullptr, alphas != nullptr);
-  };
   const auto pass = [&](auto pose) -> int {
-    switch (model) {
-      case pg::PINHOLE: return pass_model(pose, std::integral_constant<int, pg::PINHOLE>{});
-      case pg::ORTHO: return pass_model(pose, std::integral_constant<int, pg::ORTHO>{});
-      case pg::FISHEYE: return pass_model(pose, std::integral_constant<int, pg::FISHEYE>{});
-      default: return set_arg_error("preprocessB: unknown camera model");
-    }
+    return with_model(sc.lens, "preprocessB: unknown camera model", [&](auto mdl) {
+      return with_flags(
+          [&](auto push, auto mom, auto depth, auto aa) -> int {
+            constexpr bool PUSH = decltype(push)::value, MOM = decltype(mom)::value, DEPTH = decltype(depth)::value,
+                           POSE = decltype(pose)::value, AA = decltype(aa)::value;
+            constexpr int MODEL = decltype(mdl)::value;
+            if constexpr (PUSH && (DEPTH || POSE)) {
+              return set_arg_error("preprocessB: no depth or camera gradient with the exchange");
+            } else if constexpr (AA && (PUSH || !MOM)) {
+              return set_arg_error("preprocessB: antialiasing needs the moment rows and no exchange");
+            } else if constexpr (MODEL != pg::PINHOLE && (PUSH || !MOM)) {
+              return set_arg_error("preprocessB: camera models need the moment rows and no exchange");
+            } else {
+              GSB_DISPATCH_K3(sc.k3, (k_preprocess_bwd<K3, PUSH, MOM, DEPTH, POSE, AA, MODEL><<<nb, PG, 0, st>>>(
+                                         N, sc.pws, sc.rots, sc.scales, sc.shs, sc.Rcw, sc.tcw, sc.twc, sc.fx, sc.fy,
+                                         sc.cx, sc.cy, tfx, tfy, b.g_us, b.g_cinv2ds, b.g_colors, b.g_pws, b.g_shs,
+                                         b.g_scales, b.g_rots, p, m, b.g_depths, part, b.alphas, lk)));
+              return 0;
+            }
+          },
+          b.gp != nullptr, moments, b.g_depths != nullptr, b.alphas != nullptr);
+    });
   };
   ProfScope ps(K_PRE_BWD, st);
   // the camera gradient first; then, unless g_pws is NULL (pose only), the per-Gaussian gradients
@@ -458,7 +456,7 @@ int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, co
       if (int rc = pass(std::true_type{})) return rc;
     k_pose_reduce<<<1, PR, 0, st>>>(nb, part, po->gcam);
   }
-  if (nb > 0 && (po == nullptr || g_pws != nullptr))
+  if (nb > 0 && (po == nullptr || b.g_pws != nullptr))
     if (int rc = pass(std::false_type{})) return rc;
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;

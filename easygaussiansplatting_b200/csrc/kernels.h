@@ -48,14 +48,26 @@ struct CamLens {
   int model;   // pg::CamModel
   float k[4];  // FISHEYE's k1..k4
 };
-int launch_preprocess_fwd(int N, int k3, const float *pws, const float *rots, const float *scales,
-                          const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                          float fy, float cx, float cy, float width, float height, float *us, float *cinv2ds,
-                          float *colors, float *depths, int32_t *areas, const float *alphas, Rec *recs,
-                          float *alphas_eff, cudaStream_t st, const CamLens *lens = nullptr);
-// alphas_eff: NULL, or antialiasing (alphas required): alphas_eff[N] = rho alpha, also in recs
-// lens: NULL or PINHOLE (the reference's projection), or ORTHO / FISHEYE with the fisheye's k1..k4
-// (pg_fused_math.h; the backward's non-pinhole forms take the moment rows and no exchange)
+// the Gaussians and the view: what every fused call is about
+struct FusedScene {
+  int N, k3;  // k3 = shs.shape[1] / 3
+  const float *pws, *rots, *scales, *shs, *Rcw, *tcw, *twc;
+  float fx, fy, cx, cy, width, height;
+  // NULL or PINHOLE (the reference's projection), or ORTHO / FISHEYE with the fisheye's k1..k4
+  // (pg_fused_math.h; the backward's non-pinhole forms take the moment rows and no exchange)
+  const CamLens *lens;
+};
+// the forward's outputs and the opacities it may read.  alphas with recs: also the rasterizers'
+// records.  alphas_eff: NULL, or antialiasing (alphas required): alphas_eff[N] = rho alpha, also in
+// recs.  (The fields of FusedFwd and FusedBwd follow the entry points' argument order.)
+struct FusedFwd {
+  float *us, *cinv2ds, *colors, *depths;
+  int32_t *areas;
+  const float *alphas;
+  Rec *recs;
+  float *alphas_eff;
+};
+int launch_preprocess_fwd(const FusedScene &sc, const FusedFwd &f, cudaStream_t st);
 // upstream gradients given as the rasterizer backward's moment rows (fused.cu, MOM variants)
 struct MomentsIn {
   const float *moments;  // [N,9]
@@ -71,21 +83,24 @@ struct PoseOut {
   float *part;
 };
 constexpr size_t pose_workspace_bytes(int N) { return N > 0 ? (size_t)((N + 127) / 128) * 16 * sizeof(float) : 0; }
-// gp == nullptr: the gradients go to g_pws, g_shs, g_scales, g_rots; otherwise into the exchange
-// staging slots gp describes (the g_* outputs are unused).  mi == nullptr: the upstream gradients
-// are g_us, g_cinv2ds, g_colors; otherwise the moment rows of *mi.  g_depths: NULL, or dL/dz[N]
-// of the RGB-D rasterizer (not with gp).  po: NULL, or also the camera gradient (not with gp; a
-// pass of its own); then g_pws == NULL (with g_shs, g_scales, g_rots and mi's outputs NULL) writes
-// only that.  alphas: NULL, or antialiasing (the raw opacities; only with mi, not with gp): the
-// moment rows' dL/dalpha is dL/dalpha_eff.  The arguments are checked by the entry points (api.cu
-// check_preprocess_backward).
-int launch_preprocess_bwd(int N, int k3, const float *pws, const float *rots, const float *scales,
-                          const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
-                          float fy, float cx, float cy, float width, float height, const float *g_us,
-                          const float *g_cinv2ds, const float *g_colors, float *g_pws, float *g_shs,
-                          float *g_scales, float *g_rots, const GradPush *gp, const MomentsIn *mi,
-                          const float *g_depths, const PoseOut *po, const float *alphas, cudaStream_t st,
-                          const CamLens *lens = nullptr);
+// The backward's gradients in and out.  gp == nullptr: the gradients go to g_pws, g_shs, g_scales,
+// g_rots; otherwise into the exchange staging slots gp describes (the g_* outputs are unused).
+// mi.moments == nullptr: the upstream gradients are g_us, g_cinv2ds, g_colors; otherwise the moment
+// rows of mi.  g_depths: NULL, or dL/dz[N] of the RGB-D rasterizer (not with gp).  po: NULL, or also
+// the camera gradient (not with gp; a pass of its own); then g_pws == NULL (with g_shs, g_scales,
+// g_rots and mi's outputs NULL) writes only that.  alphas: NULL, or antialiasing (the raw
+// opacities; only with mi, not with gp): the moment rows' dL/dalpha is dL/dalpha_eff.  The fields
+// are checked by the entry points (api.cu check_preprocess_backward).
+struct FusedBwd {
+  const float *g_us, *g_cinv2ds, *g_colors;
+  float *g_pws, *g_shs, *g_scales, *g_rots;
+  MomentsIn mi;
+  const float *g_depths;
+  const float *alphas;
+  const PoseOut *po;
+  const GradPush *gp;
+};
+int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,

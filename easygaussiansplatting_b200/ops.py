@@ -75,6 +75,23 @@ def _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc):
     return (pws, rots, scales, shs, Rcw, tcw, twc), N, k
 
 
+def _scene_args(params, N, k, focal_x, focal_y, center_x, center_y, width, height):
+    """The 15 leading arguments of every gsb_preprocess_* entry point, from `_gaussian_params`'
+    result (the caller keeps the tensors alive over the call) and the intrinsics"""
+    pws, rots, scales, shs, Rcw, tcw, twc = params
+    return (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
+            float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height))
+
+
+def _per_gaussian(t, name, N, ref):
+    """t: a float32 CUDA tensor with N elements on the device of `ref` -> t contiguous"""
+    t = _chk(t, name)
+    _same_device(ref, t)
+    if t.numel() != N:
+        raise ValueError("%s must have N elements" % name)
+    return t
+
+
 def _upstream_grads(N, ref, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments, cinv2ds):
     """Checks the upstream gradients the fused backward reads, float32 CUDA tensors on the device
     of `ref`: moments[N,9] with the forward's cinv2ds[N,3] or, when moments is None, dloss_dus,
@@ -659,7 +676,8 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
     projection (gsb_preprocess_forward_model; pinhole runs the calls above).  width/height feed
     only pinhole's fov clamp."""
     cm = _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y)
-    (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    params, N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    pws = params[0]
     if antialiased and alphas is None:
         raise ValueError("antialiased=True needs alphas")
     o = dict(dtype=torch.float32, device=pws.device)
@@ -667,17 +685,12 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
     depths = torch.empty((N,), **o); areas = torch.empty((N, 2), dtype=torch.int32, device=pws.device)
     records = None
     if alphas is not None:
-        alphas = _chk(alphas, "alphas")
-        if antialiased:
-            _same_device(pws, alphas)
-        if alphas.numel() != N:
-            raise ValueError("alphas must have N elements")
+        alphas = _per_gaussian(alphas, "alphas", N, pws)
         records = torch.empty((N, 12), **o)
     lib = _L()
     with torch.cuda.device(pws.device):
-        args = (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
-                float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
-                _ptr(us), _ptr(cinv), _ptr(col), _ptr(depths), _ptr(areas), _ptr(alphas), _ptr(records))
+        args = _scene_args(params, N, k, focal_x, focal_y, center_x, center_y, width, height) + (
+            _ptr(us), _ptr(cinv), _ptr(col), _ptr(depths), _ptr(areas), _ptr(alphas), _ptr(records))
         alphas_eff = torch.empty((N,), **o) if antialiased else None
         if cm is not None:
             _lib.check(lib.gsb_preprocess_forward_model(*args, _ptr(alphas_eff), cm, _stream()), lib)
@@ -725,19 +738,14 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
         raise ValueError("camera_grad does not combine with compact")
     if antialiased and (moments is None or alphas is None):
         raise ValueError("antialiased=True needs the moment rows and alphas")
-    (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    params, N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    pws = params[0]
     gu, gc, gcol, moments, cinv2ds = _upstream_grads(N, pws, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
                                                      cinv2ds)
     if antialiased:
-        alphas = _chk(alphas, "alphas")
-        _same_device(pws, alphas)
-        if alphas.numel() != N:
-            raise ValueError("alphas must have N elements")
+        alphas = _per_gaussian(alphas, "alphas", N, pws)
     if dloss_ddepths is not None:
-        dloss_ddepths = _chk(dloss_ddepths, "dloss_ddepths")
-        _same_device(pws, dloss_ddepths)
-        if dloss_ddepths.numel() != N:
-            raise ValueError("dloss_ddepths must have N elements")
+        dloss_ddepths = _per_gaussian(dloss_ddepths, "dloss_ddepths", N, pws)
     o = dict(dtype=torch.float32, device=pws.device)
     # one flat bucket [dshs | drots | dpws | dscales]: a multi-GPU caller can all-reduce the four
     # gradients in place with a single collective (parallel.allreduce_grads); every view starts
@@ -764,10 +772,9 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     dus = torch.empty((N, 2), **o) if moments is not None and not pose_only else None
     lib = _L()
     with torch.cuda.device(pws.device):
-        args = (N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
-                float(focal_x), float(focal_y), float(center_x), float(center_y), float(width), float(height),
-                _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(moments), _ptr(cinv2ds),
-                _ptr(dus), _ptr(dal))
+        args = _scene_args(params, N, k, focal_x, focal_y, center_x, center_y, width, height) + (
+            _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(moments), _ptr(cinv2ds),
+            _ptr(dus), _ptr(dal))
         gcam = ws = None
         ws_bytes = 0
         if camera_grad:

@@ -171,14 +171,14 @@ class GradExchange:
         `splatB(..., moments_only=True)`) + the forward's cinv2ds -- then this view's own
         dloss_dus[N,2] is returned (it is not part of the exchange)."""
         from . import _lib
-        from .ops import _chk, _gaussian_params, _ptr, _same_device, _stream, _upstream_grads
+        from .ops import _gaussian_params, _per_gaussian, _ptr, _scene_args, _stream, _upstream_grads
         if getattr(cam, "antialiased", False):
             raise ValueError("GradExchange has no antialiased form (cam.antialiased): use MultiViewStep")
         if getattr(cam, "camera_model", "pinhole") != "pinhole":
             raise ValueError("GradExchange takes pinhole cameras only (camera_model=%r): use MultiViewStep"
                              % cam.camera_model)
-        (pws, rots, scales, shs, Rcw, tcw, twc), N, k = _gaussian_params(pws, rots, scales, shs, cam.Rcw, cam.tcw,
-                                                                         cam.twc)
+        params, N, k = _gaussian_params(pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc)
+        pws = params[0]
         if N != self.N or k != self.k3:
             raise ValueError("GradExchange was built for N=%d, sh_dim3=%d" % (self.N, self.k3))
         gu, gc, gcol, moments, cinv2ds = _upstream_grads(N, pws, dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments,
@@ -187,17 +187,13 @@ class GradExchange:
         if moments is not None:
             dus = torch.empty((N, 2), dtype=torch.float32, device=pws.device)
         else:  # dL/dalpha goes into the exchange as it is
-            ga = _chk(dloss_dalphas, "dloss_dalphas")
-            _same_device(pws, ga)
-            if ga.numel() != N:
-                raise ValueError("dloss_dalphas must have N elements")
+            ga = _per_gaussian(dloss_dalphas, "dloss_dalphas", N, pws)
         self.epoch += 1
         with torch.cuda.device(pws.device):
             _lib.check(self.lib.gsb_preprocess_backward_push(
-                N, self.k3, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), _ptr(Rcw), _ptr(tcw), _ptr(twc),
-                float(cam.fx), float(cam.fy), float(cam.cx), float(cam.cy), float(cam.width), float(cam.height), _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(ga),
-                _ptr(moments), _ptr(cinv2ds), _ptr(dus), self.world, self.rank, self.regions, self.epoch, _stream()),
-                self.lib)
+                *_scene_args(params, N, k, cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height),
+                _ptr(gu), _ptr(gc), _ptr(gcol), _ptr(ga), _ptr(moments), _ptr(cinv2ds), _ptr(dus), self.world,
+                self.rank, self.regions, self.epoch, _stream()), self.lib)
         return dus
 
     def reduce(self):

@@ -333,7 +333,7 @@ def test_python_validation_and_refusals_without_a_device():
     with pytest.raises(ValueError, match="pinhole"):
         ops.camera_table([cam])
     with pytest.raises(ValueError, match="pinhole"):
-        ops.filter3d(x, [cam]) if torch.cuda.is_available() else ops.camera_table([Camera(8, 8, 5, 5, 4, 4, R, t),
+        ops.filter3d(x.cuda(), [cam]) if torch.cuda.is_available() else ops.camera_table([Camera(8, 8, 5, 5, 4, 4, R, t),
                                                                                    cam])
     # ops: unknown model, coefficients without the fisheye, and a non-pinhole preprocessB without moment rows
     with pytest.raises(ValueError, match="camera_model"):
