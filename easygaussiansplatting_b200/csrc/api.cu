@@ -4,6 +4,7 @@
 #include <string.h>
 
 #include <cmath>
+#include <initializer_list>
 #include <mutex>
 #include <vector>
 
@@ -813,6 +814,14 @@ static float *const *gau_ptrs(const gsb_gaussians *g) {
   static_assert(sizeof(gsb_gaussians) == 6 * sizeof(float *), "gsb_gaussians layout");
   return reinterpret_cast<float *const *>(g);
 }
+// the Adam moments of a call: all of `m` given or all NULL.  tables: `m` are gsb_gaussians, and a
+// given one must also hold all six tensors
+static bool moments_ok(std::initializer_list<const void *> m, bool tables = false) {
+  bool any = false, all = true;
+  for (const void *p : m)
+    any |= p != nullptr, all &= tables ? gau_complete(static_cast<const gsb_gaussians *>(p)) : p != nullptr;
+  return all || !any;
+}
 
 int gsb_density_accumulate(int64_t N, const float *dloss_dus, const uint8_t *mask, float *grad_accum,
                            int32_t *cunt, int first, gsb_stream_t stream) {
@@ -840,14 +849,15 @@ int gsb_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64
                       const gsb_gaussians *src, const gsb_gaussians *src_m, const gsb_gaussians *src_v,
                       const float *z, const gsb_gaussians *dst, const gsb_gaussians *dst_m,
                       const gsb_gaussians *dst_v, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0 && K >= 0 && C >= 0 && S >= 0 && K <= N && C + S <= K, "density_apply: bad counts");
+  // N < 2^30: the rebuild's row table packs the class into bits 30-31 of the survivor slot
+  GSB_REQUIRE(N >= 0 && N < ((int64_t)1 << 30) && K >= 0 && C >= 0 && S >= 0 && K <= N && C + S <= K,
+              "density_apply: bad counts");
   if (N == 0) return 0;
   GSB_REQUIRE(cls && slots, "density_apply: null plan");
   GSB_REQUIRE(gau_complete(src), "density_apply: src has a null tensor");
   GSB_REQUIRE(K + C + S == 0 || gau_complete(dst), "density_apply: dst has a null tensor");
   const bool state = src_m != nullptr;
-  GSB_REQUIRE((src_v != nullptr) == state && (dst_m != nullptr) == state && (dst_v != nullptr) == state,
-              "density_apply: Adam moments must be all given or all NULL");
+  GSB_REQUIRE(moments_ok({src_m, src_v, dst_m, dst_v}), "density_apply: Adam moments must be all given or all NULL");
   if (state)
     GSB_REQUIRE(gau_complete(src_m) && gau_complete(src_v) && (K + C + S == 0 || (gau_complete(dst_m) && gau_complete(dst_v))),
                 "density_apply: a moment tensor is null");
@@ -864,8 +874,7 @@ int gsb_density_apply_rows(int64_t N, const uint8_t *cls, const int32_t *slots, 
   GSB_REQUIRE(N >= 0 && K >= 0 && C >= 0 && S >= 0 && K <= N && C + S <= K && D >= 1, "density_apply_rows: bad counts");
   if (N == 0 || K + C + S == 0) return 0;
   GSB_REQUIRE(cls && slots && src && dst, "density_apply_rows: null pointer");
-  const bool state = src_m != nullptr;
-  GSB_REQUIRE((src_v != nullptr) == state && (dst_m != nullptr) == state && (dst_v != nullptr) == state,
+  GSB_REQUIRE(moments_ok({src_m, src_v, dst_m, dst_v}),
               "density_apply_rows: Adam moments must be all given or all NULL");
   return launch_density_apply_rows(N, cls, slots, K, C, D, src, src_m, src_v, dst, dst_m, dst_v, (cudaStream_t)stream);
 }
@@ -912,10 +921,6 @@ int gsb_mcmc_sample(int64_t N, int64_t n, const double *u, void *ws, size_t ws_b
   return launch_mcmc_sample(N, n, u, ws, sampled, (cudaStream_t)stream);
 }
 
-static bool mcmc_moments_ok(const gsb_gaussians *m, const gsb_gaussians *v) {
-  return (m == nullptr) == (v == nullptr) && (m == nullptr || (gau_complete(m) && gau_complete(v)));
-}
-
 int gsb_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, size_t ws_bytes, double min_opacity,
                       int n_max, const gsb_gaussians *params, const gsb_gaussians *exp_avg,
                       const gsb_gaussians *exp_avg_sq, gsb_stream_t stream) {
@@ -924,7 +929,7 @@ int gsb_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, si
   GSB_REQUIRE(min_opacity > 0.0 && min_opacity < 1.0, "mcmc_relocate: min_opacity must be in (0, 1)");
   if (n == 0) return 0;
   GSB_REQUIRE(sampled && gau_complete(params), "mcmc_relocate: null pointer");
-  GSB_REQUIRE(mcmc_moments_ok(exp_avg, exp_avg_sq), "mcmc_relocate: Adam moments must be both given or both NULL");
+  GSB_REQUIRE(moments_ok({exp_avg, exp_avg_sq}, true), "mcmc_relocate: Adam moments must be both given or both NULL");
   GSB_MCMC_WS(ws, ws_bytes, N, n, "mcmc_relocate");
   return launch_mcmc_relocate(N, n, sampled, ws, min_opacity, n_max, gau_ptrs(params),
                               exp_avg ? gau_ptrs(exp_avg) : nullptr, exp_avg_sq ? gau_ptrs(exp_avg_sq) : nullptr,
@@ -936,8 +941,7 @@ int gsb_mcmc_relocate_rows(int64_t N, int64_t n, const int32_t *sampled, const v
   GSB_REQUIRE(N >= 0 && N < kMcmcMaxN && n >= 0 && n <= N && D >= 1, "mcmc_relocate_rows: bad counts");
   if (n == 0) return 0;
   GSB_REQUIRE(sampled && x, "mcmc_relocate_rows: null pointer");
-  GSB_REQUIRE((exp_avg == nullptr) == (exp_avg_sq == nullptr),
-              "mcmc_relocate_rows: Adam moments must be both given or both NULL");
+  GSB_REQUIRE(moments_ok({exp_avg, exp_avg_sq}), "mcmc_relocate_rows: Adam moments must be both given or both NULL");
   GSB_MCMC_WS(ws, ws_bytes, N, 0, "mcmc_relocate_rows");
   return launch_mcmc_relocate_rows(N, n, sampled, ws, D, x, exp_avg, exp_avg_sq, (cudaStream_t)stream);
 }
@@ -953,8 +957,7 @@ int gsb_mcmc_grow(int64_t N, int64_t n, const int32_t *sampled, void *ws, size_t
   if (N == 0) return 0;
   GSB_REQUIRE(gau_complete(src) && gau_complete(dst) && (n == 0 || sampled), "mcmc_grow: null pointer");
   const bool state = src_m != nullptr;
-  GSB_REQUIRE(mcmc_moments_ok(src_m, src_v) && mcmc_moments_ok(dst_m, dst_v) && (dst_m != nullptr) == state,
-              "mcmc_grow: Adam moments must be all given or all NULL");
+  GSB_REQUIRE(moments_ok({src_m, src_v, dst_m, dst_v}, true), "mcmc_grow: Adam moments must be all given or all NULL");
   GSB_MCMC_WS(ws, ws_bytes, N, n, "mcmc_grow");
   return launch_mcmc_grow(N, n, sampled, ws, min_opacity, n_max, gau_ptrs(src), state ? gau_ptrs(src_m) : nullptr,
                           state ? gau_ptrs(src_v) : nullptr, gau_ptrs(dst), state ? gau_ptrs(dst_m) : nullptr,
@@ -968,9 +971,7 @@ int gsb_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const void 
   GSB_REQUIRE(n == 0 || N > 0, "mcmc_grow_rows: draws from no rows");
   if (N == 0) return 0;
   GSB_REQUIRE(src && dst && (n == 0 || sampled), "mcmc_grow_rows: null pointer");
-  const bool state = src_m != nullptr;
-  GSB_REQUIRE((src_v != nullptr) == state && (dst_m != nullptr) == state && (dst_v != nullptr) == state,
-              "mcmc_grow_rows: Adam moments must be all given or all NULL");
+  GSB_REQUIRE(moments_ok({src_m, src_v, dst_m, dst_v}), "mcmc_grow_rows: Adam moments must be all given or all NULL");
   GSB_MCMC_WS(ws, ws_bytes, N, 0, "mcmc_grow_rows");
   return launch_mcmc_grow_rows(N, n, sampled, ws, D, src, src_m, src_v, dst, dst_m, dst_v, (cudaStream_t)stream);
 }

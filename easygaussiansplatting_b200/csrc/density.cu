@@ -79,20 +79,127 @@ __device__ __forceinline__ uint8_t classify_row(int64_t i, const float *__restri
   return c;
 }
 
-// ---- the slots (exclusive scan of the three class counters in row order), hand-written:
-//   k_density_classify_count  classify 1024 rows per CTA and leave the CTA's three counts;
-//   k_density_scan_blocks     one CTA turns the per-CTA counts into exclusive offsets + totals;
-//   k_density_slots           every CTA re-reads its 1024 class bytes (4 consecutive rows per
-//                             thread), scans them locally and writes the 12-byte slots.
-// 25 B per Gaussian in total; three launches, no library scan.
+// ---- the plan scans.  Both plans (density slots, MCMC sampler) are an exclusive scan in row
+// order, hand-written as three launches and no library scan:
+//   a row kernel      classifies / weighs 1024 rows per CTA and leaves the CTA's counters;
+//   scan_blocks       one CTA turns the per-CTA counters into exclusive offsets + totals;
+//   a row kernel      re-reads its CTA's rows (4 consecutive rows per thread), scans them
+//                     locally and writes the per-row results.
+// The counter tuples: inside a CTA the density kernels count (survivors | clones << 16, splits),
+// at most SC_ROWS each, so a shuffle ladder step is two shuffles, not three; the density block
+// counts are three int32 (Slot3); MCMC counts (uint64 weight, int32 dead) everywhere.
 constexpr int SC_THREADS = 256, SC_PER = 4, SC_ROWS = SC_THREADS * SC_PER;
+
+struct KcSp {
+  uint32_t kc, sp;
+};
+struct WDead {
+  uint64_t w;
+  int32_t d;
+};
+__device__ __forceinline__ KcSp operator+(KcSp a, KcSp b) { return {a.kc + b.kc, a.sp + b.sp}; }
+__device__ __forceinline__ KcSp operator-(KcSp a, KcSp b) { return {a.kc - b.kc, a.sp - b.sp}; }
+__device__ __forceinline__ Slot3 operator+(Slot3 a, Slot3 b) { return {a.k + b.k, a.c + b.c, a.s + b.s}; }
+__device__ __forceinline__ Slot3 operator-(Slot3 a, Slot3 b) { return {a.k - b.k, a.c - b.c, a.s - b.s}; }
+__device__ __forceinline__ WDead operator+(WDead a, WDead b) { return {a.w + b.w, a.d + b.d}; }
+__device__ __forceinline__ WDead operator-(WDead a, WDead b) { return {a.w - b.w, a.d - b.d}; }
+__device__ __forceinline__ KcSp shfl_up(KcSp x, int o) {
+  return {__shfl_up_sync(0xffffffffu, x.kc, o), __shfl_up_sync(0xffffffffu, x.sp, o)};
+}
+__device__ __forceinline__ Slot3 shfl_up(Slot3 x, int o) {
+  return {__shfl_up_sync(0xffffffffu, x.k, o), __shfl_up_sync(0xffffffffu, x.c, o),
+          __shfl_up_sync(0xffffffffu, x.s, o)};
+}
+__device__ __forceinline__ WDead shfl_up(WDead x, int o) {
+  return {__shfl_up_sync(0xffffffffu, x.w, o), __shfl_up_sync(0xffffffffu, x.d, o)};
+}
+__device__ __forceinline__ KcSp warp_sum(KcSp x) {
+  return {__reduce_add_sync(0xffffffffu, x.kc), __reduce_add_sync(0xffffffffu, x.sp)};
+}
+__device__ __forceinline__ WDead warp_sum(WDead x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x.w += __shfl_xor_sync(0xffffffffu, x.w, o);
+  return {x.w, (int32_t)__reduce_add_sync(0xffffffffu, (uint32_t)x.d)};
+}
+
+// the sum of x over the CTA of NT threads, valid in thread 0; warp_tot: NT / 32 entries
+template <int NT, class T>
+__device__ __forceinline__ T cta_sum(T x, T *warp_tot) {
+  x = warp_sum(x);
+  if ((threadIdx.x & 31) == 0) warp_tot[threadIdx.x >> 5] = x;
+  __syncthreads();
+  T s = warp_tot[0];
+#pragma unroll
+  for (int w = 1; w < NT / 32; w++) s = s + warp_tot[w];
+  return s;
+}
+
+// the sum of x over the CTA's threads before this one (thread order) and, in `total`, over all of
+// them; warp_tot: NT / 32 entries, which the caller may rewrite only after a __syncthreads
+template <int NT, class T>
+__device__ __forceinline__ T cta_exclusive_scan(T x, T *warp_tot, T &total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  T inc = x;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = shfl_up(inc, o);
+    if (lane >= o) inc = inc + y;
+  }
+  if (lane == 31) warp_tot[wid] = inc;
+  __syncthreads();
+  T before = inc - x;
+  total = T{};
+#pragma unroll
+  for (int w = 0; w < NT / 32; w++) {
+    if (w < wid) before = before + warp_tot[w];
+    total = total + warp_tot[w];
+  }
+  return before;
+}
+
+// The body of the block-scan kernels (one CTA of 1024 threads), in place: the counters of CTA b ->
+// the counters of the CTAs before b; the totals = their sums.  The CTA walks the counters 1024
+// CTAs at a time, carrying the sum from pass to pass.
+template <class Blocks>
+__device__ __forceinline__ void scan_blocks(int nb, Blocks B, int64_t *__restrict__ totals) {
+  using T = typename Blocks::T;
+  __shared__ T warp_tot[32];
+  T carry{};
+  for (int base = 0; base < nb; base += 1024) {
+    const int b = base + threadIdx.x;
+    const T v = b < nb ? B.load(b) : T{};
+    T pass;
+    const T before = cta_exclusive_scan<1024>(v, warp_tot, pass);
+    if (b < nb) B.store(b, carry + before);
+    carry = carry + pass;
+    __syncthreads();  // warp_tot is rewritten by the next pass
+  }
+  if (threadIdx.x == 0) B.totals(totals, carry);
+}
+
+// the density block counts: three int32 per CTA
+struct DensityBlocks {
+  using T = Slot3;
+  int32_t *c;
+  __device__ Slot3 load(int b) const { return {c[3 * b], c[3 * b + 1], c[3 * b + 2]}; }
+  __device__ void store(int b, Slot3 x) const { c[3 * b] = x.k, c[3 * b + 1] = x.c, c[3 * b + 2] = x.s; }
+  __device__ void totals(int64_t *t, Slot3 x) const { t[0] = x.k, t[1] = x.c, t[2] = x.s; }
+};
+
+__global__ void __launch_bounds__(1024) k_density_scan_blocks(int nb, DensityBlocks B, int64_t *__restrict__ totals) {
+  scan_blocks(nb, B, totals);
+}
+
+__device__ __forceinline__ KcSp class_count(uint8_t c) {
+  return {(c != CLS_PRUNE) + ((uint32_t)(c == CLS_CLONE) << 16), (uint32_t)(c == CLS_SPLIT)};
+}
 
 __global__ void __launch_bounds__(SC_THREADS) k_density_classify_count(
     int64_t N, const float *__restrict__ alphas_raw, const float *__restrict__ scales_raw,
     const float *__restrict__ acc, const int32_t *__restrict__ cnt, float alpha_raw_min, float scale_raw_max,
     float grad_min, float scale_clone_max, uint8_t *__restrict__ cls, int32_t *__restrict__ block_counts) {
-  __shared__ uint32_t red[2][SC_THREADS / 32];
-  uint32_t kc = 0, sp = 0;  // (survivors | clones << 16), splits: at most SC_ROWS each per CTA
+  __shared__ KcSp red[SC_THREADS / 32];
+  KcSp n{0, 0};
 #pragma unroll
   for (int j = 0; j < SC_PER; j++) {
     const int64_t i = (int64_t)blockIdx.x * SC_ROWS + j * SC_THREADS + threadIdx.x;
@@ -100,92 +207,29 @@ __global__ void __launch_bounds__(SC_THREADS) k_density_classify_count(
       const uint8_t c =
           classify_row(i, alphas_raw, scales_raw, acc, cnt, alpha_raw_min, scale_raw_max, grad_min, scale_clone_max);
       cls[i] = c;
-      kc += (c != CLS_PRUNE) + ((uint32_t)(c == CLS_CLONE) << 16);
-      sp += c == CLS_SPLIT;
+      n = n + class_count(c);
     }
   }
-  kc = __reduce_add_sync(0xffffffffu, kc);
-  sp = __reduce_add_sync(0xffffffffu, sp);
-  if ((threadIdx.x & 31) == 0) red[0][threadIdx.x >> 5] = kc, red[1][threadIdx.x >> 5] = sp;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t a = 0, b = 0;
-#pragma unroll
-    for (int w = 0; w < SC_THREADS / 32; w++) a += red[0][w], b += red[1][w];
-    block_counts[3 * blockIdx.x + 0] = (int32_t)(a & 0xffffu);
-    block_counts[3 * blockIdx.x + 1] = (int32_t)(a >> 16);
-    block_counts[3 * blockIdx.x + 2] = (int32_t)b;
-  }
-}
-
-// in place: block_counts[b] -> the counts before CTA b; totals = the three sums
-__global__ void __launch_bounds__(1024) k_density_scan_blocks(int nb, int32_t *__restrict__ block_counts,
-                                                              int64_t *__restrict__ totals) {
-  __shared__ int warp_tot[3][32];
-  __shared__ int carry[3];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x < 3) carry[threadIdx.x] = 0;
-  __syncthreads();
-  for (int base = 0; base < nb; base += 1024) {
-    const int b = base + threadIdx.x;
-    int v[3] = {0, 0, 0}, inc[3];
-    if (b < nb) v[0] = block_counts[3 * b], v[1] = block_counts[3 * b + 1], v[2] = block_counts[3 * b + 2];
-#pragma unroll
-    for (int q = 0; q < 3; q++) {
-      int x = v[q];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-      }
-      inc[q] = x;
-      if (lane == 31) warp_tot[q][wid] = x;
-    }
-    __syncthreads();
-    int c0[3];
-#pragma unroll
-    for (int q = 0; q < 3; q++) {
-      int before = carry[q];
-      for (int w = 0; w < wid; w++) before += warp_tot[q][w];
-      c0[q] = before + inc[q] - v[q];
-    }
-    if (b < nb) block_counts[3 * b] = c0[0], block_counts[3 * b + 1] = c0[1], block_counts[3 * b + 2] = c0[2];
-    __syncthreads();
-    if (threadIdx.x == 1023) {
-#pragma unroll
-      for (int q = 0; q < 3; q++) carry[q] = c0[q] + v[q];
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x < 3) totals[threadIdx.x] = carry[threadIdx.x];
+  n = cta_sum<SC_THREADS>(n, red);
+  if (threadIdx.x == 0)
+    DensityBlocks{block_counts}.store(blockIdx.x, {(int)(n.kc & 0xffffu), (int)(n.kc >> 16), (int)n.sp});
 }
 
 __global__ void __launch_bounds__(SC_THREADS) k_density_slots(int64_t N, const uint8_t *__restrict__ cls,
-                                                              const int32_t *__restrict__ block_offsets,
+                                                              const DensityBlocks block_offsets,
                                                               Slot3 *__restrict__ slots) {
-  __shared__ uint32_t warp_tot[2][SC_THREADS / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  __shared__ KcSp warp_tot[SC_THREADS / 32];
   const int64_t row0 = (int64_t)blockIdx.x * SC_ROWS + (int64_t)threadIdx.x * SC_PER;
   uint8_t c[SC_PER];
-  uint32_t kc = 0, sp = 0;
+  KcSp n{0, 0};
 #pragma unroll
   for (int j = 0; j < SC_PER; j++) {
     c[j] = row0 + j < N ? cls[row0 + j] : (uint8_t)CLS_PRUNE;
-    kc += (c[j] != CLS_PRUNE) + ((uint32_t)(c[j] == CLS_CLONE) << 16);
-    sp += c[j] == CLS_SPLIT;
+    n = n + class_count(c[j]);
   }
-  uint32_t ikc = kc, isp = sp;  // inclusive over the warp
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t a = __shfl_up_sync(0xffffffffu, ikc, o), b = __shfl_up_sync(0xffffffffu, isp, o);
-    if (lane >= o) ikc += a, isp += b;
-  }
-  if (lane == 31) warp_tot[0][wid] = ikc, warp_tot[1][wid] = isp;
-  __syncthreads();
-  uint32_t bkc = ikc - kc, bsp = isp - sp;  // exclusive within the CTA
-  for (int w = 0; w < wid; w++) bkc += warp_tot[0][w], bsp += warp_tot[1][w];
-  Slot3 run{block_offsets[3 * blockIdx.x] + (int)(bkc & 0xffffu), block_offsets[3 * blockIdx.x + 1] + (int)(bkc >> 16),
-            block_offsets[3 * blockIdx.x + 2] + (int)bsp};
+  KcSp total;
+  const KcSp b = cta_exclusive_scan<SC_THREADS>(n, warp_tot, total);
+  Slot3 run = block_offsets.load(blockIdx.x) + Slot3{(int)(b.kc & 0xffffu), (int)(b.kc >> 16), (int)b.sp};
 #pragma unroll
   for (int j = 0; j < SC_PER; j++) {
     if (row0 + j < N) slots[row0 + j] = run;
@@ -193,10 +237,26 @@ __global__ void __launch_bounds__(SC_THREADS) k_density_slots(int64_t N, const u
   }
 }
 
-struct Sets {
-  const float *p[6], *m[6], *v[6];  // m / v entries may be null (no optimizer state yet)
-  float *dp[6], *dm[6], *dv[6];
+// One per-Gaussian tensor and its Adam moments (m, v: both or neither, NULL without optimizer
+// state), source and destination; the six training tensors are Jobs::j[0..5] (kWidth).  An extra
+// tensor [N, D] (per-Gaussian features) is one Job of width D.
+struct Job {
+  const float *p, *m, *v;  // sources
+  float *dp, *dm, *dv;     // destinations (relocate: the sources)
+  int w;
 };
+struct Jobs {
+  Job j[6];
+};
+// from the six-pointer tables of gsb_gaussians; NULL moment tables give NULL moments
+Jobs jobs(float *const *src, float *const *src_m, float *const *src_v, float *const *dst, float *const *dst_m,
+          float *const *dst_v) {
+  Jobs J;
+  for (int a = 0; a < 6; a++)
+    J.j[a] = Job{src[a], src_m ? src_m[a] : nullptr, src_v ? src_v[a] : nullptr, dst[a],
+                 dst_m ? dst_m[a] : nullptr, dst_v ? dst_v[a] : nullptr, kWidth[a]};
+  return J;
+}
 
 __device__ __forceinline__ float logit_of_sigmoid(float x) {
   const float a = 1.f / (1.f + expf(-x));  // get_alphas
@@ -220,85 +280,13 @@ __device__ __forceinline__ float split_offset(const float *__restrict__ q4, cons
   return 2.f * u * uv + v * (w * w - uu) + 2.f * c * w;
 }
 
-// One "job" per (tensor, set) pair -- 6 tensors x {parameter, exp_avg, exp_avg_sq} = 18 jobs on
-// blockIdx.y, grid-stride over the job's N*w elements, four independent elements in flight
-// per thread (loads first, then stores).  Survivors move to their compacted row; clones /
-// splits additionally produce a new row at K + slot (clones) or K + C + slot (splits): the
-// recomputed value for a parameter, zero for an Adam moment.  This kernel serves N >= 23 M,
-// where element indices need 64 bits; smaller N take the row-group kernel below.
-template <int A, int SET>
-__device__ __forceinline__ void apply_job(int64_t N, const uint8_t *__restrict__ cls, const Slot3 *__restrict__ slots,
-                                          int64_t K, int64_t C, const Sets &S, const float *__restrict__ z) {
-  constexpr int w = kWidth[A];
-  constexpr int U = 4;
-  const float *__restrict__ src = SET == 0 ? S.p[A] : (SET == 1 ? S.m[A] : S.v[A]);
-  float *__restrict__ dst = SET == 0 ? S.dp[A] : (SET == 1 ? S.dm[A] : S.dv[A]);
-  if (src == nullptr) return;
-  const int64_t total = N * w;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t e0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e0 < total; e0 += stride * U) {
-    int64_t row[U];
-    uint8_t cl[U];
-    float val[U];
-    Slot3 sl[U];
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const int64_t e = e0 + (int64_t)u * stride;
-      row[u] = e < total ? e / w : 0;
-      cl[u] = e < total ? cls[row[u]] : (uint8_t)CLS_PRUNE;
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (cl[u] == CLS_PRUNE) continue;
-      val[u] = src[e0 + (int64_t)u * stride];
-      sl[u] = slots[row[u]];
-    }
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      if (cl[u] == CLS_PRUNE) continue;
-      const int64_t i = row[u];
-      const int c = (int)(e0 + (int64_t)u * stride - i * w);
-      dst[(int64_t)sl[u].k * w + c] = val[u];
-      if (cl[u] == CLS_KEEP) continue;
-      const bool split = cl[u] == CLS_SPLIT;
-      const int64_t r = (split ? K + C + (int64_t)sl[u].s : K + (int64_t)sl[u].c) * w + c;
-      float nv = 0.f;
-      if (SET == 0) {
-        nv = val[u];
-        if (A == 0) {
-          if (split) nv += split_offset(S.p[5] + 4 * (int64_t)i, S.p[4] + 3 * (int64_t)i, z + 3 * (int64_t)sl[u].s, c);
-        } else if (A == 3) {
-          nv = logit_of_sigmoid(nv);
-        } else if (A == 4) {
-          const float s = expf(nv);               // get_scales
-          nv = logf(split ? s * 0.6f : s);        // gsmodel.py:281 then get_scales_raw
-        } else if (A == 5) {
-          const float *q = src + 4 * (int64_t)i;
-          nv = nv / fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
-        }
-      }
-      dst[r] = nv;
-    }
-  }
-}
-
-__global__ void __launch_bounds__(256) k_density_apply(int64_t N, const uint8_t *__restrict__ cls,
-                                                       const Slot3 *__restrict__ slots, int64_t K, int64_t C, Sets S,
-                                                       const float *__restrict__ z) {
-#define GSB_JOB(a, s) \
-  case 3 * a + s: apply_job<a, s>(N, cls, slots, K, C, S, z); break;
-  switch (blockIdx.y) {
-    GSB_JOB(0, 0) GSB_JOB(0, 1) GSB_JOB(0, 2) GSB_JOB(1, 0) GSB_JOB(1, 1) GSB_JOB(1, 2)
-    GSB_JOB(2, 0) GSB_JOB(2, 1) GSB_JOB(2, 2) GSB_JOB(3, 0) GSB_JOB(3, 1) GSB_JOB(3, 2)
-    GSB_JOB(4, 0) GSB_JOB(4, 1) GSB_JOB(4, 2) GSB_JOB(5, 0) GSB_JOB(5, 1) GSB_JOB(5, 2)
-  }
-#undef GSB_JOB
-}
-
-// ---- row-group kernel (N < 23 M): a warp moves 32 consecutive Gaussians of one array.
-// The per-Gaussian plan (class, survivor slot, new-row slot) is read once per group into a
-// 32-entry shared-memory table instead of once per element (13 B per 4-byte element in the
-// kernel above).  Loads and stores are 4-byte but fully coalesced: lane l handles elements
+// ---- the rebuild: one job per (tensor, set) pair -- 6 tensors x {parameter, exp_avg,
+// exp_avg_sq} = 18 jobs on blockIdx.y.  Survivors move to their compacted row; clones / splits
+// additionally produce a new row at K + slot (clones) or K + C + slot (splits): the recomputed
+// value for a parameter, zero for an Adam moment.  A warp moves 32 consecutive Gaussians of one
+// array.  The per-Gaussian plan (class, survivor slot, new-row slot) is read once per group into
+// a 32-entry shared-memory table instead of once per element.  Loads and stores are 4-byte but
+// fully coalesced: lane l handles elements
 // l, l + 32, ... of the group's contiguous source span, 12 loads in flight per lane for the wide
 // arrays; consecutive survivors are consecutive in the destination too, so a store instruction
 // writes whole 32-byte sectors.  (Reading the span with float4 loads would force the four
@@ -308,50 +296,50 @@ constexpr int DG_PAIRS = 4;  // pairs of 45-wide rows in flight per lane (3 load
 
 // the value a clone / split writes at its new row (parameters; Adam moments start at 0)
 template <int A>
-__device__ __forceinline__ float new_row_value(float val, bool split, int64_t i, int s, int c, const Sets &S,
+__device__ __forceinline__ float new_row_value(float val, bool split, int64_t i, int s, int c, const Jobs &J,
                                                const float *__restrict__ z) {
   float nv = val;
   if (A == 0) {
-    if (split) nv += split_offset(S.p[5] + 4 * i, S.p[4] + 3 * i, z + 3 * (int64_t)s, c);
+    if (split) nv += split_offset(J.j[5].p + 4 * i, J.j[4].p + 3 * i, z + 3 * (int64_t)s, c);
   } else if (A == 3) {
     nv = logit_of_sigmoid(nv);
   } else if (A == 4) {
     const float e = expf(nv);          // get_scales
     nv = logf(split ? e * 0.6f : e);   // gsmodel.py:281 then get_scales_raw
   } else if (A == 5) {
-    const float *q = S.p[5] + 4 * i;
+    const float *q = J.j[5].p + 4 * i;
     nv = nv / fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
   }
   return nv;
 }
 
-template <int A, int SET>
-__device__ __forceinline__ void rows_job(int row0, const int2 *__restrict__ tab, int K, int C, const Sets &S,
+template <class Off, int A, int SET>
+__device__ __forceinline__ void rows_job(int row0, const int2 *__restrict__ tab, int K, int C, const Jobs &J,
                                          const float *__restrict__ z, int lane) {
   constexpr int w = kWidth[A];
-  const float *__restrict__ src = SET == 0 ? S.p[A] : (SET == 1 ? S.m[A] : S.v[A]);
-  float *__restrict__ dst = SET == 0 ? S.dp[A] : (SET == 1 ? S.dm[A] : S.dv[A]);
+  const float *__restrict__ src = SET == 0 ? J.j[A].p : (SET == 1 ? J.j[A].m : J.j[A].v);
+  float *__restrict__ dst = SET == 0 ? J.j[A].dp : (SET == 1 ? J.j[A].dm : J.j[A].dv);
   if (src == nullptr) return;
   const float *__restrict__ gsrc = src + (size_t)row0 * w;
   // element (row r of the group, column col) with plan entry `info`
   auto emit = [&](int r, int col, int2 info, float val) {
     const unsigned cl = (unsigned)info.x >> 30;
     if (cl == CLS_PRUNE) return;
-    dst[(size_t)(info.x & 0x3fffffff) * w + col] = val;
+    dst[(Off)(info.x & 0x3fffffff) * w + col] = val;
     if (cl == CLS_KEEP) return;
     float nv = 0.f;
-    if (SET == 0) nv = new_row_value<A>(val, cl == CLS_SPLIT, (int64_t)row0 + r, info.y - K - C, col, S, z);
-    dst[(size_t)info.y * w + col] = nv;
+    if (SET == 0) nv = new_row_value<A>(val, cl == CLS_SPLIT, (int64_t)row0 + r, info.y - K - C, col, J, z);
+    dst[(Off)info.y * w + col] = nv;
   };
   const int2 pruned = make_int2((int)((unsigned)CLS_PRUNE << 30), 0);
   // Fixed lane -> (row, column) maps: table entries of rows past the end of the array are
-  // CLS_PRUNE, so no row bound is checked; destination element indices fit 32 bits (2 N * 45 < 2^32 for N < 23 M)
+  // CLS_PRUNE, so no row bound is checked; destination element offsets (up to 2 N * 45) are Off
   constexpr bool plain = SET != 0 || A == 1 || A == 2;  // the new row is a copy (parameters) or zero (moments)
   auto emit_fixed = [&](int r, int col, int2 info, float val) {
     if constexpr (plain) {  // two predicated stores, no branches
       const unsigned cl = (unsigned)info.x >> 30;
-      if (cl != CLS_PRUNE) dst[(unsigned)(info.x & 0x3fffffff) * w + col] = val;
-      if (cl == CLS_CLONE || cl == CLS_SPLIT) dst[(unsigned)info.y * w + col] = SET == 0 ? val : 0.f;
+      if (cl != CLS_PRUNE) dst[(Off)(info.x & 0x3fffffff) * w + col] = val;
+      if (cl == CLS_CLONE || cl == CLS_SPLIT) dst[(Off)info.y * w + col] = SET == 0 ? val : 0.f;
     } else {
       emit(r, col, info, val);
     }
@@ -406,9 +394,9 @@ __device__ __forceinline__ void rows_job(int row0, const int2 *__restrict__ tab,
   }
 }
 
-template <int A, int SET>
+template <class Off, int A, int SET>
 __device__ __noinline__ void rows_loop(int N, const uint8_t *__restrict__ cls, const Slot3 *__restrict__ slots, int K,
-                                       int C, const Sets &S, const float *__restrict__ z, int2 *tab) {
+                                       int C, const Jobs &J, const float *__restrict__ z, int2 *tab) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int groups = (N + 31) / 32;
   for (int g = blockIdx.x * DG_WARPS + wid; g < groups; g += gridDim.x * DG_WARPS) {
@@ -419,22 +407,26 @@ __device__ __noinline__ void rows_loop(int N, const uint8_t *__restrict__ cls, c
       c = cls[row];
       sl = slots[row];
     }
-    // (class | survivor slot, new-row slot); slots < N < 2^30
+    // (class | survivor slot, new-row slot); slots < N < 2^30 (gsb_density_apply checks N)
     tab[lane] = make_int2((int)((unsigned)c << 30) | sl.k, c == CLS_SPLIT ? K + C + sl.s : K + sl.c);
     __syncwarp();
-    rows_job<A, SET>(row0, tab, K, C, S, z, lane);
+    rows_job<Off, A, SET>(row0, tab, K, C, J, z, lane);
     __syncwarp();  // the table is rewritten for the next group
   }
 }
 
+// Off: the type of the destination element offsets.  uint32_t while they stay below 2^31 (2 N * 45 <
+// 2^31 for N < 23 M): the narrower address arithmetic makes the rebuild ~7 % faster at N = 1 M
+// (DESIGN §3, kernel table); size_t above
+template <class Off>
 __global__ void __launch_bounds__(32 * DG_WARPS) k_density_apply_rows(int N, const uint8_t *__restrict__ cls,
                                                                        const Slot3 *__restrict__ slots, int K, int C,
-                                                                       const __grid_constant__ Sets S,
+                                                                       const __grid_constant__ Jobs J,
                                                                        const float *__restrict__ z) {
   __shared__ int2 tabs[DG_WARPS][32];
   int2 *tab = tabs[threadIdx.x >> 5];
 #define GSB_JOB(y, a, s) \
-  case y: rows_loop<a, s>(N, cls, slots, K, C, S, z, tab); break;
+  case y: rows_loop<Off, a, s>(N, cls, slots, K, C, J, z, tab); break;
   switch (blockIdx.y) {
     GSB_JOB(0, 2, 0) GSB_JOB(1, 2, 1) GSB_JOB(2, 2, 2) GSB_JOB(3, 0, 0) GSB_JOB(4, 0, 1) GSB_JOB(5, 0, 2)
     GSB_JOB(6, 1, 0) GSB_JOB(7, 1, 1) GSB_JOB(8, 1, 2) GSB_JOB(9, 3, 0) GSB_JOB(10, 3, 1) GSB_JOB(11, 3, 2)
@@ -578,11 +570,11 @@ inline int stream_grid(int64_t total, int block) {
 // The sampler is integer arithmetic so that its ids do not depend on summation order: row i has
 // the weight q_i = floor(o_i 2^32) (o_i = sigmoid of the fp32 raw value, in fp64; 0 for excluded
 // rows), W = the uint64 inclusive prefix sum, and a uniform u picks the first i with
-// W_i > floor(u W_total).  The scan has the density scan's three-kernel shape:
-//   k_mcmc_weight_count  per-CTA weight sum and dead count of 1024 rows;
-//   k_mcmc_scan_blocks   one CTA turns them into exclusive offsets and the totals;
-//   k_mcmc_prefix        every CTA rescans its rows, writes W, the dead-row list, and clears the
-//                        per-row sample counts.
+// W_i > floor(u W_total).  The scan is a plan scan (above):
+//   k_mcmc_weight_count         per-CTA weight sum and dead count of 1024 rows;
+//   k_mcmc_scan_blocks          one CTA turns them into exclusive offsets and the totals;
+//   k_mcmc_prefix               every CTA rescans its rows, writes W, the dead-row list, and
+//                               clears the per-row sample counts.
 enum : int { MCMC_RELOCATE = 0, MCMC_GROW = 1 };
 
 // relocate samples alive rows (dead = !(a > alpha_raw_min), NaN included); grow samples every
@@ -594,111 +586,57 @@ __device__ __forceinline__ uint64_t mcmc_weight(float a, float alpha_raw_min, in
   return (uint64_t)floor(o * 4294967296.0);
 }
 
-__device__ __forceinline__ uint64_t warp_sum_u64(uint64_t x) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-  return x;
+// the MCMC block counters: a uint64 weight sum and an int32 dead count per CTA, in two arrays
+struct McmcBlocks {
+  using T = WDead;
+  uint64_t *w;
+  int32_t *d;
+  __device__ WDead load(int b) const { return {w[b], d[b]}; }
+  __device__ void store(int b, WDead x) const { w[b] = x.w, d[b] = x.d; }
+  __device__ void totals(int64_t *t, WDead x) const { t[0] = (int64_t)x.w, t[1] = x.d; }
+};
+
+__global__ void __launch_bounds__(1024) k_mcmc_scan_blocks(int nb, McmcBlocks B, int64_t *__restrict__ totals) {
+  scan_blocks(nb, B, totals);
 }
 
 __global__ void __launch_bounds__(SC_THREADS) k_mcmc_weight_count(int64_t N, const float *__restrict__ alphas_raw,
                                                                    float alpha_raw_min, int mode,
-                                                                   uint64_t *__restrict__ block_w,
-                                                                   int32_t *__restrict__ block_dead) {
-  __shared__ uint64_t red_w[SC_THREADS / 32];
-  __shared__ uint32_t red_d[SC_THREADS / 32];
-  uint64_t w = 0;
-  uint32_t d = 0;
+                                                                   const McmcBlocks blocks) {
+  __shared__ WDead red[SC_THREADS / 32];
+  WDead n{0, 0};
 #pragma unroll
   for (int j = 0; j < SC_PER; j++) {
     const int64_t i = (int64_t)blockIdx.x * SC_ROWS + j * SC_THREADS + threadIdx.x;
     if (i < N) {
       bool dd;
-      w += mcmc_weight(alphas_raw[i], alpha_raw_min, mode, dd);
-      d += dd;
+      n.w += mcmc_weight(alphas_raw[i], alpha_raw_min, mode, dd);
+      n.d += dd;
     }
   }
-  w = warp_sum_u64(w);
-  d = __reduce_add_sync(0xffffffffu, d);
-  if ((threadIdx.x & 31) == 0) red_w[threadIdx.x >> 5] = w, red_d[threadIdx.x >> 5] = d;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint64_t a = 0;
-    uint32_t b = 0;
-#pragma unroll
-    for (int k = 0; k < SC_THREADS / 32; k++) a += red_w[k], b += red_d[k];
-    block_w[blockIdx.x] = a;
-    block_dead[blockIdx.x] = (int32_t)b;
-  }
-}
-
-// in place: block sums -> the sums before each CTA; totals = (W_total, dead count)
-__global__ void __launch_bounds__(1024) k_mcmc_scan_blocks(int nb, uint64_t *__restrict__ block_w,
-                                                           int32_t *__restrict__ block_dead,
-                                                           int64_t *__restrict__ totals) {
-  __shared__ uint64_t tot_w[32];
-  __shared__ int tot_d[32];
-  __shared__ uint64_t carry_w;
-  __shared__ int carry_d;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry_w = 0, carry_d = 0;
-  __syncthreads();
-  for (int base = 0; base < nb; base += 1024) {
-    const int b = base + threadIdx.x;
-    const uint64_t vw = b < nb ? block_w[b] : 0;
-    const int vd = b < nb ? block_dead[b] : 0;
-    uint64_t iw = vw;
-    int id = vd;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint64_t yw = __shfl_up_sync(0xffffffffu, iw, o);
-      const int yd = __shfl_up_sync(0xffffffffu, id, o);
-      if (lane >= o) iw += yw, id += yd;
-    }
-    if (lane == 31) tot_w[wid] = iw, tot_d[wid] = id;
-    __syncthreads();
-    uint64_t ew = carry_w + iw - vw;
-    int ed = carry_d + id - vd;
-    for (int k = 0; k < wid; k++) ew += tot_w[k], ed += tot_d[k];
-    if (b < nb) block_w[b] = ew, block_dead[b] = ed;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_w = ew + vw, carry_d = ed + vd;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) totals[0] = (int64_t)carry_w, totals[1] = carry_d;
+  n = cta_sum<SC_THREADS>(n, red);
+  if (threadIdx.x == 0) blocks.store(blockIdx.x, n);
 }
 
 __global__ void __launch_bounds__(SC_THREADS) k_mcmc_prefix(int64_t N, const float *__restrict__ alphas_raw,
-                                                             float alpha_raw_min, int mode,
-                                                             const uint64_t *__restrict__ block_w,
-                                                             const int32_t *__restrict__ block_dead,
+                                                             float alpha_raw_min, int mode, const McmcBlocks blocks,
                                                              uint64_t *__restrict__ W, int32_t *__restrict__ dead,
                                                              int32_t *__restrict__ count) {
-  __shared__ uint64_t tot_w[SC_THREADS / 32];
-  __shared__ uint32_t tot_d[SC_THREADS / 32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  __shared__ WDead warp_tot[SC_THREADS / 32];
   const int64_t row0 = (int64_t)blockIdx.x * SC_ROWS + (int64_t)threadIdx.x * SC_PER;
-  uint64_t w[SC_PER], sw = 0;
+  uint64_t w[SC_PER];
   bool dd[SC_PER];
-  uint32_t sd = 0;
+  WDead n{0, 0};
 #pragma unroll
   for (int j = 0; j < SC_PER; j++) {
     w[j] = 0, dd[j] = false;
     if (row0 + j < N) w[j] = mcmc_weight(alphas_raw[row0 + j], alpha_raw_min, mode, dd[j]);
-    sw += w[j], sd += dd[j];
+    n.w += w[j], n.d += dd[j];
   }
-  uint64_t iw = sw;
-  uint32_t id = sd;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint64_t a = __shfl_up_sync(0xffffffffu, iw, o);
-    const uint32_t b = __shfl_up_sync(0xffffffffu, id, o);
-    if (lane >= o) iw += a, id += b;
-  }
-  if (lane == 31) tot_w[wid] = iw, tot_d[wid] = id;
-  __syncthreads();
-  uint64_t rw = block_w[blockIdx.x] + iw - sw;
-  int rd = block_dead[blockIdx.x] + (int)(id - sd);
-  for (int k = 0; k < wid; k++) rw += tot_w[k], rd += (int)tot_d[k];
+  WDead total;
+  const WDead before = blocks.load(blockIdx.x) + cta_exclusive_scan<SC_THREADS>(n, warp_tot, total);
+  uint64_t rw = before.w;
+  int rd = before.d;
 #pragma unroll
   for (int j = 0; j < SC_PER; j++) {
     const int64_t i = row0 + j;
@@ -767,17 +705,6 @@ __global__ void k_mcmc_values(int64_t n, const int32_t *__restrict__ sampled, co
   vals[j] = relocation_value(alphas_raw[i], scales_raw + 3 * i, count[i], min_opacity, n_max);
 }
 
-// One more per-Gaussian tensor [N, D] and its Adam moments (m, v: both or neither) for the
-// row-moving kernels below; the six training tensors are jobs 0-5 (kWidth), an extra tensor job 6.
-struct McmcJob {
-  const float *p, *m, *v;  // sources
-  float *dp, *dm, *dv;     // destinations (grow: fresh [N + n] tensors; relocate: the sources)
-  int w;
-};
-struct McmcJobs {
-  McmcJob j[6];
-};
-
 // the value a sampled source row gets at column c (alphas_raw, scales_raw: the relocation value)
 template <int A>
 __device__ __forceinline__ float source_value(const float *__restrict__ p, int64_t src, int c, int w,
@@ -794,7 +721,7 @@ __device__ __forceinline__ float source_value(const float *__restrict__ p, int64
 template <int A>
 __device__ __forceinline__ void relocate_job(int64_t n, const int32_t *__restrict__ sampled,
                                              const int32_t *__restrict__ dead, const float4 *__restrict__ vals,
-                                             const McmcJob &J) {
+                                             const Job &J) {
   const int w = A < 6 ? kWidth[A < 6 ? A : 0] : J.w;
   const int64_t total = n * w, stride = (int64_t)gridDim.x * blockDim.x;
   float *__restrict__ p = J.dp;
@@ -817,7 +744,7 @@ __device__ __forceinline__ void relocate_job(int64_t n, const int32_t *__restric
 __global__ void __launch_bounds__(256) k_mcmc_relocate(int64_t n, const int32_t *__restrict__ sampled,
                                                        const int32_t *__restrict__ dead,
                                                        const float4 *__restrict__ vals,
-                                                       const __grid_constant__ McmcJobs J) {
+                                                       const __grid_constant__ Jobs J) {
   switch (blockIdx.y) {
     case 0: relocate_job<0>(n, sampled, dead, vals, J.j[0]); break;
     case 1: relocate_job<1>(n, sampled, dead, vals, J.j[1]); break;
@@ -830,7 +757,7 @@ __global__ void __launch_bounds__(256) k_mcmc_relocate(int64_t n, const int32_t 
 
 __global__ void __launch_bounds__(256) k_mcmc_relocate_rows(int64_t n, const int32_t *__restrict__ sampled,
                                                             const int32_t *__restrict__ dead,
-                                                            const __grid_constant__ McmcJob J) {
+                                                            const __grid_constant__ Job J) {
   relocate_job<6>(n, sampled, dead, nullptr, J);
 }
 
@@ -838,7 +765,7 @@ __global__ void __launch_bounds__(256) k_mcmc_relocate_rows(int64_t n, const int
 // gets zero moments.  blockIdx.y = the set (parameter, exp_avg, exp_avg_sq); four independent
 // elements in flight per thread.
 template <int A>
-__device__ __forceinline__ void grow_copy_job(int64_t N, const int32_t *__restrict__ count, const McmcJob &J,
+__device__ __forceinline__ void grow_copy_job(int64_t N, const int32_t *__restrict__ count, const Job &J,
                                               int set) {
   const int w = A < 6 ? kWidth[A < 6 ? A : 0] : J.w;
   const float *__restrict__ src = set == 0 ? J.p : (set == 1 ? J.m : J.v);
@@ -863,7 +790,7 @@ __device__ __forceinline__ void grow_copy_job(int64_t N, const int32_t *__restri
 }
 
 __global__ void __launch_bounds__(256) k_mcmc_grow_copy(int64_t N, const int32_t *__restrict__ count,
-                                                        const __grid_constant__ McmcJobs J) {
+                                                        const __grid_constant__ Jobs J) {
   const int set = blockIdx.y % 3;
   switch (blockIdx.y / 3) {
     case 0: grow_copy_job<0>(N, count, J.j[0], set); break;
@@ -879,7 +806,7 @@ __global__ void __launch_bounds__(256) k_mcmc_grow_copy(int64_t N, const int32_t
 // moments, and the source row itself gets the relocation value
 template <int A>
 __device__ __forceinline__ void grow_append_job(int64_t N, int64_t n, const int32_t *__restrict__ sampled,
-                                                const float4 *__restrict__ vals, const McmcJob &J) {
+                                                const float4 *__restrict__ vals, const Job &J) {
   const int w = A < 6 ? kWidth[A < 6 ? A : 0] : J.w;
   const int64_t total = n * w, stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += stride) {
@@ -897,7 +824,7 @@ __device__ __forceinline__ void grow_append_job(int64_t N, int64_t n, const int3
 
 __global__ void __launch_bounds__(256) k_mcmc_grow_append(int64_t N, int64_t n, const int32_t *__restrict__ sampled,
                                                           const float4 *__restrict__ vals,
-                                                          const __grid_constant__ McmcJobs J) {
+                                                          const __grid_constant__ Jobs J) {
   switch (blockIdx.y) {
     case 0: grow_append_job<0>(N, n, sampled, vals, J.j[0]); break;
     case 1: grow_append_job<1>(N, n, sampled, vals, J.j[1]); break;
@@ -910,7 +837,7 @@ __global__ void __launch_bounds__(256) k_mcmc_grow_append(int64_t N, int64_t n, 
 
 __global__ void __launch_bounds__(256) k_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *__restrict__ count,
                                                         const int32_t *__restrict__ sampled,
-                                                        const __grid_constant__ McmcJob J, int part) {
+                                                        const __grid_constant__ Job J, int part) {
   if (part == 0) grow_copy_job<6>(N, count, J, blockIdx.y);
   else if (blockIdx.y == 0) grow_append_job<6>(N, n, sampled, nullptr, J);
 }
@@ -994,8 +921,8 @@ int launch_density_plan(int64_t N, const float *alphas_raw, const float *scales_
   }
   {
     ProfScope ps(K_DENSITY_SCAN, st);
-    k_density_scan_blocks<<<1, 1024, 0, st>>>(nb, block_counts, totals);
-    k_density_slots<<<nb, SC_THREADS, 0, st>>>(N, cls, block_counts, reinterpret_cast<Slot3 *>(slots));
+    k_density_scan_blocks<<<1, 1024, 0, st>>>(nb, DensityBlocks{block_counts}, totals);
+    k_density_slots<<<nb, SC_THREADS, 0, st>>>(N, cls, DensityBlocks{block_counts}, reinterpret_cast<Slot3 *>(slots));
     GSB_CUDA_TRY(cudaGetLastError());
   }
   GSB_CUDA_TRY(cudaMemcpyAsync(counts_host, totals, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
@@ -1007,30 +934,15 @@ int launch_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, in
                          float *const *src, float *const *src_m, float *const *src_v, const float *z,
                          float *const *dst, float *const *dst_m, float *const *dst_v, cudaStream_t st) {
   if (N == 0) return 0;
-  Sets S;
-  for (int a = 0; a < 6; a++) {
-    S.p[a] = src[a];
-    S.m[a] = src_m ? src_m[a] : nullptr;
-    S.v[a] = src_v ? src_v[a] : nullptr;
-    S.dp[a] = dst[a];
-    S.dm[a] = dst_m ? dst_m[a] : nullptr;
-    S.dv[a] = dst_v ? dst_v[a] : nullptr;
-  }
   ProfScope ps(K_DENSITY_APPLY, st);
-  if (N < 23000000) {  // row groups; the per-element kernel below takes the 64-bit indices of larger N
-    int dev = 0, sms = 132;
-    GSB_CUDA_TRY(cudaGetDevice(&dev));
-    GSB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const int64_t blocks = (N + 32 * DG_WARPS - 1) / (32 * DG_WARPS);
-    const int grid_x = (int)(blocks < (int64_t)sms * 8 ? blocks : (int64_t)sms * 8);
-    const dim3 grid(grid_x, 18);
-    const Slot3 *sl = reinterpret_cast<const Slot3 *>(slots);
-    k_density_apply_rows<<<grid, 32 * DG_WARPS, 0, st>>>((int)N, cls, sl, (int)K, (int)C, S, z);
-    GSB_CUDA_TRY(cudaGetLastError());
-    return 0;
-  }
-  dim3 grid(stream_grid((N * 45 + 3) / 4, 256), 18);
-  k_density_apply<<<grid, 256, 0, st>>>(N, cls, reinterpret_cast<const Slot3 *>(slots), K, C, S, z);
+  int dev = 0, sms = 132;
+  GSB_CUDA_TRY(cudaGetDevice(&dev));
+  GSB_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int64_t blocks = (N + 32 * DG_WARPS - 1) / (32 * DG_WARPS);
+  const dim3 grid((int)(blocks < (int64_t)sms * 8 ? blocks : (int64_t)sms * 8), 18);
+  auto *kernel = N < 23000000 ? k_density_apply_rows<uint32_t> : k_density_apply_rows<size_t>;
+  kernel<<<grid, 32 * DG_WARPS, 0, st>>>((int)N, cls, reinterpret_cast<const Slot3 *>(slots), (int)K, (int)C,
+                                         jobs(src, src_m, src_v, dst, dst_m, dst_v), z);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -1092,14 +1004,13 @@ int launch_mcmc_plan(int64_t N, const float *alphas_raw, float alpha_raw_min, in
   const McmcLayout L = mcmc_layout(N, 0);
   char *b = static_cast<char *>(ws);
   int64_t *totals = reinterpret_cast<int64_t *>(b);
-  uint64_t *block_w = reinterpret_cast<uint64_t *>(b + L.block_w);
-  int32_t *block_dead = reinterpret_cast<int32_t *>(b + L.block_dead);
+  const McmcBlocks blocks{reinterpret_cast<uint64_t *>(b + L.block_w), reinterpret_cast<int32_t *>(b + L.block_dead)};
   const int nb = (int)((N + SC_ROWS - 1) / SC_ROWS);
   {
     ProfScope ps(K_MCMC_SCAN, st);
-    k_mcmc_weight_count<<<nb, SC_THREADS, 0, st>>>(N, alphas_raw, alpha_raw_min, mode, block_w, block_dead);
-    k_mcmc_scan_blocks<<<1, 1024, 0, st>>>(nb, block_w, block_dead, totals);
-    k_mcmc_prefix<<<nb, SC_THREADS, 0, st>>>(N, alphas_raw, alpha_raw_min, mode, block_w, block_dead,
+    k_mcmc_weight_count<<<nb, SC_THREADS, 0, st>>>(N, alphas_raw, alpha_raw_min, mode, blocks);
+    k_mcmc_scan_blocks<<<1, 1024, 0, st>>>(nb, blocks, totals);
+    k_mcmc_prefix<<<nb, SC_THREADS, 0, st>>>(N, alphas_raw, alpha_raw_min, mode, blocks,
                                              reinterpret_cast<uint64_t *>(b + L.W),
                                              reinterpret_cast<int32_t *>(b + L.dead),
                                              reinterpret_cast<int32_t *>(b + L.count));
@@ -1133,15 +1044,6 @@ static int launch_mcmc_values(int64_t N, int64_t n, const int32_t *sampled, void
   return 0;
 }
 
-static McmcJobs mcmc_jobs(float *const *src, float *const *src_m, float *const *src_v, float *const *dst,
-                          float *const *dst_m, float *const *dst_v) {
-  McmcJobs J;
-  for (int a = 0; a < 6; a++)
-    J.j[a] = McmcJob{src[a], src_m ? src_m[a] : nullptr, src_v ? src_v[a] : nullptr, dst[a],
-                     dst_m ? dst_m[a] : nullptr, dst_v ? dst_v[a] : nullptr, kWidth[a]};
-  return J;
-}
-
 int launch_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws, double min_opacity, int n_max,
                          float *const *p, float *const *m, float *const *v, cudaStream_t st) {
   if (n == 0) return 0;
@@ -1151,7 +1053,7 @@ int launch_mcmc_relocate(int64_t N, int64_t n, const int32_t *sampled, void *ws,
   char *b = static_cast<char *>(ws);
   const dim3 grid(stream_grid(n * 45, 256), 6);
   k_mcmc_relocate<<<grid, 256, 0, st>>>(n, sampled, reinterpret_cast<const int32_t *>(b + L.dead),
-                                        reinterpret_cast<const float4 *>(b + L.vals), mcmc_jobs(p, m, v, p, m, v));
+                                        reinterpret_cast<const float4 *>(b + L.vals), jobs(p, m, v, p, m, v));
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -1161,7 +1063,7 @@ int launch_mcmc_relocate_rows(int64_t N, int64_t n, const int32_t *sampled, cons
   if (n == 0) return 0;
   ProfScope ps(K_MCMC_ROWS, st);
   const McmcLayout L = mcmc_layout(N, 0);
-  const McmcJob J{x, m, v, x, m, v, D};
+  const Job J{x, m, v, x, m, v, D};
   k_mcmc_relocate_rows<<<stream_grid(n * D, 256), 256, 0, st>>>(
       n, sampled, reinterpret_cast<const int32_t *>(static_cast<const char *>(ws) + L.dead), J);
   GSB_CUDA_TRY(cudaGetLastError());
@@ -1175,7 +1077,7 @@ int launch_mcmc_grow(int64_t N, int64_t n, const int32_t *sampled, void *ws, dou
   ProfScope ps(K_MCMC_GROW, st);
   const McmcLayout L = mcmc_layout(N, n);
   char *b = static_cast<char *>(ws);
-  const McmcJobs J = mcmc_jobs(src, src_m, src_v, dst, dst_m, dst_v);
+  const Jobs J = jobs(src, src_m, src_v, dst, dst_m, dst_v);
   const dim3 grid(stream_grid((N * 45 + 3) / 4, 256), 18);
   k_mcmc_grow_copy<<<grid, 256, 0, st>>>(N, reinterpret_cast<const int32_t *>(b + L.count), J);
   GSB_CUDA_TRY(cudaGetLastError());
@@ -1194,7 +1096,7 @@ int launch_mcmc_grow_rows(int64_t N, int64_t n, const int32_t *sampled, const vo
   ProfScope ps(K_MCMC_ROWS, st);
   const McmcLayout L = mcmc_layout(N, 0);
   const int32_t *count = reinterpret_cast<const int32_t *>(static_cast<const char *>(ws) + L.count);
-  const McmcJob J{src, src_m, src_v, dst, dst_m, dst_v, D};
+  const Job J{src, src_m, src_v, dst, dst_m, dst_v, D};
   k_mcmc_grow_rows<<<dim3(stream_grid((N * D + 3) / 4, 256), 3), 256, 0, st>>>(N, n, count, sampled, J, 0);
   GSB_CUDA_TRY(cudaGetLastError());
   if (n == 0) return 0;

@@ -51,12 +51,86 @@ def gaussians_struct(tensors):
     return g, keep
 
 
-def check_params(params, what="params"):
+def _structs(*dicts):
+    """-> (C.byref gsb_gaussians of each dict of the six tensors, None for None; keep-alive list)"""
+    structs, keep = [], []
+    for d in dicts:
+        if d is None:
+            structs.append(None)
+        else:
+            g, ka = gaussians_struct(d)
+            keep.append((g, ka))
+            structs.append(C.byref(g))
+    return structs, keep
+
+
+def _copy(t, name, shape):
+    """a checked contiguous float32 CUDA view of `shape` (a copy if `t` is not contiguous)"""
+    return _check(t.detach(), name, shape)
+
+
+def _in_place(t, name, shape):
+    """the tensor itself (contiguous float32 CUDA of `shape`): the kernels write through its pointer"""
+    c = _check(t.detach(), name, shape)
+    if c.data_ptr() != t.data_ptr():
+        raise ValueError("%s must be contiguous (it is updated in place)" % name)
+    return c
+
+
+def gather_state(params, optimizer, extra, take):
+    """checked (N, tensors, Adam moments m / v or None, groups) of the six tensors and the [N, D]
+    `extra` entries of `params`; take: _copy or _in_place.  The moments are those of the optimizer
+    groups named after the tensors, for all of them or for none."""
     N = params["pws"].shape[0]
-    out = {}
+    src = {}
     for k, w in zip(GAUSSIAN_TENSORS, GAUSSIAN_WIDTHS):
-        out[k] = _check(params[k].detach(), "%s[%r]" % (what, k), (N, w))
-    return N, out
+        src[k] = take(params[k], "params[%r]" % k, (N, w))
+    for k in extra:
+        if k in GAUSSIAN_TENSORS:
+            raise ValueError("extra names a built-in tensor: %r" % (k,))
+        t = params[k]
+        if not (isinstance(t, torch.Tensor) and t.dim() == 2 and t.shape[0] == N and t.shape[1] >= 1):
+            raise ValueError("params[%r] must be [N, D] with N = %d and D >= 1" % (k, N))
+        src[k] = take(t, "params[%r]" % (k,), tuple(t.shape))
+    groups = {g["name"]: g for g in optimizer.param_groups}
+    names = GAUSSIAN_TENSORS + tuple(extra)
+    missing = [k for k in names if k not in groups]
+    if missing:
+        raise ValueError("the optimizer has no param group named %s" % ", ".join(map(repr, missing)))
+    states = {k: optimizer.state.get(groups[k]["params"][0], None) for k in names}
+    have = [s is not None and "exp_avg" in s for s in states.values()]
+    if any(have) and not all(have):
+        raise ValueError("optimizer state must exist for all groups or for none")
+    m = v = None
+    if all(have):
+        m = {k: take(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape) for k in names}
+        v = {k: take(states[k]["exp_avg_sq"], "exp_avg_sq[%r]" % k, src[k].shape) for k in names}
+    return N, src, m, v, groups
+
+
+def swap_parameters(params, optimizer, groups, dst, dst_m, dst_v):
+    """params[k] and the optimizer group k become a new Parameter of dst[k] for every k in dst; the
+    group's optimizer state moves to it with the moments dst_m[k] / dst_v[k] (none without them)"""
+    for k in dst:
+        group = groups[k]
+        old = group["params"][0]
+        new = torch.nn.Parameter(dst[k].requires_grad_(True))
+        st = optimizer.state.pop(old, None)
+        if st is not None and dst_m is not None:
+            st["exp_avg"], st["exp_avg_sq"] = dst_m[k], dst_v[k]
+            optimizer.state[new] = st
+        group["params"][0] = new
+        params[k] = new
+
+
+def report(verbose, title, rows):
+    """the reference's printed report: "gaussian <title> report", then "<name>:  <value>" rows"""
+    if verbose:
+        print("---------------------")
+        print("gaussian %s report" % title)
+        for name, val in rows:
+            print("%s: " % name, val)
+        print("---------------------")
 
 
 def raw_thresholds(sense_size, alpha_threshold=0.005, grad_threshold=4e-7):
@@ -107,16 +181,7 @@ def apply(cls, slots, counts, src, src_m, src_v, z):
     dst = fresh()
     state = src_m is not None
     dst_m, dst_v = (fresh(), fresh()) if state else (None, None)
-    keep = []
-    structs = []
-    for d in (src, src_m, src_v, dst, dst_m, dst_v):
-        if d is None:
-            structs.append(None)
-        else:
-            g, ka = gaussians_struct(d)
-            keep.append(ka)
-            structs.append(C.byref(g))
-            keep.append(g)
+    structs, keep = _structs(src, src_m, src_v, dst, dst_m, dst_v)
     _lib.check(lib.gsb_density_apply(N, _ptr(cls), _ptr(slots), K, Cn, S, structs[0], structs[1], structs[2], _ptr(z),
                                      structs[3], structs[4], structs[5], _stream()), lib)
     return dst, dst_m, dst_v
@@ -179,62 +244,23 @@ class DensityController:
         moments) by gsb_density_apply_rows.  extra=() is exactly the six-tensor update."""
         if self.cunt is None:
             raise RuntimeError("update_gaussian_density needs at least one update_density_info call")
-        N, src = check_params(params)
         extra = tuple(extra)
-        for k in extra:
-            if k in GAUSSIAN_TENSORS:
-                raise ValueError("extra names a built-in tensor: %r" % (k,))
-            t = params[k]
-            if not (isinstance(t, torch.Tensor) and t.dim() == 2 and t.shape[0] == N and t.shape[1] >= 1):
-                raise ValueError("params[%r] must be [N, D] with N = %d and D >= 1" % (k, N))
-            src[k] = _check(t.detach(), "params[%r]" % (k,), tuple(t.shape))
-        groups = {g["name"]: g for g in optimizer.param_groups}
-        names = GAUSSIAN_TENSORS + extra
-        missing = [k for k in names if k not in groups]
-        if missing:
-            raise ValueError("the optimizer has no param group named %s" % ", ".join(map(repr, missing)))
-        states = {k: optimizer.state.get(groups[k]["params"][0], None) for k in names}
-        have = [s is not None and "exp_avg" in s for s in states.values()]
-        if any(have) and not all(have):
-            raise ValueError("optimizer state must exist for all groups or for none")
-        src_m = src_v = None
-        if all(have):
-            src_m = {k: _check(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape) for k in GAUSSIAN_TENSORS}
-            src_v = {k: _check(states[k]["exp_avg_sq"], "exp_avg_sq[%r]" % k, src[k].shape) for k in GAUSSIAN_TENSORS}
+        N, src, src_m, src_v, groups = gather_state(params, optimizer, extra, _copy)
         cls, slots, (K, Cn, S) = plan(src["alphas_raw"], src["scales_raw"], self.grad_accum, self.cunt, self.th)
         # the reference's torch.normal(mean=zeros(S,3), std=scales[split]) (:276-277)
         z = torch.empty((S, 3), dtype=torch.float32, device=src["pws"].device).normal_(0, 1, generator=generator)
         dst, dst_m, dst_v = apply(cls, slots, (K, Cn, S), src, src_m, src_v, z)
         for k in extra:
-            m = v = None
-            if src_m is not None:
-                m = _check(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape)
-                v = _check(states[k]["exp_avg_sq"], "exp_avg_sq[%r]" % k, src[k].shape)
-            dst[k], dm, dv = apply_rows(cls, slots, (K, Cn, S), src[k], m, v)
+            dst[k], dm, dv = apply_rows(cls, slots, (K, Cn, S), src[k], src_m[k] if src_m else None,
+                                        src_v[k] if src_v else None)
             if dst_m is not None:
                 dst_m[k], dst_v[k] = dm, dv
-        for k in names:
-            group = groups[k]
-            old = group["params"][0]
-            new = torch.nn.Parameter(dst[k].requires_grad_(True))
-            st = optimizer.state.pop(old, None)
-            if st is not None and dst_m is not None:
-                st["exp_avg"], st["exp_avg_sq"] = dst_m[k], dst_v[k]
-                optimizer.state[new] = st
-            group["params"][0] = new
-            params[k] = new
-        report = dict(pruned=N - K, cloned=Cn, splited=S, total=K + Cn + S)
-        if self.verbose:
-            print("---------------------")
-            print("gaussian density update report")
-            print("pruned num: ", report["pruned"])
-            print("cloned num: ", report["cloned"])
-            print("splited num: ", report["splited"])
-            print("total gaussian number: ", report["total"])
-            print("---------------------")
+        swap_parameters(params, optimizer, groups, dst, dst_m, dst_v)
+        report(self.verbose, "density update", [("pruned num", N - K), ("cloned num", Cn), ("splited num", S),
+                                                ("total gaussian number", K + Cn + S)])
         self.grad_accum = None
         self.cunt = None
-        return report
+        return dict(pruned=N - K, cloned=Cn, splited=S, total=K + Cn + S)
 
     @torch.no_grad()
     def reset_alpha(self, params, optimizer):
@@ -280,14 +306,6 @@ def mcmc_sample(ws, N, u):
     return sampled
 
 
-def _in_place(t, name, shape):
-    """the tensor itself (contiguous float32 CUDA of `shape`): the kernels write through its pointer"""
-    c = _check(t.detach(), name, shape)
-    if c.data_ptr() != t.data_ptr():
-        raise ValueError("%s must be contiguous (it is updated in place)" % name)
-    return c
-
-
 class MCMCController:
     """MCMC densification (Kheradmand et al., "3D Gaussian Splatting as Markov Chain Monte Carlo",
     2024; gsplat's MCMCStrategy): at most `cap_max` Gaussians, dead ones (opacity <= min_opacity)
@@ -320,43 +338,6 @@ class MCMCController:
         # the fp32 logit the kernels compare alphas_raw with, as raw_thresholds computes it
         self.alpha_raw_min = float(np.float32(np.log(self.min_opacity / (1 - self.min_opacity))))
 
-    def _state(self, params, optimizer, extra, in_place):
-        """checked (N, tensors, moments m / v or None, groups) for the six tensors and `extra`"""
-        N = params["pws"].shape[0]
-        take = _in_place if in_place else (lambda t, name, shape: _check(t.detach(), name, shape))
-        src = {}
-        for k, w in zip(GAUSSIAN_TENSORS, GAUSSIAN_WIDTHS):
-            src[k] = take(params[k], "params[%r]" % k, (N, w))
-        for k in extra:
-            if k in GAUSSIAN_TENSORS:
-                raise ValueError("extra names a built-in tensor: %r" % (k,))
-            t = params[k]
-            if not (isinstance(t, torch.Tensor) and t.dim() == 2 and t.shape[0] == N and t.shape[1] >= 1):
-                raise ValueError("params[%r] must be [N, D] with N = %d and D >= 1" % (k, N))
-            src[k] = take(t, "params[%r]" % (k,), tuple(t.shape))
-        groups = {g["name"]: g for g in optimizer.param_groups}
-        names = GAUSSIAN_TENSORS + tuple(extra)
-        missing = [k for k in names if k not in groups]
-        if missing:
-            raise ValueError("the optimizer has no param group named %s" % ", ".join(map(repr, missing)))
-        states = {k: optimizer.state.get(groups[k]["params"][0], None) for k in names}
-        have = [s is not None and "exp_avg" in s for s in states.values()]
-        if any(have) and not all(have):
-            raise ValueError("optimizer state must exist for all groups or for none")
-        m = v = None
-        if all(have):
-            m = {k: take(states[k]["exp_avg"], "exp_avg[%r]" % k, src[k].shape) for k in names}
-            v = {k: take(states[k]["exp_avg_sq"], "exp_avg_sq[%r]" % k, src[k].shape) for k in names}
-        return N, src, m, v, groups
-
-    def _report(self, title, rows):
-        if self.verbose:
-            print("---------------------")
-            print("gaussian %s report" % title)
-            for name, val in rows:
-                print("%s: " % name, val)
-            print("---------------------")
-
     @torch.no_grad()
     def relocate(self, params, optimizer, generator=None, extra=()):
         """Moves every dead Gaussian (!(alphas_raw > logit(min_opacity)), NaN included) onto a live
@@ -367,7 +348,7 @@ class MCMCController:
         SYNCHRONISATION: one read of the dead count.  -> dict(relocated, total)"""
         lib = _lib.load()
         extra = tuple(extra)
-        N, src, m, v, _ = self._state(params, optimizer, extra, in_place=True)
+        N, src, m, v, _ = gather_state(params, optimizer, extra, _in_place)
         n = 0
         if N:
             ws, w_total, n = mcmc_plan(src["alphas_raw"], self.alpha_raw_min, MCMC_RELOCATE, N)
@@ -376,19 +357,15 @@ class MCMCController:
         if n:
             u = torch.rand(n, dtype=torch.float64, device=src["pws"].device, generator=generator)
             sampled = mcmc_sample(ws, N, u)
-            g, keep = gaussians_struct(src)
-            gm, keep_m = gaussians_struct(m) if m is not None else (None, None)
-            gv, keep_v = gaussians_struct(v) if m is not None else (None, None)
+            structs, keep = _structs(src, m, v)
             _lib.check(lib.gsb_mcmc_relocate(N, n, _ptr(sampled), _ptr(ws), ws.numel(), self.min_opacity, self.n_max,
-                                             C.byref(g), C.byref(gm) if gm is not None else None,
-                                             C.byref(gv) if gv is not None else None, _stream()), lib)
+                                             *structs, _stream()), lib)
             for k in extra:
                 _lib.check(lib.gsb_mcmc_relocate_rows(N, n, _ptr(sampled), _ptr(ws), ws.numel(), src[k].shape[1],
                                                       _ptr(src[k]), _ptr(m[k] if m else None),
                                                       _ptr(v[k] if v else None), _stream()), lib)
-        report = dict(relocated=n, total=N)
-        self._report("relocation", [("relocated num", n), ("total gaussian number", N)])
-        return report
+        report(self.verbose, "relocation", [("relocated num", n), ("total gaussian number", N)])
+        return dict(relocated=n, total=N)
 
     @torch.no_grad()
     def grow(self, params, optimizer, generator=None, extra=()):
@@ -401,7 +378,7 @@ class MCMCController:
         total.  -> dict(added, total)"""
         lib = _lib.load()
         extra = tuple(extra)
-        N, src, m, v, groups = self._state(params, optimizer, extra, in_place=False)
+        N, src, m, v, groups = gather_state(params, optimizer, extra, _copy)
         n = max(0, min(self.cap_max, int(N * (1.0 + self.grow_rate))) - N)
         if n:
             ws, w_total, _ = mcmc_plan(src["alphas_raw"], self.alpha_raw_min, MCMC_GROW, n)
@@ -415,14 +392,7 @@ class MCMCController:
             dst = {k: fresh(k) for k in src}
             dst_m = {k: fresh(k) for k in src} if m is not None else None
             dst_v = {k: fresh(k) for k in src} if m is not None else None
-            structs, keep = [], []
-            for d in (src, m, v, dst, dst_m, dst_v):
-                if d is None:
-                    structs.append(None)
-                else:
-                    g, ka = gaussians_struct(d)
-                    keep.append((g, ka))
-                    structs.append(C.byref(g))
+            structs, keep = _structs(src, m, v, dst, dst_m, dst_v)
             _lib.check(lib.gsb_mcmc_grow(N, n, _ptr(sampled), _ptr(ws), ws.numel(), self.min_opacity, self.n_max,
                                          *structs, _stream()), lib)
             for k in extra:
@@ -430,19 +400,9 @@ class MCMCController:
                 _lib.check(lib.gsb_mcmc_grow_rows(N, n, _ptr(sampled), _ptr(ws), ws.numel(), src[k].shape[1],
                                                   _ptr(src[k]), mk(m), mk(v), _ptr(dst[k]), mk(dst_m), mk(dst_v),
                                                   _stream()), lib)
-            for k in GAUSSIAN_TENSORS + extra:
-                group = groups[k]
-                old = group["params"][0]
-                new = torch.nn.Parameter(dst[k].requires_grad_(True))
-                st = optimizer.state.pop(old, None)
-                if st is not None and dst_m is not None:
-                    st["exp_avg"], st["exp_avg_sq"] = dst_m[k], dst_v[k]
-                    optimizer.state[new] = st
-                group["params"][0] = new
-                params[k] = new
-        report = dict(added=n, total=N + n)
-        self._report("growth", [("added num", n), ("total gaussian number", N + n)])
-        return report
+            swap_parameters(params, optimizer, groups, dst, dst_m, dst_v)
+        report(self.verbose, "growth", [("added num", n), ("total gaussian number", N + n)])
+        return dict(added=n, total=N + n)
 
     @torch.no_grad()
     def inject_noise(self, params, optimizer, generator=None):

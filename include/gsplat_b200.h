@@ -502,7 +502,8 @@ int gsb_density_plan(int64_t N, const float *alphas_raw, const float *scales_raw
  * normalize(rots_raw)); a split row moves pws by R(q) (z * exp(scales_raw)) with z[S,3] the
  * caller's unit normals (the reference draws torch.normal(0, std=scales) = z * std, :276-277)
  * and shrinks the NEW Gaussian's scale by 0.6 (the original keeps its size, :281-282).  New
- * rows get zero Adam moments.  src_m/src_v/dst_m/dst_v: NULL, or all four set. */
+ * rows get zero Adam moments.  src_m/src_v/dst_m/dst_v: NULL, or all four set.  N < 2^30
+ * (253 GB of parameters): a larger N is refused as bad counts. */
 int gsb_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C, int64_t S,
                       const gsb_gaussians *src, const gsb_gaussians *src_m, const gsb_gaussians *src_v,
                       const float *z, const gsb_gaussians *dst, const gsb_gaussians *dst_m,

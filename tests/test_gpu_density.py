@@ -173,9 +173,9 @@ def random_state_device(N, seed, sense=5.0):
 
 
 def test_apply_64bit_kernel_equals_row_group_slices():
-    """N = 23 000 037 takes the per-element kernel with 64-bit indices (all 18 parameter /
-    Adam-moment jobs, element offsets past 1e9 in high_shs); two row slices below 23 M take the
-    row-group kernel.  Classification is per row and slots are prefix sums, so each output row
+    """N = 23 000 037 takes the row-group kernel with 64-bit destination offsets (all 18 parameter
+    / Adam-moment jobs, element offsets past 1e9 in high_shs); two row slices below 23 M take its
+    32-bit instantiation.  Classification is per row and slots are prefix sums, so each output row
     of the full run has a known place in one slice's output: kept row k of slice 2 is full row
     K1 + k, its clones K + C1 + c, its splits K + C + S1 + s.  All rows must be bit-identical."""
     from easygaussiansplatting_b200 import density

@@ -205,8 +205,8 @@ def test_apply_row_group_edges(spec):
 
 
 def test_apply_per_element_kernel_without_state():
-    """N = 23 000 000, the smallest N the per-element kernel takes, without Adam moments (six
-    jobs).  Peak device memory: the parameters (236 B / row, 5.4 GB), the plan inputs and slots
+    """N = 23 000 000, the smallest N the row-group kernel takes with 64-bit destination offsets,
+    without Adam moments (six jobs).  Peak device memory: the parameters (236 B / row, 5.4 GB), the plan inputs and slots
     (25 B / row, 0.6 GB), the rebuilt parameters (<= 1.1 N rows, 6.0 GB) and one boolean gather
     of high_shs for the check (<= 4.1 GB): at most 16.1 GB, 13.9 GB with this seed on an H100."""
     from easygaussiansplatting_b200 import density

@@ -314,7 +314,7 @@ SC_THREADS, SC_PER = 256, 4
 SC_ROWS = SC_THREADS * SC_PER
 
 def warp_inclusive_scan(x, axis):
-    """the __shfl_up_sync ladder of both scan kernels along the 32-lane `axis`: a lane below the
+    """the __shfl_up_sync ladder of cta_exclusive_scan along the 32-lane `axis`: a lane below the
     offset keeps its value"""
     x = np.moveaxis(x, axis, -1)
     lane = np.arange(32)
@@ -324,50 +324,60 @@ def warp_inclusive_scan(x, axis):
         x = x + np.where(lane >= o, y, 0).astype(x.dtype)
     return np.moveaxis(x, -1, axis)
 
+def cta_exclusive_scan(x):
+    """cta_exclusive_scan on x [..., NT, F], one counter tuple per thread in thread order -> (the
+    sum over the threads before each one, the CTA total): the ladder per warp, then the earlier
+    warps' totals from shared memory"""
+    w = x.reshape(x.shape[:-2] + (x.shape[-2] // 32, 32, x.shape[-1]))
+    inc = warp_inclusive_scan(w, -2)
+    warp_tot = inc[..., 31, :]
+    before = inc - w + (np.cumsum(warp_tot, axis=-2, dtype=x.dtype) - warp_tot)[..., None, :]
+    return before.reshape(x.shape), warp_tot.sum(axis=-2, dtype=x.dtype)
+
+def class_count(c):
+    """class_count: class bytes -> (survivors | clones << 16, splits) [..., 2] uint32"""
+    return np.stack([(c != PRUNE).astype(np.uint32) + ((c == CLONE).astype(np.uint32) << 16),
+                     (c == SPLIT).astype(np.uint32)], axis=-1)
+
+def unpack(kcsp):
+    """the density block counts (survivors, clones, splits) of packed pairs [..., 2]"""
+    return np.stack([kcsp[..., 0] & 0xffff, kcsp[..., 0] >> 16, kcsp[..., 1]], axis=-1).astype(np.int64)
+
 def classify_count(cls, nb):
-    """k_density_classify_count's per-CTA counts, through its (survivors | clones << 16) packing"""
+    """k_density_classify_count: thread t counts rows t, t + 256, ... of its CTA; cta_sum of the
+    packed pairs (warp sums, then the warp totals)"""
     c = np.full(nb * SC_ROWS, PRUNE, np.uint8)
     c[:cls.size] = cls
-    c = c.reshape(nb, SC_ROWS)
-    kc = ((c != PRUNE).astype(np.uint32) + ((c == CLONE).astype(np.uint32) << 16)).sum(axis=1, dtype=np.uint32)
-    sp = (c == SPLIT).sum(axis=1, dtype=np.uint32)
-    return np.stack([kc & 0xffff, kc >> 16, sp], axis=1).astype(np.int32)
+    n = class_count(c.reshape(nb, SC_PER, SC_THREADS)).sum(axis=1, dtype=np.uint32)
+    warp = n.reshape(nb, SC_THREADS // 32, 32, 2).sum(axis=2, dtype=np.uint32)
+    return unpack(warp.sum(axis=1, dtype=np.uint32)).astype(np.int32)
 
 def scan_blocks(block_counts):
-    """k_density_scan_blocks: one 1024-thread CTA walks the counts 1024 CTAs at a time; within a
-    pass, warp scans + the earlier warps' totals; across passes, the carry"""
+    """k_density_scan_blocks (scan_blocks): one 1024-thread CTA walks the counters 1024 CTAs at a
+    time: cta_exclusive_scan within a pass, the carry across passes"""
     nb = block_counts.shape[0]
     out = block_counts.copy()
-    carry = np.zeros(3, np.int64)
+    carry = np.zeros(block_counts.shape[1], np.int64)
     tid = np.arange(1024)
     for base in range(0, nb, 1024):
         b = base + tid
         ok = b < nb
-        v = np.zeros((1024, 3), np.int64)
+        v = np.zeros((1024, block_counts.shape[1]), np.int64)
         v[ok] = block_counts[b[ok]]
-        inc = warp_inclusive_scan(v.reshape(32, 32, 3), 1).reshape(1024, 3)
-        warp_tot = inc.reshape(32, 32, 3)[:, 31]
-        before = carry + (np.cumsum(warp_tot, axis=0) - warp_tot)[tid >> 5]
-        c0 = before + inc - v
-        out[b[ok]] = c0[ok]
-        carry = c0[1023] + v[1023]
+        before, total = cta_exclusive_scan(v)
+        out[b[ok]] = (carry + before)[ok]
+        carry = carry + total
     return out, carry
 
 def slots_kernel(cls, block_offsets):
-    """k_density_slots: 4 consecutive rows per thread, a packed warp scan, the earlier warps'
-    totals and the CTA's offset from scan_blocks"""
+    """k_density_slots: 4 consecutive rows per thread, cta_exclusive_scan of the packed pairs and
+    the CTA's offset from scan_blocks"""
     nb = block_offsets.shape[0]
     c = np.full(nb * SC_ROWS, PRUNE, np.uint8)
     c[:cls.size] = cls
-    c = c.reshape(nb, SC_THREADS // 32, 32, SC_PER)
-    kc = ((c != PRUNE).astype(np.uint32) + ((c == CLONE).astype(np.uint32) << 16)).sum(axis=3, dtype=np.uint32)
-    sp = (c == SPLIT).sum(axis=3, dtype=np.uint32)
-    ikc, isp = warp_inclusive_scan(kc, -1), warp_inclusive_scan(sp, -1)
-    wkc, wsp = ikc[:, :, 31], isp[:, :, 31]
-    bkc = ikc - kc + (np.cumsum(wkc, axis=1, dtype=np.uint32) - wkc)[:, :, None]
-    bsp = isp - sp + (np.cumsum(wsp, axis=1, dtype=np.uint32) - wsp)[:, :, None]
-    off = block_offsets.astype(np.int64)[:, None, None, :]
-    run = np.stack([bkc & 0xffff, bkc >> 16, bsp], axis=-1).astype(np.int64) + off
+    c = c.reshape(nb, SC_THREADS, SC_PER)
+    before, _ = cta_exclusive_scan(class_count(c).sum(axis=2, dtype=np.uint32))
+    run = block_offsets.astype(np.int64)[:, None, :] + unpack(before)
     out = np.empty(c.shape + (3,), np.int64)
     for j in range(SC_PER):
         out[..., j, :] = run
