@@ -102,6 +102,12 @@ SIGNATURES = {
     "gsb_preprocess_backward_push": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 7 + [_i, _i, C.POINTER(_vp),
                                                                                           C.c_uint32, _vp]),
     "gsb_grad_reduce_broadcast": (_i, [_i, _i, _i, _i, C.POINTER(_vp), C.c_uint32, _vp]),
+    "gsb_surfel_preprocess_forward": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 7),
+    "gsb_surfel_preprocess_backward": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 8),
+    "gsb_splat_surfel_workspace_bytes": (_sz, [_i, _i, _i, _i64]),
+    "gsb_splat_surfel_render": (_i, [_i, _i, _i, _i64, C.c_uint32] + [_vp] * 5 + [_sz] + [_vp] * 9),
+    "gsb_splat_surfel_forward": (_i, [_i, _i, _i] + [_vp] * 4 + [_i64, C.c_uint32, _vp, _sz, _vp, _sz] + [_vp] * 10),
+    "gsb_splat_surfel_backward": (_i, [_i, _i, _i, _i64] + [_vp] * 10 + [_sz] + [_vp] * 2),
     "gsb_profile_enable": (None, [_i]),
     "gsb_profile_kernels": (_i, []),
     "gsb_profile_kernel_name": (C.c_char_p, [_i]),

@@ -44,7 +44,9 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
                                              "draw_features", "draw_backward_features", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
-                                             "mcmc_noise", "draw_backward_abs", "draw_backward_rgbd_abs",
+                                             "mcmc_noise", "surfel_forward", "draw_surfel",
+                                             "draw_surfel_backward", "surfel_backward", "draw_backward_abs",
+                                             "draw_backward_rgbd_abs",
                                              "adam", "draw_rgbd",
                                              "draw_backward_rgbd"};
 
@@ -721,6 +723,138 @@ int gsb_splat_backward_rgbd_abs(int H, int W, int N, int64_t P, const float *us,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
                              dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, dloss_dus_abs,
                              stream);
+}
+
+// ---- 2D Gaussian Splatting (surfel.cu, DESIGN 3.15)
+
+static int surfel_scene(const char *who, FusedScene &sc) {
+  sc.lens = nullptr;
+  if (sc.N < 0) return arg_error(who, "N < 0");
+  if (!sh_dim3_ok(sc.k3)) return arg_error(who, "shs.shape[1]/3 must be 1, 4, 9 or 16");
+  if (sc.N > 0 && !(sc.pws && sc.rots && sc.scales && sc.shs && sc.Rcw && sc.tcw && sc.twc))
+    return arg_error(who, "null pointer");
+  return 0;
+}
+
+int gsb_surfel_preprocess_forward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                  const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                  float fy, float cx, float cy, float width, float height, const float *alphas,
+                                  float *us, float *depths, int32_t *areas, float *colors, float *records,
+                                  gsb_stream_t stream) {
+  const char *who = "surfel_preprocess";
+  FusedScene sc{N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height, nullptr};
+  if (int rc = surfel_scene(who, sc)) return rc;
+  if (!aligned(records, 16)) return arg_error(who, "records misaligned");
+  if (N > 0 && !(alphas && us && depths && areas && colors && records)) return arg_error(who, "null pointer");
+  return launch_surfel_fwd(sc, alphas, us, depths, areas, colors, records, (cudaStream_t)stream);
+}
+
+int gsb_surfel_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                   const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                   float fy, float cx, float cy, float width, float height, const float *rows,
+                                   float *dloss_dpws, float *dloss_dshs, float *dloss_dalphas, float *dloss_dscales,
+                                   float *dloss_drots, float *dloss_dus, gsb_stream_t stream) {
+  const char *who = "surfel_preprocessB";
+  FusedScene sc{N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height, nullptr};
+  if (int rc = surfel_scene(who, sc)) return rc;
+  if (N > 0 && !(rows && dloss_dpws && dloss_dshs && dloss_dalphas && dloss_dscales && dloss_drots && dloss_dus))
+    return arg_error(who, "null pointer");
+  return launch_surfel_bwd(sc, rows, dloss_dpws, dloss_dshs, dloss_dalphas, dloss_dscales, dloss_drots, dloss_dus,
+                           (cudaStream_t)stream);
+}
+
+size_t gsb_splat_surfel_workspace_bytes(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).bytes; }
+
+// The surfel frame from the sort to the planes, shared by the exact (P) and the capacity (P_cap,
+// with `sr`: binned here first) entry points, as render_frame is for the colour frame.
+static int surfel_frame(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us, float *depths,
+                        int32_t *areas, const float *records, void *bin_ws, void *ws, size_t ws_bytes, float *image,
+                        int32_t *contrib, float *final_tau, int32_t *ranges, int32_t *gsid, float *depth_image,
+                        float *alpha_image, float *normal_image, const StatusRead *sr, cudaStream_t st) {
+  GSB_REQUIRE(image && contrib && final_tau && ranges && depth_image && alpha_image && normal_image,
+              "splat_surfel: null output");
+  GSB_REQUIRE(aligned(image, 16) && aligned(contrib, 16) && aligned(final_tau, 16) && aligned(depth_image, 16) &&
+                  aligned(alpha_image, 16) && aligned(normal_image, 16) && aligned(ranges, 8),
+              "splat_surfel: misaligned output");
+  GSB_REQUIRE(aligned(records, 16), "splat_surfel: records misaligned");
+  GSB_REQUIRE(aligned(ws, 16), "splat_surfel: ws misaligned");
+  const SortLayout SL = sort_layout(N, H, W, P);
+  GSB_REQUIRE(ws != nullptr && ws_bytes >= SL.bytes, "splat_surfel: workspace too small");
+  const BinLayout BL = bin_layout(N);
+  int rc = sr ? launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st) : 0;
+  if (rc) return rc;
+  rc = launch_sort_and_pack(H, W, N, P, depth_key_max, us, nullptr, nullptr, depths, nullptr, bin_ws, BL, ws, SL,
+                            ranges, gsid, false, sr, st);
+  if (rc) return rc;
+  char *b = static_cast<char *>(ws);
+  return launch_draw_surfel(H, W, ranges, P > 0 && N > 0 ? records : nullptr, gsid, image, contrib, final_tau,
+                            depth_image, alpha_image, normal_image, reinterpret_cast<int *>(b + SL.counters), st);
+}
+
+int gsb_splat_surfel_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                            const float *depths, const float *records, const void *bin_ws, void *ws, size_t ws_bytes,
+                            float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                            int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
+                            gsb_stream_t stream) {
+  int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
+  if (rc) return rc;
+  GSB_REQUIRE(P >= 0, "splat_surfel: bad P");
+  GSB_REQUIRE(P == 0 || (us && depths && records && bin_ws && ws && gsid_per_patch), "splat_surfel: null pointer");
+  return surfel_frame(H, W, N, P, depth_key_max, us, const_cast<float *>(depths), nullptr, records,
+                      const_cast<void *>(bin_ws), ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
+                      gsid_per_patch, depth_image, alpha_image, normal_image, nullptr, (cudaStream_t)stream);
+}
+
+int gsb_splat_surfel_forward(int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                             const float *records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                             size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                             float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                             uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                             gsb_stream_t stream) {
+  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
+  if (rc) return rc;
+  GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_surfel_forward: bad P_cap");
+  GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_surfel_forward: null pointer");
+  GSB_REQUIRE(N == 0 || (us && depths && areas && records), "splat_surfel_forward: null pointer");
+  static thread_local cudaEvent_t ready_ev = nullptr;
+  if (ready_ev == nullptr) GSB_CUDA_TRY(cudaEventCreateWithFlags(&ready_ev, cudaEventDisableTiming));
+  const StatusRead sr{status_host, ready_ev};
+  status_host[0] = status_host[1] = status_host[2] = 0;
+  rc = surfel_frame(H, W, N, P_cap, depth_key_cap, us, depths, areas, records, bin_ws, ws, ws_bytes, image, contrib,
+                    final_tau, patch_range_per_tile, gsid_per_patch, depth_image, alpha_image, normal_image, &sr,
+                    (cudaStream_t)stream);
+  if (rc) return rc;
+  GSB_CUDA_TRY(cudaEventSynchronize(sr.ready));
+  const uint32_t P = status_host[0], flags = status_host[2];
+  if ((flags & GSB_STATUS_TOO_MANY_PATCHES) != 0 || P >= (1u << 30))
+    return set_arg_error("splat_surfel: more than 2^30 patches");
+  if ((flags & (GSB_STATUS_P_CAP | GSB_STATUS_DEPTH_KEY)) != 0 || (int64_t)P > P_cap) {
+    snprintf(g_err, sizeof(g_err), "splat_surfel_forward: capacity exceeded (P = %u of %lld, flags %u)", P,
+             (long long)P_cap, flags);
+    return GSB_CAPACITY_EXCEEDED;
+  }
+  return 0;
+}
+
+int gsb_splat_surfel_backward(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                              const float *final_tau, const int32_t *patch_range_per_tile,
+                              const int32_t *gsid_per_patch, const float *dloss_dimage, const float *dloss_ddepth,
+                              const float *dloss_dalpha, const float *dloss_dnormal, void *ws, size_t ws_bytes,
+                              float *rows, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splatB_surfel: bad N/H/W/P");
+  GSB_REQUIRE(grid_fits(H, W), "splatB_surfel: more than 65535 tiles in a row or column");
+  if (N == 0) return 0;
+  GSB_REQUIRE(rows != nullptr, "splatB_surfel: null output");
+  const SortLayout SL = sort_layout(N, H, W, 0);
+  GSB_REQUIRE(ws != nullptr && aligned(ws, 16) && ws_bytes >= SL.bytes, "splatB_surfel: workspace too small");
+  if (P > 0) {
+    GSB_REQUIRE(records && contrib && final_tau && patch_range_per_tile && gsid_per_patch, "splatB_surfel: null pointer");
+    GSB_REQUIRE(aligned(records, 16) && aligned(patch_range_per_tile, 8), "splatB_surfel: misaligned input");
+  }
+  char *b = static_cast<char *>(ws);
+  return launch_draw_surfel_backward(H, W, N, patch_range_per_tile, P > 0 ? records : nullptr, gsid_per_patch, contrib,
+                                     final_tau, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, rows,
+                                     reinterpret_cast<int *>(b + SL.counters), (cudaStream_t)stream);
 }
 
 // ---- feature rendering (raster_feat.cu)

@@ -19,7 +19,7 @@ enum KernelId {
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
   K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
-  K_MCMC_ROWS, K_MCMC_NOISE, K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_MCMC_ROWS, K_MCMC_NOISE, K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -286,5 +286,23 @@ struct FeatLayout {
   size_t recs, work, bytes;
 };
 FeatLayout feat_layout(int N, int H, int W, int64_t P, uintptr_t base);
+
+// ---- 2D Gaussian Splatting (surfel.cu, DESIGN 3.15; the math is surfel_math.h).  recs: one 80-byte
+// record per surfel ([N,20] floats, 16-byte aligned); rows: the backward rasterizer's [N,18]
+// gradient rows [dM (9), dalpha, dcolour (3), dn (3), ddelta (2)], zeroed by its launcher.
+int launch_surfel_fwd(const FusedScene &sc, const float *alphas, float *us, float *depths, int32_t *areas, float *colors,
+                      float *recs, cudaStream_t st);
+int launch_surfel_bwd(const FusedScene &sc, const float *rows, float *g_pws, float *g_shs, float *g_alphas,
+                      float *g_scales, float *g_rots, float *g_us, cudaStream_t st);
+// work: launch_tile_list's work area; recs == nullptr: no patches (zeros only).  The normal plane
+// [3,H,W] is written like the image planes.
+int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid, float *image,
+                       int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, float *normal_image,
+                       int *work, cudaStream_t st);
+// the upstream planes dl_*: NULL reads as zero (all NULL: the rows stay 0)
+int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, const float *recs, const int32_t *gsid,
+                                const int32_t *contrib, const float *final_tau, const float *dl_image,
+                                const float *dl_depth, const float *dl_alpha, const float *dl_normal, float *rows,
+                                int *work, cudaStream_t st);
 
 }  // namespace gsb

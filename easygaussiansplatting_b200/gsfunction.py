@@ -384,3 +384,55 @@ class GSFunctionFusedRGBDPose(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):
         return _fused_backward(ctx, True, True, dloss_dgammas, dloss_ddepth, dloss_dalpha)
+
+
+class GSFunctionSurfel(torch.autograd.Function):
+    """2D Gaussian Splatting (DESIGN 3.15): every Gaussian is a flat disk (surfel) with axes
+    scales[:, 0] R e0 and scales[:, 1] R e1 (scales[:, 2] is not read; rots is normalised), drawn
+    where the pixel's ray meets it.  `apply(pws, shs, alphas, scales, rots, us, cam)` ->
+    (image[3,H,W], depth[H,W], alpha[H,W], normal[3,H,W], depths > 0.2) with
+        depth[p] = sum_i w_i(p) z_i(p),  alpha[p] = sum_i w_i(p),  normal[p] = sum_i w_i(p) n_i
+    (w = tau alpha'; z_i(p) the camera-frame depth of the ray-splat hit; n_i the camera-frame
+    normal facing the camera).  depth is not normalised: depth / alpha is the expected depth.
+    Gradients of all four planes reach pws, shs, alphas, scales (column 2: 0), rots and us; us's
+    is dL/d of a screen-space shift of the whole surfel, the statistic
+    DensityController.update_density_info reads.  A plane the loss does not use is not read in the
+    backward (its upstream gradient stays None); with none used, the backward rasterizer is skipped.
+    Pinhole cameras only: cam.antialiased, other camera models and cam.grad_exchange are refused,
+    and so are filter3d and us_abs."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, filter3d=None, us_abs=None):
+        from . import ops
+        if getattr(cam, "antialiased", False):
+            raise ValueError("GSFunctionSurfel has no antialiased mode: cam.antialiased must be False")
+        _pinhole_only(cam, "GSFunctionSurfel")
+        if getattr(cam, "grad_exchange", None) is not None:
+            raise ValueError("GSFunctionSurfel is single-view: cam.grad_exchange must not be set")
+        if filter3d is not None:
+            raise ValueError("GSFunctionSurfel has no 3D filter: filter3d must be None")
+        if us_abs is not None:
+            raise ValueError("GSFunctionSurfel has no absolute-gradient statistic: us_abs must be None")
+        ctx.set_materialize_grads(False)
+        us_, depths, areas, colors, records = ops.surfel_preprocess(
+            pws, rots, scales, shs, alphas.reshape(-1), cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+            cam.width, cam.height)
+        image, contrib, final_tau, ranges, gsid, depth, alpha, normal = ops.splat_surfel(
+            cam.height, cam.width, us_, depths, areas, records, capacity=True)
+        ctx.cam = cam
+        ctx.alpha_shape = alphas.shape
+        ctx.save_for_backward(pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid)
+        return image, depth, alpha, normal, depths > 0.2
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, _):
+        from . import ops
+        cam = ctx.cam
+        pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid = ctx.saved_tensors
+        rows = ops.splatB_surfel(cam.height, cam.width, records, contrib, final_tau, ranges, gsid,
+                                 dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal)
+        dpws, dshs, dalphas, dscales, drots, dus = ops.surfel_preprocessB(
+            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height,
+            rows)
+        grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
+        return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))

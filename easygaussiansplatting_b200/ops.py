@@ -938,3 +938,150 @@ def sh_grad_expand(pws, twcs, dloss_dcolors, sh_dim3, out=None):
     with torch.cuda.device(pws.device):
         _lib.check(lib.gsb_sh_grad_expand(N, k, V, _ptr(pws), _ptr(twcs), _ptr(g), _ptr(out), _stream()), lib)
     return out
+
+
+# ---------------------------------------------------------------------------------------
+# 2D Gaussian Splatting (extension; DESIGN 3.15): surfels drawn by ray-splat intersection.
+SURFEL_RECORD = 20  # floats per surfel record (80 bytes)
+SURFEL_ROW = 18     # floats per gradient row: dM (9), dalpha, dcolour (3), dn (3), ddelta (2)
+
+
+def surfel_preprocess(pws, rots, scales, shs, alphas, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width,
+                      height):
+    """The per-surfel forward (gsb_surfel_preprocess_forward): scales[:, 0] and scales[:, 1] are the
+    disk's axes (column 2 is not read), rots its (normalised here) quaternion, pinhole camera.
+    -> (us[N,2], depths[N] (-1 = culled), areas[N,2] i32, colors[N,3], records[N,20])"""
+    params, N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    alphas = _per_gaussian(alphas, "alphas", N, params[0])
+    o = dict(dtype=torch.float32, device=params[0].device)
+    us = torch.empty((N, 2), **o); depths = torch.empty((N,), **o); colors = torch.empty((N, 3), **o)
+    areas = torch.empty((N, 2), dtype=torch.int32, device=params[0].device)
+    records = torch.empty((N, SURFEL_RECORD), **o)
+    lib = _L()
+    with torch.cuda.device(params[0].device):
+        _lib.check(lib.gsb_surfel_preprocess_forward(
+            *_scene_args(params, N, k, focal_x, focal_y, center_x, center_y, width, height), _ptr(alphas), _ptr(us),
+            _ptr(depths), _ptr(areas), _ptr(colors), _ptr(records), _stream()), lib)
+    return us, depths, areas, colors, records
+
+
+def surfel_preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
+                       rows):
+    """The per-surfel backward (gsb_surfel_preprocess_backward) from splatB_surfel's rows[N,18].
+    -> (dpws[N,3], dshs[N,3k], dalphas[N], dscales[N,3] (column 2: 0), drots[N,4], dus[N,2])"""
+    params, N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
+    rows = _chk(rows, "rows", last=SURFEL_ROW, ndim=2)
+    _same_device(params[0], rows)
+    if rows.shape[0] != N:
+        raise ValueError("rows must be [N, %d]" % SURFEL_ROW)
+    o = dict(dtype=torch.float32, device=params[0].device)
+    out = (torch.empty((N, 3), **o), torch.empty((N, 3 * k), **o), torch.empty((N,), **o), torch.empty((N, 3), **o),
+           torch.empty((N, 4), **o), torch.empty((N, 2), **o))
+    lib = _L()
+    with torch.cuda.device(params[0].device):
+        _lib.check(lib.gsb_surfel_preprocess_backward(
+            *_scene_args(params, N, k, focal_x, focal_y, center_x, center_y, width, height), _ptr(rows),
+            *[_ptr(t) for t in out], _stream()), lib)
+    return out
+
+
+def _surfel_buffers(lib, dev, H, W, N, P):
+    T = ((W + 15) // 16) * ((H + 15) // 16)
+    f = dict(dtype=torch.float32, device=dev)
+    ws = _bytes(lib.gsb_splat_surfel_workspace_bytes(N, H, W, P), dev)
+    return ws, [torch.empty((3, H, W), **f), torch.empty((H, W), dtype=torch.int32, device=dev),
+                torch.empty((H, W), **f), torch.empty((T, 2), dtype=torch.int32, device=dev),
+                torch.empty((P,), dtype=torch.int32, device=dev), torch.empty((H, W), **f), torch.empty((H, W), **f),
+                torch.empty((3, H, W), **f)]
+
+
+def splat_surfel(height, width, us, depths, areas, records, capacity=False):
+    """Bins the surfels (us, areas, depths: the binning of `splat`, which MUTATES depths / areas of
+    surfels that touch no tile) and draws them.  -> [image[3,H,W], contrib[H,W] i32,
+    final_tau[H,W], patch_range_per_tile[T,2] i32, gsid_per_patch[P] i32, depth[H,W], alpha[H,W],
+    normal[3,H,W]] with depth = sum w z(p) (the camera-frame depth of each ray-splat hit, not
+    normalised), alpha = sum w, normal = sum w n (camera frame), w = tau alpha'.
+    capacity: as for `splat` (sort sized from the previous frame of this shape; an outgrown frame
+    is redone the exact way)."""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    us = _chk(us, "us", last=2, ndim=2); depths = _chk(depths, "depths")
+    areas = _chk(areas, "areas", dtype=torch.int32, last=2, ndim=2)
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    _same_device(us, depths, areas, records)
+    N = us.shape[0]
+    if not (depths.numel() == N and areas.shape[0] == N and records.shape[0] == N):
+        raise ValueError("splat_surfel inputs disagree on N")
+    dev, lib = us.device, _L()
+    cap_key = ("surfel", dev.index, H, W, N)
+    with torch.cuda.device(dev):
+        if capacity and cap_key in _CAPACITY and N > 0:
+            P_cap, dk_cap = _CAPACITY[cap_key]
+            status = _STATUS.get(dev.index)
+            if status is None:
+                status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
+            bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
+            ws, out = _surfel_buffers(lib, dev, H, W, N, P_cap)
+            rc = lib.gsb_splat_surfel_forward(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(records), P_cap,
+                                              dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
+                                              *[_ptr(o) for o in out[:5]], status.data_ptr(),
+                                              *[_ptr(o) for o in out[5:]], _stream())
+            if rc != GSB_CAPACITY_EXCEEDED:
+                _lib.check(rc, lib)
+                CAPACITY_STATS["capacity_frames"] += 1
+                P, dkmax, _ = _decode_status(status)
+                _CAPACITY[cap_key] = _next_capacity(P, dkmax)
+                out[4] = out[4][:P]
+                return out
+            CAPACITY_STATS["outgrown"] += 1
+            del _CAPACITY[cap_key]  # outgrown: this frame the exact way (the in-place culls are idempotent)
+        bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
+        P, dkmax = C.c_int64(0), C.c_uint32(0)
+        _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
+                                     C.byref(P), C.byref(dkmax), _stream()), lib)
+        P = int(P.value)
+        ws, out = _surfel_buffers(lib, dev, H, W, N, P)
+        if capacity:
+            CAPACITY_STATS["exact_frames"] += 1
+            _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
+        _lib.check(lib.gsb_splat_surfel_render(H, W, N, P, dkmax.value, _ptr(us), _ptr(depths), _ptr(records),
+                                               _ptr(bin_ws), _ptr(ws), ws.numel(), *[_ptr(o) for o in out],
+                                               _stream()), lib)
+    return out
+
+
+def splatB_surfel(height, width, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                  dloss_dimage=None, dloss_ddepth=None, dloss_dalpha=None, dloss_dnormal=None):
+    """Backward of `splat_surfel` from the planes' upstream gradients ([3,H,W], [H,W], [H,W],
+    [3,H,W]; None = zero and not read; all None: no rasterizer pass, zero rows).
+    -> rows[N,18] = [dL/dM (9), dL/dalpha, dL/dcolour (3), dL/dn (3), dL/ddelta (2)] per surfel,
+    for `surfel_preprocessB`"""
+    H, W = int(height), int(width)
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    contrib = _chk(contrib, "contrib", dtype=torch.int32); final_tau = _chk(final_tau, "final_tau")
+    ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
+    gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
+    _same_device(records, contrib, final_tau, ranges, gsid)
+    T = ((W + 15) // 16) * ((H + 15) // 16)
+    if contrib.numel() != H * W or final_tau.numel() != H * W:
+        raise ValueError("contrib / final_tau do not match height x width")
+    if ranges.shape[0] != T:
+        raise ValueError("patch_range_per_tile does not match the tile grid")
+    planes = []
+    for name, t, n in (("dloss_dimage", dloss_dimage, 3), ("dloss_ddepth", dloss_ddepth, 1),
+                       ("dloss_dalpha", dloss_dalpha, 1), ("dloss_dnormal", dloss_dnormal, 3)):
+        if t is not None:
+            t = _chk(t, name)
+            _same_device(records, t)
+            if t.numel() != n * H * W:
+                raise ValueError("%s does not match height x width" % name)
+        planes.append(t)
+    N, P, dev, lib = records.shape[0], gsid.numel(), records.device, _L()
+    rows = torch.empty((N, SURFEL_ROW), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_splat_surfel_workspace_bytes(N, H, W, 0), dev)
+        _lib.check(lib.gsb_splat_surfel_backward(H, W, N, P, _ptr(records), _ptr(contrib), _ptr(final_tau),
+                                                 _ptr(ranges), _ptr(gsid), *[_ptr(t) for t in planes], _ptr(ws),
+                                                 ws.numel(), _ptr(rows), _stream()), lib)
+    return rows

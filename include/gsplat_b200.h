@@ -654,6 +654,57 @@ int gsb_preprocess_backward_push(int N, int sh_dim3, const float *pws, const flo
 int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *const *regions_host, uint32_t epoch,
                               gsb_stream_t stream);
 
+/* ---- 2D Gaussian Splatting (extension; DESIGN 3.15): each Gaussian is a flat disk (surfel) with
+ * axes scales[:,0] R e0 and scales[:,1] R e1 (scales[:,2] is not read), drawn where the pixel's ray
+ * meets it; pinhole cameras only.
+ * gsb_surfel_preprocess_forward: us[N,2], depths[N] (-1 = culled), areas[N,2] (integer half-extents
+ * of the 3-sigma footprint), colors[N,3] (the SH colour of gsb_preprocess_forward) and records
+ * [N,20] floats (16-byte aligned), the rasterizers' per-surfel input.  alphas[N] is read into the
+ * records.  N == 0 does nothing. */
+int gsb_surfel_preprocess_forward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                  const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                  float fy, float cx, float cy, float width, float height, const float *alphas,
+                                  float *us, float *depths, int32_t *areas, float *colors, float *records,
+                                  gsb_stream_t stream);
+/* rows[N,18]: the gradient rows gsb_splat_surfel_backward wrote.  Writes dloss_dpws[N,3],
+ * dloss_dshs[N,3k], dloss_dalphas[N], dloss_dscales[N,3] (column 2: 0), dloss_drots[N,4] and
+ * dloss_dus[N,2] (dL/d of a screen-space shift of the whole surfel: the densification statistic). */
+int gsb_surfel_preprocess_backward(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                   const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
+                                   float fy, float cx, float cy, float width, float height, const float *rows,
+                                   float *dloss_dpws, float *dloss_dshs, float *dloss_dalphas, float *dloss_dscales,
+                                   float *dloss_drots, float *dloss_dus, gsb_stream_t stream);
+/* Workspace of gsb_splat_surfel_render / _forward for P patches (P_cap), and of
+ * gsb_splat_surfel_backward with P = 0.  The binning is gsb_splat_bin's (its bin_ws). */
+size_t gsb_splat_surfel_workspace_bytes(int N, int H, int W, int64_t P);
+/* The frame binned by gsb_splat_bin (P patches, largest depth key depth_key_max), drawn from the
+ * records: image[3,H,W], contrib, final_tau, patch_range_per_tile, gsid_per_patch as gsb_splat_render,
+ * depth_image[H,W] = sum w z(p) (the camera-frame depth of each ray-splat hit, not normalised),
+ * alpha_image[H,W] = sum w and normal_image[3,H,W] = sum w n (camera frame).  Every plane and
+ * records 16-byte aligned, patch_range_per_tile 8-byte aligned. */
+int gsb_splat_surfel_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                            const float *depths, const float *records, const void *bin_ws, void *ws, size_t ws_bytes,
+                            float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                            int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
+                            gsb_stream_t stream);
+/* The capacity form (as gsb_splat_forward): bins here, sorts into P_cap slots, and returns
+ * GSB_CAPACITY_EXCEEDED when the frame outgrew P_cap or depth_key_cap (status_host as there). */
+int gsb_splat_surfel_forward(int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                             const float *records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                             size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                             float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                             uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                             gsb_stream_t stream);
+/* Backward of the surfel frame: upstream planes dloss_dimage[3,H,W], dloss_ddepth[H,W],
+ * dloss_dalpha[H,W], dloss_dnormal[3,H,W], each nullable (NULL = zero; a frame with none of them
+ * costs one memset).  rows[N,18] (written in full): [dL/dM (9), dL/dalpha, dL/dcolour (3), dL/dn (3),
+ * dL/ddelta (2)] per surfel, for gsb_surfel_preprocess_backward. */
+int gsb_splat_surfel_backward(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                              const float *final_tau, const int32_t *patch_range_per_tile,
+                              const int32_t *gsid_per_patch, const float *dloss_dimage, const float *dloss_ddepth,
+                              const float *dloss_dalpha, const float *dloss_dnormal, void *ws, size_t ws_bytes,
+                              float *rows, gsb_stream_t stream);
+
 /* ---- launch accounting and optional per-kernel timing (no reference counterpart; used by
  * bench.py for `gpu_launches` and the roofline's live CUDA-event kernel durations).
  * Kernel ids 0..gsb_profile_kernels()-1, names from gsb_profile_kernel_name().
