@@ -482,41 +482,98 @@ size_t gsb_splat_records_offset(int N, int H, int W, int64_t P) { return sort_la
 
 size_t gsb_splat_workspace_bytes(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).bytes; }
 
-// A binned frame from the sort to the image, shared by both ways of rendering one: P is the patch
-// count (gsb_splat_render) or its capacity (gsb_splat_forward).  With `sr` (the capacity path) the
-// frame is binned here first, after every argument has been checked, and its status is copied to
-// sr->host behind the keys.
-static int render_frame(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
-                        const float *cinv2ds, const float *alphas, float *depths, const float *colors,
-                        int32_t *areas, const void *packed_records, void *bin_ws, void *ws, size_t ws_bytes,
-                        float *image, int32_t *contrib, float *final_tau, int32_t *ranges, int32_t *gsid,
-                        float *depth_image, float *alpha_image, const StatusRead *sr, cudaStream_t st) {
-  GSB_REQUIRE(image && contrib && final_tau && ranges, "splat: null output");
-  // RGB-D frames (the *_rgbd entry points pass both planes, written like the image planes)
-  GSB_REQUIRE((depth_image == nullptr) == (alpha_image == nullptr), "splat: depth_image and alpha_image go together");
-  GSB_REQUIRE(aligned(depth_image, 16) && aligned(alpha_image, 16), "splat: misaligned depth_image / alpha_image");
-  // the rasterizer writes the three image planes with 16-byte stores and the binning writes the
-  // tile ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h)
-  GSB_REQUIRE(aligned(image, 16) && aligned(contrib, 16) && aligned(final_tau, 16) && aligned(ranges, 8),
-              "splat: misaligned output");
-  GSB_REQUIRE(aligned(packed_records, 16), "splat: packed_records misaligned");
+// The outputs every frame writes: the image planes [3,H,W], contrib and final_tau [H,W], the tile
+// ranges [T,2] and the sorted patch list
+struct FrameOut {
+  float *image;
+  int32_t *contrib;
+  float *final_tau;
+  int32_t *ranges, *gsid;
+};
+
+// The draw step of the colour frame and, with both planes, of the RGB-D frame: the records are
+// packed_records, or those the sort packed into ws (ws_recs).
+struct ColourDraw {
+  const void *packed_records;
+  float *depth_image, *alpha_image;
+
+  int check() const {
+    // RGB-D frames (the *_rgbd entry points pass both planes, written like the image planes)
+    GSB_REQUIRE((depth_image == nullptr) == (alpha_image == nullptr), "splat: depth_image and alpha_image go together");
+    GSB_REQUIRE(aligned(depth_image, 16) && aligned(alpha_image, 16), "splat: misaligned depth_image / alpha_image");
+    GSB_REQUIRE(aligned(packed_records, 16), "splat: packed_records misaligned");
+    return 0;
+  }
+  int draw(int H, int W, int, int64_t P, const FrameOut &o, const void *ws_recs, int *work, cudaStream_t st) const {
+    const Rec *recs = static_cast<const Rec *>(packed_records ? packed_records : ws_recs);
+    // with P == 0 (or N == 0) every tile is empty: the rasterizer only writes zeros
+    return launch_draw(H, W, o.ranges, P > 0 ? recs : nullptr, o.gsid, o.image, o.contrib, o.final_tau, depth_image,
+                       alpha_image, work, st);
+  }
+};
+
+extern "C++" {  // (templates)
+
+// A binned frame from the sort to its planes, shared by every way of rendering one: P is the patch
+// count (gsb_splat_render, gsb_splat_surfel_render) or its capacity (the *_forward entry points).
+// With `sr` (the capacity path) the frame is binned here first, after every argument has been
+// checked, and its status is copied to sr->host behind the keys.  `who` prefixes the error texts;
+// the sort packs the 48-byte records into ws when `pack`; `draw` checks the planes and records of
+// its frame family (draw.check()) and draws them (draw.draw()).
+template <class Draw>
+static int render_frame(const char *who, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                        const float *cinv2ds, const float *alphas, float *depths, const float *colors, int32_t *areas,
+                        bool pack, void *bin_ws, void *ws, size_t ws_bytes, const FrameOut &o, const Draw &draw,
+                        const StatusRead *sr, cudaStream_t st) {
+  if (!(o.image && o.contrib && o.final_tau && o.ranges)) return arg_error(who, "null output");
+  // the rasterizers write the image planes with 16-byte stores and the binning writes the tile
+  // ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h)
+  if (!(aligned(o.image, 16) && aligned(o.contrib, 16) && aligned(o.final_tau, 16) && aligned(o.ranges, 8)))
+    return arg_error(who, "misaligned output");
+  if (int rc = draw.check()) return rc;
   // 64-bit keys at ws + 0, records gathered 16 bytes at a time (the layout's offsets are 256-B multiples)
-  GSB_REQUIRE(aligned(ws, 16), "splat: ws misaligned");
+  if (!aligned(ws, 16)) return arg_error(who, "ws misaligned");
   const SortLayout SL = sort_layout(N, H, W, P);
-  GSB_REQUIRE(ws != nullptr && ws_bytes >= SL.bytes, "splat: workspace too small");
+  if (!(ws != nullptr && ws_bytes >= SL.bytes)) return arg_error(who, "workspace too small");
   const BinLayout BL = bin_layout(N);
   int rc = sr ? launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st) : 0;
   if (rc) return rc;
   rc = launch_sort_and_pack(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
-                            ranges, gsid, packed_records == nullptr, sr, st);
+                            o.ranges, o.gsid, pack, sr, st);
   if (rc) return rc;
   char *b = static_cast<char *>(ws);
-  const Rec *recs =
-      packed_records ? static_cast<const Rec *>(packed_records) : reinterpret_cast<const Rec *>(b + SL.recs);
-  // with P == 0 (or N == 0) every tile is empty: the rasterizer only writes zeros
-  return launch_draw(H, W, ranges, P > 0 ? recs : nullptr, gsid, image, contrib, final_tau, depth_image, alpha_image,
-                     reinterpret_cast<int *>(b + SL.counters), st);
+  return draw.draw(H, W, N, P, o, b + SL.recs, reinterpret_cast<int *>(b + SL.counters), st);
 }
+
+// The status event of the capacity path, one per host thread
+static thread_local cudaEvent_t g_status_ready = nullptr;
+
+// The capacity path's wait, shared by gsb_splat_forward{,_rgbd,_enqueue} and gsb_splat_surfel_forward:
+// frame(sr) checks and queues the frame (render_frame with `sr`).  With `wait` status_host is zeroed
+// first, and then the binning's status is waited for and judged; without it (CUDA graph capture)
+// the caller inspects status_host later.  `who` prefixes the verdict's texts.
+template <class Frame>
+static int capacity_wait(const char *who, int64_t P_cap, uint32_t *status_host, bool wait, const Frame &frame) {
+  if (wait && g_status_ready == nullptr)
+    GSB_CUDA_TRY(cudaEventCreateWithFlags(&g_status_ready, cudaEventDisableTiming));
+  const StatusRead sr{status_host, wait ? g_status_ready : nullptr};
+  if (wait) status_host[0] = status_host[1] = status_host[2] = 0;
+  const int rc = frame(&sr);
+  if (rc || !wait) return rc;
+  // the sort and the rasterizer are queued; now look at what the binning found (N == 0: nothing
+  // was copied, the zeros stand)
+  GSB_CUDA_TRY(cudaEventSynchronize(sr.ready));
+  const uint32_t P = status_host[0], flags = status_host[2];
+  if ((flags & GSB_STATUS_TOO_MANY_PATCHES) != 0 || P >= (1u << 30)) return arg_error(who, "more than 2^30 patches");
+  if ((flags & (GSB_STATUS_P_CAP | GSB_STATUS_DEPTH_KEY)) != 0 || (int64_t)P > P_cap) {
+    snprintf(g_err, sizeof(g_err), "%s_forward: capacity exceeded (P = %u of %lld, flags %u)", who, P,
+             (long long)P_cap, flags);
+    return GSB_CAPACITY_EXCEEDED;
+  }
+  return 0;
+}
+
+}  // extern "C++"
 
 static int splat_render_impl(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
                              const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
@@ -529,9 +586,10 @@ static int splat_render_impl(int H, int W, int N, int64_t P, uint32_t depth_key_
   GSB_REQUIRE(P == 0 || (us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch),
               "splat: null pointer");
   // (without `sr` nothing is binned: depths and bin_ws are only read)
-  return render_frame(H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors, nullptr,
-                      packed_records, const_cast<void *>(bin_ws), ws, ws_bytes, image, contrib, final_tau,
-                      patch_range_per_tile, gsid_per_patch, depth_image, alpha_image, nullptr, (cudaStream_t)stream);
+  return render_frame("splat", H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors,
+                      nullptr, packed_records == nullptr, const_cast<void *>(bin_ws), ws, ws_bytes,
+                      {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                      ColourDraw{packed_records, depth_image, alpha_image}, nullptr, (cudaStream_t)stream);
 }
 
 int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
@@ -566,26 +624,12 @@ static int splat_forward_impl(int H, int W, int N, const float *us, const float 
   GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad P_cap");
   GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_forward: null pointer");
   GSB_REQUIRE(N == 0 || (us && cinv2ds && alphas && depths && colors && areas), "splat_forward: null pointer");
-  static thread_local cudaEvent_t ready_ev = nullptr;
-  if (wait && ready_ev == nullptr) GSB_CUDA_TRY(cudaEventCreateWithFlags(&ready_ev, cudaEventDisableTiming));
-  const StatusRead sr{status_host, wait ? ready_ev : nullptr};
-  if (wait) status_host[0] = status_host[1] = status_host[2] = 0;
-  rc = render_frame(H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas, packed_records, bin_ws,
-                    ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, depth_image,
-                    alpha_image, &sr, (cudaStream_t)stream);
-  if (rc || !wait) return rc;  // enqueue-only (CUDA graph capture): the caller inspects status_host later
-  // the sort and the rasterizer are queued; now look at what the binning found (N == 0: nothing
-  // was copied, the zeros stand)
-  GSB_CUDA_TRY(cudaEventSynchronize(sr.ready));
-  const uint32_t P = status_host[0], flags = status_host[2];
-  if ((flags & GSB_STATUS_TOO_MANY_PATCHES) != 0 || P >= (1u << 30))
-    return set_arg_error("splat: more than 2^30 patches");
-  if ((flags & (GSB_STATUS_P_CAP | GSB_STATUS_DEPTH_KEY)) != 0 || (int64_t)P > P_cap) {
-    snprintf(g_err, sizeof(g_err), "splat_forward: capacity exceeded (P = %u of %lld, flags %u)", P,
-             (long long)P_cap, flags);
-    return GSB_CAPACITY_EXCEEDED;
-  }
-  return 0;
+  return capacity_wait("splat", P_cap, status_host, wait, [&](const StatusRead *sr) {
+    return render_frame("splat", H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas,
+                        packed_records == nullptr, bin_ws, ws, ws_bytes,
+                        {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                        ColourDraw{packed_records, depth_image, alpha_image}, sr, (cudaStream_t)stream);
+  });
 }
 
 int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -765,31 +809,23 @@ int gsb_surfel_preprocess_backward(int N, int sh_dim3, const float *pws, const f
 
 size_t gsb_splat_surfel_workspace_bytes(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).bytes; }
 
-// The surfel frame from the sort to the planes, shared by the exact (P) and the capacity (P_cap,
-// with `sr`: binned here first) entry points, as render_frame is for the colour frame.
-static int surfel_frame(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us, float *depths,
-                        int32_t *areas, const float *records, void *bin_ws, void *ws, size_t ws_bytes, float *image,
-                        int32_t *contrib, float *final_tau, int32_t *ranges, int32_t *gsid, float *depth_image,
-                        float *alpha_image, float *normal_image, const StatusRead *sr, cudaStream_t st) {
-  GSB_REQUIRE(image && contrib && final_tau && ranges && depth_image && alpha_image && normal_image,
-              "splat_surfel: null output");
-  GSB_REQUIRE(aligned(image, 16) && aligned(contrib, 16) && aligned(final_tau, 16) && aligned(depth_image, 16) &&
-                  aligned(alpha_image, 16) && aligned(normal_image, 16) && aligned(ranges, 8),
-              "splat_surfel: misaligned output");
-  GSB_REQUIRE(aligned(records, 16), "splat_surfel: records misaligned");
-  GSB_REQUIRE(aligned(ws, 16), "splat_surfel: ws misaligned");
-  const SortLayout SL = sort_layout(N, H, W, P);
-  GSB_REQUIRE(ws != nullptr && ws_bytes >= SL.bytes, "splat_surfel: workspace too small");
-  const BinLayout BL = bin_layout(N);
-  int rc = sr ? launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st) : 0;
-  if (rc) return rc;
-  rc = launch_sort_and_pack(H, W, N, P, depth_key_max, us, nullptr, nullptr, depths, nullptr, bin_ws, BL, ws, SL,
-                            ranges, gsid, false, sr, st);
-  if (rc) return rc;
-  char *b = static_cast<char *>(ws);
-  return launch_draw_surfel(H, W, ranges, P > 0 && N > 0 ? records : nullptr, gsid, image, contrib, final_tau,
-                            depth_image, alpha_image, normal_image, reinterpret_cast<int *>(b + SL.counters), st);
-}
+// The draw step of the surfel frame: its 80-byte records and its three further planes
+struct SurfelDraw {
+  const float *records;
+  float *depth_image, *alpha_image, *normal_image;
+
+  int check() const {
+    GSB_REQUIRE(depth_image && alpha_image && normal_image, "splat_surfel: null output");
+    GSB_REQUIRE(aligned(depth_image, 16) && aligned(alpha_image, 16) && aligned(normal_image, 16),
+                "splat_surfel: misaligned output");
+    GSB_REQUIRE(aligned(records, 16), "splat_surfel: records misaligned");
+    return 0;
+  }
+  int draw(int H, int W, int N, int64_t P, const FrameOut &o, const void *, int *work, cudaStream_t st) const {
+    return launch_draw_surfel(H, W, o.ranges, P > 0 && N > 0 ? records : nullptr, o.gsid, o.image, o.contrib,
+                              o.final_tau, depth_image, alpha_image, normal_image, work, st);
+  }
+};
 
 int gsb_splat_surfel_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
                             const float *depths, const float *records, const void *bin_ws, void *ws, size_t ws_bytes,
@@ -800,9 +836,10 @@ int gsb_splat_surfel_render(int H, int W, int N, int64_t P, uint32_t depth_key_m
   if (rc) return rc;
   GSB_REQUIRE(P >= 0, "splat_surfel: bad P");
   GSB_REQUIRE(P == 0 || (us && depths && records && bin_ws && ws && gsid_per_patch), "splat_surfel: null pointer");
-  return surfel_frame(H, W, N, P, depth_key_max, us, const_cast<float *>(depths), nullptr, records,
-                      const_cast<void *>(bin_ws), ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
-                      gsid_per_patch, depth_image, alpha_image, normal_image, nullptr, (cudaStream_t)stream);
+  return render_frame("splat_surfel", H, W, N, P, depth_key_max, us, nullptr, nullptr, const_cast<float *>(depths),
+                      nullptr, nullptr, false, const_cast<void *>(bin_ws), ws, ws_bytes,
+                      {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                      SurfelDraw{records, depth_image, alpha_image, normal_image}, nullptr, (cudaStream_t)stream);
 }
 
 int gsb_splat_surfel_forward(int H, int W, int N, const float *us, float *depths, int32_t *areas,
@@ -816,24 +853,11 @@ int gsb_splat_surfel_forward(int H, int W, int N, const float *us, float *depths
   GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_surfel_forward: bad P_cap");
   GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_surfel_forward: null pointer");
   GSB_REQUIRE(N == 0 || (us && depths && areas && records), "splat_surfel_forward: null pointer");
-  static thread_local cudaEvent_t ready_ev = nullptr;
-  if (ready_ev == nullptr) GSB_CUDA_TRY(cudaEventCreateWithFlags(&ready_ev, cudaEventDisableTiming));
-  const StatusRead sr{status_host, ready_ev};
-  status_host[0] = status_host[1] = status_host[2] = 0;
-  rc = surfel_frame(H, W, N, P_cap, depth_key_cap, us, depths, areas, records, bin_ws, ws, ws_bytes, image, contrib,
-                    final_tau, patch_range_per_tile, gsid_per_patch, depth_image, alpha_image, normal_image, &sr,
-                    (cudaStream_t)stream);
-  if (rc) return rc;
-  GSB_CUDA_TRY(cudaEventSynchronize(sr.ready));
-  const uint32_t P = status_host[0], flags = status_host[2];
-  if ((flags & GSB_STATUS_TOO_MANY_PATCHES) != 0 || P >= (1u << 30))
-    return set_arg_error("splat_surfel: more than 2^30 patches");
-  if ((flags & (GSB_STATUS_P_CAP | GSB_STATUS_DEPTH_KEY)) != 0 || (int64_t)P > P_cap) {
-    snprintf(g_err, sizeof(g_err), "splat_surfel_forward: capacity exceeded (P = %u of %lld, flags %u)", P,
-             (long long)P_cap, flags);
-    return GSB_CAPACITY_EXCEEDED;
-  }
-  return 0;
+  return capacity_wait("splat_surfel", P_cap, status_host, true, [&](const StatusRead *sr) {
+    return render_frame("splat_surfel", H, W, N, P_cap, depth_key_cap, us, nullptr, nullptr, depths, nullptr, areas,
+                        false, bin_ws, ws, ws_bytes, {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                        SurfelDraw{records, depth_image, alpha_image, normal_image}, sr, (cudaStream_t)stream);
+  });
 }
 
 int gsb_splat_surfel_backward(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,

@@ -160,7 +160,7 @@ __device__ __forceinline__ void draw_bwd_body(
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
     float *__restrict__ dus_abs, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<>];  // gathered records, per warp
   __shared__ __align__(16) unsigned char s_w[4][WALK_W_BYTES];                   // weight rows, per warp
   __shared__ __align__(16) float s_dl[4][RGBD ? 4 : 3][64];                    // dL/dgamma (dL/dD) of the block
   __shared__ __align__(16) uint2 s_list[4][34];  // (record address, patch index) of a chunk's survivors
@@ -246,7 +246,7 @@ __device__ __forceinline__ void draw_bwd_body(
     // gather of chunk c: lane j copies the record of patch 32 c + j (if below wmax) into ring slot c & 1
     auto issue = [&](int c, int id) {
       if (c >= 0 && c * 32 + lane < wmax)
-        gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
+        gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<> + lane * 48);
       cp_async_commit();
     };
     auto load_id = [&](int c) { return (c >= 0 && c * 32 + lane < wmax) ? __ldg(ids + c * 32 + lane) : 0; };

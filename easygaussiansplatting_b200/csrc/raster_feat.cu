@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
     int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ features, int D,
     int c0, float *__restrict__ feature_image, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<>];  // gathered records, per warp
   __shared__ __align__(16) uint2 s_list[4][34];       // (record address, patch index) of a chunk's survivors
   __shared__ __align__(16) float s_feat[4][34][G];    // their features, same order
   __shared__ __align__(16) Rec s_dummy;               // all-zero record: pads an odd survivor count
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(128, DRAW_FEAT_MINBLOCKS) k_draw_feat(
         const int32_t *ids = gsid + range.x;
         auto issue = [&](int c, int id) {
           if (c < nch && c * 32 + lane < wmax)
-            gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
+            gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<> + lane * 48);
           cp_async_commit();
         };
         auto load_id = [&](int c) { return (c < nch && c * 32 + lane < wmax) ? __ldg(ids + c * 32 + lane) : 0; };
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ features, int D, int c0, const float *__restrict__ dloss_dfeature_image,
     float *__restrict__ moments, float *__restrict__ dfeat, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<>];  // gathered records, per warp
   __shared__ __align__(16) unsigned char s_w[4][WALK_W_BYTES];                    // weight rows, per warp
   __shared__ __align__(16) float s_dl[4][G][64];       // dL/dF of the block, channel-major
   __shared__ __align__(16) uint2 s_list[4][34];        // (record address, patch index) of a chunk's survivors
@@ -380,7 +380,7 @@ __global__ void __launch_bounds__(128, feat_bwd_minblocks<G>()) k_draw_feat_bwd(
     const int32_t *ids = gsid + range.x;
     auto issue = [&](int c, int id) {
       if (c >= 0 && c * 32 + lane < wmax)
-        gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
+        gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<> + lane * 48);
       cp_async_commit();
     };
     auto load_id = [&](int c) { return (c >= 0 && c * 32 + lane < wmax) ? __ldg(ids + c * 32 + lane) : 0; };

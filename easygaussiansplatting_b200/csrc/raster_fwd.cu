@@ -121,7 +121,7 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
                                           float *__restrict__ image, int32_t *__restrict__ contrib,
                                           float *__restrict__ final_tau, float *__restrict__ depth_image,
                                           float *__restrict__ alpha_image, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES];  // gathered records, per warp
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<>];  // gathered records, per warp
   __shared__ __align__(16) uint2 s_list[4][34];  // (record address, patch index + 1) of a chunk's survivors
   __shared__ __align__(16) Rec s_dummy;          // all-zero record (alpha = 0): pads an odd survivor count
 
@@ -161,7 +161,7 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
       const int32_t *ids = gsid + range.x;
       auto issue = [&](int c, int id) {
         if (c < nch && c * 32 + lane < len)
-          gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48);
+          gather_record(recs + id, ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<> + lane * 48);
         cp_async_commit();
       };
       auto load_id = [&](int c) { return (c < nch && c * 32 + lane < len) ? __ldg(ids + c * 32 + lane) : 0; };

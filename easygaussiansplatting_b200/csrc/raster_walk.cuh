@@ -8,7 +8,8 @@
 //    patch 32 c + j with three 16-byte cp.async (gather_record) into ring slot c % WALK_RING, one
 //    cp.async group per chunk and lane, WALK_RING chunks in flight, cp.async groups + __syncwarp
 //    (wait_chunk) and no CTA barrier after start-up (zero_dummy).  The forward passes walk the chunks
-//    front to back, the backward passes back to front from the block's largest contrib;
+//    front to back, the backward passes back to front from the block's largest contrib.  The surfel
+//    rasterizers (surfel.cu) walk their 80-byte records with the same chunk helpers at that width;
 //  - each lane tests its record against the warp's block with rec_can_touch (exact: no output
 //    changes), a ballot compacts the survivors in walk order into a list of (record address, patch
 //    index), and an entry pointing at the all-zero record (alpha = 0) pads an odd count, so the
@@ -22,7 +23,8 @@
 namespace gsb {
 
 constexpr int WALK_RING = 2;  // 32-record chunks in flight per warp
-constexpr int WALK_CHUNK_BYTES = 32 * 48;
+template <int RecBytes = sizeof(Rec)>
+constexpr int WALK_CHUNK_BYTES = 32 * RecBytes;  // one chunk of RecBytes-byte records
 // phase-B weight rows of the backward passes: a slot = 2 rows of 64 floats (w, wc) + 16 floats of
 // padding; a stride of 16 (mod 32) floats makes the 128-bit reads (2 slots x 4 parts per 8-lane
 // wavefront) conflict-free
@@ -55,12 +57,13 @@ __device__ __forceinline__ void walk_drain() {
   __syncwarp();
 }
 
-// The 48-byte record at `rec` into shared memory at `dst`.
-__device__ __forceinline__ void gather_record(const Rec *rec, uint32_t dst) {
-  const char *src = reinterpret_cast<const char *>(rec);
-  cp_async16_sa(dst, src);
-  cp_async16_sa(dst + 16, src + 16);
-  cp_async16_sa(dst + 32, src + 32);
+// The RecBytes-byte record at `rec` (the 48-byte Rec, or the 80-byte surfel record of surfel.cu)
+// into shared memory at `dst`, 16 bytes per cp.async.
+template <int RecBytes = sizeof(Rec)>
+__device__ __forceinline__ void gather_record(const void *rec, uint32_t dst) {
+  const char *src = static_cast<const char *>(rec);
+#pragma unroll
+  for (int k = 0; k < RecBytes / 16; k++) cp_async16_sa(dst + 16 * k, src + 16 * k);
 }
 
 // A tile of <= 32 patches: its single chunk into ring slot 0, gathered once for all four blocks.
@@ -74,10 +77,11 @@ __device__ __forceinline__ void gather_whole_tile(uint32_t ring, const Rec *__re
 
 // The lane's record of chunk c in a ring of WALK_RING slots, once the chunk has landed in every lane
 // (a chunk is one cp.async group per lane, empty where the lane has no record in it).
+template <int RecBytes = sizeof(Rec)>
 __device__ __forceinline__ uint32_t wait_chunk(uint32_t ring, int c, int lane) {
   cp_async_wait<WALK_RING - 1>();  // this lane's copy of chunk c has landed ...
   __syncwarp();                   // ... and so have the other lanes'
-  return ring + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES + lane * 48;
+  return ring + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<RecBytes> + lane * RecBytes;
 }
 
 // Cull and compact one chunk of a front-to-back walk: the lane's record my_rec (patch index my_idx,

@@ -27,7 +27,6 @@ namespace gsb {
 #endif
 
 constexpr int SREC_BYTES = sf::kRecFloats * 4;  // 80
-constexpr int SCHUNK_BYTES = 32 * SREC_BYTES;   // one 32-record chunk of the ring
 static_assert(SREC_BYTES == 80, "surfel record must be 80 bytes");
 
 __device__ __forceinline__ pg::Cam surfel_cam(const float *__restrict__ Rcw, const float *__restrict__ tcw,
@@ -50,12 +49,6 @@ __device__ __forceinline__ void surfel_rows(const float *__restrict__ pws, const
 }
 
 #define ROWK(K) (sm + tid * TileT<K>::S)
-
-__device__ __forceinline__ uint2 lds64u(uint32_t a) {
-  uint2 v;
-  asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
-  return v;
-}
 
 template <int K3>
 __global__ void __launch_bounds__(PG) k_surfel_fwd(int N, const float *__restrict__ pws, const float *__restrict__ rots,
@@ -131,22 +124,8 @@ __global__ void __launch_bounds__(PG) k_surfel_bwd(int N, const float *__restric
   st_pair(g_us, o, row[16], row[17]);
 }
 
-// ---- the rasterizers' 80-byte record walk (raster_walk.cuh's protocol; these helpers sit beside
-// its 48-byte ones)
-
-// The 80-byte record at `rec` into shared memory at `dst`: five 16-byte cp.async.
-__device__ __forceinline__ void gather_surfel(const float4 *rec, uint32_t dst) {
-  const char *src = reinterpret_cast<const char *>(rec);
-#pragma unroll
-  for (int k = 0; k < 5; k++) cp_async16_sa(dst + 16 * k, src + 16 * k);
-}
-
-// The lane's record of chunk c, once the chunk has landed in every lane.
-__device__ __forceinline__ uint32_t wait_surfel_chunk(uint32_t ring, int c, int lane) {
-  cp_async_wait<WALK_RING - 1>();
-  __syncwarp();
-  return ring + (c & (WALK_RING - 1)) * SCHUNK_BYTES + lane * SREC_BYTES;
-}
+// ---- the rasterizers' 80-byte record walk: raster_walk.cuh's protocol and chunk helpers at
+// SREC_BYTES, with the surfel record's own cull
 
 // Can the record reach alpha' >= 0.002 in the block [bx0, bx1] x [by0, by1]?  Its cull box (u +-
 // the half-extents of sf::cull_extent) bounds {G3 <= t} and {G2 <= t}: outside it min(G3, G2) > t.
@@ -217,7 +196,7 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
     const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
     float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
     float *__restrict__ normal_image, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * SCHUNK_BYTES];
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<SREC_BYTES>];
   __shared__ __align__(16) uint2 s_list[4][32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const size_t HW = (size_t)H * W;
@@ -248,16 +227,17 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
         const int nch = (len + 31) >> 5;
         auto issue = [&](int c) {
           if (c < nch && c * 32 + lane < len)
-            gather_surfel(recs + 5 * (size_t)__ldg(ids + c * 32 + lane),
-                          ring_addr + (c & (WALK_RING - 1)) * SCHUNK_BYTES + lane * SREC_BYTES);
+            gather_record<SREC_BYTES>(recs + 5 * (size_t)__ldg(ids + c * 32 + lane),
+                                      ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<SREC_BYTES> +
+                                          lane * SREC_BYTES);
           cp_async_commit();
         };
 #pragma unroll
         for (int r = 0; r < WALK_RING; r++) issue(r);
         const float bx0 = (float)bp.rx0, bx1 = (float)(bp.rx0 + 7), by0 = (float)bp.ry0, by1 = (float)(bp.ry0 + 7);
         for (int c = 0; c < nch; c++) {
-          const int n = surfel_compact(wait_surfel_chunk(ring_addr, c, lane), c * 32 + lane, len, bx0, bx1, by0, by1,
-                                       list_addr, lane, false);
+          const int n = surfel_compact(wait_chunk<SREC_BYTES>(ring_addr, c, lane), c * 32 + lane, len, bx0, bx1, by0,
+                                       by1, list_addr, lane, false);
           for (int i = 0; i < n; i++) {
             const uint2 e = lds64u(list_addr + i * 8);
             SRecRegs r;
@@ -314,7 +294,7 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
     int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     SurfelGrads dl, float *__restrict__ rows, int *__restrict__ work) {
-  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * SCHUNK_BYTES];
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<SREC_BYTES>];
   __shared__ __align__(16) uint2 s_list[4][32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const size_t HW = (size_t)H * W;
@@ -359,16 +339,17 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
       const int nch = (wmax + 31) >> 5;
       auto issue = [&](int c) {
         if (c >= 0 && c * 32 + lane < wmax)
-          gather_surfel(recs + 5 * (size_t)__ldg(ids + c * 32 + lane),
-                        ring_addr + (c & (WALK_RING - 1)) * SCHUNK_BYTES + lane * SREC_BYTES);
+          gather_record<SREC_BYTES>(recs + 5 * (size_t)__ldg(ids + c * 32 + lane),
+                                    ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<SREC_BYTES> +
+                                        lane * SREC_BYTES);
         cp_async_commit();
       };
 #pragma unroll
       for (int r = 0; r < WALK_RING; r++) issue(nch - 1 - r);
       const float bx0 = (float)bp.rx0, bx1 = (float)(bp.rx0 + 7), by0 = (float)bp.ry0, by1 = (float)(bp.ry0 + 7);
       for (int c = nch - 1; c >= 0; c--) {
-        const int n = surfel_compact(wait_surfel_chunk(ring_addr, c, lane), c * 32 + lane, wmax, bx0, bx1, by0, by1,
-                                     list_addr, lane, true);
+        const int n = surfel_compact(wait_chunk<SREC_BYTES>(ring_addr, c, lane), c * 32 + lane, wmax, bx0, bx1, by0,
+                                     by1, list_addr, lane, true);
         for (int i = 0; i < n; i++) {
           const uint2 e = lds64u(list_addr + i * 8);
           const int idx = (int)e.y;

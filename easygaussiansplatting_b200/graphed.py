@@ -71,9 +71,11 @@ class GraphedFusedStep:
                              **camera_model_kwargs(cam))
         us, ci, col, dep, ar, rec = pre[:6]
         drawn = pre[6] if aa else alphas  # antialiased: the rasterizers composite alpha_eff
+        lib = ops._L()
+        enqueue = (lib.gsb_splat_forward_enqueue, [ops._ptr(t) for t in (us, ci, drawn, dep, col, ar, rec)])
         _, self._keep, (image, contrib, final_tau, ranges, gsid) = ops._capacity_frame(
-            cam.height, cam.width, us, ci, drawn, dep, col, ar, rec, self.P_cap, self.dk_cap, self.status,
-            enqueue=True)
+            cam.height, cam.width, us, [], lib.gsb_splat_workspace_bytes, enqueue, self.P_cap, self.dk_cap,
+            self.status)
         self._fwd = dict(us=us, cinv2ds=ci, colors=col, depths=dep, areas=ar, records=rec, contrib=contrib,
                          final_tau=final_tau, ranges=ranges, gsid=gsid, alphas=drawn, aa=aa, scales_f=scales,
                          alphas_f=alphas)

@@ -115,6 +115,11 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
+def _ptrs_if(on, *ts):
+    """the pointers of ts when `on`, else none: the arguments only some forms of an entry point take"""
+    return [_ptr(t) for t in ts] if on else []
+
+
 def _stream():
     return torch.cuda.current_stream().cuda_stream
 
@@ -239,41 +244,83 @@ def _bytes(n, dev):
     return torch.empty((n,), dtype=torch.uint8, device=dev)
 
 
-def _frame_buffers(lib, dev, H, W, N, P, rgbd=False):
-    """the sort workspace for P patch slots and splat's five outputs (+ the depth and alpha planes)"""
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    ws = _bytes(lib.gsb_splat_workspace_bytes(N, H, W, P), dev)
-    planes = [torch.empty((H, W), dtype=torch.float32, device=dev) for _ in range(2)] if rgbd else []
+def _tiles(H, W):
+    return ((W + 15) // 16) * ((H + 15) // 16)
+
+
+def _check_drawn(H, W, ranges, planes, text):
+    """the per-pixel tensors of a drawn frame, (tensor, channels) in `planes`, against H x W (else
+    ValueError(text)), and its patch_range_per_tile against the tile grid"""
+    if any(t.numel() != c * H * W for t, c in planes):
+        raise ValueError(text)
+    if ranges.shape[0] != _tiles(H, W):
+        raise ValueError("patch_range_per_tile does not match the tile grid")
+
+
+def _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes):
+    """the sort workspace for P patch slots (ws_bytes: the family's workspace query) and splat's
+    five outputs, + one float32 plane of each shape in `planes`"""
+    ws = _bytes(ws_bytes(N, H, W, P), dev)
     return ws, [torch.empty((3, H, W), dtype=torch.float32, device=dev),
                 torch.empty((H, W), dtype=torch.int32, device=dev),
                 torch.empty((H, W), dtype=torch.float32, device=dev),
-                torch.empty((T, 2), dtype=torch.int32, device=dev),
-                torch.empty((P,), dtype=torch.int32, device=dev)] + planes
+                torch.empty((_tiles(H, W), 2), dtype=torch.int32, device=dev),
+                torch.empty((P,), dtype=torch.int32, device=dev)] + \
+        [torch.empty(shape, dtype=torch.float32, device=dev) for shape in planes]
 
 
-def _capacity_frame(H, W, us, cinv2ds, alphas, depths, colors, areas, records, P_cap, dk_cap, status,
-                    enqueue=False, rgbd=False):
-    """Bins, sorts and draws one frame with the sort sized from the bounds (P_cap, dk_cap):
-    gsb_splat_forward, or gsb_splat_forward_enqueue (no host wait: for CUDA graph capture), or
-    with rgbd gsb_splat_forward_rgbd.
-    -> (False when the frame outgrew a bound, its workspaces, the five outputs with P_cap
-    gsid slots, + depth and alpha with rgbd); `status` (pinned int32[4]) receives the status word."""
+def _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status):
+    """Bins, sorts and draws one frame with the sort sized from the bounds (P_cap, dk_cap) through
+    forward = (gsb_splat_forward, _rgbd, _enqueue or gsb_splat_surfel_forward, the pointers of its
+    frame's own inputs).  planes, ws_bytes: as for `_frame_buffers`.
+    -> (False when the frame outgrew a bound, its workspaces, the five outputs with P_cap gsid
+    slots + the planes); `status` (pinned int32[4]) receives the status word."""
     lib, N, dev = _L(), us.shape[0], us.device
-    if rgbd and enqueue:
-        raise ValueError("the RGB-D frame has no enqueue-only form")
     bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
-    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap, rgbd)
-    args = (H, W, N, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors), _ptr(areas),
-            _ptr(records), P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
-            *[_ptr(o) for o in out[:5]], status.data_ptr())
-    if rgbd:
-        rc = lib.gsb_splat_forward_rgbd(*args, _ptr(out[5]), _ptr(out[6]), _stream())
-    else:
-        forward = lib.gsb_splat_forward_enqueue if enqueue else lib.gsb_splat_forward
-        rc = forward(*args, _stream())
+    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap, planes, ws_bytes)
+    entry, inputs = forward
+    rc = entry(H, W, N, *inputs, P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
+               *[_ptr(o) for o in out[:5]], status.data_ptr(), *[_ptr(o) for o in out[5:]], _stream())
     if rc != GSB_CAPACITY_EXCEEDED:
         _lib.check(rc, lib)
     return rc == 0, (bin_ws, ws), out
+
+
+def _frame(H, W, us, depths, areas, planes, ws_bytes, forward, render, capacity, cap_key):
+    """The one frame driver of `splat`, `splat_rgbd` and `splat_surfel`: bins the frame (MUTATES
+    depths / areas of what touches no tile) and draws it.  planes, ws_bytes: as for
+    `_frame_buffers`; forward, render: (the capacity / the exact entry point, the pointers of the
+    frame's own inputs to it).  capacity: size the sort from the bounds learnt for cap_key by the
+    previous frame of the same shape; a frame that outgrows them is redone the exact way.
+    -> (the sort workspace, its patch slots, the outputs with gsid_per_patch of the frame's P)"""
+    lib, N, dev = _L(), us.shape[0], us.device
+    if capacity and cap_key in _CAPACITY and N > 0:
+        P_cap, dk_cap = _CAPACITY[cap_key]
+        status = _STATUS.get(dev.index)
+        if status is None:
+            status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
+        ok, (_, ws), out = _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status)
+        if ok:
+            CAPACITY_STATS["capacity_frames"] += 1
+            P, dkmax, _ = _decode_status(status)
+            _CAPACITY[cap_key] = _next_capacity(P, dkmax)
+            out[4] = out[4][:P]
+            return ws, P_cap, out
+        CAPACITY_STATS["outgrown"] += 1
+        del _CAPACITY[cap_key]  # outgrown: this frame the exact way (the in-place culls are idempotent)
+    bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
+    P, dkmax = C.c_int64(0), C.c_uint32(0)
+    _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
+                                 C.byref(P), C.byref(dkmax), _stream()), lib)
+    P = int(P.value)
+    ws, out = _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes)
+    if capacity:
+        CAPACITY_STATS["exact_frames"] += 1
+        _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
+    entry, inputs = render
+    _lib.check(entry(H, W, N, P, dkmax.value, *inputs, _ptr(bin_ws), _ptr(ws), ws.numel(), *[_ptr(o) for o in out],
+                     _stream()), lib)
+    return ws, P, out
 
 
 def _attach_records(gsid, records, ws, N, H, W, P_slots, inputs):
@@ -330,39 +377,15 @@ def _splat(height, width, us, cinv2ds, alphas, depths, colors, areas, records, c
     # the record cache key: what the records are packed from (depths last: only the RGB-D
     # backward reads the records' depth word, and it looks the records up with depths included)
     inputs = (us, cinv2ds, alphas, colors, depths)
-    cap_key = (dev.index, H, W, N)
+    own = [_ptr(t) for t in (us, cinv2ds, alphas, depths, colors)]
+    forward = (lib.gsb_splat_forward_rgbd if rgbd else lib.gsb_splat_forward, own + [_ptr(areas), _ptr(records)])
+    render = (lib.gsb_splat_render_rgbd if rgbd else lib.gsb_splat_render, own + [_ptr(records)])
     # the workspaces are consumed by kernels already enqueued on the current stream; the caching
     # allocator only reuses them for later work on the same stream
     with torch.cuda.device(dev):
-        if capacity and cap_key in _CAPACITY and N > 0:
-            P_cap, dk_cap = _CAPACITY[cap_key]
-            status = _STATUS.get(dev.index)
-            if status is None:
-                status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
-            ok, (_, ws), out = _capacity_frame(H, W, us, cinv2ds, alphas, depths, colors, areas, records, P_cap,
-                                               dk_cap, status, rgbd=rgbd)
-            if ok:
-                CAPACITY_STATS["capacity_frames"] += 1
-                P, dkmax, _ = _decode_status(status)
-                _CAPACITY[cap_key] = _next_capacity(P, dkmax)
-                out[4] = out[4][:P]
-                _attach_records(out[4], records, ws, N, H, W, P_cap, inputs)
-                return out
-            CAPACITY_STATS["outgrown"] += 1
-            del _CAPACITY[cap_key]  # outgrown: this frame the exact way (the in-place culls are idempotent)
-        bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
-        P, dkmax = C.c_int64(0), C.c_uint32(0)
-        _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
-                                     C.byref(P), C.byref(dkmax), _stream()), lib)
-        P = int(P.value)
-        ws, out = _frame_buffers(lib, dev, H, W, N, P, rgbd)
-        if capacity:
-            CAPACITY_STATS["exact_frames"] += 1
-            _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
-        render = lib.gsb_splat_render_rgbd if rgbd else lib.gsb_splat_render
-        _lib.check(render(H, W, N, P, dkmax.value, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(depths), _ptr(colors),
-                          _ptr(records), _ptr(bin_ws), _ptr(ws), ws.numel(), *[_ptr(o) for o in out], _stream()), lib)
-        _attach_records(out[4], records, ws, N, H, W, P, inputs)
+        ws, P_slots, out = _frame(H, W, us, depths, areas, [(H, W)] * 2 if rgbd else [], lib.gsb_splat_workspace_bytes,
+                                  forward, render, capacity, (dev.index, H, W, N))
+        _attach_records(out[4], records, ws, N, H, W, P_slots, inputs)
     return out
 
 
@@ -459,20 +482,17 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
     dl = _chk(dloss_dgammas, "dloss_dgammas")
     _same_device(us, cinv2ds, alphas, colors, contrib, final_tau, ranges, gsid, dl)
     N = us.shape[0]
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    if contrib.numel() != H * W or final_tau.numel() != H * W or dl.numel() != 3 * H * W:
-        raise ValueError("contrib / final_tau / dloss_dgammas do not match height x width")
-    if ranges.shape[0] != T:
-        raise ValueError("patch_range_per_tile does not match the tile grid")
+    _check_drawn(H, W, ranges, ((contrib, 1), (final_tau, 1), (dl, 3)),
+                 "contrib / final_tau / dloss_dgammas do not match height x width")
     if not (cinv2ds.shape[0] == N and alphas.numel() == N and colors.shape[0] == N):
         raise ValueError("splatB inputs disagree on N")
     if rgbd:
         depths = _chk(depths, "depths")
-        dld = _chk(dloss_ddepth, "dloss_ddepth"); dla = _chk(dloss_dalpha, "dloss_dalpha")
-        _same_device(us, depths, dld, dla)
+        dloss_ddepth = _chk(dloss_ddepth, "dloss_ddepth"); dloss_dalpha = _chk(dloss_dalpha, "dloss_dalpha")
+        _same_device(us, depths, dloss_ddepth, dloss_dalpha)
         if depths.numel() != N:
             raise ValueError("splatB_rgbd inputs disagree on N")
-        if dld.numel() != H * W or dla.numel() != H * W:
+        if dloss_ddepth.numel() != H * W or dloss_dalpha.numel() != H * W:
             raise ValueError("dloss_ddepth / dloss_dalpha do not match height x width")
     if records is not None:
         records = _chk(records, "records", last=12, ndim=2)
@@ -500,26 +520,14 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
             recs = _cached_records(gsid, key) if P > 0 else None
         # with cached records only the [N,9] moment rows are needed from the workspace
         ws = _bytes(lib.gsb_splat_backward_workspace_bytes(N, H, W, 0 if recs else P), dev)
-        if rgbd and absgrad:
-            _lib.check(lib.gsb_splat_backward_rgbd_abs(
-                H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
-                _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dld), _ptr(dla), recs, _ptr(ws), ws.numel(),
-                _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol), _ptr(moments), _ptr(ddepths), _ptr(dabs), _stream()), lib)
-        elif rgbd:
-            _lib.check(lib.gsb_splat_backward_rgbd(
-                H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
-                _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dld), _ptr(dla), recs, _ptr(ws), ws.numel(),
-                _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol), _ptr(moments), _ptr(ddepths), _stream()), lib)
-        elif absgrad:
-            _lib.check(lib.gsb_splat_backward_abs(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
-                                                  _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
-                                                  recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da),
-                                                  _ptr(dcol), _ptr(moments), _ptr(dabs), _stream()), lib)
-        else:
-            _lib.check(lib.gsb_splat_backward(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors),
-                                              _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
-                                              recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc), _ptr(da), _ptr(dcol),
-                                              _ptr(moments), _stream()), lib)
+        # gsb_splat_backward{,_rgbd}{,_abs}: the RGB-D forms take depths, the two planes' gradients and
+        # dloss_ddepths, the _abs forms dloss_dus_abs last
+        entry = getattr(lib, "gsb_splat_backward" + ("_rgbd" if rgbd else "") + ("_abs" if absgrad else ""))
+        _lib.check(entry(H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), *_ptrs_if(rgbd, depths),
+                         _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
+                         *_ptrs_if(rgbd, dloss_ddepth, dloss_dalpha), recs, _ptr(ws), ws.numel(), _ptr(du), _ptr(dc),
+                         _ptr(da), _ptr(dcol), _ptr(moments), *_ptrs_if(rgbd, ddepths), *_ptrs_if(absgrad, dabs),
+                         _stream()), lib)
     if moments_only:
         out = [moments, ddepths] if rgbd else moments
     else:
@@ -548,10 +556,7 @@ def _feature_frame(height, width, features, contrib, patch_range_per_tile, gsid_
     ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
     gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
     _same_device(features, contrib, ranges, gsid)
-    if contrib.numel() != H * W:
-        raise ValueError("contrib does not match height x width")
-    if ranges.shape[0] != ((W + 15) // 16) * ((H + 15) // 16):
-        raise ValueError("patch_range_per_tile does not match the tile grid")
+    _check_drawn(H, W, ranges, ((contrib, 1),), "contrib does not match height x width")
     P = gsid.numel()
     attrs = (None,) * 4
     recs = None
@@ -985,16 +990,6 @@ def surfel_preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, 
     return out
 
 
-def _surfel_buffers(lib, dev, H, W, N, P):
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    f = dict(dtype=torch.float32, device=dev)
-    ws = _bytes(lib.gsb_splat_surfel_workspace_bytes(N, H, W, P), dev)
-    return ws, [torch.empty((3, H, W), **f), torch.empty((H, W), dtype=torch.int32, device=dev),
-                torch.empty((H, W), **f), torch.empty((T, 2), dtype=torch.int32, device=dev),
-                torch.empty((P,), dtype=torch.int32, device=dev), torch.empty((H, W), **f), torch.empty((H, W), **f),
-                torch.empty((3, H, W), **f)]
-
-
 def splat_surfel(height, width, us, depths, areas, records, capacity=False):
     """Bins the surfels (us, areas, depths: the binning of `splat`, which MUTATES depths / areas of
     surfels that touch no tile) and draws them.  -> [image[3,H,W], contrib[H,W] i32,
@@ -1014,40 +1009,11 @@ def splat_surfel(height, width, us, depths, areas, records, capacity=False):
     if not (depths.numel() == N and areas.shape[0] == N and records.shape[0] == N):
         raise ValueError("splat_surfel inputs disagree on N")
     dev, lib = us.device, _L()
-    cap_key = ("surfel", dev.index, H, W, N)
     with torch.cuda.device(dev):
-        if capacity and cap_key in _CAPACITY and N > 0:
-            P_cap, dk_cap = _CAPACITY[cap_key]
-            status = _STATUS.get(dev.index)
-            if status is None:
-                status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
-            bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
-            ws, out = _surfel_buffers(lib, dev, H, W, N, P_cap)
-            rc = lib.gsb_splat_surfel_forward(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(records), P_cap,
-                                              dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
-                                              *[_ptr(o) for o in out[:5]], status.data_ptr(),
-                                              *[_ptr(o) for o in out[5:]], _stream())
-            if rc != GSB_CAPACITY_EXCEEDED:
-                _lib.check(rc, lib)
-                CAPACITY_STATS["capacity_frames"] += 1
-                P, dkmax, _ = _decode_status(status)
-                _CAPACITY[cap_key] = _next_capacity(P, dkmax)
-                out[4] = out[4][:P]
-                return out
-            CAPACITY_STATS["outgrown"] += 1
-            del _CAPACITY[cap_key]  # outgrown: this frame the exact way (the in-place culls are idempotent)
-        bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
-        P, dkmax = C.c_int64(0), C.c_uint32(0)
-        _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
-                                     C.byref(P), C.byref(dkmax), _stream()), lib)
-        P = int(P.value)
-        ws, out = _surfel_buffers(lib, dev, H, W, N, P)
-        if capacity:
-            CAPACITY_STATS["exact_frames"] += 1
-            _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
-        _lib.check(lib.gsb_splat_surfel_render(H, W, N, P, dkmax.value, _ptr(us), _ptr(depths), _ptr(records),
-                                               _ptr(bin_ws), _ptr(ws), ws.numel(), *[_ptr(o) for o in out],
-                                               _stream()), lib)
+        _, _, out = _frame(H, W, us, depths, areas, [(H, W), (H, W), (3, H, W)], lib.gsb_splat_surfel_workspace_bytes,
+                           (lib.gsb_splat_surfel_forward, [_ptr(us), _ptr(depths), _ptr(areas), _ptr(records)]),
+                           (lib.gsb_splat_surfel_render, [_ptr(us), _ptr(depths), _ptr(records)]), capacity,
+                           ("surfel", dev.index, H, W, N))
     return out
 
 
@@ -1063,11 +1029,7 @@ def splatB_surfel(height, width, records, contrib, final_tau, patch_range_per_ti
     ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
     gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
     _same_device(records, contrib, final_tau, ranges, gsid)
-    T = ((W + 15) // 16) * ((H + 15) // 16)
-    if contrib.numel() != H * W or final_tau.numel() != H * W:
-        raise ValueError("contrib / final_tau do not match height x width")
-    if ranges.shape[0] != T:
-        raise ValueError("patch_range_per_tile does not match the tile grid")
+    _check_drawn(H, W, ranges, ((contrib, 1), (final_tau, 1)), "contrib / final_tau do not match height x width")
     planes = []
     for name, t, n in (("dloss_dimage", dloss_dimage, 3), ("dloss_ddepth", dloss_ddepth, 1),
                        ("dloss_dalpha", dloss_dalpha, 1), ("dloss_dnormal", dloss_dnormal, 3)):
