@@ -18,6 +18,7 @@ namespace sf {
 
 constexpr float kFilterInvSquare = 2.0f;  // G2 = 2 |p - u|^2 (2DGS's FilterInvSquare)
 constexpr float kCutoff2 = 9.0f;          // binning footprint: the 3-sigma disk a^2 + b^2 <= 9
+constexpr float kAreaCap = 16777216.0f;   // 2^24: the largest binning half-extent (areas), exact in fp32
 constexpr int kRecFloats = 20;            // the rasterizers' 80-byte record
 constexpr int kRowFloats = 18;            // the backward rasterizer's per-Gaussian gradient row
 
@@ -68,7 +69,8 @@ GSB_HD void geometry(const float pw[3], const float q[4], const float s[3], cons
 }
 
 // Half-extents around u of the bounding box of {a^2 + b^2 <= lv} (through M) and of the filter disk
-// {2 |p - u|^2 <= lv}.  The ellipse's box comes from its dual conic M diag(1, 1, -1/lv) M^T:
+// {2 |p - u|^2 <= lv}.  The ellipse's box comes from its dual conic M diag(1, 1, -1/lv) M^T, with
+// rows 1 and 2 of M taken relative to u (M[k][j] - u_k M[2][j]):
 //   D = m3z^2 - lv (m3x^2 + m3y^2)  (> 0: the disk lies in front of the camera, a bounded ellipse)
 //   centre_k = (M[k][2] M[2][2] - lv (M[k][0] M[2][0] + M[k][1] M[2][1])) / D
 //   half_k^2 = centre_k^2 - (M[k][2]^2 - lv (M[k][0]^2 + M[k][1]^2)) / D
@@ -79,11 +81,13 @@ GSB_HD bool footprint(const float M[9], const float u[2], float lv, float ext[2]
   const float Di = 1.0f / D;
   const float r = sqrtf(lv / kFilterInvSquare);
   for (int k = 0; k < 2; k++) {
-    const float *m = M + 3 * k;
+    // row k shifted to u (pixel coordinate p_k - u_k): centre and half^2 are then O(half), not O(u),
+    // and half^2 does not cancel two terms of size u^2 (0.4 px of error at u ~ 4000 px otherwise)
+    const float m[3] = {fmaf(-u[k], M[6], M[3 * k]), fmaf(-u[k], M[7], M[3 * k + 1]), fmaf(-u[k], M[8], M[3 * k + 2])};
     const float cen = (m[2] * M[8] - lv * (m[0] * M[6] + m[1] * M[7])) * Di;
     const float hh = cen * cen - (m[2] * m[2] - lv * (m[0] * m[0] + m[1] * m[1])) * Di;
     const float h = sqrtf(fmaxf(hh, 0.f));
-    ext[k] = fmaxf(fmaxf(fabsf(cen + h - u[k]), fabsf(cen - h - u[k])), r);
+    ext[k] = fmaxf(fmaxf(fabsf(cen + h), fabsf(cen - h)), r);
   }
   return true;
 }
@@ -182,7 +186,7 @@ GSB_HD void fold_du(const float M[9], const float gu[2], float gM[9]) {
 }
 
 // Forward of one surfel: u, depth (-1 when culled), areas (integer half-extents of the 3-sigma
-// footprint, 0 when culled), colour, and its 80-byte record
+// footprint, at most 2^24, 0 when culled), colour, and its 80-byte record
 //   [M (9), alpha, u (2), cull half-extents (2), colour (3), n (3)]
 template <int K3>
 GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], const float *sh /*[K3][3]*/,
@@ -198,11 +202,12 @@ GSB_HD void forward_one(const float pw[3], const float q[4], const float s[3], c
   for (int l = 0; l < K3; l++)
     for (int c = 0; c < 3; c++) col[c] = fmaf(Y[l], sh[3 * l + c], col[c]);
   float ext[2] = {0.f, 0.f};
-  bool keep = g.keep && footprint(g.M, g.u, kCutoff2, ext);
+  const bool keep = g.keep && footprint(g.M, g.u, kCutoff2, ext);
   if (keep) {
-    area[0] = (int)ceilf(ext[0]);
-    area[1] = (int)ceilf(ext[1]);
-    keep = area[0] < (1 << 24) && area[1] < (1 << 24);
+    // clamped, not culled: a disk whose near edge grazes the camera plane has a finite visible part
+    // however large its footprint, and a 2^24 px half-extent still covers every tile of a frame
+    area[0] = ext[0] < kAreaCap ? (int)ceilf(ext[0]) : (int)kAreaCap;
+    area[1] = ext[1] < kAreaCap ? (int)ceilf(ext[1]) : (int)kAreaCap;
   }
   for (int k = 0; k < kRecFloats; k++) rec[k] = 0.f;
   if (!keep) {

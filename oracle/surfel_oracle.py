@@ -14,6 +14,7 @@ from . import oracle as orc
 ALPHA_CLAMP, ALPHA_SKIP, TAU_STOP = 0.99, 0.002, 1e-4
 FILTER = 2.0    # G2 = 2 |p - u|^2
 CUTOFF2 = 9.0   # the binning footprint: a^2 + b^2 <= 9
+AREA_CAP = 2 ** 24  # binning half-extents at or above it are clamped to it, not culled
 
 _C1 = 0.4886025119029199
 _C20, _C22, _C24 = 1.0925484305920792, 0.31539156525252005, 0.5462742152960396
@@ -67,7 +68,8 @@ def footprint(M, u, lv):
 
 
 def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy):
-    """per-surfel stages -> dict(M[N,3,3], u[N,2], depths[N] (-1 culled), areas[N,2] i32,
+    """per-surfel stages -> dict(M[N,3,3], u[N,2], depths[N] (-1 culled), areas[N,2] i32 (at most AREA_CAP),
+    ext[N,2] (the fp64 binning half-extents),
     colors[N,3], n[N,3], keep[N], and what the backward needs)"""
     f = lambda a: np.asarray(a, dtype=np.float64)
     pws, rots, scales, shs = f(pws), f(rots), f(scales), f(shs).reshape(len(pws), -1)
@@ -88,13 +90,14 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy):
     u = np.stack([fx * pc[:, 0] / z + cx, fy * pc[:, 1] / z + cy], 1)
     ext, ok = footprint(M, u, CUTOFF2)
     keep &= ok
-    areas = np.where(keep[:, None], np.ceil(ext), 0).astype(np.int32)
+    areas = np.where(keep[:, None], np.where(ext < AREA_CAP, np.ceil(np.minimum(ext, AREA_CAP)), AREA_CAP), 0)
+    areas = areas.astype(np.int32)
     d = pws - twc
     dn = np.linalg.norm(d, axis=1)
     r = d / dn[:, None] if k > 1 else np.zeros_like(d)
     Y, dY = sh_basis(r, k)
     col = 0.5 + np.einsum("nl,nlc->nc", Y, shs.reshape(N, k, 3))
-    return dict(M=M, u=np.where(keep[:, None], u, 0), depths=np.where(keep, pc[:, 2], -1.0), areas=areas,
+    return dict(M=M, u=np.where(keep[:, None], u, 0), depths=np.where(keep, pc[:, 2], -1.0), areas=areas, ext=ext,
                 colors=col, n=n, keep=keep, pc=pc, qn=qn, qnorm=qnorm, R=R, axes=axes, sgn=sgn, scales=scales,
                 Y=Y, dY=dY, r=r, dn=dn, shs=shs, Rcw=Rcw, K=K, k=k)
 
@@ -166,22 +169,26 @@ def render(H, W, pre, alphas, bins, delta=None, margin=2e-5):
     return out
 
 
-def render_backward(H, W, pre, alphas, bins, fwd, dl_image, dl_depth, dl_alpha, dl_normal):
+def render_backward(H, W, pre, alphas, bins, fwd, dl_image, dl_depth, dl_alpha, dl_normal, abs_rows=False):
     """the analytic backward of `render` on its own forward state -> rows[N,18] =
-    [dL/dM (row-major 9), dL/dalpha, dL/dcolour (3), dL/dn (3), dL/ddelta (2)], dL/du folded into dL/dM"""
+    [dL/dM (row-major 9), dL/dalpha, dL/dcolour (3), dL/dn (3), dL/ddelta (2)], dL/du folded into dL/dM.
+    abs_rows: also -> the same rows summed over the absolute values of every per-pixel product that
+    makes up an entry (the scale of an fp32 sum's rounding: the conditioning of that entry)"""
     alphas = np.asarray(alphas, dtype=np.float64).reshape(-1)
     N = len(alphas)
     _, ranges, gsid, _ = bins
     z2 = lambda a, s: np.zeros(s) if a is None else np.asarray(a, dtype=np.float64).reshape(s)
     dli, dld, dla, dln = z2(dl_image, (3, H, W)), z2(dl_depth, (H, W)), z2(dl_alpha, (H, W)), z2(dl_normal, (3, H, W))
     rows = np.zeros((N, 18))
-    gU = np.zeros((N, 2))
+    absr = np.zeros((N, 18))
+    across = lambda p, q: np.stack([p[:, 1] * q[:, 2] + p[:, 2] * q[:, 1], p[:, 2] * q[:, 0] + p[:, 0] * q[:, 2],
+                                    p[:, 0] * q[:, 1] + p[:, 1] * q[:, 0]], 1)
     for t, X, Y in _tiles(H, W, ranges):
         Xf, Yf = X.astype(np.float64), Y.astype(np.float64)
         tau = fwd["final_tau"][Y, X].copy()
         cont = fwd["contrib"][Y, X]
         D = np.concatenate([dli[:, Y, X], dld[None, Y, X], dla[None, Y, X], dln[:, Y, X]])
-        sdot = np.zeros(len(X))
+        sdot, sabs = np.zeros(len(X)), np.zeros(len(X))
         ids = gsid[ranges[t, 0]:ranges[t, 1]]
         for j in range(len(ids) - 1, -1, -1):
             i = ids[j]
@@ -201,45 +208,58 @@ def render_backward(H, W, pre, alphas, bins, fwd, dl_image, dl_depth, dl_alpha, 
             diff = v - sdot
             sdot = sdot + ap * diff
             dap = np.where(on, tau * diff, 0.0)
+            vabs = np.sum(np.abs(D * vals), 0)
+            dapm = np.where(on, tau * (vabs + sabs), 0.0)  # |dL/dalpha'| before its cancellations
+            sabs = sabs + ap * (vabs + sabs)
             w = tau * ap
-            rows[i, 10:13] += D[:3] @ w
-            rows[i, 13:16] += D[5:] @ w
             unc = on & (ag <= ALPHA_CLAMP)
-            rows[i, 9] += np.sum(np.where(unc, dap * g, 0))
             dG = np.where(unc, -0.5 * dap * ap, 0.0)
             dz = w * D[3]
-            gM = np.zeros((3, 3))
-            gM[2, 2] += dz.sum()
             b3 = e["b3"] & on
             a, b = np.where(b3, e["a"], 0), np.where(b3, e["b"], 0)
             da = np.where(b3, dG * 2 * a + dz * M[2, 0], 0)
             db = np.where(b3, dG * 2 * b + dz * M[2, 1], 0)
-            gM[2, 0] += np.sum(dz * a)
-            gM[2, 1] += np.sum(dz * b)
             c2 = np.where(b3, e["c"][:, 2], 1.0)
             gc = np.stack([da / c2, db / c2, -(da * a + db * b) / c2], 1)
             ex = np.cross(e["hy"], gc)
             ey = np.cross(gc, e["hx"])
-            gM[0] -= ex.sum(0)
-            gM[1] -= ey.sum(0)
-            gM[2] += (Xf[:, None] * ex + Yf[:, None] * ey).sum(0)
-            rows[i, 16] -= np.sum(ex @ M[2])
-            rows[i, 17] -= np.sum(ey @ M[2])
-            f2 = on & ~e["b3"]
-            kk = np.where(f2, -2 * FILTER * dG, 0)
-            rows[i, 16] += np.sum(kk * e["dx"])
-            rows[i, 17] += np.sum(kk * e["dy"])
-            gU[i] += [np.sum(kk * e["dx"]), np.sum(kk * e["dy"])]
-            rows[i, :9] += gM.ravel()
-    # u = (m1z, m2z) / m3z
-    for i in range(N):
-        if pre["keep"][i] and gU[i].any():
-            M = pre["M"][i]
+            kk = np.where(on & ~e["b3"], -2 * FILTER * dG, 0)
+            # u = (m1z, m2z) / m3z: the filter branch's dL/du folded into dL/dM
             zi = 1.0 / M[2, 2]
-            rows[i, 2] += gU[i, 0] * zi
-            rows[i, 5] += gU[i, 1] * zi
-            rows[i, 8] -= (gU[i, 0] * M[0, 2] + gU[i, 1] * M[1, 2]) * zi * zi
-    return rows
+            gux, guy = kk * e["dx"], kk * e["dy"]
+            # every entry as a sum of per-pixel terms; mag: the size of the products inside a term
+            # (ex, ey are cross products of h with dL/dc, and dL/dc is made of dL/da, dL/db)
+            dGm = np.where(unc, 0.5 * dapm * ap, 0.0)
+            dam = np.where(b3, dGm * 2 * np.abs(a) + np.abs(dz * M[2, 0]), 0)
+            dbm = np.where(b3, dGm * 2 * np.abs(b) + np.abs(dz * M[2, 1]), 0)
+            aga = np.stack([dam, dbm, dam * np.abs(a) + dbm * np.abs(b)], 1) / np.abs(c2)[:, None]
+            guxm, guym = np.where(kk != 0, 2 * FILTER * dGm, 0) * np.abs(e["dx"]), \
+                np.where(kk != 0, 2 * FILTER * dGm, 0) * np.abs(e["dy"])
+            exa, eya = across(np.abs(e["hy"]), aga), across(aga, np.abs(e["hx"]))
+
+            def add(k, term, mag=None):
+                rows[i, k] += np.sum(term)
+                absr[i, k] += np.sum(np.abs(term) if mag is None else mag)
+
+            for k in range(3):
+                add(k, -ex[:, k], exa[:, k])
+                add(3 + k, -ey[:, k], eya[:, k])
+                add(6 + k, Xf * ex[:, k], Xf * exa[:, k])
+                add(6 + k, Yf * ey[:, k], Yf * eya[:, k])
+                add(16, -ex[:, k] * M[2, k], exa[:, k] * abs(M[2, k]))
+                add(17, -ey[:, k] * M[2, k], eya[:, k] * abs(M[2, k]))
+                add(10 + k, w * D[k])
+                add(13 + k, w * D[5 + k])
+            add(6, dz * a)
+            add(7, dz * b)
+            add(8, dz)
+            add(2, gux * zi, guxm * abs(zi))
+            add(5, guy * zi, guym * abs(zi))
+            add(8, -(gux * M[0, 2] + guy * M[1, 2]) * zi * zi, (guxm * abs(M[0, 2]) + guym * abs(M[1, 2])) * zi * zi)
+            add(9, np.where(unc, dap * g, 0), np.where(unc, dapm * g, 0))
+            add(16, gux, guxm)
+            add(17, guy, guym)
+    return (rows, absr) if abs_rows else rows
 
 
 def preprocess_backward(pre, rows, twc=None):
