@@ -65,6 +65,24 @@ def splat_backward_abs(height, width, us, cinv2ds, alphas, colors, fwd, dloss_dg
     return du, dabs, amb.astype(bool)
 
 
+def splat_backward_abs_rows(height, width, us, cinv2ds, alphas, colors, fwd, dloss_dgammas, depths=None,
+                            dloss_ddepth=None, dloss_dalpha=None, margin=2e-5):
+    """The absolute sums of k_draw_bwd_abs (given depths and the two planes, k_draw_bwd_rgbd_abs) next to
+    their moment rows, in fp64, with their conditioning.  -> the dict of `oracle.splat_backward_rows`
+    (`rgbd_oracle.splat_backward_rgbd_rows`) plus dus_abs[N,2], dus_abs_abs, dus_abs_maha, dus_abs_amb.
+    Every term of dus_abs is >= 0; dus_abs_abs also counts the cancellation inside A dx + B dy."""
+    from . import oracle as orc
+    from . import rgbd_oracle as org
+    if depths is None:
+        out = orc.splat_backward_rows(height, width, us, cinv2ds, alphas, colors, fwd, dloss_dgammas, margin)
+    else:
+        out = org.splat_backward_rgbd_rows(height, width, us, cinv2ds, alphas, colors, depths, fwd, dloss_dgammas,
+                                           dloss_ddepth, dloss_dalpha, margin)
+    for name, a in zip(("dus_abs", "dus_abs_abs", "dus_abs_maha", "dus_abs_amb"), out["raw"][:4]):
+        out[name] = a[:, 6:8].copy()
+    return out
+
+
 def splat_backward_rgbd_abs(height, width, us, cinv2ds, alphas, colors, depths, fwd, dloss_dgammas, dloss_ddepth,
                             dloss_dalpha, margin=2e-5):
     """orc_drawB_rgbd_abs on the RGB-D oracle's forward state `fwd` (dict from

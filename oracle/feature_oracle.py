@@ -48,14 +48,36 @@ def splat_features(height, width, us, cinv2ds, alphas, depths, areas, features, 
 
 
 def splat_backward_features(height, width, us, cinv2ds, alphas, fwd, features, dloss_dfeatures_map,
-                            return_ambiguous=False, margin=2e-5):
+                            return_ambiguous=False, margin=2e-5, rows=False):
     """Backward of `splat_features` on the forward state `fwd` (contrib, final_tau, ranges, gsid):
     dL/dF [D,H,W] -> dloss_dus[N,1,2], dloss_dcinv2ds[N,1,3], dloss_dalphas[N,1,1] (the sums over
-    the triples) and dloss_dfeatures[N,D] (+ bool[N], the union of the triples' ambiguity flags)"""
+    the triples) and dloss_dfeatures[N,D] (+ bool[N], the union of the triples' ambiguity flags).
+    rows: instead, the moment rows k_draw_feat_bwd adds (`oracle.splat_backward_rows`' dict summed over
+    the triples; rows 6-8 zero) and dfeatures[N,D] with dfeatures_abs / _maha / _amb.  Every conditioning
+    sum is linear in the per-channel magnitudes, so the triples' sums are the all-channel ones."""
     f = np.asarray(features, np.float32)
     N, D = f.shape
     dl = np.asarray(dloss_dfeatures_map, np.float64)
     dl_t = _triples(np.moveaxis(dl, 0, -1), D)  # [H,W,3] each
+    if rows:
+        out = None
+        dfeat = [np.zeros((N, len(dl_t) * 3)) for _ in range(4)]
+        for k, (trip, g) in enumerate(zip(_triples(f.astype(np.float64), D), dl_t)):
+            r = orc.splat_backward_rows(height, width, us, cinv2ds, alphas, np.ascontiguousarray(trip, np.float32),
+                                        fwd, np.ascontiguousarray(np.moveaxis(g, -1, 0), np.float32), margin=margin)
+            for j, key in enumerate(("rows", "abs_rows", "maha_rows", "amb_rows")):
+                dfeat[j][:, 3 * k:3 * k + 3] = r[key][:, 6:9]
+                r[key][:, 6:9] = 0
+            if out is None:
+                out = r
+            else:
+                for key in ("rows", "abs_rows", "maha_rows", "amb_rows"):
+                    out[key] = out[key] + r[key]
+                out["ambiguous"] = out["ambiguous"] | r["ambiguous"]
+        out.pop("raw")
+        for j, key in enumerate(("dfeatures", "dfeatures_abs", "dfeatures_maha", "dfeatures_amb")):
+            out[key] = dfeat[j][:, :D]
+        return out
     du = np.zeros((N, 1, 2)); dc = np.zeros((N, 1, 3)); da = np.zeros((N, 1, 1))
     dfeat = np.zeros((N, len(dl_t) * 3))
     amb = np.zeros(N, bool)

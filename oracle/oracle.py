@@ -173,6 +173,64 @@ def splat_backward(height, width, us, cinv2ds, alphas, colors, fwd, dloss_dgamma
     return (du, dc, da, dcol, amb.astype(bool)) if return_ambiguous else (du, dc, da, dcol)
 
 
+MOMENT_COLS = [0, 1, 2, 3, 4, 5, 8, 9, 10]  # the nine moment rows of the colour frame in drawB_rows' columns
+
+
+def drawB_rows(height, width, us, cinv2ds, alphas, values, fwd, dl_planes, margin=2e-5):
+    """orc_drawB_rows: orc_drawB's replay with nch channels (values[N,nch], dl_planes[nch,H,W]) on the
+    forward state `fwd`.  -> (rows, abs_rows, maha_rows, amb_rows) [N, 8 + nch] f64 and the bool[N] flags
+    of splat_backward; columns: w dx, w dy, w dx^2, w dx dy, w dy^2, dL/dalpha' g, the AbsGS terms
+    |w (A dx + B dy)|, |w (B dx + C dy)|, then wc dl_c per channel (gs_oracle.c)"""
+    us, cinv2ds = _f32(us), _f32(cinv2ds)
+    alphas, vals, dl = _f32(alphas).reshape(-1), _f32(values), _f32(dl_planes)
+    N, nch = vals.shape
+    H, W = int(height), int(width)
+    assert dl.shape == (nch, H, W)
+    out = [np.empty((N, 8 + nch)) for _ in range(4)]
+    amb = np.zeros(max(N, 1), dtype=np.uint8)[:N]
+    lib().orc_drawB_rows(H, W, N, nch, _p(fwd["ranges"]), _p(fwd["gsid"]), _p(us), _p(cinv2ds), _p(alphas),
+                         _p(vals), _p(np.ascontiguousarray(fwd["final_tau"], np.float64)),
+                         _p(np.ascontiguousarray(fwd["contrib"], np.int32)), _p(dl), *[_p(a) for a in out], _p(amb),
+                         C.c_double(margin))
+    return tuple(out) + (amb.astype(bool),)
+
+
+def rows_dict(raw):
+    """drawB_rows' output -> dict(rows[N,9], abs_rows, maha_rows, amb_rows, ambiguous bool[N]) in the moment-row
+    layout k_draw_bwd writes, plus raw: the [N, 8 + nch] arrays"""
+    c = MOMENT_COLS
+    R, Ab, Mh, Am, amb = raw
+    return dict(rows=R[:, c], abs_rows=Ab[:, c], maha_rows=Mh[:, c], amb_rows=Am[:, c], ambiguous=amb, raw=raw)
+
+
+def splat_backward_rows(height, width, us, cinv2ds, alphas, colors, fwd, dloss_dgammas, margin=2e-5):
+    """The moment rows k_draw_bwd writes (`splatB(..., moments_only=True)`), in fp64, with their conditioning.
+    -> rows_dict: rows[N,9] are w dx, w dy, w dx^2, w dx dy, w dy^2, dL/dalpha' g, wc dL/dgamma_rgb
+    (DESIGN 3.2); abs_rows the same sums over the magnitudes of every product in a term, maha_rows the
+    effect of the exponents' rounding, amb_rows the most a threshold decision within `margin` can move
+    an entry (gs_oracle.c)"""
+    return rows_dict(drawB_rows(height, width, us, cinv2ds, alphas, colors, fwd, dloss_dgammas, margin))
+
+
+def moments_to_grads(rows, cinv2ds):
+    """k_finalize_grads' conversion in fp64: rows[N,9] -> du[N,2], dconic[N,3], dalpha[N], dcolour[N,3]"""
+    m = np.asarray(rows, np.float64)
+    c = np.asarray(cinv2ds, np.float64)
+    A, B, Cc = c[:, 0], c[:, 1], c[:, 2]
+    du = -np.stack([A * m[:, 0] + B * m[:, 1], B * m[:, 0] + Cc * m[:, 1]], 1)
+    dc = np.stack([-0.5 * m[:, 2], -m[:, 3], -0.5 * m[:, 4]], 1)
+    return du, dc, m[:, 5].copy(), m[:, 6:9].copy()
+
+
+def moments_to_grads_bound(bound_rows, cinv2ds):
+    """the same conversion applied to a conditioning row (abs / maha / amb, >= 0): |A| b0 + |B| b1 for du.x
+    and so on -> du[N,2], dconic[N,3], dalpha[N], dcolour[N,3]"""
+    b = np.asarray(bound_rows, np.float64)
+    c = np.abs(np.asarray(cinv2ds, np.float64))
+    du = np.stack([c[:, 0] * b[:, 0] + c[:, 1] * b[:, 1], c[:, 1] * b[:, 0] + c[:, 2] * b[:, 1]], 1)
+    return du, np.stack([0.5 * b[:, 2], b[:, 3], 0.5 * b[:, 4]], 1), b[:, 5].copy(), b[:, 6:9].copy()
+
+
 def forward_cpu_splat(height, width, us, cinv2d, alpha, depth, color, areas):
     """gsplat/gausplat.py:185-245 (the forward_cpu.py renderer).  -> image[H,W,3] f64"""
     f64 = lambda a: np.ascontiguousarray(a, dtype=np.float64)

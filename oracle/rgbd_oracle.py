@@ -90,6 +90,23 @@ def splat_backward_rgbd(height, width, us, cinv2ds, alphas, colors, depths, fwd,
     return out + (amb.astype(bool),) if return_ambiguous else out
 
 
+def splat_backward_rgbd_rows(height, width, us, cinv2ds, alphas, colors, depths, fwd, dloss_dgammas, dloss_ddepth,
+                             dloss_dalpha, margin=2e-5):
+    """The moment rows and dL/dz k_draw_bwd_rgbd writes, in fp64, with their conditioning:
+    `oracle.drawB_rows` with the channels (colour, z, 1) against (dL/dimage, dL/dD, dL/dA).
+    -> oracle.rows_dict plus ddepths[N], ddepths_abs, ddepths_maha, ddepths_amb"""
+    from .oracle import drawB_rows, rows_dict
+    H, W = int(height), int(width)
+    vals = np.concatenate([_f32(colors).reshape(-1, 3), _f32(depths).reshape(-1, 1),
+                           np.ones((len(colors), 1), np.float32)], axis=1)
+    dl = np.concatenate([_f32(dloss_dgammas).reshape(3, H, W), _f32(dloss_ddepth).reshape(1, H, W),
+                         _f32(dloss_dalpha).reshape(1, H, W)])
+    out = rows_dict(drawB_rows(H, W, us, cinv2ds, alphas, vals, fwd, dl, margin))
+    for name, a in zip(("ddepths", "ddepths_abs", "ddepths_maha", "ddepths_amb"), out["raw"][:4]):
+        out[name] = a[:, 11].copy()
+    return out
+
+
 def chain_depth(Rcw, dloss_ddepths, depths):
     """The depth term of the chain: z = (Rcw pw + tcw)[2], so dL/dpws gains dL/dz Rcw[2,:];
     Gaussians culled for z < 0.2 (depths < 0.2) get 0.  -> [N,3] f64, added to chain_backward's pws."""
