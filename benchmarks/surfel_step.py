@@ -1,10 +1,11 @@
 """Cost of a 2D Gaussian Splatting step at BASELINE config 2 (1M Gaussians, SH degree 3, 1920x1080).
 
 The training step (forward + backward through autograd, every plane with an upstream gradient) of
-GSFunctionSurfel against GSFunctionFusedRGBD on the same scene, and per-kernel CUDA-event times
-(gsb_profile_*) of both: the per-Gaussian passes, the binning and the rasterizer pairs.  The two
-variants alternate in rounds so that clock and thermal drift hit both alike; medians over rounds
-are reported with the card's name and power limit, read in the same run.  Prints one JSON line.
+GSFunctionSurfel, GSFunctionSurfelGeometry (the 2DGS geometry terms, DESIGN 3.16: gradients on all
+six planes) and GSFunctionFusedRGBD on the same scene, and per-kernel CUDA-event times
+(gsb_profile_*) of each: the per-Gaussian passes, the binning and the rasterizer pairs.  The three
+variants take turns in rounds (their order rotating) so that clock and thermal drift hit all alike;
+medians over rounds are reported with the card's name and power limit, read in the same run.  Prints one JSON line.
 
     python benchmarks/surfel_step.py [--rounds 7] [--steps 10]
 """
@@ -22,7 +23,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from easygaussiansplatting_b200 import _lib  # noqa: E402
-from easygaussiansplatting_b200.gsfunction import Camera, GSFunctionFusedRGBD, GSFunctionSurfel  # noqa: E402
+from easygaussiansplatting_b200.gsfunction import (Camera, GSFunctionFusedRGBD, GSFunctionSurfel,  # noqa: E402
+                                                   GSFunctionSurfelGeometry)
 from easygaussiansplatting_b200.scene import synthetic_scene, upstream_gradient  # noqa: E402
 
 N, W, H, SH = 1_000_000, 1920, 1080, 48
@@ -49,6 +51,7 @@ def main():
     names = [lib.gsb_profile_kernel_name(i).decode() for i in range(lib.gsb_profile_kernels())]
     kid = {k: names.index(k) for k in ("preprocess_forward", "draw_rgbd", "draw_backward_rgbd", "preprocess_backward",
                                        "surfel_forward", "draw_surfel", "draw_surfel_backward", "surfel_backward",
+                                       "draw_2dgs", "draw_2dgs_backward",
                                        "rects+scan", "keys", "sort", "ranges")}
     sc = synthetic_scene(N, W, H, sh_dim=SH, seed=0)
     T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
@@ -62,6 +65,7 @@ def main():
     dld, dla = T(rng.normal(size=(H, W)).astype(np.float32) / 12.0), T(rng.normal(size=(H, W)).astype(np.float32))
 
     dln = T(rng.normal(size=(3, H, W)).astype(np.float32))
+    dlx, dlm = T(rng.normal(size=(H, W)).astype(np.float32)), T(rng.normal(size=(H, W)).astype(np.float32) / 12.0)
 
     def step_rgbd():
         for p in leaves:
@@ -76,6 +80,13 @@ def main():
         image, depth, alpha, normal, _ = GSFunctionSurfel.apply(params["pws"], params["shs"], alphas,
                                                                 params["scales"], params["rots"], us0, cam)
         torch.autograd.backward([image, depth, alpha, normal], [dl, dld, dla, dln])
+
+    def step_geometry():
+        for p in leaves:
+            p.grad = None
+        image, depth, alpha, normal, dist, med, _ = GSFunctionSurfelGeometry.apply(
+            params["pws"], params["shs"], alphas, params["scales"], params["rots"], us0, cam)
+        torch.autograd.backward([image, depth, alpha, normal, dist, med], [dl, dld, dla, dln, dlx, dlm])
 
     def timed(fn):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -105,15 +116,16 @@ def main():
         return out
 
     C_d, C_ll = ctypes.c_double, ctypes.c_longlong
-    for fn in (step_rgbd, step_surfel):  # warm-up: library load, capacity bounds, allocator
+    arms = {"rgbd": step_rgbd, "surfel": step_surfel, "geometry": step_geometry}
+    for fn in arms.values():  # warm-up: library load, capacity bounds, allocator
         for _ in range(3):
             fn()
     gpu, power = card()
-    res = {"rgbd": {"step": []}, "surfel": {"step": []}}
+    res = {m: {"step": []} for m in arms}
+    names_ = list(arms)
     for r in range(args.rounds):
-        order = (step_rgbd, step_surfel) if r % 2 == 0 else (step_surfel, step_rgbd)
-        for fn in order:
-            d = res["rgbd" if fn is step_rgbd else "surfel"]
+        for m in names_[r % 3:] + names_[:r % 3]:
+            fn, d = arms[m], res[m]
             d["step"].append(timed(fn))
             for k, v in kernels(fn).items():
                 d.setdefault(k, []).append(v)
@@ -124,6 +136,7 @@ def main():
         "ms_per_step": med,
         "spread_ms": {m: {k: round(float(np.max(v) - np.min(v)), 4) for k, v in d.items()} for m, d in res.items()},
         "surfel_vs_rgbd_step": round(med["surfel"]["step"] / med["rgbd"]["step"], 4),
+        "geometry_vs_surfel_step": round(med["geometry"]["step"] / med["surfel"]["step"], 4),
     }
     print(json.dumps(out))
 

@@ -108,6 +108,11 @@ SIGNATURES = {
     "gsb_splat_surfel_render": (_i, [_i, _i, _i, _i64, C.c_uint32] + [_vp] * 5 + [_sz] + [_vp] * 9),
     "gsb_splat_surfel_forward": (_i, [_i, _i, _i] + [_vp] * 4 + [_i64, C.c_uint32, _vp, _sz, _vp, _sz] + [_vp] * 10),
     "gsb_splat_surfel_backward": (_i, [_i, _i, _i, _i64] + [_vp] * 10 + [_sz] + [_vp] * 2),
+    "gsb_splat_2dgs_render": (_i, [_i, _i, _i, _i64, C.c_uint32] + [_vp] * 3 + [_f, _f] + [_vp] * 2 + [_sz]
+                              + [_vp] * 13),
+    "gsb_splat_2dgs_forward": (_i, [_i, _i, _i] + [_vp] * 4 + [_f, _f, _i64, C.c_uint32, _vp, _sz, _vp, _sz]
+                               + [_vp] * 14),
+    "gsb_splat_2dgs_backward": (_i, [_i, _i, _i, _i64] + [_vp] * 10 + [_sz, _vp, _f, _f] + [_vp] * 6),
     "gsb_profile_enable": (None, [_i]),
     "gsb_profile_kernels": (_i, []),
     "gsb_profile_kernel_name": (C.c_char_p, [_i]),

@@ -45,7 +45,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "draw_features", "draw_backward_features", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
                                              "mcmc_noise", "surfel_forward", "draw_surfel",
-                                             "draw_surfel_backward", "surfel_backward", "draw_backward_abs",
+                                             "draw_surfel_backward", "surfel_backward", "draw_2dgs",
+                                             "draw_2dgs_backward", "draw_backward_abs",
                                              "draw_backward_rgbd_abs",
                                              "adam", "draw_rgbd",
                                              "draw_backward_rgbd"};
@@ -809,23 +810,45 @@ int gsb_surfel_preprocess_backward(int N, int sh_dim3, const float *pws, const f
 
 size_t gsb_splat_surfel_workspace_bytes(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).bytes; }
 
-// The draw step of the surfel frame: its 80-byte records and its three further planes
+// The draw step of the surfel frame: its 80-byte records, its three further planes and, for the
+// 2DGS geometry frame (gsb_splat_2dgs_*), the geometry planes
 struct SurfelDraw {
   const float *records;
   float *depth_image, *alpha_image, *normal_image;
+  const GeoPlanes *geo = nullptr;
 
   int check() const {
-    GSB_REQUIRE(depth_image && alpha_image && normal_image, "splat_surfel: null output");
-    GSB_REQUIRE(aligned(depth_image, 16) && aligned(alpha_image, 16) && aligned(normal_image, 16),
-                "splat_surfel: misaligned output");
-    GSB_REQUIRE(aligned(records, 16), "splat_surfel: records misaligned");
+    const char *who = geo ? "splat_2dgs" : "splat_surfel";
+    if (!(depth_image && alpha_image && normal_image)) return arg_error(who, "null output");
+    if (!(aligned(depth_image, 16) && aligned(alpha_image, 16) && aligned(normal_image, 16)))
+      return arg_error(who, "misaligned output");
+    if (!aligned(records, 16)) return arg_error(who, "records misaligned");
     return 0;
   }
   int draw(int H, int W, int N, int64_t P, const FrameOut &o, const void *, int *work, cudaStream_t st) const {
     return launch_draw_surfel(H, W, o.ranges, P > 0 && N > 0 ? records : nullptr, o.gsid, o.image, o.contrib,
-                              o.final_tau, depth_image, alpha_image, normal_image, work, st);
+                              o.final_tau, depth_image, alpha_image, normal_image, geo, work, st);
   }
 };
+
+// near / far of the geometry planes: 0 < near < far, both finite
+static int check_near_far(const char *who, float near, float far) {
+  if (!(std::isfinite(near) && std::isfinite(far))) return arg_error(who, "near / far not finite");
+  if (!(near > 0.f)) return arg_error(who, "near <= 0");
+  if (!(far > near)) return arg_error(who, "far <= near");
+  return 0;
+}
+
+// The geometry planes of a 2DGS frame, checked (who = "splat_2dgs"): every plane present and 16-byte aligned
+static int geo_planes(const char *who, float near, float far, float *distortion, float *moments, float *median_depth,
+                      int32_t *median_contrib, GeoPlanes &g) {
+  if (int rc = check_near_far(who, near, far)) return rc;
+  if (!(distortion && moments && median_depth && median_contrib)) return arg_error(who, "null geometry plane");
+  if (!(aligned(distortion, 16) && aligned(moments, 16) && aligned(median_depth, 16) && aligned(median_contrib, 16)))
+    return arg_error(who, "misaligned geometry plane");
+  g = GeoPlanes{distortion, moments, median_depth, median_contrib, near, (float)((double)far / ((double)far - near))};
+  return 0;
+}
 
 int gsb_splat_surfel_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
                             const float *depths, const float *records, const void *bin_ws, void *ws, size_t ws_bytes,
@@ -877,7 +900,80 @@ int gsb_splat_surfel_backward(int H, int W, int N, int64_t P, const float *recor
   }
   char *b = static_cast<char *>(ws);
   return launch_draw_surfel_backward(H, W, N, patch_range_per_tile, P > 0 ? records : nullptr, gsid_per_patch, contrib,
-                                     final_tau, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, rows,
+                                     final_tau, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, nullptr, rows,
+                                     reinterpret_cast<int *>(b + SL.counters), (cudaStream_t)stream);
+}
+
+// ---- 2DGS geometry frames (surfel.cu k_draw_2dgs / k_draw_2dgs_bwd, DESIGN 3.16): the surfel frame
+// through the same render core, with the geometry planes
+
+int gsb_splat_2dgs_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us, const float *depths,
+                          const float *records, float near, float far, const void *bin_ws, void *ws, size_t ws_bytes,
+                          float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                          int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
+                          float *distortion, float *moments, float *median_depth, int32_t *median_contrib,
+                          gsb_stream_t stream) {
+  int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
+  if (rc) return rc;
+  GSB_REQUIRE(P >= 0, "splat_2dgs: bad P");
+  GSB_REQUIRE(P == 0 || (us && depths && records && bin_ws && ws && gsid_per_patch), "splat_2dgs: null pointer");
+  GeoPlanes g;
+  if ((rc = geo_planes("splat_2dgs", near, far, distortion, moments, median_depth, median_contrib, g))) return rc;
+  return render_frame("splat_2dgs", H, W, N, P, depth_key_max, us, nullptr, nullptr, const_cast<float *>(depths),
+                      nullptr, nullptr, false, const_cast<void *>(bin_ws), ws, ws_bytes,
+                      {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                      SurfelDraw{records, depth_image, alpha_image, normal_image, &g}, nullptr, (cudaStream_t)stream);
+}
+
+int gsb_splat_2dgs_forward(int H, int W, int N, const float *us, float *depths, int32_t *areas, const float *records,
+                           float near, float far, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                           size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                           float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                           uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                           float *distortion, float *moments, float *median_depth, int32_t *median_contrib,
+                           gsb_stream_t stream) {
+  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
+  if (rc) return rc;
+  GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_2dgs_forward: bad P_cap");
+  GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_2dgs_forward: null pointer");
+  GSB_REQUIRE(N == 0 || (us && depths && areas && records), "splat_2dgs_forward: null pointer");
+  GeoPlanes g;
+  if ((rc = geo_planes("splat_2dgs", near, far, distortion, moments, median_depth, median_contrib, g))) return rc;
+  return capacity_wait("splat_2dgs", P_cap, status_host, true, [&](const StatusRead *sr) {
+    return render_frame("splat_2dgs", H, W, N, P_cap, depth_key_cap, us, nullptr, nullptr, depths, nullptr, areas,
+                        false, bin_ws, ws, ws_bytes, {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                        SurfelDraw{records, depth_image, alpha_image, normal_image, &g}, sr, (cudaStream_t)stream);
+  });
+}
+
+int gsb_splat_2dgs_backward(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                            const float *final_tau, const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                            const float *dloss_dimage, const float *dloss_ddepth, const float *dloss_dalpha,
+                            const float *dloss_dnormal, void *ws, size_t ws_bytes, float *rows, float near, float far,
+                            const float *alpha_image, const float *moments, const int32_t *median_contrib,
+                            const float *dloss_ddistortion, const float *dloss_dmedian, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splatB_2dgs: bad N/H/W/P");
+  GSB_REQUIRE(grid_fits(H, W), "splatB_2dgs: more than 65535 tiles in a row or column");
+  if (int rc = check_near_far("splatB_2dgs", near, far)) return rc;
+  if (N == 0) return 0;
+  GSB_REQUIRE(rows != nullptr, "splatB_2dgs: null output");
+  const SortLayout SL = sort_layout(N, H, W, 0);
+  GSB_REQUIRE(ws != nullptr && aligned(ws, 16) && ws_bytes >= SL.bytes, "splatB_2dgs: workspace too small");
+  const bool with_geo = dloss_ddistortion != nullptr || dloss_dmedian != nullptr;
+  if (P > 0) {
+    GSB_REQUIRE(records && contrib && final_tau && patch_range_per_tile && gsid_per_patch, "splatB_2dgs: null pointer");
+    GSB_REQUIRE(aligned(records, 16) && aligned(patch_range_per_tile, 8), "splatB_2dgs: misaligned input");
+    GSB_REQUIRE(!with_geo || (alpha_image && moments && median_contrib), "splatB_2dgs: null geometry plane");
+    // the kernel reads these planes one 4-byte element at a time
+    GSB_REQUIRE(!with_geo || (aligned(alpha_image, 4) && aligned(moments, 4) && aligned(median_contrib, 4) &&
+                              aligned(dloss_ddistortion, 4) && aligned(dloss_dmedian, 4)),
+                "splatB_2dgs: misaligned geometry plane");
+  }
+  const GeoGrads g{dloss_ddistortion, dloss_dmedian, alpha_image, moments, median_contrib, near,
+                   (float)((double)far / ((double)far - near))};
+  char *b = static_cast<char *>(ws);
+  return launch_draw_surfel_backward(H, W, N, patch_range_per_tile, P > 0 ? records : nullptr, gsid_per_patch, contrib,
+                                     final_tau, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, &g, rows,
                                      reinterpret_cast<int *>(b + SL.counters), (cudaStream_t)stream);
 }
 

@@ -19,7 +19,8 @@ enum KernelId {
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
   K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
-  K_MCMC_ROWS, K_MCMC_NOISE, K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
+  K_MCMC_ROWS, K_MCMC_NOISE, K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
+  K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
   ProfScope(int id, cudaStream_t st);
@@ -294,15 +295,34 @@ int launch_surfel_fwd(const FusedScene &sc, const float *alphas, float *us, floa
                       float *recs, cudaStream_t st);
 int launch_surfel_bwd(const FusedScene &sc, const float *rows, float *g_pws, float *g_shs, float *g_alphas,
                       float *g_scales, float *g_rots, float *g_us, cudaStream_t st);
+// The 2DGS geometry planes (DESIGN 3.16) of one frame, on the NDC-mapped hit depth
+// m(z) = mscale (1 - near / max(z, near)), mscale = far / (far - near):
+// distortion[H,W] = sum_{j<i} w_i w_j (m_i - m_j)^2, moments[2,H,W] = (sum w m, sum w m^2),
+// median_depth[H,W] = z of the last contributing record whose incoming tau > 0.5 (0: none) and
+// median_contrib[H,W] = its patch index in the tile + 1 (0: none).
+struct GeoPlanes {
+  float *distortion, *moments, *median_depth;
+  int32_t *median_contrib;
+  float near, mscale;
+};
+// Their backward: the upstream dL/d(distortion), dL/d(median_depth) (NULL reads as zero) and the
+// forward's alpha plane (the final sum w), moments and median_contrib.
+struct GeoGrads {
+  const float *distortion, *median, *alpha, *moments;
+  const int32_t *median_contrib;
+  float near, mscale;
+};
 // work: launch_tile_list's work area; recs == nullptr: no patches (zeros only).  The normal plane
-// [3,H,W] is written like the image planes.
+// [3,H,W] is written like the image planes.  geo: also the geometry planes (k_draw_2dgs), or NULL
+// (k_draw_surfel).
 int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid, float *image,
                        int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, float *normal_image,
-                       int *work, cudaStream_t st);
-// the upstream planes dl_*: NULL reads as zero (all NULL: the rows stay 0)
+                       const GeoPlanes *geo, int *work, cudaStream_t st);
+// the upstream planes dl_*: NULL reads as zero (all NULL: the rows stay 0).  geo with an upstream
+// geometry plane: k_draw_2dgs_bwd adds the geometry terms; otherwise k_draw_surfel_bwd runs.
 int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, const float *recs, const int32_t *gsid,
                                 const int32_t *contrib, const float *final_tau, const float *dl_image,
-                                const float *dl_depth, const float *dl_alpha, const float *dl_normal, float *rows,
-                                int *work, cudaStream_t st);
+                                const float *dl_depth, const float *dl_alpha, const float *dl_normal,
+                                const GeoGrads *geo, float *rows, int *work, cudaStream_t st);
 
 }  // namespace gsb

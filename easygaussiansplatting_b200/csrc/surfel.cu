@@ -10,6 +10,10 @@
 //  k_draw_surfel_bwd   back to front from final_tau and contrib, the recurrence of k_draw_bwd over
 //                      3 + 1 + 1 + 3 channels; each (record, 8x8 block) is reduced in the warp and added
 //                      to the surfel's gradient row [dM (9), dalpha, dcolour (3), dn (3), ddelta (2)]
+//  k_draw_2dgs         k_draw_surfel's walk (draw_walk<true>) that also composites the 2DGS geometry
+//                      planes (DESIGN 3.16): depth distortion, its moments and the median depth
+//  k_draw_2dgs_bwd     k_draw_surfel_bwd's walk (draw_bwd_walk<true>) with the geometry terms added to
+//                      the alpha' recurrence and to the hit-depth gradient; the rows are the same
 //  k_surfel_bwd<K3>    the rows -> dL/dpws, dL/dshs, dL/dalphas, dL/dscales, dL/drots, dL/dus (= ddelta)
 #include "common.cuh"
 #include "kernels.h"
@@ -24,6 +28,9 @@ namespace gsb {
 #endif
 #ifndef DRAW_SURFEL_BWD_MINBLOCKS
 #define DRAW_SURFEL_BWD_MINBLOCKS 4
+#endif
+#ifndef DRAW_2DGS_BWD_MINBLOCKS
+#define DRAW_2DGS_BWD_MINBLOCKS 4
 #endif
 
 constexpr int SREC_BYTES = sf::kRecFloats * 4;  // 80
@@ -191,11 +198,23 @@ __device__ __forceinline__ bool block_pix(int W, int H, int gx, int tile, int bl
   return true;
 }
 
-__global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
-    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
-    const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
-    float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
-    float *__restrict__ normal_image, int *__restrict__ work) {
+// the NDC-mapped hit depth of the geometry planes and its derivative (0 at and below near)
+__device__ __forceinline__ float geo_m(float z, float near, float mscale) {
+  return mscale * (1.0f - near / fmaxf(z, near));
+}
+__device__ __forceinline__ float geo_dm(float z, float near, float mscale) {
+  return z > near ? mscale * near / (z * z) : 0.f;
+}
+
+// The forward walk of k_draw_surfel and (GEO) k_draw_2dgs: GEO also accumulates the moments
+// D = sum w m, D2 = sum w m^2, the distortion sum_{j<i} w_i w_j (m_i - m_j)^2 and the median
+template <bool GEO>
+__device__ __forceinline__ void draw_walk(int W, int H, int gx, const int2 *__restrict__ ranges,
+                                          const float4 *__restrict__ recs, const int32_t *__restrict__ gsid,
+                                          float *__restrict__ image, int32_t *__restrict__ contrib,
+                                          float *__restrict__ final_tau, float *__restrict__ depth_image,
+                                          float *__restrict__ alpha_image, float *__restrict__ normal_image,
+                                          const GeoPlanes &geo, int *__restrict__ work) {
   __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<SREC_BYTES>];
   __shared__ __align__(16) uint2 s_list[4][32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -223,6 +242,8 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
       for (int p = 0; p < 2; p++)
 #pragma unroll
         for (int k = 0; k < 8; k++) acc[p][k] = 0.f;
+      float mD[2] = {0.f, 0.f}, mD2[2] = {0.f, 0.f}, dist[2] = {0.f, 0.f}, medz[2] = {0.f, 0.f};
+      int medc[2] = {0, 0};
       if (len > 0) {
         const int nch = (len + 31) >> 5;
         auto issue = [&](int c) {
@@ -250,6 +271,17 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
               const float ap = surfel_alpha(r, xs[p], y, pe, g, clamped);
               if (tau[p] >= TAU_STOP && ap >= ALPHA_SKIP) {
                 const float w = tau[p] * ap;
+                if constexpr (GEO) {
+                  // before this record joins the totals: w (m^2 A + D2 - 2 m D), A = acc[p][4]
+                  const float m = geo_m(pe.z, geo.near, geo.mscale);
+                  dist[p] = fmaf(w, fmaf(m, fmaf(m, acc[p][4], -2.0f * mD[p]), mD2[p]), dist[p]);
+                  mD[p] = fmaf(w, m, mD[p]);
+                  mD2[p] = fmaf(w * m, m, mD2[p]);
+                  if (tau[p] > 0.5f) {
+                    medz[p] = pe.z;
+                    medc[p] = (int)e.y + 1;
+                  }
+                }
                 acc[p][0] = fmaf(w, r.col[0], acc[p][0]);
                 acc[p][1] = fmaf(w, r.col[1], acc[p][1]);
                 acc[p][2] = fmaf(w, r.col[2], acc[p][2]);
@@ -278,9 +310,33 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
         contrib[q] = cont[p]; final_tau[q] = tau[p];
         depth_image[q] = acc[p][3]; alpha_image[q] = acc[p][4];
         normal_image[q] = acc[p][5]; normal_image[HW + q] = acc[p][6]; normal_image[2 * HW + q] = acc[p][7];
+        if constexpr (GEO) {
+          geo.distortion[q] = dist[p];
+          geo.moments[q] = mD[p]; geo.moments[HW + q] = mD2[p];
+          geo.median_depth[q] = medz[p]; geo.median_contrib[q] = medc[p];
+        }
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
+    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
+    float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
+    float *__restrict__ normal_image, int *__restrict__ work) {
+  draw_walk<false>(W, H, gx, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image, normal_image,
+                   GeoPlanes{}, work);
+}
+
+// 2DGS (DESIGN 3.16): k_draw_surfel's planes, bit for bit, and the geometry planes
+__global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_2dgs(
+    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
+    float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
+    float *__restrict__ normal_image, GeoPlanes geo, int *__restrict__ work) {
+  draw_walk<true>(W, H, gx, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image, normal_image, geo,
+                  work);
 }
 
 // the upstream gradient planes of the backward; NULL reads as zero
@@ -290,10 +346,15 @@ struct SurfelGrads {
 
 __device__ __forceinline__ float ld_plane(const float *__restrict__ p, size_t q) { return p ? __ldg(p + q) : 0.f; }
 
-__global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_bwd(
-    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
-    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
-    SurfelGrads dl, float *__restrict__ rows, int *__restrict__ work) {
+// The backward walk of k_draw_surfel_bwd and (GEO) k_draw_2dgs_bwd: GEO adds dL/ddistortion's
+// dDelta/dw_i to the per-record value of the alpha' recurrence and its dDelta/dz_i, with dL/dmedian
+// at the median record, to the hit-depth coefficient
+template <bool GEO>
+__device__ __forceinline__ void draw_bwd_walk(int W, int H, int gx, const int2 *__restrict__ ranges,
+                                              const float4 *__restrict__ recs, const int32_t *__restrict__ gsid,
+                                              const int32_t *__restrict__ contrib,
+                                              const float *__restrict__ final_tau, const SurfelGrads &dl,
+                                              const GeoGrads &geo, float *__restrict__ rows, int *__restrict__ work) {
   __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<SREC_BYTES>];
   __shared__ __align__(16) uint2 s_list[4][32];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -331,6 +392,23 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
         d[p][5] = in ? ld_plane(dl.normal, q) : 0.f;
         d[p][6] = in ? ld_plane(dl.normal ? dl.normal + HW : nullptr, q) : 0.f;
         d[p][7] = in ? ld_plane(dl.normal ? dl.normal + 2 * HW : nullptr, q) : 0.f;
+      }
+      // GEO: dL/ddistortion, dL/dmedian, the final A, D, D2 and the median record of each pixel
+      float gdist[2] = {0.f, 0.f}, gmed[2] = {0.f, 0.f}, fA[2] = {0.f, 0.f}, fD[2] = {0.f, 0.f},
+            fD2[2] = {0.f, 0.f};
+      int medc[2] = {0, 0};
+      if constexpr (GEO) {
+#pragma unroll
+        for (int p = 0; p < 2; p++) {
+          if (!(p ? bp.in1 : bp.in0)) continue;
+          const size_t q = bp.pix + p;
+          gdist[p] = ld_plane(geo.distortion, q);
+          gmed[p] = ld_plane(geo.median, q);
+          fA[p] = __ldg(geo.alpha + q);
+          fD[p] = __ldg(geo.moments + q);
+          fD2[p] = __ldg(geo.moments + HW + q);
+          medc[p] = __ldg(geo.median_contrib + q);
+        }
       }
       int wmax = max(cont[0], cont[1]);
 #pragma unroll
@@ -370,8 +448,13 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
               any = true;
               tau[p] = tau[p] / (1.0f - ap);
               const float *dp = d[p];
-              const float v = fmaf(dp[0], r.col[0], fmaf(dp[1], r.col[1], fmaf(dp[2], r.col[2],
-                              fmaf(dp[3], pe.z, fmaf(dp[5], r.n[0], fmaf(dp[6], r.n[1], fmaf(dp[7], r.n[2], dp[4])))))));
+              float v = fmaf(dp[0], r.col[0], fmaf(dp[1], r.col[1], fmaf(dp[2], r.col[2],
+                        fmaf(dp[3], pe.z, fmaf(dp[5], r.n[0], fmaf(dp[6], r.n[1], fmaf(dp[7], r.n[2], dp[4])))))));
+              float m = 0.f;
+              if constexpr (GEO) {
+                m = geo_m(pe.z, geo.near, geo.mscale);
+                v = fmaf(gdist[p], fmaf(m, fmaf(m, fA[p], -2.0f * fD[p]), fD2[p]), v);
+              }
               const float diff = v - sdot[p];
               sdot[p] = fmaf(ap, diff, sdot[p]);
               const float dap = tau[p] * diff;  // dL/dalpha'
@@ -386,7 +469,12 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
                 gal = fmaf(dap, g, gal);
                 dG = -0.5f * dap * ap;
               }
-              sf::pixel_grad(r.M, xs[p], y, pe, dG, w * dp[3], gM, gd, gu);
+              float dz = w * dp[3];
+              if constexpr (GEO) {
+                dz = fmaf(2.0f * gdist[p] * w * fmaf(m, fA[p], -fD[p]), geo_dm(pe.z, geo.near, geo.mscale), dz);
+                if (idx == medc[p] - 1) dz += gmed[p];
+              }
+              sf::pixel_grad(r.M, xs[p], y, pe, dG, dz, gM, gd, gu);
             }
           }
           if (!__any_sync(0xffffffffu, any)) continue;
@@ -416,6 +504,27 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
       walk_drain();
     }
   }
+}
+
+__global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_bwd(
+    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    SurfelGrads dl, float *__restrict__ rows, int *__restrict__ work) {
+  draw_bwd_walk<false>(W, H, gx, ranges, recs, gsid, contrib, final_tau, dl, GeoGrads{}, rows, work);
+}
+
+// the upstream planes of k_draw_2dgs_bwd: k_draw_surfel_bwd's and the geometry terms' (one struct,
+// so the kernel's name stays its own)
+struct GeoBwdArgs {
+  SurfelGrads dl;
+  GeoGrads geo;
+};
+
+__global__ void __launch_bounds__(128, DRAW_2DGS_BWD_MINBLOCKS) k_draw_2dgs_bwd(
+    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    GeoBwdArgs a, float *__restrict__ rows, int *__restrict__ work) {
+  draw_bwd_walk<true>(W, H, gx, ranges, recs, gsid, contrib, final_tau, a.dl, a.geo, rows, work);
 }
 
 // ---- launchers
@@ -457,44 +566,66 @@ int launch_surfel_bwd(const FusedScene &sc, const float *rows, float *g_pws, flo
 
 int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid, float *image,
                        int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, float *normal_image,
-                       int *work, cudaStream_t st) {
+                       const GeoPlanes *geo, int *work, cudaStream_t st) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0) return 0;
   if (work == nullptr) return set_arg_error("draw_surfel: work area missing");
-  // the normal planes of empty tiles: k_tile_list zeroes the other five planes
-  GSB_CUDA_TRY(cudaMemsetAsync(normal_image, 0, sizeof(float) * 3 * (size_t)H * W, st));
+  // the normal (and geometry) planes of empty tiles: k_tile_list zeroes the other five planes
+  const size_t HW = (size_t)H * W;
+  GSB_CUDA_TRY(cudaMemsetAsync(normal_image, 0, sizeof(float) * 3 * HW, st));
+  if (geo) {
+    GSB_CUDA_TRY(cudaMemsetAsync(geo->distortion, 0, sizeof(float) * HW, st));
+    GSB_CUDA_TRY(cudaMemsetAsync(geo->moments, 0, sizeof(float) * 2 * HW, st));
+    GSB_CUDA_TRY(cudaMemsetAsync(geo->median_depth, 0, sizeof(float) * HW, st));
+    GSB_CUDA_TRY(cudaMemsetAsync(geo->median_contrib, 0, sizeof(int32_t) * HW, st));
+  }
   int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st);
   if (rc || recs == nullptr) return rc;
   int grid = 0;
   rc = persistent_grid(gx * gy, DRAW_SURFEL_MINBLOCKS, grid);
   if (rc) return rc;
-  ProfScope ps(K_DRAW_SURFEL, st);
-  k_draw_surfel<<<grid, 128, 0, st>>>(W, H, gx, reinterpret_cast<const int2 *>(ranges),
-                                      reinterpret_cast<const float4 *>(recs), gsid, image, contrib, final_tau,
-                                      depth_image, alpha_image, normal_image, work);
+  const int2 *r2 = reinterpret_cast<const int2 *>(ranges);
+  const float4 *r4 = reinterpret_cast<const float4 *>(recs);
+  if (geo) {
+    ProfScope ps(K_DRAW_2DGS, st);
+    k_draw_2dgs<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                                      normal_image, *geo, work);
+  } else {
+    ProfScope ps(K_DRAW_SURFEL, st);
+    k_draw_surfel<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                                        normal_image, work);
+  }
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
 int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, const float *recs, const int32_t *gsid,
                                 const int32_t *contrib, const float *final_tau, const float *dl_image,
-                                const float *dl_depth, const float *dl_alpha, const float *dl_normal, float *rows,
-                                int *work, cudaStream_t st) {
+                                const float *dl_depth, const float *dl_alpha, const float *dl_normal,
+                                const GeoGrads *geo, float *rows, int *work, cudaStream_t st) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0 || N <= 0) return 0;
   GSB_CUDA_TRY(cudaMemsetAsync(rows, 0, sizeof(float) * sf::kRowFloats * (size_t)N, st));
   if (recs == nullptr) return 0;
-  if (dl_image == nullptr && dl_depth == nullptr && dl_alpha == nullptr && dl_normal == nullptr) return 0;
+  const bool with_geo = geo != nullptr && (geo->distortion != nullptr || geo->median != nullptr);
+  if (dl_image == nullptr && dl_depth == nullptr && dl_alpha == nullptr && dl_normal == nullptr && !with_geo) return 0;
   if (work == nullptr) return set_arg_error("draw_surfel_backward: work area missing");
   int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);
   if (rc) return rc;
   int grid = 0;
-  rc = persistent_grid(gx * gy, DRAW_SURFEL_BWD_MINBLOCKS, grid);
+  rc = persistent_grid(gx * gy, with_geo ? DRAW_2DGS_BWD_MINBLOCKS : DRAW_SURFEL_BWD_MINBLOCKS, grid);
   if (rc) return rc;
-  ProfScope ps(K_DRAW_SURFEL_BWD, st);
-  k_draw_surfel_bwd<<<grid, 128, 0, st>>>(W, H, gx, reinterpret_cast<const int2 *>(ranges),
-                                          reinterpret_cast<const float4 *>(recs), gsid, contrib, final_tau,
-                                          SurfelGrads{dl_image, dl_depth, dl_alpha, dl_normal}, rows, work);
+  const int2 *r2 = reinterpret_cast<const int2 *>(ranges);
+  const float4 *r4 = reinterpret_cast<const float4 *>(recs);
+  const SurfelGrads dl{dl_image, dl_depth, dl_alpha, dl_normal};
+  if (with_geo) {
+    ProfScope ps(K_DRAW_2DGS_BWD, st);
+    k_draw_2dgs_bwd<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, contrib, final_tau, GeoBwdArgs{dl, *geo}, rows,
+                                          work);
+  } else {
+    ProfScope ps(K_DRAW_SURFEL_BWD, st);
+    k_draw_surfel_bwd<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, contrib, final_tau, dl, rows, work);
+  }
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

@@ -436,3 +436,59 @@ class GSFunctionSurfel(torch.autograd.Function):
             rows)
         grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
         return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
+
+
+class GSFunctionSurfelGeometry(torch.autograd.Function):
+    """GSFunctionSurfel with 2D Gaussian Splatting's geometry terms (DESIGN 3.16).
+    `apply(pws, shs, alphas, scales, rots, us, cam, near=0.2, far=100.0)` -> (image, depth, alpha,
+    normal, distortion[H,W], median_depth[H,W], depths > 0.2): the first four planes are
+    GSFunctionSurfel's (bit for bit), and per pixel, over the surfels in compositing order
+    (w = tau alpha', z_i the hit depth, m(z) = far / (far - near) (1 - near / max(z, near))),
+        distortion = sum_{j<i} w_i w_j (m_i - m_j)^2      (2DGS's depth-distortion loss, per pixel)
+        median_depth = z of the last surfel whose incoming tau > 0.5 (0 where none contributes).
+    Unlike 2DGS, m clamps z at near (a hit at or behind the camera would give inf / NaN); below near
+    m and its gradient are 0.  All six float planes are differentiable; a plane the loss does not
+    use is not read in the backward, and with none used the backward rasterizer is skipped.  With
+    no gradient on distortion and median_depth the backward is GSFunctionSurfel's.
+    Training loss of 2DGS: L_rgb + lambda_d distortion.mean() + lambda_n L_normal with
+    L_normal = (1 - (normal * loss.depth_to_normal(median_depth, cam) * alpha.detach()).sum(0)).mean()
+    (2DGS's form, alpha detached; see loss.depth_to_normal).  Refuses cam.antialiased, other camera
+    models and cam.grad_exchange, as GSFunctionSurfel does; it takes no filter3d or us_abs, and near /
+    far must be numbers with 0 < near < far."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cam, near=0.2, far=100.0):
+        from . import ops
+        who = "GSFunctionSurfelGeometry"
+        if getattr(cam, "antialiased", False):
+            raise ValueError("%s has no antialiased mode: cam.antialiased must be False" % who)
+        _pinhole_only(cam, who)
+        if getattr(cam, "grad_exchange", None) is not None:
+            raise ValueError("%s is single-view: cam.grad_exchange must not be set" % who)
+        ctx.set_materialize_grads(False)
+        us_, depths, areas, colors, records = ops.surfel_preprocess(
+            pws, rots, scales, shs, alphas.reshape(-1), cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+            cam.width, cam.height)
+        (image, contrib, final_tau, ranges, gsid, depth, alpha, normal, distortion, median_depth, moments,
+         median_contrib) = ops.splat_surfel_geometry(cam.height, cam.width, us_, depths, areas, records, near, far,
+                                                     capacity=True)
+        ctx.cam, ctx.near, ctx.far = cam, near, far
+        ctx.alpha_shape = alphas.shape
+        ctx.save_for_backward(pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid, alpha, moments,
+                              median_contrib)
+        return image, depth, alpha, normal, distortion, median_depth, depths > 0.2
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, dloss_ddistortion, dloss_dmedian, _):
+        from . import ops
+        cam = ctx.cam
+        pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid, alpha, moments, median_contrib = \
+            ctx.saved_tensors
+        rows = ops.splatB_surfel_geometry(cam.height, cam.width, records, contrib, final_tau, ranges, gsid, alpha,
+                                          moments, median_contrib, dloss_dimage, dloss_ddepth, dloss_dalpha,
+                                          dloss_dnormal, dloss_ddistortion, dloss_dmedian, ctx.near, ctx.far)
+        dpws, dshs, dalphas, dscales, drots, dus = ops.surfel_preprocessB(
+            pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width, cam.height,
+            rows)
+        grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
+        return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))

@@ -45,3 +45,35 @@ class _GauLoss(torch.autograd.Function):
 def gau_loss(image, gt_image, loss_lambda=0.2):
     """Same signature and value as the reference's gau_loss; differentiable w.r.t. `image`."""
     return _GauLoss.apply(image, gt_image, loss_lambda)
+
+
+def depth_to_normal(depth, cam):
+    """The camera-frame normal of a depth map, for 2D Gaussian Splatting's depth-normal consistency
+    term (DESIGN 3.16).  Pure torch, differentiable by autograd; no kernel.
+    depth[H,W] (or [1,H,W]): camera-frame z per pixel, e.g. GSFunctionSurfelGeometry's median_depth
+    or depth / alpha.  Each pixel is unprojected through the pinhole K of `cam` (fx, fy, cx, cy) to
+    X(u, v) = depth (u - cx) / fx, depth (v - cy) / fy, depth); the normal is the unit cross product of
+    the central differences X(u+1, v) - X(u-1, v) and X(u, v+1) - X(u, v-1), oriented to face the
+    camera (n . X <= 0), which is the surfel normal plane's convention: -z for a fronto-parallel
+    plane.  -> [3,H,W]; the one-pixel border is 0.
+    A pixel without a surface to differentiate gets a zero normal with a zero gradient: one whose own
+    depth or a neighbour's is <= 0 (median_depth is 0 where nothing contributes: a thin covered strip
+    against an empty background has no vertical difference), or whose cross product is exactly 0.
+    2DGS's normal term (alpha detached, as there) is then
+        L_n = (1 - (normal * depth_to_normal(median_depth, cam) * alpha.detach()).sum(0)).mean()
+    with normal and alpha GSFunctionSurfelGeometry's planes (its normal plane is sum w n)."""
+    d = depth.reshape(depth.shape[-2], depth.shape[-1])
+    H, W = d.shape
+    v, u = torch.meshgrid(torch.arange(H, dtype=d.dtype, device=d.device),
+                          torch.arange(W, dtype=d.dtype, device=d.device), indexing="ij")
+    X = torch.stack([d * (u - float(cam.cx)) / float(cam.fx), d * (v - float(cam.cy)) / float(cam.fy), d])
+    dx = X[:, 1:-1, 2:] - X[:, 1:-1, :-2]
+    dy = X[:, 2:, 1:-1] - X[:, :-2, 1:-1]
+    n = torch.linalg.cross(dx, dy, dim=0)
+    sq = (n * n).sum(0, keepdim=True)
+    valid = ((d[1:-1, 1:-1] > 0) & (d[1:-1, 2:] > 0) & (d[1:-1, :-2] > 0) & (d[2:, 1:-1] > 0) &
+             (d[:-2, 1:-1] > 0))[None] & (sq > 0)
+    # both branches finite, and the invalid one constant: no gradient reaches a degenerate pixel
+    n = torch.where(valid, n * torch.rsqrt(torch.where(valid, sq, torch.ones_like(sq))), torch.zeros_like(n))
+    n = torch.where((n * X[:, 1:-1, 1:-1]).sum(0, keepdim=True) > 0, -n, n)
+    return torch.nn.functional.pad(n, (1, 1, 1, 1))

@@ -13,6 +13,7 @@ libgsplat_b200.so.  Differences from the reference, all deliberate:
 """
 import ctypes as C
 import math
+import numbers
 
 import torch
 
@@ -259,14 +260,15 @@ def _check_drawn(H, W, ranges, planes, text):
 
 def _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes):
     """the sort workspace for P patch slots (ws_bytes: the family's workspace query) and splat's
-    five outputs, + one float32 plane of each shape in `planes`"""
+    five outputs, + one plane of each shape in `planes`: float32, or (shape, dtype)"""
     ws = _bytes(ws_bytes(N, H, W, P), dev)
+    typed = [pl if isinstance(pl[-1], torch.dtype) else (pl, torch.float32) for pl in planes]
     return ws, [torch.empty((3, H, W), dtype=torch.float32, device=dev),
                 torch.empty((H, W), dtype=torch.int32, device=dev),
                 torch.empty((H, W), dtype=torch.float32, device=dev),
                 torch.empty((_tiles(H, W), 2), dtype=torch.int32, device=dev),
                 torch.empty((P,), dtype=torch.int32, device=dev)] + \
-        [torch.empty(shape, dtype=torch.float32, device=dev) for shape in planes]
+        [torch.empty(shape, dtype=dtype, device=dev) for shape, dtype in typed]
 
 
 def _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status):
@@ -1046,4 +1048,89 @@ def splatB_surfel(height, width, records, contrib, final_tau, patch_range_per_ti
         _lib.check(lib.gsb_splat_surfel_backward(H, W, N, P, _ptr(records), _ptr(contrib), _ptr(final_tau),
                                                  _ptr(ranges), _ptr(gsid), *[_ptr(t) for t in planes], _ptr(ws),
                                                  ws.numel(), _ptr(rows), _stream()), lib)
+    return rows
+
+
+# 2DGS geometry terms (extension; DESIGN 3.16): depth distortion and median depth of the surfel frame.
+def _near_far(near, far):
+    """near / far of the geometry planes: plain numbers (not tensors), finite, 0 < near < far"""
+    if not all(isinstance(x, numbers.Real) and not isinstance(x, bool) for x in (near, far)):
+        raise ValueError("near and far must be numbers (there is no filter3d or us_abs argument)")
+    near, far = float(near), float(far)
+    if not (math.isfinite(near) and math.isfinite(far) and 0.0 < near < far):
+        raise ValueError("near and far must be finite with 0 < near < far")
+    return near, far
+
+
+def splat_surfel_geometry(height, width, us, depths, areas, records, near=0.2, far=100.0, capacity=False):
+    """`splat_surfel` (the same binning, the same eight outputs bit for bit) with 2DGS's geometry
+    planes.  -> splat_surfel's eight outputs + [distortion[H,W], median_depth[H,W], moments[2,H,W],
+    median_contrib[H,W] i32], per pixel over the contributing surfels in compositing order
+    (w = tau alpha', z the hit depth, m(z) = far / (far - near) (1 - near / max(z, near))):
+        distortion = sum_{j<i} w_i w_j (m_i - m_j)^2,   moments = (sum w m, sum w m^2),
+        median_depth = z of the last surfel whose incoming tau > 0.5 (0 where none contributes),
+    median_contrib its patch index in the tile + 1 (as contrib).  moments and median_contrib are
+    what `splatB_surfel_geometry` reads back."""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    near, far = _near_far(near, far)
+    us = _chk(us, "us", last=2, ndim=2); depths = _chk(depths, "depths")
+    areas = _chk(areas, "areas", dtype=torch.int32, last=2, ndim=2)
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    _same_device(us, depths, areas, records)
+    N = us.shape[0]
+    if not (depths.numel() == N and areas.shape[0] == N and records.shape[0] == N):
+        raise ValueError("splat_surfel_geometry inputs disagree on N")
+    dev, lib = us.device, _L()
+    planes = [(H, W), (H, W), (3, H, W), (H, W), (2, H, W), (H, W), ((H, W), torch.int32)]
+    nf = [C.c_float(near), C.c_float(far)]
+    with torch.cuda.device(dev):
+        _, _, out = _frame(H, W, us, depths, areas, planes, lib.gsb_splat_surfel_workspace_bytes,
+                           (lib.gsb_splat_2dgs_forward, [_ptr(us), _ptr(depths), _ptr(areas), _ptr(records)] + nf),
+                           (lib.gsb_splat_2dgs_render, [_ptr(us), _ptr(depths), _ptr(records)] + nf), capacity,
+                           ("surfel", dev.index, H, W, N))
+    distortion, moments, median_depth, median_contrib = out[8:]
+    return out[:8] + [distortion, median_depth, moments, median_contrib]
+
+
+def splatB_surfel_geometry(height, width, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                           alpha, moments, median_contrib, dloss_dimage=None, dloss_ddepth=None, dloss_dalpha=None,
+                           dloss_dnormal=None, dloss_ddistortion=None, dloss_dmedian=None, near=0.2, far=100.0):
+    """Backward of `splat_surfel_geometry`: `splatB_surfel`'s upstream planes plus
+    dloss_ddistortion[H,W] and dloss_dmedian[H,W] (None = zero and not read); alpha, moments and
+    median_contrib are the forward's planes.  -> rows[N,18] as `splatB_surfel`.  With both geometry
+    gradients None this is `splatB_surfel` (same kernel, same rows)."""
+    if dloss_ddistortion is None and dloss_dmedian is None:
+        return splatB_surfel(height, width, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                             dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal)
+    H, W = int(height), int(width)
+    near, far = _near_far(near, far)
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    contrib = _chk(contrib, "contrib", dtype=torch.int32); final_tau = _chk(final_tau, "final_tau")
+    ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
+    gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
+    alpha = _chk(alpha, "alpha"); moments = _chk(moments, "moments")
+    median_contrib = _chk(median_contrib, "median_contrib", dtype=torch.int32)
+    _same_device(records, contrib, final_tau, ranges, gsid, alpha, moments, median_contrib)
+    _check_drawn(H, W, ranges, ((contrib, 1), (final_tau, 1), (alpha, 1), (moments, 2), (median_contrib, 1)),
+                 "contrib / final_tau / alpha / moments / median_contrib do not match height x width")
+    planes = []
+    for name, t, n in (("dloss_dimage", dloss_dimage, 3), ("dloss_ddepth", dloss_ddepth, 1),
+                       ("dloss_dalpha", dloss_dalpha, 1), ("dloss_dnormal", dloss_dnormal, 3),
+                       ("dloss_ddistortion", dloss_ddistortion, 1), ("dloss_dmedian", dloss_dmedian, 1)):
+        if t is not None:
+            t = _chk(t, name)
+            _same_device(records, t)
+            if t.numel() != n * H * W:
+                raise ValueError("%s does not match height x width" % name)
+        planes.append(t)
+    N, P, dev, lib = records.shape[0], gsid.numel(), records.device, _L()
+    rows = torch.empty((N, SURFEL_ROW), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_splat_surfel_workspace_bytes(N, H, W, 0), dev)
+        _lib.check(lib.gsb_splat_2dgs_backward(H, W, N, P, _ptr(records), _ptr(contrib), _ptr(final_tau),
+                                               _ptr(ranges), _ptr(gsid), *[_ptr(t) for t in planes[:4]], _ptr(ws),
+                                               ws.numel(), _ptr(rows), near, far, _ptr(alpha), _ptr(moments),
+                                               _ptr(median_contrib), *[_ptr(t) for t in planes[4:]], _stream()), lib)
     return rows

@@ -705,6 +705,40 @@ int gsb_splat_surfel_backward(int H, int W, int N, int64_t P, const float *recor
                               const float *dloss_dalpha, const float *dloss_dnormal, void *ws, size_t ws_bytes,
                               float *rows, gsb_stream_t stream);
 
+/* ---- 2D Gaussian Splatting geometry terms (extension; DESIGN 3.16): the surfel frame of
+ * gsb_splat_surfel_render / _forward / _backward (same arguments, same workspace:
+ * gsb_splat_surfel_workspace_bytes, same planes bit for bit) with 2DGS's depth-distortion and
+ * median-depth planes.  Per pixel, over the contributing records in compositing order (w = tau alpha'):
+ *   m(z) = far / (far - near) (1 - near / max(z, near))   (z: the record's hit depth; 0 < near < far)
+ *   distortion[H,W] = sum_{j<i} w_i w_j (m_i - m_j)^2,  moments[2,H,W] = (sum w m, sum w m^2),
+ *   median_depth[H,W] = z of the last record whose incoming tau > 0.5 (0 where none contributes),
+ *   median_contrib[H,W] (int32) = that record's patch index in its tile + 1 (0: none), as contrib.
+ * Every geometry plane is 16-byte aligned; all are written in full. */
+int gsb_splat_2dgs_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us, const float *depths,
+                          const float *records, float near, float far, const void *bin_ws, void *ws, size_t ws_bytes,
+                          float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                          int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
+                          float *distortion, float *moments, float *median_depth, int32_t *median_contrib,
+                          gsb_stream_t stream);
+/* The capacity form (as gsb_splat_surfel_forward). */
+int gsb_splat_2dgs_forward(int H, int W, int N, const float *us, float *depths, int32_t *areas, const float *records,
+                           float near, float far, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                           size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                           float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                           uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                           float *distortion, float *moments, float *median_depth, int32_t *median_contrib,
+                           gsb_stream_t stream);
+/* Backward of the geometry frame: gsb_splat_surfel_backward's arguments, plus the forward's
+ * alpha_image, moments and median_contrib and the upstream dloss_ddistortion[H,W] and
+ * dloss_dmedian[H,W] (each nullable; with both NULL this is gsb_splat_surfel_backward and the three
+ * forward planes are not read).  Those five planes are 4-byte aligned.  rows[N,18] as there. */
+int gsb_splat_2dgs_backward(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                            const float *final_tau, const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                            const float *dloss_dimage, const float *dloss_ddepth, const float *dloss_dalpha,
+                            const float *dloss_dnormal, void *ws, size_t ws_bytes, float *rows, float near, float far,
+                            const float *alpha_image, const float *moments, const int32_t *median_contrib,
+                            const float *dloss_ddistortion, const float *dloss_dmedian, gsb_stream_t stream);
+
 /* ---- launch accounting and optional per-kernel timing (no reference counterpart; used by
  * bench.py for `gpu_launches` and the roofline's live CUDA-event kernel durations).
  * Kernel ids 0..gsb_profile_kernels()-1, names from gsb_profile_kernel_name().
