@@ -113,6 +113,10 @@ SIGNATURES = {
     "gsb_splat_2dgs_forward": (_i, [_i, _i, _i] + [_vp] * 4 + [_f, _f, _i64, C.c_uint32, _vp, _sz, _vp, _sz]
                                + [_vp] * 14),
     "gsb_splat_2dgs_backward": (_i, [_i, _i, _i, _i64] + [_vp] * 10 + [_sz, _vp, _f, _f] + [_vp] * 6),
+    "gsb_tsdf_integrate": (_i, [_i, _i, _i] + [_f] * 6 + [_i, _i, _i] + [_vp] * 7),
+    "gsb_tsdf_extract_workspace_bytes": (_sz, [_i, _i, _i]),
+    "gsb_tsdf_extract_plan": (_i, [_i, _i, _i, _vp, _vp, _vp, _sz, C.POINTER(_i64), _vp]),
+    "gsb_tsdf_extract_emit": (_i, [_i, _i, _i] + [_f] * 4 + [_vp] * 4 + [_sz, _i64, _i64] + [_vp] * 4),
     "gsb_profile_enable": (None, [_i]),
     "gsb_profile_kernels": (_i, []),
     "gsb_profile_kernel_name": (C.c_char_p, [_i]),

@@ -44,7 +44,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
                                              "draw_features", "draw_backward_features", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
-                                             "mcmc_noise", "surfel_forward", "draw_surfel",
+                                             "mcmc_noise", "tsdf_integrate", "tsdf_plan", "tsdf_emit",
+                                             "surfel_forward", "draw_surfel",
                                              "draw_surfel_backward", "surfel_backward", "draw_2dgs",
                                              "draw_2dgs_backward", "draw_backward_abs",
                                              "draw_backward_rgbd_abs",
@@ -1378,6 +1379,78 @@ int gsb_grad_reduce_broadcast(int N, int sh_dim3, int world, int rank, void *con
   for (int p = 0; p < world; p++) GSB_REQUIRE(regions_host[p] != nullptr, "grad_reduce_broadcast: null region");
   const ExchangeGeom G = exchange_geom(N, sh_dim3, world);
   return launch_grad_reduce_bcast(G, rank, regions_host, epoch, (cudaStream_t)stream);
+}
+
+// ---- mesh extraction (tsdf.cu, DESIGN 3.17)
+// the grid checks every TSDF entry point makes; 0 or the argument error "<who>: <reason>"
+static int tsdf_grid_check(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const char *who) {
+  if (nx < 1 || ny < 1 || nz < 1) return arg_error(who, "bad grid dimension");
+  if ((int64_t)nx * ny * nz >= ((int64_t)1 << 31)) return arg_error(who, "2^31 or more voxels");
+  if (!(std::isfinite(voxel) && voxel > 0.f)) return arg_error(who, "voxel must be finite and > 0");
+  if (!(std::isfinite(ox) && std::isfinite(oy) && std::isfinite(oz))) return arg_error(who, "origin not finite");
+  return 0;
+}
+
+int gsb_tsdf_integrate(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc,
+                       float depth_trunc, int V, int H, int W, const float *cams, const float *depth,
+                       const float *color, float *tsdf, float *weight, float *color_grid, gsb_stream_t stream) {
+  if (int rc = tsdf_grid_check(nx, ny, nz, ox, oy, oz, voxel, "tsdf_integrate")) return rc;
+  GSB_REQUIRE(std::isfinite(trunc) && trunc > 0.f, "tsdf_integrate: trunc must be finite and > 0");
+  GSB_REQUIRE(depth_trunc > 0.f, "tsdf_integrate: depth_trunc must be > 0");
+  GSB_REQUIRE(V >= 1 && H >= 1 && W >= 1, "tsdf_integrate: V, H and W must be >= 1");
+  GSB_REQUIRE((color == nullptr) == (color_grid == nullptr), "tsdf_integrate: colour given to one side only");
+  GSB_REQUIRE(cams && depth && tsdf && weight, "tsdf_integrate: null pointer");
+  for (const void *p : {(const void *)cams, (const void *)depth, (const void *)color, (const void *)tsdf,
+                        (const void *)weight, (const void *)color_grid})
+    GSB_REQUIRE(aligned(p, 4), "tsdf_integrate: misaligned array");
+  const TsdfGrid g{nx, ny, nz, ox, oy, oz, voxel};
+  return launch_tsdf_integrate(g, trunc, depth_trunc, V, H, W, cams, depth, color, tsdf, weight, color_grid,
+                               (cudaStream_t)stream);
+}
+
+size_t gsb_tsdf_extract_workspace_bytes(int nx, int ny, int nz) {
+  if (nx < 1 || ny < 1 || nz < 1 || (int64_t)nx * ny * nz >= ((int64_t)1 << 31)) return 0;
+  return tsdf_extract_workspace_bytes((int64_t)nx * ny * nz);
+}
+
+// the volume and workspace checks of the plan and the emit
+static int tsdf_extract_args(int nx, int ny, int nz, const float *tsdf, const float *weight, const void *ws,
+                             size_t ws_bytes, const char *who) {
+  if (!(tsdf && weight && ws)) return arg_error(who, "null pointer");
+  if (!(aligned(tsdf, 4) && aligned(weight, 4) && aligned(ws, 256)))
+    return arg_error(who, "misaligned array or workspace");
+  if (ws_bytes < gsb_tsdf_extract_workspace_bytes(nx, ny, nz)) return arg_error(who, "workspace too small");
+  return 0;
+}
+
+int gsb_tsdf_extract_plan(int nx, int ny, int nz, const float *tsdf, const float *weight, void *ws, size_t ws_bytes,
+                          int64_t *counts_host, gsb_stream_t stream) {
+  if (int rc = tsdf_grid_check(nx, ny, nz, 0.f, 0.f, 0.f, 1.f, "tsdf_extract_plan")) return rc;  // no geometry
+  GSB_REQUIRE(counts_host != nullptr, "tsdf_extract_plan: counts_host is null");
+  if (int rc = tsdf_extract_args(nx, ny, nz, tsdf, weight, ws, ws_bytes, "tsdf_extract_plan")) return rc;
+  const TsdfGrid g{nx, ny, nz, 0.f, 0.f, 0.f, 1.f};
+  if (int rc = launch_tsdf_extract_plan(g, tsdf, weight, ws, counts_host, (cudaStream_t)stream)) return rc;
+  GSB_REQUIRE(counts_host[0] <= INT32_MAX && counts_host[1] <= INT32_MAX,
+              "tsdf_extract_plan: 2^31 or more vertices or faces");
+  return 0;
+}
+
+int gsb_tsdf_extract_emit(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const float *tsdf,
+                          const float *weight, const float *color_grid, const void *ws, size_t ws_bytes,
+                          int64_t n_verts, int64_t n_faces, float *verts, float *vcolors, int32_t *faces,
+                          gsb_stream_t stream) {
+  if (int rc = tsdf_grid_check(nx, ny, nz, ox, oy, oz, voxel, "tsdf_extract_emit")) return rc;
+  if (int rc = tsdf_extract_args(nx, ny, nz, tsdf, weight, ws, ws_bytes, "tsdf_extract_emit")) return rc;
+  GSB_REQUIRE(n_verts >= 0 && n_faces >= 0 && n_verts <= INT32_MAX && n_faces <= INT32_MAX,
+              "tsdf_extract_emit: vertex or face count out of range");
+  GSB_REQUIRE(vcolors == nullptr || color_grid != nullptr, "tsdf_extract_emit: vertex colours without a colour grid");
+  GSB_REQUIRE((n_verts == 0 || verts) && (n_faces == 0 || faces), "tsdf_extract_emit: null pointer");
+  GSB_REQUIRE(aligned(verts, 4) && aligned(vcolors, 4) && aligned(faces, 4) && aligned(color_grid, 4),
+              "tsdf_extract_emit: misaligned array");
+  if (n_verts == 0 && n_faces == 0) return 0;
+  const TsdfGrid g{nx, ny, nz, ox, oy, oz, voxel};
+  return launch_tsdf_extract_emit(g, tsdf, weight, color_grid, ws, (int)n_verts, (int)n_faces, verts, vcolors, faces,
+                                  (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -19,7 +19,8 @@ enum KernelId {
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
   K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
-  K_MCMC_ROWS, K_MCMC_NOISE, K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
+  K_MCMC_ROWS, K_MCMC_NOISE, K_TSDF_INTEGRATE, K_TSDF_PLAN, K_TSDF_EMIT,
+  K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
   K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
 };
 struct ProfScope {
@@ -324,5 +325,27 @@ int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, cons
                                 const int32_t *contrib, const float *final_tau, const float *dl_image,
                                 const float *dl_depth, const float *dl_alpha, const float *dl_normal,
                                 const GeoGrads *geo, float *rows, int *work, cudaStream_t st);
+
+// ---- mesh extraction (tsdf.cu, DESIGN 3.17; the fp64 model is oracle/tsdf_oracle.py).  The grid:
+// nx x ny x nz points, point (i, j, k) at origin + voxel (i, j, k), arrays [nz, ny, nx] (x fastest),
+// colour [3, nz, ny, nx]; N = nx ny nz < 2^31, checked by the entry points.
+struct TsdfGrid {
+  int nx, ny, nz;
+  float ox, oy, oz, voxel;
+};
+// cams: V rows of the [V, 20] camera table (ops.camera_table); depth [V, H, W]; color [V, 3, H, W]
+// and color_grid: both NULL or both set
+int launch_tsdf_integrate(const TsdfGrid &g, float trunc, float depth_trunc, int V, int H, int W, const float *cams,
+                          const float *depth, const float *color, float *tsdf, float *weight, float *color_grid,
+                          cudaStream_t st);
+// ws: tsdf_extract_workspace_bytes(N) bytes, 256-B aligned, carried from the plan to the emit;
+// counts_host <- (vertices, faces) after a host synchronisation
+size_t tsdf_extract_workspace_bytes(int64_t N);
+int launch_tsdf_extract_plan(const TsdfGrid &g, const float *tsdf, const float *weight, void *ws,
+                             int64_t *counts_host, cudaStream_t st);
+// writes vertex ids < n_verts and face slots < n_faces only, whatever the workspace holds
+int launch_tsdf_extract_emit(const TsdfGrid &g, const float *tsdf, const float *weight, const float *color_grid,
+                             const void *ws, int n_verts, int n_faces, float *verts, float *vcolors, int32_t *faces,
+                             cudaStream_t st);
 
 }  // namespace gsb

@@ -236,6 +236,38 @@ def save_ply(path, gs):
         f.write(np.ascontiguousarray(rows, "<f4").tobytes())
 
 
+def save_mesh_ply(path, verts, faces, colors=None):
+    """Writes a triangle mesh (mesh.TSDFVolume.extract's output; tensors or arrays) as binary
+    little-endian PLY: float x, y, z, with colors[V, 3] in [0, 1] also uchar red, green, blue
+    (round(255 c), clamped), and a `uchar int vertex_indices` face list."""
+    as_np = lambda a: a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)  # noqa: E731
+    v = as_np(verts).astype("<f4").reshape(-1, 3)
+    fc = as_np(faces).astype("<i4").reshape(-1, 3)
+    if len(fc) and (fc.min() < 0 or fc.max() >= len(v)):
+        raise ValueError("faces index outside the %d vertices" % len(v))
+    vdt = [("xyz", "<f4", (3,))]
+    if colors is not None:
+        c = as_np(colors).reshape(-1, 3)
+        if len(c) != len(v):
+            raise ValueError("colors must have one row per vertex")
+        vdt.append(("rgb", "u1", (3,)))
+    vrows = np.empty(len(v), vdt)
+    vrows["xyz"] = v
+    if colors is not None:
+        vrows["rgb"] = np.clip(np.rint(c.astype(np.float64) * 255), 0, 255).astype(np.uint8)
+    frows = np.empty(len(fc), [("n", "u1"), ("idx", "<i4", (3,))])
+    frows["n"], frows["idx"] = 3, fc
+    head = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % len(v)
+    head += "property float x\nproperty float y\nproperty float z\n"
+    if colors is not None:
+        head += "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+    head += "element face %d\nproperty list uchar int vertex_indices\nend_header\n" % len(fc)
+    with open(path, "wb") as f:
+        f.write(head.encode("ascii"))
+        f.write(vrows.tobytes())
+        f.write(frows.tobytes())
+
+
 def get_example_gs():
     """gau_io.py:156-183: the 4-Gaussian test scene"""
     s = 1.772484

@@ -1134,3 +1134,78 @@ def splatB_surfel_geometry(height, width, records, contrib, final_tau, patch_ran
                                                ws.numel(), _ptr(rows), near, far, _ptr(alpha), _ptr(moments),
                                                _ptr(median_contrib), *[_ptr(t) for t in planes[4:]], _stream()), lib)
     return rows
+
+
+# ---------------------------------------------------------------------------------------
+# Mesh extraction (gsb_tsdf_*, DESIGN 3.17): projective TSDF fusion of depth maps and marching
+# cubes.  The grid: point (i, j, k) at origin + voxel_size (i, j, k); tsdf, weight [nz, ny, nx] and
+# color_grid [3, nz, ny, nx] (or None), float32 CUDA tensors, contiguous (updated in place).
+def _tsdf_grid(tsdf, weight, color_grid, origin, voxel_size):
+    """checks the volume tensors and geometry -> (nx, ny, nz, ox, oy, oz, voxel)"""
+    for t, name in ((tsdf, "tsdf"), (weight, "weight")):
+        _chk(t, name, ndim=3)
+        if not t.is_contiguous():
+            raise ValueError("%s must be contiguous (it is updated in place)" % name)
+    if weight.shape != tsdf.shape:
+        raise ValueError("weight must have the shape of tsdf %s, got %s" % (tuple(tsdf.shape), tuple(weight.shape)))
+    _same_device(tsdf, weight)
+    nz, ny, nx = tsdf.shape
+    if color_grid is not None:
+        _chk(color_grid, "color_grid", ndim=4)
+        if not color_grid.is_contiguous() or color_grid.shape != (3, nz, ny, nx):
+            raise ValueError("color_grid must be a contiguous [3, nz, ny, nx] tensor")
+        _same_device(tsdf, color_grid)
+    origin = [float(x) for x in origin]
+    if len(origin) != 3:
+        raise ValueError("origin must have 3 values")
+    return (nx, ny, nz, *origin, float(voxel_size))
+
+
+def tsdf_integrate(tsdf, weight, color_grid, origin, voxel_size, trunc, depth_trunc, cams, depth, color=None):
+    """Fuses V depth maps into the volume in place, in view order (gsb_tsdf_integrate): cams is a
+    [V, 20] camera table (`camera_table`, pinhole), depth [V, H, W] and color [V, 3, H, W] float32
+    CUDA tensors; color with color_grid only.  A depth that is not finite, <= 0 or > depth_trunc
+    leaves its points alone.  One call with V views gives bit-identical grids to V calls."""
+    grid = _tsdf_grid(tsdf, weight, color_grid, origin, voxel_size)
+    cams = _chk(cams, "cams", last=CAMERA_ROW, ndim=2)
+    depth = _chk(depth, "depth", ndim=3)
+    V, H, W = depth.shape
+    if cams.shape[0] != V:
+        raise ValueError("cams must have one row per depth map")
+    size = cams[:, 16:18].cpu()  # the table's W, H: intrinsics for another resolution would be fused silently
+    if not (size == torch.tensor([float(W), float(H)])).all():
+        raise ValueError("the camera table's width and height must be the depth map's %dx%d, got %s"
+                         % (W, H, size.tolist()))
+    if (color is None) != (color_grid is None):
+        raise ValueError("color and color_grid go together: pass both or neither")
+    if color is not None:
+        color = _chk(color, "color", ndim=4)
+        if color.shape != (V, 3, H, W):
+            raise ValueError("color must be [V, 3, H, W] = %s, got %s" % ((V, 3, H, W), tuple(color.shape)))
+    _same_device(tsdf, cams, depth, *([color] if color is not None else []))
+    lib = _L()
+    with torch.cuda.device(tsdf.device):
+        _lib.check(lib.gsb_tsdf_integrate(*grid, float(trunc), float(depth_trunc), V, H, W, _ptr(cams), _ptr(depth),
+                                          _ptr(color), _ptr(tsdf), _ptr(weight), _ptr(color_grid), _stream()), lib)
+
+
+def tsdf_extract(tsdf, weight, color_grid, origin, voxel_size):
+    """Marching cubes over the observed part of the volume (gsb_tsdf_extract_*): -> (verts[V, 3]
+    float32, faces[F, 3] int32, colors[V, 3] float32 or None), deterministic.  Waits for the
+    counts on the host once."""
+    grid = _tsdf_grid(tsdf, weight, color_grid, origin, voxel_size)
+    nx, ny, nz = grid[:3]
+    lib = _L()
+    dev = tsdf.device
+    ws = _bytes(max(int(lib.gsb_tsdf_extract_workspace_bytes(nx, ny, nz)), 256), dev)
+    counts = (C.c_int64 * 2)()
+    with torch.cuda.device(dev):
+        _lib.check(lib.gsb_tsdf_extract_plan(nx, ny, nz, _ptr(tsdf), _ptr(weight), _ptr(ws), ws.numel(), counts,
+                                             _stream()), lib)
+        nv, nf = int(counts[0]), int(counts[1])
+        verts = torch.empty((nv, 3), dtype=torch.float32, device=dev)
+        faces = torch.empty((nf, 3), dtype=torch.int32, device=dev)
+        colors = torch.empty((nv, 3), dtype=torch.float32, device=dev) if color_grid is not None else None
+        _lib.check(lib.gsb_tsdf_extract_emit(*grid, _ptr(tsdf), _ptr(weight), _ptr(color_grid), _ptr(ws), ws.numel(),
+                                             nv, nf, _ptr(verts), _ptr(colors), _ptr(faces), _stream()), lib)
+    return verts, faces, colors

@@ -739,6 +739,52 @@ int gsb_splat_2dgs_backward(int H, int W, int N, int64_t P, const float *records
                             const float *alpha_image, const float *moments, const int32_t *median_contrib,
                             const float *dloss_ddistortion, const float *dloss_dmedian, gsb_stream_t stream);
 
+/* ---- mesh extraction (extension; DESIGN 3.17): projective TSDF fusion of depth maps into a
+ * dense grid and marching cubes over it, the step that turns a trained 2D Gaussian Splatting
+ * model into a mesh.
+ *
+ * The grid has nx x ny x nz sample points; point (i, j, k) sits at (ox, oy, oz) + voxel (i, j, k).
+ * Arrays are [nz, ny, nx] float32 with x fastest: tsdf, weight, and the optional color_grid
+ * [3, nz, ny, nx].  A new volume is tsdf 1, weight 0, colour 0 (the caller fills it).  Every
+ * dimension >= 1 and nx ny nz < 2^31.  Device arrays are 4-byte aligned.
+ *
+ * gsb_tsdf_integrate fuses V views in one launch, in view order.  cams: V rows of the [V, 20]
+ * camera table (Rcw row-major 9, tcw 3, fx, fy, cx, cy, W, H, 2 unused; pinhole), depth[V, H, W],
+ * color[V, 3, H, W] (NULL with color_grid NULL).  For every point p and view:
+ *   pc = Rcw p + tcw, skipped unless pc.z > 0;  u = fx pc.x / pc.z + cx, v = fy pc.y / pc.z + cy;
+ *   skipped unless 0 <= u + 1/2 < W and 0 <= v + 1/2 < H;  pixel (floor(u + 1/2), floor(v + 1/2));
+ *   D = depth there, skipped unless finite and 0 < D <= depth_trunc;  sdf = D - pc.z, skipped if
+ *   sdf < -trunc;  t = min(1, sdf / trunc);
+ *   tsdf <- (tsdf w + t) / (w + 1), colour <- (colour w + c) / (w + 1), w <- w + 1.
+ * One launch of V views and V launches of one view give bit-identical grids.  Refused: a bad
+ * dimension or voxel count, voxel or trunc not finite and > 0, depth_trunc not > 0 (inf allowed),
+ * an origin not finite, V, H or W < 1, colour on one side only.
+ *
+ * Extraction: a point is observed when w > 0 and inside when tsdf < 0; a cell (8 points, lowest
+ * corner g) is valid when all 8 are observed.  Edge (g, axis a) has a vertex when its ends differ
+ * in insideness and a valid cell contains it, at p_g + voxel e_a f, f = T_g / (T_g - T_{g+e_a}),
+ * colour C_g + f (C_{g+e_a} - C_g); vertices in order of (linear index of g, a).  Faces: valid
+ * cells in linear order, each cell's triangles in table order (mc_table.h), oriented from inside to
+ * outside; int32 indices into the vertices.  The output is deterministic.
+ * gsb_tsdf_extract_plan -> counts_host[2] = (vertices, faces).  HOST SYNCHRONISATION: it waits for
+ * the counts; the caller sizes verts[V, 3], vcolors[V, 3] and faces[F, 3] from them and passes the
+ * same workspace, grid and counts to gsb_tsdf_extract_emit.  n_verts and n_faces must be exactly the
+ * plan's counts: the emit writes no vertex id >= n_verts and no face slot >= n_faces, so smaller
+ * counts, or a workspace planned for another grid, give a wrong mesh but no write past the
+ * buffers.  A count of 2^31 or more is refused
+ * (by the plan, after writing the counts).  A grid with a dimension of 1 has no cells: 0, 0.
+ * vcolors: NULL, or with color_grid. */
+int gsb_tsdf_integrate(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, float trunc,
+                       float depth_trunc, int V, int H, int W, const float *cams, const float *depth,
+                       const float *color, float *tsdf, float *weight, float *color_grid, gsb_stream_t stream);
+size_t gsb_tsdf_extract_workspace_bytes(int nx, int ny, int nz);
+int gsb_tsdf_extract_plan(int nx, int ny, int nz, const float *tsdf, const float *weight, void *ws, size_t ws_bytes,
+                          int64_t *counts_host, gsb_stream_t stream);
+int gsb_tsdf_extract_emit(int nx, int ny, int nz, float ox, float oy, float oz, float voxel, const float *tsdf,
+                          const float *weight, const float *color_grid, const void *ws, size_t ws_bytes,
+                          int64_t n_verts, int64_t n_faces, float *verts, float *vcolors, int32_t *faces,
+                          gsb_stream_t stream);
+
 /* ---- launch accounting and optional per-kernel timing (no reference counterpart; used by
  * bench.py for `gpu_launches` and the roofline's live CUDA-event kernel durations).
  * Kernel ids 0..gsb_profile_kernels()-1, names from gsb_profile_kernel_name().
