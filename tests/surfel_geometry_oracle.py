@@ -24,27 +24,36 @@ def dm_of(z, near, far):
     return np.where(z > near, far / (far - near) * near / np.where(z > near, z, 1.0) ** 2, 0.0)
 
 
-def render_geometry(H, W, pre, alphas, bins, near=0.2, far=100.0, delta=None, margin=2e-5):
-    """so.render's planes plus distortion[H,W], moments[2,H,W] = (D, D2), median_depth[H,W] and
-    median_contrib[H,W] i32.  `ambiguous` also flags pixels where a contributing record's incoming
-    tau lies within margin of 0.5 or its hit depth within margin of near."""
+def render_geometry(H, W, pre, alphas, bins, near=0.2, far=100.0, delta=None, margin=2e-5, exact=False):
+    """so.render's planes plus distortion[H,W], moments[2,H,W] = (D, D2), median_depth[H,W],
+    median_contrib[H,W] i32 and count[H,W] i32 (the contributing records).  `ambiguous` also flags
+    pixels where a contributing record's incoming tau lies within margin of 0.5 or its hit depth within
+    margin of near.  exact: a tau of exactly 0.5 or a hit depth of exactly near is not flagged (scenes
+    built so that fp32 computes the same values); the pixels where one occurs are returned as
+    ties[H,W] and at_near[H,W]."""
     out = so.render(H, W, pre, alphas, bins, delta=delta, margin=margin)
     alphas = np.asarray(alphas, dtype=np.float64).reshape(-1)
     _, ranges, gsid, _ = bins
     out.update(distortion=np.zeros((H, W)), moments=np.zeros((2, H, W)), median_depth=np.zeros((H, W)),
-               median_contrib=np.zeros((H, W), np.int32))
+               median_contrib=np.zeros((H, W), np.int32), count=np.zeros((H, W), np.int32),
+               ties=np.zeros((H, W), bool), at_near=np.zeros((H, W), bool))
     for t, X, Y in so._tiles(H, W, ranges):
         Xf, Yf = X.astype(np.float64), Y.astype(np.float64)
         tau = np.ones(len(X))
         A, D, D2, dist, medz = (np.zeros(len(X)) for _ in range(5))
-        medc = np.zeros(len(X), np.int32)
-        amb = np.zeros(len(X), bool)
+        medc, cnt = np.zeros(len(X), np.int32), np.zeros(len(X), np.int32)
+        amb, tie, atn = np.zeros(len(X), bool), np.zeros(len(X), bool), np.zeros(len(X), bool)
         for j, i in enumerate(gsid[ranges[t, 0]:ranges[t, 1]]):
             sh = (0.0, 0.0) if delta is None else delta[i]
             e = so._eval(pre["M"][i], pre["u"][i], Xf - sh[0], Yf - sh[1])
             ap = np.minimum(so.ALPHA_CLAMP, alphas[i] * np.exp(-0.5 * e["G"]))
             on = (tau >= so.TAU_STOP) & (ap >= so.ALPHA_SKIP)
-            amb |= on & ((np.abs(tau - 0.5) < margin) | (np.abs(e["z"] - near) < margin * max(1.0, near)))
+            t5, zn = on & (tau == 0.5), on & (e["z"] == near)
+            amb |= on & (((np.abs(tau - 0.5) < margin) & ~(exact & t5)) |
+                         ((np.abs(e["z"] - near) < margin * max(1.0, near)) & ~(exact & zn)))
+            tie |= t5
+            atn |= zn
+            cnt += on
             w = np.where(on, tau * ap, 0.0)
             m = np.where(on, m_of(e["z"], near, far), 0.0)
             dist += w * (m * m * A + D2 - 2 * m * D)
@@ -59,7 +68,10 @@ def render_geometry(H, W, pre, alphas, bins, near=0.2, far=100.0, delta=None, ma
         out["moments"][:, Y, X] = np.stack([D, D2])
         out["median_depth"][Y, X] = medz
         out["median_contrib"][Y, X] = medc
+        out["count"][Y, X] = cnt
         out["ambiguous"][Y, X] |= amb
+        out["ties"][Y, X] = tie
+        out["at_near"][Y, X] = atn
     return out
 
 
@@ -162,6 +174,27 @@ def render_backward_geometry(H, W, pre, alphas, bins, fwd, dl_image=None, dl_dep
             add(16, gux, guxm)
             add(17, guy, guym)
     return (rows, absr) if abs_rows else rows
+
+
+def composited_at(H, W, pre, alphas, bins, fwd, mask):
+    """bool[N]: the surfels with a contributing record (list position < contrib, alpha' >= the skip
+    threshold) at some pixel of mask[H,W]"""
+    alphas = np.asarray(alphas, dtype=np.float64).reshape(-1)
+    _, ranges, gsid, _ = bins
+    hit = np.zeros(len(alphas), bool)
+    for t, X, Y in so._tiles(H, W, ranges):
+        m = mask[Y, X]
+        if not m.any():
+            continue
+        X, Y = X[m], Y[m]
+        cont = fwd["contrib"][Y, X]
+        for j, i in enumerate(gsid[ranges[t, 0]:ranges[t, 1]]):
+            if hit[i] or j >= cont.max():
+                continue
+            e = so._eval(pre["M"][i], pre["u"][i], X.astype(np.float64), Y.astype(np.float64))
+            ap = np.minimum(so.ALPHA_CLAMP, alphas[i] * np.exp(-0.5 * e["G"]))
+            hit[i] = ((j < cont) & (ap >= so.ALPHA_SKIP)).any()
+    return hit
 
 
 def brute_force(ws, ms, zs, taus_in, idxs):
