@@ -72,6 +72,10 @@ SIGNATURES = {
     "gsb_splat_features": (_i, [_i, _i, _i, _i64, _i] + [_vp] * 9 + [_vp, _sz, _vp, _vp]),
     "gsb_splat_features_backward": (_i, [_i, _i, _i, _i64, _i] + [_vp] * 11 + [_vp, _sz, _vp, _vp, _vp]),
     "gsb_density_apply_rows": (_i, [_i64, _vp, _vp, _i64, _i64, _i64, _i] + [_vp] * 7),
+    "gsb_splat_stats_workspace_bytes": (_sz, [_i, _i, _i, _i64]),
+    "gsb_splat_stats": (_i, [_i, _i, _i, _i64] + [_vp] * 8 + [_vp, _sz, _vp, _vp, _vp, _vp]),
+    "gsb_splat_stats_2dgs": (_i, [_i, _i, _i, _i64] + [_vp] * 8),
+    "gsb_density_plan_keep": (_i, [_i64, _vp, _vp, _sz, _vp, _vp, C.POINTER(_i64), _vp]),
     "gsb_small_bmm": (_i, [C.c_longlong, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "gsb_gau_loss_workspace_bytes": (_sz, [_i, _i]),
     "gsb_gau_loss": (_i, [_i, _i, _vp, _vp, _f, _vp, _vp, _vp, _sz, _vp]),

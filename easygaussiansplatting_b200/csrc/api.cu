@@ -42,7 +42,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
                                              "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
-                                             "draw_features", "draw_backward_features", "mcmc_scan",
+                                             "draw_features", "draw_backward_features", "draw_stats",
+                                             "draw_surfel_stats", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
                                              "mcmc_noise", "tsdf_integrate", "tsdf_plan", "tsdf_emit",
                                              "surfel_forward", "draw_surfel",
@@ -1059,6 +1060,52 @@ int gsb_splat_features_backward(int H, int W, int N, int64_t P, int D, const flo
                                        features, dloss_dfeature_image, moments, dloss_dfeatures, work, st);
 }
 
+// ---- contribution statistics (raster_stats.cu, surfel.cu k_draw_stats_2dgs; DESIGN 3.18)
+
+size_t gsb_splat_stats_workspace_bytes(int N, int H, int W, int64_t P) {
+  return feat_layout(N, H, W, P, 1).bytes;  // the feature replay's records and work area
+}
+
+// the outputs both statistics entry points accumulate into
+static int stats_outputs(const char *who, int N, const float *weight_sum, const float *weight_max,
+                         const int64_t *hit_count) {
+  if (N > 0 && !(weight_sum && weight_max && hit_count)) return arg_error(who, "null output");
+  // 4-byte atomics on the two float arrays, 8-byte atomics on the counts
+  if (!aligned(weight_sum, 4) || !aligned(weight_max, 4) || !aligned(hit_count, 8))
+    return arg_error(who, "misaligned output");
+  return 0;
+}
+
+int gsb_splat_stats(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds, const float *alphas,
+                    const float *colors, const void *packed_records, const int32_t *contrib,
+                    const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch, void *ws, size_t ws_bytes,
+                    float *weight_sum, float *weight_max, int64_t *hit_count, gsb_stream_t stream) {
+  if (int rc = stats_outputs("splat_stats", N, weight_sum, weight_max, hit_count)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const Rec *recs = nullptr;
+  int *work = nullptr;
+  // feature_frame's checks and records with one "feature" channel: the statistics read no features,
+  // so any non-null pointer stands in for them
+  if (int rc = feature_frame("splat_stats", H, W, N, P, 1, us, cinv2ds, alphas, colors, weight_sum, contrib,
+                             patch_range_per_tile, gsid_per_patch, packed_records, ws, ws_bytes, &recs, &work, st))
+    return rc;
+  return launch_draw_stats(H, W, patch_range_per_tile, recs, gsid_per_patch, contrib, weight_sum, weight_max,
+                           hit_count, work, st);
+}
+
+int gsb_splat_stats_2dgs(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                           const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch, float *weight_sum,
+                           float *weight_max, int64_t *hit_count, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splat_stats_2dgs: bad N/H/W/P");
+  GSB_REQUIRE(grid_fits(H, W), "splat_stats_2dgs: more than 65535 tiles in a row or column");
+  if (int rc = stats_outputs("splat_stats_2dgs", N, weight_sum, weight_max, hit_count)) return rc;
+  if (N == 0 || P == 0) return 0;
+  GSB_REQUIRE(records && contrib && patch_range_per_tile && gsid_per_patch, "splat_stats_2dgs: null pointer");
+  GSB_REQUIRE(aligned(records, 16) && aligned(patch_range_per_tile, 8), "splat_stats_2dgs: misaligned input");
+  return launch_draw_surfel_stats(H, W, patch_range_per_tile, records, gsid_per_patch, contrib, weight_sum, weight_max,
+                                  hit_count, (cudaStream_t)stream);
+}
+
 // ---- density control + record conversion (density.cu)
 
 static bool gau_complete(const gsb_gaussians *g) {
@@ -1098,6 +1145,15 @@ int gsb_density_plan(int64_t N, const float *alphas_raw, const float *scales_raw
   GSB_REQUIRE(N == 0 || ws_bytes >= density_workspace_bytes(N), "density_plan: workspace too small");
   return launch_density_plan(N, alphas_raw, scales_raw, grad_accum, cunt, alpha_raw_min, scale_raw_max, grad_min,
                              scale_clone_max, ws, ws_bytes, cls, slots, counts_host, (cudaStream_t)stream);
+}
+
+int gsb_density_plan_keep(int64_t N, const uint8_t *keep, void *ws, size_t ws_bytes, uint8_t *cls, int32_t *slots,
+                          int64_t *counts_host, gsb_stream_t stream) {
+  GSB_REQUIRE(N >= 0 && N < ((int64_t)1 << 31), "density_plan_keep: N out of range");
+  GSB_REQUIRE(counts_host != nullptr, "density_plan_keep: counts_host is null");
+  GSB_REQUIRE(N == 0 || (keep && ws && cls && slots), "density_plan_keep: null pointer");
+  GSB_REQUIRE(N == 0 || ws_bytes >= density_workspace_bytes(N), "density_plan_keep: workspace too small");
+  return launch_density_plan_keep(N, keep, ws, cls, slots, counts_host, (cudaStream_t)stream);
 }
 
 int gsb_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C, int64_t S,

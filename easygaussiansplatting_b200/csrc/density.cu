@@ -161,6 +161,25 @@ __global__ void __launch_bounds__(SC_THREADS) k_density_classify_count(
     DensityBlocks{block_counts}.store(blockIdx.x, {(int)(n.kc & 0xffffu), (int)(n.kc >> 16), (int)n.sp});
 }
 
+// the classify pass of a prune by mask (gsb_density_plan_keep): keep[i] != 0 -> CLS_KEEP, else CLS_PRUNE
+__global__ void __launch_bounds__(SC_THREADS) k_density_keep_count(int64_t N, const uint8_t *__restrict__ keep,
+                                                                   uint8_t *__restrict__ cls,
+                                                                   int32_t *__restrict__ block_counts) {
+  __shared__ KcSp red[SC_THREADS / 32];
+  KcSp n{0, 0};
+#pragma unroll
+  for (int j = 0; j < SC_PER; j++) {
+    const int64_t i = (int64_t)blockIdx.x * SC_ROWS + j * SC_THREADS + threadIdx.x;
+    if (i < N) {
+      const uint8_t c = keep[i] != 0 ? CLS_KEEP : CLS_PRUNE;
+      cls[i] = c;
+      n = n + class_count(c);
+    }
+  }
+  n = cta_sum<SC_THREADS>(n, red);
+  if (threadIdx.x == 0) DensityBlocks{block_counts}.store(blockIdx.x, {(int)(n.kc & 0xffffu), 0, 0});
+}
+
 __global__ void __launch_bounds__(SC_THREADS) k_density_slots(int64_t N, const uint8_t *__restrict__ cls,
                                                               const DensityBlocks block_offsets,
                                                               Slot3 *__restrict__ slots) {
@@ -850,6 +869,21 @@ int launch_density_accumulate(int64_t N, const float *dloss_dus, const uint8_t *
   return 0;
 }
 
+// the scan of both plans once cls and the per-CTA counts are written: slots, then the three totals
+// read back (the plan's one host synchronisation)
+static int density_slots(int64_t N, int nb, const uint8_t *cls, int64_t *totals, int32_t *block_counts,
+                         int32_t *slots, int64_t *counts_host, cudaStream_t st) {
+  {
+    ProfScope ps(K_DENSITY_SCAN, st);
+    k_density_scan_blocks<<<1, 1024, 0, st>>>(nb, DensityBlocks{block_counts}, totals);
+    k_density_slots<<<nb, SC_THREADS, 0, st>>>(N, cls, DensityBlocks{block_counts}, reinterpret_cast<Slot3 *>(slots));
+    GSB_CUDA_TRY(cudaGetLastError());
+  }
+  GSB_CUDA_TRY(cudaMemcpyAsync(counts_host, totals, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  GSB_CUDA_TRY(cudaStreamSynchronize(st));
+  return 0;
+}
+
 int launch_density_plan(int64_t N, const float *alphas_raw, const float *scales_raw, const float *grad_accum,
                         const int32_t *cunt, float alpha_raw_min, float scale_raw_max, float grad_min,
                         float scale_clone_max, void *ws, size_t ws_bytes, uint8_t *cls, int32_t *slots,
@@ -865,15 +899,22 @@ int launch_density_plan(int64_t N, const float *alphas_raw, const float *scales_
                                                        scale_raw_max, grad_min, scale_clone_max, cls, block_counts);
     GSB_CUDA_TRY(cudaGetLastError());
   }
+  return density_slots(N, nb, cls, totals, block_counts, slots, counts_host, st);
+}
+
+int launch_density_plan_keep(int64_t N, const uint8_t *keep, void *ws, uint8_t *cls, int32_t *slots,
+                             int64_t *counts_host, cudaStream_t st) {
+  counts_host[0] = counts_host[1] = counts_host[2] = 0;
+  if (N == 0) return 0;
+  int64_t *totals = static_cast<int64_t *>(ws);
+  int32_t *block_counts = reinterpret_cast<int32_t *>(static_cast<char *>(ws) + 256);
+  const int nb = (int)((N + SC_ROWS - 1) / SC_ROWS);
   {
-    ProfScope ps(K_DENSITY_SCAN, st);
-    k_density_scan_blocks<<<1, 1024, 0, st>>>(nb, DensityBlocks{block_counts}, totals);
-    k_density_slots<<<nb, SC_THREADS, 0, st>>>(N, cls, DensityBlocks{block_counts}, reinterpret_cast<Slot3 *>(slots));
+    ProfScope ps(K_DENSITY_CLASSIFY, st);
+    k_density_keep_count<<<nb, SC_THREADS, 0, st>>>(N, keep, cls, block_counts);
     GSB_CUDA_TRY(cudaGetLastError());
   }
-  GSB_CUDA_TRY(cudaMemcpyAsync(counts_host, totals, 3 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  GSB_CUDA_TRY(cudaStreamSynchronize(st));
-  return 0;
+  return density_slots(N, nb, cls, totals, block_counts, slots, counts_host, st);
 }
 
 int launch_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C,

@@ -18,7 +18,7 @@ enum KernelId {
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
-  K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
+  K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
   K_MCMC_ROWS, K_MCMC_NOISE, K_TSDF_INTEGRATE, K_TSDF_PLAN, K_TSDF_EMIT,
   K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
   K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
@@ -169,6 +169,10 @@ int launch_density_plan(int64_t N, const float *alphas_raw, const float *scales_
                         const int32_t *cunt, float alpha_raw_min, float scale_raw_max, float grad_min,
                         float scale_clone_max, void *ws, size_t ws_bytes, uint8_t *cls, int32_t *slots,
                         int64_t *counts_host, cudaStream_t st);
+// the plan of a prune by mask: cls = CLS_KEEP where keep[i] != 0, else CLS_PRUNE, the same slots
+// scan; counts_host <- (K, 0, 0)
+int launch_density_plan_keep(int64_t N, const uint8_t *keep, void *ws, uint8_t *cls, int32_t *slots,
+                             int64_t *counts_host, cudaStream_t st);
 int launch_density_apply(int64_t N, const uint8_t *cls, const int32_t *slots, int64_t K, int64_t C,
                          float *const *src, float *const *src_m, float *const *src_v, const float *z,
                          float *const *dst, float *const *dst_m, float *const *dst_v, cudaStream_t st);
@@ -288,6 +292,19 @@ struct FeatLayout {
   size_t recs, work, bytes;
 };
 FeatLayout feat_layout(int N, int H, int W, int64_t P, uintptr_t base);
+
+// ---- contribution statistics (raster_stats.cu, surfel.cu; DESIGN 3.18): replays of a drawn frame
+// that ADD per-Gaussian sums of the blending weights w, their maximum (weight_max[N] updated as the
+// uint bits of w >= 0) and the count of pixels with w > 0.  weight_sum / weight_max: any 4-byte
+// alignment, hit_count 8-byte aligned.  recs == nullptr: no patches, nothing added.  The colour
+// replay takes feat_layout's records and work area (launch_tile_list's); the surfel replay launches
+// one CTA per tile and needs no work area.
+int launch_draw_stats(int H, int W, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
+                      const int32_t *contrib, float *weight_sum, float *weight_max, int64_t *hit_count, int *work,
+                      cudaStream_t st);
+int launch_draw_surfel_stats(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid,
+                             const int32_t *contrib, float *weight_sum, float *weight_max, int64_t *hit_count,
+                             cudaStream_t st);
 
 // ---- 2D Gaussian Splatting (surfel.cu, DESIGN 3.15; the math is surfel_math.h).  recs: one 80-byte
 // record per surfel ([N,20] floats, 16-byte aligned); rows: the backward rasterizer's [N,18]

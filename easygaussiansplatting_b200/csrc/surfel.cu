@@ -15,6 +15,7 @@
 //  k_draw_2dgs_bwd     k_draw_surfel_bwd's walk (draw_bwd_walk<true>) with the geometry terms added to
 //                      the alpha' recurrence and to the hit-depth gradient; the rows are the same
 //  k_surfel_bwd<K3>    the rows -> dL/dpws, dL/dshs, dL/dalphas, dL/dscales, dL/drots, dL/dus (= ddelta)
+//  k_draw_stats_2dgs   per-surfel sums, maxima and counts of a drawn frame's weights (DESIGN 3.18)
 #include "common.cuh"
 #include "kernels.h"
 #include "raster_walk.cuh"
@@ -31,6 +32,11 @@ namespace gsb {
 #endif
 #ifndef DRAW_2DGS_BWD_MINBLOCKS
 #define DRAW_2DGS_BWD_MINBLOCKS 4
+#endif
+// k_draw_stats_2dgs: 56 registers and 21 KiB of shared memory without spills (-Xptxas -v), so 8
+// CTAs of 128 threads fit the register file
+#ifndef DRAW_STATS_2DGS_MINBLOCKS
+#define DRAW_STATS_2DGS_MINBLOCKS 8
 #endif
 
 constexpr int SREC_BYTES = sf::kRecFloats * 4;  // 80
@@ -527,9 +533,89 @@ __global__ void __launch_bounds__(128, DRAW_2DGS_BWD_MINBLOCKS) k_draw_2dgs_bwd(
   draw_bwd_walk<true>(W, H, gx, ranges, recs, gsid, contrib, final_tau, a.dl, a.geo, rows, work);
 }
 
+// Contribution statistics of a drawn surfel frame (DESIGN 3.18): k_draw_stats' three reductions
+// (raster_stats.cu) over the 80-byte records.  One CTA per tile, warp = 8x8 block, front to back to
+// the block's largest contrib; a record reaches a pixel exactly when its patch index is below the
+// pixel's contrib and alpha' >= 0.002 (k_draw_surfel's stop rule: tau only falls, so every record
+// before the last contributing one met tau >= 1e-4), and alpha' (surfel_alpha), tau and w are
+// k_draw_surfel's fp32 operations, so the weights are its bits.  The record has no id word: the
+// surfel's id is the patch list's entry at the survivor's patch index.
+__global__ void __launch_bounds__(128, DRAW_STATS_2DGS_MINBLOCKS) k_draw_stats_2dgs(
+    int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, float *__restrict__ weight_sum,
+    uint32_t *__restrict__ weight_max, unsigned long long *__restrict__ hit_count) {
+  __shared__ __align__(16) unsigned char s_ring[4][WALK_RING * WALK_CHUNK_BYTES<SREC_BYTES>];
+  __shared__ __align__(16) uint2 s_list[4][32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned F = 0xffffffffu;
+  const uint32_t ring_addr = opaque_u32(smem_u32(&s_ring[warp][0]));
+  const uint32_t list_addr = opaque_u32(smem_u32(&s_list[warp][0]));
+  const int tile = blockIdx.x;
+  const int2 range = __ldg(ranges + tile);
+  const int len = range.y - range.x;
+  const int32_t *ids = gsid + range.x;
+  BlockPix bp;
+  if (len <= 0 || !block_pix(W, H, gx, tile, warp, lane, bp)) return;
+  const float xs[2] = {(float)bp.px, (float)(bp.px + 1)}, y = (float)bp.py;
+  const int cont[2] = {bp.in0 ? min(__ldg(contrib + bp.pix), len) : 0,
+                       bp.in1 ? min(__ldg(contrib + bp.pix + 1), len) : 0};
+  int wmax = max(cont[0], cont[1]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(F, wmax, o));
+  if (wmax <= 0) return;
+  const int nch = (wmax + 31) >> 5;
+  auto issue = [&](int c) {
+    if (c < nch && c * 32 + lane < wmax)
+      gather_record<SREC_BYTES>(recs + 5 * (size_t)__ldg(ids + c * 32 + lane),
+                                ring_addr + (c & (WALK_RING - 1)) * WALK_CHUNK_BYTES<SREC_BYTES> + lane * SREC_BYTES);
+    cp_async_commit();
+  };
+#pragma unroll
+  for (int r = 0; r < WALK_RING; r++) issue(r);
+  const float bx0 = (float)bp.rx0, bx1 = (float)(bp.rx0 + 7), by0 = (float)bp.ry0, by1 = (float)(bp.ry0 + 7);
+  float tau[2] = {1.0f, 1.0f};
+  for (int c = 0; c < nch; c++) {
+    const int n = surfel_compact(wait_chunk<SREC_BYTES>(ring_addr, c, lane), c * 32 + lane, wmax, bx0, bx1, by0, by1,
+                                 list_addr, lane, false);
+    for (int i = 0; i < n; i++) {
+      const uint2 e = lds64u(list_addr + i * 8);
+      SRecRegs r;
+      load_srec(e.x, r);
+      float w[2];
+#pragma unroll
+      for (int p = 0; p < 2; p++) {
+        sf::PixEval pe;
+        float g;
+        bool clamped;
+        const float ap = surfel_alpha(r, xs[p], y, pe, g, clamped);
+        w[p] = 0.0f;
+        if ((int)e.y < cont[p] && ap >= ALPHA_SKIP) {
+          w[p] = tau[p] * ap;
+          tau[p] = tau[p] * (1.0f - ap);
+        }
+      }
+      const unsigned cnt = __reduce_add_sync(F, (unsigned)(w[0] > 0.0f) + (unsigned)(w[1] > 0.0f));
+      if (cnt == 0) continue;  // warp-uniform
+      const unsigned mx = __reduce_max_sync(F, max(__float_as_uint(w[0]), __float_as_uint(w[1])));
+      float s = w[0] + w[1];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(F, s, o);
+      if (lane == 0) {
+        const int id = __ldg(ids + (int)e.y);
+        atomicAdd(weight_sum + id, s);
+        atomicMax(weight_max + id, mx);
+        atomicAdd(hit_count + id, (unsigned long long)cnt);
+      }
+    }
+    __syncwarp();  // every lane is done with this ring slot and with the list
+    issue(c + WALK_RING);
+  }
+  walk_drain();
+}
+
 // ---- launchers
 
-#define GSB_SURFEL_K3(k3, CALL)                                             \
+#define GSB_SURFEL_K3(k3, CALL)                                           \
   switch (k3) {                                                             \
     case 1: { constexpr int K3 = 1; CALL; } break;                          \
     case 4: { constexpr int K3 = 4; CALL; } break;                          \
@@ -626,6 +712,20 @@ int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, cons
     ProfScope ps(K_DRAW_SURFEL_BWD, st);
     k_draw_surfel_bwd<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, contrib, final_tau, dl, rows, work);
   }
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_draw_surfel_stats(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid,
+                             const int32_t *contrib, float *weight_sum, float *weight_max, int64_t *hit_count,
+                             cudaStream_t st) {
+  const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
+  if (gx <= 0 || gy <= 0 || recs == nullptr) return 0;  // no patches: nothing to add
+  ProfScope ps(K_DRAW_SURFEL_STATS, st);
+  k_draw_stats_2dgs<<<gx * gy, 128, 0, st>>>(W, H, gx, reinterpret_cast<const int2 *>(ranges),
+                                               reinterpret_cast<const float4 *>(recs), gsid, contrib, weight_sum,
+                                               reinterpret_cast<uint32_t *>(weight_max),
+                                               reinterpret_cast<unsigned long long *>(hit_count));
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

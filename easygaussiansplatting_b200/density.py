@@ -202,6 +202,63 @@ def apply_rows(cls, slots, counts, src, src_m=None, src_v=None):
     return dst, dst_m, dst_v
 
 
+def plan_keep(keep):
+    """gsb_density_plan_keep -> (cls uint8 [N], slots int32 [N,3], (K, 0, 0)).  Waits for K (one D2H)."""
+    lib = _lib.load()
+    N = keep.shape[0]
+    dev = keep.device
+    cls = torch.empty(N, dtype=torch.uint8, device=dev)
+    slots = torch.empty((N, 3), dtype=torch.int32, device=dev)
+    nbytes = lib.gsb_density_workspace_bytes(N)
+    ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    counts = (C.c_int64 * 3)()
+    _lib.check(lib.gsb_density_plan_keep(N, _ptr(keep), _ptr(ws), nbytes, _ptr(cls), _ptr(slots), counts, _stream()),
+               lib)
+    return cls, slots, (int(counts[0]), int(counts[1]), int(counts[2]))
+
+
+@torch.no_grad()
+def prune(params, optimizer, keep, extra=(), verbose=True):
+    """Removes the Gaussians where keep[N] (bool, CUDA) is False: the six tensors of `params`, the
+    [N, D] `extra` entries (per-Gaussian features) and their Adam moments, through one plan scan
+    (gsb_density_plan_keep) and the density rebuild (gsb_density_apply / _rows).  Survivors keep
+    their order and their moments; the optimizer groups get the new Parameters, and the other
+    fields of their state (`step`) are left as they were.  Works with torch.optim.Adam and
+    GaussianAdam, with or without optimizer state.  Prints the reference-style report when verbose.
+    A captured GraphedFusedStep must be captured again afterwards.  -> dict(pruned, total)"""
+    extra = tuple(extra)
+    N, src, src_m, src_v, groups = gather_state(params, optimizer, extra, _copy)
+    keep = _check(keep, "keep", (N,), torch.bool)
+    if keep.device != src["pws"].device:
+        raise ValueError("keep must be on the device of the parameters")
+    cls, slots, counts = plan_keep(keep)
+    K = counts[0]
+    dst, dst_m, dst_v = apply(cls, slots, counts, src, src_m, src_v, None)
+    for k in extra:
+        dst[k], dm, dv = apply_rows(cls, slots, counts, src[k], src_m[k] if src_m else None, src_v[k] if src_v else None)
+        if dst_m is not None:
+            dst_m[k], dst_v[k] = dm, dv
+    swap_parameters(params, optimizer, groups, dst, dst_m, dst_v)
+    report(verbose, "prune", [("pruned num", N - K), ("total gaussian number", K)])
+    return dict(pruned=N - K, total=K)
+
+
+def lowest(score, fraction):
+    """A keep mask over score[N] that drops exactly floor(fraction * N) rows: those with the lowest
+    scores, ties broken by the lower index (a stable ascending sort), so the mask is deterministic.
+    -> bool [N] on the device of score"""
+    if not isinstance(score, torch.Tensor) or score.dim() != 1:
+        raise ValueError("score must be a 1-D tensor")
+    if not 0.0 <= float(fraction) <= 1.0:
+        raise ValueError("fraction must be in [0, 1]")
+    N = score.shape[0]
+    n_drop = int(np.floor(float(fraction) * N))
+    keep = torch.ones(N, dtype=torch.bool, device=score.device)
+    order = torch.sort(score, stable=True).indices
+    keep[order[:n_drop]] = False
+    return keep
+
+
 class DensityController:
     """the density-control half of gsplat.gsmodel.GSModel (gsmodel.py:168-331), same attribute
     names (`grad_accum`, `cunt`) and the same printed report.
@@ -261,6 +318,15 @@ class DensityController:
         self.grad_accum = None
         self.cunt = None
         return dict(pruned=N - K, cloned=Cn, splited=S, total=K + Cn + S)
+
+    def prune(self, params, optimizer, keep, extra=()):
+        """`prune` with this controller's verbosity.  It also drops the accumulated densification
+        statistics (`grad_accum`, `cunt`): they are indexed by the old rows, so the next
+        update_gaussian_density needs update_density_info calls made after the prune."""
+        out = prune(params, optimizer, keep, extra, self.verbose)
+        self.grad_accum = None
+        self.cunt = None
+        return out
 
     @torch.no_grad()
     def reset_alpha(self, params, optimizer):

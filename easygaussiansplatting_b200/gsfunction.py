@@ -492,3 +492,49 @@ class GSFunctionSurfelGeometry(torch.autograd.Function):
             rows)
         grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
         return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
+
+
+@torch.no_grad()
+def contribution_stats(pws, shs, alphas, scales, rots, cams, filter3d=None, surfel=False):
+    """Per-Gaussian contribution statistics over the views `cams` (DESIGN 3.18), with exactly the
+    blending weights w = tau alpha' those views render.  Each camera runs the fused forward the
+    training classes run -- 3DGS: ops.preprocess (antialiasing, filter3d and the camera model as in
+    GSFunctionFused) and ops.splat; surfel=True: ops.surfel_preprocess and ops.splat_surfel, pinhole
+    cameras only, as GSFunctionSurfel -- then the replay (ops.splat_stats / ops.splat_surfel_stats).
+    -> dict(weight_sum[N] f32 = sum over views and pixels of w, weight_max[N] f32 = the largest w,
+    hit_count[N] i64 = the (view, pixel) pairs with w > 0, views[N] i32 = the cameras in which the
+    Gaussian had at least one hit).  The compaction scores built on them are plain torch
+    (INTEGRATION.md, "Contribution pruning")."""
+    from . import ops
+    N, dev = pws.shape[0], pws.device
+    weight_sum = torch.zeros(N, dtype=torch.float32, device=dev)
+    weight_max = torch.zeros(N, dtype=torch.float32, device=dev)
+    hit_count = torch.zeros(N, dtype=torch.int64, device=dev)
+    views = torch.zeros(N, dtype=torch.int32, device=dev)
+    out = (weight_sum, weight_max, hit_count)
+    if surfel and filter3d is not None:
+        raise ValueError("surfels have no 3D filter: filter3d must be None")
+    if filter3d is not None:
+        scales, alphas = ops.filter3d_apply(scales, alphas, filter3d)
+    for cam in cams:
+        before = hit_count.clone()
+        if surfel:
+            if getattr(cam, "antialiased", False):
+                raise ValueError("surfels have no antialiased mode: cam.antialiased must be False")
+            _pinhole_only(cam, "contribution_stats(surfel=True)")
+            us, depths, areas, _, records = ops.surfel_preprocess(
+                pws, rots, scales, shs, alphas.reshape(-1), cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+                cam.width, cam.height)
+            frame = ops.splat_surfel(cam.height, cam.width, us, depths, areas, records, capacity=True)
+            ops.splat_surfel_stats(cam.height, cam.width, records, frame[1], frame[3], frame[4], out=out)
+        else:
+            aa = bool(getattr(cam, "antialiased", False))
+            pre = ops.preprocess(pws, rots, scales, shs, cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy, cam.cx, cam.cy,
+                                 cam.width, cam.height, alphas=alphas, antialiased=aa, **camera_model_kwargs(cam))
+            us, cinv2ds, colors, depths, areas, records = pre[:6]
+            drawn = pre[6] if aa else alphas  # the opacities the rasterizer composites
+            frame = ops.splat(cam.height, cam.width, us, cinv2ds, drawn, depths, colors, areas, records=records,
+                              capacity=True)
+            ops.splat_stats(cam.height, cam.width, frame[1], frame[3], frame[4], records=records, out=out)
+        views += (hit_count > before).to(torch.int32)
+    return dict(weight_sum=weight_sum, weight_max=weight_max, hit_count=hit_count, views=views)

@@ -636,6 +636,53 @@ def splatB_features(height, width, features, contrib, final_tau, patch_range_per
 
 
 # ---------------------------------------------------------------------------------------
+# Contribution statistics (extension; DESIGN 3.18): per-Gaussian sums of the blending weights.
+def _stats_out(out, N, dev):
+    """the accumulators of `splat_stats` / `splat_surfel_stats`: fresh zeros, or the caller's
+    (weight_sum[N] f32, weight_max[N] f32, hit_count[N] i64), contiguous, on `dev`"""
+    if out is None:
+        return (torch.zeros(N, dtype=torch.float32, device=dev), torch.zeros(N, dtype=torch.float32, device=dev),
+                torch.zeros(N, dtype=torch.int64, device=dev))
+    if not (isinstance(out, (tuple, list)) and len(out) == 3):
+        raise ValueError("out must be (weight_sum, weight_max, hit_count)")
+    for t, name, dt in zip(out, ("weight_sum", "weight_max", "hit_count"), (torch.float32, torch.float32, torch.int64)):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dt and tuple(t.shape) == (N,) and
+                t.is_contiguous() and t.device == dev):
+            raise ValueError("%s must be a contiguous %s [N] tensor on the frame's device" % (name, dt))
+    return tuple(out)
+
+
+def splat_stats(height, width, contrib, patch_range_per_tile, gsid_per_patch, records=None, us=None, cinv2ds=None,
+                alphas=None, colors=None, out=None):
+    """Contribution statistics of a frame `splat` (or `splat_rgbd`) drew (gsb_splat_stats), with the
+    blending weights w = tau alpha' the image composited (the same bits):
+        weight_sum[i] += sum_p w_i(p),  weight_max[i] = max(weight_max[i], max_p w_i(p)),
+        hit_count[i] += #{p : w_i(p) > 0}.
+    contrib, patch_range_per_tile, gsid_per_patch: that frame's outputs.  records, us, cinv2ds,
+    alphas, colors: as for `splat_features` (given, attached to gsid_per_patch by `splat`, or
+    re-packed); N is taken from records, else from us.  out: (weight_sum[N] f32, weight_max[N] f32,
+    hit_count[N] i64) to accumulate into, in place (weight_max must hold values >= 0); None: fresh
+    zeros.  -> (weight_sum, weight_max, hit_count)"""
+    ref = records if records is not None else us
+    if ref is None:
+        raise ValueError("give the forward's records, or us, cinv2ds, alphas and colors to find or re-pack them")
+    N = ref.shape[0]
+    # _feature_frame's checks and record rules, with a [N, 1] stand-in for the features it checks
+    H, W, N, _, P, _, contrib, ranges, gsid, recs, attrs = _feature_frame(
+        height, width, torch.empty((N, 1), dtype=torch.float32, device=ref.device), contrib, patch_range_per_tile,
+        gsid_per_patch, records, us, cinv2ds, alphas, colors)
+    dev = contrib.device
+    ws_sum, ws_max, hits = _stats_out(out, N, dev)
+    lib = _L()
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_splat_stats_workspace_bytes(N, H, W, 0 if recs else P), dev)
+        _lib.check(lib.gsb_splat_stats(H, W, N, P, *[_ptr(a) for a in attrs], recs, _ptr(contrib), _ptr(ranges),
+                                       _ptr(gsid), _ptr(ws), ws.numel(), _ptr(ws_sum), _ptr(ws_max), _ptr(hits),
+                                       _stream()), lib)
+    return ws_sum, ws_max, hits
+
+
+# ---------------------------------------------------------------------------------------
 # Extensions (not in the reference module): the fused per-Gaussian path, SURVEY 8f row N1.
 CAMERA_MODELS = ("pinhole", "ortho", "fisheye")  # GSB_CAMERA_PINHOLE, _ORTHO, _FISHEYE
 
@@ -1049,6 +1096,27 @@ def splatB_surfel(height, width, records, contrib, final_tau, patch_range_per_ti
                                                  _ptr(ranges), _ptr(gsid), *[_ptr(t) for t in planes], _ptr(ws),
                                                  ws.numel(), _ptr(rows), _stream()), lib)
     return rows
+
+
+def splat_surfel_stats(height, width, records, contrib, patch_range_per_tile, gsid_per_patch, out=None):
+    """`splat_stats` for a frame `splat_surfel` / `splat_surfel_geometry` drew from records[N,20]
+    (gsb_splat_stats_2dgs): the same three statistics with the surfel frame's weights (its bits).
+    out: as for `splat_stats`.  -> (weight_sum, weight_max, hit_count)"""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    contrib = _chk(contrib, "contrib", dtype=torch.int32)
+    ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
+    gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
+    _same_device(records, contrib, ranges, gsid)
+    _check_drawn(H, W, ranges, ((contrib, 1),), "contrib does not match height x width")
+    N, P, dev, lib = records.shape[0], gsid.numel(), records.device, _L()
+    ws_sum, ws_max, hits = _stats_out(out, N, dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.gsb_splat_stats_2dgs(H, W, N, P, _ptr(records), _ptr(contrib), _ptr(ranges), _ptr(gsid),
+                                              _ptr(ws_sum), _ptr(ws_max), _ptr(hits), _stream()), lib)
+    return ws_sum, ws_max, hits
 
 
 # 2DGS geometry terms (extension; DESIGN 3.16): depth distortion and median depth of the surfel frame.

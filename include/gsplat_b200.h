@@ -441,6 +441,32 @@ int gsb_splat_features_backward(int H, int W, int N, int64_t P, int D, const flo
                                 const float *dloss_dfeature_image, void *ws, size_t ws_bytes, float *moments,
                                 float *dloss_dfeatures, gsb_stream_t stream);
 
+/* ---- contribution statistics (extension; DESIGN 3.18).  Per Gaussian, over the pixels of one
+ * drawn frame, with the blending weights w = tau alpha' the frame composited (same clamp, skip and
+ * stop rules, same fp32 operations: every w is the bit pattern the image used):
+ *   weight_sum[i] += sum_p w_i(p)            (fp32 atomics: the order of the additions varies)
+ *   weight_max[i]  = max(weight_max[i], max_p w_i(p))   (exact; updated through its uint bits,
+ *                    so it must hold values >= 0, e.g. zeros, before the first frame)
+ *   hit_count[i]  += #{p : w_i(p) > 0}       (exact)
+ * All three are READ-MODIFY-WRITE: zero them once, then call once per view to accumulate.
+ * weight_sum, weight_max: any 4-byte alignment; hit_count: 8-byte aligned.  N == 0 or P == 0:
+ * nothing is added.
+ * gsb_splat_stats replays a frame gsb_splat_render / _forward (colour or RGB-D) drew: its contrib,
+ *   patch_range_per_tile, gsid_per_patch and records, given as packed_records or packed into `ws`
+ *   from us, cinv2ds, alphas and colors, as gsb_splat_features does.  ws:
+ *   gsb_splat_stats_workspace_bytes(N, H, W, P) bytes, any alignment (P = 0 when packed_records is
+ *   given).
+ * gsb_splat_stats_2dgs replays a surfel frame (2D Gaussian Splatting) that gsb_splat_surfel_* or
+ *   gsb_splat_2dgs_* drew, from its 80-byte records (16-byte aligned); no workspace. */
+size_t gsb_splat_stats_workspace_bytes(int N, int H, int W, int64_t P);
+int gsb_splat_stats(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds, const float *alphas,
+                    const float *colors, const void *packed_records, const int32_t *contrib,
+                    const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch, void *ws, size_t ws_bytes,
+                    float *weight_sum, float *weight_max, int64_t *hit_count, gsb_stream_t stream);
+int gsb_splat_stats_2dgs(int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                           const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch, float *weight_sum,
+                           float *weight_max, int64_t *hit_count, gsb_stream_t stream);
+
 /* ---- batched tiny matmul (extension).  C[b] = A[b] (m x k) . B[b] (k x n), or B shared by all
  * batches when b_shared != 0; dense row-major f32.  This is the product the reference's
  * GSFunction.backward applies ~12 times over the per-Gaussian Jacobians (gsmodel.py:72-85);
@@ -496,6 +522,14 @@ int gsb_density_plan(int64_t N, const float *alphas_raw, const float *scales_raw
                      const int32_t *cunt, float alpha_raw_min, float scale_raw_max, float grad_min,
                      float scale_clone_max, void *ws, size_t ws_bytes, uint8_t *cls, int32_t *slots,
                      int64_t *counts_host, gsb_stream_t stream);
+
+/* The plan of a prune by mask: cls[i] = 0 (keep) where keep[i] != 0, else 3 (prune), and slots
+ * as gsb_density_plan writes them; counts_host[3] <- (K survivors, 0, 0), so gsb_density_apply /
+ * gsb_density_apply_rows with C = S = 0 keep the survivors in order with their Adam moments.
+ * Workspace: gsb_density_workspace_bytes(N).  HOST SYNCHRONISATION: one read of K, as
+ * gsb_density_plan. */
+int gsb_density_plan_keep(int64_t N, const uint8_t *keep, void *ws, size_t ws_bytes, uint8_t *cls, int32_t *slots,
+                          int64_t *counts_host, gsb_stream_t stream);
 
 /* The rebuild (:236-318 + :132-166).  dst rows: survivors in order, then clones, then splits.
  * A clone row is (pws, shs, logit(sigmoid(alphas_raw)), log(exp(scales_raw)),
