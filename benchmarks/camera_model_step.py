@@ -1,6 +1,7 @@
 """Cost of the camera models at BASELINE config 2 (1M Gaussians, SH degree 3, 1920x1080).
 
-For pinhole, ortho, fisheye (k = 0) and fisheye with COLMAP-like k1..k4: the fused training step of
+For pinhole, ortho, fisheye (k = 0), fisheye with COLMAP-like k1..k4, opencv (k = p = 0) and opencv with
+COLMAP-like k1, k2, p1, p2: the fused training step of
 GSFunctionFused (forward + backward through autograd) and the per-launch CUDA-event times
 (gsb_profile_*) of the preprocess_forward, preprocess_backward, draw and draw_backward scopes, and P
 (the patches the frame binned).  Each model's scene is scene.camera_model_scene: the generator's target
@@ -25,13 +26,15 @@ sys.path.insert(0, ROOT)
 
 from easygaussiansplatting_b200 import _lib, ops  # noqa: E402
 from easygaussiansplatting_b200.gsfunction import Camera, GSFunctionFused  # noqa: E402
-from easygaussiansplatting_b200.scene import (COLMAP_LIKE_FISHEYE_K, camera_model_scene,  # noqa: E402
-                                               upstream_gradient)
+from easygaussiansplatting_b200.scene import (COLMAP_LIKE_FISHEYE_K, COLMAP_LIKE_OPENCV,  # noqa: E402
+                                               camera_model_scene, upstream_gradient)
 
 N, W, H, SH = 1_000_000, 1920, 1080, 48
 KERNELS = ("preprocess_forward", "preprocess_backward", "draw", "draw_backward")
-MODELS = (("pinhole", "pinhole", None), ("ortho", "ortho", None), ("fisheye", "fisheye", None),
-          ("fisheye_k", "fisheye", COLMAP_LIKE_FISHEYE_K))
+# label, camera_model, radial_coeffs, tangential_coeffs
+MODELS = (("pinhole", "pinhole", None, None), ("ortho", "ortho", None, None), ("fisheye", "fisheye", None, None),
+          ("fisheye_k", "fisheye", COLMAP_LIKE_FISHEYE_K, None), ("opencv", "opencv", None, None),
+          ("opencv_k", "opencv") + COLMAP_LIKE_OPENCV)
 
 
 def card():
@@ -57,16 +60,16 @@ def main():
     T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)  # noqa: E731
     dl = T(upstream_gradient(W, H, 0) * (3.0 * W * H))
     steps, patches = {}, {}
-    for label, model, k in MODELS:
-        sc = camera_model_scene(N, W, H, model, k, sh_dim=SH, seed=0)
+    for label, model, k, p in MODELS:
+        sc = camera_model_scene(N, W, H, model, k, sh_dim=SH, seed=0, tangential_coeffs=p)
         cam = Camera(W, H, sc["fx"], sc["fy"], sc["cx"], sc["cy"], T(sc["Rcw"]), T(sc["tcw"]), T(sc["twc"]),
-                     camera_model=model, radial_coeffs=k)
+                     camera_model=model, radial_coeffs=k, tangential_coeffs=p)
         leaves = [T(sc[n]).requires_grad_() for n in ("pws", "shs")] + [T(sc["alphas"][:, None]).requires_grad_()] + \
                  [T(sc[n]).requires_grad_() for n in ("scales", "rots")] + \
                  [torch.zeros((N, 2), device=dev, requires_grad=True)]
         with torch.no_grad():
             pre = ops.preprocess(leaves[0], leaves[4], leaves[3], leaves[1], cam.Rcw, cam.tcw, cam.twc, cam.fx, cam.fy,
-                                 cam.cx, cam.cy, W, H, camera_model=model, radial_coeffs=k)
+                                 cam.cx, cam.cy, W, H, camera_model=model, radial_coeffs=k, tangential_coeffs=p)
             patches[label] = int(ops.splat(H, W, pre[0], pre[1], leaves[2], pre[3], pre[2], pre[4])[4].numel())
 
         def fn(leaves=leaves, cam=cam):
@@ -119,6 +122,7 @@ def main():
     out = {
         "gpu": gpu, "power_limit_w": power, "config": "N=%d %dx%d SH degree 3" % (N, W, H),
         "rounds": args.rounds, "steps_per_round": args.steps, "fisheye_k": list(COLMAP_LIKE_FISHEYE_K),
+        "opencv_k": list(COLMAP_LIKE_OPENCV[0] + COLMAP_LIKE_OPENCV[1]),
         "P": patches,
         "ms": {lb: {k: round(float(np.median(v)), 4) for k, v in d.items()} for lb, d in res.items()},
         "spread_ms": {lb: {k: round(float(np.max(v) - np.min(v)), 4) for k, v in d.items()} for lb, d in res.items()},

@@ -173,25 +173,69 @@ static int arg_error(const char *who, const char *err) {
   return set_arg_error(msg);
 }
 
-// ---- camera models (DESIGN 3.14).  NULL or PINHOLE passes no CamLens: the kernels of the
-// entry points without a model.
-static int camera_lens(const char *who, const gsb_camera_model *cm, float fx, float fy, CamLens &out,
-                       const CamLens *&lens) {
-  lens = nullptr;
+// OPENCV's clamp stretch c = r_u / r_d (DESIGN 3.19): r_d is the largest normalised distorted radius
+// |((u - cx) / fx, (v - cy) / fy)| of the four image corners, r_u solves r (1 + k1 r^2 + k2 r^4) = r_d
+// on [0, sqrt(rho_valid)) by bisection (sqrt(rho_valid) when r_d lies beyond the curve's maximum).
+// Exactly 1 without radial terms; the tangential ones are left to the 1.3 margin.
+static float opencv_stretch(const float k[4], float fx, float fy, float cx, float cy, float width, float height) {
+  const double k1 = k[0], k2 = k[1];
+  if (k1 == 0.0 && k2 == 0.0) return 1.f;
+  double rd = 0.0;
+  for (double u : {0.0, (double)width})
+    for (double v : {0.0, (double)height}) rd = std::fmax(rd, std::hypot((u - cx) / fx, (v - cy) / fy));
+  if (!(rd > 0.0)) return 1.f;
+  const auto dist = [&](double r) { const double r2 = r * r; return r * (1.0 + r2 * (k1 + r2 * k2)); };
+  // rho_valid: the smallest positive root of 1 + 3 k1 rho + 5 k2 rho^2
+  double rv = INFINITY;
+  if (k2 == 0.0) {
+    if (k1 < 0.0) rv = -1.0 / (3.0 * k1);
+  } else {
+    const double b = 3.0 * k1, a = 5.0 * k2, disc = b * b - 4.0 * a;
+    if (disc >= 0.0) {
+      const double q = -0.5 * (b + std::copysign(std::sqrt(disc), b));
+      for (double r : {q / a, 1.0 / q})
+        if (r > 0.0) rv = std::fmin(rv, r);
+    }
+  }
+  double lo = 0.0, hi;
+  if (std::isfinite(rv)) {
+    hi = std::sqrt(rv);
+    if (dist(hi) <= rd) return (float)(hi / rd);
+  } else {
+    hi = rd;
+    while (dist(hi) < rd) hi *= 2.0;
+  }
+  for (int it = 0; it < 200 && hi - lo > 1e-15 * hi; it++) {
+    const double m = 0.5 * (lo + hi);
+    (dist(m) < rd ? lo : hi) = m;
+  }
+  return (float)(0.5 * (lo + hi) / rd);
+}
+
+// ---- camera models (DESIGN 3.14, 3.19).  NULL or PINHOLE passes no CamLens: the kernels of the
+// entry points without a model.  Sets sc.lens.
+static int camera_lens(const char *who, const gsb_camera_model *cm, FusedScene &sc, CamLens &out) {
+  sc.lens = nullptr;
   if (cm == nullptr) return 0;
   const bool fin = std::isfinite(cm->k[0]) && std::isfinite(cm->k[1]) && std::isfinite(cm->k[2]) &&
                    std::isfinite(cm->k[3]);
   const bool k0 = cm->k[0] == 0.f && cm->k[1] == 0.f && cm->k[2] == 0.f && cm->k[3] == 0.f;
-  if (cm->model != GSB_CAMERA_PINHOLE && cm->model != GSB_CAMERA_ORTHO && cm->model != GSB_CAMERA_FISHEYE)
+  if (cm->model != GSB_CAMERA_PINHOLE && cm->model != GSB_CAMERA_ORTHO && cm->model != GSB_CAMERA_FISHEYE &&
+      cm->model != GSB_CAMERA_OPENCV)
     return arg_error(who, "unknown camera model");
   if (!fin) return arg_error(who, "non-finite radial coefficient");
-  if (cm->model != GSB_CAMERA_FISHEYE && !k0)
-    return arg_error(who, "radial coefficients are for the fisheye model only");
-  if (cm->model != GSB_CAMERA_PINHOLE && !(fx > 0.f && fy > 0.f)) return arg_error(who, "fx and fy must be > 0");
+  if (cm->model != GSB_CAMERA_FISHEYE && cm->model != GSB_CAMERA_OPENCV && !k0)
+    return arg_error(who, "radial coefficients are for the fisheye and opencv models only");
+  if (cm->model != GSB_CAMERA_PINHOLE && !(sc.fx > 0.f && sc.fy > 0.f)) return arg_error(who, "fx and fy must be > 0");
+  if (cm->model == GSB_CAMERA_OPENCV && !(sc.width > 0.f && sc.height > 0.f))
+    return arg_error(who, "the opencv model needs width and height > 0");
   if (cm->model == GSB_CAMERA_PINHOLE) return 0;
   out.model = cm->model;
   for (int i = 0; i < 4; i++) out.k[i] = cm->k[i];
-  lens = &out;
+  out.stretch = cm->model == GSB_CAMERA_OPENCV
+                    ? opencv_stretch(out.k, sc.fx, sc.fy, sc.cx, sc.cy, sc.width, sc.height)
+                    : 1.f;
+  sc.lens = &out;
   return 0;
 }
 
@@ -200,7 +244,7 @@ static int camera_lens(const char *who, const gsb_camera_model *cm, float fx, fl
 static int preprocess_forward(const char *who, bool antialiased, const gsb_camera_model *camera_model, FusedScene sc,
                               const FusedFwd &f, gsb_stream_t stream) {
   CamLens cl;
-  if (int rc = camera_lens(who, camera_model, sc.fx, sc.fy, cl, sc.lens)) return rc;
+  if (int rc = camera_lens(who, camera_model, sc, cl)) return rc;
   if (sc.N < 0) return arg_error(who, "N < 0");
   if (!antialiased && (f.alphas == nullptr) != (f.recs == nullptr))
     return arg_error(who, "alphas and records go together");
@@ -284,7 +328,7 @@ static int preprocess_backward(const char *who, unsigned needs, const char *need
                                const gsb_camera_model *camera_model, FusedScene sc, FusedBwd b, float *dloss_dcamera,
                                void *ws, size_t ws_bytes, gsb_stream_t stream) {
   CamLens cl;
-  if (int rc = camera_lens(who, camera_model, sc.fx, sc.fy, cl, sc.lens)) return rc;
+  if (int rc = camera_lens(who, camera_model, sc, cl)) return rc;
   const int N = sc.N;
   if ((needs & kNeedDepths) && N > 0 && b.g_depths == nullptr) return arg_error(who, "null dloss_ddepths");
   const bool pose = dloss_dcamera != nullptr;

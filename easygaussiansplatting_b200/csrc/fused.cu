@@ -47,7 +47,7 @@ __device__ __forceinline__ void load_small_rows(const float *__restrict__ pws, c
 // AA = antialiasing (pg::aa_scale): alphas is read, alpha_eff = rho alpha goes to alphas_eff[N]
 // and into the record's alpha word (so its culling threshold follows); every other output is the
 // non-AA kernel's.
-// MODEL = pg::CamModel; lk = FISHEYE's k1..k4 (unread by the other models)
+// MODEL = pg::CamModel; lk = FISHEYE's k1..k4 or OPENCV's k1, k2, p1, p2 (unread by the other models)
 template <int K3, bool AA, int MODEL>
 __global__ void __launch_bounds__(PG) k_preprocess_fwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
@@ -64,7 +64,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
   const int nv = min(PG, (int)(N - base));
   const bool valid = tid < nv;
   pg::Cam cam = load_cam(Rcw, tcw, twc, fx, fy, cx, cy, tan_fovx, tan_fovy);
-  if (MODEL == pg::FISHEYE) { cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w; }
+  if (MODEL == pg::FISHEYE || MODEL == pg::OPENCV) { cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w; }
   float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
   // The 10 floats of position / scale / rotation go straight from global memory to registers
   // (a warp's strided loads use every byte of the sectors they touch; L1 serves the repeats) and
@@ -117,7 +117,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
 // AA = antialiasing (only with MOM, not with PUSH): the moment rows' dL/dalpha is dL/dalpha_eff of
 // the forward's alpha_eff = rho alpha; alphas (raw, 4 B/Gaussian) is read, dL/dalpha = rho m[5]
 // is written and alpha m[5] drho feeds the geometry (and camera) gradients (pg::backward_one).
-// MODEL, lk: as for k_preprocess_fwd (ORTHO and FISHEYE only with MOM, not with PUSH).
+// MODEL, lk: as for k_preprocess_fwd (ORTHO, FISHEYE and OPENCV only with MOM, not with PUSH).
 template <int K3, bool PUSH, bool MOM, bool DEPTH, bool POSE, bool AA, int MODEL>
 __global__ void __launch_bounds__(PG) k_preprocess_bwd(
     int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   const int nv = min(PG, (int)(N - base));
   const bool valid = tid < nv;
   pg::Cam cam = load_cam(Rcw, tcw, twc, fx, fy, cx, cy, tan_fovx, tan_fovy);
-  if (MODEL == pg::FISHEYE) { cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w; }
+  if (MODEL == pg::FISHEYE || MODEL == pg::OPENCV) { cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w; }
   float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
   float gu[2] = {0.f, 0.f}, gci[3] = {0.f, 0.f, 0.f}, gcol[3] = {0.f, 0.f, 0.f};
   load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);  // see k_preprocess_fwd
@@ -367,6 +367,7 @@ static auto with_model(const CamLens *lens, const char *unknown, F &&f) {
     case pg::PINHOLE: return f(std::integral_constant<int, pg::PINHOLE>{});
     case pg::ORTHO: return f(std::integral_constant<int, pg::ORTHO>{});
     case pg::FISHEYE: return f(std::integral_constant<int, pg::FISHEYE>{});
+    case pg::OPENCV: return f(std::integral_constant<int, pg::OPENCV>{});
     default: return set_arg_error(unknown);
   }
 }
@@ -374,11 +375,17 @@ static auto with_model(const CamLens *lens, const char *unknown, F &&f) {
 static float4 lens_k(const CamLens *lens) {
   return lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
 }
+// the kernels' tan_fovx, tan_fovy: W / (2 fx), H / (2 fy), stretched by OPENCV's lens (exactly 1 otherwise)
+static float2 lens_tan_fov(const FusedScene &sc) {
+  const float c = sc.lens ? sc.lens->stretch : 1.f;
+  return make_float2(sc.width / (2 * sc.fx) * c, sc.height / (2 * sc.fy) * c);
+}
 
 int launch_preprocess_fwd(const FusedScene &sc, const FusedFwd &f, cudaStream_t st) {
   const int N = sc.N;
   if (N <= 0) return 0;
-  const float tfx = sc.width / (2 * sc.fx), tfy = sc.height / (2 * sc.fy);
+  const float2 tf = lens_tan_fov(sc);
+  const float tfx = tf.x, tfy = tf.y;
   const int nb = (N + PG - 1) / PG;
   const float4 lk = lens_k(sc.lens);
   ProfScope ps(K_PRE_FWD, st);
@@ -413,7 +420,8 @@ int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t 
   const int N = sc.N;
   const PoseOut *po = b.po;
   if (N <= 0 && po == nullptr) return 0;
-  const float tfx = sc.width / (2 * sc.fx), tfy = sc.height / (2 * sc.fy);
+  const float2 tf = lens_tan_fov(sc);
+  const float tfx = tf.x, tfy = tf.y;
   const int nb = N > 0 ? (N + PG - 1) / PG : 0;
   const bool moments = b.mi.moments != nullptr;
   const GradPush p = b.gp ? *b.gp : GradPush{};

@@ -47,15 +47,16 @@ int launch_inv_cov2d(int N, const float *cov2ds, float *depths, float *cinv2ds, 
 // ---- fused per-Gaussian path (fused.cu)
 // camera model of the fused per-Gaussian kernels (gsb_camera_model)
 struct CamLens {
-  int model;   // pg::CamModel
-  float k[4];  // FISHEYE's k1..k4
+  int model;      // pg::CamModel
+  float k[4];     // FISHEYE's k1..k4, OPENCV's k1, k2, p1, p2
+  float stretch;  // OPENCV: the clamp limits' factor r_u / r_d (DESIGN 3.19); 1 otherwise
 };
 // the Gaussians and the view: what every fused call is about
 struct FusedScene {
   int N, k3;  // k3 = shs.shape[1] / 3
   const float *pws, *rots, *scales, *shs, *Rcw, *tcw, *twc;
   float fx, fy, cx, cy, width, height;
-  // NULL or PINHOLE (the reference's projection), or ORTHO / FISHEYE with the fisheye's k1..k4
+  // NULL or PINHOLE (the reference's projection), or ORTHO / FISHEYE / OPENCV with their k
   // (pg_fused_math.h; the backward's non-pinhole forms take the moment rows and no exchange)
   const CamLens *lens;
 };

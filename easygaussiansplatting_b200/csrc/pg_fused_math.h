@@ -29,15 +29,17 @@
 namespace gsb {
 namespace pg {
 
-// Camera models (DESIGN 3.14).  PINHOLE is the reference's projection; ORTHO and FISHEYE
-// (Kannala-Brandt, COLMAP's OPENCV_FISHEYE) only change the mean u and the Jacobian J of the
-// EWA splat -- everything after cov2d is model-independent.
-enum CamModel : int { PINHOLE = 0, ORTHO = 1, FISHEYE = 2 };
+// Camera models (DESIGN 3.14, 3.19).  PINHOLE is the reference's projection; ORTHO, FISHEYE
+// (Kannala-Brandt, COLMAP's OPENCV_FISHEYE) and OPENCV (radial-tangential, COLMAP's OPENCV) only
+// change the mean u and the Jacobian J of the EWA splat -- everything after cov2d is
+// model-independent.  3 is unassigned (the C ABI's GSB_CAMERA_* keep it unknown).
+enum CamModel : int { PINHOLE = 0, ORTHO = 1, FISHEYE = 2, OPENCV = 4 };
 
 struct Cam {
   float R[9], t[3], twc[3];
   float fx, fy, cx, cy, tan_fovx, tan_fovy;
   float k[4];  // FISHEYE: theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8)
+               // OPENCV: k1, k2, p1, p2 (opencv_delta)
 };
 
 constexpr float kMinDepth = 0.2f;  // kernel.cu:10: (float)z < 0.2 (double)  <=>  z < 0.2f
@@ -126,19 +128,74 @@ GSB_HD void cov2d(const float pc[3], bool keep, const float S6[6], const float R
 constexpr float kFishSeries = 0.03f;
 
 struct Lens {
-  float J[6];           // du/dpc (2x3, row-major)
+  float J[6];           // du/dpc (2x3, row-major); OPENCV: the clamped J of cov2d
   float s, g, h;        // FISHEYE
   float G, H, hz;       // FISHEYE, backward only
+  float dlt[2];         // OPENCV: delta(xn, yn)
+  float Ju[6];          // OPENCV: du/dpc at the unclamped (xn, yn), backward only
 };
 
+// ---- OPENCV (COLMAP's OpenCVCameraModel), on (a, b) = (x, y) / z with rho = a^2 + b^2,
+// R = 1 + k1 rho + k2 rho^2, R' = dR/drho = k1 + 2 k2 rho:
+//   delta = (a R + 2 p1 a b + p2 (rho + 2 a^2),  b R + p1 (rho + 2 b^2) + 2 p2 a b),
+//   u = (fx delta_x(xn, yn) + cx, fy delta_y(xn, yn) + cy)                      (never clamped)
+//   J = diag(fx, fy) Ddelta(xh, yh) (1/z) [[1, 0, -xh], [0, 1, -yh]],  (xh, yh) = clamp((xn, yn), +-1.3 tan_fov)
+// Ddelta is symmetric:  D00 = R + 2 a^2 R' + 2 p1 b + 6 p2 a,  D01 = D10 = 2 a b R' + 2 p1 a + 2 p2 b,
+//   D11 = R + 2 b^2 R' + 6 p1 b + 2 p2 a.  The host stretches tan_fov by the lens (DESIGN 3.19).
+// A Gaussian is culled like z < 0.2 where rho >= rho_valid (the radial map r R(r^2) stops
+// increasing) or det Ddelta(xn, yn) <= 0: beyond either the polynomial folds back.
+GSB_HD void opencv_delta(float a, float b, const float k[4], float dlt[2]) {
+  const float rho = fmaf(a, a, b * b), R = fmaf(rho, fmaf(rho, k[1], k[0]), 1.f), ab = a * b;
+  dlt[0] = fmaf(a, R, fmaf(2.f * k[2], ab, k[3] * fmaf(2.f * a, a, rho)));
+  dlt[1] = fmaf(b, R, fmaf(k[2], fmaf(2.f * b, b, rho), 2.f * k[3] * ab));
+}
+
+// Ddelta at (a, b) as (D00, D01, D11)
+GSB_HD void opencv_D(float a, float b, const float k[4], float D[3]) {
+  const float rho = fmaf(a, a, b * b), R = fmaf(rho, fmaf(rho, k[1], k[0]), 1.f), R1 = fmaf(2.f * k[1], rho, k[0]);
+  D[0] = fmaf(2.f * a * a, R1, R) + fmaf(2.f * k[2], b, 6.f * k[3] * a);
+  D[1] = fmaf(2.f * a * b, R1, fmaf(2.f * k[2], a, 2.f * k[3] * b));
+  D[2] = fmaf(2.f * b * b, R1, R) + fmaf(6.f * k[2], b, 2.f * k[3] * a);
+}
+
+// rho_valid: the smallest positive root of d(r R)/dr = 1 + 3 k1 rho + 5 k2 rho^2, +inf if none
+GSB_HD float opencv_rho_valid(float k1, float k2) {
+  if (k2 == 0.f) return k1 < 0.f ? -1.f / (3.f * k1) : INFINITY;
+  const float b = 3.f * k1, a = 5.f * k2, disc = fmaf(b, b, -4.f * a);
+  if (disc < 0.f) return INFINITY;
+  const float q = -0.5f * (b + copysignf(sqrtf(disc), b));  // roots q / a and 1 / q, q != 0
+  const float r1 = q / a, r2 = 1.f / q;
+  return fminf(r1 > 0.f ? r1 : INFINITY, r2 > 0.f ? r2 : INFINITY);
+}
+
+// J = (1/z) diag(f) [[D0, D1, -(D0 a + D1 b)], [D1, D2, -(D1 a + D2 b)]] with D = Ddelta(a, b)
+GSB_HD void opencv_J(float a, float b, float zi, float fx, float fy, const float D[3], float J[6]) {
+  const float fxz = fx * zi, fyz = fy * zi;
+  J[0] = fxz * D[0]; J[1] = fxz * D[1]; J[2] = -fmaf(J[0], a, J[1] * b);
+  J[3] = fyz * D[1]; J[4] = fyz * D[2]; J[5] = -fmaf(J[3], a, J[4] * b);
+}
+
 // false when the Gaussian lies beyond the range where the fisheye's theta_d increases
-// (theta_d' <= 0): culled like z < 0.2.  A culled Gaussian (keep false) is evaluated at (0, 0, 1).
+// (theta_d' <= 0), or OPENCV's fold: culled like z < 0.2.  A culled Gaussian (keep false) is
+// evaluated at (0, 0, 1).
 template <int MODEL>
 GSB_HD bool lens(const float pc_in[3], bool keep, const Cam &cam, Lens &L) {
   if constexpr (MODEL == ORTHO) {
     L.J[0] = cam.fx; L.J[1] = 0.f; L.J[2] = 0.f;
     L.J[3] = 0.f; L.J[4] = cam.fy; L.J[5] = 0.f;
     return true;
+  } else if constexpr (MODEL == OPENCV) {
+    const float x = keep ? pc_in[0] : 0.f, y = keep ? pc_in[1] : 0.f, z = keep ? pc_in[2] : 1.f;
+    const float zi = 1.0f / z, xn = x * zi, yn = y * zi;
+    const float limx = 1.3f * cam.tan_fovx, limy = 1.3f * cam.tan_fovy;
+    const float xh = fminf(limx, fmaxf(-limx, xn)), yh = fminf(limy, fmaxf(-limy, yn));
+    opencv_delta(xn, yn, cam.k, L.dlt);
+    float Du[3], D[3];
+    opencv_D(xn, yn, cam.k, Du);
+    opencv_D(xh, yh, cam.k, D);
+    opencv_J(xn, yn, zi, cam.fx, cam.fy, Du, L.Ju);
+    opencv_J(xh, yh, zi, cam.fx, cam.fy, D, L.J);
+    return fmaf(xn, xn, yn * yn) < opencv_rho_valid(cam.k[0], cam.k[1]) && Du[0] * Du[2] - Du[1] * Du[1] > 0.f;
   } else {
     static_assert(MODEL == FISHEYE, "unknown camera model");
     const float x = keep ? pc_in[0] : 0.f, y = keep ? pc_in[1] : 0.f, z = keep ? pc_in[2] : 1.f;
@@ -177,19 +234,22 @@ GSB_HD bool lens(const float pc_in[3], bool keep, const Cam &cam, Lens &L) {
   }
 }
 
-// projected mean of a kept Gaussian under ORTHO / FISHEYE (PINHOLE: project_mean)
+// projected mean of a kept Gaussian under ORTHO / FISHEYE / OPENCV (PINHOLE: project_mean)
 template <int MODEL>
 GSB_HD void lens_mean(const float pc[3], const Cam &cam, const Lens &L, float u[2]) {
   if constexpr (MODEL == ORTHO) {
     u[0] = fmaf(cam.fx, pc[0], cam.cx);
     u[1] = fmaf(cam.fy, pc[1], cam.cy);
+  } else if constexpr (MODEL == OPENCV) {
+    u[0] = fmaf(cam.fx, L.dlt[0], cam.cx);
+    u[1] = fmaf(cam.fy, L.dlt[1], cam.cy);
   } else {
     u[0] = fmaf(cam.fx * L.s, pc[0], cam.cx);
     u[1] = fmaf(cam.fy * L.s, pc[1], cam.cy);
   }
 }
 
-// cov2d (Cov2d's M, MS, c2, raw; not xc, yc, zi) under ORTHO / FISHEYE: M = J Rcw with J = L.J
+// cov2d (Cov2d's M, MS, c2, raw; not xc, yc, zi) under ORTHO / FISHEYE / OPENCV: M = J Rcw with J = L.J
 GSB_HD void cov2d_lens(const Lens &L, const float S6[6], const float R[9], Cov2d &o) {
   for (int a = 0; a < 2; a++)
     for (int c = 0; c < 3; c++)
@@ -205,19 +265,51 @@ GSB_HD void cov2d_lens(const Lens &L, const float S6[6], const float R[9], Cov2d
   o.c2[2] = o.raw[1] + kBlur;
 }
 
-// dL/dpc of the cov2d term under FISHEYE: sum_ab dL/dJ_ab dJ_ab/dpc (ORTHO: J is constant)
+// dL/dpc of the cov2d term under FISHEYE / OPENCV: sum_ab dL/dJ_ab dJ_ab/dpc (ORTHO: J is constant)
+template <int MODEL>
 GSB_HD void lens_dJ_dpc(const float pc[3], const Cam &cam, const Lens &L, const float dJ[6], float gpc[3]) {
-  const float x = pc[0], y = pc[1], fx = cam.fx, fy = cam.fy;
-  const float g = L.g, G = L.G, h = L.h, H = L.H, xx = x * x, yy = y * y, xy = x * y;
-  // row 0: J00 = fx (s + x^2 g), J01 = fx x y g, J02 = -fx x h
-  const float a0 = dJ[0] * fx, a1 = dJ[1] * fx, a2 = dJ[2] * fx;
-  const float b0 = dJ[3] * fy, b1 = dJ[4] * fy, b2 = dJ[5] * fy;
-  gpc[0] = a0 * x * fmaf(xx, G, 3.f * g) + a1 * y * fmaf(xx, G, g) - a2 * fmaf(xx, H, h) +
-           b0 * y * fmaf(xx, G, g) + b1 * x * fmaf(yy, G, g) - b2 * xy * H;
-  gpc[1] = a0 * y * fmaf(xx, G, g) + a1 * x * fmaf(yy, G, g) - a2 * xy * H +
-           b0 * x * fmaf(yy, G, g) + b1 * y * fmaf(yy, G, 3.f * g) - b2 * fmaf(yy, H, h);
-  gpc[2] = -a0 * fmaf(xx, H, h) - a1 * xy * H - a2 * x * L.hz -
-           b0 * xy * H - b1 * fmaf(yy, H, h) - b2 * y * L.hz;
+  if constexpr (MODEL == OPENCV) {
+    // J = (1/z) K(xh, yh): 1/z carries dL/dz; a clamped coordinate has no derivative, an unclamped
+    // one dxh/dx = 1/z, dxh/dz = -xh/z.  dD/da = (6 a R' + 4 a^3 R'' + 6 p2, 2 b R' + 4 a^2 b R'' + 2 p1,
+    // 2 a R' + 4 a b^2 R'' + 2 p2), dD/db = (dD01/da, dD11/da, 6 b R' + 4 b^3 R'' + 6 p1), R'' = 2 k2.
+    const float *k = cam.k;
+    const float zi = 1.0f / pc[2], xn = pc[0] * zi, yn = pc[1] * zi;
+    const float limx = 1.3f * cam.tan_fovx, limy = 1.3f * cam.tan_fovy;
+    const float a = fminf(limx, fmaxf(-limx, xn)), b = fminf(limy, fmaxf(-limy, yn));
+    const float rho = fmaf(a, a, b * b), R1 = fmaf(2.f * k[1], rho, k[0]), R2 = 2.f * k[1];
+    float D[3];
+    opencv_D(a, b, k, D);
+    const float Da0 = fmaf(6.f * a, R1, fmaf(4.f * a * a * a, R2, 6.f * k[3]));
+    const float Da1 = fmaf(2.f * b, R1, fmaf(4.f * a * a * b, R2, 2.f * k[2]));
+    const float Da2 = fmaf(2.f * a, R1, fmaf(4.f * a * b * b, R2, 2.f * k[3]));
+    const float Db2 = fmaf(6.f * b, R1, fmaf(4.f * b * b * b, R2, 6.f * k[2]));
+    const float A0 = dJ[0] * cam.fx, A1 = dJ[1] * cam.fx, A2 = dJ[2] * cam.fx;
+    const float B0 = dJ[3] * cam.fy, B1 = dJ[4] * cam.fy, B2 = dJ[5] * cam.fy;
+    // dL/da, dL/db of K (row 0: [D0, D1, -(D0 a + D1 b)], row 1: [D1, D2, -(D1 a + D2 b)])
+    const float ga = A0 * Da0 + A1 * Da1 - A2 * fmaf(Da0, a, fmaf(Da1, b, D[0])) + B0 * Da1 + B1 * Da2 -
+                     B2 * fmaf(Da1, a, fmaf(Da2, b, D[1]));
+    const float gb = A0 * Da1 + A1 * Da2 - A2 * fmaf(Da1, a, fmaf(Da2, b, D[1])) + B0 * Da2 + B1 * Db2 -
+                     B2 * fmaf(Da2, a, fmaf(Db2, b, D[2]));
+    const float gK = A0 * D[0] + A1 * D[1] - A2 * fmaf(D[0], a, D[1] * b) + B0 * D[1] + B1 * D[2] -
+                     B2 * fmaf(D[1], a, D[2] * b);
+    const float gx = a == xn ? ga : 0.f, gy = b == yn ? gb : 0.f, zi2 = zi * zi;
+    gpc[0] = gx * zi2;
+    gpc[1] = gy * zi2;
+    gpc[2] = -(gK + fmaf(gx, a, gy * b)) * zi2;
+  } else {
+    static_assert(MODEL == FISHEYE, "dJ/dpc of a camera model without one");
+    const float x = pc[0], y = pc[1], fx = cam.fx, fy = cam.fy;
+    const float g = L.g, G = L.G, h = L.h, H = L.H, xx = x * x, yy = y * y, xy = x * y;
+    // row 0: J00 = fx (s + x^2 g), J01 = fx x y g, J02 = -fx x h
+    const float a0 = dJ[0] * fx, a1 = dJ[1] * fx, a2 = dJ[2] * fx;
+    const float b0 = dJ[3] * fy, b1 = dJ[4] * fy, b2 = dJ[5] * fy;
+    gpc[0] = a0 * x * fmaf(xx, G, 3.f * g) + a1 * y * fmaf(xx, G, g) - a2 * fmaf(xx, H, h) +
+             b0 * y * fmaf(xx, G, g) + b1 * x * fmaf(yy, G, g) - b2 * xy * H;
+    gpc[1] = a0 * y * fmaf(xx, G, g) + a1 * x * fmaf(yy, G, g) - a2 * xy * H +
+             b0 * x * fmaf(yy, G, g) + b1 * y * fmaf(yy, G, 3.f * g) - b2 * fmaf(yy, H, h);
+    gpc[2] = -a0 * fmaf(xx, H, h) - a1 * xy * H - a2 * x * L.hz -
+             b0 * xy * H - b1 * fmaf(yy, H, h) - b2 * y * L.hz;
+  }
 }
 
 // Antialiasing (2D-filter opacity compensation, Mip-Splatting; gsplat's rasterize_mode
@@ -307,8 +399,8 @@ struct Geo : Cov2d {
   float S6[6];        // cov3d upper triangle
   float di;           // 1 / det(cov2d)
   float cn[3];        // conic
-  bool keep;          // z >= 0.2 and 1/det not NaN (FISHEYE: and theta_d' > 0)
-  Lens L;             // ORTHO / FISHEYE only
+  bool keep;          // z >= 0.2 and 1/det not NaN (FISHEYE: and theta_d' > 0; OPENCV: unfolded)
+  Lens L;             // ORTHO / FISHEYE / OPENCV only
 };
 
 template <int MODEL = PINHOLE>
@@ -497,14 +589,15 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
     }
   } else {
     // ORTHO / FISHEYE: u has the exact Jacobian J (no clamp), and the cov2d term goes through dJ/dpc
-    // (0 for ORTHO, whose J is constant)
+    // (0 for ORTHO, whose J is constant).  OPENCV: u's Jacobian is the unclamped Ju, cov2d's the clamped J.
     const float *J = g.L.J;
-    if constexpr (MODEL == FISHEYE) {
-      lens_dJ_dpc(g.pc, cam, g.L, dJ, gpc);
+    if constexpr (MODEL == FISHEYE || MODEL == OPENCV) {
+      lens_dJ_dpc<MODEL>(g.pc, cam, g.L, dJ, gpc);
     } else {
       gpc[0] = gpc[1] = gpc[2] = 0.f;
     }
-    for (int k = 0; k < 3; k++) gpc[k] = fmaf(gu[0], J[k], fmaf(gu[1], J[3 + k], gpc[k]));
+    const float *Ju = MODEL == OPENCV ? g.L.Ju : J;
+    for (int k = 0; k < 3; k++) gpc[k] = fmaf(gu[0], Ju[k], fmaf(gu[1], Ju[3 + k], gpc[k]));
     if (DEPTH) gpc[2] += gdepth;
     for (int j = 0; j < 3; j++) gpw[j] += gpc[0] * R[j] + gpc[1] * R[3 + j] + gpc[2] * R[6 + j];
     if (POSE) {

@@ -14,20 +14,25 @@ class Camera:
     extension, read by the fused classes, GraphedFusedStep and MultiViewStep): render with the
     2D-filter opacity compensation, alpha_eff = rho * alpha (ops.preprocess).
     camera_model (an extension, read by the same classes): "pinhole" (the reference's projection),
-    "ortho" (u = (fx x + cx, fy y + cy)) or "fisheye" (Kannala-Brandt, COLMAP's OPENCV_FISHEYE, with
-    radial_coeffs = (k1, k2, k3, k4); None = the equidistant lens).  The seven-operator GSFunction,
-    GradExchange and the 3D filter's camera table take pinhole cameras only."""
+    "ortho" (u = (fx x + cx, fy y + cy)), "fisheye" (Kannala-Brandt, COLMAP's OPENCV_FISHEYE, with
+    radial_coeffs = (k1, k2, k3, k4); None = the equidistant lens) or "opencv" (radial-tangential,
+    COLMAP's OPENCV / RADIAL / SIMPLE_RADIAL, with radial_coeffs = (k1, k2) and tangential_coeffs =
+    (p1, p2); None = 0).  `colmap_intrinsics` maps COLMAP's camera records onto these fields.  The
+    seven-operator GSFunction, GradExchange, the surfel classes, the 3D filter's camera table and
+    TSDF fusion take pinhole cameras only."""
 
     def __init__(self, width, height, fx, fy, cx, cy, Rcw, tcw, twc=None, antialiased=False, camera_model="pinhole",
-                 radial_coeffs=None):
+                 radial_coeffs=None, tangential_coeffs=None):
         from .ops import camera_model_args
         self.width, self.height = int(width), int(height)
         self.fx, self.fy, self.cx, self.cy = float(fx), float(fy), float(cx), float(cy)
         self.Rcw, self.tcw = Rcw, tcw
         self.twc = twc if twc is not None else -torch.linalg.inv(Rcw) @ tcw
         self.antialiased = bool(antialiased)
-        self.camera_model, k = camera_model_args(camera_model, radial_coeffs)
-        self.radial_coeffs = k if radial_coeffs is not None else None
+        self.camera_model, k = camera_model_args(camera_model, radial_coeffs, tangential_coeffs)
+        nk = 2 if self.camera_model == "opencv" else 4
+        self.radial_coeffs = k[:nk] if radial_coeffs is not None else None
+        self.tangential_coeffs = k[2:] if tangential_coeffs is not None else None
         if self.camera_model != "pinhole" and not (self.fx > 0 and self.fy > 0):
             raise ValueError("camera_model=%r needs fx, fy > 0" % self.camera_model)
 
@@ -35,7 +40,51 @@ class Camera:
 def camera_model_kwargs(cam):
     """ops.preprocess / preprocessB keywords of a camera; one without the fields (the reference's
     dataset Camera) is pinhole"""
-    return dict(camera_model=getattr(cam, "camera_model", "pinhole"), radial_coeffs=getattr(cam, "radial_coeffs", None))
+    return dict(camera_model=getattr(cam, "camera_model", "pinhole"), radial_coeffs=getattr(cam, "radial_coeffs", None),
+                tangential_coeffs=getattr(cam, "tangential_coeffs", None))
+
+
+# COLMAP camera model -> (number of params, camera_model); params as in COLMAP's cameras.txt / .bin
+_COLMAP_MODELS = {"SIMPLE_PINHOLE": (3, "pinhole"), "PINHOLE": (4, "pinhole"), "SIMPLE_RADIAL": (4, "opencv"),
+                  "RADIAL": (5, "opencv"), "OPENCV": (8, "opencv"), "OPENCV_FISHEYE": (8, "fisheye")}
+
+
+def colmap_intrinsics(model_name, params, width, height, image_width=None, image_height=None):
+    """The `Camera` fields of a COLMAP camera record -> dict(fx, fy, cx, cy, camera_model, radial_coeffs,
+    tangential_coeffs), for images resized from (width, height) to (image_width, image_height) (default:
+    not resized).  Focal lengths and the principal point scale with the image; distortion coefficients
+    are in normalised coordinates and do not.
+      SIMPLE_PINHOLE f, cx, cy            -> pinhole
+      PINHOLE        fx, fy, cx, cy       -> pinhole
+      SIMPLE_RADIAL  f, cx, cy, k         -> opencv, radial (k, 0)
+      RADIAL         f, cx, cy, k1, k2    -> opencv, radial (k1, k2)
+      OPENCV         fx, fy, cx, cy, k1, k2, p1, p2 -> opencv
+      OPENCV_FISHEYE fx, fy, cx, cy, k1, k2, k3, k4 -> fisheye
+    Any other model, or a wrong number of params, is a ValueError.  Reads no files."""
+    if model_name not in _COLMAP_MODELS:
+        raise ValueError("COLMAP camera model %r is not supported (one of %s)" % (model_name, tuple(_COLMAP_MODELS)))
+    n, camera_model = _COLMAP_MODELS[model_name]
+    p = [float(v) for v in params]
+    if len(p) != n:
+        raise ValueError("COLMAP camera model %s takes %d params, got %d" % (model_name, n, len(p)))
+    if model_name in ("SIMPLE_PINHOLE", "SIMPLE_RADIAL", "RADIAL"):
+        fx = fy = p[0]
+        cx, cy, rest = p[1], p[2], p[3:]
+    else:
+        fx, fy, cx, cy, rest = p[0], p[1], p[2], p[3], p[4:]
+    sx = 1.0 if image_width is None else float(image_width) / float(width)
+    sy = 1.0 if image_height is None else float(image_height) / float(height)
+    radial = tangential = None
+    if model_name == "SIMPLE_RADIAL":
+        radial = (rest[0], 0.0)
+    elif model_name == "RADIAL":
+        radial = tuple(rest)
+    elif model_name == "OPENCV":
+        radial, tangential = tuple(rest[:2]), tuple(rest[2:])
+    elif model_name == "OPENCV_FISHEYE":
+        radial = tuple(rest)
+    return dict(fx=fx * sx, fy=fy * sy, cx=cx * sx, cy=cy * sy, camera_model=camera_model, radial_coeffs=radial,
+                tangential_coeffs=tangential)
 
 
 def _pinhole_only(cam, what):

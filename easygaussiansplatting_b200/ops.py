@@ -684,41 +684,56 @@ def splat_stats(height, width, contrib, patch_range_per_tile, gsid_per_patch, re
 
 # ---------------------------------------------------------------------------------------
 # Extensions (not in the reference module): the fused per-Gaussian path, SURVEY 8f row N1.
-CAMERA_MODELS = ("pinhole", "ortho", "fisheye")  # GSB_CAMERA_PINHOLE, _ORTHO, _FISHEYE
+CAMERA_MODELS = ("pinhole", "ortho", "fisheye", "opencv")
+# GSB_CAMERA_*: 3 is not a model (gsplat_b200.h)
+_CAMERA_MODEL_ID = {"pinhole": 0, "ortho": 1, "fisheye": 2, "opencv": 4}
 
 
 class _CameraModel(C.Structure):
     _fields_ = [("model", C.c_int32), ("k", C.c_float * 4)]
 
 
-def camera_model_args(camera_model="pinhole", radial_coeffs=None):
-    """Checks a camera model on the host -> (name, (k1, k2, k3, k4) as floats).  camera_model is
-    "pinhole", "ortho" or "fisheye"; radial_coeffs (k1..k4 of the Kannala-Brandt lens, COLMAP's
-    OPENCV_FISHEYE; None = all 0) is accepted only with "fisheye" and must be finite."""
+def _finite(coeffs, n, what):
+    k = tuple(float(x) for x in coeffs)
+    if len(k) != n or not all(math.isfinite(x) for x in k):
+        raise ValueError("%s must be %d finite numbers %s" % (what[0], n, what[1]))
+    return k
+
+
+def camera_model_args(camera_model="pinhole", radial_coeffs=None, tangential_coeffs=None):
+    """Checks a camera model on the host -> (name, the four coefficients of gsb_camera_model.k as
+    floats).  camera_model is "pinhole", "ortho", "fisheye" or "opencv"; None coefficients are 0.
+    fisheye: radial_coeffs = (k1, k2, k3, k4) of the Kannala-Brandt lens (COLMAP's OPENCV_FISHEYE).
+    opencv: radial_coeffs = (k1, k2) and tangential_coeffs = (p1, p2) of COLMAP's OPENCV model
+    (RADIAL: p = 0; SIMPLE_RADIAL: k2 = p = 0); k = (k1, k2, p1, p2).  All must be finite."""
     if camera_model not in CAMERA_MODELS:
         raise ValueError("camera_model must be one of %s, got %r" % (CAMERA_MODELS, camera_model))
+    if radial_coeffs is not None and camera_model not in ("fisheye", "opencv"):
+        raise ValueError("radial_coeffs are for camera_model='fisheye' or 'opencv' only")
+    if tangential_coeffs is not None and camera_model != "opencv":
+        raise ValueError("tangential_coeffs are for camera_model='opencv' only")
+    if camera_model == "opencv":
+        k = (0.0, 0.0) if radial_coeffs is None else _finite(radial_coeffs, 2, ("radial_coeffs", "(k1, k2)"))
+        p = (0.0, 0.0) if tangential_coeffs is None else _finite(tangential_coeffs, 2,
+                                                                ("tangential_coeffs", "(p1, p2)"))
+        return camera_model, k + p
     if radial_coeffs is None:
         return camera_model, (0.0, 0.0, 0.0, 0.0)
-    if camera_model != "fisheye":
-        raise ValueError("radial_coeffs are for camera_model='fisheye' only")
-    k = tuple(float(x) for x in radial_coeffs)
-    if len(k) != 4 or not all(math.isfinite(x) for x in k):
-        raise ValueError("radial_coeffs must be four finite numbers (k1, k2, k3, k4)")
-    return camera_model, k
+    return camera_model, _finite(radial_coeffs, 4, ("radial_coeffs", "(k1, k2, k3, k4)"))
 
 
-def _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y):
+def _camera_model_ptr(camera_model, radial_coeffs, tangential_coeffs, focal_x, focal_y):
     """-> None for pinhole (today's entry points), else the gsb_camera_model to pass by pointer"""
-    name, k = camera_model_args(camera_model, radial_coeffs)
+    name, k = camera_model_args(camera_model, radial_coeffs, tangential_coeffs)
     if name == "pinhole":
         return None
     if not (float(focal_x) > 0 and float(focal_y) > 0):
         raise ValueError("camera_model=%r needs focal_x, focal_y > 0" % name)
-    return C.pointer(_CameraModel(CAMERA_MODELS.index(name), (C.c_float * 4)(*k)))
+    return C.pointer(_CameraModel(_CAMERA_MODEL_ID[name], (C.c_float * 4)(*k)))
 
 
 def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
-               alphas=None, antialiased=False, camera_model="pinhole", radial_coeffs=None):
+               alphas=None, antialiased=False, camera_model="pinhole", radial_coeffs=None, tangential_coeffs=None):
     """project + computeCov3D + computeCov2D + sh2Color + inverseCov2D (calc_J=False) in one
     kernel.  -> [us[N,2], cinv2ds[N,3], colors[N,3], depths[N], areas[N,2] int32], ready for
     `splat`.  With alphas[N] a sixth output: the packed per-Gaussian records [N,12] for
@@ -726,10 +741,11 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
     antialiased (alphas required): a seventh output alphas_eff[N] = rho * alphas, the opacity
     scaled by how much the 0.3 px blur spread each Gaussian (gsb_preprocess_forward_aa); the records
     carry it.  Render with alphas_eff; the other outputs are the same bits as without.
-    camera_model ("pinhole", "ortho" or "fisheye") and radial_coeffs (fisheye's k1..k4): the
-    projection (gsb_preprocess_forward_model; pinhole runs the calls above).  width/height feed
-    only pinhole's fov clamp."""
-    cm = _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y)
+    camera_model ("pinhole", "ortho", "fisheye" or "opencv"), radial_coeffs (fisheye's k1..k4,
+    opencv's k1, k2) and tangential_coeffs (opencv's p1, p2): the projection
+    (gsb_preprocess_forward_model; pinhole runs the calls above; `camera_model_args`).
+    width/height feed only pinhole's and opencv's clamp of the EWA Jacobian."""
+    cm = _camera_model_ptr(camera_model, radial_coeffs, tangential_coeffs, focal_x, focal_y)
     params, N, k = _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc)
     pws = params[0]
     if antialiased and alphas is None:
@@ -760,7 +776,7 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
 def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
                 dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False,
                 dloss_ddepths=None, camera_grad=False, pose_only=False, antialiased=False, alphas=None,
-                camera_model="pinhole", radial_coeffs=None):
+                camera_model="pinhole", radial_coeffs=None, tangential_coeffs=None):
     """Vector-Jacobian products of the five per-Gaussian stages (== the torch.bmm chain of
     gsmodel.py:72-85).  -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4]]
     With moments[N,9] (from `splatB(..., moments_only=True)`) and the forward's cinv2ds[N,3] the
@@ -781,9 +797,9 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     dloss_dalphas = rho * dL/dalphas_eff and the geometry (and camera) gradients gain the term
     through rho (gsb_preprocess_backward_aa).  Combines with compact, dloss_ddepths, camera_grad
     and pose_only.
-    camera_model, radial_coeffs: as for `preprocess` (gsb_preprocess_backward_model); a model other
-    than pinhole needs the moment rows and combines with everything above."""
-    cm = _camera_model_ptr(camera_model, radial_coeffs, focal_x, focal_y)
+    camera_model, radial_coeffs, tangential_coeffs: as for `preprocess` (gsb_preprocess_backward_model);
+    a model other than pinhole needs the moment rows and combines with everything above."""
+    cm = _camera_model_ptr(camera_model, radial_coeffs, tangential_coeffs, focal_x, focal_y)
     if cm is not None and moments is None:
         raise ValueError("camera_model=%r needs the moment rows" % camera_model)
     if pose_only and not camera_grad:

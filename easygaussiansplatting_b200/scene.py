@@ -58,18 +58,70 @@ def ring_camera(k, n_views, radius=0.6):
 
 
 COLMAP_LIKE_FISHEYE_K = (0.05, -0.01, 0.002, -0.0005)  # k1..k4 of a typical OPENCV_FISHEYE calibration
+# (k1, k2), (p1, p2) of a typical OPENCV calibration of a moderately wide lens
+COLMAP_LIKE_OPENCV = ((-0.12, 0.03), (4e-4, -6e-4))
 
 
-def camera_model_scene(N, width, height, camera_model="pinhole", radial_coeffs=None, sh_dim=48, seed=0):
+def opencv_undistort(mx, my, k, iters=20):
+    """(xn, yn) with delta(xn, yn) = (mx, my) for the opencv lens k = (k1, k2, p1, p2) (ops.preprocess).
+    The radial part is solved first by bisection on [0, r_max), where r (1 + k1 r^2 + k2 r^4) increases;
+    Newton steps on delta then add the tangential part.  A target beyond the radial curve's maximum
+    lands at 1.02 r_max on its ray: past the fold, where the kernels cull."""
+    k1, k2, p1, p2 = (float(v) for v in k)
+    mx, my = np.asarray(mx, np.float64), np.asarray(my, np.float64)
+    rd = np.hypot(mx, my)
+    # r_max^2: the smallest positive root of 1 + 3 k1 rho + 5 k2 rho^2
+    roots = np.roots([5 * k2, 3 * k1, 1.0]) if k2 != 0 else ([-1 / (3 * k1)] if k1 != 0 else [])
+    pos = [r.real for r in np.atleast_1d(roots) if abs(np.imag(r)) < 1e-12 and r.real > 0]
+    rmax = math.sqrt(min(pos)) if pos else math.inf
+    dist = lambda r: r * (1 + r * r * (k1 + r * r * k2))
+    lo = np.zeros_like(rd)
+    if math.isfinite(rmax):
+        hi = np.full_like(rd, rmax)
+        beyond = dist(hi) < rd
+    else:
+        hi = np.maximum(2 * rd, 1.0)
+        while (dist(hi) < rd).any():
+            hi = np.where(dist(hi) < rd, 2 * hi, hi)
+        beyond = np.zeros(rd.shape, bool)
+    for _ in range(80):
+        m = 0.5 * (lo + hi)
+        below = dist(m) < rd
+        lo, hi = np.where(below, m, lo), np.where(below, hi, m)
+    ru = np.where(beyond, 1.02 * rmax if math.isfinite(rmax) else 0.0, 0.5 * (lo + hi))
+    with np.errstate(invalid="ignore", divide="ignore"):
+        s = np.where(rd > 0, ru / rd, 1.0)
+    x, y = mx * s, my * s
+    for _ in range(iters):
+        rho = x * x + y * y
+        R, R1 = 1 + rho * (k1 + rho * k2), k1 + 2 * k2 * rho
+        ex = x * R + 2 * p1 * x * y + p2 * (rho + 2 * x * x) - mx
+        ey = y * R + p1 * (rho + 2 * y * y) + 2 * p2 * x * y - my
+        d00 = R + 2 * x * x * R1 + 2 * p1 * y + 6 * p2 * x
+        d01 = 2 * x * y * R1 + 2 * p1 * x + 2 * p2 * y
+        d11 = R + 2 * y * y * R1 + 6 * p1 * y + 2 * p2 * x
+        det = d00 * d11 - d01 * d01
+        with np.errstate(invalid="ignore", divide="ignore"):
+            nx, ny = x - (d11 * ex - d01 * ey) / det, y - (d00 * ey - d01 * ex) / det
+        x, y = np.where(beyond, x, nx), np.where(beyond, y, ny)
+    return x, y
+
+
+def camera_model_scene(N, width, height, camera_model="pinhole", radial_coeffs=None, sh_dim=48, seed=0,
+                       tangential_coeffs=None):
     """synthetic_scene with its target pixels unprojected through a camera model instead of the pinhole,
     so that scenes of different models cover the frame alike.  pinhole: synthetic_scene itself.
     ortho: fx = fy = W / 16 (16 world units across); pw = ((u - cx) / fx, (v - cy) / fy, z).
     fisheye (Kannala-Brandt k1..k4 = radial_coeffs, default 0): fx = fy = W / pi, 180 degrees across the
     width; the pixel's ray (theta_d -> theta by Newton) at distance z.  Targets beyond theta = 90 degrees (the
-    corners) land behind the camera and are culled.  Scales: the pixel sigma times the metres per pixel at
-    the Gaussian (z / fx; 1 / fx for ortho).  -> the dict of synthetic_scene plus camera_model, radial_coeffs"""
+    corners) land behind the camera and are culled.
+    opencv (k1, k2 = radial_coeffs, p1, p2 = tangential_coeffs, default 0): synthetic_scene's fx, fy;
+    the pixel's undistorted point (`opencv_undistort`) at depth z.
+    Scales: the pixel sigma times the metres per pixel at the Gaussian (z / fx; 1 / fx for ortho).
+    -> the dict of synthetic_scene plus camera_model, radial_coeffs, tangential_coeffs"""
     sc = synthetic_scene(N, width, height, sh_dim=sh_dim, seed=seed)
     sc["camera_model"], sc["radial_coeffs"] = camera_model, radial_coeffs
+    sc["tangential_coeffs"] = tangential_coeffs
     if camera_model == "pinhole":
         return sc
     rng = np.random.default_rng(seed)  # the same draws as synthetic_scene
@@ -95,6 +147,12 @@ def camera_model_scene(N, width, height, camera_model="pinhole", radial_coeffs=N
             th -= fth / (1 + t2 * (3 * k1 + t2 * (5 * k2 + t2 * (7 * k3 + t2 * 9 * k4))))
         phi = np.arctan2(my, mx)
         pws = np.stack([z * np.sin(th) * np.cos(phi), z * np.sin(th) * np.sin(phi), z * np.cos(th)], axis=1)
+        scales = sig * z[:, None] / f
+    elif camera_model == "opencv":
+        f = sc["fx"]
+        k = tuple(radial_coeffs or (0.0, 0.0)) + tuple(tangential_coeffs or (0.0, 0.0))
+        xn, yn = opencv_undistort((u - cx) / f, (v - cy) / f, k)
+        pws = np.stack([xn * z, yn * z, z], axis=1)
         scales = sig * z[:, None] / f
     else:
         raise ValueError("unknown camera model %r" % (camera_model,))

@@ -181,7 +181,7 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
                                const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
                                size_t ws_bytes, gsb_stream_t stream);
 
-/* Camera models (extension; gsplat's camera_model="pinhole" | "ortho" | "fisheye").  Only the
+/* Camera models (extension; gsplat's camera_model="pinhole" | "ortho" | "fisheye", and "opencv").  Only the
  * projected mean u and the Jacobian J of the EWA splat change; everything after cov2d (conic,
  * radius, records, the rasterizers) is the same.  Depth stays the camera-frame z, and every model
  * culls z < 0.2.
@@ -191,18 +191,29 @@ int gsb_preprocess_backward_aa(int N, int sh_dim3, const float *pws, const float
  *            theta = atan2(|(x, y)|, z),  theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6
  *            + k4 theta^8),  u = (fx theta_d x / r + cx, fy theta_d y / r + cy), J its exact
  *            Jacobian; no clamp.  A Gaussian where d theta_d / d theta <= 0 is culled like z < 0.2.
- * k must be 0 for the models other than FISHEYE; fx, fy > 0 for ORTHO and FISHEYE.
+ *   OPENCV   radial-tangential (COLMAP's OPENCV; RADIAL is p1 = p2 = 0, SIMPLE_RADIAL also k2 = 0 and
+ *            fx = fy), k = (k1, k2, p1, p2).  With (a, b) = (x/z, y/z), rho = a^2 + b^2 and
+ *            R = 1 + k1 rho + k2 rho^2:  u = (fx (a R + 2 p1 a b + p2 (rho + 2 a^2)) + cx,
+ *            fy (b R + p1 (rho + 2 b^2) + 2 p2 a b) + cy), never clamped.  J is the distortion's
+ *            Jacobian times pinhole's at (a, b) clamped to +-1.3 W / (2 fx) c, +-1.3 H / (2 fy) c, where
+ *            c is how far the radial terms move the image corners (1 when k1 = k2 = 0).  A Gaussian
+ *            beyond the first maximum of r (1 + k1 r^2 + k2 r^4), or where the distortion's Jacobian
+ *            has det <= 0, is culled like z < 0.2.  Needs width, height > 0.
+ * k must be 0 for PINHOLE and ORTHO and finite for all; fx, fy > 0 for every model but PINHOLE.
+ * The ids skip 3, which stays an unknown model: callers built against an earlier header that
+ * passed 3 as an invalid id still get an argument error.
  * gsb_preprocess_forward_model: gsb_preprocess_forward_aa's arguments with alphas_eff nullable
  * (NULL: no antialiasing, and then alphas and records go together as in gsb_preprocess_forward).
  * gsb_preprocess_backward_model: gsb_preprocess_backward_aa's arguments with alphas nullable (NULL:
  * no antialiasing) and the moment rows required.  A NULL camera_model, or PINHOLE, runs the
- * kernels the entry points above run.  width/height feed only PINHOLE's clamp. */
+ * kernels the entry points above run.  width/height feed only PINHOLE's and OPENCV's clamp. */
 #define GSB_CAMERA_PINHOLE 0
 #define GSB_CAMERA_ORTHO 1
 #define GSB_CAMERA_FISHEYE 2
+#define GSB_CAMERA_OPENCV 4
 typedef struct gsb_camera_model {
   int32_t model; /* GSB_CAMERA_* */
-  float k[4];    /* FISHEYE: k1..k4 */
+  float k[4];    /* FISHEYE: k1..k4;  OPENCV: k1, k2, p1, p2 */
 } gsb_camera_model;
 int gsb_preprocess_forward_model(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
                                  const float *shs, const float *Rcw, const float *tcw, const float *twc, float fx,
