@@ -42,6 +42,7 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
                                              "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
                                              "filter3d_apply", "filter3d_backward", "density_apply_rows",
+                                             "bilagrid_slice", "bilagrid_slice_backward", "bilagrid_tv",
                                              "draw_features", "draw_backward_features", "draw_stats",
                                              "draw_surfel_stats", "mcmc_scan",
                                              "mcmc_sample", "mcmc_relocate", "mcmc_grow", "mcmc_rows",
@@ -1551,6 +1552,67 @@ int gsb_tsdf_extract_emit(int nx, int ny, int nz, float ox, float oy, float oz, 
   const TsdfGrid g{nx, ny, nz, ox, oy, oz, voxel};
   return launch_tsdf_extract_emit(g, tsdf, weight, color_grid, ws, (int)n_verts, (int)n_faces, verts, vcolors, faces,
                                   (cudaStream_t)stream);
+}
+
+// ---- bilateral-grid colour correction (bilagrid.cu, DESIGN 3.20)
+static_assert(BILAGRID_MAX_DIM == GSB_BILAGRID_MAX_DIM && BILAGRID_MAX_BATCH == GSB_BILAGRID_MAX_BATCH,
+              "gsplat_b200.h and kernels.h disagree on the bilateral-grid limits");
+
+static int bilagrid_shape(int M, int L, int Y, int X, const char *who) {
+  if (M < 1) return arg_error(who, "M < 1");
+  if (L < 1 || Y < 1 || X < 1 || L > GSB_BILAGRID_MAX_DIM || Y > GSB_BILAGRID_MAX_DIM || X > GSB_BILAGRID_MAX_DIM)
+    return arg_error(who, "grid size out of [1, 64]");
+  return 0;
+}
+
+// the checks of the slice and its backward; 0 or the argument error "<who>: <reason>"
+static int bilagrid_slice_args(int M, int L, int Y, int X, const float *grids, int B, const int32_t *image_ids,
+                               int H, int W, std::initializer_list<const void *> images, const char *who) {
+  if (int rc = bilagrid_shape(M, L, Y, X, who)) return rc;
+  if (B < 1 || B > GSB_BILAGRID_MAX_BATCH) return arg_error(who, "batch out of [1, 64]");
+  if (H < 1 || W < 1) return arg_error(who, "bad H/W");
+  if ((int64_t)H * W >= ((int64_t)1 << 31)) return arg_error(who, "2^31 or more pixels");
+  if (image_ids == nullptr) return arg_error(who, "image_ids is null");
+  for (int b = 0; b < B; b++)
+    if (image_ids[b] < 0 || image_ids[b] >= M) return arg_error(who, "image id out of [0, M)");
+  if (grids == nullptr) return arg_error(who, "null pointer");
+  if (!aligned(grids, 4)) return arg_error(who, "misaligned array");
+  for (const void *p : images) {
+    if (p == nullptr) return arg_error(who, "null pointer");
+    if (!aligned(p, 4)) return arg_error(who, "misaligned array");
+  }
+  return 0;
+}
+
+int gsb_bilagrid_slice(int M, int L, int Y, int X, const float *grids, int B, const int32_t *image_ids, int H, int W,
+                       const float *rgb, float *out, gsb_stream_t stream) {
+  if (int rc = bilagrid_slice_args(M, L, Y, X, grids, B, image_ids, H, W, {rgb, out}, "bilagrid_slice")) return rc;
+  return launch_bilagrid_slice({M, L, Y, X}, grids, B, image_ids, H, W, rgb, out, (cudaStream_t)stream);
+}
+
+int gsb_bilagrid_slice_backward(int M, int L, int Y, int X, const float *grids, int B, const int32_t *image_ids,
+                                int H, int W, const float *rgb, const float *dloss_dout, float *dloss_drgb,
+                                float *dloss_dgrids, gsb_stream_t stream) {
+  if (int rc = bilagrid_slice_args(M, L, Y, X, grids, B, image_ids, H, W, {rgb, dloss_dout, dloss_drgb, dloss_dgrids},
+                                   "bilagrid_slice_backward"))
+    return rc;
+  return launch_bilagrid_slice_bwd({M, L, Y, X}, grids, B, image_ids, H, W, rgb, dloss_dout, dloss_drgb, dloss_dgrids,
+                                   (cudaStream_t)stream);
+}
+
+size_t gsb_bilagrid_tv_workspace_bytes(int M, int L, int Y, int X) {
+  if (bilagrid_shape(M, L, Y, X, "bilagrid_tv_workspace_bytes")) return 0;
+  return bilagrid_tv_workspace_bytes({M, L, Y, X});
+}
+
+int gsb_bilagrid_tv(int M, int L, int Y, int X, const float *grids, float *tv_out, float *dloss_dgrids, void *ws,
+                    size_t ws_bytes, gsb_stream_t stream) {
+  if (int rc = bilagrid_shape(M, L, Y, X, "bilagrid_tv")) return rc;
+  GSB_REQUIRE(grids && tv_out && ws, "bilagrid_tv: null pointer");
+  GSB_REQUIRE(aligned(grids, 4) && aligned(tv_out, 4) && aligned(dloss_dgrids, 4) && aligned(ws, 8),
+              "bilagrid_tv: misaligned array");
+  GSB_REQUIRE(ws_bytes >= bilagrid_tv_workspace_bytes({M, L, Y, X}), "bilagrid_tv: workspace too small");
+  return launch_bilagrid_tv({M, L, Y, X}, grids, tv_out, dloss_dgrids, ws, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -18,7 +18,7 @@ enum KernelId {
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
-  K_DENSITY_ROWS, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
+  K_DENSITY_ROWS, K_BILAGRID_SLICE, K_BILAGRID_SLICE_BWD, K_BILAGRID_TV, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
   K_MCMC_ROWS, K_MCMC_NOISE, K_TSDF_INTEGRATE, K_TSDF_PLAN, K_TSDF_EMIT,
   K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
   K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
@@ -365,5 +365,21 @@ int launch_tsdf_extract_plan(const TsdfGrid &g, const float *tsdf, const float *
 int launch_tsdf_extract_emit(const TsdfGrid &g, const float *tsdf, const float *weight, const float *color_grid,
                              const void *ws, int n_verts, int n_faces, float *verts, float *vcolors, int32_t *faces,
                              cudaStream_t st);
+
+// ---- bilateral-grid colour correction (bilagrid.cu, DESIGN 3.20).  grids[M, 12, L, Y, X]; the shape
+// and the ids are checked by the entry points.  rgb, out, dout, drgb: B planar [3, H, W] images; item
+// b reads grid ids[b].  The backward writes drgb and ADDS into dgrids.  The TV writes dgrids (when
+// not NULL) and the value to tv[0] through bilagrid_tv_workspace_bytes of per-CTA partial sums.
+constexpr int BILAGRID_MAX_DIM = 64, BILAGRID_MAX_BATCH = 64;
+struct BilagridShape {
+  int M, L, Y, X;
+};
+int launch_bilagrid_slice(const BilagridShape &s, const float *grids, int B, const int32_t *ids, int H, int W,
+                          const float *rgb, float *out, cudaStream_t st);
+int launch_bilagrid_slice_bwd(const BilagridShape &s, const float *grids, int B, const int32_t *ids, int H, int W,
+                              const float *rgb, const float *dout, float *drgb, float *dgrids, cudaStream_t st);
+size_t bilagrid_tv_workspace_bytes(const BilagridShape &s);
+int launch_bilagrid_tv(const BilagridShape &s, const float *grids, float *tv, float *dgrids, void *ws,
+                       cudaStream_t st);
 
 }  // namespace gsb

@@ -1293,3 +1293,100 @@ def tsdf_extract(tsdf, weight, color_grid, origin, voxel_size):
         _lib.check(lib.gsb_tsdf_extract_emit(*grid, _ptr(tsdf), _ptr(weight), _ptr(color_grid), _ptr(ws), ws.numel(),
                                              nv, nf, _ptr(verts), _ptr(colors), _ptr(faces), _stream()), lib)
     return verts, faces, colors
+
+
+# ---------------------------------------------------------------------------------------
+# Bilateral-grid colour correction (gsb_bilagrid_*, DESIGN 3.20).  grids[M, 12, L, Y, X] float32,
+# channel 4 r + k = A[r][k] of a 3 x 4 affine colour matrix; rgb is one planar image [3, H, W] with
+# one grid index, or a batch [B, 3, H, W] with B indices.  Indices are host integers: an int, a
+# sequence of ints or a CPU tensor; a CUDA tensor is refused, so no index is ever read back from
+# the device and none can reach the kernels unchecked.
+BILAGRID_MAX_DIM = 64
+BILAGRID_MAX_BATCH = 64
+
+
+def _bilagrid_dims(shape):
+    """checks a grids shape [M, 12, L, Y, X] -> (M, L, Y, X)"""
+    if len(shape) != 5 or shape[1] != 12 or shape[0] < 1 or min(shape[2:]) < 1 or max(shape[2:]) > BILAGRID_MAX_DIM:
+        raise ValueError("grids must be [M, 12, L, Y, X] with M >= 1 and 1 <= L, Y, X <= %d, got %s"
+                         % (BILAGRID_MAX_DIM, tuple(shape)))
+    return (int(shape[0]),) + tuple(int(d) for d in shape[2:])
+
+
+def _bilagrid_shape(grids):
+    """checks grids -> (grids contiguous, (M, L, Y, X))"""
+    grids = _chk(grids, "grids", ndim=5)
+    return grids, _bilagrid_dims(grids.shape)
+
+
+def _bilagrid_images(rgb, name, image_ids, M):
+    """rgb [3,H,W] or [B,3,H,W] and its grid indices -> (rgb contiguous, B, H, W, ids as c_int32[B])"""
+    rgb = _chk(rgb, name)
+    if rgb.dim() not in (3, 4) or rgb.shape[-3] != 3:
+        raise ValueError("%s must be [3, H, W] or [B, 3, H, W], got %s" % (name, tuple(rgb.shape)))
+    B = 1 if rgb.dim() == 3 else rgb.shape[0]
+    if isinstance(image_ids, torch.Tensor):
+        if image_ids.is_cuda:
+            raise TypeError("image_ids must be host integers, not a CUDA tensor")
+        image_ids = image_ids.reshape(-1).tolist()
+    ids = [image_ids] if isinstance(image_ids, numbers.Integral) else list(image_ids)
+    if not all(isinstance(i, numbers.Integral) and not isinstance(i, bool) for i in ids):
+        raise TypeError("image_ids must be integers")
+    if len(ids) != B:
+        raise ValueError("%d image ids for a batch of %d images" % (len(ids), B))
+    if not 1 <= B <= BILAGRID_MAX_BATCH:
+        raise ValueError("the batch must hold 1 to %d images, got %d" % (BILAGRID_MAX_BATCH, B))
+    if not all(0 <= i < M for i in ids):
+        raise ValueError("image ids must lie in [0, %d), got %s" % (M, ids))
+    return rgb, B, rgb.shape[-2], rgb.shape[-1], (C.c_int32 * B)(*[int(i) for i in ids])
+
+
+def bilagrid_slice(grids, rgb, image_ids):
+    """out = A rgb + b per pixel, A read from grids[image_ids[b]] at the pixel's position and
+    luminance (gsb_bilagrid_slice) -> a tensor shaped like rgb"""
+    grids, shape = _bilagrid_shape(grids)
+    rgb, B, H, W, ids = _bilagrid_images(rgb, "rgb", image_ids, shape[0])
+    _same_device(grids, rgb)
+    out = torch.empty_like(rgb)
+    lib = _L()
+    with torch.cuda.device(grids.device):
+        _lib.check(lib.gsb_bilagrid_slice(*shape, _ptr(grids), B, ids, H, W, _ptr(rgb), _ptr(out), _stream()), lib)
+    return out
+
+
+def bilagrid_sliceB(grids, rgb, image_ids, dloss_dout, dloss_dgrids=None):
+    """The slice's backward (gsb_bilagrid_slice_backward) -> (dloss_drgb shaped like rgb,
+    dloss_dgrids [M, 12, L, Y, X]).  dloss_dgrids: None (a zeroed tensor is made), or a contiguous
+    float32 tensor of grids' shape that the grid gradient is ADDED to."""
+    grids, shape = _bilagrid_shape(grids)
+    rgb, B, H, W, ids = _bilagrid_images(rgb, "rgb", image_ids, shape[0])
+    dout = _chk(dloss_dout, "dloss_dout")
+    if dout.shape != rgb.shape:
+        raise ValueError("dloss_dout must have rgb's shape %s, got %s" % (tuple(rgb.shape), tuple(dout.shape)))
+    if dloss_dgrids is None:
+        dloss_dgrids = torch.zeros_like(grids)
+    else:
+        _chk(dloss_dgrids, "dloss_dgrids")
+        if dloss_dgrids.shape != grids.shape or not dloss_dgrids.is_contiguous():
+            raise ValueError("dloss_dgrids must be a contiguous tensor of grids' shape (it is added to)")
+    _same_device(grids, rgb, dout, dloss_dgrids)
+    drgb = torch.empty_like(rgb)
+    lib = _L()
+    with torch.cuda.device(grids.device):
+        _lib.check(lib.gsb_bilagrid_slice_backward(*shape, _ptr(grids), B, ids, H, W, _ptr(rgb), _ptr(dout),
+                                                   _ptr(drgb), _ptr(dloss_dgrids), _stream()), lib)
+    return drgb, dloss_dgrids
+
+
+def bilagrid_tv(grids, want_grad=True):
+    """Total variation of the grids (gsb_bilagrid_tv): sum over the axes L, Y, X of the mean squared
+    difference of neighbours along that axis -> (value [1], dTV/dgrids or None)"""
+    grids, shape = _bilagrid_shape(grids)
+    lib = _L()
+    tv = torch.empty((1,), dtype=torch.float32, device=grids.device)
+    grad = torch.empty_like(grids) if want_grad else None
+    ws = _bytes(int(lib.gsb_bilagrid_tv_workspace_bytes(*shape)), grids.device)
+    with torch.cuda.device(grids.device):
+        _lib.check(lib.gsb_bilagrid_tv(*shape, _ptr(grids), _ptr(tv), _ptr(grad), _ptr(ws), ws.numel(), _stream()),
+                   lib)
+    return tv, grad

@@ -830,6 +830,42 @@ int gsb_tsdf_extract_emit(int nx, int ny, int nz, float ox, float oy, float oz, 
                           int64_t n_verts, int64_t n_faces, float *verts, float *vcolors, int32_t *faces,
                           gsb_stream_t stream);
 
+/* ---- bilateral-grid colour correction (extension; DESIGN 3.20; Wang et al., "Bilateral Guided
+ * Radiance Field Processing", SIGGRAPH 2024).  One learnable grid of 3 x 4 affine colour matrices per
+ * training image, sliced on the rendered image before the loss.
+ *
+ * grids[M, 12, L, Y, X] float32 (gsplat's layout): channel c = 4 r + k holds A[r][k]; identity is
+ * A = [I | 0].  1 <= X, Y, L <= GSB_BILAGRID_MAX_DIM, M >= 1.  rgb, out, dloss_dout, dloss_drgb:
+ * B planar images [B, 3, H, W], 1 <= B <= GSB_BILAGRID_MAX_BATCH, H, W >= 1, H W < 2^31.
+ * image_ids: a HOST array of B grid indices in [0, M), read by the call (no device read, no
+ * synchronisation); two items may name the same grid.  Device arrays are 4-byte aligned.
+ * For pixel (px, py) of item b, with G = grids[image_ids[b]]:
+ *   g  = 0.299 r + 0.587 g + 0.114 b                      (guidance: the luminance of the input)
+ *   gx = (px + 1/2) / W (X - 1),  gy = (py + 1/2) / H (Y - 1),  gz = clamp(g, 0, 1) (L - 1)
+ *   A  = trilinear interpolation of G at (gx, gy, gz)     (an axis of size 1 is constant along it)
+ *   out[:, p] = A[:, :3] rgb[:, p] + A[:, 3]
+ * i.e. F.grid_sample(G[None], 2 xyz - 1, bilinear, padding "border", align_corners=True) at
+ * xyz = ((px + 1/2) / W, (py + 1/2) / H, g).
+ * gsb_bilagrid_slice_backward writes dloss_drgb = A[:, :3]^T dL/dout + (dL/dout . dA/dgz [rgb; 1])
+ * (L - 1) (0.299, 0.587, 0.114), the last term only where 0 < g < 1, and ADDS
+ * w_corner dL/dout_r [rgb, 1]_k into dloss_dgrids[M, 12, L, Y, X] (the caller zeroes it).  The grid
+ * gradient is summed with one float atomicAdd per CTA and window element, so it is not
+ * bit-reproducible from run to run; dloss_drgb is.
+ * gsb_bilagrid_tv: TV = sum over the axes a in {L, Y, X} of mean((G shifted by one along a - G)^2)
+ * over all M grids (an axis of size 1 adds 0); writes *tv_out (device) and, when dloss_dgrids is not
+ * NULL, dTV/dgrids (written, not added).  ws: gsb_bilagrid_tv_workspace_bytes bytes, 8-byte aligned.
+ * The value is bit-reproducible. */
+#define GSB_BILAGRID_MAX_DIM 64
+#define GSB_BILAGRID_MAX_BATCH 64
+int gsb_bilagrid_slice(int M, int L, int Y, int X, const float *grids, int B, const int32_t *image_ids, int H, int W,
+                       const float *rgb, float *out, gsb_stream_t stream);
+int gsb_bilagrid_slice_backward(int M, int L, int Y, int X, const float *grids, int B, const int32_t *image_ids,
+                                int H, int W, const float *rgb, const float *dloss_dout, float *dloss_drgb,
+                                float *dloss_dgrids, gsb_stream_t stream);
+size_t gsb_bilagrid_tv_workspace_bytes(int M, int L, int Y, int X);
+int gsb_bilagrid_tv(int M, int L, int Y, int X, const float *grids, float *tv_out, float *dloss_dgrids, void *ws,
+                    size_t ws_bytes, gsb_stream_t stream);
+
 /* ---- launch accounting and optional per-kernel timing (no reference counterpart; used by
  * bench.py for `gpu_launches` and the roofline's live CUDA-event kernel durations).
  * Kernel ids 0..gsb_profile_kernels()-1, names from gsb_profile_kernel_name().
