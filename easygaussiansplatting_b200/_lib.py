@@ -63,6 +63,22 @@ SIGNATURES = {
     "gsb_preprocess_backward_aa": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 15 + [_sz, _vp]),
     "gsb_preprocess_forward_model": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 10),
     "gsb_preprocess_backward_model": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 15 + [_sz, _vp, _vp]),
+    "gsb_preprocess_forward_batch": (_i, [_i, _i, _i] + [_vp] * 6 + [_i, _f, _f] + [_vp] * 9),
+    "gsb_preprocess_backward_batch": (_i, [_i, _i, _i] + [_vp] * 6 + [_i, _f, _f] + [_vp] * 11),
+    "gsb_splat_bin_batch_workspace_bytes": (_sz, [_i, _i]),
+    "gsb_splat_bin_batch": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, C.POINTER(_i64), C.POINTER(C.c_uint32),
+                                 _vp]),
+    "gsb_splat_batch_workspace_bytes": (_sz, [_i, _i, _i, _i, _i64]),
+    "gsb_splat_batch_records_offset": (_sz, [_i, _i, _i, _i, _i64]),
+    "gsb_splat_render_batch": (_i, [_i, _i, _i, _i, _i64, C.c_uint32] + [_vp] * 8 + [_sz] + [_vp] * 6),
+    "gsb_splat_render_batch_rgbd": (_i, [_i, _i, _i, _i, _i64, C.c_uint32] + [_vp] * 8 + [_sz] + [_vp] * 8),
+    "gsb_splat_forward_batch": (_i, [_i, _i, _i, _i] + [_vp] * 7 + [_i64, C.c_uint32, _vp, _sz, _vp, _sz] +
+                                [_vp] * 7),
+    "gsb_splat_forward_batch_rgbd": (_i, [_i, _i, _i, _i] + [_vp] * 7 + [_i64, C.c_uint32, _vp, _sz, _vp, _sz] +
+                                     [_vp] * 9),
+    "gsb_splat_backward_batch_workspace_bytes": (_sz, [_i, _i, _i, _i, _i64]),
+    "gsb_splat_backward_batch": (_i, [_i, _i, _i, _i, _i64] + [_vp] * 11 + [_sz, _vp, _vp]),
+    "gsb_splat_backward_batch_rgbd": (_i, [_i, _i, _i, _i, _i64] + [_vp] * 14 + [_sz, _vp, _vp, _vp]),
     "gsb_sh_grad_expand": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "gsb_filter3d_workspace_bytes": (_sz, [_i, _i]),
     "gsb_filter3d": (_i, [_i, _vp, _i, _vp, _f, _vp, _vp, _sz, _vp]),

@@ -41,7 +41,10 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "density_scan", "density_apply", "reset_alpha",
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
                                              "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
-                                             "filter3d_apply", "filter3d_backward", "density_apply_rows",
+                                             "filter3d_apply", "filter3d_backward", "rects+scan_batch",
+                                             "preprocess_forward_batch", "preprocess_backward_batch",
+                                             "draw_batch", "draw_rgbd_batch", "draw_backward_batch",
+                                             "draw_backward_rgbd_batch", "density_apply_rows",
                                              "bilagrid_slice", "bilagrid_slice_backward", "bilagrid_tv",
                                              "draw_features", "draw_backward_features", "draw_stats",
                                              "draw_surfel_stats", "mcmc_scan",
@@ -504,6 +507,24 @@ static int check_frame(int H, int W, int N, const void *bin_ws, size_t bin_ws_by
   return 0;
 }
 
+// The batch's own checks (DESIGN 3.21): C >= 1 frames, record ids c N + n that fit int32, and a
+// tall frame of C gy tile rows that fits the rectangles' 16-bit fields
+static int check_batch(const char *who, int C, int H, int W, int N) {
+  if (C < 1) return arg_error(who, "C < 1");
+  if (!(N >= 0 && H > 0 && W > 0)) return arg_error(who, "bad N/H/W");
+  if ((int64_t)C * N >= ((int64_t)1 << 31)) return arg_error(who, "C N >= 2^31 records");
+  if (!grid_fits(H, W) || (int64_t)C * ((H + GSB_TILE - 1) / GSB_TILE) > GSB_MAX_GRID_TILES)
+    return arg_error(who, "more than 65535 tiles in a row or in the C frames' column");
+  return 0;
+}
+// check_frame of a batch: the bin workspace holds the C N records
+static int check_frame_batch(const char *who, int C, int H, int W, int N, const void *bin_ws, size_t bin_ws_bytes) {
+  if (int rc = check_batch(who, C, H, W, N)) return rc;
+  if (!aligned(bin_ws, 16)) return arg_error(who, "bin_ws misaligned");
+  if (bin_ws_bytes < bin_layout(C * N).bytes) return arg_error(who, "bin workspace too small");
+  return 0;
+}
+
 size_t gsb_splat_bin_workspace_bytes(int N) { return bin_layout(N).bytes; }
 
 int gsb_splat_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
@@ -544,6 +565,7 @@ struct FrameOut {
 struct ColourDraw {
   const void *packed_records;
   float *depth_image, *alpha_image;
+  int frames = 0;  // > 0: the planes are [frames, ..., H, W] of a batch (launch_draw)
 
   int check() const {
     // RGB-D frames (the *_rgbd entry points pass both planes, written like the image planes)
@@ -556,7 +578,7 @@ struct ColourDraw {
     const Rec *recs = static_cast<const Rec *>(packed_records ? packed_records : ws_recs);
     // with P == 0 (or N == 0) every tile is empty: the rasterizer only writes zeros
     return launch_draw(H, W, o.ranges, P > 0 ? recs : nullptr, o.gsid, o.image, o.contrib, o.final_tau, depth_image,
-                       alpha_image, work, st);
+                       alpha_image, work, st, frames);
   }
 };
 
@@ -572,7 +594,7 @@ template <class Draw>
 static int render_frame(const char *who, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
                         const float *cinv2ds, const float *alphas, float *depths, const float *colors, int32_t *areas,
                         bool pack, void *bin_ws, void *ws, size_t ws_bytes, const FrameOut &o, const Draw &draw,
-                        const StatusRead *sr, cudaStream_t st) {
+                        const StatusRead *sr, cudaStream_t st, int frames = 0) {
   if (!(o.image && o.contrib && o.final_tau && o.ranges)) return arg_error(who, "null output");
   // the rasterizers write the image planes with 16-byte stores and the binning writes the tile
   // ranges as 8-byte pairs; these are outputs a caller allocates fresh (gsplat_b200.h)
@@ -581,16 +603,21 @@ static int render_frame(const char *who, int H, int W, int N, int64_t P, uint32_
   if (int rc = draw.check()) return rc;
   // 64-bit keys at ws + 0, records gathered 16 bytes at a time (the layout's offsets are 256-B multiples)
   if (!aligned(ws, 16)) return arg_error(who, "ws misaligned");
-  const SortLayout SL = sort_layout(N, H, W, P);
+  // frames > 0: a batch binned as one tall frame of the C N records (DESIGN 3.21); its sort is the
+  // single frame's at the tall frame's height
+  const int Ht = frames > 0 ? batch_height(frames, H) : H, Nt = frames > 0 ? frames * N : N;
+  const SortLayout SL = sort_layout(Nt, Ht, W, P);
   if (!(ws != nullptr && ws_bytes >= SL.bytes)) return arg_error(who, "workspace too small");
-  const BinLayout BL = bin_layout(N);
-  int rc = sr ? launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st) : 0;
+  const BinLayout BL = bin_layout(Nt);
+  int rc = !sr ? 0
+               : frames > 0 ? launch_bin_batch(frames, H, W, N, us, depths, areas, bin_ws, BL, st)
+                            : launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st);
   if (rc) return rc;
-  rc = launch_sort_and_pack(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
+  rc = launch_sort_and_pack(Ht, W, Nt, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
                             o.ranges, o.gsid, pack, sr, st);
   if (rc) return rc;
   char *b = static_cast<char *>(ws);
-  return draw.draw(H, W, N, P, o, b + SL.recs, reinterpret_cast<int *>(b + SL.counters), st);
+  return draw.draw(H, W, Nt, P, o, b + SL.recs, reinterpret_cast<int *>(b + SL.counters), st);
 }
 
 // The status event of the capacity path, one per host thread
@@ -815,6 +842,254 @@ int gsb_splat_backward_rgbd_abs(int H, int W, int N, int64_t P, const float *us,
                              patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
                              dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, dloss_dus_abs,
                              stream);
+}
+
+// ---- batched rendering (DESIGN 3.21): C cameras of one image size and camera model, binned and drawn
+// as one tall frame.  The entry points mirror the single-camera ones with C in front.
+
+// The per-camera intrinsics rows (fx, fy, cx, cy, k[4]) checked as camera_lens checks one camera,
+// into the kernels' parameter table; tan_fov exactly as the single-camera path computes it.
+static int batch_scene(const char *who, int C, int N, int sh_dim3, int camera_model, const float *intrinsics,
+                       float width, float height, BatchCams &bc, BatchScene &b) {
+  if (C < 1) return arg_error(who, "C < 1");
+  if (C > BATCH_MAX_CAMERAS) return arg_error(who, "C > GSB_BATCH_MAX_CAMERAS");
+  if (N < 0) return arg_error(who, "N < 0");
+  if ((int64_t)C * N >= ((int64_t)1 << 31)) return arg_error(who, "C N >= 2^31 records");
+  if (!sh_dim3_ok(sh_dim3)) return arg_error(who, "shs.shape[1]/3 must be 1, 4, 9 or 16");
+  if (intrinsics == nullptr) return arg_error(who, "null intrinsics");
+  for (int c = 0; c < C; c++) {
+    const float *r = intrinsics + (size_t)c * GSB_BATCH_INTRINSICS_ROW;
+    const gsb_camera_model cm{camera_model, {r[4], r[5], r[6], r[7]}};
+    FusedScene sc{N, sh_dim3};
+    sc.fx = r[0]; sc.fy = r[1]; sc.cx = r[2]; sc.cy = r[3]; sc.width = width; sc.height = height;
+    CamLens cl;
+    if (int rc = camera_lens(who, &cm, sc, cl)) return rc;
+    const float2 tf = lens_tan_fov(sc);
+    bc.f[c] = make_float4(r[0], r[1], r[2], r[3]);
+    bc.k[c] = make_float4(r[4], r[5], r[6], r[7]);
+    bc.tf[c] = tf;
+  }
+  b.C = C; b.N = N; b.k3 = sh_dim3; b.model = camera_model; b.cams = &bc;
+  return 0;
+}
+
+int gsb_preprocess_forward_batch(int C, int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *poses, const float *intrinsics, int camera_model,
+                                 float width, float height, float *us, float *cinv2ds, float *colors, float *depths,
+                                 int32_t *areas, const float *alphas, void *records, float *alphas_eff,
+                                 gsb_stream_t stream) {
+  const char *who = "preprocess_batch";
+  BatchCams bc;
+  BatchScene b{};
+  if (int rc = batch_scene(who, C, N, sh_dim3, camera_model, intrinsics, width, height, bc, b)) return rc;
+  if (!aligned(records, 16)) return arg_error(who, "records misaligned");
+  if (N > 0 && !(pws && rots && scales && shs && poses && us && cinv2ds && colors && depths && areas && alphas &&
+                 records))
+    return arg_error(who, "null pointer");
+  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
+  return launch_preprocess_fwd_batch(b, {us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records),
+                                         alphas_eff},
+                                     (cudaStream_t)stream);
+}
+
+int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                  const float *shs, const float *poses, const float *intrinsics, int camera_model,
+                                  float width, float height, const float *moments, const float *cinv2ds,
+                                  const float *dloss_ddepths, const float *alphas, float *dloss_dpws,
+                                  float *dloss_dshs, float *dloss_dscales, float *dloss_drots, float *dloss_dus_out,
+                                  float *dloss_dalphas_out, gsb_stream_t stream) {
+  const char *who = "preprocessB_batch";
+  BatchCams bc;
+  BatchScene b{};
+  if (int rc = batch_scene(who, C, N, sh_dim3, camera_model, intrinsics, width, height, bc, b)) return rc;
+  if (N > 0 && !(pws && rots && scales && shs && poses && moments && cinv2ds))
+    return arg_error(who, "null pointer");
+  if (N > 0 && !(dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots && dloss_dus_out && dloss_dalphas_out))
+    return arg_error(who, "null output");
+  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
+  return launch_preprocess_bwd_batch(b, {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
+                                         dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots},
+                                     (cudaStream_t)stream);
+}
+
+// The batch's workspace queries answer 0 for what its entry points refuse: C < 1, N < 0, C N >= 2^31
+static bool batch_records_ok(int C, int N) { return C >= 1 && N >= 0 && (int64_t)C * N < ((int64_t)1 << 31); }
+
+size_t gsb_splat_bin_batch_workspace_bytes(int C, int N) { return batch_records_ok(C, N) ? bin_layout(C * N).bytes : 0; }
+
+int gsb_splat_bin_batch(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
+                        size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host, gsb_stream_t stream) {
+  if (int rc = check_frame_batch("splat_bin_batch", C, H, W, N, bin_ws, bin_ws_bytes)) return rc;
+  GSB_REQUIRE(P_host != nullptr && bin_ws != nullptr, "splat_bin_batch: null workspace / P_host");
+  GSB_REQUIRE(N == 0 || (us && depths && areas), "splat_bin_batch: null pointer");
+  const BinLayout L = bin_layout(C * N);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = launch_bin_batch(C, H, W, N, us, depths, areas, bin_ws, L, st)) return rc;
+  uint32_t total[3] = {0, 0, 0};  // [patch count, largest depth key, flags]
+  GSB_CUDA_TRY(cudaMemcpyAsync(total, static_cast<char *>(bin_ws) + L.total, 3 * sizeof(uint32_t),
+                               cudaMemcpyDeviceToHost, st));
+  GSB_CUDA_TRY(cudaStreamSynchronize(st));
+  GSB_REQUIRE((total[2] & GSB_STATUS_TOO_MANY_PATCHES) == 0 && total[0] < (1u << 30),
+              "splat_bin_batch: more than 2^30 patches");
+  *P_host = (int64_t)total[0];
+  if (depth_key_max_host) *depth_key_max_host = total[1];
+  return 0;
+}
+
+size_t gsb_splat_batch_records_offset(int C, int N, int H, int W, int64_t P) {
+  return batch_records_ok(C, N) ? sort_layout(C * N, batch_height(C, H), W, P).recs : 0;
+}
+
+size_t gsb_splat_batch_workspace_bytes(int C, int N, int H, int W, int64_t P) {
+  return batch_records_ok(C, N) ? sort_layout(C * N, batch_height(C, H), W, P).bytes : 0;
+}
+
+static int splat_render_batch_impl(const char *who, int C, int H, int W, int N, int64_t P, uint32_t depth_key_max,
+                                   const float *us, const float *cinv2ds, const float *alphas, const float *depths,
+                                   const float *colors, const void *packed_records, const void *bin_ws, void *ws,
+                                   size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                                   int32_t *patch_range_per_tile, int32_t *gsid_per_patch, float *depth_image,
+                                   float *alpha_image, gsb_stream_t stream) {
+  if (int rc = check_frame_batch(who, C, H, W, N, bin_ws, SIZE_MAX)) return rc;
+  if (P < 0) return arg_error(who, "bad P");
+  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
+  if (P > 0 && !(us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch))
+    return arg_error(who, "null pointer");
+  return render_frame(who, H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors,
+                      nullptr, packed_records == nullptr, const_cast<void *>(bin_ws), ws, ws_bytes,
+                      {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                      ColourDraw{packed_records, depth_image, alpha_image, C}, nullptr, (cudaStream_t)stream, C);
+}
+
+int gsb_splat_render_batch(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                           const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                           const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
+                           int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                           int32_t *gsid_per_patch, gsb_stream_t stream) {
+  return splat_render_batch_impl("splat_batch", C, H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors,
+                                 packed_records, bin_ws, ws, ws_bytes, image, contrib, final_tau,
+                                 patch_range_per_tile, gsid_per_patch, nullptr, nullptr, stream);
+}
+
+int gsb_splat_render_batch_rgbd(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                                const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                                const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes,
+                                float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                                int32_t *gsid_per_patch, float *depth_image, float *alpha_image, gsb_stream_t stream) {
+  GSB_REQUIRE(depth_image && alpha_image, "splat_batch_rgbd: null depth_image / alpha_image");
+  return splat_render_batch_impl("splat_batch_rgbd", C, H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths,
+                                 colors, packed_records, bin_ws, ws, ws_bytes, image, contrib, final_tau,
+                                 patch_range_per_tile, gsid_per_patch, depth_image, alpha_image, stream);
+}
+
+static int splat_forward_batch_impl(const char *who, int C, int H, int W, int N, const float *us,
+                                    const float *cinv2ds, const float *alphas, float *depths, const float *colors,
+                                    int32_t *areas, const void *packed_records, int64_t P_cap, uint32_t depth_key_cap,
+                                    void *bin_ws, size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image,
+                                    int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                                    int32_t *gsid_per_patch, uint32_t *status_host, float *depth_image,
+                                    float *alpha_image, gsb_stream_t stream) {
+  if (int rc = check_frame_batch(who, C, H, W, N, bin_ws, bin_ws_bytes)) return rc;
+  if (!(P_cap > 0 && P_cap < ((int64_t)1 << 30))) return arg_error(who, "bad P_cap (2^30 patches or more)");
+  if (!(gsid_per_patch && status_host && bin_ws)) return arg_error(who, "null pointer");
+  if (N > 0 && !(us && cinv2ds && alphas && depths && colors && areas)) return arg_error(who, "null pointer");
+  return capacity_wait(who, P_cap, status_host, true, [&](const StatusRead *sr) {
+    return render_frame(who, H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas,
+                        packed_records == nullptr, bin_ws, ws, ws_bytes,
+                        {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
+                        ColourDraw{packed_records, depth_image, alpha_image, C}, sr, (cudaStream_t)stream, C);
+  });
+}
+
+int gsb_splat_forward_batch(int C, int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
+                            float *depths, const float *colors, int32_t *areas, const void *packed_records,
+                            int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
+                            size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                            int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
+                            gsb_stream_t stream) {
+  return splat_forward_batch_impl("splat_batch", C, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
+                                  packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image,
+                                  contrib, final_tau, patch_range_per_tile, gsid_per_patch, status_host, nullptr,
+                                  nullptr, stream);
+}
+
+int gsb_splat_forward_batch_rgbd(int C, int H, int W, int N, const float *us, const float *cinv2ds,
+                                 const float *alphas, float *depths, const float *colors, int32_t *areas,
+                                 const void *packed_records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                                 size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                                 float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                                 uint32_t *status_host, float *depth_image, float *alpha_image, gsb_stream_t stream) {
+  GSB_REQUIRE(depth_image && alpha_image, "splat_batch_rgbd: null depth_image / alpha_image");
+  return splat_forward_batch_impl("splat_batch_rgbd", C, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
+                                  packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image,
+                                  contrib, final_tau, patch_range_per_tile, gsid_per_patch, status_host, depth_image,
+                                  alpha_image, stream);
+}
+
+size_t gsb_splat_backward_batch_workspace_bytes(int C, int N, int H, int W, int64_t P) {
+  return batch_records_ok(C, N) ? bwd_layout(C * N, batch_height(C, H), W, P, 1).bytes : 0;
+}
+
+// the batch's backward rasterizer: the moment rows [C N, 9] (and dL/dz [C N]) for
+// gsb_preprocess_backward_batch; the records are packed_records or re-packed into ws
+static int splat_backward_batch_impl(const char *who, int C, int H, int W, int N, int64_t P, const float *us,
+                                     const float *cinv2ds, const float *alphas, const float *colors,
+                                     const float *depths, const int32_t *contrib, const float *final_tau,
+                                     const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                                     const float *dloss_dgammas, const DepthGrads *dg, const void *packed_records,
+                                     void *ws, size_t ws_bytes, float *moments_out, gsb_stream_t stream) {
+  if (int rc = check_batch(who, C, H, W, N)) return rc;
+  if (P < 0) return arg_error(who, "bad P");
+  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
+  if (N == 0) return 0;
+  if (!(cinv2ds && ws && moments_out)) return arg_error(who, "null pointer");
+  const int NT = C * N;
+  const int64_t P_ws = packed_records != nullptr ? 0 : P;
+  if (ws_bytes < gsb_splat_backward_batch_workspace_bytes(C, N, H, W, P_ws)) return arg_error(who, "workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  char *b = static_cast<char *>(ws);
+  const BwdLayout L = bwd_layout(NT, batch_height(C, H), W, P_ws, reinterpret_cast<uintptr_t>(ws));
+  Rec *recs = reinterpret_cast<Rec *>(b + L.recs);
+  if (P > 0) {
+    if (!(us && alphas && colors && contrib && final_tau && patch_range_per_tile && gsid_per_patch && dloss_dgammas))
+      return arg_error(who, "null pointer");
+    if (dg != nullptr && !(depths && dg->dloss_ddepth_image && dg->dloss_dalpha_image && dg->ddepths))
+      return arg_error(who, "null pointer");
+    if (!aligned(packed_records, 16)) return arg_error(who, "packed_records misaligned");
+    if (packed_records != nullptr) {
+      recs = const_cast<Rec *>(static_cast<const Rec *>(packed_records));
+    } else if (int rc = launch_pack_only(NT, nullptr, us, cinv2ds, alphas, colors, depths, recs, st)) {
+      return rc;
+    }
+  } else if (dg != nullptr && dg->ddepths == nullptr) {
+    return arg_error(who, "null pointer");
+  }
+  return launch_draw_backward(H, W, NT, patch_range_per_tile, P > 0 ? recs : nullptr, gsid_per_patch, contrib,
+                              final_tau, dloss_dgammas, dg, cinv2ds, moments_out, reinterpret_cast<int *>(b + L.work),
+                              nullptr, nullptr, nullptr, nullptr, false, nullptr, st, C);
+}
+
+int gsb_splat_backward_batch(int C, int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                             const float *alphas, const float *colors, const int32_t *contrib, const float *final_tau,
+                             const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                             const float *dloss_dgammas, const void *packed_records, void *ws, size_t ws_bytes,
+                             float *moments_out, gsb_stream_t stream) {
+  return splat_backward_batch_impl("splatB_batch", C, H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib,
+                                   final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr,
+                                   packed_records, ws, ws_bytes, moments_out, stream);
+}
+
+int gsb_splat_backward_batch_rgbd(int C, int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                                  const float *alphas, const float *colors, const float *depths,
+                                  const int32_t *contrib, const float *final_tau, const int32_t *patch_range_per_tile,
+                                  const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                                  const float *dloss_ddepth_image, const float *dloss_dalpha_image,
+                                  const void *packed_records, void *ws, size_t ws_bytes, float *moments_out,
+                                  float *dloss_ddepths, gsb_stream_t stream) {
+  const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
+  return splat_backward_batch_impl("splatB_batch_rgbd", C, H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib,
+                                   final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg,
+                                   packed_records, ws, ws_bytes, moments_out, stream);
 }
 
 // ---- 2D Gaussian Splatting (surfel.cu, DESIGN 3.15)

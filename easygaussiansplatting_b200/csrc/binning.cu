@@ -22,6 +22,7 @@
 #include "../../include/gsplat_b200.h"
 #include "common.cuh"
 #include "kernels.h"
+#include "rect_math.h"
 #include "tile_io.cuh"
 
 namespace gsb {
@@ -92,17 +93,19 @@ __device__ unsigned long long scan_lookback(unsigned long long *desc, int blk, u
 
 // =================================================================== phase 1: rects + scan
 // One CTA = 1024 consecutive Gaussians (4 per thread, strided so every access is coalesced).
-// Rectangle arithmetic: kernel.cu:105-110; DIV_ROUND_UP(X,16) on floats is ((X) + 16 - 1) / 16
-// (common.cuh:15).  Explicit _rn intrinsics: these decide the patch list, no contraction.
+// Rectangle arithmetic: rect_math.h tile_rect (explicitly rounded: it decides the patch list).
 // The inclusive prefix sum of the patch counts uses the decoupled look-back above.
 constexpr int RS_CTA = 256, RS_ITEMS = 4, RS_SPAN = RS_CTA * RS_ITEMS;
 
-__global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__restrict__ us,
-                                                       int32_t *__restrict__ areas, float *__restrict__ depths,
-                                                       int gx, int gy, uint2 *__restrict__ rects,
-                                                       uint32_t *__restrict__ incl, uint32_t *__restrict__ total,
-                                                       unsigned long long *__restrict__ desc,
-                                                       uint32_t *__restrict__ claim) {
+// BATCH: the N = C nc records of a batch of C frames, record i = c nc + n in frame c (DESIGN 3.21):
+// its rectangle is the single frame's (the same operations on its camera-local mean), clamped to
+// frame c's gy tile rows [0, gy] and then moved down by c gy rows of the tall frame.
+template <bool BATCH>
+__device__ __forceinline__ void rects_scan_body(int N, const float *__restrict__ us, int32_t *__restrict__ areas,
+                                                float *__restrict__ depths, int gx, int gy, int nc,
+                                                uint2 *__restrict__ rects, uint32_t *__restrict__ incl,
+                                                uint32_t *__restrict__ total, unsigned long long *__restrict__ desc,
+                                                uint32_t *__restrict__ claim) {
   __shared__ uint32_t s_warp[RS_CTA / 32];
   __shared__ unsigned long long s_prefix;
   __shared__ uint32_t s_max[RS_CTA / 32];
@@ -124,10 +127,8 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__res
         const float2 u = ld_pair(us, i);  // us / areas: any contiguous [N,2] view (tile_io.cuh)
         const int2 ar = ld_pair_rw(areas, i);
         const float xs = (float)ar.x, ys = (float)ar.y;
-        const int x0 = min(gx, max(0, (int)__fdiv_rn(__fsub_rn(u.x, xs), 16.0f)));
-        const int y0 = min(gy, max(0, (int)__fdiv_rn(__fsub_rn(u.y, ys), 16.0f)));
-        const int x1 = min(gx, max(0, (int)__fdiv_rn(__fsub_rn(__fadd_rn(__fadd_rn(u.x, xs), 16.0f), 1.0f), 16.0f)));
-        const int y1 = min(gy, max(0, (int)__fdiv_rn(__fsub_rn(__fadd_rn(__fadd_rn(u.y, ys), 16.0f), 1.0f), 16.0f)));
+        int x0, x1, y0, y1;  // BATCH: in frame i / nc's rows of the tall frame
+        tile_rect(u.x, u.y, xs, ys, gx, gy, BATCH ? (i / nc) * gy : 0, x0, x1, y0, y1);
         n = (uint32_t)(y1 - y0) * (uint32_t)(x1 - x0);
         if (n == 0) {  // kernel.cu:114-119: in-place cull
           depths[i] = BAD_MARKER;
@@ -188,6 +189,24 @@ __global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__res
     if (m > 0) atomicMax(total + 1, m);  // largest depth key of a binned Gaussian
     if (s_prefix + run > 0xffffffffull) atomicOr(total + 2, GSB_STATUS_TOO_MANY_PATCHES);  // P does not fit 32 bits
   }
+}
+
+__global__ void __launch_bounds__(RS_CTA) k_rects_scan(int N, const float *__restrict__ us,
+                                                       int32_t *__restrict__ areas, float *__restrict__ depths,
+                                                       int gx, int gy, uint2 *__restrict__ rects,
+                                                       uint32_t *__restrict__ incl, uint32_t *__restrict__ total,
+                                                       unsigned long long *__restrict__ desc,
+                                                       uint32_t *__restrict__ claim) {
+  rects_scan_body<false>(N, us, areas, depths, gx, gy, 0, rects, incl, total, desc, claim);
+}
+
+__global__ void __launch_bounds__(RS_CTA) k_rects_scan_batch(int N, const float *__restrict__ us,
+                                                             int32_t *__restrict__ areas, float *__restrict__ depths,
+                                                             int gx, int gy, int nc, uint2 *__restrict__ rects,
+                                                             uint32_t *__restrict__ incl, uint32_t *__restrict__ total,
+                                                             unsigned long long *__restrict__ desc,
+                                                             uint32_t *__restrict__ claim) {
+  rects_scan_body<true>(N, us, areas, depths, gx, gy, nc, rects, incl, total, desc, claim);
 }
 
 // =================================================================== phase 2: keys
@@ -573,6 +592,23 @@ int launch_bin(int H, int W, int N, const float *us, float *depths, int32_t *are
       N, us, areas, depths, gx, gy,
       reinterpret_cast<uint2 *>(b + L.rects), reinterpret_cast<uint32_t *>(b + L.offsets), total,
       reinterpret_cast<unsigned long long *>(b + L.scan_desc), total + 3);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_bin_batch(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas, void *ws,
+                     const BinLayout &L, cudaStream_t st) {
+  char *b = static_cast<char *>(ws);
+  uint32_t *total = reinterpret_cast<uint32_t *>(b + L.total);
+  GSB_CUDA_TRY(cudaMemsetAsync(total, 0, L.bytes - L.total, st));
+  const int NT = C * N;  // (C N < 2^31: checked by the entry points)
+  if (NT <= 0) return 0;
+  const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
+  ProfScope ps(K_RECTS_BATCH, st);
+  k_rects_scan_batch<<<(NT + RS_SPAN - 1) / RS_SPAN, RS_CTA, 0, st>>>(
+      NT, us, areas, depths, gx, gy, N, reinterpret_cast<uint2 *>(b + L.rects),
+      reinterpret_cast<uint32_t *>(b + L.offsets), total, reinterpret_cast<unsigned long long *>(b + L.scan_desc),
+      total + 3);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

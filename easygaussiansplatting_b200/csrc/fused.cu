@@ -341,6 +341,134 @@ __global__ void __launch_bounds__(PG) k_sh_expand(int N, int V, const float *__r
   tile_flush<KS>(g_shs, base, nv, sm, tid);
 }
 
+// ---- batched per-Gaussian path (DESIGN 3.21): C cameras in one launch.  A thread loads its
+// Gaussian's rows once (the 10 small floats to registers, the SH row through the shared tile) and
+// runs pg::forward_one / pg::backward_one once per camera, camera c from poses[c] (Rcw 9, tcw 3,
+// twc 3 floats, device memory) and cams (its intrinsics, kernel parameter memory).  Outputs of
+// camera c go to rows c N + n of the [C, N, ...] arrays; record c N + n carries id c N + n.
+__device__ __forceinline__ pg::Cam batch_cam(const float *__restrict__ poses, const BatchCams &bc, int c, bool lens) {
+  const float *p = poses + 15 * c;
+  const float4 f = bc.f[c];
+  const float2 tf = bc.tf[c];
+  pg::Cam cam = load_cam(p, p + 9, p + 12, f.x, f.y, f.z, f.w, tf.x, tf.y);
+  if (lens) {
+    const float4 lk = bc.k[c];
+    cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w;
+  }
+  return cam;
+}
+
+// the forward: k_preprocess_fwd's outputs per camera (alphas and records required)
+template <int K3, bool AA, int MODEL>
+__global__ void __launch_bounds__(PG) k_preprocess_fwd_batch(
+    int C, int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
+    const float *__restrict__ shs, const float *__restrict__ poses, const __grid_constant__ BatchCams bc,
+    float *__restrict__ us, float *__restrict__ cinv2ds, float *__restrict__ colors, float *__restrict__ depths,
+    int32_t *__restrict__ areas, const float *__restrict__ alphas, Rec *__restrict__ recs,
+    float *__restrict__ alphas_eff) {
+  constexpr int KS = 3 * K3;
+  constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
+  __shared__ float sm[SMF];
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * PG;
+  const int nv = min(PG, (int)(N - base));
+  const bool valid = tid < nv;
+  float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
+  load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);
+  tile_fetch<KS>(shs, base, nv, sm, tid);
+  __syncthreads();
+  if (!valid) return;
+  const long long i = base + tid;
+  const float alpha = __ldg(alphas + i);
+  for (int c = 0; c < C; c++) {
+    const pg::Cam cam = batch_cam(poses, bc, c, MODEL == pg::FISHEYE || MODEL == pg::OPENCV);
+    float u[2] = {0.f, 0.f}, conic[3] = {0.f, 0.f, 0.f}, col[3] = {0.f, 0.f, 0.f}, depth = -1.f;
+    int area[2] = {0, 0};
+    const float rho = pg::forward_one<K3, AA, MODEL>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
+    const long long o = (long long)c * N + i;
+    st_pair(us, o, u[0], u[1]);
+    cinv2ds[3 * o] = conic[0]; cinv2ds[3 * o + 1] = conic[1]; cinv2ds[3 * o + 2] = conic[2];
+    colors[3 * o] = col[0]; colors[3 * o + 1] = col[1]; colors[3 * o + 2] = col[2];
+    st_pair(areas, o, area[0], area[1]);
+    depths[o] = depth;
+    float al = alpha;
+    if (AA) {
+      al = rho * alpha;
+      alphas_eff[o] = al;
+    }
+    recs[o] = build_record(u[0], u[1], conic[0], conic[1], conic[2], al, col[0], col[1], col[2], depth, (int)o);
+  }
+}
+
+// the backward from the C moment rows [C, N, 9] (and dL/dz [C, N] with DEPTH): the C contributions
+// to each per-Gaussian gradient, dL/dsh included, are summed in fp32 registers in camera order; one
+// gradient row per Gaussian, dL/du per camera [C, N, 2] and the summed dL/dalpha [N].  AA: as
+// k_preprocess_bwd's (dL/dalpha = sum_c rho_c m_c[5]).
+template <int K3, bool DEPTH, bool AA, int MODEL>
+__global__ void __launch_bounds__(PG) k_preprocess_bwd_batch(
+    int C, int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
+    const float *__restrict__ shs, const float *__restrict__ poses, const __grid_constant__ BatchCams bc,
+    const float *__restrict__ moments, const float *__restrict__ cinv2ds, const float *__restrict__ g_depths,
+    const float *__restrict__ alphas, float *__restrict__ dus_out, float *__restrict__ dalphas_out,
+    float *__restrict__ g_pws, float *__restrict__ g_shs, float *__restrict__ g_scales, float *__restrict__ g_rots) {
+  constexpr int KS = 3 * K3;
+  constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
+  __shared__ float sm[SMF];
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * PG;
+  const int nv = min(PG, (int)(N - base));
+  const bool valid = tid < nv;
+  float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
+  load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);
+  tile_fetch<KS>(shs, base, nv, sm, tid);
+  __syncthreads();
+  float gpw[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gsh[KS], gal = 0.f;
+#pragma unroll
+  for (int e = 0; e < KS; e++) gsh[e] = 0.f;
+  const long long i = base + tid;
+  if (valid) {
+    const float al = AA ? __ldg(alphas + i) : 0.f;
+    for (int c = 0; c < C; c++) {
+      const long long o = (long long)c * N + i;
+      float m[9];
+#pragma unroll
+      for (int k = 0; k < 9; k++) m[k] = __ldg(moments + 9 * o + k);
+      const float A = __ldg(cinv2ds + 3 * o), B = __ldg(cinv2ds + 3 * o + 1), Cc = __ldg(cinv2ds + 3 * o + 2);
+      const bool none = (m[0] == 0.f) && (m[1] == 0.f);  // as k_preprocess_bwd's MOM form
+      const float gu[2] = {none ? 0.f : -(A * m[0] + B * m[1]), none ? 0.f : -(B * m[0] + Cc * m[1])};
+      const float gci[3] = {-0.5f * m[2], -m[3], -0.5f * m[4]}, gcol[3] = {m[6], m[7], m[8]};
+      st_pair(dus_out, o, gu[0], gu[1]);
+      const float gz = DEPTH ? __ldg(g_depths + o) : 0.f;
+      const pg::Cam cam = batch_cam(poses, bc, c, MODEL == pg::FISHEYE || MODEL == pg::OPENCV);
+      float xpw[3], xq[4], xs[3], xsh[KS];
+      gal += pg::backward_one<K3, DEPTH, false, AA, MODEL>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh,
+                                                           gz, nullptr, m[5], al);
+#pragma unroll
+      for (int e = 0; e < 3; e++) { gpw[e] += xpw[e]; gs[e] += xs[e]; }
+#pragma unroll
+      for (int e = 0; e < 4; e++) gq[e] += xq[e];
+#pragma unroll
+      for (int e = 0; e < KS; e++) gsh[e] += xsh[e];
+    }
+    // dL/dsh replaces the thread's own SH row (no other thread reads it before the barrier)
+    float *row = ROWK(KS);
+#pragma unroll
+    for (int e = 0; e < KS; e++) row[e] = gsh[e];
+    dalphas_out[i] = gal;
+  }
+  __syncthreads();
+  tile_flush<KS>(g_shs, base, nv, sm, tid);
+  if (valid) {
+    g_pws[3 * i] = gpw[0]; g_pws[3 * i + 1] = gpw[1]; g_pws[3 * i + 2] = gpw[2];
+    g_scales[3 * i] = gs[0]; g_scales[3 * i + 1] = gs[1]; g_scales[3 * i + 2] = gs[2];
+    if (aligned16(g_rots)) {
+      reinterpret_cast<float4 *>(g_rots)[i] = make_float4(gq[0], gq[1], gq[2], gq[3]);
+    } else {
+      g_rots[4 * i] = gq[0]; g_rots[4 * i + 1] = gq[1]; g_rots[4 * i + 2] = gq[2]; g_rots[4 * i + 3] = gq[3];
+    }
+  }
+}
+
 #define GSB_DISPATCH_K3(k3, CALL)                                           \
   switch (k3) {                                                             \
     case 1: { constexpr int K3 = 1; CALL; } break;                          \
@@ -376,7 +504,7 @@ static float4 lens_k(const CamLens *lens) {
   return lens ? make_float4(lens->k[0], lens->k[1], lens->k[2], lens->k[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 // the kernels' tan_fovx, tan_fovy: W / (2 fx), H / (2 fy), stretched by OPENCV's lens (exactly 1 otherwise)
-static float2 lens_tan_fov(const FusedScene &sc) {
+float2 lens_tan_fov(const FusedScene &sc) {
   const float c = sc.lens ? sc.lens->stretch : 1.f;
   return make_float2(sc.width / (2 * sc.fx) * c, sc.height / (2 * sc.fy) * c);
 }
@@ -466,6 +594,50 @@ int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t 
   }
   if (nb > 0 && (po == nullptr || b.g_pws != nullptr))
     if (int rc = pass(std::false_type{})) return rc;
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_preprocess_fwd_batch(const BatchScene &b, const FusedFwd &f, cudaStream_t st) {
+  if (b.N <= 0) return 0;
+  const int nb = (b.N + PG - 1) / PG;
+  const CamLens model{b.model, {0.f, 0.f, 0.f, 0.f}, 1.f};
+  ProfScope ps(K_PRE_FWD_BATCH, st);
+  const auto launch = [&](auto aa) {
+    return with_model(&model, "preprocess_batch: unknown camera model", [&](auto mdl) -> int {
+      constexpr bool AA = decltype(aa)::value;
+      constexpr int MODEL = decltype(mdl)::value;
+      GSB_DISPATCH_K3(b.k3, (k_preprocess_fwd_batch<K3, AA, MODEL><<<nb, PG, 0, st>>>(
+                                b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses, *b.cams, f.us, f.cinv2ds, f.colors,
+                                f.depths, f.areas, f.alphas, f.recs, f.alphas_eff)));
+      return 0;
+    });
+  };
+  const int rc = f.alphas_eff != nullptr ? launch(std::true_type{}) : launch(std::false_type{});
+  if (rc) return rc;
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStream_t st) {
+  if (b.N <= 0) return 0;
+  const int nb = (b.N + PG - 1) / PG;
+  const CamLens model{b.model, {0.f, 0.f, 0.f, 0.f}, 1.f};
+  ProfScope ps(K_PRE_BWD_BATCH, st);
+  const int rc = with_model(&model, "preprocessB_batch: unknown camera model", [&](auto mdl) {
+    return with_flags(
+        [&](auto depth, auto aa) -> int {
+          constexpr bool DEPTH = decltype(depth)::value, AA = decltype(aa)::value;
+          constexpr int MODEL = decltype(mdl)::value;
+          GSB_DISPATCH_K3(b.k3, (k_preprocess_bwd_batch<K3, DEPTH, AA, MODEL><<<nb, PG, 0, st>>>(
+                                    b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses, *b.cams, g.moments,
+                                    g.cinv2ds, g.g_depths, g.alphas, g.dus_out, g.dalphas_out, g.g_pws, g.g_shs,
+                                    g.g_scales, g.g_rots)));
+          return 0;
+        },
+        g.g_depths != nullptr, g.alphas != nullptr);
+  });
+  if (rc) return rc;
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

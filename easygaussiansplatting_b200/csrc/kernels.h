@@ -18,7 +18,8 @@ enum KernelId {
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
-  K_DENSITY_ROWS, K_BILAGRID_SLICE, K_BILAGRID_SLICE_BWD, K_BILAGRID_TV, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
+  K_RECTS_BATCH, K_PRE_FWD_BATCH, K_PRE_BWD_BATCH, K_DRAW_BATCH, K_DRAW_RGBD_BATCH, K_DRAW_BWD_BATCH,
+  K_DRAW_BWD_RGBD_BATCH, K_DENSITY_ROWS, K_BILAGRID_SLICE, K_BILAGRID_SLICE_BWD, K_BILAGRID_TV, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
   K_MCMC_ROWS, K_MCMC_NOISE, K_TSDF_INTEGRATE, K_TSDF_PLAN, K_TSDF_EMIT,
   K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
   K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
@@ -104,6 +105,35 @@ struct FusedBwd {
   const GradPush *gp;
 };
 int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t st);
+
+// the kernels' tan_fovx, tan_fovy of a scene whose lens camera_lens (api.cu) has set
+float2 lens_tan_fov(const FusedScene &sc);
+
+// ---- batched per-Gaussian path (fused.cu, DESIGN 3.21).  The intrinsics of the C cameras travel
+// in kernel parameter memory (nothing to copy to the device, nothing to wait for): C <= 64.
+constexpr int BATCH_MAX_CAMERAS = 64;
+struct BatchCams {
+  float4 f[BATCH_MAX_CAMERAS];   // fx, fy, cx, cy
+  float4 k[BATCH_MAX_CAMERAS];   // the lens's k (FISHEYE, OPENCV)
+  float2 tf[BATCH_MAX_CAMERAS];  // tan_fovx, tan_fovy (lens_tan_fov)
+};
+// the Gaussians and C cameras of one model and image size: poses [C,15] = Rcw (9), tcw (3), twc (3)
+// per camera in device memory, cams on the host
+struct BatchScene {
+  int C, N, k3;
+  const float *pws, *rots, *scales, *shs, *poses;
+  int model;  // pg::CamModel
+  const BatchCams *cams;
+};
+// f: the [C, N, ...] outputs (alphas [N] and recs [C N] required; alphas_eff [C, N]: antialiasing)
+int launch_preprocess_fwd_batch(const BatchScene &b, const FusedFwd &f, cudaStream_t st);
+// moments [C N, 9], cinv2ds [C N, 3], g_depths NULL or [C N] (RGB-D), alphas NULL or the raw
+// opacities [N] (antialiasing); outputs dus_out [C N, 2], dalphas_out [N] and the four gradients
+struct BatchBwd {
+  const float *moments, *cinv2ds, *g_depths, *alphas;
+  float *dus_out, *dalphas_out, *g_pws, *g_shs, *g_scales, *g_rots;
+};
+int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)
 int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, const float *gcols, float *g_shs,
@@ -219,6 +249,13 @@ struct BinLayout {  // carve-up of the phase-1 workspace
 BinLayout bin_layout(int N);
 int launch_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas, void *ws,
                const BinLayout &L, cudaStream_t st);
+// phase 1 of a batch of C frames binned as one tall frame (DESIGN 3.21): us / depths / areas hold
+// the C N records (record c N + n: Gaussian n in camera c), L = bin_layout(C N); record c N + n's
+// rectangle is the single frame's, clamped to frame c's gy tile rows and moved down by c gy rows.
+int launch_bin_batch(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas, void *ws,
+                     const BinLayout &L, cudaStream_t st);
+// the tall frame's height in pixels: C whole-tile frames (its phase 2 is the single frame's at this height)
+constexpr int batch_height(int C, int H) { return C * ((H + 15) / 16) * 16; }
 
 struct SortLayout {  // carve-up of the phase-2 workspace
   size_t keys_a, keys_b, vals_a, vals_b, recs, counters;
@@ -255,11 +292,13 @@ int launch_pack_only(int64_t P, const int32_t *gsid_per_patch, const float *us, 
 // zero-filled there.
 // depth_image / alpha_image: both NULL (colour frame), or the RGB-D frame's D and A planes [H,W]
 // (k_draw_rgbd; the records' depth word must hold z).
+// frames > 0: the tall frame of a batch of `frames` H x W frames (DESIGN 3.21): ranges of its
+// frames * gx * gy tiles, planes [frames, ..., H, W] (k_tile_list_batch, k_draw_batch, k_draw_rgbd_batch)
 int launch_tile_list(int H, int W, const int32_t *ranges, float *image, int32_t *contrib, float *final_tau,
-                     float *depth_image, float *alpha_image, int *work, cudaStream_t st);
+                     float *depth_image, float *alpha_image, int *work, cudaStream_t st, int frames = 0);
 int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int32_t *gsid, float *image,
                 int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, int *work,
-                cudaStream_t st);
+                cudaStream_t st, int frames = 0);
 // the RGB-D backward's extra upstream planes [H,W] and its dL/dz output [N] (zeroed here)
 struct DepthGrads {
   const float *dloss_ddepth_image;
@@ -268,12 +307,13 @@ struct DepthGrads {
 };
 // dg == nullptr: k_draw_bwd; otherwise k_draw_bwd_rgbd.  dus_abs: NULL, or [N,2] (any 4-byte
 // alignment, zeroed here) for the per-pixel absolute sums of dL/du: then k_draw_bwd_abs /
-// k_draw_bwd_rgbd_abs
+// k_draw_bwd_rgbd_abs.  frames > 0: as for launch_draw (N = all records of the batch; no dus_abs):
+// k_draw_bwd_batch / k_draw_bwd_rgbd_batch
 int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *recs, const int32_t *gsid,
                          const int32_t *contrib, const float *final_tau, const float *dloss_dgammas,
                          const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
                          float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
-                         float *dus_abs, cudaStream_t st);
+                         float *dus_abs, cudaStream_t st, int frames = 0);
 
 // ---- feature rasterizers (raster_feat.cu): replays of the colour forward's binning that composite
 // features[N,D] (row stride D, any 4-byte alignment) with the image's weights.  ranges: any

@@ -152,10 +152,11 @@ __device__ __forceinline__ void bwd_flush(uint32_t w_addr, const float4 &inf, co
 // dL/dgamma . c (the sdot recurrence carries the sum of all five channels), and phase B sums
 // wc dL/dD into dL/dz from a fourth per-pixel table.  dL/dA needs no table: opacity has no
 // per-Gaussian value to differentiate.  ABS: the _abs kernels; phase A also keeps the lane's slot's
-// record word q1 (the conic) for bwd_flush's absolute sums into dus_abs.
-template <bool RGBD, bool ABS>
+// record word q1 (the conic) for bwd_flush's absolute sums into dus_abs.  BATCH: the tall frame of a
+// batch, as draw_body's BATCH (raster_fwd.cu): the per-pixel planes are frame r / gy's of [C,...,H,W].
+template <bool RGBD, bool ABS, bool BATCH>
 __device__ __forceinline__ void draw_bwd_body(
-    int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    int W, int H, int gx, int gy, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
@@ -202,12 +203,19 @@ __device__ __forceinline__ void draw_bwd_body(
       if (whole_tile) gather_whole_tile(ring_addr, recs, gsid + range.x, len, lane);
     }
     const int cur = blk++;
-    const int tx = tile % gx, ty = tile / gx;
+    int tx = tile % gx, ty = tile / gx;
+    size_t fo = 0;  // BATCH: offset of the tile's frame in every [H,W] plane
+    if (BATCH) {
+      const int f = ty / gy;
+      ty -= f * gy;
+      fo = (size_t)f * HW;
+    }
     const int rx0 = tx * TILE + (cur & 1) * 8, ry0 = ty * TILE + (cur >> 1) * 8;
-    if (rx0 >= W || ry0 >= H) continue;  // block entirely outside the image
+    if (rx0 >= W || ry0 >= H) continue;  // block entirely outside the image (BATCH: or in a pad row)
     const int px = rx0 + 2 * (lane & 3), py = ry0 + (lane >> 2);
     const bool in0 = px < W && py < H, in1 = px + 1 < W && py < H;
-    const size_t pix = (size_t)py * W + px;
+    const size_t pix = fo + (size_t)py * W + px;
+    const float *const dl_f = dloss_dgammas + 2 * fo;  // pix holds fo; the frame's [3,H,W] planes start at 3 fo
 
     int cont0 = 0, cont1 = 0;
     float2 tau = p2s(0.f), dlr = p2s(0.f), dlg = p2s(0.f), dlb = p2s(0.f);
@@ -219,16 +227,16 @@ __device__ __forceinline__ void draw_bwd_body(
     if (in0) {
       cont0 = min(__ldg(contrib + pix), len);
       tau.x = __ldg(final_tau + pix);
-      dlr.x = __ldg(dloss_dgammas + pix);
-      dlg.x = __ldg(dloss_dgammas + HW + pix);
-      dlb.x = __ldg(dloss_dgammas + 2 * HW + pix);
+      dlr.x = __ldg(dl_f + pix);
+      dlg.x = __ldg(dl_f + HW + pix);
+      dlb.x = __ldg(dl_f + 2 * HW + pix);
     }
     if (in1) {
       cont1 = min(__ldg(contrib + pix + 1), len);
       tau.y = __ldg(final_tau + pix + 1);
-      dlr.y = __ldg(dloss_dgammas + pix + 1);
-      dlg.y = __ldg(dloss_dgammas + HW + pix + 1);
-      dlb.y = __ldg(dloss_dgammas + 2 * HW + pix + 1);
+      dlr.y = __ldg(dl_f + pix + 1);
+      dlg.y = __ldg(dl_f + HW + pix + 1);
+      dlb.y = __ldg(dl_f + 2 * HW + pix + 1);
     }
     int wmax = max(cont0, cont1);
 #pragma unroll
@@ -354,7 +362,7 @@ __global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd(
     int W, int H, int gx, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ dloss_dgammas, float *__restrict__ moments, int *__restrict__ work) {
-  draw_bwd_body<false, false>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr,
+  draw_bwd_body<false, false, false>(W, H, gx, 0, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr,
                               moments, nullptr, nullptr, work);
 }
 
@@ -364,7 +372,7 @@ __global__ void __launch_bounds__(128, DRAW_BWD_RGBD_MINBLOCKS) k_draw_bwd_rgbd(
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
     int *__restrict__ work) {
-  draw_bwd_body<true, false>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
+  draw_bwd_body<true, false, false>(W, H, gx, 0, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
                              dloss_dalpha_image, moments, ddepths, nullptr, work);
 }
 
@@ -373,7 +381,7 @@ __global__ void __launch_bounds__(128, DRAW_BWD_ABS_MINBLOCKS) k_draw_bwd_abs(
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     const float *__restrict__ dloss_dgammas, float *__restrict__ moments, float *__restrict__ dus_abs,
     int *__restrict__ work) {
-  draw_bwd_body<false, true>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr,
+  draw_bwd_body<false, true, false>(W, H, gx, 0, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr, nullptr,
                              moments, nullptr, dus_abs, work);
 }
 
@@ -383,8 +391,26 @@ __global__ void __launch_bounds__(128, DRAW_BWD_RGBD_ABS_MINBLOCKS) k_draw_bwd_r
     const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
     const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
     float *__restrict__ dus_abs, int *__restrict__ work) {
-  draw_bwd_body<true, true>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
+  draw_bwd_body<true, true, false>(W, H, gx, 0, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, dloss_ddepth_image,
                             dloss_dalpha_image, moments, ddepths, dus_abs, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_BWD_MINBLOCKS) k_draw_bwd_batch(
+    int W, int H, int gx, int gy, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    const float *__restrict__ dloss_dgammas, float *__restrict__ moments, int *__restrict__ work) {
+  draw_bwd_body<false, false, true>(W, H, gx, gy, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas, nullptr,
+                                    nullptr, moments, nullptr, nullptr, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_BWD_RGBD_MINBLOCKS) k_draw_bwd_rgbd_batch(
+    int W, int H, int gx, int gy, int T, const int32_t *__restrict__ ranges, const Rec *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    const float *__restrict__ dloss_dgammas, const float *__restrict__ dloss_ddepth_image,
+    const float *__restrict__ dloss_dalpha_image, float *__restrict__ moments, float *__restrict__ ddepths,
+    int *__restrict__ work) {
+  draw_bwd_body<true, false, true>(W, H, gx, gy, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
+                                   dloss_ddepth_image, dloss_dalpha_image, moments, ddepths, nullptr, work);
 }
 
 constexpr int MOM = 9;  // floats per moment row
@@ -433,23 +459,34 @@ int launch_draw_backward(int H, int W, int N, const int32_t *ranges, const Rec *
                          const int32_t *contrib, const float *final_tau, const float *dloss_dgammas,
                          const DepthGrads *dg, const float *cinv2ds, float *moments, int *work, float *dloss_dus,
                          float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, bool finalize,
-                         float *dus_abs, cudaStream_t st) {
+                         float *dus_abs, cudaStream_t st, int frames) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0 || N <= 0) return 0;
+  if (frames > 0 && dus_abs != nullptr) return set_arg_error("drawB: no absolute gradients for a batch of frames");
   GSB_CUDA_TRY(cudaMemsetAsync(moments, 0, sizeof(float) * MOM * (size_t)N, st));
   if (dg != nullptr) GSB_CUDA_TRY(cudaMemsetAsync(dg->ddepths, 0, sizeof(float) * (size_t)N, st));
   if (dus_abs != nullptr) GSB_CUDA_TRY(cudaMemsetAsync(dus_abs, 0, sizeof(float) * 2 * (size_t)N, st));
   if (recs != nullptr) {
-    const int T = gx * gy;
+    const int T = gx * gy * (frames > 0 ? frames : 1);
     if (work == nullptr) return set_arg_error("drawB: work area missing");
-    int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);  // tiles with patches
+    // tiles with patches
+    int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st, frames);
     if (rc) return rc;
     int grid = 0;
     const int per_sm = dus_abs != nullptr ? (dg != nullptr ? DRAW_BWD_RGBD_ABS_MINBLOCKS : DRAW_BWD_ABS_MINBLOCKS)
                                           : (dg != nullptr ? DRAW_BWD_RGBD_MINBLOCKS : DRAW_BWD_MINBLOCKS);
     rc = persistent_grid(T, per_sm, grid);
     if (rc) return rc;
-    if (dus_abs != nullptr && dg != nullptr) {
+    if (frames > 0 && dg != nullptr) {
+      ProfScope ps(K_DRAW_BWD_RGBD_BATCH, st);
+      k_draw_bwd_rgbd_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, T, ranges, recs, gsid, contrib, final_tau,
+                                                  dloss_dgammas, dg->dloss_ddepth_image, dg->dloss_dalpha_image,
+                                                  moments, dg->ddepths, work);
+    } else if (frames > 0) {
+      ProfScope ps(K_DRAW_BWD_BATCH, st);
+      k_draw_bwd_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
+                                             moments, work);
+    } else if (dus_abs != nullptr && dg != nullptr) {
       ProfScope ps(K_DRAW_BWD_RGBD_ABS, st);
       k_draw_bwd_rgbd_abs<<<grid, 128, 0, st>>>(W, H, gx, T, ranges, recs, gsid, contrib, final_tau, dloss_dgammas,
                                                 dg->dloss_ddepth_image, dg->dloss_dalpha_image, moments, dg->ddepths,

@@ -28,10 +28,13 @@ namespace gsb {
 // zeros itself with 16-byte stores -- one warp per empty tile -- so the sparse corner of BASELINE config 4
 // (50k Gaussians at 4K: 32 400 tiles, most of them empty) costs one streaming pass over the
 // frame instead of one queue item per 8x8 block.
-__global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, const int32_t *__restrict__ ranges,
-                                                   float *__restrict__ image, int32_t *__restrict__ contrib,
-                                                   float *__restrict__ final_tau, float *__restrict__ depth_image,
-                                                   float *__restrict__ alpha_image, int *__restrict__ work) {
+// BATCH: a batch of frames binned as one tall frame (DESIGN 3.21): tile row r belongs to frame
+// r / gy (gy = tile rows per frame), and its empty tiles are zeroed in that frame's planes.
+template <bool BATCH>
+__device__ __forceinline__ void tile_list_body(int W, int H, int gx, int gy, int T, const int32_t *__restrict__ ranges,
+                                               float *__restrict__ image, int32_t *__restrict__ contrib,
+                                               float *__restrict__ final_tau, float *__restrict__ depth_image,
+                                               float *__restrict__ alpha_image, int *__restrict__ work) {
   __shared__ unsigned s_empty[8];  // per warp: which of its 32 tiles have no patches
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int tile = blockIdx.x * 256 + threadIdx.x;  // phase 1: one thread per tile
@@ -71,16 +74,18 @@ __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, 
       if ((k & 7) != warp) continue;
       const int t = blockIdx.x * 256 + w * 32 + bit;
       if (t >= T) break;
-      const int x0 = (t % gx) * TILE + (lane & 1) * 8, y = (t / gx) * TILE + (lane >> 1);
+      const int x0 = (t % gx) * TILE + (lane & 1) * 8, y = (BATCH ? t / gx % gy : t / gx) * TILE + (lane >> 1);
       if (y >= H || x0 >= W) continue;
-      const size_t pix = (size_t)y * W + x0;
+      const size_t fo = BATCH ? (size_t)(t / gx / gy) * HW : 0;  // BATCH: the tile's frame in every [H,W] plane
+      const size_t pix = fo + (size_t)y * W + x0;
+      float *const image_f = image + 2 * fo;  // pix holds fo; the frame's [3,H,W] planes start at 3 fo
       if ((W & 3) == 0 && x0 + 8 <= W) {  // 8 pixels = two 16-byte stores per plane
         const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-          *reinterpret_cast<float4 *>(image + pix + 4 * h) = z;
-          *reinterpret_cast<float4 *>(image + HW + pix + 4 * h) = z;
-          *reinterpret_cast<float4 *>(image + 2 * HW + pix + 4 * h) = z;
+          *reinterpret_cast<float4 *>(image_f + pix + 4 * h) = z;
+          *reinterpret_cast<float4 *>(image_f + HW + pix + 4 * h) = z;
+          *reinterpret_cast<float4 *>(image_f + 2 * HW + pix + 4 * h) = z;
           *reinterpret_cast<int4 *>(contrib + pix + 4 * h) = make_int4(0, 0, 0, 0);
           *reinterpret_cast<float4 *>(final_tau + pix + 4 * h) = z;
           if (depth_image != nullptr) {  // (the RGB-D frame's D and A planes: zero too)
@@ -90,8 +95,8 @@ __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, 
         }
       } else {
         for (int x = x0; x < min(x0 + 8, W); x++) {
-          const size_t q = (size_t)y * W + x;
-          image[q] = 0.f; image[HW + q] = 0.f; image[2 * HW + q] = 0.f;
+          const size_t q = fo + (size_t)y * W + x;
+          image_f[q] = 0.f; image_f[HW + q] = 0.f; image_f[2 * HW + q] = 0.f;
           contrib[q] = 0; final_tau[q] = 0.f;
           if (depth_image != nullptr) { depth_image[q] = 0.f; alpha_image[q] = 0.f; }
         }
@@ -100,13 +105,32 @@ __global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, 
   }
 }
 
+__global__ void __launch_bounds__(256) k_tile_list(int W, int H, int gx, int T, const int32_t *__restrict__ ranges,
+                                                   float *__restrict__ image, int32_t *__restrict__ contrib,
+                                                   float *__restrict__ final_tau, float *__restrict__ depth_image,
+                                                   float *__restrict__ alpha_image, int *__restrict__ work) {
+  tile_list_body<false>(W, H, gx, 0, T, ranges, image, contrib, final_tau, depth_image, alpha_image, work);
+}
+
+__global__ void __launch_bounds__(256) k_tile_list_batch(int W, int H, int gx, int gy, int T,
+                                                         const int32_t *__restrict__ ranges, float *__restrict__ image,
+                                                         int32_t *__restrict__ contrib, float *__restrict__ final_tau,
+                                                         float *__restrict__ depth_image,
+                                                         float *__restrict__ alpha_image, int *__restrict__ work) {
+  tile_list_body<true>(W, H, gx, gy, T, ranges, image, contrib, final_tau, depth_image, alpha_image, work);
+}
+
 int launch_tile_list(int H, int W, const int32_t *ranges, float *image, int32_t *contrib, float *final_tau,
-                     float *depth_image, float *alpha_image, int *work, cudaStream_t st) {
+                     float *depth_image, float *alpha_image, int *work, cudaStream_t st, int frames) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
-  const int T = gx * gy;
+  const int T = gx * gy * (frames > 0 ? frames : 1);
   GSB_CUDA_TRY(cudaMemsetAsync(work, 0, 2 * sizeof(int), st));
-  k_tile_list<<<(T + 255) / 256, 256, 0, st>>>(W, H, gx, T, ranges, image, contrib,
-                                           final_tau, depth_image, alpha_image, work);
+  if (frames > 0)
+    k_tile_list_batch<<<(T + 255) / 256, 256, 0, st>>>(W, H, gx, gy, T, ranges, image, contrib, final_tau, depth_image,
+                                                       alpha_image, work);
+  else
+    k_tile_list<<<(T + 255) / 256, 256, 0, st>>>(W, H, gx, T, ranges, image, contrib,
+                                             final_tau, depth_image, alpha_image, work);
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -115,8 +139,11 @@ int launch_tile_list(int H, int W, const int32_t *ranges, float *image, int32_t 
 // RGBD: depth and opacity composite like two more colour channels whose per-record values are
 // z = q2.w and 1 -- D = sum w z, A = sum w with the image's weights w = tau alpha' -- two more
 // pair accumulators and two more [H,W] planes.
-template <bool RGBD>
-__device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int2 *__restrict__ ranges,
+// BATCH: the tall frame of a batch (DESIGN 3.21): tile row r is row r - f gy of frame f = r / gy; the
+// pixels are that frame's own coordinates (the records' means are camera-local) and its planes are
+// frame f of image[C,3,H,W], contrib / final_tau / depth / alpha [C,H,W].
+template <bool RGBD, bool BATCH>
+__device__ __forceinline__ void draw_body(int W, int H, int gx, int gy, int T, const int2 *__restrict__ ranges,
                                           const Rec *__restrict__ recs, const int32_t *__restrict__ gsid,
                                           float *__restrict__ image, int32_t *__restrict__ contrib,
                                           float *__restrict__ final_tau, float *__restrict__ depth_image,
@@ -146,12 +173,19 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
     const int len = range.y - range.x;
     if (whole_tile) gather_whole_tile(ring_addr, recs, gsid + range.x, len, lane);
    for (int blk = whole_tile ? 0 : code; blk < (whole_tile ? 4 : code + 1); blk++) {
-    const int tx = tile % gx, ty = tile / gx;
+    int tx = tile % gx, ty = tile / gx;
+    size_t fo = 0;  // BATCH: offset of the tile's frame in every [H,W] plane
+    if (BATCH) {
+      const int f = ty / gy;
+      ty -= f * gy;
+      fo = (size_t)f * HW;
+    }
     const int rx0 = tx * TILE + (blk & 1) * 8, ry0 = ty * TILE + (blk >> 1) * 8;
-    if (rx0 >= W || ry0 >= H) continue;  // block entirely outside the image
+    if (rx0 >= W || ry0 >= H) continue;  // block entirely outside the image (BATCH: or in a pad row)
     const int px = rx0 + 2 * (lane & 3), py = ry0 + (lane >> 2);
     const bool in0 = px < W && py < H, in1 = px + 1 < W && py < H;
-    const size_t pix = (size_t)py * W + px;
+    const size_t pix = fo + (size_t)py * W + px;
+    float *const image_f = image + 2 * fo;  // pix holds fo; the frame's [3,H,W] planes start at 3 fo
 
     float2 tau = p2s(0.f), cr = p2s(0.f), cg = p2s(0.f), cb = p2s(0.f);
     float2 cd = p2s(0.f), ca = p2s(0.f);  // RGBD only: D and A
@@ -232,9 +266,9 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
       walk_drain();
     }
     if (in0 && in1 && vec2) {
-      *reinterpret_cast<float2 *>(image + pix) = cr;
-      *reinterpret_cast<float2 *>(image + HW + pix) = cg;
-      *reinterpret_cast<float2 *>(image + 2 * HW + pix) = cb;
+      *reinterpret_cast<float2 *>(image_f + pix) = cr;
+      *reinterpret_cast<float2 *>(image_f + HW + pix) = cg;
+      *reinterpret_cast<float2 *>(image_f + 2 * HW + pix) = cb;
       *reinterpret_cast<int2 *>(contrib + pix) = make_int2(cont0, cont1);
       *reinterpret_cast<float2 *>(final_tau + pix) = tau;
       if (RGBD) {
@@ -243,12 +277,12 @@ __device__ __forceinline__ void draw_body(int W, int H, int gx, int T, const int
       }
     } else {
       if (in0) {
-        image[pix] = cr.x; image[HW + pix] = cg.x; image[2 * HW + pix] = cb.x;
+        image_f[pix] = cr.x; image_f[HW + pix] = cg.x; image_f[2 * HW + pix] = cb.x;
         contrib[pix] = cont0; final_tau[pix] = tau.x;
         if (RGBD) { depth_image[pix] = cd.x; alpha_image[pix] = ca.x; }
       }
       if (in1) {
-        image[pix + 1] = cr.y; image[HW + pix + 1] = cg.y; image[2 * HW + pix + 1] = cb.y;
+        image_f[pix + 1] = cr.y; image_f[HW + pix + 1] = cg.y; image_f[2 * HW + pix + 1] = cb.y;
         contrib[pix + 1] = cont1; final_tau[pix + 1] = tau.y;
         if (RGBD) { depth_image[pix + 1] = cd.y; alpha_image[pix + 1] = ca.y; }
       }
@@ -265,7 +299,7 @@ __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw(int W, int H, int 
                                                               int32_t *__restrict__ contrib,
                                                               float *__restrict__ final_tau,
                                                               int *__restrict__ work) {
-  draw_body<false>(W, H, gx, T, ranges, recs, gsid, image, contrib, final_tau, nullptr, nullptr, work);
+  draw_body<false, false>(W, H, gx, 0, T, ranges, recs, gsid, image, contrib, final_tau, nullptr, nullptr, work);
 }
 
 __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw_rgbd(int W, int H, int gx, int T,
@@ -278,25 +312,59 @@ __global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw_rgbd(int W, int H,
                                                                    float *__restrict__ depth_image,
                                                                    float *__restrict__ alpha_image,
                                                                    int *__restrict__ work) {
-  draw_body<true>(W, H, gx, T, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image, work);
+  draw_body<true, false>(W, H, gx, 0, T, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                         work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw_batch(int W, int H, int gx, int gy, int T,
+                                                                    const int2 *__restrict__ ranges,
+                                                                    const Rec *__restrict__ recs,
+                                                                    const int32_t *__restrict__ gsid,
+                                                                    float *__restrict__ image,
+                                                                    int32_t *__restrict__ contrib,
+                                                                    float *__restrict__ final_tau,
+                                                                    int *__restrict__ work) {
+  draw_body<false, true>(W, H, gx, gy, T, ranges, recs, gsid, image, contrib, final_tau, nullptr, nullptr, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_MINBLOCKS) k_draw_rgbd_batch(int W, int H, int gx, int gy, int T,
+                                                                         const int2 *__restrict__ ranges,
+                                                                         const Rec *__restrict__ recs,
+                                                                         const int32_t *__restrict__ gsid,
+                                                                         float *__restrict__ image,
+                                                                         int32_t *__restrict__ contrib,
+                                                                         float *__restrict__ final_tau,
+                                                                         float *__restrict__ depth_image,
+                                                                         float *__restrict__ alpha_image,
+                                                                         int *__restrict__ work) {
+  draw_body<true, true>(W, H, gx, gy, T, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                        work);
 }
 
 int launch_draw(int H, int W, const int32_t *ranges, const Rec *recs, const int32_t *gsid, float *image,
                 int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, int *work,
-                cudaStream_t st) {
+                cudaStream_t st, int frames) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0) return 0;
-  const int T = gx * gy;
+  const int T = gx * gy * (frames > 0 ? frames : 1);
   if (work == nullptr) return set_arg_error("draw: work area missing");
   // (k_draw reads `ranges` as int2: the splat entry points only accept an 8-byte aligned
   // patch_range_per_tile, which the binning just wrote)
   // work list (and the zeros of the empty tiles) first; it also clears the item counter
-  int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st);
+  int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st, frames);
   if (rc) return rc;
   int grid = 0;
   rc = persistent_grid(T, DRAW_MINBLOCKS, grid);
   if (rc) return rc;
-  if (depth_image != nullptr) {
+  if (frames > 0 && depth_image != nullptr) {
+    ProfScope ps(K_DRAW_RGBD_BATCH, st);
+    k_draw_rgbd_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, T, reinterpret_cast<const int2 *>(ranges), recs, gsid,
+                                            image, contrib, final_tau, depth_image, alpha_image, work);
+  } else if (frames > 0) {
+    ProfScope ps(K_DRAW_BATCH, st);
+    k_draw_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, image,
+                                       contrib, final_tau, work);
+  } else if (depth_image != nullptr) {
     ProfScope ps(K_DRAW_RGBD, st);
     k_draw_rgbd<<<grid, 128, 0, st>>>(W, H, gx, T, reinterpret_cast<const int2 *>(ranges), recs, gsid, image,
                                       contrib, final_tau, depth_image, alpha_image, work);

@@ -374,6 +374,81 @@ def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, sca
     return grads + (dfeat,) if feat is not None else grads
 
 
+class GSFunctionFusedBatch(torch.autograd.Function):
+    """GSFunctionFused for C cameras in one call (DESIGN 3.21): `apply(pws, shs, alphas, scales, rots,
+    us, cams, filter3d=None)` -> (image[C,3,H,W], mask[C,N]) with image[c] and mask[c] those of
+    camera cams[c].  The cameras share width, height, antialiased and camera_model (else ValueError);
+    each has its own pose, intrinsics and lens coefficients.  us is the [C,N,2] dummy whose gradient
+    is each camera's dL/du, so `DensityController.update_density_info(us.grad[c], mask[c])` works per
+    camera.  The map gradients are the sums over the cameras, taken in one per-Gaussian pass.
+    filter3d: as for GSFunctionFused, applied once per call.  No pose gradient, features, AbsGS or
+    gradient exchange in batch form."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cams, filter3d=None):
+        return _batch_forward(ctx, False, pws, shs, alphas, scales, rots, us, cams, filter3d)
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, _):
+        return _batch_backward(ctx, dloss_dimage)
+
+
+class GSFunctionFusedBatchRGBD(torch.autograd.Function):
+    """GSFunctionFusedBatch with GSFunctionFusedRGBD's planes: -> (image[C,3,H,W], depth[C,H,W],
+    alpha[C,H,W], mask[C,N])"""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cams, filter3d=None):
+        return _batch_forward(ctx, True, pws, shs, alphas, scales, rots, us, cams, filter3d)
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, _):
+        return _batch_backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha)
+
+
+def _batch_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cams, filter3d):
+    from . import ops
+    bc = ops.BatchCameras(cams, pws.device)
+    N = pws.shape[0]
+    if not isinstance(us, torch.Tensor) or tuple(us.shape) != (bc.C, N, 2):
+        raise ValueError("us must be a [C, N, 2] tensor (C = %d, N = %d), got %s"
+                         % (bc.C, N, tuple(getattr(us, "shape", ()))))
+    ctx.filtered = filter3d is not None
+    raw = ()
+    if ctx.filtered:
+        filter3d = filter3d.detach()
+        raw = (scales, alphas, filter3d)
+        scales, alphas = ops.filter3d_apply(scales, alphas, filter3d)
+    pre = ops.preprocess_batch(pws, rots, scales, shs, bc, alphas)
+    us_, cinv2ds, colors, depths, areas, records = pre[:6]
+    drawn = pre[6] if bc.antialiased else alphas  # (with the records the frame reads no alphas)
+    out = ops.splat_batch(bc.height, bc.width, us_, cinv2ds, drawn, depths, colors, areas, records=records,
+                          capacity=True, rgbd=rgbd)
+    ctx.bc = bc
+    ctx.rgbd = rgbd
+    ctx.alpha_shape = alphas.shape
+    ctx.save_for_backward(pws, shs, alphas, drawn, scales, rots, us_, cinv2ds, depths, colors, records, *out[1:5],
+                          *raw)
+    mask = depths > 0.2
+    return (out[0], out[5], out[6], mask) if rgbd else (out[0], mask)
+
+
+def _batch_backward(ctx, dloss_dimage, dloss_ddepth=None, dloss_dalpha=None):
+    from . import ops
+    bc = ctx.bc
+    (pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths, colors, records, contrib, final_tau, ranges, gsid,
+     *raw) = ctx.saved_tensors
+    rb = ops.splatB_batch(bc.height, bc.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau, ranges, gsid,
+                          dloss_dimage, dloss_ddepth if ctx.rgbd else None, dloss_dalpha, records=records)
+    moments, ddepths = rb if ctx.rgbd else (rb, None)
+    dpws, dshs, dscales, drots, dus, dalphas = ops.preprocessB_batch(
+        pws, rots, scales, shs, bc, moments, cinv2ds, dloss_ddepths=ddepths, alphas=alphas if bc.antialiased else None)
+    if ctx.filtered:  # the gradients are those of s', alpha'; the filter's backward runs once, after the batch sum
+        dscales, dalphas = ops.filter3d_backward(*raw, dscales, dalphas, inplace=True)
+    return (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus) + \
+        (None,) * (len(ctx.needs_input_grad) - 6)
+
+
 class GSFunctionFusedFeatures(torch.autograd.Function):
     """GSFunctionFused with per-Gaussian features: `apply(pws, shs, alphas, scales, rots, us, features, cam,
     filter3d=None)` -> (image[3,H,W], feature_map[D,H,W], depths > 0.2) with

@@ -258,50 +258,56 @@ def _check_drawn(H, W, ranges, planes, text):
         raise ValueError("patch_range_per_tile does not match the tile grid")
 
 
-def _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes):
+def _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes, frames=None):
     """the sort workspace for P patch slots (ws_bytes: the family's workspace query) and splat's
-    five outputs, + one plane of each shape in `planes`: float32, or (shape, dtype)"""
-    ws = _bytes(ws_bytes(N, H, W, P), dev)
+    five outputs, + one plane of each shape in `planes`: float32, or (shape, dtype).  frames: None,
+    or the C of a batch: every per-pixel output gets a leading C and the tile ranges C times the rows"""
+    lead = () if frames is None else (frames,)
+    ws = _bytes(ws_bytes(*lead, N, H, W, P), dev)
     typed = [pl if isinstance(pl[-1], torch.dtype) else (pl, torch.float32) for pl in planes]
-    return ws, [torch.empty((3, H, W), dtype=torch.float32, device=dev),
-                torch.empty((H, W), dtype=torch.int32, device=dev),
-                torch.empty((H, W), dtype=torch.float32, device=dev),
-                torch.empty((_tiles(H, W), 2), dtype=torch.int32, device=dev),
+    return ws, [torch.empty(lead + (3, H, W), dtype=torch.float32, device=dev),
+                torch.empty(lead + (H, W), dtype=torch.int32, device=dev),
+                torch.empty(lead + (H, W), dtype=torch.float32, device=dev),
+                torch.empty(((frames or 1) * _tiles(H, W), 2), dtype=torch.int32, device=dev),
                 torch.empty((P,), dtype=torch.int32, device=dev)] + \
-        [torch.empty(shape, dtype=dtype, device=dev) for shape, dtype in typed]
+        [torch.empty(lead + tuple(shape), dtype=dtype, device=dev) for shape, dtype in typed]
 
 
-def _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status):
+def _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status, frames=None):
     """Bins, sorts and draws one frame with the sort sized from the bounds (P_cap, dk_cap) through
     forward = (gsb_splat_forward, _rgbd, _enqueue or gsb_splat_surfel_forward, the pointers of its
-    frame's own inputs).  planes, ws_bytes: as for `_frame_buffers`.
+    frame's own inputs).  planes, ws_bytes, frames: as for `_frame_buffers`.
     -> (False when the frame outgrew a bound, its workspaces, the five outputs with P_cap gsid
     slots + the planes); `status` (pinned int32[4]) receives the status word."""
-    lib, N, dev = _L(), us.shape[0], us.device
-    bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
-    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap, planes, ws_bytes)
+    lib, N, dev = _L(), us.shape[-2], us.device
+    lead = () if frames is None else (frames,)
+    bin_ws = _bytes(lib.gsb_splat_bin_batch_workspace_bytes(frames, N) if frames else
+                    lib.gsb_splat_bin_workspace_bytes(N), dev)
+    ws, out = _frame_buffers(lib, dev, H, W, N, P_cap, planes, ws_bytes, frames)
     entry, inputs = forward
-    rc = entry(H, W, N, *inputs, P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
+    rc = entry(*lead, H, W, N, *inputs, P_cap, dk_cap, _ptr(bin_ws), bin_ws.numel(), _ptr(ws), ws.numel(),
                *[_ptr(o) for o in out[:5]], status.data_ptr(), *[_ptr(o) for o in out[5:]], _stream())
     if rc != GSB_CAPACITY_EXCEEDED:
         _lib.check(rc, lib)
     return rc == 0, (bin_ws, ws), out
 
 
-def _frame(H, W, us, depths, areas, planes, ws_bytes, forward, render, capacity, cap_key):
-    """The one frame driver of `splat`, `splat_rgbd` and `splat_surfel`: bins the frame (MUTATES
-    depths / areas of what touches no tile) and draws it.  planes, ws_bytes: as for
+def _frame(H, W, us, depths, areas, planes, ws_bytes, forward, render, capacity, cap_key, frames=None):
+    """The one frame driver of `splat`, `splat_rgbd`, `splat_surfel` and `splat_batch`: bins the
+    frame (MUTATES depths / areas of what touches no tile) and draws it.  planes, ws_bytes: as for
     `_frame_buffers`; forward, render: (the capacity / the exact entry point, the pointers of the
     frame's own inputs to it).  capacity: size the sort from the bounds learnt for cap_key by the
     previous frame of the same shape; a frame that outgrows them is redone the exact way.
+    frames: None, or the C of a batch (us [C, N, 2]): the *_batch entry points, C in front.
     -> (the sort workspace, its patch slots, the outputs with gsid_per_patch of the frame's P)"""
-    lib, N, dev = _L(), us.shape[0], us.device
+    lib, N, dev = _L(), us.shape[-2], us.device
+    lead = () if frames is None else (frames,)
     if capacity and cap_key in _CAPACITY and N > 0:
         P_cap, dk_cap = _CAPACITY[cap_key]
         status = _STATUS.get(dev.index)
         if status is None:
             status = _STATUS[dev.index] = torch.zeros(4, dtype=torch.int32).pin_memory()
-        ok, (_, ws), out = _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status)
+        ok, (_, ws), out = _capacity_frame(H, W, us, planes, ws_bytes, forward, P_cap, dk_cap, status, frames)
         if ok:
             CAPACITY_STATS["capacity_frames"] += 1
             P, dkmax, _ = _decode_status(status)
@@ -310,18 +316,20 @@ def _frame(H, W, us, depths, areas, planes, ws_bytes, forward, render, capacity,
             return ws, P_cap, out
         CAPACITY_STATS["outgrown"] += 1
         del _CAPACITY[cap_key]  # outgrown: this frame the exact way (the in-place culls are idempotent)
-    bin_ws = _bytes(lib.gsb_splat_bin_workspace_bytes(N), dev)
+    bin_ws = _bytes(lib.gsb_splat_bin_batch_workspace_bytes(frames, N) if frames else
+                    lib.gsb_splat_bin_workspace_bytes(N), dev)
     P, dkmax = C.c_int64(0), C.c_uint32(0)
-    _lib.check(lib.gsb_splat_bin(H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(),
-                                 C.byref(P), C.byref(dkmax), _stream()), lib)
+    _lib.check((lib.gsb_splat_bin_batch if frames else lib.gsb_splat_bin)(
+        *lead, H, W, N, _ptr(us), _ptr(depths), _ptr(areas), _ptr(bin_ws), bin_ws.numel(), C.byref(P),
+        C.byref(dkmax), _stream()), lib)
     P = int(P.value)
-    ws, out = _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes)
+    ws, out = _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes, frames)
     if capacity:
         CAPACITY_STATS["exact_frames"] += 1
         _CAPACITY[cap_key] = _next_capacity(P, dkmax.value)
     entry, inputs = render
-    _lib.check(entry(H, W, N, P, dkmax.value, *inputs, _ptr(bin_ws), _ptr(ws), ws.numel(), *[_ptr(o) for o in out],
-                     _stream()), lib)
+    _lib.check(entry(*lead, H, W, N, P, dkmax.value, *inputs, _ptr(bin_ws), _ptr(ws), ws.numel(),
+                     *[_ptr(o) for o in out], _stream()), lib)
     return ws, P, out
 
 
@@ -539,6 +547,214 @@ def _splatB(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_t
     if not absgrad:
         return out
     return (out if isinstance(out, list) else [out]) + [dabs]
+
+
+# ---------------------------------------------------------------------------------------
+# Batched rendering (extension, DESIGN 3.21): C cameras of one image size, camera model and
+# antialiasing mode in one call.  The per-Gaussian kernels read each Gaussian's rows once for all
+# C cameras; the C frames are binned, sorted and drawn as one tall frame.  Record c N + n is
+# Gaussian n seen by camera c; per-record outputs are [C, N, ...], per-pixel ones [C, ..., H, W].
+BATCH_MAX_CAMERAS = 64     # cameras per call (GSB_BATCH_MAX_CAMERAS)
+BATCH_INTRINSICS_ROW = 8   # fx, fy, cx, cy, k[4] (GSB_BATCH_INTRINSICS_ROW)
+
+
+class BatchCameras:
+    """The cameras of one batch, checked on the host: poses [C, 15] (Rcw row-major, tcw, twc) on the
+    device, intrinsics [C, 8] (fx, fy, cx, cy, k[4]) on the host, and what they share: width,
+    height, antialiased, camera_model.  Cameras that disagree on a shared field are a ValueError."""
+
+    def __init__(self, cams, device):
+        from .gsfunction import camera_model_kwargs
+        cams = list(cams)
+        if not 1 <= len(cams) <= BATCH_MAX_CAMERAS:
+            raise ValueError("a batch takes 1 to %d cameras, got %d" % (BATCH_MAX_CAMERAS, len(cams)))
+        c0 = cams[0]
+        self.width, self.height = int(c0.width), int(c0.height)
+        self.antialiased = bool(getattr(c0, "antialiased", False))
+        self.camera_model = getattr(c0, "camera_model", "pinhole")
+        rows, poses = [], []
+        for k, c in enumerate(cams):
+            shared = (int(c.width), int(c.height), bool(getattr(c, "antialiased", False)),
+                      getattr(c, "camera_model", "pinhole"))
+            if shared != (self.width, self.height, self.antialiased, self.camera_model):
+                raise ValueError("camera %d: the cameras of a batch share width, height, antialiased and "
+                                 "camera_model, got %s and %s" % (k, shared, (self.width, self.height,
+                                                                            self.antialiased, self.camera_model)))
+            _, lk = camera_model_args(**camera_model_kwargs(c))
+            rows.append([float(c.fx), float(c.fy), float(c.cx), float(c.cy)] + list(lk))
+            pose = [torch.as_tensor(t).detach().reshape(-1).to(device=device, dtype=torch.float32)
+                    for t in (c.Rcw, c.tcw, c.twc)]
+            if [t.numel() for t in pose] != [9, 3, 3]:
+                raise ValueError("camera %d: Rcw must have 9, tcw and twc 3 elements" % k)
+            poses.append(torch.cat(pose))
+        self.C = len(cams)
+        self.model_id = _CAMERA_MODEL_ID[self.camera_model]
+        self.poses = torch.stack(poses).contiguous()
+        self.intrinsics = torch.tensor(rows, dtype=torch.float32)
+
+    def args(self):
+        """poses, intrinsics, camera_model, width, height as the batch entry points take them"""
+        return (_ptr(self.poses), self.intrinsics.data_ptr(), self.model_id, float(self.width), float(self.height))
+
+
+def _batch_cams(cams, device):
+    return cams if isinstance(cams, BatchCameras) else BatchCameras(cams, device)
+
+
+def preprocess_batch(pws, rots, scales, shs, cams, alphas):
+    """`preprocess(..., alphas=alphas, antialiased=..., camera_model=...)` for C cameras at once
+    (gsb_preprocess_forward_batch).  cams: a list of `gsfunction.Camera` (or a `BatchCameras`)
+    sharing width, height, antialiased and camera_model.  -> [us[C,N,2], cinv2ds[C,N,3],
+    colors[C,N,3], depths[C,N], areas[C,N,2] int32, records[C N, 12]] + [alphas_eff[C,N]] when
+    antialiased; camera c's rows are the bits `preprocess` gives for camera c alone."""
+    params, N, k = _gaussian_params(pws, rots, scales, shs, torch.zeros(9, device=pws.device),
+                                    torch.zeros(3, device=pws.device), torch.zeros(3, device=pws.device))
+    pws, rots, scales, shs = params[:4]
+    bc = _batch_cams(cams, pws.device)
+    alphas = _per_gaussian(alphas, "alphas", N, pws)
+    Cn = bc.C
+    o = dict(dtype=torch.float32, device=pws.device)
+    us = torch.empty((Cn, N, 2), **o); cinv = torch.empty((Cn, N, 3), **o); col = torch.empty((Cn, N, 3), **o)
+    depths = torch.empty((Cn, N), **o); areas = torch.empty((Cn, N, 2), dtype=torch.int32, device=pws.device)
+    records = torch.empty((Cn * N, 12), **o)
+    alphas_eff = torch.empty((Cn, N), **o) if bc.antialiased else None
+    lib = _L()
+    with torch.cuda.device(pws.device):
+        _lib.check(lib.gsb_preprocess_forward_batch(
+            Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(us), _ptr(cinv), _ptr(col),
+            _ptr(depths), _ptr(areas), _ptr(alphas), _ptr(records), _ptr(alphas_eff), _stream()), lib)
+    out = [us, cinv, col, depths, areas, records]
+    return out + [alphas_eff] if bc.antialiased else out
+
+
+def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddepths=None, alphas=None):
+    """Backward of `preprocess_batch` from the moment rows [C N, 9] of `splatB_batch` and the
+    forward's cinv2ds [C,N,3] (gsb_preprocess_backward_batch): the C cameras' contributions summed
+    in fp32 registers in camera order.  dloss_ddepths [C N]: the RGB-D term; alphas [N]: the raw
+    opacities, required when the cameras are antialiased.
+    -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4], dloss_dus[C,N,2]
+    (per camera), dloss_dalphas[N]]"""
+    params, N, k = _gaussian_params(pws, rots, scales, shs, torch.zeros(9, device=pws.device),
+                                    torch.zeros(3, device=pws.device), torch.zeros(3, device=pws.device))
+    pws, rots, scales, shs = params[:4]
+    bc = _batch_cams(cams, pws.device)
+    Cn = bc.C
+    moments = _chk(moments, "moments", last=9); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3)
+    _same_device(pws, moments, cinv2ds)
+    if moments.numel() != 9 * Cn * N or cinv2ds.numel() != 3 * Cn * N:
+        raise ValueError("moments / cinv2ds must have C N rows")
+    if dloss_ddepths is not None:
+        dloss_ddepths = _per_gaussian(dloss_ddepths, "dloss_ddepths", Cn * N, pws)
+    if bc.antialiased and alphas is None:
+        raise ValueError("antialiased cameras need the raw alphas")
+    alphas = _per_gaussian(alphas, "alphas", N, pws) if bc.antialiased else None
+    o = dict(dtype=torch.float32, device=pws.device)
+    gpw = torch.empty((N, 3), **o); gsh = torch.empty((N, 3 * k), **o)
+    gs = torch.empty((N, 3), **o); gq = torch.empty((N, 4), **o)
+    dus = torch.empty((Cn, N, 2), **o); dal = torch.empty((N,), **o)
+    lib = _L()
+    with torch.cuda.device(pws.device):
+        _lib.check(lib.gsb_preprocess_backward_batch(
+            Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(moments), _ptr(cinv2ds),
+            _ptr(dloss_ddepths), _ptr(alphas), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(dus), _ptr(dal),
+            _stream()), lib)
+    return [gpw, gsh, gs, gq, dus, dal]
+
+
+def _batch_frame_inputs(us, cinv2ds, alphas, depths, colors, records):
+    """the [C, N, ...] inputs of a batch frame, checked -> (C, N, the inputs contiguous).  alphas:
+    [C, N] (the drawn opacities per camera), or [N] when records are given (then not read)."""
+    us = _chk(us, "us", last=2, ndim=3)
+    Cn, N = us.shape[0], us.shape[1]
+    cinv2ds = _chk(cinv2ds, "cinv2ds", last=3, ndim=3); colors = _chk(colors, "colors", last=3, ndim=3)
+    depths = _chk(depths, "depths"); alphas = _chk(alphas, "alphas")
+    _same_device(us, cinv2ds, colors, depths, alphas)
+    if not (tuple(cinv2ds.shape[:2]) == (Cn, N) and tuple(colors.shape[:2]) == (Cn, N)
+            and depths.numel() == Cn * N):
+        raise ValueError("batch frame inputs disagree on C, N")
+    if alphas.numel() != Cn * N and not (records is not None and alphas.numel() == N):
+        raise ValueError("alphas must be [C, N] (or [N] with records)")
+    if records is not None:
+        records = _chk(records, "records", last=12, ndim=2)
+        _same_device(us, records)
+        if records.shape[0] != Cn * N:
+            raise ValueError("records must be [C N, 12]")
+    return Cn, N, us, cinv2ds, alphas, depths, colors, records
+
+
+def splat_batch(height, width, us, cinv2ds, alphas, depths, colors, areas, records=None, capacity=False,
+                rgbd=False):
+    """`splat` (or, rgbd, `splat_rgbd`) of C frames of height x width at once, binned and drawn as
+    one tall frame (gsb_splat_render_batch / gsb_splat_forward_batch and their _rgbd forms).
+    Inputs are `preprocess_batch`'s [C, N, ...] outputs; MUTATES depths / areas of records that
+    touch no tile.  -> [image[C,3,H,W], contrib[C,H,W] i32, final_tau[C,H,W],
+    patch_range_per_tile[C T, 2] i32, gsid_per_patch[P] i32 (record ids c N + n)]
+    + [depth[C,H,W], alpha[C,H,W]] with rgbd.  Frame c is the single frame of camera c, bit for bit.
+    records, capacity: as for `splat`."""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    Cn, N, us, cinv2ds, alphas, depths, colors, records = _batch_frame_inputs(us, cinv2ds, alphas, depths, colors,
+                                                                              records)
+    areas = _chk(areas, "areas", dtype=torch.int32, last=2, ndim=3)
+    if tuple(areas.shape[:2]) != (Cn, N):
+        raise ValueError("areas must be [C, N, 2]")
+    if records is None and alphas.numel() != Cn * N:
+        raise ValueError("alphas must be [C, N] without records")
+    dev = us.device
+    lib = _L()
+    own = [_ptr(t) for t in (us, cinv2ds, alphas, depths, colors)]
+    sfx = "_rgbd" if rgbd else ""
+    forward = (getattr(lib, "gsb_splat_forward_batch" + sfx), own + [_ptr(areas), _ptr(records)])
+    render = (getattr(lib, "gsb_splat_render_batch" + sfx), own + [_ptr(records)])
+    with torch.cuda.device(dev):
+        _, _, out = _frame(H, W, us, depths, areas, [(H, W)] * 2 if rgbd else [], lib.gsb_splat_batch_workspace_bytes,
+                           forward, render, capacity, ("batch", dev.index, Cn, H, W, N), frames=Cn)
+    return out
+
+
+def splatB_batch(height, width, us, cinv2ds, alphas, depths, colors, contrib, final_tau, patch_range_per_tile,
+                 gsid_per_patch, dloss_dgammas, dloss_ddepth=None, dloss_dalpha=None, records=None):
+    """Backward of `splat_batch` (gsb_splat_backward_batch, or _rgbd when dloss_ddepth[C,H,W] and
+    dloss_dalpha[C,H,W] are given): dloss_dgammas [C,3,H,W] -> the moment rows [C N, 9] for
+    `preprocessB_batch` (+ dloss_ddepths [C N] with RGB-D).  records: the forward's [C N, 12], or
+    None (re-packed from us, cinv2ds, alphas [C,N], colors and depths)."""
+    rgbd = dloss_ddepth is not None
+    H, W = int(height), int(width)
+    Cn, N, us, cinv2ds, alphas, depths, colors, records = _batch_frame_inputs(us, cinv2ds, alphas, depths, colors,
+                                                                              records)
+    contrib = _chk(contrib, "contrib", dtype=torch.int32); final_tau = _chk(final_tau, "final_tau")
+    ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
+    gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
+    dl = _chk(dloss_dgammas, "dloss_dgammas")
+    _same_device(us, contrib, final_tau, ranges, gsid, dl)
+    if any(t.numel() != c * Cn * H * W for t, c in ((contrib, 1), (final_tau, 1), (dl, 3))):
+        raise ValueError("contrib / final_tau / dloss_dgammas do not match C x height x width")
+    if ranges.shape[0] != Cn * _tiles(H, W):
+        raise ValueError("patch_range_per_tile does not match the batch's tile grid")
+    if rgbd:
+        dloss_ddepth = _chk(dloss_ddepth, "dloss_ddepth"); dloss_dalpha = _chk(dloss_dalpha, "dloss_dalpha")
+        _same_device(us, dloss_ddepth, dloss_dalpha)
+        if dloss_ddepth.numel() != Cn * H * W or dloss_dalpha.numel() != Cn * H * W:
+            raise ValueError("dloss_ddepth / dloss_dalpha do not match C x height x width")
+    P = gsid.numel()
+    dev = us.device
+    moments = torch.empty((Cn * N, 9), dtype=torch.float32, device=dev)
+    ddepths = torch.empty((Cn * N,), dtype=torch.float32, device=dev) if rgbd else None
+    lib = _L()
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_splat_backward_batch_workspace_bytes(Cn, N, H, W, 0 if records is not None else P), dev)
+        if rgbd:
+            _lib.check(lib.gsb_splat_backward_batch_rgbd(
+                Cn, H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
+                _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dloss_ddepth), _ptr(dloss_dalpha),
+                _ptr(records), _ptr(ws), ws.numel(), _ptr(moments), _ptr(ddepths), _stream()), lib)
+        else:
+            _lib.check(lib.gsb_splat_backward_batch(
+                Cn, H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(contrib), _ptr(final_tau),
+                _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(records), _ptr(ws), ws.numel(), _ptr(moments), _stream()),
+                lib)
+    return [moments, ddepths] if rgbd else moments
 
 
 # ---------------------------------------------------------------------------------------

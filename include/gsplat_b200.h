@@ -866,6 +866,89 @@ size_t gsb_bilagrid_tv_workspace_bytes(int M, int L, int Y, int X);
 int gsb_bilagrid_tv(int M, int L, int Y, int X, const float *grids, float *tv_out, float *dloss_dgrids, void *ws,
                     size_t ws_bytes, gsb_stream_t stream);
 
+/* ---- batched rendering (DESIGN 3.21): C cameras in one call.  The cameras share width, height,
+ * the camera model and (in the callers) antialiasing; each has its own pose, intrinsics and lens
+ * coefficients.  The entry points mirror the single-camera ones with C in front, so one frame
+ * driver serves both; the batch's records are c N + n (Gaussian n seen by camera c), its
+ * per-record arrays [C, N, ...] and its per-pixel planes [C, ..., H, W].  Frame c occupies tile
+ * rows [c gy, (c + 1) gy), gy = ceil(H / 16), of one ceil(W / 16) x C gy tall frame; its tile
+ * ranges are [C gx gy, 2] and gsid_per_patch holds record ids.  Errors before any launch: C < 1,
+ * C N >= 2^31, C gy > GSB_MAX_GRID_TILES, 2^30 patches or more, and, for the per-Gaussian entry
+ * points, C > GSB_BATCH_MAX_CAMERAS (the intrinsics travel in kernel parameter memory) and every
+ * check gsb_preprocess_forward_model makes of each camera.
+ *
+ * poses: [C, 15] floats in device memory, Rcw (row-major 9), tcw (3), twc (3) per camera.
+ * intrinsics: [C, GSB_BATCH_INTRINSICS_ROW] floats in HOST memory, fx, fy, cx, cy, k[4] per camera
+ * (k as gsb_camera_model.k).  camera_model: GSB_CAMERA_*.
+ * gsb_preprocess_forward_batch: gsb_preprocess_forward_model's outputs per camera into
+ * us[C,N,2], cinv2ds[C,N,3], colors[C,N,3], depths[C,N], areas[C,N,2], records[C N] (alphas[N] and
+ * records required), alphas_eff[C,N] (nullable: antialiasing when set); for camera c the same bits
+ * as the single-camera call.
+ * gsb_preprocess_backward_batch: from the moment rows moments[C N, 9] of gsb_splat_backward_batch
+ * and the forward's cinv2ds (dloss_ddepths [C N] nullable: RGB-D; alphas [N] nullable: antialiasing)
+ * the four gradients summed over the cameras in fp32 in camera order, dloss_dus_out[C,N,2] per
+ * camera and dloss_dalphas_out[N] summed. */
+#define GSB_BATCH_MAX_CAMERAS 64
+#define GSB_BATCH_INTRINSICS_ROW 8
+int gsb_preprocess_forward_batch(int C, int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                 const float *shs, const float *poses, const float *intrinsics, int camera_model,
+                                 float width, float height, float *us, float *cinv2ds, float *colors, float *depths,
+                                 int32_t *areas, const float *alphas, void *records, float *alphas_eff,
+                                 gsb_stream_t stream);
+int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                  const float *shs, const float *poses, const float *intrinsics, int camera_model,
+                                  float width, float height, const float *moments, const float *cinv2ds,
+                                  const float *dloss_ddepths, const float *alphas, float *dloss_dpws,
+                                  float *dloss_dshs, float *dloss_dscales, float *dloss_drots, float *dloss_dus_out,
+                                  float *dloss_dalphas_out, gsb_stream_t stream);
+/* Phase 1 of the tall frame (gsb_splat_bin with C): record c N + n's rectangle is the single
+ * frame's, clamped to frame c's tile rows, then moved down by c gy rows; N = per camera.  The batch's
+ * workspace queries return 0 for C < 1, N < 0 or C N >= 2^31, which its entry points refuse. */
+size_t gsb_splat_bin_batch_workspace_bytes(int C, int N);
+int gsb_splat_bin_batch(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
+                        size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host, gsb_stream_t stream);
+size_t gsb_splat_batch_workspace_bytes(int C, int N, int H, int W, int64_t P);
+size_t gsb_splat_batch_records_offset(int C, int N, int H, int W, int64_t P);
+/* gsb_splat_render{,_rgbd} and gsb_splat_forward{,_rgbd} (the capacity path) of the batch */
+int gsb_splat_render_batch(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                           const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                           const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
+                           int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                           int32_t *gsid_per_patch, gsb_stream_t stream);
+int gsb_splat_render_batch_rgbd(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                                const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
+                                const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes,
+                                float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                                int32_t *gsid_per_patch, float *depth_image, float *alpha_image, gsb_stream_t stream);
+int gsb_splat_forward_batch(int C, int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
+                            float *depths, const float *colors, int32_t *areas, const void *packed_records,
+                            int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
+                            size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                            int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
+                            gsb_stream_t stream);
+int gsb_splat_forward_batch_rgbd(int C, int H, int W, int N, const float *us, const float *cinv2ds,
+                                 const float *alphas, float *depths, const float *colors, int32_t *areas,
+                                 const void *packed_records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                                 size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                                 float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                                 uint32_t *status_host, float *depth_image, float *alpha_image, gsb_stream_t stream);
+/* The batch's backward rasterizer: always the raw moment rows moments_out[C N, 9] (and, RGB-D,
+ * dloss_ddepths[C N]) for gsb_preprocess_backward_batch; packed_records: the forward's, or NULL
+ * (re-packed into ws) */
+size_t gsb_splat_backward_batch_workspace_bytes(int C, int N, int H, int W, int64_t P);
+int gsb_splat_backward_batch(int C, int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                             const float *alphas, const float *colors, const int32_t *contrib, const float *final_tau,
+                             const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                             const float *dloss_dgammas, const void *packed_records, void *ws, size_t ws_bytes,
+                             float *moments_out, gsb_stream_t stream);
+int gsb_splat_backward_batch_rgbd(int C, int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
+                                  const float *alphas, const float *colors, const float *depths,
+                                  const int32_t *contrib, const float *final_tau, const int32_t *patch_range_per_tile,
+                                  const int32_t *gsid_per_patch, const float *dloss_dgammas,
+                                  const float *dloss_ddepth_image, const float *dloss_dalpha_image,
+                                  const void *packed_records, void *ws, size_t ws_bytes, float *moments_out,
+                                  float *dloss_ddepths, gsb_stream_t stream);
+
 /* ---- launch accounting and optional per-kernel timing (no reference counterpart; used by
  * bench.py for `gpu_launches` and the roofline's live CUDA-event kernel durations).
  * Kernel ids 0..gsb_profile_kernels()-1, names from gsb_profile_kernel_name().
