@@ -915,6 +915,41 @@ int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, c
 // The batch's workspace queries answer 0 for what its entry points refuse: C < 1, N < 0, C N >= 2^31
 static bool batch_records_ok(int C, int N) { return C >= 1 && N >= 0 && (int64_t)C * N < ((int64_t)1 << 31); }
 
+size_t gsb_preprocess_backward_batch_pose_workspace_bytes(int C, int N) {
+  return batch_records_ok(C, N) ? batch_pose_workspace_bytes(C, N) : 0;
+}
+
+// gsb_preprocess_backward_batch plus the C camera gradients (DESIGN 3.22): the per-Gaussian outputs all
+// set (pose and map) or all NULL (pose only)
+int gsb_preprocess_backward_batch_pose(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                       const float *scales, const float *shs, const float *poses,
+                                       const float *intrinsics, int camera_model, float width, float height,
+                                       const float *moments, const float *cinv2ds, const float *dloss_ddepths,
+                                       const float *alphas, float *dloss_dpws, float *dloss_dshs, float *dloss_dscales,
+                                       float *dloss_drots, float *dloss_dus_out, float *dloss_dalphas_out,
+                                       float *dloss_dposes, void *ws, size_t ws_bytes, gsb_stream_t stream) {
+  const char *who = "preprocessB_batch_pose";
+  BatchCams bc;
+  BatchScene b{};
+  if (int rc = batch_scene(who, C, N, sh_dim3, camera_model, intrinsics, width, height, bc, b)) return rc;
+  if (N > 0 && !(pws && rots && scales && shs && poses && moments && cinv2ds))
+    return arg_error(who, "null pointer");
+  const bool all = dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots && dloss_dus_out && dloss_dalphas_out;
+  const bool none = !dloss_dpws && !dloss_dshs && !dloss_dscales && !dloss_drots && !dloss_dus_out &&
+                    !dloss_dalphas_out;
+  if (N > 0 && !all && !none) return arg_error(who, "per-Gaussian outputs must be all set or all null");
+  if (dloss_dposes == nullptr) return arg_error(who, "null dloss_dposes");
+  if (!aligned(ws, 16)) return arg_error(who, "workspace misaligned");
+  const size_t need = batch_pose_workspace_bytes(C, N);
+  if (!(ws_bytes >= need && (need == 0 || ws != nullptr))) return arg_error(who, "workspace too small");
+  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
+  const PoseOut po{dloss_dposes, static_cast<float *>(ws)};
+  // (N == 0 launches no per-Gaussian pass: only the C rows of zeros)
+  return launch_preprocess_bwd_batch(b, {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
+                                         dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, &po},
+                                     (cudaStream_t)stream);
+}
+
 size_t gsb_splat_bin_batch_workspace_bytes(int C, int N) { return batch_records_ok(C, N) ? bin_layout(C * N).bytes : 0; }
 
 int gsb_splat_bin_batch(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,

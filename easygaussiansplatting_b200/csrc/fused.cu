@@ -258,8 +258,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
 // one CTA in a fixed order (thread t takes rows t, t + PR, ...; then a fixed shuffle tree and the
 // warps in index order), so the result is the same bits on every run.  nrows == 0 writes zeros.
 constexpr int PR = 512;
-__global__ void __launch_bounds__(PR) k_pose_reduce(int nrows, const float *__restrict__ part,
-                                                    float *__restrict__ gcam) {
+__device__ __forceinline__ void pose_reduce(int nrows, const float *__restrict__ part, float *__restrict__ gcam) {
   const int tid = threadIdx.x;
   double acc[15];
 #pragma unroll
@@ -291,6 +290,15 @@ __global__ void __launch_bounds__(PR) k_pose_reduce(int nrows, const float *__re
     for (int w = 0; w < PR / 32; w++) t += red[w][tid];
     gcam[tid] = (float)t;
   }
+}
+__global__ void __launch_bounds__(PR) k_pose_reduce(int nrows, const float *__restrict__ part,
+                                                    float *__restrict__ gcam) {
+  pose_reduce(nrows, part, gcam);
+}
+// the batch's: CTA c sums camera c's nrows rows of part[C][nrows][16] into gcam[c][15]
+__global__ void __launch_bounds__(PR) k_pose_reduce_batch(int nrows, const float *__restrict__ part,
+                                                          float *__restrict__ gcam) {
+  pose_reduce(nrows, part + (size_t)blockIdx.x * nrows * 16, gcam + (size_t)blockIdx.x * 15);
 }
 
 // dL/dsh of one Gaussian summed over V views from the views' dL/dcolor:
@@ -469,6 +477,78 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd_batch(
   }
 }
 
+// The camera gradients of the batch (DESIGN 3.22): k_preprocess_bwd_batch's reads and
+// k_preprocess_bwd<..., POSE>'s math per camera.  Camera c's 15 contributions are summed over the
+// CTA's Gaussians with that kernel's tree (warp shuffles, then the 4 warps in index order, fp32):
+// each warp's sum waits in red[c][warp] (dynamic shared memory, C x 256 B) and one barrier at the end
+// hands the C rows to the CTA, which writes row part[c][blockIdx.x][16] (summed by
+// k_pose_reduce_batch).  Nothing per Gaussian is written.  Every thread runs the camera loop (the
+// shuffles take the whole warp); a thread past N contributes zeros.  (The minimum of 1 CTA per SM in
+// the launch bounds lets ptxas keep the values that live across the lens's and the divisions'
+// slow-path calls in registers: without it a third of the instantiations save 1-3 of them on the stack.
+// They use 51-96 registers either way.)
+template <int K3, bool DEPTH, bool AA, int MODEL>
+__global__ void __launch_bounds__(PG, 1) k_preprocess_bwd_batch_pose(
+    int C, int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
+    const float *__restrict__ shs, const float *__restrict__ poses, const __grid_constant__ BatchCams bc,
+    const float *__restrict__ moments, const float *__restrict__ cinv2ds, const float *__restrict__ g_depths,
+    const float *__restrict__ alphas, float *__restrict__ part) {
+  constexpr int KS = 3 * K3;
+  constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
+  __shared__ float sm[SMF];
+  extern __shared__ float red[];  // [C][PG / 32][16]
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * PG;
+  const int nv = min(PG, (int)(N - base));
+  const bool valid = tid < nv;
+  float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
+  load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);
+  tile_fetch<KS>(shs, base, nv, sm, tid);
+  __syncthreads();
+  const long long i = base + tid;
+  const float al = AA && valid ? __ldg(alphas + i) : 0.f;
+  for (int c = 0; c < C; c++) {
+    float gcam[15];
+#pragma unroll
+    for (int e = 0; e < 15; e++) gcam[e] = 0.f;
+    if (valid) {
+      const long long o = (long long)c * N + i;
+      float m[9];
+#pragma unroll
+      for (int k = 0; k < 9; k++) m[k] = __ldg(moments + 9 * o + k);
+      const float A = __ldg(cinv2ds + 3 * o), B = __ldg(cinv2ds + 3 * o + 1), Cc = __ldg(cinv2ds + 3 * o + 2);
+      const bool none = (m[0] == 0.f) && (m[1] == 0.f);  // as k_preprocess_bwd's MOM form
+      const float gu[2] = {none ? 0.f : -(A * m[0] + B * m[1]), none ? 0.f : -(B * m[0] + Cc * m[1])};
+      const float gci[3] = {-0.5f * m[2], -m[3], -0.5f * m[4]}, gcol[3] = {m[6], m[7], m[8]};
+      const float gz = DEPTH ? __ldg(g_depths + o) : 0.f;
+      const pg::Cam cam = batch_cam(poses, bc, c, MODEL == pg::FISHEYE || MODEL == pg::OPENCV);
+      float xpw[3], xq[4], xs[3], xsh[KS];  // the per-Gaussian outputs: not written by this form
+      pg::backward_one<K3, DEPTH, true, AA, MODEL>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam,
+                                                   m[5], al);
+    }
+#pragma unroll
+    for (int e = 0; e < 15; e++) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) gcam[e] += __shfl_down_sync(0xffffffffu, gcam[e], o);
+    }
+    if ((tid & 31) == 0) {
+      float *r = red + ((size_t)c * (PG / 32) + (tid >> 5)) * 16;
+#pragma unroll
+      for (int e = 0; e < 15; e++) r[e] = gcam[e];
+    }
+  }
+  __syncthreads();
+  for (int k = tid; k < C * 16; k += PG) {
+    const int c = k >> 4, e = k & 15;
+    float v = 0.f;
+    if (e < 15) {
+#pragma unroll
+      for (int w = 0; w < PG / 32; w++) v += red[((size_t)c * (PG / 32) + w) * 16 + e];
+    }
+    part[((size_t)c * gridDim.x + blockIdx.x) * 16 + e] = v;
+  }
+}
+
 #define GSB_DISPATCH_K3(k3, CALL)                                           \
   switch (k3) {                                                             \
     case 1: { constexpr int K3 = 1; CALL; } break;                          \
@@ -620,24 +700,44 @@ int launch_preprocess_fwd_batch(const BatchScene &b, const FusedFwd &f, cudaStre
 }
 
 int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStream_t st) {
-  if (b.N <= 0) return 0;
-  const int nb = (b.N + PG - 1) / PG;
+  const PoseOut *po = g.po;
+  if (b.N <= 0 && po == nullptr) return 0;
+  const int nb = b.N > 0 ? (b.N + PG - 1) / PG : 0;
   const CamLens model{b.model, {0.f, 0.f, 0.f, 0.f}, 1.f};
+  // one pass: k_preprocess_bwd_batch_pose (pose) or k_preprocess_bwd_batch, DEPTH and AA set by which
+  // optional inputs are given
+  const auto pass = [&](auto pose) {
+    return with_model(&model, "preprocessB_batch: unknown camera model", [&](auto mdl) {
+      return with_flags(
+          [&](auto depth, auto aa) -> int {
+            constexpr bool DEPTH = decltype(depth)::value, AA = decltype(aa)::value;
+            constexpr int MODEL = decltype(mdl)::value;
+            if constexpr (decltype(pose)::value) {
+              const size_t red = (size_t)b.C * (PG / 32) * 16 * sizeof(float);
+              GSB_DISPATCH_K3(b.k3, (k_preprocess_bwd_batch_pose<K3, DEPTH, AA, MODEL><<<nb, PG, red, st>>>(
+                                        b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses, *b.cams, g.moments,
+                                        g.cinv2ds, g.g_depths, g.alphas, po->part)));
+            } else {
+              GSB_DISPATCH_K3(b.k3, (k_preprocess_bwd_batch<K3, DEPTH, AA, MODEL><<<nb, PG, 0, st>>>(
+                                        b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses, *b.cams, g.moments,
+                                        g.cinv2ds, g.g_depths, g.alphas, g.dus_out, g.dalphas_out, g.g_pws, g.g_shs,
+                                        g.g_scales, g.g_rots)));
+            }
+            return 0;
+          },
+          g.g_depths != nullptr, g.alphas != nullptr);
+    });
+  };
   ProfScope ps(K_PRE_BWD_BATCH, st);
-  const int rc = with_model(&model, "preprocessB_batch: unknown camera model", [&](auto mdl) {
-    return with_flags(
-        [&](auto depth, auto aa) -> int {
-          constexpr bool DEPTH = decltype(depth)::value, AA = decltype(aa)::value;
-          constexpr int MODEL = decltype(mdl)::value;
-          GSB_DISPATCH_K3(b.k3, (k_preprocess_bwd_batch<K3, DEPTH, AA, MODEL><<<nb, PG, 0, st>>>(
-                                    b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses, *b.cams, g.moments,
-                                    g.cinv2ds, g.g_depths, g.alphas, g.dus_out, g.dalphas_out, g.g_pws, g.g_shs,
-                                    g.g_scales, g.g_rots)));
-          return 0;
-        },
-        g.g_depths != nullptr, g.alphas != nullptr);
-  });
-  if (rc) return rc;
+  // the camera gradients first (DESIGN 3.22); then, unless g_pws is NULL (pose only), the per-Gaussian
+  // gradients from the kernel without the camera terms, so that they are the same bits either way
+  if (po != nullptr) {
+    if (nb > 0)
+      if (int rc = pass(std::true_type{})) return rc;
+    k_pose_reduce_batch<<<b.C, PR, 0, st>>>(nb, po->part, po->gcam);
+  }
+  if (nb > 0 && (po == nullptr || g.g_pws != nullptr))
+    if (int rc = pass(std::false_type{})) return rc;
   GSB_CUDA_TRY(cudaGetLastError());
   return 0;
 }

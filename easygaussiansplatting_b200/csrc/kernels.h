@@ -128,11 +128,16 @@ struct BatchScene {
 // f: the [C, N, ...] outputs (alphas [N] and recs [C N] required; alphas_eff [C, N]: antialiasing)
 int launch_preprocess_fwd_batch(const BatchScene &b, const FusedFwd &f, cudaStream_t st);
 // moments [C N, 9], cinv2ds [C N, 3], g_depths NULL or [C N] (RGB-D), alphas NULL or the raw
-// opacities [N] (antialiasing); outputs dus_out [C N, 2], dalphas_out [N] and the four gradients
+// opacities [N] (antialiasing); outputs dus_out [C N, 2], dalphas_out [N] and the four gradients.
+// po: NULL, or also the camera gradients (DESIGN 3.22): gcam [C, 15], part C ceil(N/128) rows of 16
+// floats (16-byte aligned), in a pass of its own; then g_pws == NULL (with the other per-Gaussian
+// outputs NULL) writes only those.
 struct BatchBwd {
   const float *moments, *cinv2ds, *g_depths, *alphas;
   float *dus_out, *dalphas_out, *g_pws, *g_shs, *g_scales, *g_rots;
+  const PoseOut *po;
 };
+constexpr size_t batch_pose_workspace_bytes(int C, int N) { return (size_t)C * pose_workspace_bytes(N); }
 int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)

@@ -381,8 +381,8 @@ class GSFunctionFusedBatch(torch.autograd.Function):
     each has its own pose, intrinsics and lens coefficients.  us is the [C,N,2] dummy whose gradient
     is each camera's dL/du, so `DensityController.update_density_info(us.grad[c], mask[c])` works per
     camera.  The map gradients are the sums over the cameras, taken in one per-Gaussian pass.
-    filter3d: as for GSFunctionFused, applied once per call.  No pose gradient, features, AbsGS or
-    gradient exchange in batch form."""
+    filter3d: as for GSFunctionFused, applied once per call.  Poses with gradients: GSFunctionFusedBatchPose
+    (DESIGN 3.22).  No features, AbsGS or gradient exchange in batch form."""
 
     @staticmethod
     def forward(ctx, pws, shs, alphas, scales, rots, us, cams, filter3d=None):
@@ -406,9 +406,61 @@ class GSFunctionFusedBatchRGBD(torch.autograd.Function):
         return _batch_backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha)
 
 
-def _batch_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cams, filter3d):
+class GSFunctionFusedBatchPose(torch.autograd.Function):
+    """GSFunctionFusedBatch with differentiable camera poses (DESIGN 3.22):
+    `apply(pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None)` -> (image[C,3,H,W],
+    mask[C,N]).  Rcws[C,3,3], tcws[C,3], twcs[C,3] replace the cameras' own poses (cams supply size,
+    intrinsics, lens, camera model and antialiasing) and get dL/dRcw, dL/dtcw, dL/dtwc per camera as
+    independent inputs, as GSFunctionFusedPose's do: a caller who builds twcs from the other two has
+    autograd chain it.  What runs follows ctx.needs_input_grad: only the poses -> the pose-only pass (a
+    frozen map: tracking several frames, or the poses' step of windowed bundle adjustment); no pose ->
+    exactly GSFunctionFusedBatch's backward; both -> the pose pass, then that backward.  filter3d as for
+    GSFunctionFusedBatch."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None):
+        return _batch_forward(ctx, False, pws, shs, alphas, scales, rots, us, cams, filter3d, (Rcws, tcws, twcs))
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, _):
+        return _batch_backward(ctx, dloss_dimage)
+
+
+class GSFunctionFusedBatchRGBDPose(torch.autograd.Function):
+    """GSFunctionFusedBatchRGBD with differentiable camera poses, as GSFunctionFusedBatchPose:
+    `apply(pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None)` -> (image[C,3,H,W],
+    depth[C,H,W], alpha[C,H,W], mask[C,N]).  The depth planes' gradients reach the poses through
+    z = (Rcw pw + tcw)[2]."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None):
+        return _batch_forward(ctx, True, pws, shs, alphas, scales, rots, us, cams, filter3d, (Rcws, tcws, twcs))
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, _):
+        return _batch_backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha)
+
+
+def _batch_poses(pose, C, dev):
+    """(Rcws, tcws, twcs) -> the [C, 15] pose rows the batch kernels read (a detached copy)"""
+    shapes = ((C, 3, 3), (C, 3), (C, 3))
+    for name, x, s in zip(("Rcws", "tcws", "twcs"), pose, shapes):
+        if not isinstance(x, torch.Tensor) or x.numel() != s[0] * (9 if len(s) == 3 else 3) or x.shape[0] != C:
+            raise ValueError("%s must be a %s tensor, got %s" % (name, list(s), tuple(getattr(x, "shape", ()))))
+        if x.device != dev:
+            raise ValueError("%s must be on the device of pws (%s), got %s" % (name, dev, x.device))
+    return torch.cat([x.detach().reshape(C, -1).to(torch.float32) for x in pose], 1).contiguous()
+
+
+def _batch_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cams, filter3d, pose=None):
+    """the forward of the batch classes; pose: None (the cameras' own poses) or (Rcws, tcws, twcs)"""
     from . import ops
-    bc = ops.BatchCameras(cams, pws.device)
+    ctx.pose = pose is not None
+    if ctx.pose:
+        bc = ops.BatchCameras(cams, pws.device, poses=_batch_poses(pose, len(cams), pws.device))
+        ctx.cam_shapes = tuple(x.shape for x in pose)
+    else:
+        bc = ops.BatchCameras(cams, pws.device)
     N = pws.shape[0]
     if not isinstance(us, torch.Tensor) or tuple(us.shape) != (bc.C, N, 2):
         raise ValueError("us must be a [C, N, 2] tensor (C = %d, N = %d), got %s"
@@ -441,12 +493,23 @@ def _batch_backward(ctx, dloss_dimage, dloss_ddepth=None, dloss_dalpha=None):
     rb = ops.splatB_batch(bc.height, bc.width, us, cinv2ds, drawn, depths, colors, contrib, final_tau, ranges, gsid,
                           dloss_dimage, dloss_ddepth if ctx.rgbd else None, dloss_dalpha, records=records)
     moments, ddepths = rb if ctx.rgbd else (rb, None)
-    dpws, dshs, dscales, drots, dus, dalphas = ops.preprocessB_batch(
-        pws, rots, scales, shs, bc, moments, cinv2ds, dloss_ddepths=ddepths, alphas=alphas if bc.antialiased else None)
-    if ctx.filtered:  # the gradients are those of s', alpha'; the filter's backward runs once, after the batch sum
-        dscales, dalphas = ops.filter3d_backward(*raw, dscales, dalphas, inplace=True)
-    return (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus) + \
-        (None,) * (len(ctx.needs_input_grad) - 6)
+    need_map = any(ctx.needs_input_grad[:6])
+    need_cam = ctx.pose and any(ctx.needs_input_grad[6:9])
+    out = ops.preprocessB_batch(pws, rots, scales, shs, bc, moments, cinv2ds, dloss_ddepths=ddepths,
+                                alphas=alphas if bc.antialiased else None, camera_grad=need_cam,
+                                pose_only=need_cam and not need_map)
+    if need_map:
+        dpws, dshs, dscales, drots, dus, dalphas = out[:6]
+        if ctx.filtered:  # the gradients are those of s', alpha'; the filter's backward runs once, after the batch sum
+            dscales, dalphas = ops.filter3d_backward(*raw, dscales, dalphas, inplace=True)
+        grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
+    else:
+        grads = (None,) * 6
+    if need_cam:
+        grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
+    elif ctx.pose:
+        grads += (None,) * 3
+    return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
 class GSFunctionFusedFeatures(torch.autograd.Function):

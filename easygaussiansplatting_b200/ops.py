@@ -561,9 +561,11 @@ BATCH_INTRINSICS_ROW = 8   # fx, fy, cx, cy, k[4] (GSB_BATCH_INTRINSICS_ROW)
 class BatchCameras:
     """The cameras of one batch, checked on the host: poses [C, 15] (Rcw row-major, tcw, twc) on the
     device, intrinsics [C, 8] (fx, fy, cx, cy, k[4]) on the host, and what they share: width,
-    height, antialiased, camera_model.  Cameras that disagree on a shared field are a ValueError."""
+    height, antialiased, camera_model.  Cameras that disagree on a shared field are a ValueError.
+    poses: None, or a [C, 15] float32 tensor on `device` that replaces the cameras' own Rcw, tcw, twc
+    (DESIGN 3.22: the poses being optimised; read as a constant, never copied to the host)."""
 
-    def __init__(self, cams, device):
+    def __init__(self, cams, device, poses=None):
         from .gsfunction import camera_model_kwargs
         cams = list(cams)
         if not 1 <= len(cams) <= BATCH_MAX_CAMERAS:
@@ -572,7 +574,7 @@ class BatchCameras:
         self.width, self.height = int(c0.width), int(c0.height)
         self.antialiased = bool(getattr(c0, "antialiased", False))
         self.camera_model = getattr(c0, "camera_model", "pinhole")
-        rows, poses = [], []
+        rows, own = [], []
         for k, c in enumerate(cams):
             shared = (int(c.width), int(c.height), bool(getattr(c, "antialiased", False)),
                       getattr(c, "camera_model", "pinhole"))
@@ -582,14 +584,25 @@ class BatchCameras:
                                                                             self.antialiased, self.camera_model)))
             _, lk = camera_model_args(**camera_model_kwargs(c))
             rows.append([float(c.fx), float(c.fy), float(c.cx), float(c.cy)] + list(lk))
+            if poses is not None:
+                continue
             pose = [torch.as_tensor(t).detach().reshape(-1).to(device=device, dtype=torch.float32)
                     for t in (c.Rcw, c.tcw, c.twc)]
             if [t.numel() for t in pose] != [9, 3, 3]:
                 raise ValueError("camera %d: Rcw must have 9, tcw and twc 3 elements" % k)
-            poses.append(torch.cat(pose))
+            own.append(torch.cat(pose))
         self.C = len(cams)
         self.model_id = _CAMERA_MODEL_ID[self.camera_model]
-        self.poses = torch.stack(poses).contiguous()
+        if poses is None:
+            self.poses = torch.stack(own).contiguous()
+        else:
+            if not isinstance(poses, torch.Tensor) or tuple(poses.shape) != (self.C, 15) or \
+                    poses.dtype != torch.float32:
+                raise ValueError("poses must be a [C, 15] float32 tensor (C = %d), got %s"
+                                 % (self.C, tuple(getattr(poses, "shape", ()))))
+            if poses.device != torch.device(device):
+                raise ValueError("poses must be on %s, got %s" % (device, poses.device))
+            self.poses = poses.detach().contiguous()
         self.intrinsics = torch.tensor(rows, dtype=torch.float32)
 
     def args(self):
@@ -627,13 +640,21 @@ def preprocess_batch(pws, rots, scales, shs, cams, alphas):
     return out + [alphas_eff] if bc.antialiased else out
 
 
-def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddepths=None, alphas=None):
+def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddepths=None, alphas=None,
+                      camera_grad=False, pose_only=False):
     """Backward of `preprocess_batch` from the moment rows [C N, 9] of `splatB_batch` and the
     forward's cinv2ds [C,N,3] (gsb_preprocess_backward_batch): the C cameras' contributions summed
     in fp32 registers in camera order.  dloss_ddepths [C N]: the RGB-D term; alphas [N]: the raw
     opacities, required when the cameras are antialiased.
     -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4], dloss_dus[C,N,2]
-    (per camera), dloss_dalphas[N]]"""
+    (per camera), dloss_dalphas[N]]
+    camera_grad (DESIGN 3.22, gsb_preprocess_backward_batch_pose): one more output follows, the
+    camera gradients (dRcws[C,3,3], dtcws[C,3], dtwcs[C,3]) -- views of one [C, 15] tensor; row c is
+    what `preprocessB(..., camera_grad=True)` gives for camera c alone.  The per-Gaussian outputs are
+    the same bits as without it.  pose_only (with camera_grad): the map is frozen; the six
+    per-Gaussian outputs are not computed and come back as None."""
+    if pose_only and not camera_grad:
+        raise ValueError("pose_only=True needs camera_grad=True")
     params, N, k = _gaussian_params(pws, rots, scales, shs, torch.zeros(9, device=pws.device),
                                     torch.zeros(3, device=pws.device), torch.zeros(3, device=pws.device))
     pws, rots, scales, shs = params[:4]
@@ -649,16 +670,27 @@ def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddep
         raise ValueError("antialiased cameras need the raw alphas")
     alphas = _per_gaussian(alphas, "alphas", N, pws) if bc.antialiased else None
     o = dict(dtype=torch.float32, device=pws.device)
-    gpw = torch.empty((N, 3), **o); gsh = torch.empty((N, 3 * k), **o)
-    gs = torch.empty((N, 3), **o); gq = torch.empty((N, 4), **o)
-    dus = torch.empty((Cn, N, 2), **o); dal = torch.empty((N,), **o)
+    if pose_only:
+        gpw = gsh = gs = gq = dus = dal = None
+    else:
+        gpw = torch.empty((N, 3), **o); gsh = torch.empty((N, 3 * k), **o)
+        gs = torch.empty((N, 3), **o); gq = torch.empty((N, 4), **o)
+        dus = torch.empty((Cn, N, 2), **o); dal = torch.empty((N,), **o)
     lib = _L()
     with torch.cuda.device(pws.device):
-        _lib.check(lib.gsb_preprocess_backward_batch(
-            Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(moments), _ptr(cinv2ds),
-            _ptr(dloss_ddepths), _ptr(alphas), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(dus), _ptr(dal),
-            _stream()), lib)
-    return [gpw, gsh, gs, gq, dus, dal]
+        args = (Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(moments), _ptr(cinv2ds),
+                _ptr(dloss_ddepths), _ptr(alphas), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(dus), _ptr(dal))
+        if camera_grad:
+            gcam = torch.empty((Cn, 15), **o)
+            ws_bytes = int(lib.gsb_preprocess_backward_batch_pose_workspace_bytes(Cn, N))
+            ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
+            _lib.check(lib.gsb_preprocess_backward_batch_pose(*args, _ptr(gcam), _ptr(ws), ws_bytes, _stream()), lib)
+        else:
+            _lib.check(lib.gsb_preprocess_backward_batch(*args, _stream()), lib)
+    out = [gpw, gsh, gs, gq, dus, dal]
+    if camera_grad:
+        out.append((gcam[:, :9].view(Cn, 3, 3), gcam[:, 9:12], gcam[:, 12:15]))
+    return out
 
 
 def _batch_frame_inputs(us, cinv2ds, alphas, depths, colors, records):

@@ -901,6 +901,26 @@ int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, c
                                   const float *dloss_ddepths, const float *alphas, float *dloss_dpws,
                                   float *dloss_dshs, float *dloss_dscales, float *dloss_drots, float *dloss_dus_out,
                                   float *dloss_dalphas_out, gsb_stream_t stream);
+/* The camera gradients of the batch (DESIGN 3.22; pose refinement, windowed bundle adjustment, tracking
+ * several frames).  gsb_preprocess_backward_batch's arguments plus dloss_dposes[C, 15]: per camera
+ * dL/dRcw (row-major 9), dL/dtcw (3), dL/dtwc (3), as gsb_preprocess_backward_pose gives for that
+ * camera alone (Rcw, tcw, twc independent inputs; intrinsics not differentiated).  The per-Gaussian
+ * outputs are all set -- then they are gsb_preprocess_backward_batch's, bit for bit (the same kernel
+ * writes them, after a pass that computes the camera gradients) -- or all NULL: pose only, for a
+ * frozen map; nothing per Gaussian is written.  ws: caller-owned, 16-byte aligned, at least
+ * gsb_preprocess_backward_batch_pose_workspace_bytes(C, N) = C ceil(N / 128) 64 bytes (0 for what the
+ * entry point refuses).  Each camera's CTA partial sums are added in a fixed order in fp64, without
+ * atomics: the same inputs give the same bits on every run.  N = 0 writes C rows of zeros.  Errors
+ * before any launch: those of gsb_preprocess_backward_batch, a NULL dloss_dposes, a workspace too
+ * small or misaligned, and per-Gaussian outputs partly NULL. */
+size_t gsb_preprocess_backward_batch_pose_workspace_bytes(int C, int N);
+int gsb_preprocess_backward_batch_pose(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                       const float *scales, const float *shs, const float *poses,
+                                       const float *intrinsics, int camera_model, float width, float height,
+                                       const float *moments, const float *cinv2ds, const float *dloss_ddepths,
+                                       const float *alphas, float *dloss_dpws, float *dloss_dshs, float *dloss_dscales,
+                                       float *dloss_drots, float *dloss_dus_out, float *dloss_dalphas_out,
+                                       float *dloss_dposes, void *ws, size_t ws_bytes, gsb_stream_t stream);
 /* Phase 1 of the tall frame (gsb_splat_bin with C): record c N + n's rectangle is the single
  * frame's, clamped to frame c's tile rows, then moved down by c gy rows; N = per camera.  The batch's
  * workspace queries return 0 for C < 1, N < 0 or C N >= 2^31, which its entry points refuse. */
