@@ -497,31 +497,59 @@ static bool grid_fits(int H, int W) {
          ((int64_t)H + GSB_TILE - 1) / GSB_TILE <= GSB_MAX_GRID_TILES;
 }
 
-// The checks of a frame every entry point that bins makes.  bin_ws holds uint2 rectangles and
-// 8-byte look-back descriptors (gsb_splat_render does not pass its size: SIZE_MAX).
-static int check_frame(int H, int W, int N, const void *bin_ws, size_t bin_ws_bytes) {
-  GSB_REQUIRE(N >= 0 && H > 0 && W > 0, "splat: bad N/H/W");
-  GSB_REQUIRE(grid_fits(H, W), "splat: more than 65535 tiles in a row or column");
-  GSB_REQUIRE(aligned(bin_ws, 16), "splat: bin_ws misaligned");
-  GSB_REQUIRE(bin_ws_bytes >= bin_layout(N).bytes, "splat: bin workspace too small");
+// The frame cores below take `frames`: 0 for one camera, or the C >= 1 cameras of a batch (DESIGN
+// 3.21), binned and drawn as one tall frame of their C N records.  A batch entry point passes its C
+// through batch_frames, so that a C < 1 reaches check_frame as -1 and is refused there.
+static int batch_frames(int C) { return C >= 1 ? C : -1; }
+
+// the frame a core bins, sorts and draws: the single frame, or the batch's tall frame
+struct Tall {
+  int H, N;
+};
+static Tall tall_frame(int frames, int H, int N) {
+  return frames > 0 ? Tall{batch_height(frames, H), frames * N} : Tall{H, N};
+}
+
+static int launch_bin_frames(int frames, int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                             void *bin_ws, const BinLayout &L, cudaStream_t st) {
+  return frames > 0 ? launch_bin_batch(frames, H, W, N, us, depths, areas, bin_ws, L, st)
+                    : launch_bin(H, W, N, us, depths, areas, bin_ws, L, st);
+}
+
+// The checks of a frame every entry point that bins makes; `who` prefixes the error texts.  A batch
+// also needs record ids c N + n that fit int32, and a tall frame of C gy tile rows that fits the
+// rectangles' 16-bit fields.  bin_ws holds uint2 rectangles and 8-byte look-back descriptors of the
+// frame's records (the entry points that do not pass its size pass SIZE_MAX).
+static int check_frame(const char *who, int frames, int H, int W, int N, const void *bin_ws, size_t bin_ws_bytes) {
+  if (frames < 0) return arg_error(who, "C < 1");
+  if (!(N >= 0 && H > 0 && W > 0)) return arg_error(who, "bad N/H/W");
+  if ((int64_t)frames * N >= ((int64_t)1 << 31)) return arg_error(who, "C N >= 2^31 records");
+  if (!grid_fits(H, W) || (int64_t)frames * ((H + GSB_TILE - 1) / GSB_TILE) > GSB_MAX_GRID_TILES)
+    return arg_error(who, frames > 0 ? "more than 65535 tiles in a row or in the C frames' column"
+                                     : "more than 65535 tiles in a row or column");
+  if (!aligned(bin_ws, 16)) return arg_error(who, "bin_ws misaligned");
+  if (bin_ws_bytes < bin_layout(tall_frame(frames, H, N).N).bytes) return arg_error(who, "bin workspace too small");
   return 0;
 }
 
-// The batch's own checks (DESIGN 3.21): C >= 1 frames, record ids c N + n that fit int32, and a
-// tall frame of C gy tile rows that fits the rectangles' 16-bit fields
-static int check_batch(const char *who, int C, int H, int W, int N) {
-  if (C < 1) return arg_error(who, "C < 1");
-  if (!(N >= 0 && H > 0 && W > 0)) return arg_error(who, "bad N/H/W");
-  if ((int64_t)C * N >= ((int64_t)1 << 31)) return arg_error(who, "C N >= 2^31 records");
-  if (!grid_fits(H, W) || (int64_t)C * ((H + GSB_TILE - 1) / GSB_TILE) > GSB_MAX_GRID_TILES)
-    return arg_error(who, "more than 65535 tiles in a row or in the C frames' column");
-  return 0;
-}
-// check_frame of a batch: the bin workspace holds the C N records
-static int check_frame_batch(const char *who, int C, int H, int W, int N, const void *bin_ws, size_t bin_ws_bytes) {
-  if (int rc = check_batch(who, C, H, W, N)) return rc;
-  if (!aligned(bin_ws, 16)) return arg_error(who, "bin_ws misaligned");
-  if (bin_ws_bytes < bin_layout(C * N).bytes) return arg_error(who, "bin workspace too small");
+// gsb_splat_bin{,_batch}: the frame's binning, its patch count and largest depth key read back
+static int splat_bin(const char *who, int frames, int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                     void *bin_ws, size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host,
+                     gsb_stream_t stream) {
+  if (int rc = check_frame(who, frames, H, W, N, bin_ws, bin_ws_bytes)) return rc;
+  if (!(P_host != nullptr && bin_ws != nullptr)) return arg_error(who, "null workspace / P_host");
+  if (N > 0 && !(us && depths && areas)) return arg_error(who, "null pointer");
+  const BinLayout L = bin_layout(tall_frame(frames, H, N).N);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = launch_bin_frames(frames, H, W, N, us, depths, areas, bin_ws, L, st)) return rc;
+  uint32_t total[3] = {0, 0, 0};  // [patch count, largest depth key, flags]
+  GSB_CUDA_TRY(cudaMemcpyAsync(total, static_cast<char *>(bin_ws) + L.total, 3 * sizeof(uint32_t),
+                               cudaMemcpyDeviceToHost, st));
+  GSB_CUDA_TRY(cudaStreamSynchronize(st));
+  if ((total[2] & GSB_STATUS_TOO_MANY_PATCHES) != 0 || total[0] >= (1u << 30))
+    return arg_error(who, "more than 2^30 patches");
+  *P_host = (int64_t)total[0];
+  if (depth_key_max_host) *depth_key_max_host = total[1];
   return 0;
 }
 
@@ -529,22 +557,7 @@ size_t gsb_splat_bin_workspace_bytes(int N) { return bin_layout(N).bytes; }
 
 int gsb_splat_bin(int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
                   size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host, gsb_stream_t stream) {
-  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
-  if (rc) return rc;
-  GSB_REQUIRE(P_host != nullptr && bin_ws != nullptr, "splat: null workspace / P_host");
-  GSB_REQUIRE(N == 0 || (us && depths && areas), "splat: null pointer");
-  const BinLayout L = bin_layout(N);
-  cudaStream_t st = (cudaStream_t)stream;
-  rc = launch_bin(H, W, N, us, depths, areas, bin_ws, L, st);
-  if (rc) return rc;
-  uint32_t total[3] = {0, 0, 0};  // [patch count, largest depth key, flags]
-  GSB_CUDA_TRY(cudaMemcpyAsync(total, static_cast<char *>(bin_ws) + L.total, 3 * sizeof(uint32_t),
-                               cudaMemcpyDeviceToHost, st));
-  GSB_CUDA_TRY(cudaStreamSynchronize(st));
-  GSB_REQUIRE((total[2] & GSB_STATUS_TOO_MANY_PATCHES) == 0 && total[0] < (1u << 30), "splat: more than 2^30 patches");
-  *P_host = (int64_t)total[0];
-  if (depth_key_max_host) *depth_key_max_host = total[1];
-  return 0;
+  return splat_bin("splat", 0, H, W, N, us, depths, areas, bin_ws, bin_ws_bytes, P_host, depth_key_max_host, stream);
 }
 
 size_t gsb_splat_records_offset(int N, int H, int W, int64_t P) { return sort_layout(N, H, W, P).recs; }
@@ -603,21 +616,18 @@ static int render_frame(const char *who, int H, int W, int N, int64_t P, uint32_
   if (int rc = draw.check()) return rc;
   // 64-bit keys at ws + 0, records gathered 16 bytes at a time (the layout's offsets are 256-B multiples)
   if (!aligned(ws, 16)) return arg_error(who, "ws misaligned");
-  // frames > 0: a batch binned as one tall frame of the C N records (DESIGN 3.21); its sort is the
-  // single frame's at the tall frame's height
-  const int Ht = frames > 0 ? batch_height(frames, H) : H, Nt = frames > 0 ? frames * N : N;
-  const SortLayout SL = sort_layout(Nt, Ht, W, P);
+  // a batch's sort is the single frame's at the tall frame's height
+  const Tall t = tall_frame(frames, H, N);
+  const SortLayout SL = sort_layout(t.N, t.H, W, P);
   if (!(ws != nullptr && ws_bytes >= SL.bytes)) return arg_error(who, "workspace too small");
-  const BinLayout BL = bin_layout(Nt);
-  int rc = !sr ? 0
-               : frames > 0 ? launch_bin_batch(frames, H, W, N, us, depths, areas, bin_ws, BL, st)
-                            : launch_bin(H, W, N, us, depths, areas, bin_ws, BL, st);
+  const BinLayout BL = bin_layout(t.N);
+  int rc = sr ? launch_bin_frames(frames, H, W, N, us, depths, areas, bin_ws, BL, st) : 0;
   if (rc) return rc;
-  rc = launch_sort_and_pack(Ht, W, Nt, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
+  rc = launch_sort_and_pack(t.H, W, t.N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, bin_ws, BL, ws, SL,
                             o.ranges, o.gsid, pack, sr, st);
   if (rc) return rc;
   char *b = static_cast<char *>(ws);
-  return draw.draw(H, W, Nt, P, o, b + SL.recs, reinterpret_cast<int *>(b + SL.counters), st);
+  return draw.draw(H, W, t.N, P, o, b + SL.recs, reinterpret_cast<int *>(b + SL.counters), st);
 }
 
 // The status event of the capacity path, one per host thread
@@ -650,21 +660,23 @@ static int capacity_wait(const char *who, int64_t P_cap, uint32_t *status_host, 
 
 }  // extern "C++"
 
-static int splat_render_impl(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
-                             const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
-                             const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
-                             int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
-                             int32_t *gsid_per_patch, float *depth_image, float *alpha_image, gsb_stream_t stream) {
-  int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
-  if (rc) return rc;
-  GSB_REQUIRE(P >= 0, "splat: bad P");
-  GSB_REQUIRE(P == 0 || (us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch),
-              "splat: null pointer");
+// gsb_splat_render{,_rgbd} and their batch forms: a frame binned by gsb_splat_bin{,_batch}
+static int splat_render(const char *who, int frames, int H, int W, int N, int64_t P, uint32_t depth_key_max,
+                        const float *us, const float *cinv2ds, const float *alphas, const float *depths,
+                        const float *colors, const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes,
+                        float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                        int32_t *gsid_per_patch, float *depth_image, float *alpha_image, gsb_stream_t stream) {
+  if (int rc = check_frame(who, frames, H, W, N, bin_ws, SIZE_MAX)) return rc;
+  if (P < 0) return arg_error(who, "bad P");
+  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
+  if (P > 0 && !(us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch))
+    return arg_error(who, "null pointer");
   // (without `sr` nothing is binned: depths and bin_ws are only read)
-  return render_frame("splat", H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors,
+  return render_frame(who, H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors,
                       nullptr, packed_records == nullptr, const_cast<void *>(bin_ws), ws, ws_bytes,
                       {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
-                      ColourDraw{packed_records, depth_image, alpha_image}, nullptr, (cudaStream_t)stream);
+                      ColourDraw{packed_records, depth_image, alpha_image, frames}, nullptr, (cudaStream_t)stream,
+                      frames);
 }
 
 int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
@@ -672,9 +684,9 @@ int gsb_splat_render(int H, int W, int N, int64_t P, uint32_t depth_key_max, con
                      const void *packed_records, const void *bin_ws,
                      void *ws, size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                      int32_t *patch_range_per_tile, int32_t *gsid_per_patch, gsb_stream_t stream) {
-  return splat_render_impl(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, packed_records, bin_ws, ws,
-                           ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, nullptr, nullptr,
-                           stream);
+  return splat_render("splat", 0, H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, packed_records,
+                      bin_ws, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, nullptr,
+                      nullptr, stream);
 }
 
 int gsb_splat_render_rgbd(int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
@@ -683,27 +695,31 @@ int gsb_splat_render_rgbd(int H, int W, int N, int64_t P, uint32_t depth_key_max
                           int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
                           float *depth_image, float *alpha_image, gsb_stream_t stream) {
   GSB_REQUIRE(depth_image && alpha_image, "splat_rgbd: null depth_image / alpha_image");
-  return splat_render_impl(H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, packed_records, bin_ws, ws,
-                           ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch, depth_image,
-                           alpha_image, stream);
+  return splat_render("splat", 0, H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors, packed_records,
+                      bin_ws, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                      depth_image, alpha_image, stream);
 }
 
-static int splat_forward_impl(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
-                              float *depths, const float *colors, int32_t *areas, const void *packed_records,
-                              int64_t P_cap, uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
-                              size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
-                              int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
-                              float *depth_image, float *alpha_image, gsb_stream_t stream, bool wait) {
-  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
-  if (rc) return rc;
-  GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_forward: bad P_cap");
-  GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_forward: null pointer");
-  GSB_REQUIRE(N == 0 || (us && cinv2ds && alphas && depths && colors && areas), "splat_forward: null pointer");
-  return capacity_wait("splat", P_cap, status_host, wait, [&](const StatusRead *sr) {
-    return render_frame("splat", H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas,
+// gsb_splat_forward{,_rgbd,_enqueue} and the batch forms: the capacity path.  `who` prefixes the
+// frame's error texts and `fwd` those of the capacity checks; `wait` as capacity_wait's.
+static int splat_forward(const char *who, const char *fwd, int frames, int H, int W, int N, const float *us,
+                         const float *cinv2ds, const float *alphas, float *depths, const float *colors, int32_t *areas,
+                         const void *packed_records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                         size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                         float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                         uint32_t *status_host, float *depth_image, float *alpha_image, gsb_stream_t stream,
+                         bool wait) {
+  if (int rc = check_frame(who, frames, H, W, N, bin_ws, bin_ws_bytes)) return rc;
+  if (!(P_cap > 0 && P_cap < ((int64_t)1 << 30)))
+    return arg_error(fwd, frames > 0 ? "bad P_cap (2^30 patches or more)" : "bad P_cap");
+  if (!(gsid_per_patch && status_host && bin_ws)) return arg_error(fwd, "null pointer");
+  if (N > 0 && !(us && cinv2ds && alphas && depths && colors && areas)) return arg_error(fwd, "null pointer");
+  return capacity_wait(who, P_cap, status_host, wait, [&](const StatusRead *sr) {
+    return render_frame(who, H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas,
                         packed_records == nullptr, bin_ws, ws, ws_bytes,
                         {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
-                        ColourDraw{packed_records, depth_image, alpha_image}, sr, (cudaStream_t)stream);
+                        ColourDraw{packed_records, depth_image, alpha_image, frames}, sr, (cudaStream_t)stream,
+                        frames);
   });
 }
 
@@ -713,9 +729,9 @@ int gsb_splat_forward(int H, int W, int N, const float *us, const float *cinv2ds
                       size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                       int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                       gsb_stream_t stream) {
-  return splat_forward_impl(H, W, N, us, cinv2ds, alphas, depths, colors, areas, packed_records, P_cap, depth_key_cap,
-                            bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
-                            gsid_per_patch, status_host, nullptr, nullptr, stream, true);
+  return splat_forward("splat", "splat_forward", 0, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
+                       packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib,
+                       final_tau, patch_range_per_tile, gsid_per_patch, status_host, nullptr, nullptr, stream, true);
 }
 
 int gsb_splat_forward_rgbd(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -725,9 +741,10 @@ int gsb_splat_forward_rgbd(int H, int W, int N, const float *us, const float *ci
                            int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                            float *depth_image, float *alpha_image, gsb_stream_t stream) {
   GSB_REQUIRE(depth_image && alpha_image, "splat_forward_rgbd: null depth_image / alpha_image");
-  return splat_forward_impl(H, W, N, us, cinv2ds, alphas, depths, colors, areas, packed_records, P_cap, depth_key_cap,
-                            bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
-                            gsid_per_patch, status_host, depth_image, alpha_image, stream, true);
+  return splat_forward("splat", "splat_forward", 0, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
+                       packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib,
+                       final_tau, patch_range_per_tile, gsid_per_patch, status_host, depth_image, alpha_image, stream,
+                       true);
 }
 
 int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -736,54 +753,66 @@ int gsb_splat_forward_enqueue(int H, int W, int N, const float *us, const float 
                               size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                               int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                               gsb_stream_t stream) {
-  return splat_forward_impl(H, W, N, us, cinv2ds, alphas, depths, colors, areas, packed_records, P_cap, depth_key_cap,
-                            bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
-                            gsid_per_patch, status_host, nullptr, nullptr, stream, false);
+  return splat_forward("splat", "splat_forward", 0, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
+                       packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib,
+                       final_tau, patch_range_per_tile, gsid_per_patch, status_host, nullptr, nullptr, stream, false);
 }
 
 // (a ws at any address: the size is the split from the worst start, 255 bytes short of a 256-B boundary)
 size_t gsb_splat_backward_workspace_bytes(int N, int H, int W, int64_t P) { return bwd_layout(N, H, W, P, 1).bytes; }
 
-// gsb_splat_backward and, with dg, its RGB-D form (depths: the re-pack's depth words)
-static int splat_backward_impl(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
-                               const float *alphas, const float *colors, const float *depths, const int32_t *contrib,
-                               const float *final_tau, const int32_t *patch_range_per_tile,
-                               const int32_t *gsid_per_patch, const float *dloss_dgammas, const DepthGrads *dg,
-                               const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
-                               float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
-                               float *dloss_dus_abs, gsb_stream_t stream) {
-  GSB_REQUIRE(N >= 0 && H > 0 && W > 0 && P >= 0, "splatB: bad N/H/W/P");
-  GSB_REQUIRE(N == 0 || moments_out || (dloss_dus && dloss_dcinv2ds && dloss_dalphas && dloss_dcolors),
-              "splatB: null output");
+// gsb_splat_backward, its RGB-D (dg; depths: the re-pack's depth words) and AbsGS forms, and the batch
+// forms: the moment rows into moments_out, or (one frame only) with moments_out NULL finalised into
+// dloss_dus .. dloss_dcolors.  The records are packed_records or re-packed into ws.
+static int splat_backward(const char *who, int frames, int H, int W, int N, int64_t P, const float *us,
+                          const float *cinv2ds, const float *alphas, const float *colors, const float *depths,
+                          const int32_t *contrib, const float *final_tau, const int32_t *patch_range_per_tile,
+                          const int32_t *gsid_per_patch, const float *dloss_dgammas, const DepthGrads *dg,
+                          const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus,
+                          float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors, float *moments_out,
+                          float *dloss_dus_abs, gsb_stream_t stream) {
+  if (frames != 0) {
+    if (int rc = check_frame(who, frames, H, W, N, nullptr, SIZE_MAX)) return rc;
+    if (P < 0) return arg_error(who, "bad P");
+  } else {
+    if (!(N >= 0 && H > 0 && W > 0 && P >= 0)) return arg_error(who, "bad N/H/W/P");
+    if (!grid_fits(H, W)) return arg_error(who, "more than 65535 tiles in a row or column");
+  }
+  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
+  // (a batch has only the moment rows)
+  if (N > 0 && !(moments_out || (dloss_dus && dloss_dcinv2ds && dloss_dalphas && dloss_dcolors)))
+    return arg_error(who, frames != 0 ? "null pointer" : "null output");
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) return 0;
-  GSB_REQUIRE(cinv2ds && ws, "splatB: null pointer");
+  if (!(cinv2ds && ws)) return arg_error(who, "null pointer");
   // with the forward's records handed in, the workspace only has to hold the moment rows
+  const Tall t = tall_frame(frames, H, N);
   const int64_t P_ws = packed_records != nullptr ? 0 : P;
-  GSB_REQUIRE(ws_bytes >= gsb_splat_backward_workspace_bytes(N, H, W, P_ws), "splatB: workspace too small");
+  if (ws_bytes < bwd_layout(t.N, t.H, W, P_ws, 1).bytes) return arg_error(who, "workspace too small");
   char *b = static_cast<char *>(ws);
-  const BwdLayout L = bwd_layout(N, H, W, P_ws, reinterpret_cast<uintptr_t>(ws));
+  const BwdLayout L = bwd_layout(t.N, t.H, W, P_ws, reinterpret_cast<uintptr_t>(ws));
   Rec *recs = reinterpret_cast<Rec *>(b + L.recs);
   float *moments = moments_out != nullptr ? moments_out : reinterpret_cast<float *>(b + L.moments);
   int *work = reinterpret_cast<int *>(b + L.work);
   if (P > 0) {
-    GSB_REQUIRE(us && alphas && colors && contrib && final_tau && patch_range_per_tile && gsid_per_patch &&
-                    dloss_dgammas,
-                "splatB: null pointer");
-    GSB_REQUIRE(dg == nullptr || (depths && dg->dloss_ddepth_image && dg->dloss_dalpha_image),
-                "splatB_rgbd: null pointer");
+    if (!(us && alphas && colors && contrib && final_tau && patch_range_per_tile && gsid_per_patch && dloss_dgammas))
+      return arg_error(who, "null pointer");
+    // (the one-frame RGB-D entry points check dloss_ddepths themselves)
+    if (dg != nullptr && !(depths && dg->dloss_ddepth_image && dg->dloss_dalpha_image && dg->ddepths))
+      return arg_error(frames != 0 ? who : "splatB_rgbd", "null pointer");
+    if (!aligned(packed_records, 16)) return arg_error(who, "packed_records misaligned");
     if (packed_records != nullptr) {  // the forward's record stream is still valid: skip the re-pack
-      GSB_REQUIRE(aligned(packed_records, 16), "splatB: packed_records misaligned");
       recs = const_cast<Rec *>(static_cast<const Rec *>(packed_records));
-    } else {
-      int rc = launch_pack_only(N, nullptr, us, cinv2ds, alphas, colors, depths, recs, st);
-      if (rc) return rc;
+    } else if (int rc = launch_pack_only(t.N, nullptr, us, cinv2ds, alphas, colors, depths, recs, st)) {
+      return rc;
     }
+  } else if (dg != nullptr && dg->ddepths == nullptr) {
+    return arg_error(who, "null pointer");
   }
   // P == 0: nothing was drawn; the zeroed moment rows finalise to all-zero gradients
-  return launch_draw_backward(H, W, N, patch_range_per_tile, P > 0 ? recs : nullptr, gsid_per_patch, contrib, final_tau,
-                              dloss_dgammas, dg, cinv2ds, moments, work, dloss_dus, dloss_dcinv2ds, dloss_dalphas,
-                              dloss_dcolors, moments_out == nullptr, dloss_dus_abs, st);
+  return launch_draw_backward(H, W, t.N, patch_range_per_tile, P > 0 ? recs : nullptr, gsid_per_patch, contrib,
+                              final_tau, dloss_dgammas, dg, cinv2ds, moments, work, dloss_dus, dloss_dcinv2ds,
+                              dloss_dalphas, dloss_dcolors, moments_out == nullptr, dloss_dus_abs, st, frames);
 }
 
 int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -793,10 +822,9 @@ int gsb_splat_backward(int H, int W, int N, int64_t P, const float *us, const fl
                        const void *packed_records, void *ws, size_t ws_bytes, float *dloss_dus, float *dloss_dcinv2ds, float *dloss_dalphas,
                        float *dloss_dcolors, float *moments_out, gsb_stream_t stream) {
   // (the re-pack leaves the records' depth word 0: k_draw_bwd never reads it)
-  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
-                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws,
-                             ws_bytes, dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, nullptr,
-                             stream);
+  return splat_backward("splatB", 0, H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
+                        patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws, ws_bytes,
+                        dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, nullptr, stream);
 }
 
 int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -809,9 +837,9 @@ int gsb_splat_backward_rgbd(int H, int W, int N, int64_t P, const float *us, con
                             float *dloss_ddepths, gsb_stream_t stream) {
   GSB_REQUIRE(N <= 0 || dloss_ddepths != nullptr, "splatB_rgbd: null dloss_ddepths");
   const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
-  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
-                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
-                             dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, nullptr, stream);
+  return splat_backward("splatB", 0, H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
+                        patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
+                        dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, nullptr, stream);
 }
 
 int gsb_splat_backward_abs(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -821,10 +849,9 @@ int gsb_splat_backward_abs(int H, int W, int N, int64_t P, const float *us, cons
                            float *dloss_dus, float *dloss_dcinv2ds, float *dloss_dalphas, float *dloss_dcolors,
                            float *moments_out, float *dloss_dus_abs, gsb_stream_t stream) {
   GSB_REQUIRE(N <= 0 || dloss_dus_abs != nullptr, "splatB_abs: null dloss_dus_abs");
-  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
-                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws,
-                             ws_bytes, dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out,
-                             dloss_dus_abs, stream);
+  return splat_backward("splatB", 0, H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib, final_tau,
+                        patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws, ws_bytes,
+                        dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, dloss_dus_abs, stream);
 }
 
 int gsb_splat_backward_rgbd_abs(int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -838,19 +865,20 @@ int gsb_splat_backward_rgbd_abs(int H, int W, int N, int64_t P, const float *us,
   GSB_REQUIRE(N <= 0 || dloss_dus_abs != nullptr, "splatB_rgbd_abs: null dloss_dus_abs");
   GSB_REQUIRE(N <= 0 || dloss_ddepths != nullptr, "splatB_rgbd: null dloss_ddepths");
   const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
-  return splat_backward_impl(H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
-                             patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
-                             dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, dloss_dus_abs,
-                             stream);
+  return splat_backward("splatB", 0, H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib, final_tau,
+                        patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records, ws, ws_bytes,
+                        dloss_dus, dloss_dcinv2ds, dloss_dalphas, dloss_dcolors, moments_out, dloss_dus_abs, stream);
 }
 
 // ---- batched rendering (DESIGN 3.21): C cameras of one image size and camera model, binned and drawn
-// as one tall frame.  The entry points mirror the single-camera ones with C in front.
+// as one tall frame through the frame cores above; the per-Gaussian kernels run the C cameras in one launch.
 
-// The per-camera intrinsics rows (fx, fy, cx, cy, k[4]) checked as camera_lens checks one camera,
-// into the kernels' parameter table; tan_fov exactly as the single-camera path computes it.
-static int batch_scene(const char *who, int C, int N, int sh_dim3, int camera_model, const float *intrinsics,
-                       float width, float height, BatchCams &bc, BatchScene &b) {
+// The batch call description: the per-camera intrinsics rows (fx, fy, cx, cy, k[4]) checked as
+// camera_lens checks one camera, into the kernels' parameter table (tan_fov exactly as the
+// single-camera path computes it), and the parameter and pose pointers.
+static int batch_scene(const char *who, int C, int N, int sh_dim3, const float *pws, const float *rots,
+                       const float *scales, const float *shs, const float *poses, int camera_model,
+                       const float *intrinsics, float width, float height, BatchCams &bc, BatchScene &b) {
   if (C < 1) return arg_error(who, "C < 1");
   if (C > BATCH_MAX_CAMERAS) return arg_error(who, "C > GSB_BATCH_MAX_CAMERAS");
   if (N < 0) return arg_error(who, "N < 0");
@@ -870,6 +898,7 @@ static int batch_scene(const char *who, int C, int N, int sh_dim3, int camera_mo
     bc.tf[c] = tf;
   }
   b.C = C; b.N = N; b.k3 = sh_dim3; b.model = camera_model; b.cams = &bc;
+  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
   return 0;
 }
 
@@ -881,15 +910,46 @@ int gsb_preprocess_forward_batch(int C, int N, int sh_dim3, const float *pws, co
   const char *who = "preprocess_batch";
   BatchCams bc;
   BatchScene b{};
-  if (int rc = batch_scene(who, C, N, sh_dim3, camera_model, intrinsics, width, height, bc, b)) return rc;
+  if (int rc = batch_scene(who, C, N, sh_dim3, pws, rots, scales, shs, poses, camera_model, intrinsics, width, height,
+                           bc, b))
+    return rc;
   if (!aligned(records, 16)) return arg_error(who, "records misaligned");
   if (N > 0 && !(pws && rots && scales && shs && poses && us && cinv2ds && colors && depths && areas && alphas &&
                  records))
     return arg_error(who, "null pointer");
-  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
   return launch_preprocess_fwd_batch(b, {us, cinv2ds, colors, depths, areas, alphas, static_cast<Rec *>(records),
                                          alphas_eff},
                                      (cudaStream_t)stream);
+}
+
+// gsb_preprocess_backward_batch and, with `pose`, its camera gradients (DESIGN 3.22): then the
+// per-Gaussian outputs may be all NULL (pose only)
+static int preprocess_backward_batch(const char *who, bool pose, int C, int N, int sh_dim3, const float *pws,
+                                     const float *rots, const float *scales, const float *shs, const float *poses,
+                                     const float *intrinsics, int camera_model, float width, float height,
+                                     BatchBwd g, float *dloss_dposes, void *ws, size_t ws_bytes,
+                                     gsb_stream_t stream) {
+  BatchCams bc;
+  BatchScene b{};
+  if (int rc = batch_scene(who, C, N, sh_dim3, pws, rots, scales, shs, poses, camera_model, intrinsics, width, height,
+                           bc, b))
+    return rc;
+  if (N > 0 && !(pws && rots && scales && shs && poses && g.moments && g.cinv2ds)) return arg_error(who, "null pointer");
+  const bool all = g.g_pws && g.g_shs && g.g_scales && g.g_rots && g.dus_out && g.dalphas_out;
+  const bool none = !g.g_pws && !g.g_shs && !g.g_scales && !g.g_rots && !g.dus_out && !g.dalphas_out;
+  if (!pose) {
+    if (N > 0 && !all) return arg_error(who, "null output");
+    return launch_preprocess_bwd_batch(b, g, (cudaStream_t)stream);
+  }
+  if (N > 0 && !all && !none) return arg_error(who, "per-Gaussian outputs must be all set or all null");
+  if (dloss_dposes == nullptr) return arg_error(who, "null dloss_dposes");
+  if (!aligned(ws, 16)) return arg_error(who, "workspace misaligned");
+  const size_t need = batch_pose_workspace_bytes(C, N);
+  if (!(ws_bytes >= need && (need == 0 || ws != nullptr))) return arg_error(who, "workspace too small");
+  const PoseOut po{dloss_dposes, static_cast<float *>(ws)};
+  g.po = &po;
+  // (N == 0 launches no per-Gaussian pass: only the C rows of zeros)
+  return launch_preprocess_bwd_batch(b, g, (cudaStream_t)stream);
 }
 
 int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
@@ -898,18 +958,11 @@ int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, c
                                   const float *dloss_ddepths, const float *alphas, float *dloss_dpws,
                                   float *dloss_dshs, float *dloss_dscales, float *dloss_drots, float *dloss_dus_out,
                                   float *dloss_dalphas_out, gsb_stream_t stream) {
-  const char *who = "preprocessB_batch";
-  BatchCams bc;
-  BatchScene b{};
-  if (int rc = batch_scene(who, C, N, sh_dim3, camera_model, intrinsics, width, height, bc, b)) return rc;
-  if (N > 0 && !(pws && rots && scales && shs && poses && moments && cinv2ds))
-    return arg_error(who, "null pointer");
-  if (N > 0 && !(dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots && dloss_dus_out && dloss_dalphas_out))
-    return arg_error(who, "null output");
-  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
-  return launch_preprocess_bwd_batch(b, {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
-                                         dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots},
-                                     (cudaStream_t)stream);
+  return preprocess_backward_batch("preprocessB_batch", false, C, N, sh_dim3, pws, rots, scales, shs, poses,
+                                   intrinsics, camera_model, width, height,
+                                   {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
+                                    dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots},
+                                   nullptr, nullptr, 0, stream);
 }
 
 // The batch's workspace queries answer 0 for what its entry points refuse: C < 1, N < 0, C N >= 2^31
@@ -919,8 +972,6 @@ size_t gsb_preprocess_backward_batch_pose_workspace_bytes(int C, int N) {
   return batch_records_ok(C, N) ? batch_pose_workspace_bytes(C, N) : 0;
 }
 
-// gsb_preprocess_backward_batch plus the C camera gradients (DESIGN 3.22): the per-Gaussian outputs all
-// set (pose and map) or all NULL (pose only)
 int gsb_preprocess_backward_batch_pose(int C, int N, int sh_dim3, const float *pws, const float *rots,
                                        const float *scales, const float *shs, const float *poses,
                                        const float *intrinsics, int camera_model, float width, float height,
@@ -928,47 +979,19 @@ int gsb_preprocess_backward_batch_pose(int C, int N, int sh_dim3, const float *p
                                        const float *alphas, float *dloss_dpws, float *dloss_dshs, float *dloss_dscales,
                                        float *dloss_drots, float *dloss_dus_out, float *dloss_dalphas_out,
                                        float *dloss_dposes, void *ws, size_t ws_bytes, gsb_stream_t stream) {
-  const char *who = "preprocessB_batch_pose";
-  BatchCams bc;
-  BatchScene b{};
-  if (int rc = batch_scene(who, C, N, sh_dim3, camera_model, intrinsics, width, height, bc, b)) return rc;
-  if (N > 0 && !(pws && rots && scales && shs && poses && moments && cinv2ds))
-    return arg_error(who, "null pointer");
-  const bool all = dloss_dpws && dloss_dshs && dloss_dscales && dloss_drots && dloss_dus_out && dloss_dalphas_out;
-  const bool none = !dloss_dpws && !dloss_dshs && !dloss_dscales && !dloss_drots && !dloss_dus_out &&
-                    !dloss_dalphas_out;
-  if (N > 0 && !all && !none) return arg_error(who, "per-Gaussian outputs must be all set or all null");
-  if (dloss_dposes == nullptr) return arg_error(who, "null dloss_dposes");
-  if (!aligned(ws, 16)) return arg_error(who, "workspace misaligned");
-  const size_t need = batch_pose_workspace_bytes(C, N);
-  if (!(ws_bytes >= need && (need == 0 || ws != nullptr))) return arg_error(who, "workspace too small");
-  b.pws = pws; b.rots = rots; b.scales = scales; b.shs = shs; b.poses = poses;
-  const PoseOut po{dloss_dposes, static_cast<float *>(ws)};
-  // (N == 0 launches no per-Gaussian pass: only the C rows of zeros)
-  return launch_preprocess_bwd_batch(b, {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
-                                         dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots, &po},
-                                     (cudaStream_t)stream);
+  return preprocess_backward_batch("preprocessB_batch_pose", true, C, N, sh_dim3, pws, rots, scales, shs, poses,
+                                   intrinsics, camera_model, width, height,
+                                   {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
+                                    dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots},
+                                   dloss_dposes, ws, ws_bytes, stream);
 }
 
 size_t gsb_splat_bin_batch_workspace_bytes(int C, int N) { return batch_records_ok(C, N) ? bin_layout(C * N).bytes : 0; }
 
 int gsb_splat_bin_batch(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas, void *bin_ws,
                         size_t bin_ws_bytes, int64_t *P_host, uint32_t *depth_key_max_host, gsb_stream_t stream) {
-  if (int rc = check_frame_batch("splat_bin_batch", C, H, W, N, bin_ws, bin_ws_bytes)) return rc;
-  GSB_REQUIRE(P_host != nullptr && bin_ws != nullptr, "splat_bin_batch: null workspace / P_host");
-  GSB_REQUIRE(N == 0 || (us && depths && areas), "splat_bin_batch: null pointer");
-  const BinLayout L = bin_layout(C * N);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (int rc = launch_bin_batch(C, H, W, N, us, depths, areas, bin_ws, L, st)) return rc;
-  uint32_t total[3] = {0, 0, 0};  // [patch count, largest depth key, flags]
-  GSB_CUDA_TRY(cudaMemcpyAsync(total, static_cast<char *>(bin_ws) + L.total, 3 * sizeof(uint32_t),
-                               cudaMemcpyDeviceToHost, st));
-  GSB_CUDA_TRY(cudaStreamSynchronize(st));
-  GSB_REQUIRE((total[2] & GSB_STATUS_TOO_MANY_PATCHES) == 0 && total[0] < (1u << 30),
-              "splat_bin_batch: more than 2^30 patches");
-  *P_host = (int64_t)total[0];
-  if (depth_key_max_host) *depth_key_max_host = total[1];
-  return 0;
+  return splat_bin("splat_bin_batch", batch_frames(C), H, W, N, us, depths, areas, bin_ws, bin_ws_bytes, P_host,
+                   depth_key_max_host, stream);
 }
 
 size_t gsb_splat_batch_records_offset(int C, int N, int H, int W, int64_t P) {
@@ -979,31 +1002,14 @@ size_t gsb_splat_batch_workspace_bytes(int C, int N, int H, int W, int64_t P) {
   return batch_records_ok(C, N) ? sort_layout(C * N, batch_height(C, H), W, P).bytes : 0;
 }
 
-static int splat_render_batch_impl(const char *who, int C, int H, int W, int N, int64_t P, uint32_t depth_key_max,
-                                   const float *us, const float *cinv2ds, const float *alphas, const float *depths,
-                                   const float *colors, const void *packed_records, const void *bin_ws, void *ws,
-                                   size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
-                                   int32_t *patch_range_per_tile, int32_t *gsid_per_patch, float *depth_image,
-                                   float *alpha_image, gsb_stream_t stream) {
-  if (int rc = check_frame_batch(who, C, H, W, N, bin_ws, SIZE_MAX)) return rc;
-  if (P < 0) return arg_error(who, "bad P");
-  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
-  if (P > 0 && !(us && cinv2ds && alphas && depths && colors && bin_ws && ws && gsid_per_patch))
-    return arg_error(who, "null pointer");
-  return render_frame(who, H, W, N, P, depth_key_max, us, cinv2ds, alphas, const_cast<float *>(depths), colors,
-                      nullptr, packed_records == nullptr, const_cast<void *>(bin_ws), ws, ws_bytes,
-                      {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
-                      ColourDraw{packed_records, depth_image, alpha_image, C}, nullptr, (cudaStream_t)stream, C);
-}
-
 int gsb_splat_render_batch(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
                            const float *cinv2ds, const float *alphas, const float *depths, const float *colors,
                            const void *packed_records, const void *bin_ws, void *ws, size_t ws_bytes, float *image,
                            int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
                            int32_t *gsid_per_patch, gsb_stream_t stream) {
-  return splat_render_batch_impl("splat_batch", C, H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors,
-                                 packed_records, bin_ws, ws, ws_bytes, image, contrib, final_tau,
-                                 patch_range_per_tile, gsid_per_patch, nullptr, nullptr, stream);
+  return splat_render("splat_batch", batch_frames(C), H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths, colors,
+                      packed_records, bin_ws, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
+                      gsid_per_patch, nullptr, nullptr, stream);
 }
 
 int gsb_splat_render_batch_rgbd(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
@@ -1012,28 +1018,9 @@ int gsb_splat_render_batch_rgbd(int C, int H, int W, int N, int64_t P, uint32_t 
                                 float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
                                 int32_t *gsid_per_patch, float *depth_image, float *alpha_image, gsb_stream_t stream) {
   GSB_REQUIRE(depth_image && alpha_image, "splat_batch_rgbd: null depth_image / alpha_image");
-  return splat_render_batch_impl("splat_batch_rgbd", C, H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths,
-                                 colors, packed_records, bin_ws, ws, ws_bytes, image, contrib, final_tau,
-                                 patch_range_per_tile, gsid_per_patch, depth_image, alpha_image, stream);
-}
-
-static int splat_forward_batch_impl(const char *who, int C, int H, int W, int N, const float *us,
-                                    const float *cinv2ds, const float *alphas, float *depths, const float *colors,
-                                    int32_t *areas, const void *packed_records, int64_t P_cap, uint32_t depth_key_cap,
-                                    void *bin_ws, size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image,
-                                    int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
-                                    int32_t *gsid_per_patch, uint32_t *status_host, float *depth_image,
-                                    float *alpha_image, gsb_stream_t stream) {
-  if (int rc = check_frame_batch(who, C, H, W, N, bin_ws, bin_ws_bytes)) return rc;
-  if (!(P_cap > 0 && P_cap < ((int64_t)1 << 30))) return arg_error(who, "bad P_cap (2^30 patches or more)");
-  if (!(gsid_per_patch && status_host && bin_ws)) return arg_error(who, "null pointer");
-  if (N > 0 && !(us && cinv2ds && alphas && depths && colors && areas)) return arg_error(who, "null pointer");
-  return capacity_wait(who, P_cap, status_host, true, [&](const StatusRead *sr) {
-    return render_frame(who, H, W, N, P_cap, depth_key_cap, us, cinv2ds, alphas, depths, colors, areas,
-                        packed_records == nullptr, bin_ws, ws, ws_bytes,
-                        {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch},
-                        ColourDraw{packed_records, depth_image, alpha_image, C}, sr, (cudaStream_t)stream, C);
-  });
+  return splat_render("splat_batch_rgbd", batch_frames(C), H, W, N, P, depth_key_max, us, cinv2ds, alphas, depths,
+                      colors, packed_records, bin_ws, ws, ws_bytes, image, contrib, final_tau, patch_range_per_tile,
+                      gsid_per_patch, depth_image, alpha_image, stream);
 }
 
 int gsb_splat_forward_batch(int C, int H, int W, int N, const float *us, const float *cinv2ds, const float *alphas,
@@ -1042,10 +1029,9 @@ int gsb_splat_forward_batch(int C, int H, int W, int N, const float *us, const f
                             size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
                             int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
                             gsb_stream_t stream) {
-  return splat_forward_batch_impl("splat_batch", C, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
-                                  packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image,
-                                  contrib, final_tau, patch_range_per_tile, gsid_per_patch, status_host, nullptr,
-                                  nullptr, stream);
+  return splat_forward("splat_batch", "splat_batch", batch_frames(C), H, W, N, us, cinv2ds, alphas, depths, colors,
+                       areas, packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image, contrib,
+                       final_tau, patch_range_per_tile, gsid_per_patch, status_host, nullptr, nullptr, stream, true);
 }
 
 int gsb_splat_forward_batch_rgbd(int C, int H, int W, int N, const float *us, const float *cinv2ds,
@@ -1055,10 +1041,10 @@ int gsb_splat_forward_batch_rgbd(int C, int H, int W, int N, const float *us, co
                                  float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
                                  uint32_t *status_host, float *depth_image, float *alpha_image, gsb_stream_t stream) {
   GSB_REQUIRE(depth_image && alpha_image, "splat_batch_rgbd: null depth_image / alpha_image");
-  return splat_forward_batch_impl("splat_batch_rgbd", C, H, W, N, us, cinv2ds, alphas, depths, colors, areas,
-                                  packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image,
-                                  contrib, final_tau, patch_range_per_tile, gsid_per_patch, status_host, depth_image,
-                                  alpha_image, stream);
+  return splat_forward("splat_batch_rgbd", "splat_batch_rgbd", batch_frames(C), H, W, N, us, cinv2ds, alphas, depths,
+                       colors, areas, packed_records, P_cap, depth_key_cap, bin_ws, bin_ws_bytes, ws, ws_bytes, image,
+                       contrib, final_tau, patch_range_per_tile, gsid_per_patch, status_host, depth_image,
+                       alpha_image, stream, true);
 }
 
 size_t gsb_splat_backward_batch_workspace_bytes(int C, int N, int H, int W, int64_t P) {
@@ -1066,52 +1052,15 @@ size_t gsb_splat_backward_batch_workspace_bytes(int C, int N, int H, int W, int6
 }
 
 // the batch's backward rasterizer: the moment rows [C N, 9] (and dL/dz [C N]) for
-// gsb_preprocess_backward_batch; the records are packed_records or re-packed into ws
-static int splat_backward_batch_impl(const char *who, int C, int H, int W, int N, int64_t P, const float *us,
-                                     const float *cinv2ds, const float *alphas, const float *colors,
-                                     const float *depths, const int32_t *contrib, const float *final_tau,
-                                     const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
-                                     const float *dloss_dgammas, const DepthGrads *dg, const void *packed_records,
-                                     void *ws, size_t ws_bytes, float *moments_out, gsb_stream_t stream) {
-  if (int rc = check_batch(who, C, H, W, N)) return rc;
-  if (P < 0) return arg_error(who, "bad P");
-  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
-  if (N == 0) return 0;
-  if (!(cinv2ds && ws && moments_out)) return arg_error(who, "null pointer");
-  const int NT = C * N;
-  const int64_t P_ws = packed_records != nullptr ? 0 : P;
-  if (ws_bytes < gsb_splat_backward_batch_workspace_bytes(C, N, H, W, P_ws)) return arg_error(who, "workspace too small");
-  cudaStream_t st = (cudaStream_t)stream;
-  char *b = static_cast<char *>(ws);
-  const BwdLayout L = bwd_layout(NT, batch_height(C, H), W, P_ws, reinterpret_cast<uintptr_t>(ws));
-  Rec *recs = reinterpret_cast<Rec *>(b + L.recs);
-  if (P > 0) {
-    if (!(us && alphas && colors && contrib && final_tau && patch_range_per_tile && gsid_per_patch && dloss_dgammas))
-      return arg_error(who, "null pointer");
-    if (dg != nullptr && !(depths && dg->dloss_ddepth_image && dg->dloss_dalpha_image && dg->ddepths))
-      return arg_error(who, "null pointer");
-    if (!aligned(packed_records, 16)) return arg_error(who, "packed_records misaligned");
-    if (packed_records != nullptr) {
-      recs = const_cast<Rec *>(static_cast<const Rec *>(packed_records));
-    } else if (int rc = launch_pack_only(NT, nullptr, us, cinv2ds, alphas, colors, depths, recs, st)) {
-      return rc;
-    }
-  } else if (dg != nullptr && dg->ddepths == nullptr) {
-    return arg_error(who, "null pointer");
-  }
-  return launch_draw_backward(H, W, NT, patch_range_per_tile, P > 0 ? recs : nullptr, gsid_per_patch, contrib,
-                              final_tau, dloss_dgammas, dg, cinv2ds, moments_out, reinterpret_cast<int *>(b + L.work),
-                              nullptr, nullptr, nullptr, nullptr, false, nullptr, st, C);
-}
-
+// gsb_preprocess_backward_batch
 int gsb_splat_backward_batch(int C, int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
                              const float *alphas, const float *colors, const int32_t *contrib, const float *final_tau,
                              const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
                              const float *dloss_dgammas, const void *packed_records, void *ws, size_t ws_bytes,
                              float *moments_out, gsb_stream_t stream) {
-  return splat_backward_batch_impl("splatB_batch", C, H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib,
-                                   final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr,
-                                   packed_records, ws, ws_bytes, moments_out, stream);
+  return splat_backward("splatB_batch", batch_frames(C), H, W, N, P, us, cinv2ds, alphas, colors, nullptr, contrib,
+                        final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas, nullptr, packed_records, ws,
+                        ws_bytes, nullptr, nullptr, nullptr, nullptr, moments_out, nullptr, stream);
 }
 
 int gsb_splat_backward_batch_rgbd(int C, int H, int W, int N, int64_t P, const float *us, const float *cinv2ds,
@@ -1122,9 +1071,9 @@ int gsb_splat_backward_batch_rgbd(int C, int H, int W, int N, int64_t P, const f
                                   const void *packed_records, void *ws, size_t ws_bytes, float *moments_out,
                                   float *dloss_ddepths, gsb_stream_t stream) {
   const DepthGrads dg{dloss_ddepth_image, dloss_dalpha_image, dloss_ddepths};
-  return splat_backward_batch_impl("splatB_batch_rgbd", C, H, W, N, P, us, cinv2ds, alphas, colors, depths, contrib,
-                                   final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg,
-                                   packed_records, ws, ws_bytes, moments_out, stream);
+  return splat_backward("splatB_batch_rgbd", batch_frames(C), H, W, N, P, us, cinv2ds, alphas, colors, depths,
+                        contrib, final_tau, patch_range_per_tile, gsid_per_patch, dloss_dgammas, &dg, packed_records,
+                        ws, ws_bytes, nullptr, nullptr, nullptr, nullptr, moments_out, nullptr, stream);
 }
 
 // ---- 2D Gaussian Splatting (surfel.cu, DESIGN 3.15)
@@ -1212,7 +1161,7 @@ int gsb_splat_surfel_render(int H, int W, int N, int64_t P, uint32_t depth_key_m
                             float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
                             int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
                             gsb_stream_t stream) {
-  int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
+  int rc = check_frame("splat", 0, H, W, N, bin_ws, SIZE_MAX);
   if (rc) return rc;
   GSB_REQUIRE(P >= 0, "splat_surfel: bad P");
   GSB_REQUIRE(P == 0 || (us && depths && records && bin_ws && ws && gsid_per_patch), "splat_surfel: null pointer");
@@ -1228,7 +1177,7 @@ int gsb_splat_surfel_forward(int H, int W, int N, const float *us, float *depths
                              float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
                              uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
                              gsb_stream_t stream) {
-  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
+  int rc = check_frame("splat", 0, H, W, N, bin_ws, bin_ws_bytes);
   if (rc) return rc;
   GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_surfel_forward: bad P_cap");
   GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_surfel_forward: null pointer");
@@ -1270,7 +1219,7 @@ int gsb_splat_2dgs_render(int H, int W, int N, int64_t P, uint32_t depth_key_max
                           int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
                           float *distortion, float *moments, float *median_depth, int32_t *median_contrib,
                           gsb_stream_t stream) {
-  int rc = check_frame(H, W, N, bin_ws, SIZE_MAX);
+  int rc = check_frame("splat", 0, H, W, N, bin_ws, SIZE_MAX);
   if (rc) return rc;
   GSB_REQUIRE(P >= 0, "splat_2dgs: bad P");
   GSB_REQUIRE(P == 0 || (us && depths && records && bin_ws && ws && gsid_per_patch), "splat_2dgs: null pointer");
@@ -1289,7 +1238,7 @@ int gsb_splat_2dgs_forward(int H, int W, int N, const float *us, float *depths, 
                            uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
                            float *distortion, float *moments, float *median_depth, int32_t *median_contrib,
                            gsb_stream_t stream) {
-  int rc = check_frame(H, W, N, bin_ws, bin_ws_bytes);
+  int rc = check_frame("splat", 0, H, W, N, bin_ws, bin_ws_bytes);
   if (rc) return rc;
   GSB_REQUIRE(P_cap > 0 && P_cap < ((int64_t)1 << 30), "splat_2dgs_forward: bad P_cap");
   GSB_REQUIRE(gsid_per_patch && status_host && bin_ws, "splat_2dgs_forward: null pointer");

@@ -30,6 +30,45 @@ __device__ __forceinline__ pg::Cam load_cam(const float *__restrict__ Rcw, const
 
 #define ROWK(K) (sm + tid * TileT<K>::S)
 
+// row o of the forward's per-Gaussian outputs (not the record, nor the effective opacity)
+__device__ __forceinline__ void store_fwd_rows(float *__restrict__ us, float *__restrict__ cinv2ds,
+                                               float *__restrict__ colors, int32_t *__restrict__ areas,
+                                               float *__restrict__ depths, long long o, const float (&u)[2],
+                                               const float (&conic)[3], const float (&col)[3], const int (&area)[2],
+                                               float depth) {
+  st_pair(us, o, u[0], u[1]);
+  cinv2ds[3 * o] = conic[0]; cinv2ds[3 * o + 1] = conic[1]; cinv2ds[3 * o + 2] = conic[2];
+  colors[3 * o] = col[0]; colors[3 * o + 1] = col[1]; colors[3 * o + 2] = col[2];
+  st_pair(areas, o, area[0], area[1]);
+  depths[o] = depth;
+}
+
+// row o of the 10 small gradient floats: direct strided stores (no staging, no barriers)
+__device__ __forceinline__ void store_grad_rows(float *g_pws, float *g_scales, float *g_rots, long long o,
+                                                const float (&gpw)[3], const float (&gs)[3], const float (&gq)[4]) {
+  g_pws[3 * o] = gpw[0]; g_pws[3 * o + 1] = gpw[1]; g_pws[3 * o + 2] = gpw[2];
+  g_scales[3 * o] = gs[0]; g_scales[3 * o + 1] = gs[1]; g_scales[3 * o + 2] = gs[2];
+  if (aligned16(g_rots)) {
+    reinterpret_cast<float4 *>(g_rots)[o] = make_float4(gq[0], gq[1], gq[2], gq[3]);
+  } else {
+    g_rots[4 * o] = gq[0]; g_rots[4 * o + 1] = gq[1]; g_rots[4 * o + 2] = gq[2]; g_rots[4 * o + 3] = gq[3];
+  }
+}
+
+// the first step of the pose kernels' CTA sum of the 15 camera terms: the warp's sum, by shuffles,
+// into lane 0's `row`
+__device__ __forceinline__ void warp_sum_pose(float (&gcam)[15], float *row) {
+#pragma unroll
+  for (int e = 0; e < 15; e++) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) gcam[e] += __shfl_down_sync(0xffffffffu, gcam[e], o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int e = 0; e < 15; e++) row[e] = gcam[e];
+  }
+}
+
 __device__ __forceinline__ void load_small_rows(const float *__restrict__ pws, const float *__restrict__ scales,
                                                 const float *__restrict__ rots, long long i, bool valid,
                                                 float (&pw)[3], float (&s)[3], float (&q)[4]) {
@@ -78,11 +117,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd(
   if (valid) {
     const float rho = pg::forward_one<K3, AA, MODEL>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
     const long long i = base + tid;
-    st_pair(us, i, u[0], u[1]);
-    cinv2ds[3 * i] = conic[0]; cinv2ds[3 * i + 1] = conic[1]; cinv2ds[3 * i + 2] = conic[2];
-    colors[3 * i] = col[0]; colors[3 * i + 1] = col[1]; colors[3 * i + 2] = col[2];
-    st_pair(areas, i, area[0], area[1]);
-    depths[i] = depth;
+    store_fwd_rows(us, cinv2ds, colors, areas, depths, i, u, conic, col, area, depth);
     float al = 0.f;
     if (AA) {
       al = rho * __ldg(alphas + i);
@@ -181,15 +216,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
                                             galpha, al);
     }
     __shared__ float red[PG / 32][16];
-#pragma unroll
-    for (int e = 0; e < 15; e++) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) gcam[e] += __shfl_down_sync(0xffffffffu, gcam[e], o);
-    }
-    if ((tid & 31) == 0) {
-#pragma unroll
-      for (int e = 0; e < 15; e++) red[tid >> 5][e] = gcam[e];
-    }
+    warp_sum_pose(gcam, red[tid >> 5]);
     __syncthreads();
     if (tid < 16) {
       float v = 0.f;
@@ -230,16 +257,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   // g_shs == nullptr: the caller re-expands dL/dsh = sum over views of Y(dir_v) (x) dL/dcolor_v itself
   // (multi-view data parallel: 12 B/view travel instead of the 192 B row, k_sh_expand below)
   if (g_shs != nullptr) tile_flush<KS>(g_shs, drow, nv, sm, tid);
-  if (valid) {  // the 10 small gradient floats: direct strided stores (no staging, no barriers)
-    const long long o = drow + tid;
-    g_pws[3 * o] = gpw[0]; g_pws[3 * o + 1] = gpw[1]; g_pws[3 * o + 2] = gpw[2];
-    g_scales[3 * o] = gs[0]; g_scales[3 * o + 1] = gs[1]; g_scales[3 * o + 2] = gs[2];
-    if (aligned16(g_rots)) {
-      reinterpret_cast<float4 *>(g_rots)[o] = make_float4(gq[0], gq[1], gq[2], gq[3]);
-    } else {
-      g_rots[4 * o] = gq[0]; g_rots[4 * o + 1] = gq[1]; g_rots[4 * o + 2] = gq[2]; g_rots[4 * o + 3] = gq[3];
-    }
-  }
+  if (valid) store_grad_rows(g_pws, g_scales, g_rots, drow + tid, gpw, gs, gq);
   if (PUSH) {
     __threadfence_system();  // this thread's peer stores are ordered before the flag below
     __syncthreads();
@@ -394,11 +412,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_fwd_batch(
     int area[2] = {0, 0};
     const float rho = pg::forward_one<K3, AA, MODEL>(pw, q, s, ROWK(KS), cam, u, conic, col, &depth, area);
     const long long o = (long long)c * N + i;
-    st_pair(us, o, u[0], u[1]);
-    cinv2ds[3 * o] = conic[0]; cinv2ds[3 * o + 1] = conic[1]; cinv2ds[3 * o + 2] = conic[2];
-    colors[3 * o] = col[0]; colors[3 * o + 1] = col[1]; colors[3 * o + 2] = col[2];
-    st_pair(areas, o, area[0], area[1]);
-    depths[o] = depth;
+    store_fwd_rows(us, cinv2ds, colors, areas, depths, o, u, conic, col, area, depth);
     float al = alpha;
     if (AA) {
       al = rho * alpha;
@@ -466,15 +480,7 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd_batch(
   }
   __syncthreads();
   tile_flush<KS>(g_shs, base, nv, sm, tid);
-  if (valid) {
-    g_pws[3 * i] = gpw[0]; g_pws[3 * i + 1] = gpw[1]; g_pws[3 * i + 2] = gpw[2];
-    g_scales[3 * i] = gs[0]; g_scales[3 * i + 1] = gs[1]; g_scales[3 * i + 2] = gs[2];
-    if (aligned16(g_rots)) {
-      reinterpret_cast<float4 *>(g_rots)[i] = make_float4(gq[0], gq[1], gq[2], gq[3]);
-    } else {
-      g_rots[4 * i] = gq[0]; g_rots[4 * i + 1] = gq[1]; g_rots[4 * i + 2] = gq[2]; g_rots[4 * i + 3] = gq[3];
-    }
-  }
+  if (valid) store_grad_rows(g_pws, g_scales, g_rots, i, gpw, gs, gq);
 }
 
 // The camera gradients of the batch (DESIGN 3.22): k_preprocess_bwd_batch's reads and
@@ -526,16 +532,7 @@ __global__ void __launch_bounds__(PG, 1) k_preprocess_bwd_batch_pose(
       pg::backward_one<K3, DEPTH, true, AA, MODEL>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh, gz, gcam,
                                                    m[5], al);
     }
-#pragma unroll
-    for (int e = 0; e < 15; e++) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) gcam[e] += __shfl_down_sync(0xffffffffu, gcam[e], o);
-    }
-    if ((tid & 31) == 0) {
-      float *r = red + ((size_t)c * (PG / 32) + (tid >> 5)) * 16;
-#pragma unroll
-      for (int e = 0; e < 15; e++) r[e] = gcam[e];
-    }
+    warp_sum_pose(gcam, red + ((size_t)c * (PG / 32) + (tid >> 5)) * 16);
   }
   __syncthreads();
   for (int k = tid; k < C * 16; k += PG) {
@@ -566,12 +563,12 @@ static int with_flags(F &&f, bool b, B... rest) {
   const auto bind = [&](auto c) { return with_flags([&](auto... cs) { return f(c, cs...); }, rest...); };
   return b ? bind(std::true_type{}) : bind(std::false_type{});
 }
-// f(std::integral_constant<int, pg::CamModel>) for the camera model of lens (NULL: PINHOLE).  The
-// deduced return type has the compiler instantiate f, and its kernels, where this is called: the
-// forward's kernels stay ahead of k_sh_expand in the cubin.
+// f(std::integral_constant<int, pg::CamModel>) for the camera model `model`.  The deduced return
+// type has the compiler instantiate f, and its kernels, where this is called: the forward's kernels
+// stay ahead of k_sh_expand in the cubin.
 template <class F>
-static auto with_model(const CamLens *lens, const char *unknown, F &&f) {
-  switch (lens ? lens->model : pg::PINHOLE) {
+static auto with_model(int model, const char *unknown, F &&f) {
+  switch (model) {
     case pg::PINHOLE: return f(std::integral_constant<int, pg::PINHOLE>{});
     case pg::ORTHO: return f(std::integral_constant<int, pg::ORTHO>{});
     case pg::FISHEYE: return f(std::integral_constant<int, pg::FISHEYE>{});
@@ -598,7 +595,7 @@ int launch_preprocess_fwd(const FusedScene &sc, const FusedFwd &f, cudaStream_t 
   const float4 lk = lens_k(sc.lens);
   ProfScope ps(K_PRE_FWD, st);
   const auto launch = [&](auto aa) {
-    return with_model(sc.lens, "preprocess: unknown camera model", [&](auto mdl) -> int {
+    return with_model(sc.lens ? sc.lens->model : pg::PINHOLE, "preprocess: unknown camera model", [&](auto mdl) -> int {
       constexpr bool AA = decltype(aa)::value;
       constexpr int MODEL = decltype(mdl)::value;
       GSB_DISPATCH_K3(sc.k3, (k_preprocess_fwd<K3, AA, MODEL><<<nb, PG, 0, st>>>(
@@ -641,7 +638,7 @@ int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t 
   // so no PUSH form with DEPTH or POSE exists (api.cu never asks for one); AA exists only with the
   // moment rows and without the exchange, and so do the camera models other than PINHOLE.
   const auto pass = [&](auto pose) -> int {
-    return with_model(sc.lens, "preprocessB: unknown camera model", [&](auto mdl) {
+    return with_model(sc.lens ? sc.lens->model : pg::PINHOLE, "preprocessB: unknown camera model", [&](auto mdl) {
       return with_flags(
           [&](auto push, auto mom, auto depth, auto aa) -> int {
             constexpr bool PUSH = decltype(push)::value, MOM = decltype(mom)::value, DEPTH = decltype(depth)::value,
@@ -681,10 +678,9 @@ int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t 
 int launch_preprocess_fwd_batch(const BatchScene &b, const FusedFwd &f, cudaStream_t st) {
   if (b.N <= 0) return 0;
   const int nb = (b.N + PG - 1) / PG;
-  const CamLens model{b.model, {0.f, 0.f, 0.f, 0.f}, 1.f};
   ProfScope ps(K_PRE_FWD_BATCH, st);
   const auto launch = [&](auto aa) {
-    return with_model(&model, "preprocess_batch: unknown camera model", [&](auto mdl) -> int {
+    return with_model(b.model, "preprocess_batch: unknown camera model", [&](auto mdl) -> int {
       constexpr bool AA = decltype(aa)::value;
       constexpr int MODEL = decltype(mdl)::value;
       GSB_DISPATCH_K3(b.k3, (k_preprocess_fwd_batch<K3, AA, MODEL><<<nb, PG, 0, st>>>(
@@ -703,11 +699,10 @@ int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStre
   const PoseOut *po = g.po;
   if (b.N <= 0 && po == nullptr) return 0;
   const int nb = b.N > 0 ? (b.N + PG - 1) / PG : 0;
-  const CamLens model{b.model, {0.f, 0.f, 0.f, 0.f}, 1.f};
   // one pass: k_preprocess_bwd_batch_pose (pose) or k_preprocess_bwd_batch, DEPTH and AA set by which
   // optional inputs are given
   const auto pass = [&](auto pose) {
-    return with_model(&model, "preprocessB_batch: unknown camera model", [&](auto mdl) {
+    return with_model(b.model, "preprocessB_batch: unknown camera model", [&](auto mdl) {
       return with_flags(
           [&](auto depth, auto aa) -> int {
             constexpr bool DEPTH = decltype(depth)::value, AA = decltype(aa)::value;

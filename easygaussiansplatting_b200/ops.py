@@ -59,21 +59,29 @@ def _shs(shs, N, ref):
     return shs, shs.shape[1] // 3
 
 
-def _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc):
-    """Checks the per-Gaussian parameters and the camera the fused kernels read: float32 CUDA
-    tensors on one device, pws[N,3], rots[N,4], scales[N,3], shs[N,3k] with k in {1,4,9,16},
-    Rcw 9, tcw 3 and twc 3 elements.  -> ((the seven tensors, contiguous), N, k)"""
+def _gaussian_map(pws, rots, scales, shs):
+    """Checks the per-Gaussian parameters the fused kernels read: float32 CUDA tensors on one
+    device, pws[N,3], rots[N,4], scales[N,3], shs[N,3k] with k in {1,4,9,16}.
+    -> ((the four tensors, contiguous), N, k)"""
     pws = _chk(pws, "pws", last=3, ndim=2); rots = _chk(rots, "rots", last=4, ndim=2)
     scales = _chk(scales, "scales", last=3, ndim=2)
-    Rcw = _chk(Rcw, "Rcw"); tcw = _chk(tcw, "tcw"); twc = _chk(twc, "twc")
-    _same_device(pws, rots, scales, Rcw, tcw, twc)
+    _same_device(pws, rots, scales)
     N = pws.shape[0]
     if rots.shape[0] != N or scales.shape[0] != N:
         raise ValueError("pws, rots, scales disagree on N")
     shs, k = _shs(shs, N, pws)
+    return (pws, rots, scales, shs), N, k
+
+
+def _gaussian_params(pws, rots, scales, shs, Rcw, tcw, twc):
+    """`_gaussian_map` and the one camera the fused kernels read: Rcw 9, tcw 3 and twc 3 elements
+    on the parameters' device.  -> ((the seven tensors, contiguous), N, k)"""
+    params, N, k = _gaussian_map(pws, rots, scales, shs)
+    Rcw = _chk(Rcw, "Rcw"); tcw = _chk(tcw, "tcw"); twc = _chk(twc, "twc")
+    _same_device(params[0], Rcw, tcw, twc)
     if Rcw.numel() != 9 or tcw.numel() != 3 or twc.numel() != 3:
         raise ValueError("Rcw must have 9, tcw and twc 3 elements")
-    return (pws, rots, scales, shs, Rcw, tcw, twc), N, k
+    return params + (Rcw, tcw, twc), N, k
 
 
 def _scene_args(params, N, k, focal_x, focal_y, center_x, center_y, width, height):
@@ -249,13 +257,15 @@ def _tiles(H, W):
     return ((W + 15) // 16) * ((H + 15) // 16)
 
 
-def _check_drawn(H, W, ranges, planes, text):
+def _check_drawn(H, W, ranges, planes, text, frames=None):
     """the per-pixel tensors of a drawn frame, (tensor, channels) in `planes`, against H x W (else
-    ValueError(text)), and its patch_range_per_tile against the tile grid"""
-    if any(t.numel() != c * H * W for t, c in planes):
+    ValueError(text)), and its patch_range_per_tile against the tile grid.  frames: None, or the C
+    of a batch, whose planes and tile ranges hold C frames"""
+    Cn = 1 if frames is None else frames
+    if any(t.numel() != c * Cn * H * W for t, c in planes):
         raise ValueError(text)
-    if ranges.shape[0] != _tiles(H, W):
-        raise ValueError("patch_range_per_tile does not match the tile grid")
+    if ranges.shape[0] != Cn * _tiles(H, W):
+        raise ValueError("patch_range_per_tile does not match the %stile grid" % ("" if frames is None else "batch's "))
 
 
 def _frame_buffers(lib, dev, H, W, N, P, planes, ws_bytes, frames=None):
@@ -620,9 +630,7 @@ def preprocess_batch(pws, rots, scales, shs, cams, alphas):
     sharing width, height, antialiased and camera_model.  -> [us[C,N,2], cinv2ds[C,N,3],
     colors[C,N,3], depths[C,N], areas[C,N,2] int32, records[C N, 12]] + [alphas_eff[C,N]] when
     antialiased; camera c's rows are the bits `preprocess` gives for camera c alone."""
-    params, N, k = _gaussian_params(pws, rots, scales, shs, torch.zeros(9, device=pws.device),
-                                    torch.zeros(3, device=pws.device), torch.zeros(3, device=pws.device))
-    pws, rots, scales, shs = params[:4]
+    (pws, rots, scales, shs), N, k = _gaussian_map(pws, rots, scales, shs)
     bc = _batch_cams(cams, pws.device)
     alphas = _per_gaussian(alphas, "alphas", N, pws)
     Cn = bc.C
@@ -655,9 +663,7 @@ def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddep
     per-Gaussian outputs are not computed and come back as None."""
     if pose_only and not camera_grad:
         raise ValueError("pose_only=True needs camera_grad=True")
-    params, N, k = _gaussian_params(pws, rots, scales, shs, torch.zeros(9, device=pws.device),
-                                    torch.zeros(3, device=pws.device), torch.zeros(3, device=pws.device))
-    pws, rots, scales, shs = params[:4]
+    (pws, rots, scales, shs), N, k = _gaussian_map(pws, rots, scales, shs)
     bc = _batch_cams(cams, pws.device)
     Cn = bc.C
     moments = _chk(moments, "moments", last=9); cinv2ds = _chk(cinv2ds, "cinv2ds", last=3)
@@ -760,10 +766,8 @@ def splatB_batch(height, width, us, cinv2ds, alphas, depths, colors, contrib, fi
     gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
     dl = _chk(dloss_dgammas, "dloss_dgammas")
     _same_device(us, contrib, final_tau, ranges, gsid, dl)
-    if any(t.numel() != c * Cn * H * W for t, c in ((contrib, 1), (final_tau, 1), (dl, 3))):
-        raise ValueError("contrib / final_tau / dloss_dgammas do not match C x height x width")
-    if ranges.shape[0] != Cn * _tiles(H, W):
-        raise ValueError("patch_range_per_tile does not match the batch's tile grid")
+    _check_drawn(H, W, ranges, ((contrib, 1), (final_tau, 1), (dl, 3)),
+                 "contrib / final_tau / dloss_dgammas do not match C x height x width", frames=Cn)
     if rgbd:
         dloss_ddepth = _chk(dloss_ddepth, "dloss_ddepth"); dloss_dalpha = _chk(dloss_dalpha, "dloss_dalpha")
         _same_device(us, dloss_ddepth, dloss_dalpha)
@@ -776,16 +780,11 @@ def splatB_batch(height, width, us, cinv2ds, alphas, depths, colors, contrib, fi
     lib = _L()
     with torch.cuda.device(dev):
         ws = _bytes(lib.gsb_splat_backward_batch_workspace_bytes(Cn, N, H, W, 0 if records is not None else P), dev)
-        if rgbd:
-            _lib.check(lib.gsb_splat_backward_batch_rgbd(
-                Cn, H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(depths), _ptr(contrib),
-                _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(dloss_ddepth), _ptr(dloss_dalpha),
-                _ptr(records), _ptr(ws), ws.numel(), _ptr(moments), _ptr(ddepths), _stream()), lib)
-        else:
-            _lib.check(lib.gsb_splat_backward_batch(
-                Cn, H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), _ptr(contrib), _ptr(final_tau),
-                _ptr(ranges), _ptr(gsid), _ptr(dl), _ptr(records), _ptr(ws), ws.numel(), _ptr(moments), _stream()),
-                lib)
+        entry = getattr(lib, "gsb_splat_backward_batch" + ("_rgbd" if rgbd else ""))
+        _lib.check(entry(Cn, H, W, N, P, _ptr(us), _ptr(cinv2ds), _ptr(alphas), _ptr(colors), *_ptrs_if(rgbd, depths),
+                         _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid), _ptr(dl),
+                         *_ptrs_if(rgbd, dloss_ddepth, dloss_dalpha), _ptr(records), _ptr(ws), ws.numel(),
+                         _ptr(moments), *_ptrs_if(rgbd, ddepths), _stream()), lib)
     return [moments, ddepths] if rgbd else moments
 
 
