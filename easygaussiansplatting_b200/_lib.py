@@ -67,6 +67,11 @@ SIGNATURES = {
     "gsb_preprocess_backward_batch": (_i, [_i, _i, _i] + [_vp] * 6 + [_i, _f, _f] + [_vp] * 11),
     "gsb_preprocess_backward_batch_pose_workspace_bytes": (_sz, [_i, _i]),
     "gsb_preprocess_backward_batch_pose": (_i, [_i, _i, _i] + [_vp] * 6 + [_i, _f, _f] + [_vp] * 12 + [_sz, _vp]),
+    "gsb_preprocess_backward_intrinsics_workspace_bytes": (_sz, [_i]),
+    "gsb_preprocess_backward_intrinsics": (_i, [_i, _i] + [_vp] * 7 + [_f] * 6 + [_vp] * 16 + [_sz, _vp, _vp]),
+    "gsb_preprocess_backward_batch_intrinsics_workspace_bytes": (_sz, [_i, _i]),
+    "gsb_preprocess_backward_batch_intrinsics": (_i, [_i, _i, _i] + [_vp] * 6 + [_i, _f, _f] + [_vp] * 13 +
+                                                 [_sz, _vp]),
     "gsb_splat_bin_batch_workspace_bytes": (_sz, [_i, _i]),
     "gsb_splat_bin_batch": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, C.POINTER(_i64), C.POINTER(C.c_uint32),
                                  _vp]),

@@ -322,15 +322,16 @@ static int check_preprocess_backward(const char *who, GradOutputs outs, const Fu
 }
 
 // What an entry point of the fused backward requires beyond check_preprocess_backward
-enum : unsigned { kNeedDepths = 1, kNeedCamera = 2, kNeedAlphas = 4 };
+enum : unsigned { kNeedDepths = 1, kNeedCamera = 2, kNeedAlphas = 4, kNeedIntrinsics = 8 };
 
 // The fused backward behind its five local entry points.  needs: the kNeed* the entry point
 // requires; need_moments: NULL, or why it requires the moment rows (the refusal's text).
 // dloss_dcamera (with its workspace): NULL, or also the camera gradient; then the per-Gaussian
-// outputs may be all NULL (pose only).
+// outputs may be all NULL (pose only).  kNeedIntrinsics: dloss_dintrinsics as well (DESIGN 3.23; the
+// workspace then holds rows of 24 floats).
 static int preprocess_backward(const char *who, unsigned needs, const char *need_moments,
                                const gsb_camera_model *camera_model, FusedScene sc, FusedBwd b, float *dloss_dcamera,
-                               void *ws, size_t ws_bytes, gsb_stream_t stream) {
+                               void *ws, size_t ws_bytes, gsb_stream_t stream, float *dloss_dintrinsics = nullptr) {
   CamLens cl;
   if (int rc = camera_lens(who, camera_model, sc, cl)) return rc;
   const int N = sc.N;
@@ -341,10 +342,12 @@ static int preprocess_backward(const char *who, unsigned needs, const char *need
   if ((needs & kNeedCamera) && !pose) return arg_error(who, "null dloss_dcamera");
   if (need_moments && N != 0 && b.mi.moments == nullptr) return arg_error(who, need_moments);
   if ((needs & kNeedAlphas) && N != 0 && b.alphas == nullptr) return arg_error(who, "null alphas");
-  const PoseOut po{dloss_dcamera, static_cast<float *>(ws)};
+  const bool intr = needs & kNeedIntrinsics;
+  if (intr && dloss_dintrinsics == nullptr) return arg_error(who, "null dloss_dintrinsics");
+  const PoseOut po{dloss_dcamera, static_cast<float *>(ws), intr ? dloss_dintrinsics : nullptr};
   if (pose) {
     if (!aligned(ws, 16)) return arg_error(who, "workspace misaligned");
-    if (!(ws_bytes >= pose_workspace_bytes(N) && (N == 0 || ws != nullptr)))
+    if (!(ws_bytes >= (intr ? intrinsics_workspace_bytes(N) : pose_workspace_bytes(N)) && (N == 0 || ws != nullptr)))
       return arg_error(who, "workspace too small");
     // (N == 0 launches no per-Gaussian pass: only the camera gradient's zeros)
     b.po = &po;
@@ -425,6 +428,25 @@ int gsb_preprocess_backward_model(int N, int sh_dim3, const float *pws, const fl
                              {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
                               dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}, dloss_ddepths, alphas},
                              dloss_dcamera, ws, ws_bytes, stream);
+}
+
+size_t gsb_preprocess_backward_intrinsics_workspace_bytes(int N) { return intrinsics_workspace_bytes(N); }
+
+int gsb_preprocess_backward_intrinsics(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                       const float *shs, const float *Rcw, const float *tcw, const float *twc,
+                                       float fx, float fy, float cx, float cy, float width, float height,
+                                       const float *dloss_dus, const float *dloss_dcinv2ds, const float *dloss_dcolors,
+                                       float *dloss_dpws, float *dloss_dshs, float *dloss_dscales, float *dloss_drots,
+                                       const float *moments, const float *cinv2ds, float *dloss_dus_out,
+                                       float *dloss_dalphas_out, const float *dloss_ddepths, const float *alphas,
+                                       float *dloss_dcamera, float *dloss_dintrinsics, void *ws, size_t ws_bytes,
+                                       const gsb_camera_model *camera_model, gsb_stream_t stream) {
+  return preprocess_backward("preprocessB_intrinsics", kNeedCamera | kNeedIntrinsics,
+                             "the intrinsics gradient takes the moment rows", camera_model,
+                             {N, sh_dim3, pws, rots, scales, shs, Rcw, tcw, twc, fx, fy, cx, cy, width, height},
+                             {dloss_dus, dloss_dcinv2ds, dloss_dcolors, dloss_dpws, dloss_dshs, dloss_dscales,
+                              dloss_drots, {moments, cinv2ds, dloss_dus_out, dloss_dalphas_out}, dloss_ddepths, alphas},
+                             dloss_dcamera, ws, ws_bytes, stream, dloss_dintrinsics);
 }
 
 // ---- Mip-Splatting 3D smoothing filter (filter3d.cu)
@@ -923,12 +945,13 @@ int gsb_preprocess_forward_batch(int C, int N, int sh_dim3, const float *pws, co
 }
 
 // gsb_preprocess_backward_batch and, with `pose`, its camera gradients (DESIGN 3.22): then the
-// per-Gaussian outputs may be all NULL (pose only)
+// per-Gaussian outputs may be all NULL (pose only).  intr (with pose): dloss_dintrinsics as well
+// (DESIGN 3.23; the workspace then holds rows of 24 floats).
 static int preprocess_backward_batch(const char *who, bool pose, int C, int N, int sh_dim3, const float *pws,
                                      const float *rots, const float *scales, const float *shs, const float *poses,
                                      const float *intrinsics, int camera_model, float width, float height,
                                      BatchBwd g, float *dloss_dposes, void *ws, size_t ws_bytes,
-                                     gsb_stream_t stream) {
+                                     gsb_stream_t stream, bool intr = false, float *dloss_dintrinsics = nullptr) {
   BatchCams bc;
   BatchScene b{};
   if (int rc = batch_scene(who, C, N, sh_dim3, pws, rots, scales, shs, poses, camera_model, intrinsics, width, height,
@@ -943,10 +966,11 @@ static int preprocess_backward_batch(const char *who, bool pose, int C, int N, i
   }
   if (N > 0 && !all && !none) return arg_error(who, "per-Gaussian outputs must be all set or all null");
   if (dloss_dposes == nullptr) return arg_error(who, "null dloss_dposes");
+  if (intr && dloss_dintrinsics == nullptr) return arg_error(who, "null dloss_dintrinsics");
   if (!aligned(ws, 16)) return arg_error(who, "workspace misaligned");
-  const size_t need = batch_pose_workspace_bytes(C, N);
+  const size_t need = intr ? batch_intrinsics_workspace_bytes(C, N) : batch_pose_workspace_bytes(C, N);
   if (!(ws_bytes >= need && (need == 0 || ws != nullptr))) return arg_error(who, "workspace too small");
-  const PoseOut po{dloss_dposes, static_cast<float *>(ws)};
+  const PoseOut po{dloss_dposes, static_cast<float *>(ws), intr ? dloss_dintrinsics : nullptr};
   g.po = &po;
   // (N == 0 launches no per-Gaussian pass: only the C rows of zeros)
   return launch_preprocess_bwd_batch(b, g, (cudaStream_t)stream);
@@ -984,6 +1008,25 @@ int gsb_preprocess_backward_batch_pose(int C, int N, int sh_dim3, const float *p
                                    {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
                                     dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots},
                                    dloss_dposes, ws, ws_bytes, stream);
+}
+
+size_t gsb_preprocess_backward_batch_intrinsics_workspace_bytes(int C, int N) {
+  return batch_records_ok(C, N) ? batch_intrinsics_workspace_bytes(C, N) : 0;
+}
+
+int gsb_preprocess_backward_batch_intrinsics(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                             const float *scales, const float *shs, const float *poses,
+                                             const float *intrinsics, int camera_model, float width, float height,
+                                             const float *moments, const float *cinv2ds, const float *dloss_ddepths,
+                                             const float *alphas, float *dloss_dpws, float *dloss_dshs,
+                                             float *dloss_dscales, float *dloss_drots, float *dloss_dus_out,
+                                             float *dloss_dalphas_out, float *dloss_dposes, float *dloss_dintrinsics,
+                                             void *ws, size_t ws_bytes, gsb_stream_t stream) {
+  return preprocess_backward_batch("preprocessB_batch_intrinsics", true, C, N, sh_dim3, pws, rots, scales, shs, poses,
+                                   intrinsics, camera_model, width, height,
+                                   {moments, cinv2ds, dloss_ddepths, alphas, dloss_dus_out, dloss_dalphas_out,
+                                    dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots},
+                                   dloss_dposes, ws, ws_bytes, stream, true, dloss_dintrinsics);
 }
 
 size_t gsb_splat_bin_batch_workspace_bytes(int C, int N) { return batch_records_ok(C, N) ? bin_layout(C * N).bytes : 0; }

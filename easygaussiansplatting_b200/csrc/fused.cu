@@ -55,17 +55,18 @@ __device__ __forceinline__ void store_grad_rows(float *g_pws, float *g_scales, f
   }
 }
 
-// the first step of the pose kernels' CTA sum of the 15 camera terms: the warp's sum, by shuffles,
-// into lane 0's `row`
-__device__ __forceinline__ void warp_sum_pose(float (&gcam)[15], float *row) {
+// the first step of the camera kernels' CTA sum of the NE camera terms (15 pose, 23 pose +
+// intrinsics): the warp's sum, by shuffles, into lane 0's `row`
+template <int NE>
+__device__ __forceinline__ void warp_sum_pose(float (&gcam)[NE], float *row) {
 #pragma unroll
-  for (int e = 0; e < 15; e++) {
+  for (int e = 0; e < NE; e++) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) gcam[e] += __shfl_down_sync(0xffffffffu, gcam[e], o);
   }
   if ((threadIdx.x & 31) == 0) {
 #pragma unroll
-    for (int e = 0; e < 15; e++) row[e] = gcam[e];
+    for (int e = 0; e < NE; e++) row[e] = gcam[e];
   }
 }
 
@@ -272,51 +273,65 @@ __global__ void __launch_bounds__(PG) k_preprocess_bwd(
   }
 }
 
-// The camera gradient: the nrows partial rows of k_preprocess_bwd<..., POSE> summed in fp64 by
-// one CTA in a fixed order (thread t takes rows t, t + PR, ...; then a fixed shuffle tree and the
-// warps in index order), so the result is the same bits on every run.  nrows == 0 writes zeros.
+// The camera gradient: the nrows partial rows of NE + 1 floats (NE = 15: k_preprocess_bwd<..., POSE>,
+// 23: k_preprocess_bwd_intrinsics) summed in fp64 by one CTA in a fixed order (thread t takes rows t,
+// t + PR, ...; then a fixed shuffle tree and the warps in index order), so the result is the same bits
+// on every run.  Columns 0-14 go to gcam, 15-22 to gint.  nrows == 0 writes zeros.
 constexpr int PR = 512;
-__device__ __forceinline__ void pose_reduce(int nrows, const float *__restrict__ part, float *__restrict__ gcam) {
+template <int NE>
+__device__ __forceinline__ void pose_reduce(int nrows, const float *__restrict__ part, float *__restrict__ gcam,
+                                            float *__restrict__ gint) {
+  constexpr int RW = NE + 1;  // the row width: 16 or 24 floats, whole float4s
   const int tid = threadIdx.x;
-  double acc[15];
+  double acc[NE];
 #pragma unroll
-  for (int e = 0; e < 15; e++) acc[e] = 0.0;
+  for (int e = 0; e < NE; e++) acc[e] = 0.0;
   for (int r = tid; r < nrows; r += PR) {
-    const float4 *row = reinterpret_cast<const float4 *>(part + (size_t)r * 16);
-    float v[16];
+    const float4 *row = reinterpret_cast<const float4 *>(part + (size_t)r * RW);
+    float v[RW];
 #pragma unroll
-    for (int c = 0; c < 4; c++) {
+    for (int c = 0; c < RW / 4; c++) {
       const float4 x = __ldg(row + c);
       v[4 * c] = x.x; v[4 * c + 1] = x.y; v[4 * c + 2] = x.z; v[4 * c + 3] = x.w;
     }
 #pragma unroll
-    for (int e = 0; e < 15; e++) acc[e] += (double)v[e];
+    for (int e = 0; e < NE; e++) acc[e] += (double)v[e];
   }
 #pragma unroll
-  for (int e = 0; e < 15; e++) {
+  for (int e = 0; e < NE; e++) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc[e] += __shfl_down_sync(0xffffffffu, acc[e], o);
   }
-  __shared__ double red[PR / 32][15];
+  __shared__ double red[PR / 32][NE];
   if ((tid & 31) == 0) {
 #pragma unroll
-    for (int e = 0; e < 15; e++) red[tid >> 5][e] = acc[e];
+    for (int e = 0; e < NE; e++) red[tid >> 5][e] = acc[e];
   }
   __syncthreads();
-  if (tid < 15) {
+  if (tid < NE) {
     double t = 0.0;
     for (int w = 0; w < PR / 32; w++) t += red[w][tid];
-    gcam[tid] = (float)t;
+    if (tid < 15)
+      gcam[tid] = (float)t;
+    else
+      gint[tid - 15] = (float)t;
   }
 }
 __global__ void __launch_bounds__(PR) k_pose_reduce(int nrows, const float *__restrict__ part,
                                                     float *__restrict__ gcam) {
-  pose_reduce(nrows, part, gcam);
+  pose_reduce<15>(nrows, part, gcam, nullptr);
 }
 // the batch's: CTA c sums camera c's nrows rows of part[C][nrows][16] into gcam[c][15]
 __global__ void __launch_bounds__(PR) k_pose_reduce_batch(int nrows, const float *__restrict__ part,
                                                           float *__restrict__ gcam) {
-  pose_reduce(nrows, part + (size_t)blockIdx.x * nrows * 16, gcam + (size_t)blockIdx.x * 15);
+  pose_reduce<15>(nrows, part + (size_t)blockIdx.x * nrows * 16, gcam + (size_t)blockIdx.x * 15, nullptr);
+}
+// pose + intrinsics (DESIGN 3.23), one camera or a batch: CTA c sums camera c's nrows rows of
+// part[C][nrows][24] into gcam[c][15] and gint[c][8]
+__global__ void __launch_bounds__(PR) k_intrinsics_reduce(int nrows, const float *__restrict__ part,
+                                                          float *__restrict__ gcam, float *__restrict__ gint) {
+  pose_reduce<23>(nrows, part + (size_t)blockIdx.x * nrows * 24, gcam + (size_t)blockIdx.x * 15,
+                  gint + (size_t)blockIdx.x * 8);
 }
 
 // dL/dsh of one Gaussian summed over V views from the views' dL/dcolor:
@@ -546,6 +561,78 @@ __global__ void __launch_bounds__(PG, 1) k_preprocess_bwd_batch_pose(
   }
 }
 
+// The camera gradients with the intrinsics' (DESIGN 3.23), for one camera (C = 1) or a batch:
+// k_preprocess_bwd_batch_pose's reads, math and CTA tree with 23 terms per camera
+// (pg::backward_one<..., POSE, ..., INTR>) -- dL/dRcw, dL/dtcw, dL/dtwc, then dL/d(fx, fy, cx, cy,
+// k[4]) -- into part[c][blockIdx.x][24] (summed by k_intrinsics_reduce).  Camera c's pose is read
+// from pp (Rcw, tcw, twc + c stride: the single camera's three arrays, or the batch's [C, 15] rows), its
+// intrinsics, lens and tan_fov from bc.  red: [C][PG / 32][24] floats of dynamic shared memory.
+// Nothing per Gaussian is written.
+struct PosePtrs {
+  const float *Rcw, *tcw, *twc;
+  int stride;  // floats from one camera's pose to the next
+};
+template <int K3, bool DEPTH, bool AA, int MODEL>
+__global__ void __launch_bounds__(PG, 1) k_preprocess_bwd_intrinsics(
+    int C, int N, const float *__restrict__ pws, const float *__restrict__ rots, const float *__restrict__ scales,
+    const float *__restrict__ shs, const PosePtrs pp, const __grid_constant__ BatchCams bc,
+    const float *__restrict__ moments, const float *__restrict__ cinv2ds, const float *__restrict__ g_depths,
+    const float *__restrict__ alphas, float *__restrict__ part) {
+  constexpr int KS = 3 * K3;
+  constexpr int SMF = TileT<KS>::FLOATS > TileT<4>::FLOATS ? TileT<KS>::FLOATS : TileT<4>::FLOATS;
+  constexpr bool LENS = MODEL == pg::FISHEYE || MODEL == pg::OPENCV;
+  __shared__ float sm[SMF];
+  extern __shared__ float red[];  // [C][PG / 32][24]
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * PG;
+  const int nv = min(PG, (int)(N - base));
+  const bool valid = tid < nv;
+  float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
+  load_small_rows(pws, scales, rots, base + tid, valid, pw, s, q);
+  tile_fetch<KS>(shs, base, nv, sm, tid);
+  __syncthreads();
+  const long long i = base + tid;
+  const float al = AA && valid ? __ldg(alphas + i) : 0.f;
+  for (int c = 0; c < C; c++) {
+    float gcam[23];
+#pragma unroll
+    for (int e = 0; e < 23; e++) gcam[e] = 0.f;
+    if (valid) {
+      const long long o = (long long)c * N + i;
+      float m[9];
+#pragma unroll
+      for (int k = 0; k < 9; k++) m[k] = __ldg(moments + 9 * o + k);
+      const float A = __ldg(cinv2ds + 3 * o), B = __ldg(cinv2ds + 3 * o + 1), Cc = __ldg(cinv2ds + 3 * o + 2);
+      const bool none = (m[0] == 0.f) && (m[1] == 0.f);  // as k_preprocess_bwd's MOM form
+      const float gu[2] = {none ? 0.f : -(A * m[0] + B * m[1]), none ? 0.f : -(B * m[0] + Cc * m[1])};
+      const float gci[3] = {-0.5f * m[2], -m[3], -0.5f * m[4]}, gcol[3] = {m[6], m[7], m[8]};
+      const float gz = DEPTH ? __ldg(g_depths + o) : 0.f;
+      const size_t po = (size_t)c * pp.stride;
+      const float4 f = bc.f[c];
+      const float2 tf = bc.tf[c];
+      pg::Cam cam = load_cam(pp.Rcw + po, pp.tcw + po, pp.twc + po, f.x, f.y, f.z, f.w, tf.x, tf.y);
+      if (LENS) {
+        const float4 lk = bc.k[c];
+        cam.k[0] = lk.x; cam.k[1] = lk.y; cam.k[2] = lk.z; cam.k[3] = lk.w;
+      }
+      float xpw[3], xq[4], xs[3], xsh[KS];  // the per-Gaussian outputs: not written by this form
+      pg::backward_one<K3, DEPTH, true, AA, MODEL, true>(pw, q, s, ROWK(KS), cam, gu, gci, gcol, xpw, xq, xs, xsh,
+                                                         gz, gcam, m[5], al);
+    }
+    warp_sum_pose(gcam, red + ((size_t)c * (PG / 32) + (tid >> 5)) * 24);
+  }
+  __syncthreads();
+  for (int k = tid; k < C * 24; k += PG) {
+    const int c = k / 24, e = k - 24 * c;
+    float v = 0.f;
+    if (e < 23) {
+#pragma unroll
+      for (int w = 0; w < PG / 32; w++) v += red[((size_t)c * (PG / 32) + w) * 24 + e];
+    }
+    part[((size_t)c * gridDim.x + blockIdx.x) * 24 + e] = v;
+  }
+}
+
 #define GSB_DISPATCH_K3(k3, CALL)                                           \
   switch (k3) {                                                             \
     case 1: { constexpr int K3 = 1; CALL; } break;                          \
@@ -621,6 +708,48 @@ int launch_sh_expand(int N, int k3, int V, const float *pws, const float *twcs, 
   return 0;
 }
 
+// one launch of k_preprocess_bwd_intrinsics.  Its static SH tile (25 KB at K3 = 16) and `red` (24 KB at
+// C = 64) together pass the 48 KB a kernel gets without asking, so it asks for `red`.
+template <int K3, bool DEPTH, bool AA, int MODEL>
+static int launch_intrinsics_kernel(int nb, size_t red, int C, int N, const float *pws, const float *rots,
+                                    const float *scales, const float *shs, const PosePtrs &pp, const BatchCams &bc,
+                                    const float *moments, const float *cinv2ds, const float *g_depths,
+                                    const float *alphas, float *part, cudaStream_t st) {
+  GSB_CUDA_TRY(cudaFuncSetAttribute(k_preprocess_bwd_intrinsics<K3, DEPTH, AA, MODEL>,
+                                    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)red));
+  k_preprocess_bwd_intrinsics<K3, DEPTH, AA, MODEL><<<nb, PG, red, st>>>(C, N, pws, rots, scales, shs, pp, bc, moments,
+                                                                         cinv2ds, g_depths, alphas, part);
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// the pose + intrinsics pass and its reduction, for launch_preprocess_bwd (C = 1) and
+// launch_preprocess_bwd_batch: moment rows, dL/dz and alphas as k_preprocess_bwd_intrinsics reads them
+static int launch_intrinsics_pass(int C, int N, int k3, int model, const float *pws, const float *rots,
+                                  const float *scales, const float *shs, const PosePtrs &pp, const BatchCams &bc,
+                                  const float *moments, const float *cinv2ds, const float *g_depths,
+                                  const float *alphas, const PoseOut &po, cudaStream_t st) {
+  const int nb = N > 0 ? (N + PG - 1) / PG : 0;
+  if (nb > 0) {
+    const size_t red = (size_t)C * (PG / 32) * 24 * sizeof(float);
+    const int rc = with_model(model, "preprocessB_intrinsics: unknown camera model", [&](auto mdl) {
+      return with_flags(
+          [&](auto depth, auto aa) -> int {
+            constexpr bool DEPTH = decltype(depth)::value, AA = decltype(aa)::value;
+            constexpr int MODEL = decltype(mdl)::value;
+            GSB_DISPATCH_K3(k3, return (launch_intrinsics_kernel<K3, DEPTH, AA, MODEL>(
+                                    nb, red, C, N, pws, rots, scales, shs, pp, bc, moments, cinv2ds, g_depths,
+                                    alphas, po.part, st)));
+            return 0;
+          },
+          g_depths != nullptr, alphas != nullptr);
+    });
+    if (rc) return rc;
+  }
+  k_intrinsics_reduce<<<C, PR, 0, st>>>(nb, po.part, po.gcam, po.gint);
+  return 0;
+}
+
 int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t st) {
   const int N = sc.N;
   const PoseOut *po = b.po;
@@ -664,7 +793,16 @@ int launch_preprocess_bwd(const FusedScene &sc, const FusedBwd &b, cudaStream_t 
   ProfScope ps(K_PRE_BWD, st);
   // the camera gradient first; then, unless g_pws is NULL (pose only), the per-Gaussian gradients
   // from the form without POSE
-  if (po != nullptr) {
+  if (po != nullptr && po->gint != nullptr) {  // with the intrinsics' (DESIGN 3.23): a one-camera batch
+    BatchCams bc;
+    bc.f[0] = make_float4(sc.fx, sc.fy, sc.cx, sc.cy);
+    bc.k[0] = lk;
+    bc.tf[0] = tf;
+    if (int rc = launch_intrinsics_pass(1, N, sc.k3, sc.lens ? sc.lens->model : pg::PINHOLE, sc.pws, sc.rots,
+                                        sc.scales, sc.shs, PosePtrs{sc.Rcw, sc.tcw, sc.twc, 0}, bc, m.moments,
+                                        m.cinv2ds, b.g_depths, b.alphas, *po, st))
+      return rc;
+  } else if (po != nullptr) {
     if (nb > 0)
       if (int rc = pass(std::true_type{})) return rc;
     k_pose_reduce<<<1, PR, 0, st>>>(nb, part, po->gcam);
@@ -726,7 +864,12 @@ int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStre
   ProfScope ps(K_PRE_BWD_BATCH, st);
   // the camera gradients first (DESIGN 3.22); then, unless g_pws is NULL (pose only), the per-Gaussian
   // gradients from the kernel without the camera terms, so that they are the same bits either way
-  if (po != nullptr) {
+  if (po != nullptr && po->gint != nullptr) {  // with the intrinsics' (DESIGN 3.23)
+    if (int rc = launch_intrinsics_pass(b.C, b.N, b.k3, b.model, b.pws, b.rots, b.scales, b.shs,
+                                        PosePtrs{b.poses, b.poses + 9, b.poses + 12, 15}, *b.cams, g.moments,
+                                        g.cinv2ds, g.g_depths, g.alphas, *po, st))
+      return rc;
+  } else if (po != nullptr) {
     if (nb > 0)
       if (int rc = pass(std::true_type{})) return rc;
     k_pose_reduce_batch<<<b.C, PR, 0, st>>>(nb, po->part, po->gcam);

@@ -81,12 +81,18 @@ struct MomentsIn {
 };
 struct GradPush;
 // the camera gradient (fused.cu, POSE variants): gcam[15] = dL/dRcw (9), dL/dtcw (3), dL/dtwc (3);
-// part = ceil(N/128) partial rows of 16 floats (16-byte aligned), one per CTA
+// part = ceil(N/128) partial rows of 16 floats (16-byte aligned), one per CTA.  gint: NULL, or also the
+// intrinsics gradient gint[8] = dL/d(fx, fy, cx, cy, k[4]) (DESIGN 3.23, k_preprocess_bwd_intrinsics;
+// moment rows required); then the rows are 24 floats wide.
 struct PoseOut {
   float *gcam;
   float *part;
+  float *gint;
 };
 constexpr size_t pose_workspace_bytes(int N) { return N > 0 ? (size_t)((N + 127) / 128) * 16 * sizeof(float) : 0; }
+constexpr size_t intrinsics_workspace_bytes(int N) {
+  return N > 0 ? (size_t)((N + 127) / 128) * 24 * sizeof(float) : 0;
+}
 // The backward's gradients in and out.  gp == nullptr: the gradients go to g_pws, g_shs, g_scales,
 // g_rots; otherwise into the exchange staging slots gp describes (the g_* outputs are unused).
 // mi.moments == nullptr: the upstream gradients are g_us, g_cinv2ds, g_colors; otherwise the moment
@@ -138,6 +144,7 @@ struct BatchBwd {
   const PoseOut *po;
 };
 constexpr size_t batch_pose_workspace_bytes(int C, int N) { return (size_t)C * pose_workspace_bytes(N); }
+constexpr size_t batch_intrinsics_workspace_bytes(int C, int N) { return (size_t)C * intrinsics_workspace_bytes(N); }
 int launch_preprocess_bwd_batch(const BatchScene &b, const BatchBwd &g, cudaStream_t st);
 
 // dL/dsh[N,3k] = sum over V views of Y(dir_v) (x) dL/dcolor_v  (fused.cu k_sh_expand)

@@ -312,6 +312,76 @@ GSB_HD void lens_dJ_dpc(const float pc[3], const Cam &cam, const Lens &L, const 
   }
 }
 
+// The intrinsics gradient of one kept Gaussian under ORTHO / FISHEYE / OPENCV (DESIGN 3.23): gint[8] =
+// dL/d(fx, fy, cx, cy, k[4]) = gu . du/dtheta + sum_ab dJ_ab dJ_ab/dtheta, with dJ = dL/dJ as backward_one
+// forms it.  Row 0 of J and u - cx are fx times factors free of fx (and row 1, v - cy fy times), so the
+// fx, fy terms are those factors; dL/dcx = gu[0], dL/dcy = gu[1].  The clamp bound is a constant (as
+// in lens_dJ_dpc): a clamped coordinate contributes dJ/dtheta at the bound.
+//   FISHEYE: ds/dk_j = theta^(2j+1) / r, dg/dk_j = ((2j+1) theta^2j z / q - ds/dk_j) / r^2, dh/dk_j =
+//   (2j+1) theta^2j / q; below kFishSeries the derivatives of s and g come from their series to O(t^4)
+//   relative, ds/dk1 = t^2 (1 - t^2) / z, ds/dk2 = t^4 (1 - 5 t^2 / 3) / z, dg/dk1 = (2 - 4 t^2) / z^3,
+//   dg/dk2 = t^2 (4 - 10 t^2) / z^3, and k3's and k4's (O(t^4) and O(t^6) relative to k1's) are taken as 0.
+//   OPENCV: ddelta/dk at the unclamped (xn, yn) (in u), dDdelta/dk at the clamped (xh, yh) (in J).
+template <int MODEL>
+GSB_HD void lens_dintr(const float pc[3], const Cam &cam, const Lens &L, const float dJ[6], const float gu[2],
+                       float gint[8]) {
+  gint[2] = gu[0];
+  gint[3] = gu[1];
+  gint[4] = gint[5] = gint[6] = gint[7] = 0.f;
+  if constexpr (MODEL == ORTHO) {
+    gint[0] = fmaf(gu[0], pc[0], dJ[0]);
+    gint[1] = fmaf(gu[1], pc[1], dJ[4]);
+  } else if constexpr (MODEL == OPENCV) {
+    const float *k = cam.k;
+    const float zi = 1.0f / pc[2], xn = pc[0] * zi, yn = pc[1] * zi;
+    const float limx = 1.3f * cam.tan_fovx, limy = 1.3f * cam.tan_fovy;
+    const float a = fminf(limx, fmaxf(-limx, xn)), b = fminf(limy, fmaxf(-limy, yn));
+    float D[3];
+    opencv_D(a, b, k, D);
+    // dL/dD (J = (1/z) diag(f) [[D0, D1, -(D0 a + D1 b)], [D1, D2, -(D1 a + D2 b)]]) without the f
+    const float r0 = zi * fmaf(-dJ[2], a, dJ[0]), r1 = zi * fmaf(-dJ[2], b, dJ[1]);
+    const float s1 = zi * fmaf(-dJ[5], a, dJ[3]), s2 = zi * fmaf(-dJ[5], b, dJ[4]);
+    gint[0] = fmaf(r0, D[0], fmaf(r1, D[1], gu[0] * L.dlt[0]));
+    gint[1] = fmaf(s1, D[1], fmaf(s2, D[2], gu[1] * L.dlt[1]));
+    const float g0 = cam.fx * r0, g1 = fmaf(cam.fx, r1, cam.fy * s1), g2 = cam.fy * s2;
+    const float A = cam.fx * gu[0], B = cam.fy * gu[1];
+    const float rc = fmaf(a, a, b * b), ru = fmaf(xn, xn, yn * yn), ab = a * b, xy = xn * yn;
+    const float gd = fmaf(A, xn, B * yn);  // gu . diag(f) (xn, yn)
+    gint[4] = fmaf(g0, fmaf(2.f * a, a, rc), fmaf(g1, 2.f * ab, fmaf(g2, fmaf(2.f * b, b, rc), ru * gd)));
+    gint[5] = fmaf(rc, fmaf(g0, fmaf(4.f * a, a, rc), fmaf(g1, 4.f * ab, g2 * fmaf(4.f * b, b, rc))), ru * ru * gd);
+    gint[6] = fmaf(2.f * g0, b, fmaf(2.f * g1, a, fmaf(6.f * g2, b, fmaf(A, 2.f * xy, B * fmaf(2.f * yn, yn, ru)))));
+    gint[7] = fmaf(6.f * g0, a, fmaf(2.f * g1, b, fmaf(2.f * g2, a, fmaf(A, fmaf(2.f * xn, xn, ru), B * 2.f * xy))));
+  } else {
+    static_assert(MODEL == FISHEYE, "no intrinsics gradient for this camera model");
+    const float x = pc[0], y = pc[1], z = pc[2], xx = x * x, yy = y * y, xy = x * y;
+    const float a0 = dJ[0], a1 = dJ[1], a2 = dJ[2], b0 = dJ[3], b1 = dJ[4], b2 = dJ[5];
+    // row 0: J = fx (s + x^2 g, x y g, -x h), u - cx = fx s x;  row 1 likewise with fy
+    gint[0] = fmaf(a0, fmaf(xx, L.g, L.s), fmaf(a1, xy * L.g, fmaf(-a2, x * L.h, gu[0] * L.s * x)));
+    gint[1] = fmaf(b0, xy * L.g, fmaf(b1, fmaf(yy, L.g, L.s), fmaf(-b2, y * L.h, gu[1] * L.s * y)));
+    const float r2 = xx + yy, r = sqrtf(r2), q = fmaf(z, z, r2), qi = 1.0f / q, zi = 1.0f / z, t = r * zi;
+    const float th = atan2f(r, z), th2 = th * th;
+    // sum over both rows of dL/d(s, g, h) with the f's: dL/dtheta_k = Ss ds/dk + Sg dg/dk + Sh dh/dk
+    const float Ss = cam.fx * fmaf(gu[0], x, a0) + cam.fy * fmaf(gu[1], y, b1);
+    const float Sg = cam.fx * fmaf(a0, xx, a1 * xy) + cam.fy * fmaf(b0, xy, b1 * yy);
+    const float Sh = -(cam.fx * a2 * x + cam.fy * b2 * y);
+    float p = 1.f;  // theta^2j
+    for (int j = 0; j < 4; j++) {
+      p *= th2;
+      const float c = 2.f * j + 3.f;
+      float ds, dg;
+      if (t < kFishSeries) {
+        const float t2 = t * t, zi3 = zi * zi * zi;
+        ds = j == 0 ? zi * t2 * fmaf(-t2, 1.f, 1.f) : (j == 1 ? zi * t2 * t2 * fmaf(-5.f / 3.f, t2, 1.f) : 0.f);
+        dg = j == 0 ? zi3 * fmaf(-4.f, t2, 2.f) : (j == 1 ? zi3 * t2 * fmaf(-10.f, t2, 4.f) : 0.f);
+      } else {
+        ds = p * th / r;
+        dg = (c * p * z * qi - ds) / r2;
+      }
+      gint[4 + j] = fmaf(Ss, ds, fmaf(Sg, dg, Sh * (c * p * qi)));
+    }
+  }
+}
+
 // Antialiasing (2D-filter opacity compensation, Mip-Splatting; gsplat's rasterize_mode
 // "antialiased"): the blur spreads a Gaussian's mass, so its opacity is scaled by
 //   rho = sqrt(max(kAaMinR, r)),  r = det(Sigma) / det(Sigma + kBlur I) = (a c - b^2) di
@@ -469,11 +539,16 @@ GSB_HD float forward_one(const float pw[3], const float q[4], const float s[3], 
 //   dr/da = w (c c' + b^2) di^2,  dr/db = -2 w b (w + a + c) di^2,  dr/dc = w (a a' + b^2) di^2,
 // drho = dr / (2 rho), and 0 where the clamp holds (r <= kAaMinR).  galpha != 0 alone makes the
 // Gaussian's geometry gradient non-zero, so it joins the zero-gradient gate.
-template <int K3, bool DEPTH = false, bool POSE = false, bool AA = false, int MODEL = PINHOLE>
+// INTR (with POSE): gcam[15..22] also receives the intrinsics gradient dL/d(fx, fy, cx, cy, k[4])
+// (lens_dintr; PINHOLE: the same with J00 = fx/z, J02 = -fx xc/z^2, u - cx = fx x/z and k's 0), from the
+// same dJ and gu, antialiasing's term included; 0 for a culled Gaussian.
+template <int K3, bool DEPTH = false, bool POSE = false, bool AA = false, int MODEL = PINHOLE, bool INTR = false>
 GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3], const float *sh,
                           const Cam &cam, const float gu[2], const float gconic[3], const float gcol[3],
                           float gpw[3], float gq[4], float gs[3], float *gsh /*[K3][3]*/, float gdepth = 0.f,
-                          float *gcam = nullptr /*[15], POSE only*/, float galpha = 0.f, float alpha = 0.f) {
+                          float *gcam = nullptr /*[15], POSE only; [23] with INTR*/, float galpha = 0.f,
+                          float alpha = 0.f) {
+  static_assert(!INTR || POSE, "the intrinsics gradient comes with the pose's");
   // ---- colour branch (independent of the depth cull, like sh2Color)
   float Y[K3], dY[K3][3];
   float d[3], ninv = 1.f, r[3] = {0.f, 0.f, 0.f};
@@ -499,6 +574,8 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
   if (POSE) {
     for (int e = 0; e < 12; e++) gcam[e] = 0.f;
     for (int a = 0; a < 3; a++) gcam[12 + a] = -gpw[a];
+    if (INTR)
+      for (int e = 15; e < 23; e++) gcam[e] = 0.f;
   }
   gq[0] = gq[1] = gq[2] = gq[3] = 0.f;
   gs[0] = gs[1] = gs[2] = 0.f;
@@ -587,6 +664,12 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
         gcam[9 + k] = gpc[k];
       }
     }
+    if (INTR) {
+      gcam[15] = fmaf(dJ[0], zi, fmaf(-dJ[2], g.xc * zi2, gu[0] * (g.pc[0] * zi)));
+      gcam[16] = fmaf(dJ[4], zi, fmaf(-dJ[5], g.yc * zi2, gu[1] * (g.pc[1] * zi)));
+      gcam[17] = gu[0];
+      gcam[18] = gu[1];
+    }
   } else {
     // ORTHO / FISHEYE: u has the exact Jacobian J (no clamp), and the cov2d term goes through dJ/dpc
     // (0 for ORTHO, whose J is constant).  OPENCV: u's Jacobian is the unclamped Ju, cov2d's the clamped J.
@@ -607,6 +690,7 @@ GSB_HD float backward_one(const float pw[3], const float q[4], const float s[3],
           gcam[3 * a2 + k] = fmaf(gpc[a2], pw[k], fmaf(J[a2], dM[k], J[3 + a2] * dM[3 + k]));
       for (int k = 0; k < 3; k++) gcam[9 + k] = gpc[k];
     }
+    if (INTR) lens_dintr<MODEL>(g.pc, cam, g.L, dJ, gu, gcam + 15);
   }
   // cov3d: dL/dM3 = 2 sym(g3) M3
   const float G3[9] = {g3[0], 0.5f * g3[1], 0.5f * g3[2], 0.5f * g3[1], g3[3], 0.5f * g3[4],

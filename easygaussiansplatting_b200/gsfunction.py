@@ -6,6 +6,8 @@ seven operators in the same order, so it is the caller contract the parity and b
 harnesses exercise on the GPU box (where the reference tree itself is not available).
 The reference's own gsplat/gsmodel.py runs unmodified on top of `gsplatcu` as well.
 """
+import math
+
 import torch
 
 
@@ -90,6 +92,41 @@ def colmap_intrinsics(model_name, params, width, height, image_width=None, image
 def _pinhole_only(cam, what):
     if getattr(cam, "camera_model", "pinhole") != "pinhole":
         raise ValueError("%s takes pinhole cameras only, got camera_model=%r" % (what, cam.camera_model))
+
+
+def _intrinsics_rows(intrinsics, shape):
+    """the host values of the pose classes' `intrinsics` tensor ([8] or [C, 8], fx, fy, cx, cy, k[4]): a
+    CUDA tensor costs one small device-to-host copy and a wait, a CPU tensor neither"""
+    if not isinstance(intrinsics, torch.Tensor) or not intrinsics.dtype.is_floating_point or \
+            tuple(intrinsics.shape) != shape:
+        raise ValueError("intrinsics must be a float tensor of shape %s, got %s"
+                         % (list(shape), tuple(getattr(intrinsics, "shape", ()))))
+    rows = intrinsics.detach().to(device="cpu", dtype=torch.float32).reshape(-1, 8).tolist()
+    if not all(math.isfinite(v) for r in rows for v in r):
+        raise ValueError("intrinsics must be finite")
+    return rows
+
+
+def _with_intrinsics(cam, row):
+    """a Camera with cam's size, pose, model and antialiasing and the intrinsics row (fx, fy, cx, cy,
+    k[4]): opencv's k = (k1, k2, p1, p2), fisheye's k1..k4, 0 for pinhole and ortho"""
+    model = getattr(cam, "camera_model", "pinhole")
+    fx, fy, cx, cy, k = row[0], row[1], row[2], row[3], tuple(row[4:])
+    radial = tangential = None
+    if model in ("pinhole", "ortho"):
+        if any(k):
+            raise ValueError("intrinsics: k must be 0 for camera_model=%r, got %s" % (model, k))
+    elif model == "opencv":
+        radial, tangential = k[:2], k[2:]
+    else:
+        radial = k
+    out = Camera(cam.width, cam.height, fx, fy, cx, cy, cam.Rcw, cam.tcw, cam.twc,
+                 antialiased=getattr(cam, "antialiased", False), camera_model=model, radial_coeffs=radial,
+                 tangential_coeffs=tangential)
+    for name, value in vars(cam).items():  # the caller's other fields (grad_exchange, ...) come along
+        if name not in vars(out):
+            setattr(out, name, value)
+    return out
 
 
 def build_gsfunction(gsc):
@@ -210,7 +247,7 @@ class GSFunctionFusedRGBD(torch.autograd.Function):
 
 
 def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None, filter3d=None, features=None,
-                   us_abs=None):
+                   us_abs=None, intrinsics=None):
     """The forward of the fused classes: the colour or (rgbd) RGB-D frame.  pose: None (the
     camera is cam.Rcw, cam.tcw, cam.twc) or the tensors (Rcw, tcw, twc), then saved for the backward.
     cam.antialiased (absent: False): the rasterizers composite alpha_eff = rho * alpha.
@@ -219,9 +256,15 @@ def _fused_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cam, pose=None
     features: None, or [N, D]: the feature map [D, H, W] follows the image (ops.splat_features,
     from the same records) and features is saved last.
     us_abs: None, or the [N,2] dummy input whose gradient is the absolute-gradient statistic; its
-    gradient slot (after cam and filter3d) is kept in ctx.abs_slot."""
+    gradient slot (after cam and filter3d) is kept in ctx.abs_slot.
+    intrinsics (pose classes): None, or the [8] tensor whose values replace cam's intrinsics and lens
+    (DESIGN 3.23); its gradient slot (after us_abs) is kept in ctx.intr_slot."""
     from . import ops
-    ctx.abs_slot = None
+    ctx.abs_slot = ctx.intr_slot = None
+    if intrinsics is not None:
+        cam = _with_intrinsics(cam, _intrinsics_rows(intrinsics, (8,))[0])
+        ctx.intr_slot = 12
+        ctx.intr_like = (intrinsics.device, intrinsics.dtype, intrinsics.shape)
     if getattr(cam, "grad_exchange", None) is not None:
         _pinhole_only(cam, "the gradient exchange (cam.grad_exchange)")
     if us_abs is not None:
@@ -289,10 +332,13 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
     Rcw, tcw, twc = rest[:3] if pose else (cam.Rcw, cam.tcw, cam.twc)
     raw = rest[3:] if pose else rest  # (scales, alphas, filter3d) of a filtered frame
     need_abs = ctx.abs_slot is not None and ctx.needs_input_grad[ctx.abs_slot]
+    need_intr = ctx.intr_slot is not None and ctx.needs_input_grad[ctx.intr_slot]
     grads = _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds,
                                  depths, colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw,
                                  twc, dloss_dgammas, dloss_ddepth, dloss_dalpha, feat if featured else None,
-                                 absgrad=need_abs)
+                                 absgrad=need_abs, intr=need_intr)
+    if need_intr:
+        grads, dintr = grads[:-1], grads[-1]
     if need_abs:
         grads, dabs = grads[:-1], grads[-1]
     if featured:  # dL/dfeatures goes right after the map inputs (the pose classes take no features)
@@ -306,19 +352,23 @@ def _fused_backward(ctx, rgbd, pose, dloss_dgammas, dloss_ddepth=None, dloss_dal
         grads = grads + (dfeat,)
     if need_abs:  # cam and filter3d get None, us_abs the statistic
         grads = grads + (None,) * (ctx.abs_slot - len(grads)) + (dabs,)
+    if need_intr:
+        dev, dtype, shape = ctx.intr_like
+        grads = grads + (None,) * (ctx.intr_slot - len(grads)) + (dintr.to(device=dev, dtype=dtype).reshape(shape),)
     # one gradient per input apply received (cam, and filter3d when passed -- also as None -- get None)
     return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
 def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, scales, rots, us, cinv2ds, depths,
                          colors, contrib, final_tau, patch_range_per_tile, gsid_per_patch, Rcw, tcw, twc,
-                         dloss_dgammas, dloss_ddepth, dloss_dalpha, feat=None, absgrad=False):
+                         dloss_dgammas, dloss_ddepth, dloss_dalpha, feat=None, absgrad=False, intr=False):
     """the gradients of the inputs the frame was rendered from, up to and including the pose's;
     feat: None, or (features, dL/dfeature map or None) -> dL/dfeatures (None when no map gradient
     came) appended; absgrad: the rasterizer's _abs kernel runs and its dloss_dus_abs[N,2] is
-    appended last (not with feat)"""
+    appended; intr (pose): dL/dintrinsics[8] is appended last"""
     need_map = any(ctx.needs_input_grad[:6])
-    need_cam = pose and any(ctx.needs_input_grad[6:9])
+    need_pose = pose and any(ctx.needs_input_grad[6:9])
+    need_cam = need_pose or intr
     # the rasterizer backward leaves its raw moment rows; the fused per-Gaussian backward converts
     # them in registers (no finalize pass, no 32 B/Gaussian round trip).  (autograd hands zeros for
     # an RGB-D output the loss does not use: all three planes are given)  With antialiasing the
@@ -359,18 +409,20 @@ def _fused_backward_core(ctx, rgbd, pose, ops, cam, pws, shs, alphas, drawn, sca
     out = ops.preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, cam.fx, cam.fy, cam.cx, cam.cy, cam.width,
                           cam.height, None, None, None, moments=moments, cinv2ds=cinv2ds, dloss_ddepths=ddepths,
                           camera_grad=need_cam, pose_only=need_cam and not need_map, antialiased=ctx.aa,
-                          alphas=alphas if ctx.aa else None, **camera_model_kwargs(cam))
+                          alphas=alphas if ctx.aa else None, intrinsics_grad=intr, **camera_model_kwargs(cam))
     if need_map:
         dpws, dshs, dscales, drots, dloss_dus, dloss_dalphas = out[:6]
         grads = (dpws, dshs, dloss_dalphas.reshape(ctx.alpha_shape), dscales, drots, dloss_dus)
     else:
         grads = (None,) * 6
-    if need_cam:
+    if need_pose:
         grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
     elif pose:
         grads += (None, None, None)
     if absgrad:
-        return grads + (dabs,)
+        grads += (dabs,)
+    if intr:
+        grads += (out[-1],)
     return grads + (dfeat,) if feat is not None else grads
 
 
@@ -415,11 +467,16 @@ class GSFunctionFusedBatchPose(torch.autograd.Function):
     autograd chain it.  What runs follows ctx.needs_input_grad: only the poses -> the pose-only pass (a
     frozen map: tracking several frames, or the poses' step of windowed bundle adjustment); no pose ->
     exactly GSFunctionFusedBatch's backward; both -> the pose pass, then that backward.  filter3d as for
-    GSFunctionFusedBatch."""
+    GSFunctionFusedBatch.
+    intrinsics (after filter3d; DESIGN 3.23): None, or a float tensor [C, 8], row c as
+    GSFunctionFusedPose's intrinsics for cams[c], with the same host-copy trade-off and the gradient
+    per camera.  One physical camera shared by every view: pass intrinsics[None].expand(C, 8) and
+    autograd sums the rows."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None):
-        return _batch_forward(ctx, False, pws, shs, alphas, scales, rots, us, cams, filter3d, (Rcws, tcws, twcs))
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None, intrinsics=None):
+        return _batch_forward(ctx, False, pws, shs, alphas, scales, rots, us, cams, filter3d, (Rcws, tcws, twcs),
+                              intrinsics)
 
     @staticmethod
     def backward(ctx, dloss_dimage, _):
@@ -430,11 +487,12 @@ class GSFunctionFusedBatchRGBDPose(torch.autograd.Function):
     """GSFunctionFusedBatchRGBD with differentiable camera poses, as GSFunctionFusedBatchPose:
     `apply(pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None)` -> (image[C,3,H,W],
     depth[C,H,W], alpha[C,H,W], mask[C,N]).  The depth planes' gradients reach the poses through
-    z = (Rcw pw + tcw)[2]."""
+    z = (Rcw pw + tcw)[2].  intrinsics (after filter3d) as for GSFunctionFusedBatchPose."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None):
-        return _batch_forward(ctx, True, pws, shs, alphas, scales, rots, us, cams, filter3d, (Rcws, tcws, twcs))
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcws, tcws, twcs, cams, filter3d=None, intrinsics=None):
+        return _batch_forward(ctx, True, pws, shs, alphas, scales, rots, us, cams, filter3d, (Rcws, tcws, twcs),
+                              intrinsics)
 
     @staticmethod
     def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, _):
@@ -452,10 +510,17 @@ def _batch_poses(pose, C, dev):
     return torch.cat([x.detach().reshape(C, -1).to(torch.float32) for x in pose], 1).contiguous()
 
 
-def _batch_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cams, filter3d, pose=None):
-    """the forward of the batch classes; pose: None (the cameras' own poses) or (Rcws, tcws, twcs)"""
+def _batch_forward(ctx, rgbd, pws, shs, alphas, scales, rots, us, cams, filter3d, pose=None, intrinsics=None):
+    """the forward of the batch classes; pose: None (the cameras' own poses) or (Rcws, tcws, twcs);
+    intrinsics: None or the [C, 8] tensor whose rows replace the cameras' intrinsics (gradient slot 11)"""
     from . import ops
     ctx.pose = pose is not None
+    ctx.intr_slot = None
+    if intrinsics is not None:
+        cams = list(cams)
+        cams = [_with_intrinsics(c, r) for c, r in zip(cams, _intrinsics_rows(intrinsics, (len(cams), 8)))]
+        ctx.intr_slot = 11
+        ctx.intr_like = (intrinsics.device, intrinsics.dtype, intrinsics.shape)
     if ctx.pose:
         bc = ops.BatchCameras(cams, pws.device, poses=_batch_poses(pose, len(cams), pws.device))
         ctx.cam_shapes = tuple(x.shape for x in pose)
@@ -494,10 +559,12 @@ def _batch_backward(ctx, dloss_dimage, dloss_ddepth=None, dloss_dalpha=None):
                           dloss_dimage, dloss_ddepth if ctx.rgbd else None, dloss_dalpha, records=records)
     moments, ddepths = rb if ctx.rgbd else (rb, None)
     need_map = any(ctx.needs_input_grad[:6])
-    need_cam = ctx.pose and any(ctx.needs_input_grad[6:9])
+    need_pose = ctx.pose and any(ctx.needs_input_grad[6:9])
+    need_intr = ctx.intr_slot is not None and ctx.needs_input_grad[ctx.intr_slot]
+    need_cam = need_pose or need_intr
     out = ops.preprocessB_batch(pws, rots, scales, shs, bc, moments, cinv2ds, dloss_ddepths=ddepths,
                                 alphas=alphas if bc.antialiased else None, camera_grad=need_cam,
-                                pose_only=need_cam and not need_map)
+                                pose_only=need_cam and not need_map, intrinsics_grad=need_intr)
     if need_map:
         dpws, dshs, dscales, drots, dus, dalphas = out[:6]
         if ctx.filtered:  # the gradients are those of s', alpha'; the filter's backward runs once, after the batch sum
@@ -505,10 +572,13 @@ def _batch_backward(ctx, dloss_dimage, dloss_ddepth=None, dloss_dalpha=None):
         grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
     else:
         grads = (None,) * 6
-    if need_cam:
+    if need_pose:
         grads += tuple(d.reshape(s) for d, s in zip(out[6], ctx.cam_shapes))
     elif ctx.pose:
         grads += (None,) * 3
+    if need_intr:
+        dev, dtype, shape = ctx.intr_like
+        grads += (None,) * (ctx.intr_slot - len(grads)) + (out[-1].to(device=dev, dtype=dtype).reshape(shape),)
     return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
@@ -544,13 +614,22 @@ class GSFunctionFusedPose(torch.autograd.Function):
     and get dL/dRcw, dL/dtcw, dL/dtwc as independent inputs: a caller that builds twc from Rcw
     and tcw with torch ops has autograd chain it.  What runs follows ctx.needs_input_grad:
     only the camera -> the pose-only kernel (a frozen map: tracking); no camera -> exactly
-    GSFunctionFused's backward.  Intrinsics are not differentiated; single view only.  us_abs (after
-    filter3d) as for GSFunctionFused, also with the pose-only backward."""
+    GSFunctionFused's backward.  Single view only.  us_abs (after filter3d) as for GSFunctionFused, also
+    with the pose-only backward.
+    intrinsics (after us_abs; DESIGN 3.23): None, or a float tensor [8] = (fx, fy, cx, cy, k[4]) (k:
+    opencv's k1, k2, p1, p2, fisheye's k1..k4, 0 for pinhole and ortho) whose values replace cam's
+    intrinsics and lens for the render and the backward (cam still supplies size, model and
+    antialiasing); it gets dL/dintrinsics when it requires a gradient.  The host needs its values: a
+    CUDA tensor costs a 32-byte device-to-host copy and a wait per forward, a CPU tensor neither; the
+    gradient comes back on the tensor's device.  Asking for the intrinsics alone runs the camera pass
+    alone (a frozen map, a fixed pose).  Tied parameters (a SIMPLE_* model's single f) are the caller's
+    autograd graph: build the tensor from them with torch ops."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None, us_abs=None):
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None, us_abs=None,
+                intrinsics=None):
         return _fused_forward(ctx, False, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d,
-                              us_abs=us_abs)
+                              us_abs=us_abs, intrinsics=intrinsics)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, _):
@@ -561,12 +640,14 @@ class GSFunctionFusedRGBDPose(torch.autograd.Function):
     """GSFunctionFusedRGBD with a differentiable camera pose, as GSFunctionFusedPose:
     `apply(pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam)` -> (image, depth, alpha,
     depths > 0.2).  The depth plane's gradient reaches the pose through z = (Rcw pw + tcw)[2].
-    us_abs (after filter3d) as for GSFunctionFusedRGBD."""
+    us_abs (after filter3d) as for GSFunctionFusedRGBD, intrinsics (after us_abs) as for
+    GSFunctionFusedPose."""
 
     @staticmethod
-    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None, us_abs=None):
+    def forward(ctx, pws, shs, alphas, scales, rots, us, Rcw, tcw, twc, cam, filter3d=None, us_abs=None,
+                intrinsics=None):
         return _fused_forward(ctx, True, pws, shs, alphas, scales, rots, us, cam, (Rcw, tcw, twc), filter3d,
-                              us_abs=us_abs)
+                              us_abs=us_abs, intrinsics=intrinsics)
 
     @staticmethod
     def backward(ctx, dloss_dgammas, dloss_ddepth, dloss_dalpha, _):

@@ -649,7 +649,7 @@ def preprocess_batch(pws, rots, scales, shs, cams, alphas):
 
 
 def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddepths=None, alphas=None,
-                      camera_grad=False, pose_only=False):
+                      camera_grad=False, pose_only=False, intrinsics_grad=False):
     """Backward of `preprocess_batch` from the moment rows [C N, 9] of `splatB_batch` and the
     forward's cinv2ds [C,N,3] (gsb_preprocess_backward_batch): the C cameras' contributions summed
     in fp32 registers in camera order.  dloss_ddepths [C N]: the RGB-D term; alphas [N]: the raw
@@ -660,9 +660,14 @@ def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddep
     camera gradients (dRcws[C,3,3], dtcws[C,3], dtwcs[C,3]) -- views of one [C, 15] tensor; row c is
     what `preprocessB(..., camera_grad=True)` gives for camera c alone.  The per-Gaussian outputs are
     the same bits as without it.  pose_only (with camera_grad): the map is frozen; the six
-    per-Gaussian outputs are not computed and come back as None."""
+    per-Gaussian outputs are not computed and come back as None.
+    intrinsics_grad (with camera_grad; DESIGN 3.23, gsb_preprocess_backward_batch_intrinsics): one more
+    output follows, dintrinsics[C, 8] in the layout of BatchCameras.intrinsics; row c is what
+    `preprocessB(..., intrinsics_grad=True)` gives for camera c alone."""
     if pose_only and not camera_grad:
         raise ValueError("pose_only=True needs camera_grad=True")
+    if intrinsics_grad and not camera_grad:
+        raise ValueError("intrinsics_grad=True needs camera_grad=True")
     (pws, rots, scales, shs), N, k = _gaussian_map(pws, rots, scales, shs)
     bc = _batch_cams(cams, pws.device)
     Cn = bc.C
@@ -686,7 +691,14 @@ def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddep
     with torch.cuda.device(pws.device):
         args = (Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(moments), _ptr(cinv2ds),
                 _ptr(dloss_ddepths), _ptr(alphas), _ptr(gpw), _ptr(gsh), _ptr(gs), _ptr(gq), _ptr(dus), _ptr(dal))
-        if camera_grad:
+        if intrinsics_grad:
+            gcam = torch.empty((Cn, 15), **o)
+            gint = torch.empty((Cn, BATCH_INTRINSICS_ROW), **o)
+            ws_bytes = int(lib.gsb_preprocess_backward_batch_intrinsics_workspace_bytes(Cn, N))
+            ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
+            _lib.check(lib.gsb_preprocess_backward_batch_intrinsics(*args, _ptr(gcam), _ptr(gint), _ptr(ws), ws_bytes,
+                                                                    _stream()), lib)
+        elif camera_grad:
             gcam = torch.empty((Cn, 15), **o)
             ws_bytes = int(lib.gsb_preprocess_backward_batch_pose_workspace_bytes(Cn, N))
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
@@ -696,6 +708,8 @@ def preprocessB_batch(pws, rots, scales, shs, cams, moments, cinv2ds, dloss_ddep
     out = [gpw, gsh, gs, gq, dus, dal]
     if camera_grad:
         out.append((gcam[:, :9].view(Cn, 3, 3), gcam[:, 9:12], gcam[:, 12:15]))
+    if intrinsics_grad:
+        out.append(gint)
     return out
 
 
@@ -1023,7 +1037,7 @@ def preprocess(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x
 def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_x, center_y, width, height,
                 dloss_dus, dloss_dcinv2ds, dloss_dcolors, moments=None, cinv2ds=None, compact=False,
                 dloss_ddepths=None, camera_grad=False, pose_only=False, antialiased=False, alphas=None,
-                camera_model="pinhole", radial_coeffs=None, tangential_coeffs=None):
+                camera_model="pinhole", radial_coeffs=None, tangential_coeffs=None, intrinsics_grad=False):
     """Vector-Jacobian products of the five per-Gaussian stages (== the torch.bmm chain of
     gsmodel.py:72-85).  -> [dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dscales[N,3], dloss_drots[N,4]]
     With moments[N,9] (from `splatB(..., moments_only=True)`) and the forward's cinv2ds[N,3] the
@@ -1045,7 +1059,14 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     through rho (gsb_preprocess_backward_aa).  Combines with compact, dloss_ddepths, camera_grad
     and pose_only.
     camera_model, radial_coeffs, tangential_coeffs: as for `preprocess` (gsb_preprocess_backward_model);
-    a model other than pinhole needs the moment rows and combines with everything above."""
+    a model other than pinhole needs the moment rows and combines with everything above.
+    intrinsics_grad (with camera_grad and the moment rows; DESIGN 3.23,
+    gsb_preprocess_backward_intrinsics): one more output follows the camera gradient, dintrinsics[8] =
+    dL/d(focal_x, focal_y, center_x, center_y, k[4]) with k the camera model's coefficients (opencv: k1,
+    k2, p1, p2; fisheye: k1..k4; 0 for pinhole and ortho).  The clamp bound, culls and tile rectangles
+    are held constant."""
+    if intrinsics_grad and (not camera_grad or moments is None):
+        raise ValueError("intrinsics_grad=True needs camera_grad=True and the moment rows")
     cm = _camera_model_ptr(camera_model, radial_coeffs, tangential_coeffs, focal_x, focal_y)
     if cm is not None and moments is None:
         raise ValueError("camera_model=%r needs the moment rows" % camera_model)
@@ -1096,9 +1117,15 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
         ws_bytes = 0
         if camera_grad:
             gcam = torch.empty((15,), **o)
-            ws_bytes = int(lib.gsb_preprocess_backward_pose_workspace_bytes(N))
+            ws_bytes = int(lib.gsb_preprocess_backward_intrinsics_workspace_bytes(N) if intrinsics_grad else
+                           lib.gsb_preprocess_backward_pose_workspace_bytes(N))
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=pws.device)
-        if cm is not None:
+        if intrinsics_grad:
+            gint = torch.empty((8,), **o)
+            _lib.check(lib.gsb_preprocess_backward_intrinsics(*args, _ptr(dloss_ddepths),
+                                                              _ptr(alphas if antialiased else None), _ptr(gcam),
+                                                              _ptr(gint), _ptr(ws), ws_bytes, cm, _stream()), lib)
+        elif cm is not None:
             _lib.check(lib.gsb_preprocess_backward_model(*args, _ptr(dloss_ddepths), _ptr(alphas if antialiased else None),
                                                          _ptr(gcam), _ptr(ws), ws_bytes, cm, _stream()), lib)
         elif antialiased:
@@ -1114,6 +1141,8 @@ def preprocessB(pws, rots, scales, shs, Rcw, tcw, twc, focal_x, focal_y, center_
     out = [gpw, gsh, gs, gq] + ([dus, dal] if moments is not None else [])
     if camera_grad:
         out.append((gcam[:9].view(3, 3), gcam[9:12], gcam[12:15]))
+    if intrinsics_grad:
+        out.append(gint)
     return out
 
 

@@ -133,8 +133,9 @@ int gsb_preprocess_backward_rgbd(int N, int sh_dim3, const float *pws, const flo
  * Gaussians:  dL/dtcw = sum dL/dpc,  dL/dRcw = sum dL/dpc (x) pw + J^T dL/d(J Rcw),
  * dL/dtwc = -sum (colour part of dL/dpw) (0 at SH degree 0).  dL/dpc is the vector the backward
  * rotates into dloss_dpws (x, y differentiated as if unclamped, as there); a culled Gaussian
- * contributes through its colour only.  Intrinsics are not differentiated, and Rcw, tcw, twc
- * are independent inputs (twc = -Rcw^T tcw is the caller's relation to chain).
+ * contributes through its colour only.  Intrinsics are differentiated by
+ * gsb_preprocess_backward_intrinsics, and Rcw, tcw, twc are independent inputs (twc = -Rcw^T tcw is
+ * the caller's relation to chain).
  * dloss_dpws, dloss_dshs, dloss_dscales, dloss_drots (and with moments dloss_dus_out,
  * dloss_dalphas_out) are all set -- the same per-Gaussian outputs as gsb_preprocess_backward,
  * bit for bit (they come from the same kernel, after a pass that computes the camera gradient)
@@ -228,6 +229,32 @@ int gsb_preprocess_backward_model(int N, int sh_dim3, const float *pws, const fl
                                   const float *cinv2ds, float *dloss_dus_out, float *dloss_dalphas_out,
                                   const float *dloss_ddepths, const float *alphas, float *dloss_dcamera, void *ws,
                                   size_t ws_bytes, const gsb_camera_model *camera_model, gsb_stream_t stream);
+
+/* Intrinsics gradient (extension, DESIGN 3.23; refining COLMAP or guessed calibration).
+ * gsb_preprocess_backward_model's arguments (moment rows required) with dloss_dcamera[15] required,
+ * plus dloss_dintrinsics[8] (required) = dL/d(fx, fy, cx, cy, k[4]) summed over the N Gaussians, k
+ * as gsb_camera_model.k (0 under PINHOLE and ORTHO).  Per Gaussian, with dL/du and dL/dJ as the
+ * backward forms them (antialiasing's term included): dL/dfx = sum_b dL/dJ_0b dJ_0b/dfx + dL/du_0
+ * (u_0 - cx) / fx (taken from the factors, not by dividing), fy likewise with row 1, dL/dcx = dL/du_0,
+ * dL/dcy = dL/du_1, and the lens's k from theta_d (FISHEYE; its series branch near the axis,
+ * r/z < 0.03, carries k1 and k2 only) or delta and Ddelta (OPENCV).  Held constant: the +-1.3 tan_fov
+ * clamp bound (OPENCV's stretch included: a clamped coordinate contributes dJ/dtheta at the bound),
+ * the culls, the radius and the tile rectangles.  A culled Gaussian contributes nothing.  The
+ * per-Gaussian outputs are all set (then gsb_preprocess_backward_model's bits) or all NULL (camera
+ * only, a frozen map).  ws: caller-owned, 16-byte aligned, at least
+ * gsb_preprocess_backward_intrinsics_workspace_bytes(N) = ceil(N / 128) 96 bytes.  Summed in a fixed
+ * order in fp64: the same inputs give the same bits.  N = 0 writes zeros.  Errors before any launch:
+ * those of gsb_preprocess_backward_pose and _model, and a NULL dloss_dintrinsics. */
+size_t gsb_preprocess_backward_intrinsics_workspace_bytes(int N);
+int gsb_preprocess_backward_intrinsics(int N, int sh_dim3, const float *pws, const float *rots, const float *scales,
+                                       const float *shs, const float *Rcw, const float *tcw, const float *twc,
+                                       float fx, float fy, float cx, float cy, float width, float height,
+                                       const float *dloss_dus, const float *dloss_dcinv2ds, const float *dloss_dcolors,
+                                       float *dloss_dpws, float *dloss_dshs, float *dloss_dscales, float *dloss_drots,
+                                       const float *moments, const float *cinv2ds, float *dloss_dus_out,
+                                       float *dloss_dalphas_out, const float *dloss_ddepths, const float *alphas,
+                                       float *dloss_dcamera, float *dloss_dintrinsics, void *ws, size_t ws_bytes,
+                                       const gsb_camera_model *camera_model, gsb_stream_t stream);
 
 /* dL/dsh from per-view dL/dcolor (extension; multi-view data parallelism, SURVEY 8e).
  * colour = 0.5 + sum_l Y_l(dir) sh_l is linear in sh and never clamped (kernel.cu:735-774), so
@@ -904,7 +931,7 @@ int gsb_preprocess_backward_batch(int C, int N, int sh_dim3, const float *pws, c
 /* The camera gradients of the batch (DESIGN 3.22; pose refinement, windowed bundle adjustment, tracking
  * several frames).  gsb_preprocess_backward_batch's arguments plus dloss_dposes[C, 15]: per camera
  * dL/dRcw (row-major 9), dL/dtcw (3), dL/dtwc (3), as gsb_preprocess_backward_pose gives for that
- * camera alone (Rcw, tcw, twc independent inputs; intrinsics not differentiated).  The per-Gaussian
+ * camera alone (Rcw, tcw, twc independent inputs; intrinsics: gsb_preprocess_backward_batch_intrinsics).  The per-Gaussian
  * outputs are all set -- then they are gsb_preprocess_backward_batch's, bit for bit (the same kernel
  * writes them, after a pass that computes the camera gradients) -- or all NULL: pose only, for a
  * frozen map; nothing per Gaussian is written.  ws: caller-owned, 16-byte aligned, at least
@@ -921,6 +948,21 @@ int gsb_preprocess_backward_batch_pose(int C, int N, int sh_dim3, const float *p
                                        const float *alphas, float *dloss_dpws, float *dloss_dshs, float *dloss_dscales,
                                        float *dloss_drots, float *dloss_dus_out, float *dloss_dalphas_out,
                                        float *dloss_dposes, void *ws, size_t ws_bytes, gsb_stream_t stream);
+/* The batch's intrinsics gradients (DESIGN 3.23): gsb_preprocess_backward_batch_pose's arguments plus
+ * dloss_dintrinsics[C, GSB_BATCH_INTRINSICS_ROW] (device memory, required), row c = what
+ * gsb_preprocess_backward_intrinsics gives for camera c alone, in the layout of the intrinsics rows.
+ * ws: at least gsb_preprocess_backward_batch_intrinsics_workspace_bytes(C, N) = C ceil(N / 128) 96
+ * bytes (0 for what the entry point refuses).  Errors before any launch: those of
+ * gsb_preprocess_backward_batch_pose and a NULL dloss_dintrinsics. */
+size_t gsb_preprocess_backward_batch_intrinsics_workspace_bytes(int C, int N);
+int gsb_preprocess_backward_batch_intrinsics(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                             const float *scales, const float *shs, const float *poses,
+                                             const float *intrinsics, int camera_model, float width, float height,
+                                             const float *moments, const float *cinv2ds, const float *dloss_ddepths,
+                                             const float *alphas, float *dloss_dpws, float *dloss_dshs,
+                                             float *dloss_dscales, float *dloss_drots, float *dloss_dus_out,
+                                             float *dloss_dalphas_out, float *dloss_dposes, float *dloss_dintrinsics,
+                                             void *ws, size_t ws_bytes, gsb_stream_t stream);
 /* Phase 1 of the tall frame (gsb_splat_bin with C): record c N + n's rectangle is the single
  * frame's, clamped to frame c's tile rows, then moved down by c gy rows; N = per camera.  The batch's
  * workspace queries return 0 for C < 1, N < 0 or C N >= 2^31, which its entry points refuse. */
