@@ -148,6 +148,11 @@ SIGNATURES = {
     "gsb_bilagrid_slice_backward": (_i, [_i] * 4 + [_vp, _i, C.POINTER(C.c_int32), _i, _i] + [_vp] * 5),
     "gsb_bilagrid_tv_workspace_bytes": (_sz, [_i] * 4),
     "gsb_bilagrid_tv": (_i, [_i] * 4 + [_vp] * 4 + [_sz, _vp]),
+    "gsb_kmeans_assign_workspace_bytes": (_sz, [_i, _i]),
+    "gsb_kmeans_assign": (_i, [_i, _i, _i, _vp, _i64] + [_vp] * 4 + [_sz, _vp]),
+    "gsb_kmeans_update": (_i, [_i, _i, _i, _vp, _i64] + [_vp] * 6),
+    "gsb_quantize": (_i, [_i, _i, _vp, _i64, _i, _i, _i, _vp, _vp, _vp]),
+    "gsb_dequantize": (_i, [_i, _i, _vp, _i, _vp, _i, _vp, _vp]),
     "gsb_profile_enable": (None, [_i]),
     "gsb_profile_kernels": (_i, []),
     "gsb_profile_kernel_name": (C.c_char_p, [_i]),

@@ -19,7 +19,7 @@ OBJ = os.path.join(HERE, "_obj" + ("_" + VARIANT if VARIANT else ""))
 LIB = os.path.join(HERE, "libgsplat_b200%s.so" % ("_" + VARIANT if VARIANT else ""))
 SOURCES = ["api.cu", "pergaussian.cu", "fused.cu", "binning.cu", "raster_fwd.cu", "raster_bwd.cu", "loss.cu",
            "smallbmm.cu", "density.cu", "comm.cu", "filter3d.cu", "raster_feat.cu",
-           "adam.cu", "surfel.cu", "tsdf.cu", "raster_stats.cu", "bilagrid.cu"]
+           "adam.cu", "surfel.cu", "tsdf.cu", "raster_stats.cu", "bilagrid.cu", "compress.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo",

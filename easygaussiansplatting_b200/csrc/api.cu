@@ -44,7 +44,8 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "filter3d_apply", "filter3d_backward", "rects+scan_batch",
                                              "preprocess_forward_batch", "preprocess_backward_batch",
                                              "draw_batch", "draw_rgbd_batch", "draw_backward_batch",
-                                             "draw_backward_rgbd_batch", "density_apply_rows",
+                                             "draw_backward_rgbd_batch", "kmeans_assign", "kmeans_update",
+                                             "quantize", "dequantize", "density_apply_rows",
                                              "bilagrid_slice", "bilagrid_slice_backward", "bilagrid_tv",
                                              "draw_features", "draw_backward_features", "draw_stats",
                                              "draw_surfel_stats", "mcmc_scan",
@@ -1915,6 +1916,73 @@ int gsb_bilagrid_tv(int M, int L, int Y, int X, const float *grids, float *tv_ou
               "bilagrid_tv: misaligned array");
   GSB_REQUIRE(ws_bytes >= bilagrid_tv_workspace_bytes({M, L, Y, X}), "bilagrid_tv: workspace too small");
   return launch_bilagrid_tv({M, L, Y, X}, grids, tv_out, dloss_dgrids, ws, (cudaStream_t)stream);
+}
+
+// ---- compressed export (compress.cu, DESIGN 3.24)
+static_assert(KMEANS_MAX_DIM == GSB_KMEANS_MAX_DIM, "gsplat_b200.h and kernels.h disagree on the k-means width");
+
+// the shape checks of the k-means entry points; 0 or the argument error "<who>: <reason>"
+static int kmeans_shape(int N, int K, int D, int64_t ldx, const char *who) {
+  if (N < 0) return arg_error(who, "N < 0");
+  if (K < 1) return arg_error(who, "K < 1");
+  if (D < 1 || D > GSB_KMEANS_MAX_DIM) return arg_error(who, "D out of [1, 64]");
+  if (K > INT32_MAX - 127) return arg_error(who, "K overflows the centroid index");
+  if (ldx < D) return arg_error(who, "ldx < D");
+  if (N > 0 && ldx > INT64_MAX / N) return arg_error(who, "N ldx overflows the row offset");
+  return 0;
+}
+
+size_t gsb_kmeans_assign_workspace_bytes(int K, int D) {
+  if (kmeans_shape(0, K, D, D, "kmeans_assign_workspace_bytes")) return 0;
+  return kmeans_assign_workspace_bytes(K, D);
+}
+
+int gsb_kmeans_assign(int N, int K, int D, const float *x, int64_t ldx, const float *centroids, int32_t *labels,
+                      float *dist, void *ws, size_t ws_bytes, gsb_stream_t stream) {
+  if (int rc = kmeans_shape(N, K, D, ldx, "kmeans_assign")) return rc;
+  GSB_REQUIRE(centroids && ws, "kmeans_assign: null pointer");
+  GSB_REQUIRE(N == 0 || (x && labels && dist), "kmeans_assign: null pointer");
+  GSB_REQUIRE(aligned(x, 4) && aligned(centroids, 4) && aligned(labels, 4) && aligned(dist, 4) && aligned(ws, 16),
+              "kmeans_assign: misaligned array or workspace");
+  GSB_REQUIRE(ws_bytes >= kmeans_assign_workspace_bytes(K, D), "kmeans_assign: workspace too small");
+  return launch_kmeans_assign(N, K, D, x, ldx, centroids, labels, dist, ws, (cudaStream_t)stream);
+}
+
+int gsb_kmeans_update(int N, int K, int D, const float *x, int64_t ldx, const int32_t *labels, const int32_t *perm,
+                      const float *centroids, float *centroids_out, int32_t *counts, gsb_stream_t stream) {
+  if (int rc = kmeans_shape(N, K, D, ldx, "kmeans_update")) return rc;
+  GSB_REQUIRE(centroids && centroids_out && counts, "kmeans_update: null pointer");
+  GSB_REQUIRE(N == 0 || (x && labels && perm), "kmeans_update: null pointer");
+  GSB_REQUIRE(aligned(x, 4) && aligned(labels, 4) && aligned(perm, 4) && aligned(centroids, 4) &&
+                  aligned(centroids_out, 4) && aligned(counts, 4),
+              "kmeans_update: misaligned array");
+  return launch_kmeans_update(N, K, D, x, ldx, labels, perm, centroids, centroids_out, counts, (cudaStream_t)stream);
+}
+
+// the checks of the quantiser and its inverse
+static int quant_shape(int N, int D, int bits, const char *who) {
+  if (N < 0) return arg_error(who, "N < 0");
+  if (D < 1 || D > GSB_KMEANS_MAX_DIM) return arg_error(who, "D out of [1, 64]");
+  if (bits != 8 && bits != 16) return arg_error(who, "bits must be 8 or 16");
+  return 0;
+}
+
+int gsb_quantize(int N, int D, const float *x, int64_t ldx, int bits, int log_transform, int fit_range, float *range,
+                 void *codes, gsb_stream_t stream) {
+  if (int rc = quant_shape(N, D, bits, "quantize")) return rc;
+  GSB_REQUIRE(ldx >= D, "quantize: ldx < D");
+  GSB_REQUIRE(N == 0 || ldx <= INT64_MAX / N, "quantize: N ldx overflows the row offset");
+  GSB_REQUIRE(range != nullptr && (N == 0 || (x && codes)), "quantize: null pointer");
+  GSB_REQUIRE(aligned(x, 4) && aligned(range, 4) && aligned(codes, bits / 8), "quantize: misaligned array");
+  return launch_quantize(N, D, x, ldx, bits, log_transform != 0, fit_range != 0, range, codes, (cudaStream_t)stream);
+}
+
+int gsb_dequantize(int N, int D, const void *codes, int bits, const float *range, int log_transform, float *out,
+                   gsb_stream_t stream) {
+  if (int rc = quant_shape(N, D, bits, "dequantize")) return rc;
+  GSB_REQUIRE(N == 0 || (codes && range && out), "dequantize: null pointer");
+  GSB_REQUIRE(aligned(codes, bits / 8) && aligned(range, 4) && aligned(out, 4), "dequantize: misaligned array");
+  return launch_dequantize(N, D, codes, bits, range, log_transform != 0, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -19,7 +19,7 @@ enum KernelId {
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
   K_RECTS_BATCH, K_PRE_FWD_BATCH, K_PRE_BWD_BATCH, K_DRAW_BATCH, K_DRAW_RGBD_BATCH, K_DRAW_BWD_BATCH,
-  K_DRAW_BWD_RGBD_BATCH, K_DENSITY_ROWS, K_BILAGRID_SLICE, K_BILAGRID_SLICE_BWD, K_BILAGRID_TV, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
+  K_DRAW_BWD_RGBD_BATCH, K_KMEANS_ASSIGN, K_KMEANS_UPDATE, K_QUANTIZE, K_DEQUANTIZE, K_DENSITY_ROWS, K_BILAGRID_SLICE, K_BILAGRID_SLICE_BWD, K_BILAGRID_TV, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
   K_MCMC_ROWS, K_MCMC_NOISE, K_TSDF_INTEGRATE, K_TSDF_PLAN, K_TSDF_EMIT,
   K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
   K_DRAW_BWD_ABS, K_DRAW_BWD_RGBD_ABS, K_ADAM, K_DRAW_RGBD, K_DRAW_BWD_RGBD, K_COUNT
@@ -433,5 +433,23 @@ int launch_bilagrid_slice_bwd(const BilagridShape &s, const float *grids, int B,
 size_t bilagrid_tv_workspace_bytes(const BilagridShape &s);
 int launch_bilagrid_tv(const BilagridShape &s, const float *grids, float *tv, float *dgrids, void *ws,
                        cudaStream_t st);
+
+// ---- compressed export (compress.cu, DESIGN 3.24).  x[N, D] rows ldx floats apart (any 4-byte
+// alignment), 1 <= D <= KMEANS_MAX_DIM; centroids [K, D] contiguous.  The arguments are checked by the
+// entry points.
+constexpr int KMEANS_MAX_DIM = 64;
+// K rounded up to the 128-centroid tile; ws of the assignment: the transposed codebook and its norms
+int kmeans_padded(int K);
+size_t kmeans_assign_workspace_bytes(int K, int D);
+int launch_kmeans_assign(int N, int K, int D, const float *x, int64_t ldx, const float *centroids, int32_t *labels,
+                         float *dist, void *ws, cudaStream_t st);
+// perm: a stable ascending sort of labels (member lists in ascending point index)
+int launch_kmeans_update(int N, int K, int D, const float *x, int64_t ldx, const int32_t *labels, const int32_t *perm,
+                         const float *centroids, float *centroids_out, int32_t *counts, cudaStream_t st);
+// range[2, D] (lo row, hi row): fit_range: reduced here, else read; codes [N, D] uint8 (bits 8) or uint16
+int launch_quantize(int N, int D, const float *x, int64_t ldx, int bits, int log_t, int fit_range, float *range,
+                    void *codes, cudaStream_t st);
+int launch_dequantize(int N, int D, const void *codes, int bits, const float *range, int log_t, float *out,
+                      cudaStream_t st);
 
 }  // namespace gsb

@@ -236,6 +236,39 @@ def save_ply(path, gs):
         f.write(np.ascontiguousarray(rows, "<f4").tobytes())
 
 
+def save_compressed(path, training_params, sh_clusters=65536, iters=10, generator=None):
+    """Writes the six raw training tensors as one compressed scene file (compress.py, DESIGN 3.24):
+    the SH rows vector-quantised against a k-means codebook of min(sh_clusters, N) rows (`iters`
+    Lloyd iterations, initial centroids drawn with `generator`), the other attributes as 8 / 16-bit
+    codes, in an np.savez_compressed archive written to `path` as given.  19 N + 45 K bytes of codes
+    before deflate, against 248 N for save_ply.
+    A model trained with the Mip-Splatting 3D filter is baked first (bake_filter3d): the file holds
+    plain 3DGS parameters.  Raises ValueError on N = 0 or non-finite parameters."""
+    from . import compress as cz
+    for k in GAUSSIAN_TENSORS:
+        if k not in training_params:
+            raise ValueError("training_params has no %r" % k)
+    N = training_params["pws"].shape[0]
+    if N == 0:
+        raise ValueError("there is nothing to save (N = 0)")
+    for k in GAUSSIAN_TENSORS:
+        if not bool(torch.isfinite(training_params[k].detach()).all()):
+            raise ValueError("training_params[%r] is not finite" % k)
+    cz.write_npz(path, cz.to_numpy(cz.compress(training_params, sh_clusters, iters, generator)))
+
+
+def load_compressed(path, device="cuda"):
+    """save_compressed's file -> (params, adam_groups) as load_training_params returns them: the six
+    decoded raw tensors on `device`, leaves with requires_grad.  Reads without pickles; raises
+    ValueError on an unknown format or version, a missing array, a wrong dtype or shape, N or K that
+    disagree between the arrays, or a label >= K."""
+    from . import compress as cz
+    arrays, _ = cz.read_npz(path)
+    params = cz.decompress(cz.to_device(arrays, device))
+    params = {k: t.requires_grad_() for k, t in params.items()}
+    return params, adam_groups(params)
+
+
 def save_mesh_ply(path, verts, faces, colors=None):
     """Writes a triangle mesh (mesh.TSDFVolume.extract's output; tensors or arrays) as binary
     little-endian PLY: float x, y, z, with colors[V, 3] in [0, 1] also uchar red, green, blue

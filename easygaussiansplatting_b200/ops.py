@@ -1666,3 +1666,117 @@ def bilagrid_tv(grids, want_grad=True):
         _lib.check(lib.gsb_bilagrid_tv(*shape, _ptr(grids), _ptr(tv), _ptr(grad), _ptr(ws), ws.numel(), _stream()),
                    lib)
     return tv, grad
+
+
+# ----------------------------------------------------------------------------- compressed export
+KMEANS_MAX_DIM = 64
+
+
+def _rows(x, name):
+    """x: a float32 CUDA [N, D] tensor, 1 <= D <= 64, whose rows may sit any whole number of floats
+    apart (a column slice of a wider tensor is read in place) -> (x, row stride in floats)"""
+    if not isinstance(x, torch.Tensor):
+        raise TypeError("%s must be a torch.Tensor" % name)
+    if not x.is_cuda:
+        raise ValueError("%s must be a CUDA tensor (there is no CPU path)" % name)
+    if x.dtype != torch.float32:
+        raise TypeError("%s must be torch.float32, got %s" % (name, x.dtype))
+    if x.dim() != 2 or not 1 <= x.shape[1] <= KMEANS_MAX_DIM:
+        raise ValueError("%s must be [N, D] with 1 <= D <= %d, got %s" % (name, KMEANS_MAX_DIM, tuple(x.shape)))
+    if x.shape[1] > 1 and x.stride(1) != 1 or x.shape[0] > 1 and x.stride(0) < x.shape[1]:
+        x = x.contiguous()
+    return x, (x.stride(0) if x.shape[0] > 1 else x.shape[1])
+
+
+def kmeans_assign(x, centroids):
+    """The nearest centroid of every row of x[N, D] (gsb_kmeans_assign): a fused distance + argmin
+    that never forms the N x K distance matrix; ties go to the lowest index and the result is the
+    same bits on every run.  -> (labels int32 [N], squared distances float32 [N])"""
+    x, ldx = _rows(x, "x")
+    c = _chk(centroids, "centroids", ndim=2)
+    _same_device(x, c)
+    N, D = x.shape
+    K = c.shape[0]
+    if c.shape[1] != D or K < 1:
+        raise ValueError("centroids must be [K >= 1, %d], got %s" % (D, tuple(c.shape)))
+    labels = torch.empty((N,), dtype=torch.int32, device=x.device)
+    dist = torch.empty((N,), dtype=torch.float32, device=x.device)
+    lib = _L()
+    ws = _bytes(int(lib.gsb_kmeans_assign_workspace_bytes(K, D)), x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.gsb_kmeans_assign(N, K, D, _ptr(x), ldx, _ptr(c), _ptr(labels), _ptr(dist), _ptr(ws),
+                                         ws.numel(), _stream()), lib)
+    return labels, dist
+
+
+def kmeans_update(x, labels, centroids):
+    """One Lloyd update (gsb_kmeans_update): each centroid becomes the mean of the rows of x[N, D]
+    labelled with it, summed in fp64 in ascending row index; an empty cluster keeps its centroid bit
+    for bit.  labels: int32 [N] in [0, K).  -> (centroids float32 [K, D], counts int32 [K])"""
+    x, ldx = _rows(x, "x")
+    c = _chk(centroids, "centroids", ndim=2)
+    labels = _chk(labels, "labels", dtype=torch.int32, ndim=1)
+    _same_device(x, c, labels)
+    N, D = x.shape
+    K = c.shape[0]
+    if c.shape[1] != D or K < 1:
+        raise ValueError("centroids must be [K >= 1, %d], got %s" % (D, tuple(c.shape)))
+    if labels.shape[0] != N:
+        raise ValueError("labels must have N = %d elements, got %d" % (N, labels.shape[0]))
+    perm = torch.sort(labels, stable=True).indices.to(torch.int32)
+    out = torch.empty_like(c)
+    counts = torch.empty((K,), dtype=torch.int32, device=x.device)
+    lib = _L()
+    with torch.cuda.device(x.device):
+        _lib.check(lib.gsb_kmeans_update(N, K, D, _ptr(x), ldx, _ptr(labels), _ptr(perm), _ptr(c), _ptr(out),
+                                         _ptr(counts), _stream()), lib)
+    return out, counts
+
+
+def quantize(x, bits, log_transform=False, value_range=None):
+    """Per-column scalar quantisation of x[N, D] (gsb_quantize) to `bits` (8 or 16) bit codes:
+    q = clamp(floor((t - lo) (2^bits - 1) / (hi - lo) + 1/2)) of t = x, or sign(x) log1p(|x|) with
+    log_transform.  value_range: None (lo, hi = each column's min and max of t, reduced on the device)
+    or a float32 [2, D] tensor (lo row, hi row) to use instead.
+    -> (codes uint8 / uint16 [N, D], range float32 [2, D])"""
+    if bits not in (8, 16):
+        raise ValueError("bits must be 8 or 16, got %r" % (bits,))
+    x, ldx = _rows(x, "x")
+    N, D = x.shape
+    if value_range is None:
+        rng = torch.empty((2, D), dtype=torch.float32, device=x.device)
+    else:
+        rng = _chk(value_range, "value_range", ndim=2).clone()
+        _same_device(x, rng)
+        if tuple(rng.shape) != (2, D):
+            raise ValueError("value_range must be [2, %d], got %s" % (D, tuple(rng.shape)))
+    codes = torch.empty((N, D), dtype=torch.uint8 if bits == 8 else torch.uint16, device=x.device)
+    lib = _L()
+    with torch.cuda.device(x.device):
+        _lib.check(lib.gsb_quantize(N, D, _ptr(x), ldx, bits, int(bool(log_transform)), int(value_range is None),
+                                    _ptr(rng), _ptr(codes), _stream()), lib)
+    return codes, rng
+
+
+def dequantize(codes, value_range, log_transform=False):
+    """The inverse of `quantize` (gsb_dequantize): lo + q (hi - lo) / (2^bits - 1), then the inverse
+    of the log transform.  codes: uint8 or uint16 [N, D]; value_range: float32 [2, D].
+    -> float32 [N, D]"""
+    if not isinstance(codes, torch.Tensor) or codes.dtype not in (torch.uint8, torch.uint16):
+        raise TypeError("codes must be a uint8 or uint16 tensor")
+    if not codes.is_cuda:
+        raise ValueError("codes must be a CUDA tensor (there is no CPU path)")
+    if codes.dim() != 2 or not 1 <= codes.shape[1] <= KMEANS_MAX_DIM:
+        raise ValueError("codes must be [N, D] with 1 <= D <= %d, got %s" % (KMEANS_MAX_DIM, tuple(codes.shape)))
+    codes = codes.contiguous()
+    N, D = codes.shape
+    rng = _chk(value_range, "value_range", ndim=2)
+    _same_device(codes, rng)
+    if tuple(rng.shape) != (2, D):
+        raise ValueError("value_range must be [2, %d], got %s" % (D, tuple(rng.shape)))
+    out = torch.empty((N, D), dtype=torch.float32, device=codes.device)
+    lib = _L()
+    with torch.cuda.device(codes.device):
+        _lib.check(lib.gsb_dequantize(N, D, _ptr(codes), 8 if codes.dtype == torch.uint8 else 16, _ptr(rng),
+                                      int(bool(log_transform)), _ptr(out), _stream()), lib)
+    return out

@@ -893,6 +893,43 @@ size_t gsb_bilagrid_tv_workspace_bytes(int M, int L, int Y, int X);
 int gsb_bilagrid_tv(int M, int L, int Y, int X, const float *grids, float *tv_out, float *dloss_dgrids, void *ws,
                     size_t ws_bytes, gsb_stream_t stream);
 
+/* ---- compressed export (extension; DESIGN 3.24): the k-means vector quantiser of the SH rows and
+ * the 8 / 16-bit scalar quantiser of the other attributes (gsplat's `--compression` scheme).
+ *
+ * x[N, D] float32, row i at x + i ldx (ldx >= D floats, any 4-byte alignment: a column view of a
+ * wider tensor is fine); 1 <= D <= GSB_KMEANS_MAX_DIM.  centroids [K, D] contiguous, K >= 1.
+ * gsb_kmeans_assign: labels[N] int32 = the index of the nearest centroid, dist[N] = its squared
+ * distance, clamped at >= 0.  The score |c|^2 - 2 x.c is formed in fp32 FMA in a fixed order and
+ * ties go to the lowest index, so labels and dist are the same bits on every run; against the fp64
+ * distances d the chosen centroid is within tau = (D + 2) 2^-22 (|x| + max_k |c_k|)^2 of the nearest,
+ * and dist within tau of d(x, c_label).  ws: gsb_kmeans_assign_workspace_bytes(K, D) =
+ * (D + 1) ceil(K / 128) 512 bytes, 16-byte aligned (0 for what the entry point refuses).
+ * gsb_kmeans_update: centroids_out[K, D] = the mean of each cluster's members, summed in fp64 in
+ * ascending point index; an empty cluster copies its row of centroids bit for bit; counts[K] int32.
+ * perm[N]: a stable ascending sort of labels (perm[i] = the point at sorted position i), so every
+ * member list is in ascending point index; labels in [0, K).  The result is bit-reproducible.
+ * Errors before any launch: N < 0, K < 1, D out of range, K > 2^31 - 128 (the padded centroid index
+ * is an int), ldx < D, N ldx past int64, null or misaligned pointers, a workspace too small.
+ *
+ * gsb_quantize: codes[N, D] (uint8 for bits 8, uint16 for bits 16, contiguous) of
+ *   t = log_transform ? sign(v) log1p(|v|) : v,
+ *   q = clamp(floor((t - lo) (2^bits - 1) / (hi - lo) + 1/2), 0, 2^bits - 1)   (hi == lo: q = 0)
+ * per column, with range[2, D] = (lo row, hi row): fit_range != 0 sets lo / hi to the column's min /
+ * max of t (an order-free integer reduction: exact, reproducible; N = 0 gives 0, 0), otherwise the
+ * caller's range is read.  gsb_dequantize: out[N, D] = inverse transform of lo + q (hi - lo) /
+ * (2^bits - 1).  Errors before any launch: N < 0, D out of range, bits not 8 or 16, ldx < D, null or
+ * misaligned pointers.  Non-finite inputs give unspecified codes and ranges. */
+#define GSB_KMEANS_MAX_DIM 64
+size_t gsb_kmeans_assign_workspace_bytes(int K, int D);
+int gsb_kmeans_assign(int N, int K, int D, const float *x, int64_t ldx, const float *centroids, int32_t *labels,
+                      float *dist, void *ws, size_t ws_bytes, gsb_stream_t stream);
+int gsb_kmeans_update(int N, int K, int D, const float *x, int64_t ldx, const int32_t *labels, const int32_t *perm,
+                      const float *centroids, float *centroids_out, int32_t *counts, gsb_stream_t stream);
+int gsb_quantize(int N, int D, const float *x, int64_t ldx, int bits, int log_transform, int fit_range, float *range,
+                 void *codes, gsb_stream_t stream);
+int gsb_dequantize(int N, int D, const void *codes, int bits, const float *range, int log_transform, float *out,
+                   gsb_stream_t stream);
+
 /* ---- batched rendering (DESIGN 3.21): C cameras in one call.  The cameras share width, height,
  * the camera model and (in the callers) antialiasing; each has its own pose, intrinsics and lens
  * coefficients.  The entry points mirror the single-camera ones with C in front, so one frame
