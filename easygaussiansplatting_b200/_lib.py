@@ -140,6 +140,17 @@ SIGNATURES = {
     "gsb_splat_2dgs_forward": (_i, [_i, _i, _i] + [_vp] * 4 + [_f, _f, _i64, C.c_uint32, _vp, _sz, _vp, _sz]
                                + [_vp] * 14),
     "gsb_splat_2dgs_backward": (_i, [_i, _i, _i, _i64] + [_vp] * 10 + [_sz, _vp, _f, _f] + [_vp] * 6),
+    "gsb_2dgs_batch_workspace_bytes": (_sz, [_i, _i, _i, _i, _i64]),
+    "gsb_2dgs_batch_preprocess_forward": (_i, [_i] * 3 + [_vp] * 6 + [_i, _f, _f] + [_vp] * 7),
+    "gsb_2dgs_batch_preprocess_backward": (_i, [_i] * 3 + [_vp] * 6 + [_i, _f, _f] + [_vp] * 8),
+    "gsb_2dgs_batch_render": (_i, [_i] * 4 + [_i64, C.c_uint32] + [_vp] * 5 + [_sz] + [_vp] * 9),
+    "gsb_2dgs_batch_forward": (_i, [_i] * 4 + [_vp] * 4 + [_i64, C.c_uint32, _vp, _sz, _vp, _sz] + [_vp] * 10),
+    "gsb_2dgs_batch_backward": (_i, [_i] * 4 + [_i64] + [_vp] * 10 + [_sz] + [_vp] * 2),
+    "gsb_2dgs_batch_render_geometry": (_i, [_i] * 4 + [_i64, C.c_uint32] + [_vp] * 3 + [_f, _f] + [_vp] * 2 + [_sz]
+                                       + [_vp] * 13),
+    "gsb_2dgs_batch_forward_geometry": (_i, [_i] * 4 + [_vp] * 4 + [_f, _f, _i64, C.c_uint32, _vp, _sz, _vp, _sz]
+                                        + [_vp] * 14),
+    "gsb_2dgs_batch_backward_geometry": (_i, [_i] * 4 + [_i64] + [_vp] * 10 + [_sz, _vp, _f, _f] + [_vp] * 6),
     "gsb_tsdf_integrate": (_i, [_i, _i, _i] + [_f] * 6 + [_i, _i, _i] + [_vp] * 7),
     "gsb_tsdf_extract_workspace_bytes": (_sz, [_i, _i, _i]),
     "gsb_tsdf_extract_plan": (_i, [_i, _i, _i, _vp, _vp, _vp, _sz, C.POINTER(_i64), _vp]),

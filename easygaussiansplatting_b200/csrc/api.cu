@@ -41,7 +41,10 @@ static const char *const g_names[K_COUNT] = {"project", "computeCov3D", "compute
                                              "density_scan", "density_apply", "reset_alpha",
                                              "ply_rows_to_gs", "gs_to_params", "params_to_gs",
                                              "grad_reduce_broadcast", "sh_grad_expand", "filter3d",
-                                             "filter3d_apply", "filter3d_backward", "rects+scan_batch",
+                                             "filter3d_apply", "filter3d_backward", "surfel_forward_batch",
+                                             "draw_surfel_batch", "draw_surfel_backward_batch",
+                                             "surfel_backward_batch", "draw_2dgs_batch",
+                                             "draw_2dgs_backward_batch", "rects+scan_batch",
                                              "preprocess_forward_batch", "preprocess_backward_batch",
                                              "draw_batch", "draw_rgbd_batch", "draw_backward_batch",
                                              "draw_backward_rgbd_batch", "kmeans_assign", "kmeans_update",
@@ -1166,6 +1169,7 @@ struct SurfelDraw {
   const float *records;
   float *depth_image, *alpha_image, *normal_image;
   const GeoPlanes *geo = nullptr;
+  int frames = 0;  // > 0: the planes are [frames, ..., H, W] of a batch (launch_draw_surfel)
 
   int check() const {
     const char *who = geo ? "splat_2dgs" : "splat_surfel";
@@ -1177,7 +1181,7 @@ struct SurfelDraw {
   }
   int draw(int H, int W, int N, int64_t P, const FrameOut &o, const void *, int *work, cudaStream_t st) const {
     return launch_draw_surfel(H, W, o.ranges, P > 0 && N > 0 ? records : nullptr, o.gsid, o.image, o.contrib,
-                              o.final_tau, depth_image, alpha_image, normal_image, geo, work, st);
+                              o.final_tau, depth_image, alpha_image, normal_image, geo, work, st, frames);
   }
 };
 
@@ -1325,6 +1329,208 @@ int gsb_splat_2dgs_backward(int H, int W, int N, int64_t P, const float *records
   return launch_draw_surfel_backward(H, W, N, patch_range_per_tile, P > 0 ? records : nullptr, gsid_per_patch, contrib,
                                      final_tau, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, &g, rows,
                                      reinterpret_cast<int *>(b + SL.counters), (cudaStream_t)stream);
+}
+
+// ---- batched 2D Gaussian Splatting (surfel.cu, DESIGN 3.25): C pinhole cameras of one image size.
+// The per-surfel kernels read each surfel's rows once for all C cameras; the C frames are binned,
+// sorted and drawn as one tall frame through the frame core above (render_frame, capacity_wait,
+// SurfelDraw with a frame count).  Record c N + n is surfel n seen by camera c.
+
+// the batch call description of the per-surfel entry points: batch_scene's checks and table, pinhole
+// cameras only
+static int surfel_batch_scene(const char *who, int C, int N, int sh_dim3, const float *pws, const float *rots,
+                              const float *scales, const float *shs, const float *poses, const float *intrinsics,
+                              int camera_model, float width, float height, BatchCams &bc, BatchScene &b) {
+  if (camera_model != GSB_CAMERA_PINHOLE) return arg_error(who, "pinhole cameras only");
+  if (int rc = batch_scene(who, C, N, sh_dim3, pws, rots, scales, shs, poses, camera_model, intrinsics, width, height,
+                           bc, b))
+    return rc;
+  if (N > 0 && !(pws && rots && scales && shs && poses)) return arg_error(who, "null pointer");
+  return 0;
+}
+
+int gsb_2dgs_batch_preprocess_forward(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                      const float *scales, const float *shs, const float *poses,
+                                      const float *intrinsics, int camera_model, float width, float height,
+                                      const float *alphas, float *us, float *depths, int32_t *areas, float *colors,
+                                      float *records, gsb_stream_t stream) {
+  const char *who = "2dgs_batch_preprocess";
+  BatchCams bc;
+  BatchScene b{};
+  if (int rc = surfel_batch_scene(who, C, N, sh_dim3, pws, rots, scales, shs, poses, intrinsics, camera_model, width,
+                                  height, bc, b))
+    return rc;
+  if (!aligned(records, 16)) return arg_error(who, "records misaligned");
+  if (N > 0 && !(alphas && us && depths && areas && colors && records)) return arg_error(who, "null pointer");
+  return launch_surfel_fwd_batch(b, alphas, us, depths, areas, colors, records, (cudaStream_t)stream);
+}
+
+int gsb_2dgs_batch_preprocess_backward(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                       const float *scales, const float *shs, const float *poses,
+                                       const float *intrinsics, int camera_model, float width, float height,
+                                       const float *rows, float *dloss_dpws, float *dloss_dshs, float *dloss_dalphas,
+                                       float *dloss_dscales, float *dloss_drots, float *dloss_dus,
+                                       gsb_stream_t stream) {
+  const char *who = "2dgs_batch_preprocessB";
+  BatchCams bc;
+  BatchScene b{};
+  if (int rc = surfel_batch_scene(who, C, N, sh_dim3, pws, rots, scales, shs, poses, intrinsics, camera_model, width,
+                                  height, bc, b))
+    return rc;
+  if (N > 0 && !(rows && dloss_dpws && dloss_dshs && dloss_dalphas && dloss_dscales && dloss_drots && dloss_dus))
+    return arg_error(who, "null pointer");
+  return launch_surfel_bwd_batch(b, rows, dloss_dpws, dloss_dshs, dloss_dalphas, dloss_dscales, dloss_drots, dloss_dus,
+                                 (cudaStream_t)stream);
+}
+
+size_t gsb_2dgs_batch_workspace_bytes(int C, int N, int H, int W, int64_t P) {
+  return batch_records_ok(C, N) && C <= BATCH_MAX_CAMERAS ? sort_layout(C * N, batch_height(C, H), W, P).bytes : 0;
+}
+
+// The checks every batched surfel frame makes first: check_frame's (C < 1, C N >= 2^31, C gy tile
+// rows) and the camera count.  `who` prefixes the error texts.
+static int surfel_batch_frame(const char *who, int C, int H, int W, int N, const void *bin_ws, size_t bin_ws_bytes) {
+  if (C > BATCH_MAX_CAMERAS) return arg_error(who, "C > GSB_BATCH_MAX_CAMERAS");
+  return check_frame(who, batch_frames(C), H, W, N, bin_ws, bin_ws_bytes);
+}
+
+// gsb_2dgs_batch_render{,_geometry}: a tall frame binned by gsb_splat_bin_batch (geo: with the geometry planes)
+static int surfel_batch_render(const char *who, int C, int H, int W, int N, int64_t P, uint32_t depth_key_max,
+                               const float *us, const float *depths, const float *records, const void *bin_ws,
+                               void *ws, size_t ws_bytes, const FrameOut &o, float *depth_image, float *alpha_image,
+                               float *normal_image, const GeoPlanes *geo, gsb_stream_t stream) {
+  if (int rc = surfel_batch_frame(who, C, H, W, N, bin_ws, SIZE_MAX)) return rc;
+  if (P < 0) return arg_error(who, "bad P");
+  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
+  if (P > 0 && !(us && depths && records && bin_ws && ws && o.gsid)) return arg_error(who, "null pointer");
+  return render_frame(who, H, W, N, P, depth_key_max, us, nullptr, nullptr, const_cast<float *>(depths), nullptr,
+                      nullptr, false, const_cast<void *>(bin_ws), ws, ws_bytes, o,
+                      SurfelDraw{records, depth_image, alpha_image, normal_image, geo, C}, nullptr,
+                      (cudaStream_t)stream, C);
+}
+
+// gsb_2dgs_batch_forward{,_geometry}: the capacity path
+static int surfel_batch_forward(const char *who, int C, int H, int W, int N, const float *us, float *depths,
+                                int32_t *areas, const float *records, int64_t P_cap, uint32_t depth_key_cap,
+                                void *bin_ws, size_t bin_ws_bytes, void *ws, size_t ws_bytes, const FrameOut &o,
+                                uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                                const GeoPlanes *geo, gsb_stream_t stream) {
+  if (int rc = surfel_batch_frame(who, C, H, W, N, bin_ws, bin_ws_bytes)) return rc;
+  if (!(P_cap > 0 && P_cap < ((int64_t)1 << 30))) return arg_error(who, "bad P_cap (2^30 patches or more)");
+  if (!(o.gsid && status_host && bin_ws)) return arg_error(who, "null pointer");
+  if (N > 0 && !(us && depths && areas && records)) return arg_error(who, "null pointer");
+  return capacity_wait(who, P_cap, status_host, true, [&](const StatusRead *sr) {
+    return render_frame(who, H, W, N, P_cap, depth_key_cap, us, nullptr, nullptr, depths, nullptr, areas, false,
+                        bin_ws, ws, ws_bytes, o, SurfelDraw{records, depth_image, alpha_image, normal_image, geo, C},
+                        sr, (cudaStream_t)stream, C);
+  });
+}
+
+// gsb_2dgs_batch_backward{,_geometry}: rows [C N, 18] from the tall frame (geo: the geometry terms)
+static int surfel_batch_backward(const char *who, int C, int H, int W, int N, int64_t P, const float *records,
+                                 const int32_t *contrib, const float *final_tau, const int32_t *ranges,
+                                 const int32_t *gsid, const float *dl_image, const float *dl_depth,
+                                 const float *dl_alpha, const float *dl_normal, void *ws, size_t ws_bytes, float *rows,
+                                 const GeoGrads *geo, gsb_stream_t stream) {
+  if (int rc = surfel_batch_frame(who, C, H, W, N, nullptr, SIZE_MAX)) return rc;
+  if (P < 0) return arg_error(who, "bad P");
+  if (P >= ((int64_t)1 << 30)) return arg_error(who, "more than 2^30 patches");
+  if (N == 0) return 0;
+  if (rows == nullptr) return arg_error(who, "null output");
+  const Tall t = tall_frame(C, H, N);
+  const SortLayout SL = sort_layout(t.N, t.H, W, 0);
+  if (!(ws != nullptr && aligned(ws, 16) && ws_bytes >= SL.bytes)) return arg_error(who, "workspace too small");
+  const bool with_geo = geo != nullptr && (geo->distortion != nullptr || geo->median != nullptr);
+  if (P > 0) {
+    if (!(records && contrib && final_tau && ranges && gsid)) return arg_error(who, "null pointer");
+    if (!(aligned(records, 16) && aligned(ranges, 8))) return arg_error(who, "misaligned input");
+    if (with_geo && !(geo->alpha && geo->moments && geo->median_contrib)) return arg_error(who, "null geometry plane");
+    // the kernel reads these planes one 4-byte element at a time
+    if (with_geo && !(aligned(geo->alpha, 4) && aligned(geo->moments, 4) && aligned(geo->median_contrib, 4) &&
+                      aligned(geo->distortion, 4) && aligned(geo->median, 4)))
+      return arg_error(who, "misaligned geometry plane");
+  }
+  char *b = static_cast<char *>(ws);
+  return launch_draw_surfel_backward(H, W, t.N, ranges, P > 0 ? records : nullptr, gsid, contrib, final_tau, dl_image,
+                                     dl_depth, dl_alpha, dl_normal, geo, rows,
+                                     reinterpret_cast<int *>(b + SL.counters), (cudaStream_t)stream, C);
+}
+
+int gsb_2dgs_batch_render(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                          const float *depths, const float *records, const void *bin_ws, void *ws, size_t ws_bytes,
+                          float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                          int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
+                          gsb_stream_t stream) {
+  return surfel_batch_render("2dgs_batch", C, H, W, N, P, depth_key_max, us, depths, records, bin_ws, ws, ws_bytes,
+                             {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch}, depth_image,
+                             alpha_image, normal_image, nullptr, stream);
+}
+
+int gsb_2dgs_batch_forward(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                           const float *records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                           size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                           float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                           uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                           gsb_stream_t stream) {
+  return surfel_batch_forward("2dgs_batch", C, H, W, N, us, depths, areas, records, P_cap, depth_key_cap, bin_ws,
+                              bin_ws_bytes, ws, ws_bytes, {image, contrib, final_tau, patch_range_per_tile,
+                                                           gsid_per_patch},
+                              status_host, depth_image, alpha_image, normal_image, nullptr, stream);
+}
+
+int gsb_2dgs_batch_backward(int C, int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                            const float *final_tau, const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                            const float *dloss_dimage, const float *dloss_ddepth, const float *dloss_dalpha,
+                            const float *dloss_dnormal, void *ws, size_t ws_bytes, float *rows, gsb_stream_t stream) {
+  return surfel_batch_backward("2dgs_batchB", C, H, W, N, P, records, contrib, final_tau, patch_range_per_tile,
+                               gsid_per_patch, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, ws, ws_bytes,
+                               rows, nullptr, stream);
+}
+
+int gsb_2dgs_batch_render_geometry(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                                   const float *depths, const float *records, float near, float far,
+                                   const void *bin_ws, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                                   float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                                   float *depth_image, float *alpha_image, float *normal_image, float *distortion,
+                                   float *moments, float *median_depth, int32_t *median_contrib,
+                                   gsb_stream_t stream) {
+  GeoPlanes g;
+  if (int rc = geo_planes("2dgs_batch", near, far, distortion, moments, median_depth, median_contrib, g)) return rc;
+  return surfel_batch_render("2dgs_batch", C, H, W, N, P, depth_key_max, us, depths, records, bin_ws, ws, ws_bytes,
+                             {image, contrib, final_tau, patch_range_per_tile, gsid_per_patch}, depth_image,
+                             alpha_image, normal_image, &g, stream);
+}
+
+int gsb_2dgs_batch_forward_geometry(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                                    const float *records, float near, float far, int64_t P_cap,
+                                    uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
+                                    size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                                    int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
+                                    float *depth_image, float *alpha_image, float *normal_image, float *distortion,
+                                    float *moments, float *median_depth, int32_t *median_contrib,
+                                    gsb_stream_t stream) {
+  GeoPlanes g;
+  if (int rc = geo_planes("2dgs_batch", near, far, distortion, moments, median_depth, median_contrib, g)) return rc;
+  return surfel_batch_forward("2dgs_batch", C, H, W, N, us, depths, areas, records, P_cap, depth_key_cap, bin_ws,
+                              bin_ws_bytes, ws, ws_bytes, {image, contrib, final_tau, patch_range_per_tile,
+                                                           gsid_per_patch},
+                              status_host, depth_image, alpha_image, normal_image, &g, stream);
+}
+
+int gsb_2dgs_batch_backward_geometry(int C, int H, int W, int N, int64_t P, const float *records,
+                                     const int32_t *contrib, const float *final_tau,
+                                     const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                                     const float *dloss_dimage, const float *dloss_ddepth, const float *dloss_dalpha,
+                                     const float *dloss_dnormal, void *ws, size_t ws_bytes, float *rows, float near,
+                                     float far, const float *alpha_image, const float *moments,
+                                     const int32_t *median_contrib, const float *dloss_ddistortion,
+                                     const float *dloss_dmedian, gsb_stream_t stream) {
+  if (int rc = check_near_far("2dgs_batchB", near, far)) return rc;
+  const GeoGrads g{dloss_ddistortion, dloss_dmedian, alpha_image, moments, median_contrib, near,
+                   (float)((double)far / ((double)far - near))};
+  return surfel_batch_backward("2dgs_batchB", C, H, W, N, P, records, contrib, final_tau, patch_range_per_tile,
+                               gsid_per_patch, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, ws, ws_bytes,
+                               rows, &g, stream);
 }
 
 // ---- feature rendering (raster_feat.cu)

@@ -18,7 +18,8 @@ enum KernelId {
   K_PACK, K_DRAW, K_DRAW_BWD, K_PRE_FWD, K_PRE_BWD, K_FINALIZE, K_LOSS_FWD, K_LOSS_BWD, K_BMM,
   K_DENSITY_ACC, K_DENSITY_CLASSIFY, K_DENSITY_SCAN, K_DENSITY_APPLY, K_RESET_ALPHA, K_GS_DECODE,
   K_GS_TO_PARAMS, K_PARAMS_TO_GS, K_GRAD_EXCHANGE, K_SH_EXPAND, K_FILTER3D, K_FILTER3D_APPLY, K_FILTER3D_BWD,
-  K_RECTS_BATCH, K_PRE_FWD_BATCH, K_PRE_BWD_BATCH, K_DRAW_BATCH, K_DRAW_RGBD_BATCH, K_DRAW_BWD_BATCH,
+  K_SURFEL_FWD_BATCH, K_DRAW_SURFEL_BATCH, K_DRAW_SURFEL_BWD_BATCH, K_SURFEL_BWD_BATCH, K_DRAW_2DGS_BATCH,
+  K_DRAW_2DGS_BWD_BATCH, K_RECTS_BATCH, K_PRE_FWD_BATCH, K_PRE_BWD_BATCH, K_DRAW_BATCH, K_DRAW_RGBD_BATCH, K_DRAW_BWD_BATCH,
   K_DRAW_BWD_RGBD_BATCH, K_KMEANS_ASSIGN, K_KMEANS_UPDATE, K_QUANTIZE, K_DEQUANTIZE, K_DENSITY_ROWS, K_BILAGRID_SLICE, K_BILAGRID_SLICE_BWD, K_BILAGRID_TV, K_DRAW_FEAT, K_DRAW_FEAT_BWD, K_DRAW_STATS, K_DRAW_SURFEL_STATS, K_MCMC_SCAN, K_MCMC_SAMPLE, K_MCMC_RELOCATE, K_MCMC_GROW,
   K_MCMC_ROWS, K_MCMC_NOISE, K_TSDF_INTEGRATE, K_TSDF_PLAN, K_TSDF_EMIT,
   K_SURFEL_FWD, K_DRAW_SURFEL, K_DRAW_SURFEL_BWD, K_SURFEL_BWD, K_DRAW_2DGS, K_DRAW_2DGS_BWD,
@@ -366,6 +367,12 @@ int launch_surfel_fwd(const FusedScene &sc, const float *alphas, float *us, floa
                       float *recs, cudaStream_t st);
 int launch_surfel_bwd(const FusedScene &sc, const float *rows, float *g_pws, float *g_shs, float *g_alphas,
                       float *g_scales, float *g_rots, float *g_us, cudaStream_t st);
+// their batch forms (DESIGN 3.25): C pinhole cameras (b.model unused), us / depths / areas / colors
+// [C, N, ...] and recs [C N, 20]; rows [C N, 18] -> the summed per-surfel gradients and g_us [C, N, 2]
+int launch_surfel_fwd_batch(const BatchScene &b, const float *alphas, float *us, float *depths, int32_t *areas,
+                            float *colors, float *recs, cudaStream_t st);
+int launch_surfel_bwd_batch(const BatchScene &b, const float *rows, float *g_pws, float *g_shs, float *g_alphas,
+                            float *g_scales, float *g_rots, float *g_us, cudaStream_t st);
 // The 2DGS geometry planes (DESIGN 3.16) of one frame, on the NDC-mapped hit depth
 // m(z) = mscale (1 - near / max(z, near)), mscale = far / (far - near):
 // distortion[H,W] = sum_{j<i} w_i w_j (m_i - m_j)^2, moments[2,H,W] = (sum w m, sum w m^2),
@@ -385,16 +392,19 @@ struct GeoGrads {
 };
 // work: launch_tile_list's work area; recs == nullptr: no patches (zeros only).  The normal plane
 // [3,H,W] is written like the image planes.  geo: also the geometry planes (k_draw_2dgs), or NULL
-// (k_draw_surfel).
+// (k_draw_surfel).  frames > 0: the tall frame of a batch of `frames` H x W frames (DESIGN 3.25):
+// ranges of its frames gx gy tiles, every plane [frames, ..., H, W] (k_draw_disk_batch, k_draw_2dgs_batch).
 int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid, float *image,
                        int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, float *normal_image,
-                       const GeoPlanes *geo, int *work, cudaStream_t st);
+                       const GeoPlanes *geo, int *work, cudaStream_t st, int frames = 0);
 // the upstream planes dl_*: NULL reads as zero (all NULL: the rows stay 0).  geo with an upstream
 // geometry plane: k_draw_2dgs_bwd adds the geometry terms; otherwise k_draw_surfel_bwd runs.
+// frames > 0: as for launch_draw_surfel, N = all records of the batch (k_draw_disk_bwd_batch,
+// k_draw_2dgs_bwd_batch).
 int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, const float *recs, const int32_t *gsid,
                                 const int32_t *contrib, const float *final_tau, const float *dl_image,
                                 const float *dl_depth, const float *dl_alpha, const float *dl_normal,
-                                const GeoGrads *geo, float *rows, int *work, cudaStream_t st);
+                                const GeoGrads *geo, float *rows, int *work, cudaStream_t st, int frames = 0);
 
 // ---- mesh extraction (tsdf.cu, DESIGN 3.17; the fp64 model is oracle/tsdf_oracle.py).  The grid:
 // nx x ny x nz points, point (i, j, k) at origin + voxel (i, j, k), arrays [nz, ny, nx] (x fastest),

@@ -16,6 +16,9 @@
 //                      the alpha' recurrence and to the hit-depth gradient; the rows are the same
 //  k_surfel_bwd<K3>    the rows -> dL/dpws, dL/dshs, dL/dalphas, dL/dscales, dL/drots, dL/dus (= ddelta)
 //  k_draw_stats_2dgs   per-surfel sums, maxima and counts of a drawn frame's weights (DESIGN 3.18)
+//  k_disk_fwd_batch<K3>, k_disk_bwd_batch<K3>, k_draw_disk_batch, k_draw_2dgs_batch, k_draw_disk_bwd_batch,
+//  k_draw_2dgs_bwd_batch: the batch forms of k_surfel_fwd, k_surfel_bwd and the four rasterizers for C
+//                      cameras drawn as one tall frame (DESIGN 3.25)
 #include "common.cuh"
 #include "kernels.h"
 #include "raster_walk.cuh"
@@ -137,6 +140,115 @@ __global__ void __launch_bounds__(PG) k_surfel_bwd(int N, const float *__restric
   st_pair(g_us, o, row[16], row[17]);
 }
 
+// ---- batched per-surfel kernels (DESIGN 3.25): C pinhole cameras in one launch, as
+// k_preprocess_fwd_batch / k_preprocess_bwd_batch (fused.cu).  A thread loads its surfel's rows once
+// (pw, q, s, alpha to registers, the SH row through the shared tile) and runs sf::forward_one /
+// sf::backward_one once per camera: camera c's pose from poses[c] (Rcw 9, tcw 3, twc 3 floats), its
+// intrinsics from the kernel parameters.  Camera c's outputs go to rows c N + n of [C, N, ...].
+__device__ __forceinline__ pg::Cam disk_batch_cam(const float *__restrict__ poses, const BatchCams &bc, int c) {
+  const float *p = poses + 15 * c;
+  const float4 f = bc.f[c];
+  return surfel_cam(p, p + 9, p + 12, f.x, f.y, f.z, f.w);
+}
+
+// the forward: k_surfel_fwd's outputs per camera; record c N + n of recs [C N, 20]
+template <int K3>
+__global__ void __launch_bounds__(PG) k_disk_fwd_batch(int C, int N, const float *__restrict__ pws,
+                                                       const float *__restrict__ rots, const float *__restrict__ scales,
+                                                       const float *__restrict__ shs, const float *__restrict__ poses,
+                                                       const __grid_constant__ BatchCams bc,
+                                                       const float *__restrict__ alphas, float *__restrict__ us,
+                                                       float *__restrict__ depths, int32_t *__restrict__ areas,
+                                                       float *__restrict__ colors, float4 *__restrict__ recs) {
+  constexpr int KS = 3 * K3;
+  __shared__ float sm[TileT<KS>::FLOATS];
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * PG;
+  const int nv = min(PG, (int)(N - base));
+  const bool valid = tid < nv;
+  float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f}, al = 0.f;
+  if (valid) {
+    surfel_rows(pws, scales, rots, base + tid, pw, s, q);
+    al = __ldg(alphas + base + tid);
+  }
+  tile_fetch<KS>(shs, base, nv, sm, tid);
+  __syncthreads();
+  if (!valid) return;
+  const long long i = base + tid;
+  for (int c = 0; c < C; c++) {
+    const pg::Cam cam = disk_batch_cam(poses, bc, c);
+    float u[2], depth, col[3], rec[sf::kRecFloats];
+    int area[2];
+    sf::forward_one<K3>(pw, q, s, ROWK(KS), al, cam, u, &depth, area, col, rec);
+    const long long o = (long long)c * N + i;
+    st_pair(us, o, u[0], u[1]);
+    depths[o] = depth;
+    st_pair(areas, o, area[0], area[1]);
+    colors[3 * o] = col[0]; colors[3 * o + 1] = col[1]; colors[3 * o + 2] = col[2];
+#pragma unroll
+    for (int k = 0; k < 5; k++) recs[5 * o + k] = make_float4(rec[4 * k], rec[4 * k + 1], rec[4 * k + 2], rec[4 * k + 3]);
+  }
+}
+
+// the backward from the rows [C N, 18]: the C contributions to each per-surfel gradient summed in
+// fp32 registers in camera order.  dL/dsh goes to registers, not over the SH tile as in
+// k_surfel_bwd: the next camera still reads the SH row.  One gradient row per surfel (dL/dalpha the
+// sum of the rows' dalpha), dL/dus per camera [C, N, 2].
+template <int K3>
+__global__ void __launch_bounds__(PG) k_disk_bwd_batch(int C, int N, const float *__restrict__ pws,
+                                                       const float *__restrict__ rots, const float *__restrict__ scales,
+                                                       const float *__restrict__ shs, const float *__restrict__ poses,
+                                                       const __grid_constant__ BatchCams bc,
+                                                       const float *__restrict__ rows, float *__restrict__ g_pws,
+                                                       float *__restrict__ g_shs, float *__restrict__ g_alphas,
+                                                       float *__restrict__ g_scales, float *__restrict__ g_rots,
+                                                       float *__restrict__ g_us) {
+  constexpr int KS = 3 * K3;
+  __shared__ float sm[TileT<KS>::FLOATS];
+  const int tid = threadIdx.x;
+  const long long base = (long long)blockIdx.x * PG;
+  const int nv = min(PG, (int)(N - base));
+  const bool valid = tid < nv;
+  float pw[3] = {0.f, 0.f, 1.f}, q[4] = {1.f, 0.f, 0.f, 0.f}, s[3] = {1.f, 1.f, 1.f};
+  if (valid) surfel_rows(pws, scales, rots, base + tid, pw, s, q);
+  tile_fetch<KS>(shs, base, nv, sm, tid);
+  __syncthreads();
+  float gpw[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, gsh[KS], gal = 0.f;
+#pragma unroll
+  for (int e = 0; e < KS; e++) gsh[e] = 0.f;
+  const long long i = base + tid;
+  if (valid) {
+    for (int c = 0; c < C; c++) {
+      const long long o = (long long)c * N + i;
+      float row[sf::kRowFloats];
+#pragma unroll
+      for (int k = 0; k < sf::kRowFloats; k++) row[k] = __ldg(rows + sf::kRowFloats * o + k);
+      const pg::Cam cam = disk_batch_cam(poses, bc, c);
+      float xpw[3], xq[4], xs[3], xsh[KS];
+      sf::backward_one<K3>(pw, q, s, ROWK(KS), cam, row, xpw, xq, xs, xsh);
+#pragma unroll
+      for (int e = 0; e < 3; e++) { gpw[e] += xpw[e]; gs[e] += xs[e]; }
+#pragma unroll
+      for (int e = 0; e < 4; e++) gq[e] += xq[e];
+#pragma unroll
+      for (int e = 0; e < KS; e++) gsh[e] += xsh[e];
+      gal += row[9];
+      st_pair(g_us, o, row[16], row[17]);
+    }
+    // dL/dsh replaces the thread's own SH row (no other thread reads it before the barrier)
+    float *row = ROWK(KS);
+#pragma unroll
+    for (int e = 0; e < KS; e++) row[e] = gsh[e];
+  }
+  __syncthreads();
+  tile_flush<KS>(g_shs, base, nv, sm, tid);
+  if (!valid) return;
+  g_pws[3 * i] = gpw[0]; g_pws[3 * i + 1] = gpw[1]; g_pws[3 * i + 2] = gpw[2];
+  g_scales[3 * i] = gs[0]; g_scales[3 * i + 1] = gs[1]; g_scales[3 * i + 2] = 0.f;
+  g_rots[4 * i] = gq[0]; g_rots[4 * i + 1] = gq[1]; g_rots[4 * i + 2] = gq[2]; g_rots[4 * i + 3] = gq[3];
+  g_alphas[i] = gal;
+}
+
 // ---- the rasterizers' 80-byte record walk: raster_walk.cuh's protocol and chunk helpers at
 // SREC_BYTES, with the surfel record's own cull
 
@@ -185,14 +297,24 @@ __device__ __forceinline__ int surfel_compact(uint32_t my_rec, int my_idx, int l
   return __popc(mask);
 }
 
-// one 8x8 block of a work-list entry: pixel coordinates of the lane's pair
+// one 8x8 block of a work-list entry: pixel coordinates of the lane's pair.  BATCH: the tall frame
+// of a batch (DESIGN 3.25, as draw_body's in raster_fwd.cu): tile row r is row r - f gy of frame
+// f = r / gy, the pixels are that frame's own coordinates, fo = f H W is the frame's offset in every
+// [H,W] plane and pix includes it; a block in a pad row lies below the frame and is skipped.
 struct BlockPix {
   int rx0, ry0, px, py;
   bool in0, in1;
-  size_t pix;
+  size_t pix, fo;
 };
-__device__ __forceinline__ bool block_pix(int W, int H, int gx, int tile, int blk, int lane, BlockPix &b) {
-  const int tx = tile % gx, ty = tile / gx;
+template <bool BATCH>
+__device__ __forceinline__ bool block_pix(int W, int H, int gx, int gy, int tile, int blk, int lane, BlockPix &b) {
+  int tx = tile % gx, ty = tile / gx;
+  b.fo = 0;
+  if constexpr (BATCH) {
+    const int f = ty / gy;
+    ty -= f * gy;
+    b.fo = (size_t)f * H * W;
+  }
   b.rx0 = tx * TILE + (blk & 1) * 8;
   b.ry0 = ty * TILE + (blk >> 1) * 8;
   if (b.rx0 >= W || b.ry0 >= H) return false;
@@ -200,7 +322,7 @@ __device__ __forceinline__ bool block_pix(int W, int H, int gx, int tile, int bl
   b.py = b.ry0 + (lane >> 2);
   b.in0 = b.px < W && b.py < H;
   b.in1 = b.px + 1 < W && b.py < H;
-  b.pix = (size_t)b.py * W + b.px;
+  b.pix = b.fo + (size_t)b.py * W + b.px;
   return true;
 }
 
@@ -213,9 +335,11 @@ __device__ __forceinline__ float geo_dm(float z, float near, float mscale) {
 }
 
 // The forward walk of k_draw_surfel and (GEO) k_draw_2dgs: GEO also accumulates the moments
-// D = sum w m, D2 = sum w m^2, the distortion sum_{j<i} w_i w_j (m_i - m_j)^2 and the median
-template <bool GEO>
-__device__ __forceinline__ void draw_walk(int W, int H, int gx, const int2 *__restrict__ ranges,
+// D = sum w m, D2 = sum w m^2, the distortion sum_{j<i} w_i w_j (m_i - m_j)^2 and the median.
+// BATCH: the tall frame of a batch of frames (k_draw_disk_batch, k_draw_2dgs_batch; block_pix): every
+// plane is frame f's of [C, ..., H, W]
+template <bool GEO, bool BATCH>
+__device__ __forceinline__ void draw_walk(int W, int H, int gx, int gy, const int2 *__restrict__ ranges,
                                           const float4 *__restrict__ recs, const int32_t *__restrict__ gsid,
                                           float *__restrict__ image, int32_t *__restrict__ contrib,
                                           float *__restrict__ final_tau, float *__restrict__ depth_image,
@@ -239,7 +363,7 @@ __device__ __forceinline__ void draw_walk(int W, int H, int gx, const int2 *__re
     const int32_t *ids = gsid + range.x;
     for (int blk = code == 4 ? 0 : code; blk < (code == 4 ? 4 : code + 1); blk++) {
       BlockPix bp;
-      if (!block_pix(W, H, gx, tile, blk, lane, bp)) continue;
+      if (!block_pix<BATCH>(W, H, gx, gy, tile, blk, lane, bp)) continue;
       const float xs[2] = {(float)bp.px, (float)(bp.px + 1)}, y = (float)bp.py;
       float tau[2] = {bp.in0 ? 1.0f : 0.0f, bp.in1 ? 1.0f : 0.0f};
       float acc[2][8];  // r, g, b, depth, alpha, nx, ny, nz
@@ -308,17 +432,21 @@ __device__ __forceinline__ void draw_walk(int W, int H, int gx, const int2 *__re
         }
         walk_drain();
       }
+      // the frame's [3,H,W] planes start at 3 fo and its moments [2,H,W] at 2 fo (pix holds fo)
+      float *const image_f = BATCH ? image + 2 * bp.fo : image;
+      float *const normal_f = BATCH ? normal_image + 2 * bp.fo : normal_image;
+      float *const moments_f = BATCH ? geo.moments + bp.fo : geo.moments;
 #pragma unroll
       for (int p = 0; p < 2; p++) {
         if (!(p ? bp.in1 : bp.in0)) continue;
         const size_t q = bp.pix + p;
-        image[q] = acc[p][0]; image[HW + q] = acc[p][1]; image[2 * HW + q] = acc[p][2];
+        image_f[q] = acc[p][0]; image_f[HW + q] = acc[p][1]; image_f[2 * HW + q] = acc[p][2];
         contrib[q] = cont[p]; final_tau[q] = tau[p];
         depth_image[q] = acc[p][3]; alpha_image[q] = acc[p][4];
-        normal_image[q] = acc[p][5]; normal_image[HW + q] = acc[p][6]; normal_image[2 * HW + q] = acc[p][7];
+        normal_f[q] = acc[p][5]; normal_f[HW + q] = acc[p][6]; normal_f[2 * HW + q] = acc[p][7];
         if constexpr (GEO) {
           geo.distortion[q] = dist[p];
-          geo.moments[q] = mD[p]; geo.moments[HW + q] = mD2[p];
+          moments_f[q] = mD[p]; moments_f[HW + q] = mD2[p];
           geo.median_depth[q] = medz[p]; geo.median_contrib[q] = medc[p];
         }
       }
@@ -331,8 +459,8 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_surfel(
     const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
     float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
     float *__restrict__ normal_image, int *__restrict__ work) {
-  draw_walk<false>(W, H, gx, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image, normal_image,
-                   GeoPlanes{}, work);
+  draw_walk<false, false>(W, H, gx, 0, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                          normal_image, GeoPlanes{}, work);
 }
 
 // 2DGS (DESIGN 3.16): k_draw_surfel's planes, bit for bit, and the geometry planes
@@ -341,8 +469,31 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_2dgs(
     const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
     float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
     float *__restrict__ normal_image, GeoPlanes geo, int *__restrict__ work) {
-  draw_walk<true>(W, H, gx, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image, normal_image, geo,
-                  work);
+  draw_walk<true, false>(W, H, gx, 0, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                         normal_image, geo, work);
+}
+
+// ---- the batched rasterizers (DESIGN 3.25): the C frames of a batch binned as one tall frame of
+// C gy tile rows, drawn from the records [C N, 20] (record c N + n: surfel n seen by camera c) into
+// image / normal [C,3,H,W], contrib / final_tau / depth / alpha [C,H,W] and the geometry planes
+// [C,...,H,W].  Frame c is the single frame of camera c, bit for bit.  (The kernels carry no
+// "surfel" in their names: that name stays with the single-camera kernels.)
+__global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_disk_batch(
+    int W, int H, int gx, int gy, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
+    float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
+    float *__restrict__ normal_image, int *__restrict__ work) {
+  draw_walk<false, true>(W, H, gx, gy, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                         normal_image, GeoPlanes{}, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_SURFEL_MINBLOCKS) k_draw_2dgs_batch(
+    int W, int H, int gx, int gy, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, float *__restrict__ image, int32_t *__restrict__ contrib,
+    float *__restrict__ final_tau, float *__restrict__ depth_image, float *__restrict__ alpha_image,
+    float *__restrict__ normal_image, GeoPlanes geo, int *__restrict__ work) {
+  draw_walk<true, true>(W, H, gx, gy, ranges, recs, gsid, image, contrib, final_tau, depth_image, alpha_image,
+                        normal_image, geo, work);
 }
 
 // the upstream gradient planes of the backward; NULL reads as zero
@@ -354,9 +505,10 @@ __device__ __forceinline__ float ld_plane(const float *__restrict__ p, size_t q)
 
 // The backward walk of k_draw_surfel_bwd and (GEO) k_draw_2dgs_bwd: GEO adds dL/ddistortion's
 // dDelta/dw_i to the per-record value of the alpha' recurrence and its dDelta/dz_i, with dL/dmedian
-// at the median record, to the hit-depth coefficient
-template <bool GEO>
-__device__ __forceinline__ void draw_bwd_walk(int W, int H, int gx, const int2 *__restrict__ ranges,
+// at the median record, to the hit-depth coefficient.  BATCH: as draw_walk's; the upstream planes
+// and the forward's alpha, moments and median_contrib are frame f's of [C, ..., H, W] as well
+template <bool GEO, bool BATCH>
+__device__ __forceinline__ void draw_bwd_walk(int W, int H, int gx, int gy, const int2 *__restrict__ ranges,
                                               const float4 *__restrict__ recs, const int32_t *__restrict__ gsid,
                                               const int32_t *__restrict__ contrib,
                                               const float *__restrict__ final_tau, const SurfelGrads &dl,
@@ -379,25 +531,31 @@ __device__ __forceinline__ void draw_bwd_walk(int W, int H, int gx, const int2 *
     const int32_t *ids = gsid + range.x;
     for (int blk = code == 4 ? 0 : code; blk < (code == 4 ? 4 : code + 1); blk++) {
       BlockPix bp;
-      if (!block_pix(W, H, gx, tile, blk, lane, bp)) continue;
+      if (!block_pix<BATCH>(W, H, gx, gy, tile, blk, lane, bp)) continue;
       const float xs[2] = {(float)bp.px, (float)(bp.px + 1)}, y = (float)bp.py;
       int cont[2] = {0, 0};
       float tau[2] = {0.f, 0.f}, sdot[2] = {0.f, 0.f};
       float d[2][8];  // dL/d(r, g, b, depth, alpha, nx, ny, nz) of the pixel
+      // the frame's [3,H,W] upstream planes start at 3 fo (pix holds fo)
+      const float *img = dl.img, *nrm = dl.normal;
+      if constexpr (BATCH) {
+        if (img) img += 2 * bp.fo;
+        if (nrm) nrm += 2 * bp.fo;
+      }
 #pragma unroll
       for (int p = 0; p < 2; p++) {
         const bool in = p ? bp.in1 : bp.in0;
         const size_t q = bp.pix + p;
         cont[p] = in ? min(__ldg(contrib + q), len) : 0;
         tau[p] = in ? __ldg(final_tau + q) : 0.f;
-        d[p][0] = in ? ld_plane(dl.img, q) : 0.f;
-        d[p][1] = in ? ld_plane(dl.img ? dl.img + HW : nullptr, q) : 0.f;
-        d[p][2] = in ? ld_plane(dl.img ? dl.img + 2 * HW : nullptr, q) : 0.f;
+        d[p][0] = in ? ld_plane(img, q) : 0.f;
+        d[p][1] = in ? ld_plane(img ? img + HW : nullptr, q) : 0.f;
+        d[p][2] = in ? ld_plane(img ? img + 2 * HW : nullptr, q) : 0.f;
         d[p][3] = in ? ld_plane(dl.depth, q) : 0.f;
         d[p][4] = in ? ld_plane(dl.alpha, q) : 0.f;
-        d[p][5] = in ? ld_plane(dl.normal, q) : 0.f;
-        d[p][6] = in ? ld_plane(dl.normal ? dl.normal + HW : nullptr, q) : 0.f;
-        d[p][7] = in ? ld_plane(dl.normal ? dl.normal + 2 * HW : nullptr, q) : 0.f;
+        d[p][5] = in ? ld_plane(nrm, q) : 0.f;
+        d[p][6] = in ? ld_plane(nrm ? nrm + HW : nullptr, q) : 0.f;
+        d[p][7] = in ? ld_plane(nrm ? nrm + 2 * HW : nullptr, q) : 0.f;
       }
       // GEO: dL/ddistortion, dL/dmedian, the final A, D, D2 and the median record of each pixel
       float gdist[2] = {0.f, 0.f}, gmed[2] = {0.f, 0.f}, fA[2] = {0.f, 0.f}, fD[2] = {0.f, 0.f},
@@ -410,9 +568,10 @@ __device__ __forceinline__ void draw_bwd_walk(int W, int H, int gx, const int2 *
           const size_t q = bp.pix + p;
           gdist[p] = ld_plane(geo.distortion, q);
           gmed[p] = ld_plane(geo.median, q);
+          const float *moments_f = BATCH ? geo.moments + bp.fo : geo.moments;  // [2,H,W] at 2 fo
           fA[p] = __ldg(geo.alpha + q);
-          fD[p] = __ldg(geo.moments + q);
-          fD2[p] = __ldg(geo.moments + HW + q);
+          fD[p] = __ldg(moments_f + q);
+          fD2[p] = __ldg(moments_f + HW + q);
           medc[p] = __ldg(geo.median_contrib + q);
         }
       }
@@ -516,7 +675,7 @@ __global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_surfel_
     int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     SurfelGrads dl, float *__restrict__ rows, int *__restrict__ work) {
-  draw_bwd_walk<false>(W, H, gx, ranges, recs, gsid, contrib, final_tau, dl, GeoGrads{}, rows, work);
+  draw_bwd_walk<false, false>(W, H, gx, 0, ranges, recs, gsid, contrib, final_tau, dl, GeoGrads{}, rows, work);
 }
 
 // the upstream planes of k_draw_2dgs_bwd: k_draw_surfel_bwd's and the geometry terms' (one struct,
@@ -530,7 +689,22 @@ __global__ void __launch_bounds__(128, DRAW_2DGS_BWD_MINBLOCKS) k_draw_2dgs_bwd(
     int W, int H, int gx, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
     const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
     GeoBwdArgs a, float *__restrict__ rows, int *__restrict__ work) {
-  draw_bwd_walk<true>(W, H, gx, ranges, recs, gsid, contrib, final_tau, a.dl, a.geo, rows, work);
+  draw_bwd_walk<true, false>(W, H, gx, 0, ranges, recs, gsid, contrib, final_tau, a.dl, a.geo, rows, work);
+}
+
+// the batched backward rasterizers (DESIGN 3.25): rows [C N, 18], one per record of the tall frame
+__global__ void __launch_bounds__(128, DRAW_SURFEL_BWD_MINBLOCKS) k_draw_disk_bwd_batch(
+    int W, int H, int gx, int gy, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    SurfelGrads dl, float *__restrict__ rows, int *__restrict__ work) {
+  draw_bwd_walk<false, true>(W, H, gx, gy, ranges, recs, gsid, contrib, final_tau, dl, GeoGrads{}, rows, work);
+}
+
+__global__ void __launch_bounds__(128, DRAW_2DGS_BWD_MINBLOCKS) k_draw_2dgs_bwd_batch(
+    int W, int H, int gx, int gy, const int2 *__restrict__ ranges, const float4 *__restrict__ recs,
+    const int32_t *__restrict__ gsid, const int32_t *__restrict__ contrib, const float *__restrict__ final_tau,
+    GeoBwdArgs a, float *__restrict__ rows, int *__restrict__ work) {
+  draw_bwd_walk<true, true>(W, H, gx, gy, ranges, recs, gsid, contrib, final_tau, a.dl, a.geo, rows, work);
 }
 
 // Contribution statistics of a drawn surfel frame (DESIGN 3.18): k_draw_stats' three reductions
@@ -555,7 +729,7 @@ __global__ void __launch_bounds__(128, DRAW_STATS_2DGS_MINBLOCKS) k_draw_stats_2
   const int len = range.y - range.x;
   const int32_t *ids = gsid + range.x;
   BlockPix bp;
-  if (len <= 0 || !block_pix(W, H, gx, tile, warp, lane, bp)) return;
+  if (len <= 0 || !block_pix<false>(W, H, gx, 0, tile, warp, lane, bp)) return;
   const float xs[2] = {(float)bp.px, (float)(bp.px + 1)}, y = (float)bp.py;
   const int cont[2] = {bp.in0 ? min(__ldg(contrib + bp.pix), len) : 0,
                        bp.in1 ? min(__ldg(contrib + bp.pix + 1), len) : 0};
@@ -650,14 +824,39 @@ int launch_surfel_bwd(const FusedScene &sc, const float *rows, float *g_pws, flo
   return 0;
 }
 
+int launch_surfel_fwd_batch(const BatchScene &b, const float *alphas, float *us, float *depths, int32_t *areas,
+                            float *colors, float *recs, cudaStream_t st) {
+  if (b.N <= 0) return 0;
+  const int nb = (b.N + PG - 1) / PG;
+  ProfScope ps(K_SURFEL_FWD_BATCH, st);
+  GSB_SURFEL_K3(b.k3, (k_disk_fwd_batch<K3><<<nb, PG, 0, st>>>(b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses,
+                                                               *b.cams, alphas, us, depths, areas, colors,
+                                                               reinterpret_cast<float4 *>(recs))));
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int launch_surfel_bwd_batch(const BatchScene &b, const float *rows, float *g_pws, float *g_shs, float *g_alphas,
+                            float *g_scales, float *g_rots, float *g_us, cudaStream_t st) {
+  if (b.N <= 0) return 0;
+  const int nb = (b.N + PG - 1) / PG;
+  ProfScope ps(K_SURFEL_BWD_BATCH, st);
+  GSB_SURFEL_K3(b.k3, (k_disk_bwd_batch<K3><<<nb, PG, 0, st>>>(b.C, b.N, b.pws, b.rots, b.scales, b.shs, b.poses,
+                                                               *b.cams, rows, g_pws, g_shs, g_alphas, g_scales, g_rots,
+                                                               g_us)));
+  GSB_CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, const int32_t *gsid, float *image,
                        int32_t *contrib, float *final_tau, float *depth_image, float *alpha_image, float *normal_image,
-                       const GeoPlanes *geo, int *work, cudaStream_t st) {
+                       const GeoPlanes *geo, int *work, cudaStream_t st, int frames) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0) return 0;
   if (work == nullptr) return set_arg_error("draw_surfel: work area missing");
-  // the normal (and geometry) planes of empty tiles: k_tile_list zeroes the other five planes
-  const size_t HW = (size_t)H * W;
+  // the normal (and geometry) planes of empty tiles, of every frame: k_tile_list zeroes the other
+  // five planes
+  const size_t HW = (size_t)H * W * (frames > 0 ? frames : 1);
   GSB_CUDA_TRY(cudaMemsetAsync(normal_image, 0, sizeof(float) * 3 * HW, st));
   if (geo) {
     GSB_CUDA_TRY(cudaMemsetAsync(geo->distortion, 0, sizeof(float) * HW, st));
@@ -665,14 +864,22 @@ int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, c
     GSB_CUDA_TRY(cudaMemsetAsync(geo->median_depth, 0, sizeof(float) * HW, st));
     GSB_CUDA_TRY(cudaMemsetAsync(geo->median_contrib, 0, sizeof(int32_t) * HW, st));
   }
-  int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st);
+  int rc = launch_tile_list(H, W, ranges, image, contrib, final_tau, depth_image, alpha_image, work, st, frames);
   if (rc || recs == nullptr) return rc;
   int grid = 0;
-  rc = persistent_grid(gx * gy, DRAW_SURFEL_MINBLOCKS, grid);
+  rc = persistent_grid(gx * gy * (frames > 0 ? frames : 1), DRAW_SURFEL_MINBLOCKS, grid);
   if (rc) return rc;
   const int2 *r2 = reinterpret_cast<const int2 *>(ranges);
   const float4 *r4 = reinterpret_cast<const float4 *>(recs);
-  if (geo) {
+  if (frames > 0 && geo) {
+    ProfScope ps(K_DRAW_2DGS_BATCH, st);
+    k_draw_2dgs_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, r2, r4, gsid, image, contrib, final_tau, depth_image,
+                                            alpha_image, normal_image, *geo, work);
+  } else if (frames > 0) {
+    ProfScope ps(K_DRAW_SURFEL_BATCH, st);
+    k_draw_disk_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, r2, r4, gsid, image, contrib, final_tau, depth_image,
+                                            alpha_image, normal_image, work);
+  } else if (geo) {
     ProfScope ps(K_DRAW_2DGS, st);
     k_draw_2dgs<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, image, contrib, final_tau, depth_image, alpha_image,
                                       normal_image, *geo, work);
@@ -688,7 +895,7 @@ int launch_draw_surfel(int H, int W, const int32_t *ranges, const float *recs, c
 int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, const float *recs, const int32_t *gsid,
                                 const int32_t *contrib, const float *final_tau, const float *dl_image,
                                 const float *dl_depth, const float *dl_alpha, const float *dl_normal,
-                                const GeoGrads *geo, float *rows, int *work, cudaStream_t st) {
+                                const GeoGrads *geo, float *rows, int *work, cudaStream_t st, int frames) {
   const int gx = (W + TILE - 1) / TILE, gy = (H + TILE - 1) / TILE;
   if (gx <= 0 || gy <= 0 || N <= 0) return 0;
   GSB_CUDA_TRY(cudaMemsetAsync(rows, 0, sizeof(float) * sf::kRowFloats * (size_t)N, st));
@@ -696,15 +903,23 @@ int launch_draw_surfel_backward(int H, int W, int N, const int32_t *ranges, cons
   const bool with_geo = geo != nullptr && (geo->distortion != nullptr || geo->median != nullptr);
   if (dl_image == nullptr && dl_depth == nullptr && dl_alpha == nullptr && dl_normal == nullptr && !with_geo) return 0;
   if (work == nullptr) return set_arg_error("draw_surfel_backward: work area missing");
-  int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st);
+  int rc = launch_tile_list(H, W, ranges, nullptr, nullptr, nullptr, nullptr, nullptr, work, st, frames);
   if (rc) return rc;
   int grid = 0;
-  rc = persistent_grid(gx * gy, with_geo ? DRAW_2DGS_BWD_MINBLOCKS : DRAW_SURFEL_BWD_MINBLOCKS, grid);
+  rc = persistent_grid(gx * gy * (frames > 0 ? frames : 1),
+                       with_geo ? DRAW_2DGS_BWD_MINBLOCKS : DRAW_SURFEL_BWD_MINBLOCKS, grid);
   if (rc) return rc;
   const int2 *r2 = reinterpret_cast<const int2 *>(ranges);
   const float4 *r4 = reinterpret_cast<const float4 *>(recs);
   const SurfelGrads dl{dl_image, dl_depth, dl_alpha, dl_normal};
-  if (with_geo) {
+  if (frames > 0 && with_geo) {
+    ProfScope ps(K_DRAW_2DGS_BWD_BATCH, st);
+    k_draw_2dgs_bwd_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, r2, r4, gsid, contrib, final_tau, GeoBwdArgs{dl, *geo},
+                                                rows, work);
+  } else if (frames > 0) {
+    ProfScope ps(K_DRAW_SURFEL_BWD_BATCH, st);
+    k_draw_disk_bwd_batch<<<grid, 128, 0, st>>>(W, H, gx, gy, r2, r4, gsid, contrib, final_tau, dl, rows, work);
+  } else if (with_geo) {
     ProfScope ps(K_DRAW_2DGS_BWD, st);
     k_draw_2dgs_bwd<<<grid, 128, 0, st>>>(W, H, gx, r2, r4, gsid, contrib, final_tau, GeoBwdArgs{dl, *geo}, rows,
                                           work);

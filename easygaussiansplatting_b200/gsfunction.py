@@ -762,6 +762,111 @@ class GSFunctionSurfelGeometry(torch.autograd.Function):
         return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
 
 
+def _surfel_batch_cams(who, cams, dev):
+    """the checks of GSFunctionSurfel / GSFunctionSurfelGeometry per camera, then the batch's own
+    (BatchCameras: one width and height for all) -> ops.BatchCameras"""
+    from . import ops
+    cams = list(cams)
+    for c in cams:
+        if getattr(c, "antialiased", False):
+            raise ValueError("%s has no antialiased mode: cam.antialiased must be False" % who)
+        _pinhole_only(c, who)
+        if getattr(c, "grad_exchange", None) is not None:
+            raise ValueError("%s takes no gradient exchange: cam.grad_exchange must not be set" % who)
+    return ops.BatchCameras(cams, dev)
+
+
+def _surfel_batch_us(us, bc, N):
+    if not isinstance(us, torch.Tensor) or tuple(us.shape) != (bc.C, N, 2):
+        raise ValueError("us must be a [C, N, 2] tensor (C = %d, N = %d), got %s"
+                         % (bc.C, N, tuple(getattr(us, "shape", ()))))
+
+
+class GSFunctionSurfelBatch(torch.autograd.Function):
+    """GSFunctionSurfel for C cameras in one call (DESIGN 3.25): `apply(pws, shs, alphas, scales, rots,
+    us, cams)` -> (image[C,3,H,W], depth[C,H,W], alpha[C,H,W], normal[C,3,H,W], mask[C,N]) with frame c
+    and mask[c] those GSFunctionSurfel gives for cams[c], bit for bit.  The cameras are pinhole, of one
+    width and height (else ValueError), each with its own pose and intrinsics.  us is the [C,N,2]
+    dummy whose gradient is each camera's dL/du, so `DensityController.update_density_info(us.grad[c],
+    mask[c])` works per camera.  The map gradients are the sums over the cameras, taken in one
+    per-surfel pass.  A plane the loss does not use is not read in the backward; with none used the
+    backward rasterizer is skipped.  Refuses what GSFunctionSurfel refuses: antialiased cameras, other
+    camera models, cam.grad_exchange, filter3d and us_abs."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cams, filter3d=None, us_abs=None):
+        from . import ops
+        who = "GSFunctionSurfelBatch"
+        bc = _surfel_batch_cams(who, cams, pws.device)
+        if filter3d is not None:
+            raise ValueError("%s has no 3D filter: filter3d must be None" % who)
+        if us_abs is not None:
+            raise ValueError("%s has no absolute-gradient statistic: us_abs must be None" % who)
+        _surfel_batch_us(us, bc, pws.shape[0])
+        ctx.set_materialize_grads(False)
+        us_, depths, areas, colors, records = ops.surfel_preprocess_batch(pws, rots, scales, shs, alphas.reshape(-1),
+                                                                          bc)
+        image, contrib, final_tau, ranges, gsid, depth, alpha, normal = ops.splat_surfel_batch(
+            bc.height, bc.width, us_, depths, areas, records, capacity=True)
+        ctx.bc = bc
+        ctx.alpha_shape = alphas.shape
+        ctx.save_for_backward(pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid)
+        return image, depth, alpha, normal, depths > 0.2
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, _):
+        from . import ops
+        bc = ctx.bc
+        pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid = ctx.saved_tensors
+        rows = ops.splatB_surfel_batch(bc.height, bc.width, records, contrib, final_tau, ranges, gsid,
+                                       dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal)
+        dpws, dshs, dalphas, dscales, drots, dus = ops.surfel_preprocessB_batch(pws, rots, scales, shs, bc, rows)
+        grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
+        return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
+
+
+class GSFunctionSurfelGeometryBatch(torch.autograd.Function):
+    """GSFunctionSurfelGeometry for C cameras in one call (DESIGN 3.25): `apply(pws, shs, alphas, scales,
+    rots, us, cams, near=0.2, far=100.0)` -> (image[C,3,H,W], depth[C,H,W], alpha[C,H,W],
+    normal[C,3,H,W], distortion[C,H,W], median_depth[C,H,W], mask[C,N]), frame c that of
+    GSFunctionSurfelGeometry for cams[c], bit for bit.  Cameras, us and the backward as
+    GSFunctionSurfelBatch's; with no gradient on distortion and median_depth the backward is
+    GSFunctionSurfelBatch's.  Under torch.no_grad() it is the batched depth renderer of the mesh
+    recipe (INTEGRATION.md)."""
+
+    @staticmethod
+    def forward(ctx, pws, shs, alphas, scales, rots, us, cams, near=0.2, far=100.0):
+        from . import ops
+        who = "GSFunctionSurfelGeometryBatch"
+        bc = _surfel_batch_cams(who, cams, pws.device)
+        _surfel_batch_us(us, bc, pws.shape[0])
+        near, far = ops._near_far(near, far)
+        ctx.set_materialize_grads(False)
+        us_, depths, areas, colors, records = ops.surfel_preprocess_batch(pws, rots, scales, shs, alphas.reshape(-1),
+                                                                          bc)
+        (image, contrib, final_tau, ranges, gsid, depth, alpha, normal, distortion, median_depth, moments,
+         median_contrib) = ops.splat_surfel_geometry_batch(bc.height, bc.width, us_, depths, areas, records, near, far,
+                                                           capacity=True)
+        ctx.bc, ctx.near, ctx.far = bc, near, far
+        ctx.alpha_shape = alphas.shape
+        ctx.save_for_backward(pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid, alpha, moments,
+                              median_contrib)
+        return image, depth, alpha, normal, distortion, median_depth, depths > 0.2
+
+    @staticmethod
+    def backward(ctx, dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal, dloss_ddistortion, dloss_dmedian, _):
+        from . import ops
+        bc = ctx.bc
+        pws, shs, scales, rots, records, contrib, final_tau, ranges, gsid, alpha, moments, median_contrib = \
+            ctx.saved_tensors
+        rows = ops.splatB_surfel_geometry_batch(bc.height, bc.width, records, contrib, final_tau, ranges, gsid, alpha,
+                                                moments, median_contrib, dloss_dimage, dloss_ddepth, dloss_dalpha,
+                                                dloss_dnormal, dloss_ddistortion, dloss_dmedian, ctx.near, ctx.far)
+        dpws, dshs, dalphas, dscales, drots, dus = ops.surfel_preprocessB_batch(pws, rots, scales, shs, bc, rows)
+        grads = (dpws, dshs, dalphas.reshape(ctx.alpha_shape), dscales, drots, dus)
+        return grads + (None,) * (len(ctx.needs_input_grad) - len(grads))
+
+
 @torch.no_grad()
 def contribution_stats(pws, shs, alphas, scales, rots, cams, filter3d=None, surfel=False):
     """Per-Gaussian contribution statistics over the views `cams` (DESIGN 3.18), with exactly the

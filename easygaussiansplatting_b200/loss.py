@@ -61,7 +61,14 @@ def depth_to_normal(depth, cam):
     against an empty background has no vertical difference), or whose cross product is exactly 0.
     2DGS's normal term (alpha detached, as there) is then
         L_n = (1 - (normal * depth_to_normal(median_depth, cam) * alpha.detach()).sum(0)).mean()
-    with normal and alpha GSFunctionSurfelGeometry's planes (its normal plane is sum w n)."""
+    with normal and alpha GSFunctionSurfelGeometry's planes (its normal plane is sum w n).
+    A batch (GSFunctionSurfelGeometryBatch, DESIGN 3.25): depth[C,H,W] with `cam` a list of C cameras
+    -> [C,3,H,W], frame c the normal of depth[c] through cam[c]."""
+    if isinstance(cam, (list, tuple)):
+        if depth.dim() != 3 or depth.shape[0] != len(cam):
+            raise ValueError("depth must be [C, H, W] for a list of C cameras, got %s for %d cameras"
+                             % (tuple(depth.shape), len(cam)))
+        return torch.stack([depth_to_normal(depth[c], cam[c]) for c in range(len(cam))])
     d = depth.reshape(depth.shape[-2], depth.shape[-1])
     H, W = d.shape
     v, u = torch.meshgrid(torch.arange(H, dtype=d.dtype, device=d.device),

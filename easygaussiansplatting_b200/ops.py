@@ -1497,6 +1497,194 @@ def splatB_surfel_geometry(height, width, records, contrib, final_tau, patch_ran
 
 
 # ---------------------------------------------------------------------------------------
+# Batched 2D Gaussian Splatting (extension; DESIGN 3.25): the surfel path for C pinhole cameras of one
+# image size in one call, laid out as the batched rendering above (record c N + n = surfel n seen by
+# camera c; per-record outputs [C, N, ...], per-pixel ones [C, ..., H, W]).  Frame c is the single
+# frame of camera c, bit for bit.
+def _surfel_batch_cams(cams, device):
+    bc = _batch_cams(cams, device)
+    if bc.camera_model != "pinhole" or bc.antialiased:
+        raise ValueError("surfel batches take pinhole cameras without antialiasing, got camera_model=%r, "
+                         "antialiased=%s" % (bc.camera_model, bc.antialiased))
+    return bc
+
+
+def surfel_preprocess_batch(pws, rots, scales, shs, alphas, cams):
+    """`surfel_preprocess` for C cameras at once (gsb_2dgs_batch_preprocess_forward).  cams: a list of
+    pinhole `gsfunction.Camera` of one size (or a `BatchCameras`).  -> (us[C,N,2], depths[C,N],
+    areas[C,N,2] i32, colors[C,N,3], records[C N, 20]); camera c's rows are the bits
+    `surfel_preprocess` gives for camera c alone."""
+    (pws, rots, scales, shs), N, k = _gaussian_map(pws, rots, scales, shs)
+    bc = _surfel_batch_cams(cams, pws.device)
+    alphas = _per_gaussian(alphas, "alphas", N, pws)
+    Cn = bc.C
+    o = dict(dtype=torch.float32, device=pws.device)
+    us = torch.empty((Cn, N, 2), **o); depths = torch.empty((Cn, N), **o); colors = torch.empty((Cn, N, 3), **o)
+    areas = torch.empty((Cn, N, 2), dtype=torch.int32, device=pws.device)
+    records = torch.empty((Cn * N, SURFEL_RECORD), **o)
+    lib = _L()
+    with torch.cuda.device(pws.device):
+        _lib.check(lib.gsb_2dgs_batch_preprocess_forward(
+            Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(alphas), _ptr(us),
+            _ptr(depths), _ptr(areas), _ptr(colors), _ptr(records), _stream()), lib)
+    return us, depths, areas, colors, records
+
+
+def surfel_preprocessB_batch(pws, rots, scales, shs, cams, rows):
+    """Backward of `surfel_preprocess_batch` from the rows [C N, 18] of `splatB_surfel_batch` /
+    `splatB_surfel_geometry_batch` (gsb_2dgs_batch_preprocess_backward): the C cameras' contributions
+    summed in fp32 registers in camera order.  -> (dpws[N,3], dshs[N,3k], dalphas[N], dscales[N,3]
+    (column 2: 0), drots[N,4], dus[C,N,2] (per camera))"""
+    (pws, rots, scales, shs), N, k = _gaussian_map(pws, rots, scales, shs)
+    bc = _surfel_batch_cams(cams, pws.device)
+    Cn = bc.C
+    rows = _chk(rows, "rows", last=SURFEL_ROW, ndim=2)
+    _same_device(pws, rows)
+    if rows.shape[0] != Cn * N:
+        raise ValueError("rows must be [C N, %d]" % SURFEL_ROW)
+    o = dict(dtype=torch.float32, device=pws.device)
+    out = (torch.empty((N, 3), **o), torch.empty((N, 3 * k), **o), torch.empty((N,), **o), torch.empty((N, 3), **o),
+           torch.empty((N, 4), **o), torch.empty((Cn, N, 2), **o))
+    lib = _L()
+    with torch.cuda.device(pws.device):
+        _lib.check(lib.gsb_2dgs_batch_preprocess_backward(
+            Cn, N, k, _ptr(pws), _ptr(rots), _ptr(scales), _ptr(shs), *bc.args(), _ptr(rows),
+            *[_ptr(t) for t in out], _stream()), lib)
+    return out
+
+
+def _surfel_batch_inputs(us, depths, areas, records):
+    """the [C, N, ...] inputs of a batched surfel frame, checked -> (C, N, us, depths, areas, records)"""
+    us = _chk(us, "us", last=2, ndim=3); depths = _chk(depths, "depths")
+    areas = _chk(areas, "areas", dtype=torch.int32, last=2, ndim=3)
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    _same_device(us, depths, areas, records)
+    Cn, N = us.shape[0], us.shape[1]
+    if not (depths.numel() == Cn * N and tuple(areas.shape[:2]) == (Cn, N) and records.shape[0] == Cn * N):
+        raise ValueError("batched surfel frame inputs disagree on C, N")
+    return Cn, N, us, depths, areas, records
+
+
+def splat_surfel_batch(height, width, us, depths, areas, records, capacity=False):
+    """`splat_surfel` of C frames at once, binned and drawn as one tall frame (gsb_2dgs_batch_render /
+    _forward).  Inputs are `surfel_preprocess_batch`'s; MUTATES depths / areas of records that touch
+    no tile.  -> [image[C,3,H,W], contrib[C,H,W] i32, final_tau[C,H,W], patch_range_per_tile[C T,2]
+    i32, gsid_per_patch[P] i32 (record ids c N + n), depth[C,H,W], alpha[C,H,W], normal[C,3,H,W]].
+    capacity: as for `splat_surfel`."""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    Cn, N, us, depths, areas, records = _surfel_batch_inputs(us, depths, areas, records)
+    dev, lib = us.device, _L()
+    with torch.cuda.device(dev):
+        _, _, out = _frame(H, W, us, depths, areas, [(H, W), (H, W), (3, H, W)], lib.gsb_2dgs_batch_workspace_bytes,
+                           (lib.gsb_2dgs_batch_forward, [_ptr(us), _ptr(depths), _ptr(areas), _ptr(records)]),
+                           (lib.gsb_2dgs_batch_render, [_ptr(us), _ptr(depths), _ptr(records)]), capacity,
+                           ("surfel_batch", dev.index, Cn, H, W, N), frames=Cn)
+    return out
+
+
+def splat_surfel_geometry_batch(height, width, us, depths, areas, records, near=0.2, far=100.0, capacity=False):
+    """`splat_surfel_geometry` of C frames at once (gsb_2dgs_batch_render_geometry / _forward_geometry):
+    `splat_surfel_batch`'s eight outputs + [distortion[C,H,W], median_depth[C,H,W], moments[C,2,H,W],
+    median_contrib[C,H,W] i32]."""
+    H, W = int(height), int(width)
+    if H <= 0 or W <= 0:
+        raise ValueError("height and width must be positive")
+    near, far = _near_far(near, far)
+    Cn, N, us, depths, areas, records = _surfel_batch_inputs(us, depths, areas, records)
+    dev, lib = us.device, _L()
+    planes = [(H, W), (H, W), (3, H, W), (H, W), (2, H, W), (H, W), ((H, W), torch.int32)]
+    nf = [C.c_float(near), C.c_float(far)]
+    with torch.cuda.device(dev):
+        _, _, out = _frame(H, W, us, depths, areas, planes, lib.gsb_2dgs_batch_workspace_bytes,
+                           (lib.gsb_2dgs_batch_forward_geometry, [_ptr(us), _ptr(depths), _ptr(areas), _ptr(records)]
+                            + nf),
+                           (lib.gsb_2dgs_batch_render_geometry, [_ptr(us), _ptr(depths), _ptr(records)] + nf), capacity,
+                           ("surfel_batch", dev.index, Cn, H, W, N), frames=Cn)
+    distortion, moments, median_depth, median_contrib = out[8:]
+    return out[:8] + [distortion, median_depth, moments, median_contrib]
+
+
+def _surfel_batch_drawn(H, W, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch, planes):
+    """the drawn batch frame of a backward, checked: C from contrib [C,H,W]; planes: (name, tensor or
+    None, channels) of [C, channels, H, W] -> (C, N, records, contrib, final_tau, ranges, gsid, tensors)"""
+    records = _chk(records, "records", last=SURFEL_RECORD, ndim=2)
+    contrib = _chk(contrib, "contrib", dtype=torch.int32, ndim=3); final_tau = _chk(final_tau, "final_tau")
+    ranges = _chk(patch_range_per_tile, "patch_range_per_tile", dtype=torch.int32, last=2)
+    gsid = _chk(gsid_per_patch, "gsid_per_patch", dtype=torch.int32)
+    _same_device(records, contrib, final_tau, ranges, gsid)
+    Cn = contrib.shape[0]
+    _check_drawn(H, W, ranges, ((contrib, 1), (final_tau, 1)), "contrib / final_tau do not match C x height x width",
+                 frames=Cn)
+    if records.shape[0] % max(Cn, 1) != 0:
+        raise ValueError("records must be [C N, %d]" % SURFEL_RECORD)
+    out = []
+    for name, t, n in planes:
+        if t is not None:
+            t = _chk(t, name)
+            _same_device(records, t)
+            if t.numel() != Cn * n * H * W:
+                raise ValueError("%s does not match C x height x width" % name)
+        out.append(t)
+    return Cn, records.shape[0] // max(Cn, 1), records, contrib, final_tau, ranges, gsid, out
+
+
+def splatB_surfel_batch(height, width, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                        dloss_dimage=None, dloss_ddepth=None, dloss_dalpha=None, dloss_dnormal=None):
+    """Backward of `splat_surfel_batch` (gsb_2dgs_batch_backward) from the planes' upstream gradients
+    ([C,3,H,W], [C,H,W], [C,H,W], [C,3,H,W]; None = zero and not read; all None: no rasterizer pass,
+    zero rows).  -> rows[C N, 18] for `surfel_preprocessB_batch`"""
+    H, W = int(height), int(width)
+    Cn, N, records, contrib, final_tau, ranges, gsid, planes = _surfel_batch_drawn(
+        H, W, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+        (("dloss_dimage", dloss_dimage, 3), ("dloss_ddepth", dloss_ddepth, 1), ("dloss_dalpha", dloss_dalpha, 1),
+         ("dloss_dnormal", dloss_dnormal, 3)))
+    P, dev, lib = gsid.numel(), records.device, _L()
+    rows = torch.empty((Cn * N, SURFEL_ROW), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_2dgs_batch_workspace_bytes(Cn, N, H, W, 0), dev)
+        _lib.check(lib.gsb_2dgs_batch_backward(Cn, H, W, N, P, _ptr(records), _ptr(contrib), _ptr(final_tau),
+                                               _ptr(ranges), _ptr(gsid), *[_ptr(t) for t in planes], _ptr(ws),
+                                               ws.numel(), _ptr(rows), _stream()), lib)
+    return rows
+
+
+def splatB_surfel_geometry_batch(height, width, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                                 alpha, moments, median_contrib, dloss_dimage=None, dloss_ddepth=None,
+                                 dloss_dalpha=None, dloss_dnormal=None, dloss_ddistortion=None, dloss_dmedian=None,
+                                 near=0.2, far=100.0):
+    """Backward of `splat_surfel_geometry_batch` (gsb_2dgs_batch_backward_geometry): `splatB_surfel_batch`'s
+    upstream planes plus dloss_ddistortion[C,H,W] and dloss_dmedian[C,H,W]; alpha, moments and
+    median_contrib are the forward's planes.  -> rows[C N, 18].  With both geometry gradients None
+    this is `splatB_surfel_batch` (same kernel, same rows)."""
+    if dloss_ddistortion is None and dloss_dmedian is None:
+        return splatB_surfel_batch(height, width, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+                                   dloss_dimage, dloss_ddepth, dloss_dalpha, dloss_dnormal)
+    H, W = int(height), int(width)
+    near, far = _near_far(near, far)
+    Cn, N, records, contrib, final_tau, ranges, gsid, planes = _surfel_batch_drawn(
+        H, W, records, contrib, final_tau, patch_range_per_tile, gsid_per_patch,
+        (("dloss_dimage", dloss_dimage, 3), ("dloss_ddepth", dloss_ddepth, 1), ("dloss_dalpha", dloss_dalpha, 1),
+         ("dloss_dnormal", dloss_dnormal, 3), ("dloss_ddistortion", dloss_ddistortion, 1),
+         ("dloss_dmedian", dloss_dmedian, 1), ("alpha", alpha, 1), ("moments", moments, 2)))
+    alpha, moments = planes[6:]
+    median_contrib = _chk(median_contrib, "median_contrib", dtype=torch.int32)
+    _same_device(records, median_contrib)
+    if median_contrib.numel() != Cn * H * W:
+        raise ValueError("median_contrib does not match C x height x width")
+    P, dev, lib = gsid.numel(), records.device, _L()
+    rows = torch.empty((Cn * N, SURFEL_ROW), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        ws = _bytes(lib.gsb_2dgs_batch_workspace_bytes(Cn, N, H, W, 0), dev)
+        _lib.check(lib.gsb_2dgs_batch_backward_geometry(
+            Cn, H, W, N, P, _ptr(records), _ptr(contrib), _ptr(final_tau), _ptr(ranges), _ptr(gsid),
+            *[_ptr(t) for t in planes[:4]], _ptr(ws), ws.numel(), _ptr(rows), near, far, _ptr(alpha), _ptr(moments),
+            _ptr(median_contrib), *[_ptr(t) for t in planes[4:6]], _stream()), lib)
+    return rows
+
+
+# ---------------------------------------------------------------------------------------
 # Mesh extraction (gsb_tsdf_*, DESIGN 3.17): projective TSDF fusion of depth maps and marching
 # cubes.  The grid: point (i, j, k) at origin + voxel_size (i, j, k); tsdf, weight [nz, ny, nx] and
 # color_grid [3, nz, ny, nx] (or None), float32 CUDA tensors, contiguous (updated in place).

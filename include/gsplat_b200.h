@@ -1048,6 +1048,78 @@ int gsb_splat_backward_batch_rgbd(int C, int H, int W, int N, int64_t P, const f
                                   const void *packed_records, void *ws, size_t ws_bytes, float *moments_out,
                                   float *dloss_ddepths, gsb_stream_t stream);
 
+/* ---- batched 2D Gaussian Splatting (extension; DESIGN 3.25): the surfel frames of
+ * gsb_surfel_preprocess_* / gsb_splat_surfel_* / gsb_splat_2dgs_* for C pinhole cameras of one image
+ * size in one call, laid out as the batched rendering above: records c N + n (surfel n seen by
+ * camera c), per-record arrays [C, N, ...], per-pixel planes [C, ..., H, W], frame c in tile rows
+ * [c gy, (c + 1) gy) of the tall frame, tile ranges [C gx gy, 2], gsid_per_patch of record ids.
+ * Frame c is the single frame of camera c, bit for bit.  The binning is gsb_splat_bin_batch's.
+ * Errors before any launch: C < 1, C > GSB_BATCH_MAX_CAMERAS, C N >= 2^31,
+ * C gy > GSB_MAX_GRID_TILES, 2^30 patches or more, misaligned planes or records, and (per-surfel
+ * entry points) a camera model other than GSB_CAMERA_PINHOLE.  poses and intrinsics as for
+ * gsb_preprocess_forward_batch (k must be 0).
+ * gsb_2dgs_batch_preprocess_forward: gsb_surfel_preprocess_forward's outputs per camera into
+ *   us[C,N,2], depths[C,N], areas[C,N,2], colors[C,N,3] and records[C N, 20] (16-byte aligned).
+ * gsb_2dgs_batch_preprocess_backward: from rows[C N, 18] of gsb_2dgs_batch_backward{,_geometry},
+ *   gsb_surfel_preprocess_backward's gradients summed over the cameras in fp32 in camera order
+ *   (dloss_dpws[N,3], dloss_dshs[N,3k], dloss_dalphas[N], dloss_dscales[N,3], dloss_drots[N,4]) and
+ *   dloss_dus[C,N,2] per camera.
+ * gsb_2dgs_batch_workspace_bytes: the workspace of the render / forward entry points for P patches
+ *   (P_cap) and of the backward ones with P = 0 (0 for a C or N they refuse).
+ * gsb_2dgs_batch_render / _forward / _backward: gsb_splat_surfel_render / _forward / _backward of the
+ *   C frames; the _geometry forms: gsb_splat_2dgs_render / _forward / _backward's, with every
+ *   geometry plane [C, ..., H, W]. */
+size_t gsb_2dgs_batch_workspace_bytes(int C, int N, int H, int W, int64_t P);
+int gsb_2dgs_batch_preprocess_forward(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                      const float *scales, const float *shs, const float *poses,
+                                      const float *intrinsics, int camera_model, float width, float height,
+                                      const float *alphas, float *us, float *depths, int32_t *areas, float *colors,
+                                      float *records, gsb_stream_t stream);
+int gsb_2dgs_batch_preprocess_backward(int C, int N, int sh_dim3, const float *pws, const float *rots,
+                                       const float *scales, const float *shs, const float *poses,
+                                       const float *intrinsics, int camera_model, float width, float height,
+                                       const float *rows, float *dloss_dpws, float *dloss_dshs, float *dloss_dalphas,
+                                       float *dloss_dscales, float *dloss_drots, float *dloss_dus,
+                                       gsb_stream_t stream);
+int gsb_2dgs_batch_render(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                          const float *depths, const float *records, const void *bin_ws, void *ws, size_t ws_bytes,
+                          float *image, int32_t *contrib, float *final_tau, int32_t *patch_range_per_tile,
+                          int32_t *gsid_per_patch, float *depth_image, float *alpha_image, float *normal_image,
+                          gsb_stream_t stream);
+int gsb_2dgs_batch_forward(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                           const float *records, int64_t P_cap, uint32_t depth_key_cap, void *bin_ws,
+                           size_t bin_ws_bytes, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                           float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                           uint32_t *status_host, float *depth_image, float *alpha_image, float *normal_image,
+                           gsb_stream_t stream);
+int gsb_2dgs_batch_backward(int C, int H, int W, int N, int64_t P, const float *records, const int32_t *contrib,
+                            const float *final_tau, const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                            const float *dloss_dimage, const float *dloss_ddepth, const float *dloss_dalpha,
+                            const float *dloss_dnormal, void *ws, size_t ws_bytes, float *rows, gsb_stream_t stream);
+int gsb_2dgs_batch_render_geometry(int C, int H, int W, int N, int64_t P, uint32_t depth_key_max, const float *us,
+                                   const float *depths, const float *records, float near, float far,
+                                   const void *bin_ws, void *ws, size_t ws_bytes, float *image, int32_t *contrib,
+                                   float *final_tau, int32_t *patch_range_per_tile, int32_t *gsid_per_patch,
+                                   float *depth_image, float *alpha_image, float *normal_image, float *distortion,
+                                   float *moments, float *median_depth, int32_t *median_contrib,
+                                   gsb_stream_t stream);
+int gsb_2dgs_batch_forward_geometry(int C, int H, int W, int N, const float *us, float *depths, int32_t *areas,
+                                    const float *records, float near, float far, int64_t P_cap,
+                                    uint32_t depth_key_cap, void *bin_ws, size_t bin_ws_bytes, void *ws,
+                                    size_t ws_bytes, float *image, int32_t *contrib, float *final_tau,
+                                    int32_t *patch_range_per_tile, int32_t *gsid_per_patch, uint32_t *status_host,
+                                    float *depth_image, float *alpha_image, float *normal_image, float *distortion,
+                                    float *moments, float *median_depth, int32_t *median_contrib,
+                                    gsb_stream_t stream);
+int gsb_2dgs_batch_backward_geometry(int C, int H, int W, int N, int64_t P, const float *records,
+                                     const int32_t *contrib, const float *final_tau,
+                                     const int32_t *patch_range_per_tile, const int32_t *gsid_per_patch,
+                                     const float *dloss_dimage, const float *dloss_ddepth, const float *dloss_dalpha,
+                                     const float *dloss_dnormal, void *ws, size_t ws_bytes, float *rows, float near,
+                                     float far, const float *alpha_image, const float *moments,
+                                     const int32_t *median_contrib, const float *dloss_ddistortion,
+                                     const float *dloss_dmedian, gsb_stream_t stream);
+
 /* ---- launch accounting and optional per-kernel timing (no reference counterpart; used by
  * bench.py for `gpu_launches` and the roofline's live CUDA-event kernel durations).
  * Kernel ids 0..gsb_profile_kernels()-1, names from gsb_profile_kernel_name().
